@@ -56,7 +56,8 @@ def get_join_schemas(df1: Any, df2: Any, how: str, on: Optional[List[str]]) -> T
 
 def _key64(t1: B200Table, t2: B200Table, keys: List[str]):
     """One 8-byte surrogate key per row on both sides + validity (NULL in any key -> never matches).
-    exact == False means the surrogate is a hash and matches must be verified."""
+    A NaN in a float key counts as NULL: it never matches, on either key path, as in the reference, where
+    pandas holds NULL as NaN.  exact == False means the surrogate is a hash and matches must be verified."""
     def norm(c: torch.Tensor) -> torch.Tensor:
         if c.dtype in (torch.float32, torch.float64):
             return torch.where(c == 0, torch.zeros_like(c), c)  # -0.0 == 0.0
@@ -67,6 +68,9 @@ def _key64(t1: B200Table, t2: B200Table, keys: List[str]):
         for k in keys:
             i = t.schema.index_of_key(k)
             c = norm(t.columns[i])
+            if c.dtype in (torch.float32, torch.float64):
+                not_nan = (c == c).to(torch.uint8)
+                val = not_nan if val is None else val & not_nan
             if remap is not None and k in remap:
                 m = remap[k]
                 c = m[c.long().clamp(min=0)]

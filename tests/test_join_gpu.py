@@ -168,13 +168,16 @@ def test_radix_join_path_matches_oracle(e, how, monkeypatch):
     df_eq(got, exp.values.tolist(), got.schema, throw=True)
 
 
-def test_radix_join_with_a_hot_key_on_the_build_side(e):
+def test_radix_join_with_a_hot_key_on_the_build_side(e, monkeypatch):
     """>= 2M rows on both sides takes the radix (region) path; a skewed build side overflows its region of
-    the hash table.  The build reports that and is redone with one region (advisor finding r1): no match
-    may be lost."""
+    the hash table.  The build reports that and is redone with one region: no match may be lost, and each
+    match must pair the right rows."""
+    from _join_spy import Launches
     from fugue_b200.dataframe import B200DataFrame
     from fugue_b200.table import B200Table
+    from oracle import join as oj
 
+    launches = Launches(monkeypatch)
     rng = np.random.default_rng(5)
     n = 2_200_000
     bk = rng.integers(0, 50_000, n).astype("int64")
@@ -184,14 +187,18 @@ def test_radix_join_with_a_hot_key_on_the_build_side(e):
     left = B200DataFrame(B200Table("key:long,lv:long", [torch.from_numpy(pk).cuda(), torch.arange(n, device="cuda")]))
     right = B200DataFrame(B200Table("key:long,rv:long", [torch.from_numpy(bk).cuda(), torch.arange(n, device="cuda")]))
     uk, cnt = np.unique(bk, return_counts=True)
-    mult = dict(zip(uk.tolist(), cnt.tolist()))
-    per_probe = np.array([mult.get(int(k), 0) for k in pk[:1000]])
     res = e.join(left, right, "inner", ["key"]).native
+    assert launches.path() == "fused-fallback", launches.calls
     expect_total = int(np.sum(cnt[np.searchsorted(uk, pk[np.isin(pk, uk)])]))
     assert res.num_rows == expect_total
-    lv = res.column("lv").cpu().numpy()
-    got = np.bincount(lv[lv < 1000], minlength=1000)
-    assert np.array_equal(got, per_probe)
+    # the pairs of the first 1000 probe rows (275 k matches each for the hot key's three), build rows included
+    lv, rv = res.column("lv").cpu().numpy(), res.column("rv").cpu().numpy()
+    first = lv < 1000
+    order = np.lexsort((rv[first], lv[first]))
+    exp_l, exp_r = oj.join_pairs(pk[:1000], None, bk, None, False)
+    assert np.array_equal(lv[first][order], exp_l) and np.array_equal(rv[first][order], exp_r)
     # semi / anti on the same data
-    semi = e.join(left, right, "semi", ["key"]).native.num_rows
-    assert semi == int(np.isin(pk, uk).sum())
+    launches.clear()
+    semi = e.join(left, right, "semi", ["key"]).native
+    assert launches.path() == "table16-fallback", launches.calls
+    assert np.array_equal(np.sort(semi.column("lv").cpu().numpy()), np.flatnonzero(np.isin(pk, uk)))

@@ -181,11 +181,32 @@ constexpr int kRankBlock = 1024, kRankWarps = kRankBlock / 32, kRankItems = kTil
 constexpr uint32_t kMetaRank = kTile, kMetaCnt = 3 * kTile, kMetaBytes = 3 * kTile + 512;
 static_assert(kRankItems * kRankBlock == kTile, "tile must be a multiple of the rank block");
 
-template <bool kSingleU64, int kBits>
+// kStaged (one 8-byte key without validity: hashed, or a radix digit): the keys of tile t+1 are copied
+// into shared memory (cp.async, one ring slot per row, each thread reads back only what it copied) while
+// tile t is ranked, so the key loads of the next tile overlap the barriers and the prefix of this one.
+// Dynamic shared memory: 2 x kTile uint64.
+constexpr size_t kRankStageBytes = 2 * (size_t)kTile * 8;
+
+__device__ __forceinline__ void cp_async8(void* dst_smem, const void* src) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"((uint32_t)__cvta_generic_to_shared(dst_smem)),
+               "l"(src) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+__device__ __forceinline__ void cp_async_wait_one() { asm volatile("cp.async.wait_group 1;" ::: "memory"); }
+
+// compute_pid of a row whose 8-byte key is `v`
+template <bool kSingleU64>
+__device__ __forceinline__ uint32_t pid_of_key(const FbKeys& keys, const FbDiv& dv, uint64_t v) {
+  if (kSingleU64) return fb_fastmod(fb_hash_single_u64(v), dv);
+  return (uint32_t)(v >> keys.digit_shift) & (dv.d - 1);
+}
+
+template <bool kSingleU64, int kBits, bool kStaged>
 __global__ void __launch_bounds__(kRankBlock, 2)
 fb_rank_kernel(FbKeys keys, FbDiv dv, uint32_t num, ChunkGeom g, uint32_t* __restrict__ hist,
                uint8_t* __restrict__ meta) {
   __shared__ uint16_t s_cnt[kRankWarps * 256];
+  extern __shared__ __align__(16) unsigned long long s_keys[];  // kStaged: [2][kTile]
   for (uint32_t i = threadIdx.x; i < (uint32_t)kRankWarps * 256; i += kRankBlock) s_cnt[i] = 0;
   __syncthreads();
   int64_t row0, row1;
@@ -194,12 +215,34 @@ fb_rank_kernel(FbKeys keys, FbDiv dv, uint32_t num, ChunkGeom g, uint32_t* __res
   const unsigned lt = fb_lanemask_lt();
   uint16_t* __restrict__ my = s_cnt + warp * 256;
   uint32_t acc = 0;  // thread b < num: rows of partition b in this chunk
+  const unsigned long long* __restrict__ kp = (const unsigned long long*)keys.ptr[0];
+  const uint32_t my_row0 = warp * (32 * kRankItems) + lane;  // rows my_row0 + r * 32 of every tile
+  if constexpr (kStaged) {
+#pragma unroll
+    for (int r = 0; r < kRankItems; ++r) cp_async8(s_keys + my_row0 + r * 32, kp + row0 + my_row0 + r * 32);
+    cp_async_commit();
+  }
+  uint32_t stage = 0;
   for (int64_t t0 = row0; t0 < row1; t0 += kTile) {
     uint8_t* __restrict__ rec = meta + (size_t)(t0 / kTile) * kMetaBytes;
     uint32_t pid[kRankItems], pos[kRankItems];
+    if constexpr (kStaged) {
+      // the other slot was read back during the previous tile: refill it with the next tile's keys
+      if (t0 + kTile < row1) {
+        unsigned long long* nxt = s_keys + (stage ^ 1) * kTile;
 #pragma unroll
-    for (int r = 0; r < kRankItems; ++r)
-      pid[r] = compute_pid<kSingleU64>(keys, dv, t0 + warp * (32 * kRankItems) + r * 32 + lane);
+        for (int r = 0; r < kRankItems; ++r) cp_async8(nxt + my_row0 + r * 32, kp + t0 + kTile + my_row0 + r * 32);
+      }
+      cp_async_commit();  // possibly empty: the group of this tile is then always the one before the last
+      cp_async_wait_one();
+      const unsigned long long* cur = s_keys + stage * kTile;
+#pragma unroll
+      for (int r = 0; r < kRankItems; ++r) pid[r] = pid_of_key<kSingleU64>(keys, dv, cur[my_row0 + r * 32]);
+      stage ^= 1;
+    } else {
+#pragma unroll
+      for (int r = 0; r < kRankItems; ++r) pid[r] = compute_pid<kSingleU64>(keys, dv, t0 + my_row0 + r * 32);
+    }
     unsigned mm[kRankItems];
 #pragma unroll
     for (int r = 0; r < kRankItems; ++r) mm[r] = match_lanes<kBits>(pid[r], 0xFFFFFFFFu);
@@ -592,6 +635,11 @@ __device__ __forceinline__ uint64_t l2_policy_evict_first() {
   asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
   return pol;
 }
+__device__ __forceinline__ uint64_t l2_policy_evict_last() {
+  uint64_t pol;
+  asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol));
+  return pol;
+}
 // 1-D bulk copy global -> shared, completion signalled on an mbarrier (TMA engine; SASS: UBLKCP)
 __device__ __forceinline__ void tma_load_1d(uint32_t dst_smem, const void* src, uint32_t bytes, uint32_t bar,
                                             uint64_t policy) {
@@ -629,10 +677,16 @@ constexpr int kWsThreads = kWsMovers + kWsRankers + 128;  // + producer warpgrou
 constexpr int kWsG = 4;  // rows per write-combined group (32 B); 8 (64 B) was slower: spills, 3 ring stages
 constexpr int kWsRankItems = 16;  // rows per ranker thread per tile: tile = 256 x 16 = 4096 rows (2048: no faster)
 
+// The units of every column group of one launch.  Group k holds units [k * per_group, min(nunits,
+// (k + 1) * per_group)).  CTA b moves group b % ngroups over chunks b / ngroups, + S, + 2S, ... with
+// S = gridDim.x / ngroups, so the ngroups CTAs of one chunk run side by side on the same tile sequence
+// and every rank record is fetched from HBM about once (the siblings find it in L2).
 struct WsUnits {
-  const uint64_t* src[kSwcMaxCols];
-  uint64_t* dst[kSwcMaxCols];
+  const uint64_t* src[FB_MAX_COLS];
+  uint64_t* dst[FB_MAX_COLS];
   int32_t nunits;
+  int32_t per_group;  // <= kSwcMaxCols: carry buffers in shared memory
+  int32_t ngroups;
 };
 
 // K4, the fused map epilogue: output unit u is not a copy of src[u] but an affine function of one or
@@ -641,10 +695,10 @@ struct WsUnits {
 //                     exactly what the expression evaluator (K8) gives for `x * a + y * b + c`
 //   mode 2 (int64)  : a * x + b * y + c  (wrapping)
 // src2 == nullptr: y does not exist (b ignored).  A two-operand unit occupies two ring stages.
-struct WsMap {
-  const uint64_t* src2[kSwcMaxCols];
-  uint64_t a[kSwcMaxCols], b[kSwcMaxCols], c[kSwcMaxCols];
-  int32_t mode[kSwcMaxCols];
+struct WsMap {  // indexed like WsUnits
+  const uint64_t* src2[FB_MAX_COLS];
+  uint64_t a[FB_MAX_COLS], b[FB_MAX_COLS], c[FB_MAX_COLS];
+  int32_t mode[FB_MAX_COLS];
 };
 
 __device__ __forceinline__ uint64_t ws_apply_map(int mode, bool two, uint64_t x, uint64_t y, uint64_t a, uint64_t b,
@@ -694,7 +748,11 @@ fb_scatter_ws_kernel(WsUnits units, uint32_t num, ChunkGeom g, int nstages,
   extern __shared__ __align__(128) uint64_t smem64[];
   const uint32_t nbp = nb_padded(num);
   const uint32_t E = num * GM;
-  const int ncols = units.nunits;
+  // this CTA's column group (units u0 .. u0 + ncols) and chunk sequence (chunk_first, + chunk_step, ...)
+  const int grp = (int)blockIdx.x % units.ngroups;
+  const int chunk_first = (int)blockIdx.x / units.ngroups, chunk_step = (int)gridDim.x / units.ngroups;
+  const int u0 = grp * units.per_group;
+  const int ncols = min(units.per_group, units.nunits - u0);
   uint64_t* ring = smem64;
   uint64_t* bars = ring + (size_t)nstages * T;
   uint64_t* carry = bars + 64;
@@ -740,11 +798,14 @@ fb_scatter_ws_kernel(WsUnits units, uint32_t num, ChunkGeom g, int nstages,
   if (warp >= kWsMoverWarps + kWsRankWarps) {
     // ============================ producer =============================================
     if (warp == kWsMoverWarps + kWsRankWarps && lane == 0) {
-      const uint64_t pol = l2_policy_evict_first();
+      // the payload is read once: evict first.  A rank record is read by every group of its chunk: kept
+      // in L2 for the sibling CTAs (H100 at 400 W, 100 M rows x 8 columns in 4 groups: records loaded
+      // evict_first 5.94 ms, evict_normal 5.77, evict_last 5.59; MEASUREMENTS.md)
+      const uint64_t pol = l2_policy_evict_first(), meta_pol = l2_policy_evict_last();
       const uint32_t ring_s = smem_u32(ring), meta_s = smem_u32(metabuf);
       uint32_t s = 0, ph = 0, seq = 0;
       // pids of the very first tile
-      int chunk = (int)blockIdx.x;
+      int chunk = chunk_first;
       int64_t r0 = 0, r1 = 0, t0 = 0;
       bool have = chunk < g.nchunks_full;
       if (have) { chunk_range(g, chunk, r0, r1); t0 = r0; }
@@ -753,7 +814,7 @@ fb_scatter_ws_kernel(WsUnits units, uint32_t num, ChunkGeom g, int nstages,
         mbar_wait(bar_pid_empty + 8 * b, pp ^ 1);
         mbar_expect_tx(bar_pid_full + 8 * b, kMetaBytes);
         tma_load_1d(meta_s + b * kMetaBytes, meta + (size_t)(row0 / T) * kMetaBytes, kMetaBytes,
-                    bar_pid_full + 8 * b, pol);
+                    bar_pid_full + 8 * b, meta_pol);
       };
       if (have) load_pid(t0, 0);
       while (have) {
@@ -762,12 +823,12 @@ fb_scatter_ws_kernel(WsUnits units, uint32_t num, ChunkGeom g, int nstages,
         int64_t nr0 = r0, nr1 = r1, nt0 = t0 + T;
         bool nhave = true;
         if (nt0 >= r1) {
-          nchunk = chunk + (int)gridDim.x;
+          nchunk = chunk + chunk_step;
           nhave = nchunk < g.nchunks_full;
           if (nhave) { chunk_range(g, nchunk, nr0, nr1); nt0 = nr0; }
         }
         if (nhave) load_pid(nt0, seq + 1);
-        for (int u = 0; u < ncols; ++u) {
+        for (int u = u0; u < u0 + ncols; ++u) {
           mbar_wait(bar_empty + 8 * s, ph ^ 1);
           mbar_expect_tx(bar_full + 8 * s, kStageBytes);
           tma_load_1d(ring_s + s * kStageBytes, units.src[u] + t0, kStageBytes, bar_full + 8 * s, pol);
@@ -793,7 +854,7 @@ fb_scatter_ws_kernel(WsUnits units, uint32_t num, ChunkGeom g, int nstages,
     const unsigned rw = warp - kWsMoverWarps;          // ranker warp 0..7
     const unsigned rtid = threadIdx.x - kWsMovers;     // 0..255
     uint32_t seq = 0, cseq = 0;
-    for (int chunk = (int)blockIdx.x; chunk < g.nchunks_full; chunk += (int)gridDim.x, ++cseq) {
+    for (int chunk = chunk_first; chunk < g.nchunks_full; chunk += chunk_step, ++cseq) {
       int64_t r0, r1;
       chunk_range(g, chunk, r0, r1);
       if (cseq > 0) mbar_wait(bar_flush_done, (cseq - 1) & 1);  // movers flushed the previous chunk
@@ -899,7 +960,7 @@ fb_scatter_ws_kernel(WsUnits units, uint32_t num, ChunkGeom g, int nstages,
 
   // ================================ movers (16 warps) ====================================
   uint32_t s = 0, ph = 0, seq = 0, astep = 0, wstep = 0;
-  for (int chunk = (int)blockIdx.x; chunk < g.nchunks_full; chunk += (int)gridDim.x) {
+  for (int chunk = chunk_first; chunk < g.nchunks_full; chunk += chunk_step) {
     int64_t r0, r1;
     chunk_range(g, chunk, r0, r1);
     for (int64_t t0 = r0; t0 < r1; t0 += T, ++seq) {
@@ -932,7 +993,7 @@ fb_scatter_ws_kernel(WsUnits units, uint32_t num, ChunkGeom g, int nstages,
       for (int u = 0; u < ncols; ++u) {
         mbar_wait(bar_full + 8 * s, ph);
         const uint64_t* __restrict__ st = ring + (size_t)s * T;
-        uint64_t* __restrict__ out = units.dst[u];
+        uint64_t* __restrict__ out = units.dst[u0 + u];
         const uint64_t* __restrict__ cbuf = carry + (size_t)u * E;
         uint64_t v[kSlotRounds], cv[kEntryRoundsM];
         uint32_t s2 = s;
@@ -940,15 +1001,15 @@ fb_scatter_ws_kernel(WsUnits units, uint32_t num, ChunkGeom g, int nstages,
         if constexpr (kMap) {
           // fused map (K4): rows taken from the staged tile(s) are mapped here; carry entries already are
           // output values
-          const int mode = map.mode[u];
-          two = map.src2[u] != nullptr;
+          const int mode = map.mode[u0 + u];
+          two = map.src2[u0 + u] != nullptr;
           const uint64_t* __restrict__ st2 = st;
           if (two) {
             s2 = s + 1 == (uint32_t)nstages ? 0 : s + 1;
             mbar_wait(bar_full + 8 * s2, s2 == 0 ? ph ^ 1 : ph);
             st2 = ring + (size_t)s2 * T;
           }
-          const uint64_t ma = map.a[u], mb = map.b[u], mc = map.c[u];
+          const uint64_t ma = map.a[u0 + u], mb = map.b[u0 + u], mc = map.c[u0 + u];
 #pragma unroll
           for (int k = 0; k < kSlotRounds; ++k)
             if (srcd[k] != 0xFFFFu)
@@ -1008,7 +1069,7 @@ fb_scatter_ws_kernel(WsUnits units, uint32_t num, ChunkGeom g, int nstages,
     // ---- chunk end: flush the pending rows (partial sector groups)
     mover_sync();
     for (int u = 0; u < ncols; ++u) {
-      uint64_t* __restrict__ out = units.dst[u];
+      uint64_t* __restrict__ out = units.dst[u0 + u];
       const uint64_t* __restrict__ cbuf = carry + (size_t)u * E;
 #pragma unroll
       for (int q = 0; q < kEntryRoundsM; ++q) {
@@ -1103,6 +1164,10 @@ cudaError_t ensure_smem_optin(int dev) {
     if (e == cudaSuccess) e = optin(fb_scatter_ws_kernel<4, kWsG, kWsRankItems, true>, (size_t)smem_max);
     if (e == cudaSuccess) e = optin(fb_scatter_ws_kernel<8, kWsG, kWsRankItems, true>, (size_t)smem_max);
   }
+  if (e == cudaSuccess) e = optin(fb_rank_kernel<true, 4, true>, kRankStageBytes);
+  if (e == cudaSuccess) e = optin(fb_rank_kernel<true, 8, true>, kRankStageBytes);
+  if (e == cudaSuccess) e = optin(fb_rank_kernel<false, 4, true>, kRankStageBytes);
+  if (e == cudaSuccess) e = optin(fb_rank_kernel<false, 8, true>, kRankStageBytes);
   FB_OPTIN(true, 4); FB_OPTIN(true, 8); FB_OPTIN(true, 10);
   FB_OPTIN(false, 4); FB_OPTIN(false, 8); FB_OPTIN(false, 10);
 #undef FB_OPTIN
@@ -1224,13 +1289,20 @@ static int plan_impl(int dev, void* stream, int64_t nrows, const FbKeys& k, bool
   int hist_chunk0 = 0;
   if (num_partitions <= kSwcMaxNum && g.nchunks_full > 0) {
     uint8_t* meta = (uint8_t*)scratch + l.pid_offset;
+#define FB_LAUNCH_RANK(S, B, STAGED)                                                                  \
+  fb_rank_kernel<S, B, STAGED><<<g.nchunks_full, kRankBlock, STAGED ? kRankStageBytes : 0, st>>>( \
+      k, dv, num_partitions, g, hist, meta)
     if (single) {
-      if (bits == 4) fb_rank_kernel<true, 4><<<g.nchunks_full, kRankBlock, 0, st>>>(k, dv, num_partitions, g, hist, meta);
-      else fb_rank_kernel<true, 8><<<g.nchunks_full, kRankBlock, 0, st>>>(k, dv, num_partitions, g, hist, meta);
+      if (bits == 4) FB_LAUNCH_RANK(true, 4, true);
+      else FB_LAUNCH_RANK(true, 8, true);
+    } else if (k.digit_shift >= 0) {
+      if (bits == 4) FB_LAUNCH_RANK(false, 4, true);
+      else FB_LAUNCH_RANK(false, 8, true);
     } else {
-      if (bits == 4) fb_rank_kernel<false, 4><<<g.nchunks_full, kRankBlock, 0, st>>>(k, dv, num_partitions, g, hist, meta);
-      else fb_rank_kernel<false, 8><<<g.nchunks_full, kRankBlock, 0, st>>>(k, dv, num_partitions, g, hist, meta);
+      if (bits == 4) FB_LAUNCH_RANK(false, 4, false);
+      else FB_LAUNCH_RANK(false, 8, false);
     }
+#undef FB_LAUNCH_RANK
     FB_CUDA(cudaGetLastError());
     hist_chunk0 = g.nchunks_full;
   }
@@ -1362,42 +1434,52 @@ static int apply_impl(int dev, void* stream, int64_t nrows, const FbKeys& k, boo
   if (nfast > 0) {
     int smem_max = 0;
     FB_CUDA(cudaDeviceGetAttribute(&smem_max, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
-    int grid = fb_sm_count(dev) < g.nchunks_full ? fb_sm_count(dev) : g.nchunks_full;
     // sm_reserve: SMs left free for kernels that must co-run with this persistent one (the
     // multi-GPU barrier / pull kernels: a scatter CTA owns the whole register file of its SM)
-    if (sm_reserve > 0 && grid > fb_sm_count(dev) - sm_reserve) grid = fb_sm_count(dev) - sm_reserve;
-    if (grid < 1) grid = 1;
+    int avail = fb_sm_count(dev) - sm_reserve;
+    if (avail < 1) avail = 1;
     const uint8_t* pid_plane = (const uint8_t*)scratch + l.pid_offset;  // rank records of pass 1
-    // measured on H100 (100 M rows x 8 cols, columns per launch; MEASUREMENTS.md): 8 -> 6.54 ms, 4 -> 6.28,
-    // 3 -> 6.00, 2 -> 5.84, 1 -> 6.29 (fewer open write streams: half-written lines meet their other half while still in the
-    // 50 MB L2; every launch pays a ramp + rank-record traffic).  Groups of at most 2, evenly sized.
-    const int ngroups = (nfast + 1) / 2;
-    int cols_per_launch = (nfast + ngroups - 1) / ngroups;
-    if (cols_per_launch_req >= 1 && cols_per_launch_req <= kSwcMaxCols) cols_per_launch = cols_per_launch_req;
-    for (int c0 = 0; c0 < nfast; c0 += cols_per_launch) {
-      const int nb = nfast - c0 < cols_per_launch ? nfast - c0 : cols_per_launch;
+    // Column groups of at most 2, evenly sized.  Measured on H100 (100 M rows x 8 cols; MEASUREMENTS.md), one
+    // launch per group at 700 W: 8 columns per group -> 6.54 ms, 4 -> 6.28, 3 -> 6.00, 2 -> 5.84, 1 -> 6.29; one
+    // launch at 400 W: 4 -> 6.25, 2 -> 5.56, 1 -> 5.88.  With more than 2 columns in flight per CTA, half-written
+    // lines no longer meet their other half in the 50 MB L2.
+    int ngroups = (nfast + 1) / 2;
+    int per_group = (nfast + ngroups - 1) / ngroups;
+    if (cols_per_launch_req >= 1 && cols_per_launch_req <= kSwcMaxCols) per_group = cols_per_launch_req;
+    ngroups = (nfast + per_group - 1) / per_group;
+    const size_t book = ws_book_bytes<kWsG, kWsRankItems>(num_partitions, per_group);
+    const size_t stage_bytes = (size_t)kWsRankers * kWsRankItems * 8;
+    int nstages = (int)(((size_t)smem_max - book) / stage_bytes);
+    if (nstages > 16) nstages = 16;
+    FB_CHECK(nstages >= 2, "not enough shared memory for the TMA ring (%d stages)", nstages);
+    const size_t tsmem = (size_t)nstages * stage_bytes + book;
+    // All groups in one launch of ngroups x S CTAs, the ngroups CTAs of a chunk side by side (WsUnits), up to
+    // FB_MAX_COLS units per launch.  With fewer free SMs than groups: one launch per group, over all chunks.
+    const int groups_per_launch = ngroups <= avail ? (ngroups < FB_MAX_COLS / per_group ? ngroups : FB_MAX_COLS / per_group) : 1;
+    for (int g0 = 0; g0 < ngroups; g0 += groups_per_launch) {
+      const int lg = ngroups - g0 < groups_per_launch ? ngroups - g0 : groups_per_launch;
+      const int c0 = g0 * per_group;
+      const int nu = nfast - c0 < lg * per_group ? nfast - c0 : lg * per_group;
       WsUnits wu;
+      WsMap wm;
       memset(&wu, 0, sizeof(wu));
-      wu.nunits = nb;
-      for (int c = 0; c < nb; ++c) {
+      memset(&wm, 0, sizeof(wm));
+      wu.nunits = nu;
+      wu.per_group = per_group;
+      wu.ngroups = lg;
+      for (int c = 0; c < nu; ++c) {
         wu.src[c] = (const uint64_t*)col_ptrs[fast_idx[c0 + c]];
         wu.dst[c] = (uint64_t*)out_col_ptrs[fast_idx[c0 + c]];
-      }
-      const size_t book = ws_book_bytes<kWsG, kWsRankItems>(num_partitions, nb);
-      const size_t stage_bytes = (size_t)kWsRankers * kWsRankItems * 8;
-      int nstages = (int)(((size_t)smem_max - book) / stage_bytes);
-      if (nstages > 16) nstages = 16;
-      FB_CHECK(nstages >= 2, "not enough shared memory for the TMA ring (%d stages)", nstages);
-      const size_t tsmem = (size_t)nstages * stage_bytes + book;
-      WsMap wm;
-      memset(&wm, 0, sizeof(wm));
-      if (maps != nullptr) {
-        for (int c = 0; c < nb; ++c) {
+        if (maps != nullptr) {
           const fb_map_unit& m = maps[fast_idx[c0 + c]];
           wm.src2[c] = (const uint64_t*)m.src2;
           wm.a[c] = m.a; wm.b[c] = m.b; wm.c[c] = m.c;
           wm.mode[c] = m.mode;
         }
+      }
+      const int64_t ctas = avail < (int64_t)lg * g.nchunks_full ? avail : (int64_t)lg * g.nchunks_full;
+      const int grid = (int)(ctas / lg) * lg;
+      if (maps != nullptr) {
         if (bits == 4)
           fb_scatter_ws_kernel<4, kWsG, kWsRankItems, true><<<grid, kWsThreads, tsmem, st>>>(
               wu, num_partitions, g, nstages, pid_plane, (const uint32_t*)scratch, part_offsets, wm);

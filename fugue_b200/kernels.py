@@ -97,7 +97,8 @@ def partition_apply(plan: PartitionPlan, cols: Sequence[torch.Tensor],
                     out: Optional[Sequence[torch.Tensor]] = None, sm_reserve: int = 0, cols_per_launch: int = 0
                     ) -> List[torch.Tensor]:
     """Pass 2 for ``cols``; ``sm_reserve`` SMs stay free for kernels that co-run (multi-GPU exchange);
-    ``cols_per_launch`` is a tuning argument of the fast kernel (0 = default)."""
+    ``cols_per_launch`` is a tuning argument of the fast kernel: 8-byte columns per group, all groups in one
+    launch (0 = default, 2)."""
     lib = _lib.load()
     dev, n = _check_cols(list(cols) + plan.keys)
     if out is None:

@@ -98,7 +98,10 @@ int fb_partition_apply(int dev, void* stream, int64_t nrows, int nkeys,
 
 /* fb_partition_apply with tuning arguments (0 = default for each).  `sm_reserve` SMs left free: the fast scatter kernel is persistent and a
  * CTA owns its SM's whole register file, so a kernel that must run at the same time (the multi-GPU
- * barrier / pull kernels of the exchange that overlaps the next column group) needs SMs of its own. */
+ * barrier / pull kernels of the exchange that overlaps the next column group) needs SMs of its own.
+ * `cols_per_launch` is the number of 8-byte columns per group of the fast kernel (default 2).  All groups
+ * run side by side in one launch, one group per CTA; when fewer than one SM per group is left free, each
+ * group gets a launch of its own.  The name is kept for ABI compatibility. */
 int fb_partition_apply_ex(int dev, void* stream, int64_t nrows, int nkeys,
                           const void* const* key_ptrs, const int32_t* key_widths,
                           const uint8_t* const* key_valid, uint32_t num_partitions,
@@ -106,7 +109,7 @@ int fb_partition_apply_ex(int dev, void* stream, int64_t nrows, int nkeys,
                           const int64_t* part_offsets, int ncols,
                           const void* const* col_ptrs, const int32_t* col_widths,
                           void* const* out_col_ptrs, int sm_reserve,
-                          int cols_per_launch /* 8-byte columns per launch of the fast kernel, 1..8 */);
+                          int cols_per_launch /* 8-byte columns per group of the fast kernel, 1..8 */);
 
 /* K4  fused map epilogue: fb_partition_apply whose output column c is not a copy of col_ptrs[c] but
  *   mode 1 (float64): (a * x + b * y) + c    mode 2 (int64): a * x + b * y + c (wrapping)    mode 0: x

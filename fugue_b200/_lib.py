@@ -98,6 +98,9 @@ SIGNATURES = {
                                _i32p, _vpp, _vpp]),
     "fb_copy_segments": (C.c_int, [C.c_int, _vp, C.c_int, _vp, _vp, _vp, C.c_int, _vp, _vp, _vp, _vp,
                                    C.c_int64]),
+    "fb_segmented_scan_scratch_bytes": (C.c_size_t, [C.c_int64, C.c_int]),
+    "fb_segmented_scan": (C.c_int, [C.c_int, _vp, C.c_int64, C.c_int64, _vp, C.c_int, _i32p, _vpp, _vpp, _vpp,
+                                    _vpp, _vp, C.c_size_t]),
 }
 
 

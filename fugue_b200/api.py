@@ -406,7 +406,11 @@ def transform(
     if tf.has_input_rules:     # needs the input schema: only then is a native input looked at here
         tf.validate_on_runtime(get_schema(df))
     res: Optional[DataFrame] = None
-    if as_local and tf.get_format_hint() == "b200" and not isinstance(df, (B200DataFrame, B200Table)):
+    from .colmap import ColumnMap
+
+    windowed = isinstance(using, ColumnMap) and using.has_window  # needs the sort of map_dataframe
+    if as_local and tf.get_format_hint() == "b200" and not isinstance(df, (B200DataFrame, B200Table)) \
+            and not windowed:
         # host input, host output, device function: overlap H2D / partition (/ exchange) / D2H column by column
         from .streaming import streaming_transform
 
@@ -562,12 +566,15 @@ def raw_sql(*statements: Any, engine: Any = None, engine_conf: Any = None, as_fu
             as_local: bool = False) -> Any:
     """``fa.raw_sql`` (fugue/sql/api.py): strings and dataframes interleaved, e.g.
     ``fa.raw_sql("SELECT key, SUM(v0) AS s, COUNT(*) AS c FROM", df, "GROUP BY key")``."""
+    from .column import has_window
     from .sql import StructuredRawSQL
 
     e = make_execution_engine(engine, engine_conf, infer_by=[s for s in statements if not isinstance(s, str)])
     dfs: Dict[str, Any] = {}
     pieces = []
     for s in statements:
+        assert_or_throw(not has_window(s), lambda: NotImplementedError(
+            f"{s}: window functions are not part of the SQL dialect; use them in a ColumnMap of fa.transform"))
         if isinstance(s, str):
             pieces.append((False, s))
         else:

@@ -7,6 +7,9 @@ from an expression is a function of ``(kind, head, args)``:
     LITERAL   head = python value (None = NULL)      UNARY     head in ``- ~ IS_NULL NOT_NULL``, one arg
     BINARY    head in ``+ - * / & | < > <= >= == !=``  CALL      head = function name (``COALESCE`` ...)
     AGG       head in ``SUM COUNT AVG MIN MAX FIRST LAST``, one arg, optional DISTINCT
+    WINDOW    head in the AGG functions (one arg, kwargs ``running``), ``ROW_NUMBER RANK DENSE_RANK`` (no
+              arg) or ``LAG LEAD`` (one arg, kwargs ``n`` and ``default``): evaluated over the logical
+              partitions of ``fa.transform`` (PartitionSpec keys, presort order) by a ``ColumnMap``
 
 plus an optional output alias and an optional cast of the node's result.  ``fugue_b200/expr.py`` compiles
 these trees into programs for the device evaluator (``fb_eval_expr``); nothing goes through SQL text.
@@ -36,11 +39,15 @@ class Kind(enum.IntEnum):
     BINARY = 4
     CALL = 5
     AGG = 6
+    WINDOW = 7
 
 
 BOOL_OPS = frozenset(["&", "|", "<", ">", "<=", ">=", "==", "!="])
 ARITH_OPS = frozenset(["+", "-", "*", "/"])
 AGG_KEEPS_ARG_TYPE = frozenset(["MIN", "MAX", "FIRST", "LAST"])
+WINDOW_AGGS = frozenset(["SUM", "COUNT", "AVG", "MIN", "MAX", "FIRST", "LAST"])
+_RANKINGS = frozenset(["ROW_NUMBER", "RANK", "DENSE_RANK"])
+_RUNNING_FRAME = "ROWS BETWEEN UNBOUNDED PRECEDING AND CURRENT ROW"
 _LITERAL_TYPES = (int, bool, float, str)
 
 
@@ -115,12 +122,12 @@ class ColumnExpr:
 
     @property
     def func(self) -> str:
-        assert self.kind in (Kind.UNARY, Kind.BINARY, Kind.CALL, Kind.AGG)
+        assert self.kind in (Kind.UNARY, Kind.BINARY, Kind.CALL, Kind.AGG, Kind.WINDOW)
         return self.head
 
     @property
     def arg(self) -> "ColumnExpr":
-        assert self.kind in (Kind.UNARY, Kind.AGG)
+        assert self.kind in (Kind.UNARY, Kind.AGG, Kind.WINDOW) and len(self.args) == 1
         return self.args[0]
 
     col = arg  # operand of a unary operator
@@ -137,7 +144,7 @@ class ColumnExpr:
 
     @property
     def has_args(self) -> bool:
-        return self.kind in (Kind.UNARY, Kind.BINARY, Kind.CALL, Kind.AGG)
+        return self.kind in (Kind.UNARY, Kind.BINARY, Kind.CALL, Kind.AGG, Kind.WINDOW)
 
     @property
     def output_name(self) -> str:
@@ -166,6 +173,8 @@ class ColumnExpr:
             return self.alias(self.head) if (self.as_name == "" and self.as_type is not None) else self
         if self.kind in (Kind.UNARY, Kind.AGG) and self.as_name == "":
             return self.alias(self.args[0].infer_alias().output_name)
+        if self.kind == Kind.WINDOW and self.as_name == "" and self.args and self.args[0].kind != Kind.WILDCARD:
+            return self.alias(self.args[0].infer_alias().output_name)
         return self
 
     def infer_type(self, schema: Schema) -> Optional[pa.DataType]:
@@ -188,6 +197,15 @@ class ColumnExpr:
             return tp if fits else None
         if k == Kind.AGG and self.head in AGG_KEEPS_ARG_TYPE:
             return self.args[0].infer_type(schema)
+        if k == Kind.WINDOW:
+            if self.head in _RANKINGS or self.head == "COUNT":
+                return pa.int64()
+            if self.head == "AVG":
+                return pa.float64()
+            tp = self.args[0].infer_type(schema)
+            if self.head == "SUM" and tp is not None:
+                return pa.float64() if pa.types.is_floating(tp) else pa.int64()
+            return tp  # SUM of an unknown type: None; MIN MAX FIRST LAST LAG LEAD keep the argument's type
         return None
 
     # ---- text -------------------------------------------------------------------------------------
@@ -199,6 +217,8 @@ class ColumnExpr:
             return "*"
         if k == Kind.LITERAL:
             return _show_literal(self.head)
+        if k == Kind.WINDOW:
+            return _window_text(self, _show_arg)
         parts = [_show_arg(x) for x in self.args] + [n + "=" + _show_arg(v) for n, v in self.kwargs.items()]
         return f"{self.head}({'DISTINCT ' if self.is_distinct else ''}{','.join(parts)})"
 
@@ -233,6 +253,24 @@ class ColumnExpr:
 
     def __invert__(self) -> "ColumnExpr":
         return ColumnExpr(Kind.UNARY, "~", [self])
+
+    def over(self, running: bool = False) -> "ColumnExpr":
+        """The aggregation as a window function of a ``ColumnMap``: over the whole logical partition
+        (``running=False``, the value repeated on every row) or over the rows up to and including the
+        current one in presort order (``running=True``)."""
+        if self.kind != Kind.AGG:
+            raise ValueError(f"{self} is not an aggregation: only an aggregation has an OVER form")
+        if self.is_distinct:
+            raise ValueError(f"{self}: DISTINCT aggregations have no window form")
+        if self.head not in WINDOW_AGGS:
+            raise ValueError(f"{self}: {self.head} has no window form")
+        if not isinstance(running, bool):
+            raise ValueError(f"running must be a bool, got {running!r}")
+        if is_agg(self.args[0]) or has_window(self.args[0]):
+            raise ValueError(f"nested aggregation {self}")
+        if self.head in ("FIRST", "LAST") and self.args[0].kind == Kind.WILDCARD:
+            raise ValueError(f"{self}: {self.head} needs a column")
+        return ColumnExpr(Kind.WINDOW, self.head, self.args, {"running": running}, False, self.as_name, self.as_type)
 
     def __bool__(self) -> bool:
         raise TypeError("a column expression has no truth value; use & | ~ to combine conditions")
@@ -308,7 +346,38 @@ def is_agg(column: Any) -> bool:
         return False
     if column.kind == Kind.AGG:
         return True
+    if column.kind == Kind.WINDOW:  # a window function is evaluated per row: not a GROUP BY aggregation
+        return False
     return any(is_agg(x) for x in column.args) or any(is_agg(x) for x in column.kwargs.values())
+
+
+def has_window(column: Any) -> bool:
+    """True when the expression contains a window function anywhere."""
+    if not isinstance(column, ColumnExpr):
+        return False
+    if column.kind == Kind.WINDOW:
+        return True
+    return any(has_window(x) for x in column.args) or any(has_window(x) for x in column.kwargs.values())
+
+
+def _window_text(e: ColumnExpr, show: Any) -> str:
+    """``FUNC(args) OVER (frame)`` of a WINDOW node; ``show`` renders one argument."""
+    parts = [show(x) for x in e.args]
+    if e.head in ("LAG", "LEAD"):
+        parts += [str(e.kwargs["n"]), _show_literal(e.kwargs["default"])]
+    frame = _RUNNING_FRAME if e.kwargs.get("running", False) else ""
+    return f"{e.head}({','.join(parts)}) OVER ({frame})"
+
+
+def _offset_fn(name: str, c: Any, n: Any, default: Any) -> ColumnExpr:
+    if isinstance(n, bool) or not isinstance(n, int) or n < 0:
+        raise ValueError(f"{name}: n must be a non-negative int, got {n!r}")
+    if not (default is None or isinstance(default, _LITERAL_TYPES)):
+        raise ValueError(f"{name}: default must be a literal or None, got {default!r}")
+    arg = col(c)
+    if arg.kind == Kind.WILDCARD or is_agg(arg) or has_window(arg):
+        raise ValueError(f"{name} needs a row-wise column expression, got {arg}")
+    return ColumnExpr(Kind.WINDOW, name, [arg], {"n": n, "default": default})
 
 
 def column_mentions(column: Any) -> Iterator[str]:
@@ -363,6 +432,31 @@ class functions:
 
     mean = avg
     is_agg = staticmethod(is_agg)
+
+    @staticmethod
+    def row_number() -> ColumnExpr:
+        """1, 2, ... in presort order inside every logical partition of ``fa.transform``."""
+        return ColumnExpr(Kind.WINDOW, "ROW_NUMBER")
+
+    @staticmethod
+    def rank() -> ColumnExpr:
+        """SQL RANK: the row number of the first of the current row's peers (equal on every presort column)."""
+        return ColumnExpr(Kind.WINDOW, "RANK")
+
+    @staticmethod
+    def dense_rank() -> ColumnExpr:
+        """SQL DENSE_RANK: 1 + the number of distinct peer groups before the current row's."""
+        return ColumnExpr(Kind.WINDOW, "DENSE_RANK")
+
+    @staticmethod
+    def lag(c: Any, n: int = 1, default: Any = None) -> ColumnExpr:
+        """``c`` of the row ``n`` rows earlier in the same logical partition, else ``default``."""
+        return _offset_fn("LAG", c, n, default)
+
+    @staticmethod
+    def lead(c: Any, n: int = 1, default: Any = None) -> ColumnExpr:
+        """``c`` of the row ``n`` rows later in the same logical partition, else ``default``."""
+        return _offset_fn("LEAD", c, n, default)
 
 
 # ---- one SELECT list ------------------------------------------------------------------------------
@@ -465,6 +559,8 @@ def to_sql(expr: ColumnExpr, enable_cast: bool = True, nested: bool = False) -> 
         inner = to_sql(expr.args[0], enable_cast, True)
         body = {"-": "-" + inner, "~": "NOT " + inner, "IS_NULL": inner + " IS NULL",
                 "NOT_NULL": inner + " IS NOT NULL"}[expr.head]
+    elif k == Kind.WINDOW:
+        body = _window_text(expr, lambda x: to_sql(_operand(x), enable_cast))
     elif k == Kind.BINARY:
         if expr.head not in BOOL_OPS and expr.head not in ARITH_OPS:
             raise NotImplementedError(expr)

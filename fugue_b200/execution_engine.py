@@ -100,7 +100,19 @@ class B200MapEngine:
         if on_init is not None:
             on_init(0, edf)
         keyed = len(partition_spec.partition_by) > 0 and not is_coarse
-        if map_func_format_hint == "b200" and len(presort) > 0:
+        cmap = getattr(map_func, "column_map", None)
+        windowed = map_func_format_hint == "b200" and cmap is not None and cmap.has_window
+        if windowed:
+            # window functions (K9) need every logical partition contiguous and in presort order on one device
+            assert_or_throw(not is_coarse, NotImplementedError(
+                "window functions over algo='coarse' partitions: a coarse partition is not a logical partition"))
+            assert_or_throw(keyed or partition_spec.num_partitions == "0", NotImplementedError(
+                "window functions without partition keys but with num: the partitions of a key-less split are "
+                "not logical partitions; give keys, or no num for one partition over the whole table"))
+            assert_or_throw(not self.is_distributed, NotImplementedError(
+                "window functions on the multi-GPU engine: the presort is local to each rank before the shuffle, "
+                "so rows of one key from different ranks would not be merged in presort order"))
+        if map_func_format_hint == "b200" and (len(presort) > 0 or windowed):
             # device presort: sort by (partition keys, presort) first; the stable hash partition below
             # keeps that order inside every physical partition, so logical partitions (distinct key
             # tuples) come out contiguous and presorted; their boundaries go to table.logical_offsets
@@ -112,8 +124,7 @@ class B200MapEngine:
             for k, v in presort.items():
                 order[k] = v
             edf = B200DataFrame(S.sort_table(edf.native, order))
-        cmap = getattr(map_func, "column_map", None)
-        if keyed and cmap is not None and map_func_format_hint == "b200" and len(presort) == 0:
+        if keyed and cmap is not None and map_func_format_hint == "b200" and len(presort) == 0 and not windowed:
             fused = engine._repartition_fused_map(edf, partition_spec, cmap, output_schema)  # K4
             if fused is not None:
                 return fused
@@ -123,12 +134,19 @@ class B200MapEngine:
             # device-vectorised map: the function is typed on B200Table and is called once per
             # device table, the physical partitions delimited by table.offsets (after a multi-GPU
             # shuffle: by table.segment_offsets, one segment per source rank and partition)
-            if len(presort) > 0 and keyed:
+            if (len(presort) > 0 or windowed) and keyed:
                 from . import sort as S
 
                 if edf.native.segment_offsets is not None:
                     edf = B200DataFrame(edf.native.compacted())
                 edf.native.logical_offsets = S.logical_offsets(edf.native, partition_spec.partition_by)
+            if windowed:
+                t = edf.native
+                t = B200Table(t.schema, t.columns, t.valid, t.dictionaries, t.offsets, t.partition_keys)
+                t.logical_offsets = edf.native.logical_offsets if keyed else \
+                    torch.tensor([0, t.num_rows], dtype=torch.int64, device=t.device)
+                t.logical_order = list(presort.keys())
+                edf = B200DataFrame(t)
             cursor.set(lambda: edf.peek_array(), 0, 0)
             out = map_func(cursor, edf)
             res = engine.to_df(out)
@@ -702,8 +720,11 @@ class B200ExecutionEngine(EngineLifecycle):
         SQL text.  Pins: fugue_test/execution_suite.py:98-155."""
         from . import expr as X
         from . import relational as R
-        from .column import ColumnExpr, Kind, SelectColumns, agg as _agg, col, is_agg
+        from .column import ColumnExpr, Kind, SelectColumns, agg as _agg, col, has_window, is_agg
 
+        for e in list(cols.all_cols) + [where, having]:
+            assert_or_throw(not has_window(e), lambda: NotImplementedError(
+                f"{e}: a window function needs PARTITION BY / ORDER BY; use it in a ColumnMap of fa.transform"))
         edf = self.to_df(df)
         t: B200Table = edf.native
         sel: SelectColumns = cols.replace_wildcard(t.schema).assert_all_with_names()
@@ -823,9 +844,11 @@ class B200ExecutionEngine(EngineLifecycle):
         """``ExecutionEngine.filter`` (execution_engine.py:808-834): rows where ``condition`` is TRUE
         (predicate evaluated on the device, stream compaction + gather).  Pins: execution_suite.py:85-95."""
         from . import expr as X
-        from .column import is_agg
+        from .column import has_window, is_agg
 
         assert_or_throw(not is_agg(condition), lambda: ValueError(f"{condition} has aggregation functions"))
+        assert_or_throw(not has_window(condition), lambda: NotImplementedError(
+            f"{condition}: a window function needs PARTITION BY / ORDER BY; use it in a ColumnMap of fa.transform"))
         edf = self.to_df(df)
         res = B200DataFrame(X.filter_table(edf.native, condition))
         if edf.has_metadata:
@@ -835,9 +858,12 @@ class B200ExecutionEngine(EngineLifecycle):
     def assign(self, df: Any, columns: List[Any]) -> B200DataFrame:
         """``ExecutionEngine.assign`` (execution_engine.py:836-887): replace / append columns.
         Pins: execution_suite.py:157-174."""
-        from .column import SelectColumns, col
+        from .column import SelectColumns, col, has_window
 
         SelectColumns(*columns).assert_no_wildcard().assert_all_with_names().assert_no_agg()
+        for c in columns:
+            assert_or_throw(not has_window(c), lambda: NotImplementedError(
+                f"{c}: a window function needs PARTITION BY / ORDER BY; use it in a ColumnMap of fa.transform"))
         edf = self.to_df(df)
         pos = {n: i for i, n in enumerate(edf.schema.names)}
         cols: List[Any] = [col(n) for n in pos]

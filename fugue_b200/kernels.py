@@ -390,6 +390,45 @@ def groupby_u64(keys: torch.Tensor, key_valid: Optional[torch.Tensor],
             [a[:ngroups] for a in out_aggs], ngroups)
 
 
+SCAN_MAX_COLS = 8
+
+
+def segmented_scan(offsets: torch.Tensor, nrows: int,
+                   columns: Sequence[Tuple[int, Optional[torch.Tensor], Optional[torch.Tensor]]]
+                   ) -> List[Tuple[Optional[torch.Tensor], torch.Tensor]]:
+    """K9: inclusive scan restarting at every segment ``[offsets[s], offsets[s + 1])``.  ``columns`` = one
+    ``(op, values or None, validity or None)`` per scan (``AGG_*`` ops; 8-byte values, none for
+    ``AGG_COUNT``).  Returns per scan ``(running op over the valid rows or None for COUNT, running count of
+    the valid rows)``; up to ``SCAN_MAX_COLS`` scans share one launch sequence."""
+    lib = _lib.load()
+    assert offsets.dtype == torch.int64 and offsets.is_cuda and offsets.is_contiguous()
+    dev = offsets.device
+    nseg = int(offsets.shape[0]) - 1
+    res: List[Tuple[Optional[torch.Tensor], torch.Tensor]] = []
+    for b in range(0, len(columns), SCAN_MAX_COLS):
+        batch = columns[b:b + SCAN_MAX_COLS]
+        outs, cnts = [], []
+        for op, v, m in batch:
+            assert (v is None) == (op == AGG_COUNT)
+            if v is not None:
+                assert v.element_size() == 8 and v.device == dev and v.is_contiguous() and v.shape[0] == nrows
+            if m is not None:
+                assert m.dtype == torch.uint8 and m.device == dev and m.is_contiguous() and m.shape[0] == nrows
+            outs.append(None if v is None else torch.empty_like(v))
+            cnts.append(torch.empty(nrows, dtype=torch.int64, device=dev))
+        nb = int(lib.fb_segmented_scan_scratch_bytes(nrows, len(batch)))
+        scratch = torch.empty(max(nb, 8), dtype=torch.uint8, device=dev)
+        _lib.check(lib.fb_segmented_scan(
+            dev.index, _stream_ptr(dev), nrows, nseg, offsets.data_ptr(), len(batch),
+            _lib.i32_array([op for op, _, _ in batch]),
+            _lib.ptr_array([0 if v is None else v.data_ptr() for _, v, _ in batch]),
+            _lib.ptr_array([0 if m is None else m.data_ptr() for _, _, m in batch]),
+            _lib.ptr_array([0 if o is None else o.data_ptr() for o in outs]),
+            _lib.ptr_array([c.data_ptr() for c in cnts]), scratch.data_ptr(), scratch.numel()))
+        res.extend(zip(outs, cnts))
+    return res
+
+
 def exclusive_scan(counts: torch.Tensor) -> Tuple[torch.Tensor, int]:
     """Exclusive prefix sum of an int64 device vector (own kernels); returns (offsets, total)."""
     lib = _lib.load()

@@ -64,6 +64,8 @@ class B200Table:
         self.partition_keys = partition_keys  # key column names the offsets refer to
         self.logical_offsets: Optional[torch.Tensor] = None  # set after a device presort: one segment
         #                                                      per distinct key tuple (logical partition)
+        self.logical_order: Optional[List[str]] = None  # presort columns the rows of a logical partition are
+        #                                                 sorted by (peers of RANK / DENSE_RANK are equal on all)
         # multi-GPU shuffle result (fugue_b200/dist.py): int64 [world, nown + 1] on the HOST; owned
         # partition j is the concatenation over source ranks s of rows
         # [segment_offsets[s, j], segment_offsets[s, j + 1]) - see compacted()

@@ -239,6 +239,29 @@ int fb_groupby_extract(int dev, void* stream, int64_t capacity, int naggs, const
                        void* const* d_out_aggs, int64_t* d_status);
 
 /* ---------------------------------------------------------------------------
+ * K9  segmented inclusive scan (window functions of a ColumnMap over the logical partitions)
+ * Replaces: the per-logical-partition pandas call of PandasMapEngine.map_dataframe
+ *             fugue/execution/native_execution_engine.py:156-164
+ *           for running totals, forward fill, ranks and partition-wide aggregates.
+ * Segment s is rows [d_offsets[s], d_offsets[s + 1]) (device, nseg + 1 int64, d_offsets[0] == 0,
+ * d_offsets[nseg] == nrows, empty segments allowed).  For every column c and row i the scan restarts at
+ * every segment start and writes, over the rows of i's segment up to and including i whose mask byte
+ * valid[c] is non-zero (valid[c] NULL: every row):
+ *   out_count[c][i]  the number of those rows (int64)
+ *   out_vals[c][i]   ops[c] over their 8-byte values vals[c]: FB_AGG_SUM_I64 (wrapping), FB_AGG_SUM_F64,
+ *                    FB_AGG_MIN/MAX_I64, FB_AGG_MIN/MAX_F64 (IEEE totalOrder, the input's own bit pattern);
+ *                    0 where the count is 0.  FB_AGG_COUNT reads no values (vals[c] may be NULL).
+ * out_vals[c] / out_count[c] may be NULL (not written).  Results are bit-identical from run to run
+ * (fixed combination order; f64 sums are not in row order).  ops, vals, valid, out_vals and out_count
+ * are HOST arrays of ncols <= FB_SCAN_MAX_COLS entries; scratch: fb_segmented_scan_scratch_bytes.
+ * --------------------------------------------------------------------------- */
+#define FB_SCAN_MAX_COLS 8
+size_t fb_segmented_scan_scratch_bytes(int64_t nrows, int ncols);
+int fb_segmented_scan(int dev, void* stream, int64_t nrows, int64_t nseg, const int64_t* d_offsets, int ncols,
+                      const int32_t* ops, const void* const* vals, const uint8_t* const* valid,
+                      void* const* out_vals, int64_t* const* out_count, void* scratch, size_t scratch_bytes);
+
+/* ---------------------------------------------------------------------------
  * K7  hash equi-join on one 8-byte key (other key shapes are packed by the host layer)
  * Replaces: NativeExecutionEngine.join -> triad PandasUtils.join -> pd.merge
  *             fugue/execution/native_execution_engine.py:230-241

@@ -101,9 +101,82 @@ def measure(device_index: int = 0):
                                   "fused_map_ms": ms_map, "partition_then_evaluator_ms": ms_unfused,
                                   "rows_per_s": n / ms_map * 1e3, "alg_GBps": (64 + 64) * n / ms_map / 1e6}
     del ucols, U
+    out["transform_window"] = measure_window(dev, e, n)
     out["transform_zipf_s1"] = {"rows": n, "ms": ms, "rows_per_s": n / ms * 1e3, "largest_partition_share":
                                 float(sizes.max()) / n, "every_row_in_its_partition": ok}
     return out
+
+
+def _card(dev):
+    """Name and power limit of the card, read in the same run as the numbers they qualify."""
+    info = {"name": torch.cuda.get_device_name(dev)}
+    try:
+        import pynvml as nv
+        nv.nvmlInit()
+        h = nv.nvmlDeviceGetHandleByIndex(dev.index)
+        info["power_limit_w"] = nv.nvmlDeviceGetPowerManagementLimit(h) / 1000.0
+    except Exception as ex:  # pragma: no cover
+        info["power_limit_w"] = f"unavailable: {type(ex).__name__}"
+    return info
+
+
+def measure_window(dev, e, n):
+    """K9: window functions over the logical partitions of the headline table (100 M rows, key over 2^16 values):
+    a running sum, a row number, a lag and a share of the partition total, PartitionSpec(by=key, presort=i1, num=256).
+    The whole call and its steps - sort by (key, presort), hash partition, window step (logical offsets, argument
+    columns, scans, gathers), evaluator - and fb_segmented_scan alone."""
+    from collections import OrderedDict
+    from fugue_b200 import api as fa
+    from fugue_b200 import expr as X
+    from fugue_b200 import sort as S
+    from fugue_b200.colmap import ColumnMap, _with_windows
+    from fugue_b200.column import col, functions as f
+    from fugue_b200.dataframe import B200DataFrame
+    from fugue_b200.partition import PartitionSpec
+    from fugue_b200.table import B200Table
+    g = torch.Generator(device=dev).manual_seed(4)
+    cols = [torch.randint(0, 1 << 16, (n,), dtype=torch.int64, device=dev, generator=g),
+            torch.randint(-(2**62), 2**62, (n,), dtype=torch.int64, device=dev, generator=g),
+            torch.randn(n, dtype=torch.float64, device=dev, generator=g),
+            torch.randn(n, dtype=torch.float64, device=dev, generator=g)]
+    T = B200DataFrame(B200Table("key:long,i1:long,v0:double,v1:double", cols))
+    spec = PartitionSpec(by="key", presort="i1", num=256)
+    cm = ColumnMap("key", "i1", "v0", f.sum(col("v0")).over(running=True).alias("run_v0"),
+                   f.row_number().alias("rn"), f.lag(col("v1")).alias("prev_v1"),
+                   (col("v0") / f.sum(col("v0")).over()).alias("share"))
+    schema = "key:long,i1:long,v0:double,run_v0:double,rn:long,prev_v1:double,share:double"
+    ms_call = timeit(lambda: fa.transform(T, cm, schema=schema, partition=spec, engine=e))
+    order = OrderedDict([("key", True), ("i1", True)])
+    srt = S.sort_table(T.native, order)
+    ms_sort = timeit(lambda: S.sort_table(T.native, order))
+    ms_part = timeit(lambda: e.repartition(B200DataFrame(srt), spec))
+    part = e.repartition(B200DataFrame(srt), spec).native
+    del srt
+    sel = cm.select(part).all_cols
+
+    def window_step():
+        part.logical_offsets = S.logical_offsets(part, ["key"])
+        part.logical_order = ["i1"]
+        return _with_windows(part, sel)
+    ms_window = timeit(window_step)
+    src = window_step()
+    outs = [X.rewrite(c, src.window_column) for c in sel]
+    ms_eval = timeit(lambda: X.project(src, outs))
+    off = part.logical_offsets
+    v0 = part.column("v0")
+    scans = [(K.AGG_SUM_F64, v0, None), (K.AGG_SUM_F64, v0, None)]  # the running and the partition sum
+    ms_scan = timeit(lambda: K.segmented_scan(off, n, scans), reps=10)
+    alg_bytes = len(scans) * n * (8 + 8 + 8)   # read the value, write the value and the count
+    return {"rows": n, "partitions": int(off.shape[0]) - 1,
+            "map": "SUM(v0) running, ROW_NUMBER, LAG(v1), v0 / SUM(v0) over the partition",
+            "ms": ms_call, "rows_per_s": n / ms_call * 1e3, "sort_ms": ms_sort, "partition_ms": ms_part,
+            "window_step_ms": ms_window, "evaluator_ms": ms_eval,
+            "segmented_scan": {"ms": ms_scan, "scans": len(scans), "alg_bytes": alg_bytes,
+                               "alg_GBps": alg_bytes / ms_scan / 1e6,
+                               "share_of_3350_GBps": alg_bytes / ms_scan / 1e6 / 3350.0,
+                               "bytes_moved": len(scans) * n * 32,
+                               "note": "reduce-then-scan reads every value twice: 32 B per row and scan move"},
+            "card": _card(dev)}
 
 
 def _dist_time(fn, dev, reps=3):

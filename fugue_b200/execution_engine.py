@@ -129,7 +129,7 @@ class B200MapEngine:
             if fused is not None:
                 return fused
         if keyed:
-            edf = engine.repartition(edf, partition_spec)  # K1+K2+K3 on the device
+            edf = engine._repartition_logical(edf, partition_spec)  # K1+K2+K3 on the device
         if map_func_format_hint == "b200":
             # device-vectorised map: the function is typed on B200Table and is called once per
             # device table, the physical partitions delimited by table.offsets (after a multi-GPU
@@ -367,6 +367,20 @@ class B200ExecutionEngine(EngineLifecycle):
         """Physical repartition.  With keys every algo co-locates equal keys by hashing them
         (``hash_pandas_object(df[keys]) % num``, fugue_dask/_utils.py:146-169); without keys the
         single-device table already is one physical partition."""
+        return self._repartition(df, partition_spec, logical=False)
+
+    def _repartition_logical(self, df: Any, partition_spec: PartitionSpec) -> B200DataFrame:
+        """``repartition`` for ``map_dataframe``: every logical partition (one key tuple as the device sort
+        groups it) lands in one physical partition.  The public ``repartition`` hashes the raw bits, like
+        pandas, which puts -0.0 and 0.0, or NaN and NULL, of a float key into different partitions; here
+        float keys are hashed with -0.0 read as 0.0 and NaN as NULL (DESIGN §7d).  The columns move unchanged."""
+        if self.is_distributed:
+            return self.repartition(df, partition_spec)  # the multi-GPU shuffle hashes raw bits
+        return self._repartition(df, partition_spec, logical=True)
+
+    def _repartition(self, df: Any, partition_spec: PartitionSpec, logical: bool) -> B200DataFrame:
+        from . import sort as S
+
         edf = self.to_df(df)
         keys = partition_spec.partition_by
         t: B200Table = edf.native
@@ -377,12 +391,17 @@ class B200ExecutionEngine(EngineLifecycle):
         if len(keys) == 0:
             return edf
         num = self._num_partitions(partition_spec, t.num_rows)
-        if t.offsets is not None and t.partition_keys == keys and t.num_partitions == num:
+        kidx = [t.schema.index_of_key(k) for k in keys]
+        kcols = [t.columns[i] for i in kidx]
+        kvalid = [t.valid[i] for i in kidx]
+        normalized = logical and any(c.dtype in (torch.float32, torch.float64) for c in kcols)
+        if normalized:
+            kvalid = [S.float_key_valid(c, v) if c.is_floating_point() else v for c, v in zip(kcols, kvalid)]
+            kcols = [S.float_key_bits(c) if c.is_floating_point() else c for c in kcols]
+        elif t.offsets is not None and t.partition_keys == keys and t.num_partitions == num:
             return edf  # already partitioned this way
         if num > K.MAX_PARTITIONS:
-            return self._repartition_wide(edf, keys, num)
-        kidx = [t.schema.index_of_key(k) for k in keys]
-        kvalid = [t.valid[i] for i in kidx]
+            return self._repartition_wide(edf, keys, num, kcols, kvalid)
         # validity masks travel as extra 1-byte columns
         cols = list(t.columns)
         vpos: Dict[int, int] = {}
@@ -391,7 +410,11 @@ class B200ExecutionEngine(EngineLifecycle):
                 vpos[i] = len(cols)
                 cols.append(v)
         scratch = self._pool.scratch(t.device, K.partition_scratch_bytes(t.device, t.num_rows, num))
-        out, offsets = K.partition_columns(cols, kidx, num, kvalid, scratch=scratch)
+        if normalized:  # pass 1 on the normalised keys, pass 2 moves the original columns
+            plan = K.partition_plan(kcols, num, kvalid, scratch=scratch)
+            out, offsets = K.partition_apply(plan, cols), plan.offsets
+        else:
+            out, offsets = K.partition_columns(cols, kidx, num, kvalid, scratch=scratch)
         ncol = len(t.columns)
         valid = [out[vpos[i]] if i in vpos else None for i in range(ncol)]
         res = B200Table(t.schema, out[:ncol], valid, t.dictionaries, offsets, list(keys))
@@ -434,7 +457,8 @@ class B200ExecutionEngine(EngineLifecycle):
         res = B200Table(output_schema, outs, None, {}, plan.offsets if keep else None, keys if keep else None)
         return B200DataFrame(res)
 
-    def _repartition_wide(self, edf: B200DataFrame, keys: List[str], num: int) -> B200DataFrame:
+    def _repartition_wide(self, edf: B200DataFrame, keys: List[str], num: int, kcols: List[torch.Tensor],
+                          kvalid: List[Optional[torch.Tensor]]) -> B200DataFrame:
         """More physical partitions than one radix pass separates (``num=65536``, ``PartitionSpec("per_row")``
         = ROWCOUNT partitions, fugue/collections/partition.py:95,115,186-207): the partition id
         ``hash % num`` of every row (K1) is sorted with stable byte-wise radix passes - the same
@@ -446,12 +470,11 @@ class B200ExecutionEngine(EngineLifecycle):
         t: B200Table = edf.native
         dev, n = t.device, t.num_rows
         assert_or_throw(num < (1 << 32), NotImplementedError(f"num_partitions={num} >= 2^32"))
-        kidx = [t.schema.index_of_key(k) for k in keys]
         if n == 0:
             res = B200Table(t.schema, t.columns, t.valid, t.dictionaries,
                             torch.zeros(num + 1, dtype=torch.int64, device=dev), list(keys))
             return B200DataFrame(res)
-        pid = K.partition_ids([t.columns[i] for i in kidx], num, [t.valid[i] for i in kidx]).to(torch.int64)
+        pid = K.partition_ids(kcols, num, kvalid).to(torch.int64)
         spid, idx = S._radix_sort_pairs(pid.contiguous(), torch.arange(n, dtype=torch.int64, device=dev))
         moved = S.take_rows(t, idx)
         offsets = torch.searchsorted(spid.contiguous(), torch.arange(num + 1, dtype=torch.int64, device=dev))
@@ -546,6 +569,8 @@ class B200ExecutionEngine(EngineLifecycle):
         """GROUP BY on named key columns with ``SUM/COUNT/MIN/MAX/AVG`` of named columns."""
         import pyarrow as pa
 
+        from . import sort as S
+
         edf = self.to_df(df)
         t: B200Table = edf.native
         keys = [] if partition_spec is None else list(partition_spec.partition_by)
@@ -556,15 +581,16 @@ class B200ExecutionEngine(EngineLifecycle):
         kidx = [t.schema.index_of_key(k) for k in keys]
 
         def key_bits64(c: torch.Tensor) -> torch.Tensor:
-            if c.dtype == torch.float64:
-                return torch.where(c == 0, torch.zeros_like(c), c).view(torch.int64)  # -0.0 groups with 0.0
-            if c.dtype == torch.float32:
-                return torch.where(c == 0, torch.zeros_like(c), c).view(torch.int32).to(torch.int64)
+            if c.is_floating_point():  # -0.0 groups with 0.0 (DESIGN §7d)
+                return S.float_key_bits(c).to(torch.int64)
             return c if c.dtype == torch.int64 else c.to(torch.int64)
 
+        # a NaN key is NULL: it groups with the NULL keys (DESIGN §7d)
+        key_valid = {i: S.float_key_valid(t.columns[i], t.valid[i]) if t.columns[i].is_floating_point()
+                     else t.valid[i] for i in kidx}
         if len(keys) == 1:
             ki = kidx[0]
-            kcol, kvalid, ktype = t.columns[ki], t.valid[ki], t.schema.types[ki]
+            kcol, kvalid, ktype = t.columns[ki], key_valid[ki], t.schema.types[ki]
             key64 = key_bits64(kcol)
         elif multi:
             # several key columns: group on the 64-bit hash of the key tuple (same hash as the
@@ -572,7 +598,7 @@ class B200ExecutionEngine(EngineLifecycle):
             # MIN != MAX (or that mixes NULL and non-NULL) is a hash collision -> error instead of a
             # silently merged group.  The key values of the output are the MINs.
             kb = [key_bits64(t.columns[i]).contiguous() for i in kidx]
-            key64 = K.row_hash64(kb, [t.valid[i] for i in kidx])
+            key64 = K.row_hash64(kb, [key_valid[i] for i in kidx])
             kvalid, ktype = None, None
         else:
             key64, kvalid, ktype = torch.zeros(n, dtype=torch.int64, device=dev), None, None
@@ -591,7 +617,7 @@ class B200ExecutionEngine(EngineLifecycle):
         key_slots: List[Any] = []
         if multi:
             for i, kbits in zip(kidx, kb):
-                m = t.valid[i]
+                m = key_valid[i]
                 key_slots.append((add(kbits, m, K.AGG_MIN_I64), add(kbits, m, K.AGG_MAX_I64),
                                   add(None, m, K.AGG_COUNT) if m is not None else None))
             rows_slot = add(None, None, K.AGG_COUNT)

@@ -9,7 +9,8 @@ Reference semantics:
   * logical partitions           one per distinct key tuple, NULLs grouped (SURVEY.md 3.2)
 
 A column becomes an order-preserving UNSIGNED 64-bit key (sign bit flipped for signed ints, the
-usual total-order transform for floats, dictionary rank for strings, complement for DESC); (key,
+usual total-order transform for floats - with NaN as NULL and -0.0 as 0.0, see ``float_key_bits`` -,
+dictionary rank for strings, complement for DESC); (key,
 row index) pairs are sorted with one stable 8-bit radix pass (``fb_radix_pass``) per varying byte, the
 least significant sort column first; NULLS FIRST/LAST is one more pass on the validity flag.  The
 payload is gathered once at the end (``fb_gather_rows``).  Key preparation uses torch integer ops on
@@ -30,6 +31,22 @@ from .table import B200Table
 _SIGN = -(1 << 63)
 
 
+# Float sort and grouping keys (DESIGN §7d): a NaN of either sign is NULL, and -0.0 equals 0.0.  Only the
+# order and the grouping follow this rule; the rows keep their own bits.
+def float_key_bits(c: torch.Tensor) -> torch.Tensor:
+    """Bit pattern (int64 for float64, int32 for float32) of a float key column, -0.0 read as 0.0."""
+    z = torch.where(c == 0, torch.zeros_like(c), c)
+    return z.view(torch.int64 if c.dtype == torch.float64 else torch.int32)
+
+
+def float_key_valid(c: torch.Tensor, v: Optional[torch.Tensor]) -> Optional[torch.Tensor]:
+    """Validity (uint8) of a float key column with NaN rows cleared; None when every row is valid."""
+    ok = c == c
+    if v is not None:
+        return v & ok.to(torch.uint8)
+    return None if bool(ok.all()) else ok.to(torch.uint8)
+
+
 def _unsigned_order_key(t: B200Table, name: str, ascending: bool) -> torch.Tensor:
     """int64 tensor whose bit pattern, read as unsigned, orders like the column."""
     i = t.schema.index_of_key(name)
@@ -42,7 +59,7 @@ def _unsigned_order_key(t: B200Table, name: str, ascending: bool) -> torch.Tenso
         r = torch.from_numpy(rank).to(c.device)
         key = r[c.long().clamp(min=0)] if len(d) > 0 else torch.zeros_like(c, dtype=torch.int64)
     elif pa.types.is_floating(tp):
-        b = (c if c.dtype == torch.float64 else c.to(torch.float64)).view(torch.int64)
+        b = float_key_bits(c if c.dtype == torch.float64 else c.to(torch.float64))
         key = b ^ ((b >> 63) | _SIGN)  # negative: flip all bits; non-negative: flip the sign bit
     elif tp in (pa.uint8(), pa.bool_()):
         key = c.to(torch.int64)
@@ -96,6 +113,9 @@ def argsort_rows(t: B200Table, sorts: "OrderedDict[str, bool]", na_position: str
     for name, asc in reversed(list(sorts.items())):
         key = _unsigned_order_key(t, name, asc)
         v = t.valid[t.schema.index_of_key(name)]
+        c = t.column(name)
+        if c.dtype in (torch.float32, torch.float64):
+            v = float_key_valid(c, v)
         if v is not None:
             # the value stored under a NULL is undefined (Arrow / parquet leave garbage there): give all
             # NULL rows one constant key, so that they keep the order set by the less significant columns
@@ -120,7 +140,7 @@ def sort_table(t: B200Table, sorts: "OrderedDict[str, bool]", na_position: str =
 
 def group_starts(t: B200Table, keys: List[str]) -> torch.Tensor:
     """For a table in which equal key tuples are adjacent: bool mask, True at the first row of
-    every logical partition (NULL == NULL for grouping)."""
+    every logical partition (NULL == NULL for grouping; float keys: NaN is NULL and -0.0 equals 0.0)."""
     n = t.num_rows
     first = torch.zeros(n, dtype=torch.bool, device=t.device)
     if n == 0:
@@ -130,7 +150,7 @@ def group_starts(t: B200Table, keys: List[str]) -> torch.Tensor:
         i = t.schema.index_of_key(k)
         c, v = t.columns[i], t.valid[i]
         if c.dtype in (torch.float32, torch.float64):
-            c = c.view(torch.int32 if c.dtype == torch.float32 else torch.int64)
+            c, v = float_key_bits(c), float_key_valid(c, v)
         if v is None:
             diff = c[1:] != c[:-1]
         else:

@@ -11,6 +11,8 @@ the window nodes of ``fugue_b200.column`` mean with SQL window semantics over th
   (NULLs last in every presort column, ties in input order: a stable sort), in input order without one;
 * peers (RANK / DENSE_RANK) are rows equal on every presort column, NULL equal to NULL; without a
   presort every row of a partition is a peer of every other;
+* ordering, partitions and peers come from oracle/sort.py, so float keys and presort columns follow its rule:
+  a NaN of either sign is NULL, -0.0 equals 0.0 (the rows keep their own bits);
 * aggregates skip NULLs; SUM / AVG / MIN / MAX over no valid row are NULL, COUNT never is; FIRST / LAST
   are the first / last valid value; ``running`` = ROWS BETWEEN UNBOUNDED PRECEDING AND CURRENT ROW;
 * types follow ``ExecutionEngine.aggregate``: integer SUM is int64 with two's-complement wrap-around,
@@ -31,6 +33,7 @@ import pyarrow.compute as pc
 from fugue_b200.column import ColumnExpr, Kind, col
 
 from . import expressions as ox
+from . import sort as S
 
 _FLIP = np.int64(0x7FFFFFFFFFFFFFFF)
 
@@ -89,23 +92,6 @@ def _column(t: pa.Table, name: str) -> Tuple[np.ndarray, np.ndarray, pa.DataType
     return vals, ok, a.type
 
 
-def _segments(t: pa.Table, names: Sequence[str]) -> np.ndarray:
-    """bool per row: True where the tuple of ``names`` differs from the previous row (NULL == NULL)."""
-    n = t.num_rows
-    first = np.zeros(n, dtype=bool)
-    if n:
-        first[0] = True
-    for nm in names:
-        v, ok, tp = _column(t, nm)
-        if pa.types.is_floating(tp):
-            v = v.astype(np.float64).view(np.int64)
-        same_v = np.array([v[i] == v[i - 1] for i in range(1, n)], dtype=bool) if v.dtype == object \
-            else (v[1:] == v[:-1])
-        diff = (ok[1:] != ok[:-1]) | (ok[1:] & ~same_v)
-        first[1:] |= diff
-    return first
-
-
 def _pandas(t: pa.Table) -> pd.DataFrame:
     m = {pa.int64(): pd.Int64Dtype(), pa.int32(): pd.Int32Dtype(), pa.float64(): pd.Float64Dtype(),
          pa.float32(): pd.Float32Dtype(), pa.string(): pd.StringDtype(), pa.bool_(): pd.BooleanDtype()}
@@ -117,17 +103,18 @@ def window_map(table: pa.Table, keys: Sequence[str], presort: "OrderedDict[str, 
     """Output columns (python values, None for NULL) of ``ColumnMap(*columns)`` under
     ``PartitionSpec(by=keys, presort=presort)``, one entry per input row in input order."""
     n = table.num_rows
-    sort_keys = [(k, "ascending") for k in keys] + [(k, "ascending" if a else "descending") for k, a in presort.items()]
-    order = np.asarray(pc.sort_indices(table, sort_keys=sort_keys, null_placement="at_end")) if sort_keys \
-        else np.arange(n)
+    sorts = OrderedDict((k, True) for k in keys)
+    for k, a in presort.items():  # a key re-listed in the presort takes the presort's direction, as map_dataframe
+        sorts[k] = a
+    order = S.argsort(table, sorts, "last")
     st = table.take(pa.array(order, type=pa.int64()))
-    seg_head = _segments(st, keys)
+    seg_head = S.group_heads(st, keys)
     offsets = np.concatenate([np.flatnonzero(seg_head), [n]]).astype(np.int64)
     lengths = np.diff(offsets)
     first = np.repeat(offsets[:-1], lengths)
     last = np.repeat(offsets[1:] - 1, lengths)
     pos = np.arange(n, dtype=np.int64)
-    peer = _segments(st, list(presort.keys())) | seg_head
+    peer = S.group_heads(st, list(presort.keys())) | seg_head
     pdf = _pandas(st)
     temps: Dict[str, pa.Array] = {}
 

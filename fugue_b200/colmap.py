@@ -28,7 +28,7 @@ import torch
 
 from . import kernels as K
 from .column import ColumnExpr, Kind, SelectColumns, col as _col, has_window, is_agg
-from .table import B200Table
+from .table import B200Table, narrow, widen
 
 
 def _f64_bits(v: float) -> int:
@@ -178,7 +178,6 @@ def _with_windows(t: B200Table, cols: List[ColumnExpr]) -> B200Table:
     from . import expr as X
     from . import sort as S
     from .schema import Schema
-    from .table import _storage_dtype
 
     nodes: Dict[str, ColumnExpr] = {}
     for c in cols:
@@ -282,7 +281,8 @@ def _with_windows(t: B200Table, cols: List[ColumnExpr]) -> B200Table:
         is_f = pa.types.is_floating(tp)
         if fn in ("SUM", "AVG"):
             f64 = fn == "AVG" or is_f
-            v8 = c.to(torch.float64 if f64 else torch.int64).contiguous()
+            v8 = widen(c, tp)
+            v8 = (v8.to(torch.float64) if f64 else v8).contiguous()
             i = scan(K.AGG_SUM_F64 if f64 else K.AGG_SUM_I64, v8, m)
             out_tp = pa.float64() if f64 else pa.int64()
 
@@ -295,14 +295,14 @@ def _with_windows(t: B200Table, cols: List[ColumnExpr]) -> B200Table:
             finish.append((uid, total))
             continue
         if fn in ("MIN", "MAX"):
-            v8 = c if c.element_size() == 8 else c.to(torch.float64 if is_f else torch.int64).contiguous()
+            v8 = widen(c, tp).contiguous()
             op = {("MIN", True): K.AGG_MIN_F64, ("MAX", True): K.AGG_MAX_F64,
                   ("MIN", False): K.AGG_MIN_I64, ("MAX", False): K.AGG_MAX_I64}[(fn, is_f)]
             i = scan(op, v8, m)
 
-            def extreme(r: Any, i: int = i, e: Any = at_end, tp: Any = tp, dt: Any = c.dtype) -> Any:
+            def extreme(r: Any, i: int = i, e: Any = at_end, tp: Any = tp) -> Any:
                 v, cnt = e(r[i][0]), e(r[i][1])
-                return v.to(dt).contiguous(), (cnt > 0).to(torch.uint8), tp, None
+                return narrow(v, tp).contiguous(), (cnt > 0).to(torch.uint8), tp, None
 
             finish.append((uid, extreme))
             continue
@@ -317,7 +317,7 @@ def _with_windows(t: B200Table, cols: List[ColumnExpr]) -> B200Table:
         window_names[uid] = nm
         names.append(nm)
         types.append(tp)
-        columns.append(c if c.dtype == _storage_dtype(tp) else c.to(_storage_dtype(tp)))
+        columns.append(narrow(c, tp))
         valid.append(v)
         if d is not None:
             dicts[nm] = d

@@ -19,6 +19,8 @@
 //     COALESCE read the validity bits.
 #include <mutex>
 
+#include <cuda_fp16.h>
+
 #include "fb_common.cuh"
 
 namespace {
@@ -51,8 +53,19 @@ __device__ __forceinline__ void load_col(const void* p, int64_t row0, int tid, i
     const int i = k * kExprThreads + tid;
     if (kFull || i < nk) {
       if (kFloat) v[k] = f_bits((double)q[i]);
-      else v[k] = (uint64_t)(int64_t)q[i];
+      else v[k] = (uint64_t)(int64_t)q[i];  // unsigned T zero-extends, signed T sign-extends
     }
+  }
+}
+
+// float16 is stored as its 16 bits; every half value is exact in a double
+template <bool kFull>
+__device__ __forceinline__ void load_f16(const void* p, int64_t row0, int tid, int nk, uint64_t (&v)[kExprItems]) {
+  const __half* __restrict__ q = (const __half*)p + row0;
+#pragma unroll
+  for (int k = 0; k < kExprItems; ++k) {
+    const int i = k * kExprThreads + tid;
+    if (kFull || i < nk) v[k] = f_bits((double)__half2float(q[i]));
   }
 }
 
@@ -68,6 +81,17 @@ __device__ __forceinline__ void store_col(void* p, int64_t row0, int tid, int nk
       if (kFloat) q[i] = (T)as_f(bits);
       else q[i] = (T)(int64_t)bits;
     }
+  }
+}
+
+template <bool kFull>
+__device__ __forceinline__ void store_f16(void* p, int64_t row0, int tid, int nk, const uint64_t (&v)[kExprItems],
+                                          unsigned valid) {
+  __half* __restrict__ q = (__half*)p + row0;
+#pragma unroll
+  for (int k = 0; k < kExprItems; ++k) {
+    const int i = k * kExprThreads + tid;
+    if (kFull || i < nk) q[i] = __double2half(as_f((valid >> k) & 1u ? v[k] : 0ull));  // one rounding, to nearest even
   }
 }
 
@@ -97,6 +121,9 @@ __device__ __forceinline__ void run_tile(const ExprProgram& P, int64_t row0, int
           case FB_T_I64: load_col<int64_t, false, kFull>(p, row0, tid, nk, b); break;
           case FB_T_U8: load_col<uint8_t, false, kFull>(p, row0, tid, nk, b); break;
           case FB_T_F32: load_col<float, true, kFull>(p, row0, tid, nk, b); break;
+          case FB_T_U16: load_col<uint16_t, false, kFull>(p, row0, tid, nk, b); break;
+          case FB_T_U32: load_col<uint32_t, false, kFull>(p, row0, tid, nk, b); break;
+          case FB_T_F16: load_f16<kFull>(p, row0, tid, nk, b); break;
           default: load_col<int64_t, false, kFull>(p, row0, tid, nk, b); break;  // FB_T_F64: raw bits
         }
         const uint8_t* m = P.col_valid[in.b];
@@ -145,6 +172,10 @@ __device__ __forceinline__ void run_tile(const ExprProgram& P, int64_t row0, int
             case FB_T_I64: store_col<int64_t, false, kFull>(p, row0, tid, nk, acc, accv); break;
             case FB_T_U8: store_col<uint8_t, false, kFull>(p, row0, tid, nk, acc, accv); break;
             case FB_T_F32: store_col<float, true, kFull>(p, row0, tid, nk, acc, accv); break;
+            // unsigned stores keep the low bits, exactly as the signed stores of the same width do
+            case FB_T_U16: store_col<int16_t, false, kFull>(p, row0, tid, nk, acc, accv); break;
+            case FB_T_U32: store_col<int32_t, false, kFull>(p, row0, tid, nk, acc, accv); break;
+            case FB_T_F16: store_f16<kFull>(p, row0, tid, nk, acc, accv); break;
             default: store_col<int64_t, false, kFull>(p, row0, tid, nk, acc, accv); break;  // FB_T_F64
           }
           uint8_t* m = P.out_valid[in.b];
@@ -242,14 +273,14 @@ extern "C" int fb_eval_expr(int dev, void* stream, int64_t nrows, int ncols, con
   ExprProgram P;
   memset(&P, 0, sizeof(P));
   for (int c = 0; c < ncols; ++c) {
-    FB_CHECK(col_types[c] >= FB_T_I8 && col_types[c] <= FB_T_F64, "column %d has unknown type %d", c, col_types[c]);
+    FB_CHECK(col_types[c] >= FB_T_I8 && col_types[c] <= FB_T_F16, "column %d has unknown type %d", c, col_types[c]);
     FB_CHECK(nrows == 0 || col_ptrs[c] != nullptr, "column %d pointer is NULL", c);
     P.col_ptr[c] = col_ptrs[c];
     P.col_type[c] = col_types[c];
     P.col_valid[c] = col_valid ? col_valid[c] : nullptr;
   }
   for (int o = 0; o < nouts; ++o) {
-    FB_CHECK(out_types[o] >= FB_T_I8 && out_types[o] <= FB_T_F64, "output %d: unknown type", o);
+    FB_CHECK(out_types[o] >= FB_T_I8 && out_types[o] <= FB_T_F16, "output %d: unknown type", o);
     FB_CHECK(nrows == 0 || out_ptrs[o] != nullptr, "output %d pointer is NULL", o);
     P.out_type[o] = out_types[o];
     P.out_ptr[o] = out_ptrs[o];

@@ -22,7 +22,7 @@ from .dataframe import (ArrowDataFrame, B200DataFrame, DataFrame, LocalDataFrame
 from .lifecycle import FUGUE_GLOBAL_CONF, EngineLifecycle
 from .partition import KEYWORD_PARALLELISM, KEYWORD_ROWCOUNT, PartitionCursor, PartitionSpec
 from .schema import Schema
-from .table import B200Table
+from .table import B200Table, narrow, widen
 
 FUGUE_B200_CONF_DEVICE = "fugue.b200.device"
 FUGUE_B200_CONF_DEFAULT_PARTITIONS = "fugue.b200.default.partitions"
@@ -644,7 +644,7 @@ class B200ExecutionEngine(EngineLifecycle):
                 continue
             assert_or_throw(arg not in t.dictionaries, NotImplementedError(f"{fn} on a string column"))
             is_f = pa.types.is_floating(tp)
-            c8 = c if c.element_size() == 8 else c.to(torch.float64 if is_f else torch.int64)
+            c8 = widen(c, tp)
             # non-null count -> result validity.  A global aggregate (no keys) always carries it: over an
             # empty input (or an empty shard of a multi-GPU aggregate) SUM / MIN / MAX are NULL, not 0
             nn = add(None, m, K.AGG_COUNT) if (m is not None or len(keys) == 0) else None
@@ -724,15 +724,8 @@ class B200ExecutionEngine(EngineLifecycle):
                 cnt = gaggs[nn].to(torch.float64)
                 col = raw.view(torch.float64) / cnt
                 v = (gaggs[nn] > 0).to(torch.uint8)
-            elif pa.types.is_floating(tp):
-                col = raw.view(torch.float64)
-                if tp == pa.float32():
-                    col = col.to(torch.float32)
             else:
-                from .table import _storage_dtype
-
-                sd = _storage_dtype(tp)
-                col = raw if sd == torch.int64 else raw.to(sd)
+                col = narrow(raw.view(torch.float64) if pa.types.is_floating(tp) else raw, tp)
             fields.append(pa.field(name, tp))
             cols.append(col.contiguous())
             valids.append(v)

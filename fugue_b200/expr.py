@@ -20,7 +20,7 @@ import torch
 from . import kernels as K
 from .column import ColumnExpr, Kind, lit as _lit
 from .schema import Schema
-from .table import B200Table, _storage_dtype
+from .table import B200Table, _storage_dtype, expr_type
 
 
 def _is_str(tp: Optional[pa.DataType]) -> bool:
@@ -64,7 +64,7 @@ class _Program:
         self.ins: List[Tuple[int, int, int, int, int]] = []
         self.cols: List[int] = []          # table column indices, in load order
         self.free = list(range(K.EXPR_NREGS - 1, -1, -1))
-        self.outs: List[Tuple[torch.dtype, bool]] = []  # (dtype, want_valid) per FB_X_OUT
+        self.outs: List[Tuple[torch.dtype, bool, int]] = []  # (dtype, want_valid, K8 type) per FB_X_OUT
 
     # -- resources
     def alloc(self) -> int:
@@ -88,11 +88,12 @@ class _Program:
         self.cols.append(ci)
         return len(self.cols) - 1
 
-    def output(self, dtype: torch.dtype, want_valid: bool) -> None:
+    def output(self, dtype: torch.dtype, want_valid: bool, tp: Optional[int] = None) -> None:
+        """``tp``: the K8 type of the output (default: the signed integer or float of ``dtype``)."""
         if len(self.outs) >= K.EXPR_MAX_OUTS:
             raise _OutOfResources("outputs")
         self.emit(K.X_OUT, K.XK_NONE, len(self.outs))
-        self.outs.append((dtype, want_valid))
+        self.outs.append((dtype, want_valid, K.expr_type_of(dtype) if tp is None else tp))
 
     def mark(self) -> Any:
         return (len(self.ins), list(self.cols), list(self.free), len(self.outs))
@@ -336,7 +337,8 @@ class _Program:
         t = self.t
         return K.eval_expr(t.num_rows, t.device, [t.columns[i] for i in self.cols],
                            [t.valid[i] for i in self.cols], self.ins, [o[0] for o in self.outs],
-                           [o[1] for o in self.outs])
+                           [o[1] for o in self.outs], col_types=[expr_type(t.schema.types[i]) for i in self.cols],
+                           out_types=[o[2] for o in self.outs])
 
 
 def _default_type(cls: str, e: ColumnExpr, schema: Schema) -> pa.DataType:
@@ -420,7 +422,7 @@ def project(t: B200Table, exprs: Sequence[ColumnExpr]) -> B200Table:
                         tp = store_tp  # an inferred type of another class than the computed value
                 else:
                     store_tp = tp
-                prog.output(_storage_dtype(store_tp), nullable)
+                prog.output(_storage_dtype(store_tp), nullable, expr_type(store_tp))
             except _OutOfResources as ex:
                 if not batch:
                     raise NotImplementedError(f"expression too large for one device program ({ex}): {e}")

@@ -652,7 +652,7 @@ def compact_indices(mask: torch.Tensor) -> torch.Tensor:
 
 # ---- K8: column-expression evaluator -----------------------------------------------------------
 EXPR_MAX_COLS, EXPR_MAX_OUTS, EXPR_MAX_INS, EXPR_NREGS = 16, 16, 96, 4
-T_I8, T_I16, T_I32, T_I64, T_U8, T_F32, T_F64 = range(7)
+T_I8, T_I16, T_I32, T_I64, T_U8, T_F32, T_F64, T_U16, T_U32, T_F16 = range(10)
 XK_NONE, XK_REG, XK_COL, XK_IMM, XK_NULL = range(5)
 XF_B_I2F = 1
 (X_MOV, X_ST, X_OUT, X_I2F, X_F2I, X_NEG_I, X_NEG_F, X_NOT, X_IS_NULL, X_NOT_NULL, X_TOBOOL_I, X_TOBOOL_F,
@@ -660,22 +660,36 @@ XF_B_I2F = 1
  X_LT_I, X_LE_I, X_GT_I, X_GE_I, X_EQ_I, X_NE_I, X_LT_F, X_LE_F, X_GT_F, X_GE_F, X_EQ_F, X_NE_F,
  X_AND, X_OR, X_COALESCE, X_RCOALESCE) = range(38)
 
+# storage dtype of each K8 type: uint16 / uint32 / float16 live in the signed tensors of their width
+EXPR_STORAGE = {T_I8: torch.int8, T_I16: torch.int16, T_I32: torch.int32, T_I64: torch.int64, T_U8: torch.uint8,
+                T_F32: torch.float32, T_F64: torch.float64, T_U16: torch.int16, T_U32: torch.int32,
+                T_F16: torch.int16}
 _EXPR_TYPE_OF_DTYPE = {torch.int8: T_I8, torch.int16: T_I16, torch.int32: T_I32, torch.int64: T_I64,
                        torch.uint8: T_U8, torch.bool: T_U8, torch.float32: T_F32, torch.float64: T_F64}
 
 
 def expr_type_of(dtype: torch.dtype) -> int:
+    """The K8 type that reads a tensor of ``dtype`` as a signed integer or a float of its width."""
     return _EXPR_TYPE_OF_DTYPE[dtype]
 
 
 def eval_expr(nrows: int, device: torch.device, cols: Sequence[torch.Tensor],
               valid: Sequence[Optional[torch.Tensor]], program: Sequence[Tuple[int, int, int, int, int]],
-              out_dtypes: Sequence[torch.dtype], want_valid: Sequence[bool]
+              out_dtypes: Sequence[torch.dtype], want_valid: Sequence[bool],
+              col_types: Optional[Sequence[int]] = None, out_types: Optional[Sequence[int]] = None
               ) -> Tuple[List[torch.Tensor], List[Optional[torch.Tensor]]]:
     """Run one accumulator-machine ``program`` (tuples ``(op, operand_kind, b, flags, imm_bits)``, see
     include/fugue_b200.h K8) over all rows; ``X_OUT b`` writes output ``b``.  Returns the output
-    columns and (where asked for) their validity byte masks."""
+    columns (``out_dtypes``) and (where asked for) their validity byte masks.
+    ``col_types`` / ``out_types`` are the K8 types (``T_*``) of the columns and outputs: the storage
+    dtype alone does not say whether 16 bits hold an int16, a uint16 or a float16.  Left out, every
+    tensor is read and written as the signed integer or float of its dtype (``expr_type_of``)."""
     lib = _lib.load()
+    col_types = [expr_type_of(c.dtype) for c in cols] if col_types is None else list(col_types)
+    out_types = [expr_type_of(dt) for dt in out_dtypes] if out_types is None else list(out_types)
+    assert len(col_types) == len(cols) and len(out_types) == len(out_dtypes)
+    for dt, tp in zip(out_dtypes, out_types):
+        assert dt.itemsize == EXPR_STORAGE[tp].itemsize, f"{dt} output can't hold K8 type {tp}"
     outs = [torch.empty(nrows, dtype=dt, device=device) for dt in out_dtypes]
     outv = [torch.empty(nrows, dtype=torch.uint8, device=device) if w else None for w in want_valid]
     if nrows == 0:
@@ -685,13 +699,14 @@ def eval_expr(nrows: int, device: torch.device, cols: Sequence[torch.Tensor],
         prog[i].op, prog[i].kind, prog[i].b, prog[i].flags = op, kind, b, flags
         imm &= (1 << 64) - 1
         prog[i].imm = imm - (1 << 64) if imm >= (1 << 63) else imm
-    for c in cols:
+    for c, tp in zip(cols, col_types):
         assert c.is_cuda and c.is_contiguous() and c.shape[0] == nrows
+        assert c.element_size() == EXPR_STORAGE[tp].itemsize, f"{c.dtype} column can't hold K8 type {tp}"
     _lib.check(lib.fb_eval_expr(
         device.index, _stream_ptr(device), nrows, len(cols), _lib.ptr_array([c.data_ptr() for c in cols]),
-        _lib.i32_array([expr_type_of(c.dtype) for c in cols]),
+        _lib.i32_array(col_types),
         _lib.ptr_array([0 if v is None else v.data_ptr() for v in valid]), len(program), prog, len(outs),
-        _lib.i32_array([expr_type_of(dt) for dt in out_dtypes]),
+        _lib.i32_array(out_types),
         _lib.ptr_array([o.data_ptr() for o in outs]),
         _lib.ptr_array([0 if v is None else v.data_ptr() for v in outv])))
     return outs, outv

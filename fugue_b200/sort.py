@@ -26,7 +26,7 @@ import torch
 
 from . import _lib
 from . import kernels as K
-from .table import B200Table
+from .table import B200Table, widen
 
 _SIGN = -(1 << 63)
 
@@ -59,7 +59,7 @@ def _unsigned_order_key(t: B200Table, name: str, ascending: bool) -> torch.Tenso
         r = torch.from_numpy(rank).to(c.device)
         key = r[c.long().clamp(min=0)] if len(d) > 0 else torch.zeros_like(c, dtype=torch.int64)
     elif pa.types.is_floating(tp):
-        b = float_key_bits(c if c.dtype == torch.float64 else c.to(torch.float64))
+        b = float_key_bits(widen(c, tp))
         key = b ^ ((b >> 63) | _SIGN)  # negative: flip all bits; non-negative: flip the sign bit
     elif tp in (pa.uint8(), pa.bool_()):
         key = c.to(torch.int64)
@@ -112,10 +112,10 @@ def argsort_rows(t: B200Table, sorts: "OrderedDict[str, bool]", na_position: str
     idx = torch.arange(n, dtype=torch.int64, device=dev)
     for name, asc in reversed(list(sorts.items())):
         key = _unsigned_order_key(t, name, asc)
-        v = t.valid[t.schema.index_of_key(name)]
-        c = t.column(name)
-        if c.dtype in (torch.float32, torch.float64):
-            v = float_key_valid(c, v)
+        i = t.schema.index_of_key(name)
+        v = t.valid[i]
+        if pa.types.is_floating(t.schema.types[i]):
+            v = float_key_valid(widen(t.columns[i], t.schema.types[i]), v)
         if v is not None:
             # the value stored under a NULL is undefined (Arrow / parquet leave garbage there): give all
             # NULL rows one constant key, so that they keep the order set by the less significant columns
@@ -149,8 +149,9 @@ def group_starts(t: B200Table, keys: List[str]) -> torch.Tensor:
     for k in keys:
         i = t.schema.index_of_key(k)
         c, v = t.columns[i], t.valid[i]
-        if c.dtype in (torch.float32, torch.float64):
-            c, v = float_key_bits(c), float_key_valid(c, v)
+        if pa.types.is_floating(t.schema.types[i]):
+            w = widen(c, t.schema.types[i]) if c.dtype == torch.int16 else c  # float16
+            c, v = float_key_bits(w), float_key_valid(w, v)
         if v is None:
             diff = c[1:] != c[:-1]
         else:

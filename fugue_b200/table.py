@@ -42,6 +42,41 @@ def _storage_dtype(tp: pa.DataType) -> torch.dtype:
     raise NotImplementedError(f"B200Table can't hold arrow type {tp} on the device")
 
 
+_EXPR_TYPE_OF_STORAGE = {torch.uint8: K.T_U8, torch.int8: K.T_I8, torch.int16: K.T_I16, torch.int32: K.T_I32,
+                         torch.int64: K.T_I64, torch.float32: K.T_F32, torch.float64: K.T_F64}
+
+
+def expr_type(tp: pa.DataType) -> int:
+    """The K8 column type (``kernels.T_*``) that reads a column of arrow type ``tp`` by its value."""
+    special = {pa.uint16(): K.T_U16, pa.uint32(): K.T_U32, pa.float16(): K.T_F16}
+    return special.get(tp, _EXPR_TYPE_OF_STORAGE[_storage_dtype(tp)])
+
+
+def widen(c: torch.Tensor, tp: pa.DataType) -> torch.Tensor:
+    """A stored column as its canonical 64-bit value: float64 for float types, int64 for the rest.
+    uint16 / uint32 zero-extend, float16 is decoded from its int16 storage (exactly); uint64 values
+    >= 2**63 stay int64 bit patterns.  Returns ``c`` itself when it already is that."""
+    if tp == pa.float16():
+        return c.view(torch.float16).to(torch.float64)
+    if pa.types.is_floating(tp):
+        return c.to(torch.float64)
+    if tp == pa.uint16():
+        return c.to(torch.int64) & 0xFFFF
+    if tp == pa.uint32():
+        return c.to(torch.int64) & 0xFFFFFFFF
+    return c.to(torch.int64)
+
+
+def narrow(v: torch.Tensor, tp: pa.DataType) -> torch.Tensor:
+    """The inverse of ``widen`` for a value the type can hold: the storage of arrow type ``tp``."""
+    sd = _storage_dtype(tp)
+    if v.dtype == sd:
+        return v
+    if tp == pa.float16():
+        return v.to(torch.float16).view(torch.int16)
+    return v.to(sd)
+
+
 def _np_storage(tp: pa.DataType) -> np.dtype:
     return {torch.uint8: np.dtype("u1"), torch.int8: np.dtype("i1"), torch.int16: np.dtype("i2"),
             torch.int32: np.dtype("i4"), torch.int64: np.dtype("i8"), torch.float32: np.dtype("f4"),

@@ -369,6 +369,10 @@ int fb_join2_emit(int dev, void* stream, int64_t nprobe, const void* probe_keys,
  *   arithmetic / comparisons: acc <- acc op B (FB_X_R*: B op acc), NULL if either side is NULL
  *   FB_X_AND / FB_X_OR: Kleene three-valued logic; FB_X_IS_NULL / FB_X_NOT_NULL / FB_X_COALESCE
  *   flags & FB_XF_B_I2F: convert operand B from int64 to float64 first
+ *   FB_X_F2I: truncate toward zero; out of range saturates to INT64_MIN / INT64_MAX; NaN -> INT64_MIN
+ * Column types: FB_T_U16 / FB_T_U32 load zero-extended, FB_T_F16 loads its IEEE half value exactly.
+ * Stores keep the low bits of an integer (unsigned stores are the signed ones of the same width) and
+ * round a float to nearest even (FB_T_F32, FB_T_F16).
  * `program`, the pointer tables and the type arrays are HOST arrays (copied into the launch);
  * column / output pointers are device memory.
  * --------------------------------------------------------------------------- */
@@ -376,7 +380,8 @@ int fb_join2_emit(int dev, void* stream, int64_t nprobe, const void* probe_keys,
 #define FB_EXPR_MAX_OUTS 16
 #define FB_EXPR_MAX_INS 96
 #define FB_EXPR_NREGS 4
-enum fb_expr_type { FB_T_I8 = 0, FB_T_I16 = 1, FB_T_I32 = 2, FB_T_I64 = 3, FB_T_U8 = 4, FB_T_F32 = 5, FB_T_F64 = 6 };
+enum fb_expr_type { FB_T_I8 = 0, FB_T_I16 = 1, FB_T_I32 = 2, FB_T_I64 = 3, FB_T_U8 = 4, FB_T_F32 = 5, FB_T_F64 = 6,
+                    FB_T_U16 = 7, FB_T_U32 = 8, FB_T_F16 = 9 };
 enum fb_expr_operand { FB_XK_NONE = 0, FB_XK_REG = 1, FB_XK_COL = 2, FB_XK_IMM = 3, FB_XK_NULL = 4 };
 #define FB_XF_B_I2F 1
 enum fb_expr_op {

@@ -5,13 +5,26 @@ import numpy as np
 from fugue_b200 import kernels as K
 
 _NP_OF_T = {K.T_I8: np.int8, K.T_I16: np.int16, K.T_I32: np.int32, K.T_I64: np.int64, K.T_U8: np.uint8,
-            K.T_F32: np.float32, K.T_F64: np.float64}
+            K.T_F32: np.float32, K.T_F64: np.float64, K.T_U16: np.uint16, K.T_U32: np.uint32, K.T_F16: np.float16}
 
 
-def _to_bits(a: np.ndarray) -> np.ndarray:
+def _to_bits(a: np.ndarray, tp: int) -> np.ndarray:
+    """A column in its storage dtype, read as K8 type ``tp``: canonical 64-bit value bits."""
+    a = a.view(_NP_OF_T[tp])
     if a.dtype.kind == "f":
         return a.astype(np.float64).view(np.uint64)
     return a.astype(np.int64).view(np.uint64)
+
+
+def f2i(x: np.ndarray) -> np.ndarray:
+    """FB_X_F2I as the H100 computes it: truncate toward zero, values outside int64 saturate to INT64_MIN /
+    INT64_MAX, and NaN (any sign or payload) gives INT64_MIN."""
+    x = np.asarray(x, dtype=np.float64)
+    t = np.trunc(np.where(np.isnan(x), -2.0 ** 64, x))
+    hi, lo = t >= 2.0 ** 63, t < -2.0 ** 63
+    out = np.where(hi | lo, 0.0, t).astype(np.int64)
+    out[hi], out[lo] = np.iinfo(np.int64).max, np.iinfo(np.int64).min
+    return out
 
 
 def _f(b):
@@ -26,8 +39,15 @@ def _ib(x):
     return np.asarray(x).astype(np.int64).view(np.uint64)
 
 
-def run(n, cols, valid, program, out_types):
-    """cols: numpy arrays (storage dtype); valid: uint8 arrays or None.  Returns ([values], [valid])."""
+_T_OF_NP = {np.dtype(v): k for k, v in _NP_OF_T.items() if k not in (K.T_U16, K.T_U32, K.T_F16)}
+
+
+def run(n, cols, valid, program, out_types, col_types=None):
+    """cols: numpy arrays (storage dtype) read as K8 types ``col_types`` (default: the signed integer or
+    float of each array's dtype); valid: uint8 arrays or None.  Returns ([values], [valid]); outputs are
+    in their storage dtype (``kernels.EXPR_STORAGE``)."""
+    if col_types is None:
+        col_types = [_T_OF_NP[np.asarray(c).dtype] for c in cols]
     acc = np.zeros(n, dtype=np.uint64)
     accv = np.ones(n, dtype=bool)
     tmp = {}
@@ -38,7 +58,7 @@ def run(n, cols, valid, program, out_types):
             bv = np.ones(n, dtype=bool)
             bb = np.full(n, imm & ((1 << 64) - 1), dtype=np.uint64)
             if kind == K.XK_COL:
-                bb = _to_bits(cols[b])
+                bb = _to_bits(cols[b], col_types[b])
                 if valid[b] is not None:
                     bv = valid[b] != 0
             elif kind == K.XK_REG:
@@ -56,19 +76,20 @@ def run(n, cols, valid, program, out_types):
             elif op == K.X_OUT:
                 t = out_types[b]
                 vals = np.where(accv, acc, np.uint64(0))
-                if t in (K.T_F32, K.T_F64):
-                    outs[b] = _f(vals).astype(_NP_OF_T[t])
+                if t in (K.T_F16, K.T_F32, K.T_F64):
+                    o = _f(vals).astype(_NP_OF_T[t])  # numpy rounds a double to nearest even once
                 else:
-                    outs[b] = vals.view(np.int64).astype(_NP_OF_T[t])
+                    o = vals.view(np.int64).astype(_NP_OF_T[t])
+                outs[b] = o.view({K.T_U16: np.int16, K.T_U32: np.int32, K.T_F16: np.int16}.get(t, o.dtype))
                 outv[b] = accv.astype(np.uint8)
             elif op == K.X_I2F:
                 acc = _fb(xi.astype(np.float64))
             elif op == K.X_F2I:
-                acc = _ib(np.trunc(np.nan_to_num(_f(x), nan=0.0, posinf=0.0, neginf=0.0)))
+                acc = _ib(f2i(_f(x)))
             elif op == K.X_NEG_I:
                 acc = _ib(-xi)
             elif op == K.X_NEG_F:
-                acc = _fb(-_f(x))
+                acc = x ^ np.uint64(1 << 63)
             elif op == K.X_NOT:
                 acc = _ib(x == 0)
             elif op == K.X_IS_NULL:

@@ -173,8 +173,9 @@ def _collect_windows(e: Any, out: Dict[str, ColumnExpr]) -> None:
 
 def _with_windows(t: B200Table, cols: List[ColumnExpr]) -> B200Table:
     """Evaluate every window node of ``cols`` over the logical partitions of ``t``: arguments pre-projected
-    by the evaluator (K8), running / partition aggregates and ranks by the segmented scan (K9), FIRST /
-    LAST / partition values / LAG / LEAD by row gathers."""
+    by the evaluator (K8), running / partition aggregates and ranks by the segmented scan (K9), moving
+    frames (``rows``) by the frame kernel with the same finishers, FIRST / LAST / partition values / LAG /
+    LEAD by row gathers."""
     from . import expr as X
     from . import sort as S
     from .schema import Schema
@@ -224,13 +225,14 @@ def _with_windows(t: B200Table, cols: List[ColumnExpr]) -> B200Table:
         heads[off[:-1][lengths > 0]] = True
         return heads
 
-    # ---- scans: collected first, all run in one call
-    scans: List[Any] = []
+    # ---- scans: collected first, all run in one call per frame (None: the running scan)
+    scans: Dict[Any, List[Any]] = {}
     finish: List[Any] = []     # per node: (fingerprint, fn(scan results) -> (column, validity, type, dictionary))
 
-    def scan(op: int, v: Any, m: Any) -> int:
-        scans.append((op, v, m))
-        return len(scans) - 1
+    def scan(op: int, v: Any, m: Any, frame: Any = None) -> Tuple[Any, int]:
+        cols_ = scans.setdefault(frame, [])
+        cols_.append((op, v, m))
+        return frame, len(cols_) - 1
 
     for uid, bare in nodes.items():
         fn = bare.func
@@ -248,28 +250,28 @@ def _with_windows(t: B200Table, cols: List[ColumnExpr]) -> B200Table:
                 i = scan(K.AGG_SUM_I64, heads.to(torch.int64), None)
             finish.append((uid, lambda r, i=i: (r[i][0], None, pa.int64(), None)))
             continue
-        running = bare.kwargs["running"]
-        whole = None if running else seg_last
+        frame = bare.kwargs.get("rows")  # ROWS BETWEEN frame[0] AND frame[1]: the moving-frame kernel
+        whole = None if frame is not None or bare.kwargs["running"] else seg_last
 
         def at_end(x: torch.Tensor, whole: Any = whole) -> torch.Tensor:  # partition value: the scan at its last row
             return x if whole is None else x[whole()]
 
         if bare.arg.kind == Kind.WILDCARD:  # COUNT(*)
-            i = scan(K.AGG_COUNT, None, None)
+            i = scan(K.AGG_COUNT, None, None, frame)
             finish.append((uid, lambda r, i=i, e=at_end: (e(r[i][1]), None, pa.int64(), None)))
             continue
         name = arg_name[bare.arg.fingerprint()]
         ci = base.schema.index_of_key(name)
         c, m, tp = base.columns[ci], base.valid[ci], base.schema.types[ci]
         if fn == "COUNT":
-            i = scan(K.AGG_COUNT, None, m)
+            i = scan(K.AGG_COUNT, None, m, frame)
             finish.append((uid, lambda r, i=i, e=at_end: (e(r[i][1]), None, pa.int64(), None)))
             continue
         if fn in ("FIRST", "LAST"):
             # first / last valid row so far: MIN / MAX of the row number over the valid rows, then a gather
-            i = scan(K.AGG_MIN_I64 if fn == "FIRST" else K.AGG_MAX_I64, rows, m)
+            i = scan(K.AGG_MIN_I64 if fn == "FIRST" else K.AGG_MAX_I64, rows, m, frame)
 
-            def pick(r: Any, i: int = i, e: Any = at_end, c: Any = c, m: Any = m, tp: Any = tp, name: str = name) -> Any:
+            def pick(r: Any, i: Any = i, e: Any = at_end, c: Any = c, m: Any = m, tp: Any = tp, name: str = name) -> Any:
                 idx = torch.where(e(r[i][1]) > 0, e(r[i][0]), torch.full_like(rows, -1))
                 (g,), (gv,) = K.gather_rows([c], [m], idx.contiguous(), want_valid=True)
                 return g, gv, tp, base.dictionaries.get(name)
@@ -283,10 +285,10 @@ def _with_windows(t: B200Table, cols: List[ColumnExpr]) -> B200Table:
             f64 = fn == "AVG" or is_f
             v8 = widen(c, tp)
             v8 = (v8.to(torch.float64) if f64 else v8).contiguous()
-            i = scan(K.AGG_SUM_F64 if f64 else K.AGG_SUM_I64, v8, m)
+            i = scan(K.AGG_SUM_F64 if f64 else K.AGG_SUM_I64, v8, m, frame)
             out_tp = pa.float64() if f64 else pa.int64()
 
-            def total(r: Any, i: int = i, e: Any = at_end, avg: bool = fn == "AVG", out_tp: Any = out_tp) -> Any:
+            def total(r: Any, i: Any = i, e: Any = at_end, avg: bool = fn == "AVG", out_tp: Any = out_tp) -> Any:
                 v, cnt = e(r[i][0]), e(r[i][1])
                 if avg:
                     v = v / cnt.to(torch.float64)
@@ -298,16 +300,20 @@ def _with_windows(t: B200Table, cols: List[ColumnExpr]) -> B200Table:
             v8 = widen(c, tp).contiguous()
             op = {("MIN", True): K.AGG_MIN_F64, ("MAX", True): K.AGG_MAX_F64,
                   ("MIN", False): K.AGG_MIN_I64, ("MAX", False): K.AGG_MAX_I64}[(fn, is_f)]
-            i = scan(op, v8, m)
+            i = scan(op, v8, m, frame)
 
-            def extreme(r: Any, i: int = i, e: Any = at_end, tp: Any = tp) -> Any:
+            def extreme(r: Any, i: Any = i, e: Any = at_end, tp: Any = tp) -> Any:
                 v, cnt = e(r[i][0]), e(r[i][1])
                 return narrow(v, tp).contiguous(), (cnt > 0).to(torch.uint8), tp, None
 
             finish.append((uid, extreme))
             continue
         raise NotImplementedError(f"window function {fn}")  # pragma: no cover - builders admit no other
-    results = K.segmented_scan(off.contiguous(), n, scans) if scans else []
+    results: Dict[Tuple[Any, int], Any] = {}
+    for frame, spec in scans.items():
+        res = K.segmented_scan(off.contiguous(), n, spec) if frame is None else \
+            K.window_frame(off.contiguous(), n, frame[0], frame[1], spec)
+        results.update(((frame, j), r) for j, r in enumerate(res))
     names, types, columns, valid = list(base.schema.names), list(base.schema.types), list(base.columns), list(base.valid)
     dicts = dict(base.dictionaries)
     window_names: Dict[str, str] = {}

@@ -7,8 +7,8 @@ from an expression is a function of ``(kind, head, args)``:
     LITERAL   head = python value (None = NULL)      UNARY     head in ``- ~ IS_NULL NOT_NULL``, one arg
     BINARY    head in ``+ - * / & | < > <= >= == !=``  CALL      head = function name (``COALESCE`` ...)
     AGG       head in ``SUM COUNT AVG MIN MAX FIRST LAST``, one arg, optional DISTINCT
-    WINDOW    head in the AGG functions (one arg, kwargs ``running``), ``ROW_NUMBER RANK DENSE_RANK`` (no
-              arg) or ``LAG LEAD`` (one arg, kwargs ``n`` and ``default``): evaluated over the logical
+    WINDOW    head in the AGG functions (one arg, kwargs ``running`` or ``rows``), ``ROW_NUMBER RANK
+              DENSE_RANK`` (no arg) or ``LAG LEAD`` (one arg, kwargs ``n`` and ``default``): evaluated over the logical
               partitions of ``fa.transform`` (PartitionSpec keys, presort order) by a ``ColumnMap``
 
 plus an optional output alias and an optional cast of the node's result.  ``fugue_b200/expr.py`` compiles
@@ -254,10 +254,13 @@ class ColumnExpr:
     def __invert__(self) -> "ColumnExpr":
         return ColumnExpr(Kind.UNARY, "~", [self])
 
-    def over(self, running: bool = False) -> "ColumnExpr":
+    def over(self, running: bool = False, rows: Optional[Tuple[Optional[int], Optional[int]]] = None) -> "ColumnExpr":
         """The aggregation as a window function of a ``ColumnMap``: over the whole logical partition
-        (``running=False``, the value repeated on every row) or over the rows up to and including the
-        current one in presort order (``running=True``)."""
+        (``running=False``, the value repeated on every row), over the rows up to and including the
+        current one in presort order (``running=True``), or over a moving frame ``rows=(start, end)``:
+        ``ROWS BETWEEN`` offsets from the current row in presort order, negative PRECEDING, 0 CURRENT ROW,
+        positive FOLLOWING, ``None`` UNBOUNDED.  ``rows=(None, 0)`` is ``running=True`` and
+        ``rows=(None, None)`` the whole partition: both give those nodes."""
         if self.kind != Kind.AGG:
             raise ValueError(f"{self} is not an aggregation: only an aggregation has an OVER form")
         if self.is_distinct:
@@ -266,11 +269,26 @@ class ColumnExpr:
             raise ValueError(f"{self}: {self.head} has no window form")
         if not isinstance(running, bool):
             raise ValueError(f"running must be a bool, got {running!r}")
+        if rows is not None:
+            if running:
+                raise ValueError("over() takes running=True or rows, not both")
+            if not isinstance(rows, tuple) or len(rows) != 2:
+                raise ValueError(f"rows must be a (start, end) tuple, got {rows!r}")
+            for b in rows:
+                if isinstance(b, bool) or not (b is None or isinstance(b, int)):
+                    raise ValueError(f"a frame bound must be an int or None, got {b!r}")
+            if rows[0] is not None and rows[1] is not None and rows[0] > rows[1]:
+                raise ValueError(f"frame start {rows[0]} is after its end {rows[1]}")
+            if rows == (None, 0):
+                running, rows = True, None
+            elif rows == (None, None):
+                rows = None
         if is_agg(self.args[0]) or has_window(self.args[0]):
             raise ValueError(f"nested aggregation {self}")
         if self.head in ("FIRST", "LAST") and self.args[0].kind == Kind.WILDCARD:
             raise ValueError(f"{self}: {self.head} needs a column")
-        return ColumnExpr(Kind.WINDOW, self.head, self.args, {"running": running}, False, self.as_name, self.as_type)
+        kwargs = {"running": running} if rows is None else {"rows": (rows[0], rows[1])}
+        return ColumnExpr(Kind.WINDOW, self.head, self.args, kwargs, False, self.as_name, self.as_type)
 
     def __bool__(self) -> bool:
         raise TypeError("a column expression has no truth value; use & | ~ to combine conditions")
@@ -366,7 +384,18 @@ def _window_text(e: ColumnExpr, show: Any) -> str:
     if e.head in ("LAG", "LEAD"):
         parts += [str(e.kwargs["n"]), _show_literal(e.kwargs["default"])]
     frame = _RUNNING_FRAME if e.kwargs.get("running", False) else ""
+    if "rows" in e.kwargs:
+        frame = f"ROWS BETWEEN {_frame_bound(e.kwargs['rows'][0], 'PRECEDING')} AND " \
+                f"{_frame_bound(e.kwargs['rows'][1], 'FOLLOWING')}"
     return f"{e.head}({','.join(parts)}) OVER ({frame})"
+
+
+def _frame_bound(b: Optional[int], unbounded: str) -> str:
+    if b is None:
+        return "UNBOUNDED " + unbounded
+    if b == 0:
+        return "CURRENT ROW"
+    return f"{-b} PRECEDING" if b < 0 else f"{b} FOLLOWING"
 
 
 def _offset_fn(name: str, c: Any, n: Any, default: Any) -> ColumnExpr:

@@ -13,6 +13,21 @@
 // prefixes or aggregates depending on timing, which changes the rounding of a float sum between runs.
 // Segment heads never exist as a per-row array in HBM: a tile binary-searches the segment offsets
 // for its first row and marks the heads that fall inside it in shared memory.
+//
+// Moving frames (ROWS BETWEEN start AND end, fb_window_frame) use van Herk / Gil-Werman: rows are cut
+// into blocks of W = end - start + 1 rows aligned to multiples of W, and two scans restart at every
+// block as well as every segment bound: P[i], op from the later of (block start, segment start) to i, and
+// S[i], op from i to the earlier of (block end, segment end).  A frame [lo, hi] clipped to its segment
+// holds at most W rows, so it lies in at most two blocks: it is S[lo] (+) P[hi] when it crosses a block
+// bound, else P[hi] when lo is where P[hi]'s run starts, else S[lo] (hi is then where S[lo]'s run ends).
+// O(1) per row for every op, exact for MIN / MAX, and every f64 sum adds frame values only.
+//   - W <= FB_FRAME_TILE_MAX_WIDTH: one launch; a CTA stages its rows plus the W - 1 halo in shared
+//     memory, scans P and S there and writes each output once (inputs read 1 + (W - 1) / tile times).
+//   - otherwise, and with an unbounded side: P and S by the three-launch scan above (block heads added,
+//     S walking rows in reverse) into scratch, then a combine launch.  (None, e) is P without blocks read
+//     at hi; (s, None) is S without blocks read at lo.
+#include <mutex>
+
 #include "fb_common.cuh"
 
 namespace {
@@ -81,17 +96,27 @@ __device__ __forceinline__ St shfl_up(const St& s, int d) {
   return r;
 }
 
+__device__ __forceinline__ St shfl_down(const St& s, int d) {
+  St r;
+  r.v = __shfl_down_sync(0xFFFFFFFFu, (unsigned long long)s.v, d);
+  r.c = __shfl_down_sync(0xFFFFFFFFu, (long long)s.c, d);
+  r.f = __shfl_down_sync(0xFFFFFFFFu, s.f, d);
+  return r;
+}
+
 // Exclusive scan of one state per thread across the CTA, and the CTA total; fixed combination order.
-template <int kWarps>
+// kRev: the scan runs from the last thread to the first.
+template <int kWarps, bool kRev = false>
 __device__ __forceinline__ St block_exclusive(int op, const St& x, St* warp_tot, St* total) {
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  const int lane = kRev ? 31 - (threadIdx.x & 31) : threadIdx.x & 31;
+  const int w = kRev ? kWarps - 1 - (int)(threadIdx.x >> 5) : threadIdx.x >> 5;
   St inc = x;
 #pragma unroll
   for (int d = 1; d < 32; d <<= 1) {
-    const St o = shfl_up(inc, d);
+    const St o = kRev ? shfl_down(inc, d) : shfl_up(inc, d);
     if (lane >= d) inc = combine(op, o, inc);
   }
-  const St ex = shfl_up(inc, 1);
+  const St ex = kRev ? shfl_down(inc, 1) : shfl_up(inc, 1);
   if (lane == 31) warp_tot[w] = inc;
   __syncthreads();
   St pre{0, 0, 0}, tot{0, 0, 0};
@@ -122,6 +147,14 @@ __device__ __forceinline__ int64_t lower_bound(const int64_t* __restrict__ a, in
   return lo;
 }
 
+// smallest multiple of b >= x (x >= 0, b >= 1, both below 2^53) without a 64-bit division call
+__device__ __forceinline__ int64_t first_multiple(int64_t x, int64_t b) {
+  int64_t q = (int64_t)((double)x * __drcp_rn((double)b));  // within a few units of x / b
+  while (q * b < x) ++q;
+  while (q > 0 && (q - 1) * b >= x) --q;
+  return q * b;
+}
+
 struct TileSmem {
   uint64_t v[padded(kTile)];
   int64_t c[padded(kTile)];
@@ -131,28 +164,47 @@ struct TileSmem {
   int64_t seg_range[2];
 };
 
-// kFinal = false: pass 1 (tile aggregates); true: pass 3 (outputs, from the carries of pass 2)
-template <bool kFinal>
+// kFinal = false: pass 1 (tile aggregates); true: pass 3 (outputs, from the carries of pass 2).
+// The scan runs over positions p; position p is row p, or row nrows - 1 - p when kReverse (then a run
+// restarts after every segment's last row).  block > 0 also restarts the runs at every row that is a
+// multiple of `block` (kReverse: every row r with r + 1 a multiple of `block`); only with kBlocks, so that the
+// plain scan compiles without it.
+template <bool kFinal, bool kReverse = false, bool kBlocks = false>
 __global__ void __launch_bounds__(kThreads)
 fb_segscan_tile_kernel(int64_t nrows, int64_t nseg, const int64_t* __restrict__ offsets,
                        const __grid_constant__ ScanCols a, int64_t ntiles, uint64_t* __restrict__ tile_v,
-                       int64_t* __restrict__ tile_c, int32_t* __restrict__ tile_f) {
+                       int64_t* __restrict__ tile_c, int32_t* __restrict__ tile_f, int64_t block = 0) {
   __shared__ __align__(16) TileSmem sm;
   const int64_t tile = blockIdx.x;
   const int64_t start = tile * kTile;
   const int64_t end = start + kTile < nrows ? start + kTile : nrows;
   const int nloc = (int)(end - start);
-  // ---- segment heads inside [start, end): offsets[s] for s in [segment of `start`, first offset >= end)
+  // row of the tile's position i
+  const int64_t row0 = kReverse ? nrows - 1 - start : start;
+  auto row = [row0](int i) -> int64_t { return kReverse ? row0 - i : row0 + i; };
+  // ---- segment heads inside [start, end): offsets[s] for s in [segment of `start`, first offset >= end);
+  // reversed, offsets o in [nrows - end + 1, nrows - start] (row o - 1 ends a segment) at position nrows - o
   for (int i = threadIdx.x; i < kTile; i += kThreads) sm.head[i] = 0;
   if (threadIdx.x == 0) {
-    const int64_t s0 = upper_bound(offsets, nseg + 1, start) - 1;
-    sm.seg_range[0] = s0 < 0 ? 0 : s0;
-    sm.seg_range[1] = lower_bound(offsets, nseg + 1, end);
+    if (kReverse) {
+      sm.seg_range[0] = upper_bound(offsets, nseg + 1, nrows - end);
+      sm.seg_range[1] = upper_bound(offsets, nseg + 1, nrows - start);
+    } else {
+      const int64_t s0 = upper_bound(offsets, nseg + 1, start) - 1;
+      sm.seg_range[0] = s0 < 0 ? 0 : s0;
+      sm.seg_range[1] = lower_bound(offsets, nseg + 1, end);
+    }
   }
   __syncthreads();
   for (int64_t s = sm.seg_range[0] + threadIdx.x; s < sm.seg_range[1]; s += kThreads) {
     const int64_t o = __ldg(offsets + s);
-    if (o >= start && o < end) sm.head[o - start] = 1;
+    const int64_t p = kReverse ? nrows - o : o;
+    if (p >= start && p < end) sm.head[p - start] = 1;
+  }
+  if (kBlocks) {  // multiples m of `block` with position (m, or nrows - m reversed) inside the tile
+    const int64_t lo = kReverse ? nrows - end + 1 : start, hi = kReverse ? nrows - start : end - 1;
+    for (int64_t m = first_multiple(lo, block) + threadIdx.x * block; m <= hi; m += kThreads * block)
+      sm.head[(kReverse ? nrows - m : m) - start] = 1;
   }
   const int j0 = threadIdx.x * kItems;
   for (int col = 0; col < a.ncols; ++col) {
@@ -163,8 +215,8 @@ fb_segscan_tile_kernel(int64_t nrows, int64_t nseg, const int64_t* __restrict__ 
     // striped (coalesced) loads into shared memory; rows past the end are invalid
     for (int i = threadIdx.x; i < kTile; i += kThreads) {
       const bool in = i < nloc;
-      if (!is_count) sm.v[padded(i)] = in ? __ldg((const unsigned long long*)src + start + i) : 0;
-      sm.valid[i] = in ? (vm == nullptr ? 1 : (__ldg(vm + start + i) != 0)) : 0;
+      if (!is_count) sm.v[padded(i)] = in ? __ldg((const unsigned long long*)src + row(i)) : 0;
+      sm.valid[i] = in ? (vm == nullptr ? 1 : (__ldg(vm + row(i)) != 0)) : 0;
     }
     __syncthreads();
     St acc{0, 0, 0};
@@ -199,8 +251,8 @@ fb_segscan_tile_kernel(int64_t nrows, int64_t nseg, const int64_t* __restrict__ 
     uint64_t* __restrict__ ov = (uint64_t*)a.out_vals[col];
     int64_t* __restrict__ oc = a.out_count[col];
     for (int i = threadIdx.x; i < nloc; i += kThreads) {
-      if (ov != nullptr) ov[start + i] = sm.v[padded(i)];
-      if (oc != nullptr) oc[start + i] = sm.c[padded(i)];
+      if (ov != nullptr) ov[row(i)] = sm.v[padded(i)];
+      if (oc != nullptr) oc[row(i)] = sm.c[padded(i)];
     }
     __syncthreads();  // shared buffers are refilled by the next column
   }
@@ -232,6 +284,281 @@ fb_segscan_carry_kernel(int64_t ntiles, const __grid_constant__ ScanCols a, uint
 
 int64_t num_tiles(int64_t nrows) { return (nrows + kTile - 1) / kTile; }
 
+// ---- moving frames -------------------------------------------------------------------------------
+constexpr int kFrameThreads = 256;
+constexpr int kFrameItems = 8;                          // consecutive staged rows per thread
+constexpr int kFrameSpan = kFrameThreads * kFrameItems;  // staged rows per CTA: outputs + W - 1 halo
+static_assert(2 * FB_FRAME_TILE_MAX_WIDTH == kFrameSpan, "a CTA at the widest frame writes about half its span");
+static_assert(kFrameItems == 8, "padded() assumes 8 rows per thread");
+
+// which of P[hi] / S[lo] make up a row's frame; packed with lo and hi (staged indices, 11 bits each)
+enum : uint32_t { kFrameEmpty = 0, kFrameP = 1, kFrameS = 2, kFrameBoth = 3 };
+
+__device__ __forceinline__ uint32_t frame_code(int lo, int hi, int blk_lo, int blk_hi, int p_start) {
+  const uint32_t mode = blk_lo != blk_hi ? kFrameBoth : (lo == p_start ? kFrameP : kFrameS);
+  return mode | (uint32_t)lo << 2 | (uint32_t)hi << 13;
+}
+
+struct FrameSmem {
+  uint64_t pv[padded(kFrameSpan)];  // staged values, then P
+  uint64_t sv[padded(kFrameSpan)];
+  int32_t pc[padded(kFrameSpan)];   // a frame has at most kFrameSpan rows: int32 counts
+  int32_t sc[padded(kFrameSpan)];
+  uint8_t valid[kFrameSpan];
+  uint8_t heads[kFrameSpan];        // bit 0: a P run starts at the row; bit 1: an S run ends at it
+  uint8_t seg_head[kFrameSpan + 1];
+  St warp_tot[kFrameThreads / 32];
+  int64_t range[4];
+};
+
+// One CTA per `per_tile` output rows [o0, o1): stage rows [s0, s1) = [o0 + start, o1 + end) clipped to the
+// table (every frame of the tile lies inside), scan P and S there, write value and count once.
+__global__ void __launch_bounds__(kFrameThreads)
+fb_window_frame_tile_kernel(int64_t nrows, int64_t nseg, const int64_t* __restrict__ offsets,
+                            const __grid_constant__ ScanCols a, int64_t start, int width, int64_t per_tile) {
+  extern __shared__ __align__(16) unsigned char frame_smem[];
+  FrameSmem& sm = *reinterpret_cast<FrameSmem*>(frame_smem);
+  const int64_t end = start + width - 1;
+  const int64_t o0 = (int64_t)blockIdx.x * per_tile;
+  const int64_t o1 = o0 + per_tile < nrows ? o0 + per_tile : nrows;
+  const int64_t s0 = o0 + start > 0 ? o0 + start : 0;
+  const int64_t s1 = o1 + end < nrows ? o1 + end : nrows;
+  const int nloc = s1 > s0 ? (int)(s1 - s0) : 0;
+  // ---- segments: starts inside [s0, s1] marked in shared memory; the segments of the output rows
+  for (int i = threadIdx.x; i <= kFrameSpan; i += kFrameThreads) sm.seg_head[i] = 0;
+  if (threadIdx.x == 0) {
+    sm.range[0] = lower_bound(offsets, nseg + 1, s0);
+    sm.range[1] = upper_bound(offsets, nseg + 1, s1);
+    sm.range[2] = upper_bound(offsets, nseg + 1, o0) - 1;      // segment of o0
+    sm.range[3] = upper_bound(offsets, nseg + 1, o1 - 1) + 1;  // one past the offset ending o1 - 1's segment
+  }
+  __syncthreads();
+  for (int64_t s = sm.range[0] + threadIdx.x; s < sm.range[1]; s += kFrameThreads)
+    sm.seg_head[__ldg(offsets + s) - s0] = 1;
+  __syncthreads();
+  const int64_t m0 = first_multiple(s0, width);
+  const int rem0 = m0 == s0 ? 0 : (int)(s0 - (m0 - width));  // s0 % W: blocks are aligned to multiples of W
+  for (int j = threadIdx.x; j < kFrameSpan; j += kFrameThreads) {
+    const bool p = sm.seg_head[j] || (rem0 + j) % width == 0;
+    const bool s = j + 1 >= nloc || sm.seg_head[j + 1] || (rem0 + j + 1) % width == 0;
+    sm.heads[j] = (uint8_t)(p | s << 1);
+  }
+  // ---- every output row's frame [lo, hi] in staged rows; thread t has rows o0 + t + kFrameThreads * k
+  uint32_t code[kFrameItems];
+  const int64_t q0 = sm.range[2], nq = sm.range[3] - q0;
+#pragma unroll
+  for (int k = 0; k < kFrameItems; ++k) {
+    const int64_t i = o0 + threadIdx.x + (int64_t)kFrameThreads * k;
+    code[k] = kFrameEmpty;
+    if (i >= o1) continue;
+    const int64_t q = q0 + upper_bound(offsets + q0, nq, i) - 1;
+    const int64_t sa = __ldg(offsets + q), sb = __ldg(offsets + q + 1);
+    const int64_t lo = i + start > sa ? i + start : sa;
+    const int64_t hi = i + end < sb - 1 ? i + end : sb - 1;
+    if (lo > hi) continue;
+    const int jl = (int)(lo - s0), jh = (int)(hi - s0);  // staged rows
+    const int bs = jh - (rem0 + jh) % width;                // start of hi's block
+    const int ja = sa > s0 ? (int)(sa - s0) : 0;            // segment start, or the first staged row
+    const int ps = bs > ja ? bs : ja;                       // where P[hi]'s run starts
+    code[k] = frame_code(jl, jh, (rem0 + jl) / width, (rem0 + jh) / width, ps);
+  }
+  const int j0 = threadIdx.x * kFrameItems;
+  for (int col = 0; col < a.ncols; ++col) {
+    const int op = a.op[col];
+    const bool is_count = op == FB_AGG_COUNT;
+    const uint64_t* __restrict__ src = (const uint64_t*)a.vals[col];
+    const uint8_t* __restrict__ vm = a.valid[col];
+    for (int i = threadIdx.x; i < kFrameSpan; i += kFrameThreads) {
+      const bool in = i < nloc;
+      if (!is_count) sm.pv[padded(i)] = in ? __ldg((const unsigned long long*)src + s0 + i) : 0;
+      sm.valid[i] = in ? (vm == nullptr ? 1 : (__ldg(vm + s0 + i) != 0)) : 0;
+    }
+    __syncthreads();
+    uint64_t x[kFrameItems];
+    uint32_t ok = 0, hd = 0;
+#pragma unroll
+    for (int k = 0; k < kFrameItems; ++k) {
+      const int j = j0 + k;
+      x[k] = is_count ? 0 : sm.pv[padded(j)];
+      ok |= (uint32_t)(sm.valid[j] != 0) << k;
+      hd |= (uint32_t)sm.heads[j] << (2 * k);
+    }
+    // P: forward over the staged rows
+    St acc{0, 0, 0}, total;
+#pragma unroll
+    for (int k = 0; k < kFrameItems; ++k) {
+      const int c = (ok >> k) & 1;
+      acc = combine(op, acc, St{c ? x[k] : 0, c, (int32_t)((hd >> (2 * k)) & 1)});
+    }
+    St run = block_exclusive<kFrameThreads / 32>(op, acc, sm.warp_tot, &total);  // all x[] read before pv is written
+#pragma unroll
+    for (int k = 0; k < kFrameItems; ++k) {
+      const int c = (ok >> k) & 1;
+      run = combine(op, run, St{c ? x[k] : 0, c, (int32_t)((hd >> (2 * k)) & 1)});
+      sm.pv[padded(j0 + k)] = run.c > 0 ? run.v : 0;
+      sm.pc[padded(j0 + k)] = (int32_t)run.c;
+    }
+    // S: backward
+    acc = St{0, 0, 0};
+#pragma unroll
+    for (int k = kFrameItems - 1; k >= 0; --k) {
+      const int c = (ok >> k) & 1;
+      acc = combine(op, acc, St{c ? x[k] : 0, c, (int32_t)((hd >> (2 * k + 1)) & 1)});
+    }
+    run = block_exclusive<kFrameThreads / 32, true>(op, acc, sm.warp_tot, &total);
+#pragma unroll
+    for (int k = kFrameItems - 1; k >= 0; --k) {
+      const int c = (ok >> k) & 1;
+      run = combine(op, run, St{c ? x[k] : 0, c, (int32_t)((hd >> (2 * k + 1)) & 1)});
+      sm.sv[padded(j0 + k)] = run.c > 0 ? run.v : 0;
+      sm.sc[padded(j0 + k)] = (int32_t)run.c;
+    }
+    __syncthreads();
+    uint64_t* __restrict__ ov = (uint64_t*)a.out_vals[col];
+    int64_t* __restrict__ oc = a.out_count[col];
+#pragma unroll
+    for (int k = 0; k < kFrameItems; ++k) {
+      const int64_t i = o0 + threadIdx.x + (int64_t)kFrameThreads * k;
+      if (i >= o1) break;
+      const uint32_t mode = code[k] & 3;
+      const int lo = (int)((code[k] >> 2) & 0x7FF), hi = (int)((code[k] >> 13) & 0x7FF);
+      St r{0, 0, 0};
+      if (mode & kFrameS) r = St{sm.sv[padded(lo)], sm.sc[padded(lo)], 0};
+      if (mode & kFrameP) r = combine(op, r, St{sm.pv[padded(hi)], sm.pc[padded(hi)], 0});
+      if (ov != nullptr) ov[i] = r.c > 0 ? r.v : 0;
+      if (oc != nullptr) oc[i] = r.c;
+    }
+    __syncthreads();  // shared buffers are refilled by the next column
+  }
+}
+
+// The frames from P and S in scratch (pv / pc / sv / sc: ncols x nrows; P or S unused with an unbounded
+// side).  width == 0: no blocks.  One CTA per kTile rows.
+__global__ void __launch_bounds__(kThreads)
+fb_window_frame_combine_kernel(int64_t nrows, int64_t nseg, const int64_t* __restrict__ offsets,
+                               const __grid_constant__ ScanCols a, int64_t start, int64_t end, int flags,
+                               int64_t width, const uint64_t* __restrict__ pv, const int64_t* __restrict__ pc,
+                               const uint64_t* __restrict__ sv, const int64_t* __restrict__ sc) {
+  __shared__ int64_t range[2];
+  const int64_t t0 = (int64_t)blockIdx.x * kTile;
+  const int64_t t1 = t0 + kTile < nrows ? t0 + kTile : nrows;
+  if (threadIdx.x == 0) {
+    range[0] = upper_bound(offsets, nseg + 1, t0) - 1;
+    range[1] = upper_bound(offsets, nseg + 1, t1 - 1) + 1;
+  }
+  __syncthreads();
+  const int64_t q0 = range[0], nq = range[1] - q0;
+  for (int64_t i = t0 + threadIdx.x; i < t1; i += kThreads) {
+    const int64_t q = q0 + upper_bound(offsets + q0, nq, i) - 1;
+    const int64_t sa = __ldg(offsets + q), sb = __ldg(offsets + q + 1);
+    const int64_t lo = (flags & FB_FRAME_UNBOUNDED_START) || i + start < sa ? sa : i + start;
+    const int64_t hi = (flags & FB_FRAME_UNBOUNDED_END) || i + end > sb - 1 ? sb - 1 : i + end;
+    uint32_t mode = kFrameEmpty;
+    if (lo <= hi) {
+      if (flags & FB_FRAME_UNBOUNDED_START) mode = kFrameP;
+      else if (flags & FB_FRAME_UNBOUNDED_END) mode = kFrameS;
+      else {
+        const int64_t bs = hi - hi % width;
+        mode = lo / width != hi / width ? kFrameBoth : (lo == (bs > sa ? bs : sa) ? kFrameP : kFrameS);
+      }
+    }
+    for (int col = 0; col < a.ncols; ++col) {
+      const int op = a.op[col];
+      const int64_t base = col * nrows;
+      St r{0, 0, 0};
+      if (mode & kFrameS) r = St{sv[base + lo], sc[base + lo], 0};
+      if (mode & kFrameP) r = combine(op, r, St{pv[base + hi], pc[base + hi], 0});
+      if (a.out_vals[col] != nullptr) ((uint64_t*)a.out_vals[col])[i] = r.c > 0 ? r.v : 0;
+      if (a.out_count[col] != nullptr) a.out_count[col][i] = r.c;
+    }
+  }
+}
+
+// A frame on `nrows` rows, bounds clipped to [-nrows, nrows] (no sum below overflows) and a bound that
+// reaches past every segment made unbounded: both exact, as no segment is longer than the table.
+struct Frame {
+  int64_t start, end, width;  // width: end - start + 1 with both sides bounded, else 0
+  int flags;
+  bool tile;                  // the one-pass path
+};
+
+Frame make_frame(int64_t nrows, int64_t start, int64_t end, int flags) {
+  Frame f;
+  f.flags = flags & (FB_FRAME_UNBOUNDED_START | FB_FRAME_UNBOUNDED_END);
+  f.start = start < -nrows ? -nrows : (start > nrows ? nrows : start);
+  f.end = end < -nrows ? -nrows : (end > nrows ? nrows : end);
+  if (f.start <= -nrows) f.flags |= FB_FRAME_UNBOUNDED_START;
+  if (f.end >= nrows) f.flags |= FB_FRAME_UNBOUNDED_END;
+  f.width = f.flags == 0 ? f.end - f.start + 1 : 0;
+  f.tile = f.flags == 0 && f.width <= FB_FRAME_TILE_MAX_WIDTH;
+  return f;
+}
+
+size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
+
+size_t frame_scratch(int64_t nrows, int ncols, const Frame& f) {
+  if (nrows <= 0 || ncols <= 0 || f.tile) return 0;
+  const int sides = f.flags == 0 ? 2 : 1;
+  return align256(fb_segmented_scan_scratch_bytes(nrows, ncols)) + (size_t)sides * 16 * ncols * (size_t)nrows;
+}
+
+// one inclusive scan (P, or S when reverse) of every column into out_vals / out_count, blocks of `block` rows
+int run_scan(cudaStream_t st, bool reverse, int64_t block, int64_t nrows, int64_t nseg, const int64_t* offsets,
+             const ScanCols& a, void* tiles) {
+  const int64_t ntiles = num_tiles(nrows);
+  uint64_t* tile_v = (uint64_t*)tiles;
+  int64_t* tile_c = (int64_t*)(tile_v + a.ncols * ntiles);
+  int32_t* tile_f = (int32_t*)(tile_c + a.ncols * ntiles);
+  const unsigned grid = (unsigned)ntiles;
+  if (reverse && block > 0)
+    fb_segscan_tile_kernel<false, true, true><<<grid, kThreads, 0, st>>>(nrows, nseg, offsets, a, ntiles, tile_v,
+                                                                         tile_c, tile_f, block);
+  else if (reverse)
+    fb_segscan_tile_kernel<false, true><<<grid, kThreads, 0, st>>>(nrows, nseg, offsets, a, ntiles, tile_v, tile_c,
+                                                                   tile_f);
+  else if (block > 0)
+    fb_segscan_tile_kernel<false, false, true><<<grid, kThreads, 0, st>>>(nrows, nseg, offsets, a, ntiles, tile_v,
+                                                                          tile_c, tile_f, block);
+  else
+    fb_segscan_tile_kernel<false><<<grid, kThreads, 0, st>>>(nrows, nseg, offsets, a, ntiles, tile_v, tile_c, tile_f);
+  FB_CUDA(cudaGetLastError());
+  fb_segscan_carry_kernel<<<a.ncols, kCarryThreads, 0, st>>>(ntiles, a, tile_v, tile_c, tile_f);
+  FB_CUDA(cudaGetLastError());
+  if (reverse && block > 0)
+    fb_segscan_tile_kernel<true, true, true><<<grid, kThreads, 0, st>>>(nrows, nseg, offsets, a, ntiles, tile_v,
+                                                                        tile_c, tile_f, block);
+  else if (reverse)
+    fb_segscan_tile_kernel<true, true><<<grid, kThreads, 0, st>>>(nrows, nseg, offsets, a, ntiles, tile_v, tile_c,
+                                                                  tile_f);
+  else if (block > 0)
+    fb_segscan_tile_kernel<true, false, true><<<grid, kThreads, 0, st>>>(nrows, nseg, offsets, a, ntiles, tile_v,
+                                                                         tile_c, tile_f, block);
+  else
+    fb_segscan_tile_kernel<true><<<grid, kThreads, 0, st>>>(nrows, nseg, offsets, a, ntiles, tile_v, tile_c, tile_f);
+  FB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// the column arrays of the C ABI -> ScanCols (checked)
+int scan_cols(int64_t nrows, int ncols, const int32_t* ops, const void* const* vals, const uint8_t* const* valid,
+              void* const* out_vals, int64_t* const* out_count, ScanCols* a) {
+  FB_CHECK(ncols >= 1 && ncols <= FB_SCAN_MAX_COLS, "ncols=%d out of range [1,%d]", ncols, FB_SCAN_MAX_COLS);
+  FB_CHECK(ops != nullptr, "NULL ops");
+  memset(a, 0, sizeof(*a));
+  a->ncols = ncols;
+  for (int c = 0; c < ncols; ++c) {
+    FB_CHECK(ops[c] >= FB_AGG_SUM_F64 && ops[c] <= FB_AGG_MAX_F64, "column %d: unknown scan op %d", c, ops[c]);
+    a->op[c] = ops[c];
+    a->vals[c] = vals != nullptr ? vals[c] : nullptr;
+    a->valid[c] = valid != nullptr ? valid[c] : nullptr;
+    a->out_vals[c] = out_vals != nullptr ? out_vals[c] : nullptr;
+    a->out_count[c] = out_count != nullptr ? out_count[c] : nullptr;
+    FB_CHECK(nrows == 0 || ops[c] == FB_AGG_COUNT || a->vals[c] != nullptr, "column %d: op %d needs a value column", c,
+             ops[c]);
+  }
+  return 0;
+}
+
 }  // namespace
 
 extern "C" size_t fb_segmented_scan_scratch_bytes(int64_t nrows, int ncols) {
@@ -244,39 +571,87 @@ extern "C" int fb_segmented_scan(int dev, void* stream, int64_t nrows, int64_t n
                                  const uint8_t* const* valid, void* const* out_vals, int64_t* const* out_count,
                                  void* scratch, size_t scratch_bytes) {
   FB_CHECK(nrows >= 0 && nseg >= 0, "negative row or segment count");
-  FB_CHECK(ncols >= 1 && ncols <= FB_SCAN_MAX_COLS, "ncols=%d out of range [1,%d]", ncols, FB_SCAN_MAX_COLS);
-  FB_CHECK(ops != nullptr, "NULL ops");
   ScanCols a;
-  memset(&a, 0, sizeof(a));
-  a.ncols = ncols;
-  for (int c = 0; c < ncols; ++c) {
-    FB_CHECK(ops[c] >= FB_AGG_SUM_F64 && ops[c] <= FB_AGG_MAX_F64, "column %d: unknown scan op %d", c, ops[c]);
-    a.op[c] = ops[c];
-    a.vals[c] = vals != nullptr ? vals[c] : nullptr;
-    a.valid[c] = valid != nullptr ? valid[c] : nullptr;
-    a.out_vals[c] = out_vals != nullptr ? out_vals[c] : nullptr;
-    a.out_count[c] = out_count != nullptr ? out_count[c] : nullptr;
-    FB_CHECK(nrows == 0 || ops[c] == FB_AGG_COUNT || a.vals[c] != nullptr, "column %d: op %d needs a value column", c, ops[c]);
-  }
+  if (scan_cols(nrows, ncols, ops, vals, valid, out_vals, out_count, &a) != 0) return 1;
   if (nrows == 0) return 0;
   FB_CHECK(nseg >= 1 && d_offsets != nullptr, "%lld rows need at least one segment", (long long)nrows);
-  const int64_t ntiles = num_tiles(nrows);
-  FB_CHECK(ntiles < (1LL << 31), "too many rows");
+  FB_CHECK(num_tiles(nrows) < (1LL << 31), "too many rows");
   FB_CHECK(scratch != nullptr && scratch_bytes >= fb_segmented_scan_scratch_bytes(nrows, ncols),
            "scratch too small: %zu < %zu", scratch_bytes, fb_segmented_scan_scratch_bytes(nrows, ncols));
   FbDeviceGuard guard(dev);
   FB_CHECK(guard.ok, "cannot select device %d", dev);
-  uint64_t* tile_v = (uint64_t*)scratch;
-  int64_t* tile_c = (int64_t*)(tile_v + ncols * ntiles);
-  int32_t* tile_f = (int32_t*)(tile_c + ncols * ntiles);
+  return run_scan((cudaStream_t)stream, false, 0, nrows, nseg, d_offsets, a, scratch);
+}
+
+extern "C" size_t fb_window_frame_scratch_bytes(int64_t nrows, int ncols, int64_t start, int64_t end, int flags) {
+  return frame_scratch(nrows, ncols, make_frame(nrows, start, end, flags));
+}
+
+extern "C" int fb_window_frame(int dev, void* stream, int64_t nrows, int64_t nseg, const int64_t* d_offsets,
+                               int64_t start, int64_t end, int flags, int ncols, const int32_t* ops,
+                               const void* const* vals, const uint8_t* const* valid, void* const* out_vals,
+                               int64_t* const* out_count, void* scratch, size_t scratch_bytes) {
+  FB_CHECK(nrows >= 0 && nseg >= 0, "negative row or segment count");
+  FB_CHECK((flags & ~(FB_FRAME_UNBOUNDED_START | FB_FRAME_UNBOUNDED_END)) == 0, "unknown frame flags %d", flags);
+  FB_CHECK(flags != 0 || start <= end, "frame start %lld > end %lld", (long long)start, (long long)end);
+  ScanCols a;
+  if (scan_cols(nrows, ncols, ops, vals, valid, out_vals, out_count, &a) != 0) return 1;
+  if (nrows == 0) return 0;
+  FB_CHECK(nseg >= 1 && d_offsets != nullptr, "%lld rows need at least one segment", (long long)nrows);
+  FB_CHECK(num_tiles(nrows) < (1LL << 31), "too many rows");
+  const Frame f = make_frame(nrows, start, end, flags);
+  const size_t need = frame_scratch(nrows, ncols, f);
+  FB_CHECK(need == 0 || (scratch != nullptr && scratch_bytes >= need), "scratch too small: %zu < %zu", scratch_bytes,
+           need);
+  FbDeviceGuard guard(dev);
+  FB_CHECK(guard.ok, "cannot select device %d", dev);
   cudaStream_t st = (cudaStream_t)stream;
-  fb_segscan_tile_kernel<false><<<(unsigned)ntiles, kThreads, 0, st>>>(nrows, nseg, d_offsets, a, ntiles, tile_v,
-                                                                         tile_c, tile_f);
-  FB_CUDA(cudaGetLastError());
-  fb_segscan_carry_kernel<<<ncols, kCarryThreads, 0, st>>>(ntiles, a, tile_v, tile_c, tile_f);
-  FB_CUDA(cudaGetLastError());
-  fb_segscan_tile_kernel<true><<<(unsigned)ntiles, kThreads, 0, st>>>(nrows, nseg, d_offsets, a, ntiles, tile_v,
-                                                                        tile_c, tile_f);
+  if (f.tile) {
+    static std::mutex mu;
+    static uint64_t optin_done = 0;
+    {
+      std::lock_guard<std::mutex> lock(mu);
+      if (!(dev >= 0 && dev < 64 && ((optin_done >> dev) & 1))) {
+        FB_CUDA(cudaFuncSetAttribute(fb_window_frame_tile_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     (int)sizeof(FrameSmem)));
+        if (dev >= 0 && dev < 64) optin_done |= 1ull << dev;
+      }
+    }
+    const int64_t per_tile = kFrameSpan - (f.width - 1);
+    const int64_t grid = (nrows + per_tile - 1) / per_tile;
+    FB_CHECK(grid < (1LL << 31), "too many rows");
+    fb_window_frame_tile_kernel<<<(unsigned)grid, kFrameThreads, sizeof(FrameSmem), st>>>(
+        nrows, nseg, d_offsets, a, f.start, (int)f.width, per_tile);
+    FB_CUDA(cudaGetLastError());
+    return 0;
+  }
+  // P and / or S into scratch, then the combine pass
+  const bool need_p = f.flags != FB_FRAME_UNBOUNDED_END;                 // bounded, (None, e), (None, None)
+  const bool need_s = f.flags == 0 || f.flags == FB_FRAME_UNBOUNDED_END;  // bounded, (s, None)
+  char* tiles = (char*)scratch;
+  char* sides = tiles + align256(fb_segmented_scan_scratch_bytes(nrows, ncols));
+  const size_t side = (size_t)ncols * (size_t)nrows;
+  uint64_t* pv = need_p ? (uint64_t*)sides : nullptr;
+  int64_t* pc = need_p ? (int64_t*)(pv + side) : nullptr;
+  uint64_t* sv = need_s ? (uint64_t*)(need_p ? (char*)sides + 16 * side : sides) : nullptr;
+  int64_t* sc = need_s ? (int64_t*)(sv + side) : nullptr;
+  ScanCols b = a;
+  if (need_p) {
+    for (int c = 0; c < ncols; ++c) {
+      b.out_vals[c] = pv + c * nrows;
+      b.out_count[c] = pc + c * nrows;
+    }
+    if (run_scan(st, false, f.width, nrows, nseg, d_offsets, b, tiles) != 0) return 2;
+  }
+  if (need_s) {
+    for (int c = 0; c < ncols; ++c) {
+      b.out_vals[c] = sv + c * nrows;
+      b.out_count[c] = sc + c * nrows;
+    }
+    if (run_scan(st, true, f.width, nrows, nseg, d_offsets, b, tiles) != 0) return 2;
+  }
+  fb_window_frame_combine_kernel<<<(unsigned)num_tiles(nrows), kThreads, 0, st>>>(
+      nrows, nseg, d_offsets, a, f.start, f.end, f.flags, f.width, pv, pc, sv, sc);
   FB_CUDA(cudaGetLastError());
   return 0;
 }

@@ -429,6 +429,54 @@ def segmented_scan(offsets: torch.Tensor, nrows: int,
     return res
 
 
+FRAME_TILE_MAX_WIDTH = 1024   # FB_FRAME_TILE_MAX_WIDTH: widest frame of the one-pass kernel
+FRAME_UNBOUNDED_START = 1
+FRAME_UNBOUNDED_END = 2
+
+
+def window_frame(offsets: torch.Tensor, nrows: int, start: Optional[int], end: Optional[int],
+                 columns: Sequence[Tuple[int, Optional[torch.Tensor], Optional[torch.Tensor]]]
+                 ) -> List[Tuple[Optional[torch.Tensor], torch.Tensor]]:
+    """K9: ``ROWS BETWEEN start AND end`` over every segment ``[offsets[s], offsets[s + 1])``: per row, the
+    op over the valid rows of ``[max(first, i + start), min(last, i + end)]`` (``None``: unbounded) and
+    their count, 0 where the count is 0.  ``columns`` and the result are shaped as in
+    :func:`segmented_scan`; up to ``SCAN_MAX_COLS`` columns share one launch sequence."""
+    lib = _lib.load()
+    assert offsets.dtype == torch.int64 and offsets.is_cuda and offsets.is_contiguous()
+    dev = offsets.device
+    nseg = int(offsets.shape[0]) - 1
+    # a bound past every segment is unbounded: exact, as no segment is longer than the table
+    if start is not None and start <= -nrows:
+        start = None
+    if end is not None and end >= nrows:
+        end = None
+    flags = (FRAME_UNBOUNDED_START if start is None else 0) | (FRAME_UNBOUNDED_END if end is None else 0)
+    s, e = (0 if start is None else start), (0 if end is None else end)
+    res: List[Tuple[Optional[torch.Tensor], torch.Tensor]] = []
+    for b in range(0, len(columns), SCAN_MAX_COLS):
+        batch = columns[b:b + SCAN_MAX_COLS]
+        outs, cnts = [], []
+        for op, v, m in batch:
+            assert (v is None) == (op == AGG_COUNT)
+            if v is not None:
+                assert v.element_size() == 8 and v.device == dev and v.is_contiguous() and v.shape[0] == nrows
+            if m is not None:
+                assert m.dtype == torch.uint8 and m.device == dev and m.is_contiguous() and m.shape[0] == nrows
+            outs.append(None if v is None else torch.empty_like(v))
+            cnts.append(torch.empty(nrows, dtype=torch.int64, device=dev))
+        nb = int(lib.fb_window_frame_scratch_bytes(nrows, len(batch), s, e, flags))
+        scratch = torch.empty(max(nb, 8), dtype=torch.uint8, device=dev)
+        _lib.check(lib.fb_window_frame(
+            dev.index, _stream_ptr(dev), nrows, nseg, offsets.data_ptr(), s, e, flags, len(batch),
+            _lib.i32_array([op for op, _, _ in batch]),
+            _lib.ptr_array([0 if v is None else v.data_ptr() for _, v, _ in batch]),
+            _lib.ptr_array([0 if m is None else m.data_ptr() for _, _, m in batch]),
+            _lib.ptr_array([0 if o is None else o.data_ptr() for o in outs]),
+            _lib.ptr_array([c.data_ptr() for c in cnts]), scratch.data_ptr(), scratch.numel()))
+        res.extend(zip(outs, cnts))
+    return res
+
+
 def exclusive_scan(counts: torch.Tensor) -> Tuple[torch.Tensor, int]:
     """Exclusive prefix sum of an int64 device vector (own kernels); returns (offsets, total)."""
     lib = _lib.load()

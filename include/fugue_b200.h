@@ -261,6 +261,26 @@ int fb_segmented_scan(int dev, void* stream, int64_t nrows, int64_t nseg, const 
                       const int32_t* ops, const void* const* vals, const uint8_t* const* valid,
                       void* const* out_vals, int64_t* const* out_count, void* scratch, size_t scratch_bytes);
 
+/* K9  moving-window aggregate: ROWS BETWEEN start AND end over the same segments.  For row i of segment
+ * [a, b) the frame is rows [max(a, i + start), min(b - 1, i + end)] (may be empty); a negative bound is
+ * PRECEDING, 0 CURRENT ROW, a positive one FOLLOWING.  FB_FRAME_UNBOUNDED_START / _END in `flags` make a
+ * side unbounded (clip to a / b - 1) and its bound is ignored; any int64 bound is accepted and clipped,
+ * start > end with both sides bounded is an error.  Writes, per column and row, the count of valid rows in
+ * the frame and ops[c] over them, 0 where the count is 0: the contract of fb_segmented_scan, with every
+ * combination in a fixed order (bit-identical runs) and f64 sums made of the frame's own values only.
+ * Both bounds given and width end - start + 1 <= FB_FRAME_TILE_MAX_WIDTH: one pass, each CTA stages its
+ * rows plus the width - 1 halo in shared memory.  Otherwise: block prefix / suffix scans in scratch and
+ * a combine pass.  Scratch: fb_window_frame_scratch_bytes (0 on the one-pass path).
+ * --------------------------------------------------------------------------- */
+#define FB_FRAME_UNBOUNDED_START 1
+#define FB_FRAME_UNBOUNDED_END 2
+#define FB_FRAME_TILE_MAX_WIDTH 1024
+size_t fb_window_frame_scratch_bytes(int64_t nrows, int ncols, int64_t start, int64_t end, int flags);
+int fb_window_frame(int dev, void* stream, int64_t nrows, int64_t nseg, const int64_t* d_offsets, int64_t start,
+                    int64_t end, int flags, int ncols, const int32_t* ops, const void* const* vals,
+                    const uint8_t* const* valid, void* const* out_vals, int64_t* const* out_count, void* scratch,
+                    size_t scratch_bytes);
+
 /* ---------------------------------------------------------------------------
  * K7  hash equi-join on one 8-byte key (other key shapes are packed by the host layer)
  * Replaces: NativeExecutionEngine.join -> triad PandasUtils.join -> pd.merge

@@ -104,6 +104,12 @@ SIGNATURES = {
     "fb_window_frame_scratch_bytes": (C.c_size_t, [C.c_int64, C.c_int, C.c_int64, C.c_int64, C.c_int]),
     "fb_window_frame": (C.c_int, [C.c_int, _vp, C.c_int64, C.c_int64, _vp, C.c_int64, C.c_int64, C.c_int, C.c_int,
                                   _i32p, _vpp, _vpp, _vpp, _vpp, _vp, C.c_size_t]),
+    "fb_window_range_bounds_scratch_bytes": (C.c_size_t, [C.c_int64]),
+    "fb_window_range_bounds": (C.c_int, [C.c_int, _vp, C.c_int64, C.c_int64, _vp, _vp, _vp, C.c_int, C.c_int,
+                                         C.c_uint64, C.c_uint64, C.c_int, _vp, _vp, _vp, C.c_size_t]),
+    "fb_window_bounded_scratch_bytes": (C.c_size_t, [C.c_int64, C.c_int]),
+    "fb_window_bounded": (C.c_int, [C.c_int, _vp, C.c_int64, _vp, _vp, C.c_int, _i32p, _vpp, _vpp, _vpp, _vpp, _vp,
+                                    C.c_size_t]),
 }
 
 

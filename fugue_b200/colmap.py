@@ -20,6 +20,7 @@ window semantics.  The map engine sorts by (keys, presort) first for such a map.
     fa.transform(df, ColumnMap("key", "v0", (col("v0") * 2 + col("v1")).alias("w")),
                  schema="key:long,v0:double,w:double", partition=PartitionSpec(by="key", algo="hash", num=256))
 """
+import datetime
 import struct
 from typing import Any, Dict, List, Optional, Tuple
 
@@ -174,8 +175,9 @@ def _collect_windows(e: Any, out: Dict[str, ColumnExpr]) -> None:
 def _with_windows(t: B200Table, cols: List[ColumnExpr]) -> B200Table:
     """Evaluate every window node of ``cols`` over the logical partitions of ``t``: arguments pre-projected
     by the evaluator (K8), running / partition aggregates and ranks by the segmented scan (K9), moving
-    frames (``rows``) by the frame kernel with the same finishers, FIRST / LAST / partition values / LAG /
-    LEAD by row gathers."""
+    frames (``rows``) by the frame kernel, value frames (``range``) by the bounds kernel (or the peer groups)
+    and the block tree, all with the same finishers, FIRST / LAST / partition values / LAG / LEAD by row
+    gathers."""
     from . import expr as X
     from . import sort as S
     from .schema import Schema
@@ -251,6 +253,8 @@ def _with_windows(t: B200Table, cols: List[ColumnExpr]) -> B200Table:
             finish.append((uid, lambda r, i=i: (r[i][0], None, pa.int64(), None)))
             continue
         frame = bare.kwargs.get("rows")  # ROWS BETWEEN frame[0] AND frame[1]: the moving-frame kernel
+        if "range" in bare.kwargs:  # RANGE BETWEEN: ("range", key class or None, start, end), the block tree
+            frame = ("range",) + _range_offsets(t, bare.kwargs["range"])
         whole = None if frame is not None or bare.kwargs["running"] else seg_last
 
         def at_end(x: torch.Tensor, whole: Any = whole) -> torch.Tensor:  # partition value: the scan at its last row
@@ -309,10 +313,34 @@ def _with_windows(t: B200Table, cols: List[ColumnExpr]) -> B200Table:
             finish.append((uid, extreme))
             continue
         raise NotImplementedError(f"window function {fn}")  # pragma: no cover - builders admit no other
+    def range_bounds(cls: Optional[int], start: Any, end: Any) -> Tuple[torch.Tensor, torch.Tensor]:
+        """First and last row of every row's RANGE frame."""
+        if cls is not None:  # an offset: a search over the one presort key
+            name = t.logical_order[0]
+            i = t.schema.index_of_key(name)
+            tp = t.schema.types[i]
+            key = widen(t.columns[i], tp).contiguous()
+            kv = S.float_key_valid(key, t.valid[i]) if cls == K.RANGE_KEY_F64 else t.valid[i]
+            asc = (getattr(t, "logical_ascending", None) or [True])[0]
+            return K.window_range_bounds(off.contiguous(), key, kv, cls, asc, start, end)
+        # CURRENT ROW / UNBOUNDED only: the current row's peer group, or the partition's end
+        heads = peer_heads()
+        peer_first = torch.cummax(torch.where(heads, rows, torch.zeros_like(rows)), 0).values
+        ends = torch.ones_like(heads)
+        ends[:-1] = heads[1:]  # the next row starts a peer group (or a partition)
+        peer_last = torch.flip(torch.cummin(torch.flip(torch.where(ends, rows, torch.full_like(rows, n)), [0]), 0)
+                               .values, [0])
+        return (seg_first() if start is None else peer_first), (seg_last() if end is None else peer_last)
+
     results: Dict[Tuple[Any, int], Any] = {}
     for frame, spec in scans.items():
-        res = K.segmented_scan(off.contiguous(), n, spec) if frame is None else \
-            K.window_frame(off.contiguous(), n, frame[0], frame[1], spec)
+        if frame is None:
+            res = K.segmented_scan(off.contiguous(), n, spec)
+        elif frame[0] == "range":
+            lo, hi = range_bounds(*frame[1:])
+            res = K.window_bounded(lo.contiguous(), hi.contiguous(), spec)
+        else:
+            res = K.window_frame(off.contiguous(), n, frame[0], frame[1], spec)
         results.update(((frame, j), r) for j, r in enumerate(res))
     names, types, columns, valid = list(base.schema.names), list(base.schema.types), list(base.columns), list(base.valid)
     dicts = dict(base.dictionaries)
@@ -332,7 +360,61 @@ def _with_windows(t: B200Table, cols: List[ColumnExpr]) -> B200Table:
     return out
 
 
-def _offset_value(base: B200Table, bare: ColumnExpr, arg_name: Dict[str, str], rows: torch.Tensor,
+_TIME_UNIT_US = {"s": 1_000_000, "ms": 1_000, "us": 1}  # microseconds per unit ("ns": 1 / 1000)
+
+
+def _range_offsets(t: B200Table, frame: Tuple[Any, Any]) -> Tuple[Optional[int], Any, Any]:
+    """A ``range=(start, end)`` frame against the presort of ``t``: ``(key class, start, end)`` with the
+    offsets in the presort column's storage units (int) or as floats, or ``(None, start, end)`` when every
+    bound is CURRENT ROW (0) or UNBOUNDED (None), which needs no offset arithmetic and works with any presort.
+    Raises ValueError for a frame the presort cannot serve."""
+    if all(b is None or b == 0 for b in frame):
+        return (None,) + tuple(frame)
+    order = list(getattr(t, "logical_order", None) or [])
+    if len(order) != 1:
+        raise ValueError(f"a RANGE frame with an offset needs exactly one presort column, got {order}: {frame}")
+    name = order[0]
+    tp = t.schema[name].type
+    temporal = pa.types.is_date(tp) or pa.types.is_timestamp(tp) or pa.types.is_duration(tp) or \
+        pa.types.is_time64(tp)
+    if name in t.dictionaries or not (pa.types.is_integer(tp) or pa.types.is_floating(tp) or temporal):
+        raise ValueError(f"a RANGE frame with an offset needs a numeric or temporal presort column; {name} is {tp}")
+    if pa.types.is_floating(tp):
+        cls = K.RANGE_KEY_F64
+    else:
+        cls = K.RANGE_KEY_U64 if pa.types.is_unsigned_integer(tp) else K.RANGE_KEY_I64
+    unit = "D" if pa.types.is_date32(tp) else ("ms" if pa.types.is_date64(tp) else getattr(tp, "unit", None))
+
+    def offset(b: Any) -> Any:
+        if b is None:
+            return None
+        if isinstance(b, datetime.timedelta):
+            if not temporal:
+                raise ValueError(f"a timedelta RANGE offset needs a temporal presort column; {name} is {tp}")
+            us = b // datetime.timedelta(microseconds=1)
+            if unit == "ns":
+                return us * 1000
+            per = 86_400_000_000 if unit == "D" else _TIME_UNIT_US[unit]
+            if us % per:
+                raise ValueError(f"RANGE offset {b} is not a whole number of {unit} units of {name} ({tp})")
+            return us // per
+        if cls == K.RANGE_KEY_F64:
+            try:
+                return float(b)
+            except OverflowError as e:
+                raise ValueError(f"RANGE offset {b} does not fit a float64 key ({name} is {tp})") from e
+        if isinstance(b, float):
+            raise ValueError(f"a float RANGE offset {b} on the {tp} presort column {name}: give an int")
+        return b
+
+    start, end = offset(frame[0]), offset(frame[1])
+    for b in (start, end):
+        if b is not None and cls != K.RANGE_KEY_F64 and not -(1 << 63) <= b < (1 << 63):
+            raise ValueError(f"RANGE offset {b} on {name} ({tp}) is outside the int64 range")
+    return cls, start, end
+
+
+def _offset_value(base: B200Table,bare: ColumnExpr, arg_name: Dict[str, str], rows: torch.Tensor,
                   seg_first: Any, seg_last: Any) -> Any:
     """LAG / LEAD: a gather of the row ``n`` before / after, NULL (then ``default``) across a partition bound."""
     name = arg_name[bare.arg.fingerprint()]

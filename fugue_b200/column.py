@@ -7,7 +7,7 @@ from an expression is a function of ``(kind, head, args)``:
     LITERAL   head = python value (None = NULL)      UNARY     head in ``- ~ IS_NULL NOT_NULL``, one arg
     BINARY    head in ``+ - * / & | < > <= >= == !=``  CALL      head = function name (``COALESCE`` ...)
     AGG       head in ``SUM COUNT AVG MIN MAX FIRST LAST``, one arg, optional DISTINCT
-    WINDOW    head in the AGG functions (one arg, kwargs ``running`` or ``rows``), ``ROW_NUMBER RANK
+    WINDOW    head in the AGG functions (one arg, kwargs ``running``, ``rows`` or ``range``), ``ROW_NUMBER RANK
               DENSE_RANK`` (no arg) or ``LAG LEAD`` (one arg, kwargs ``n`` and ``default``): evaluated over the logical
               partitions of ``fa.transform`` (PartitionSpec keys, presort order) by a ``ColumnMap``
 
@@ -22,8 +22,10 @@ against ``fugue.column`` reads the same here: ``col, lit, null, all_cols, functi
 ``fugue_b200.fugue_plugin.translate_expr``; tests/test_column_golden.py pins this module to vectors
 produced by the reference's code.
 """
+import datetime
 import enum
 import hashlib
+import math
 from typing import Any, Dict, Iterable, Iterator, List, Optional, Sequence, Tuple
 
 import pyarrow as pa
@@ -254,13 +256,17 @@ class ColumnExpr:
     def __invert__(self) -> "ColumnExpr":
         return ColumnExpr(Kind.UNARY, "~", [self])
 
-    def over(self, running: bool = False, rows: Optional[Tuple[Optional[int], Optional[int]]] = None) -> "ColumnExpr":
+    def over(self, running: bool = False, rows: Optional[Tuple[Optional[int], Optional[int]]] = None,
+             range: Optional[Tuple[Any, Any]] = None) -> "ColumnExpr":  # noqa: A002 - the SQL word
         """The aggregation as a window function of a ``ColumnMap``: over the whole logical partition
         (``running=False``, the value repeated on every row), over the rows up to and including the
-        current one in presort order (``running=True``), or over a moving frame ``rows=(start, end)``:
+        current one in presort order (``running=True``), over a moving frame ``rows=(start, end)``:
         ``ROWS BETWEEN`` offsets from the current row in presort order, negative PRECEDING, 0 CURRENT ROW,
-        positive FOLLOWING, ``None`` UNBOUNDED.  ``rows=(None, 0)`` is ``running=True`` and
-        ``rows=(None, None)`` the whole partition: both give those nodes."""
+        positive FOLLOWING, ``None`` UNBOUNDED, or over a value frame ``range=(start, end)``: ``RANGE
+        BETWEEN`` offsets in the units of the presort column (``int``, finite ``float`` or
+        ``datetime.timedelta``; 0 is CURRENT ROW, the current row's peers).  ``rows=(None, 0)`` is
+        ``running=True``, and ``rows=(None, None)`` and ``range=(None, None)`` are the whole partition: they
+        give those nodes.  ``range=(None, 0)`` is not ``running=True``: it includes the current row's peers."""
         if self.kind != Kind.AGG:
             raise ValueError(f"{self} is not an aggregation: only an aggregation has an OVER form")
         if self.is_distinct:
@@ -269,6 +275,12 @@ class ColumnExpr:
             raise ValueError(f"{self}: {self.head} has no window form")
         if not isinstance(running, bool):
             raise ValueError(f"running must be a bool, got {running!r}")
+        if range is not None:
+            if running or rows is not None:
+                raise ValueError("over() takes one of running=True, rows and range")
+            range = _range_frame(range)
+            if range == (None, None):
+                range = None
         if rows is not None:
             if running:
                 raise ValueError("over() takes running=True or rows, not both")
@@ -287,7 +299,10 @@ class ColumnExpr:
             raise ValueError(f"nested aggregation {self}")
         if self.head in ("FIRST", "LAST") and self.args[0].kind == Kind.WILDCARD:
             raise ValueError(f"{self}: {self.head} needs a column")
-        kwargs = {"running": running} if rows is None else {"rows": (rows[0], rows[1])}
+        if range is not None:
+            kwargs: Dict[str, Any] = {"range": range}
+        else:
+            kwargs = {"running": running} if rows is None else {"rows": (rows[0], rows[1])}
         return ColumnExpr(Kind.WINDOW, self.head, self.args, kwargs, False, self.as_name, self.as_type)
 
     def __bool__(self) -> bool:
@@ -384,18 +399,57 @@ def _window_text(e: ColumnExpr, show: Any) -> str:
     if e.head in ("LAG", "LEAD"):
         parts += [str(e.kwargs["n"]), _show_literal(e.kwargs["default"])]
     frame = _RUNNING_FRAME if e.kwargs.get("running", False) else ""
-    if "rows" in e.kwargs:
-        frame = f"ROWS BETWEEN {_frame_bound(e.kwargs['rows'][0], 'PRECEDING')} AND " \
-                f"{_frame_bound(e.kwargs['rows'][1], 'FOLLOWING')}"
+    for unit in ("rows", "range"):
+        if unit in e.kwargs:
+            frame = f"{unit.upper()} BETWEEN {_frame_bound(e.kwargs[unit][0], 'PRECEDING')} AND " \
+                    f"{_frame_bound(e.kwargs[unit][1], 'FOLLOWING')}"
     return f"{e.head}({','.join(parts)}) OVER ({frame})"
 
 
-def _frame_bound(b: Optional[int], unbounded: str) -> str:
+def _frame_bound(b: Any, unbounded: str) -> str:
     if b is None:
         return "UNBOUNDED " + unbounded
     if b == 0:
         return "CURRENT ROW"
-    return f"{-b} PRECEDING" if b < 0 else f"{b} FOLLOWING"
+    neg = b < (datetime.timedelta(0) if isinstance(b, datetime.timedelta) else 0)
+    mag = -b if neg else b
+    text = _interval_text(mag) if isinstance(mag, datetime.timedelta) else str(mag)
+    return f"{text} PRECEDING" if neg else f"{text} FOLLOWING"
+
+
+def _interval_text(d: datetime.timedelta) -> str:
+    """A positive timedelta as an SQL day-time INTERVAL literal: ``INTERVAL '7' DAY`` for whole days, else
+    ``INTERVAL '1 02:03:04[.000005]' DAY TO SECOND``."""
+    if d.seconds == 0 and d.microseconds == 0:
+        return f"INTERVAL '{d.days}' DAY"
+    hms = f"{d.seconds // 3600:02d}:{d.seconds // 60 % 60:02d}:{d.seconds % 60:02d}"
+    frac = f".{d.microseconds:06d}" if d.microseconds else ""
+    return f"INTERVAL '{d.days} {hms}{frac}' DAY TO SECOND"
+
+
+def _range_frame(frame: Any) -> Tuple[Any, Any]:
+    """Check a ``range=(start, end)`` frame and read a zero bound (``0.0``, ``timedelta(0)``) as the int 0."""
+    if not isinstance(frame, tuple) or len(frame) != 2:
+        raise ValueError(f"range must be a (start, end) tuple, got {frame!r}")
+    out = []
+    for b in frame:
+        if b is None:
+            out.append(None)
+            continue
+        if isinstance(b, bool) or not isinstance(b, (int, float, datetime.timedelta)):
+            raise ValueError(f"a RANGE bound must be an int, a float, a timedelta or None, got {b!r}")
+        if isinstance(b, float) and not math.isfinite(b):
+            raise ValueError(f"a RANGE bound must be finite, got {b!r}")
+        out.append(0 if b == (datetime.timedelta(0) if isinstance(b, datetime.timedelta) else 0) else b)
+    start, end = out
+    if start is not None and end is not None:
+        if isinstance(start, datetime.timedelta) != isinstance(end, datetime.timedelta) and start != 0 and end != 0:
+            raise ValueError(f"RANGE bounds mix a timedelta and a number: {frame!r}")
+        us = datetime.timedelta(microseconds=1)  # a timedelta as exact integer microseconds
+        if (start // us if isinstance(start, datetime.timedelta) else start) > \
+                (end // us if isinstance(end, datetime.timedelta) else end):
+            raise ValueError(f"frame start {start} is after its end {end}")
+    return start, end
 
 
 def _offset_fn(name: str, c: Any, n: Any, default: Any) -> ColumnExpr:

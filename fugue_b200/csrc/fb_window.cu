@@ -26,6 +26,16 @@
 //   - otherwise, and with an unbounded side: P and S by the three-launch scan above (block heads added,
 //     S walking rows in reverse) into scratch, then a combine launch.  (None, e) is P without blocks read
 //     at hi; (s, None) is S without blocks read at lo.
+//
+// Value frames (RANGE BETWEEN) have a different width on every row, so they take two other kernels:
+//   - fb_window_range_bounds: per row, [lo, hi] by a galloping lower_bound / upper_bound from the row over
+//     its segment's non-NULL run (the NULL keys are the segment's tail), in the order-key domain of the sort.
+//   - fb_window_bounded: the op over any [lo, hi] from an aligned power-of-two block tree.  Level l holds op
+//     and count of rows [m 2^l, (m + 1) 2^l), built pairwise level by level; an interval is at most two
+//     blocks per level (the canonical decomposition of a bottom-up segment tree), combined left to right.
+//     Blocks ignore segments: a frame never crosses its segment and its blocks lie inside it.  The counts
+//     live in the tree beside the values because the combination needs them anyway (a block without a
+//     valid row takes no part, so MIN / MAX need no identity).
 #include <mutex>
 
 #include "fb_common.cuh"
@@ -539,6 +549,216 @@ int run_scan(cudaStream_t st, bool reverse, int64_t block, int64_t nrows, int64_
   return 0;
 }
 
+// ---- value frames (RANGE BETWEEN) ----------------------------------------------------------------
+constexpr int kRangeThreads = 256;  // one row per thread: neighbouring rows search neighbouring keys
+
+// The presort key as an unsigned order key, as sort._unsigned_order_key builds it: sign bit flipped for
+// signed integers, the value itself for unsigned ones, the total-order transform for f64 (-0.0 read as 0.0).
+__device__ __forceinline__ uint64_t range_order_bits(uint64_t k, int cls) {
+  if (cls == FB_RANGE_KEY_I64) return k ^ 0x8000000000000000ULL;
+  if (cls == FB_RANGE_KEY_U64) return k;
+  if (__longlong_as_double((long long)k) == 0.0) k = 0;
+  return (int64_t)k < 0 ? ~k : k ^ 0x8000000000000000ULL;
+}
+
+// A bound key k + off (ASC) or k - off (DESC) in the searched order (ASC: the order key, DESC: its
+// complement, so that the non-NULL run of a segment is ascending either way).  inf = -1 / +1: below /
+// above every key of the type (an integer sum past the type's range); then v is unused.
+struct RangeTarget {
+  uint64_t v;
+  int inf;
+};
+
+__device__ __forceinline__ RangeTarget range_target(uint64_t k, uint64_t off, int cls, bool desc) {
+  RangeTarget t{0, 0};
+  if (cls == FB_RANGE_KEY_F64) {  // one IEEE addition, round to nearest even; overflow gives +-inf, a key
+    const double o = __longlong_as_double((long long)off);
+    const double x = __longlong_as_double((long long)k) + (desc ? -o : o);
+    t.v = range_order_bits((uint64_t)__double_as_longlong(x), cls);
+  } else {  // exact: 128-bit sum, compared with the type's range
+    const __int128 kk = cls == FB_RANGE_KEY_I64 ? (__int128)(int64_t)k : (__int128)k;
+    const __int128 oo = (__int128)(int64_t)off;
+    const __int128 x = desc ? kk - oo : kk + oo;
+    const __int128 lo = cls == FB_RANGE_KEY_I64 ? -((__int128)1 << 63) : (__int128)0;
+    const __int128 hi = cls == FB_RANGE_KEY_I64 ? ((__int128)1 << 63) - 1 : ((__int128)1 << 64) - 1;
+    if (x < lo) t.inf = -1;
+    else if (x > hi) t.inf = 1;
+    else t.v = range_order_bits((uint64_t)x, cls);
+  }
+  if (desc) {
+    t.v = ~t.v;
+    t.inf = -t.inf;
+  }
+  return t;
+}
+
+// First row j of [a, e) with key(j) >= t (kStrict: key(j) > t) in the searched order, e if none.  The
+// non-NULL run [a, e) is sorted, so this is a lower_bound (upper_bound when kStrict) over it, found by
+// galloping from row i in [a, e): O(log |answer - i|) loads, not O(log (e - a)).
+template <bool kStrict>
+__device__ __forceinline__ int64_t range_search(const uint64_t* __restrict__ keys, int cls, bool desc, int64_t a,
+                                                int64_t e, int64_t i, const RangeTarget& t) {
+  if (t.inf < 0) return a;
+  if (t.inf > 0) return e;
+  auto hit = [&](int64_t j) {
+    uint64_t o = range_order_bits(__ldg((const unsigned long long*)keys + j), cls);
+    if (desc) o = ~o;
+    return kStrict ? o > t.v : o >= t.v;
+  };
+  int64_t lo, hi;  // hit() is false on [a, lo) and true on [hi, e): the answer is in [lo, hi]
+  if (hit(i)) {
+    hi = i;
+    lo = a;
+    for (int64_t step = 1;; step <<= 1) {
+      const int64_t j = hi - step;
+      if (j < a) break;
+      if (!hit(j)) { lo = j + 1; break; }
+      hi = j;
+    }
+  } else {
+    lo = i + 1;
+    hi = e;
+    for (int64_t step = 1;; step <<= 1) {
+      const int64_t j = lo - 1 + step;
+      if (j >= e) break;
+      if (hit(j)) { hi = j; break; }
+      lo = j + 1;
+    }
+  }
+  while (lo < hi) {
+    const int64_t m = lo + ((hi - lo) >> 1);
+    if (hit(m)) hi = m; else lo = m + 1;
+  }
+  return lo;
+}
+
+// first NULL-key row of every segment (its NULL rows are its tail): a binary search on the validity bytes
+__global__ void __launch_bounds__(kRangeThreads)
+fb_range_null_start_kernel(int64_t nseg, const int64_t* __restrict__ offsets, const uint8_t* __restrict__ valid,
+                           int64_t* __restrict__ null_start) {
+  const int64_t s = (int64_t)blockIdx.x * kRangeThreads + threadIdx.x;
+  if (s >= nseg) return;
+  int64_t lo = __ldg(offsets + s), hi = __ldg(offsets + s + 1);
+  if (valid == nullptr) lo = hi;  // no NULL keys
+  while (lo < hi) {
+    const int64_t m = lo + ((hi - lo) >> 1);
+    if (__ldg(valid + m) != 0) lo = m + 1; else hi = m;
+  }
+  null_start[s] = lo;
+}
+
+__global__ void __launch_bounds__(kRangeThreads)
+fb_range_bounds_kernel(int64_t nrows, int64_t nseg, const int64_t* __restrict__ offsets,
+                       const int64_t* __restrict__ null_start, const uint64_t* __restrict__ keys, int cls, int desc,
+                       uint64_t start, uint64_t end, int flags, int64_t* __restrict__ out_lo,
+                       int64_t* __restrict__ out_hi) {
+  __shared__ int64_t range[2];
+  const int64_t t0 = (int64_t)blockIdx.x * kRangeThreads;
+  const int64_t t1 = t0 + kRangeThreads < nrows ? t0 + kRangeThreads : nrows;
+  if (threadIdx.x == 0) {
+    range[0] = upper_bound(offsets, nseg + 1, t0) - 1;
+    range[1] = upper_bound(offsets, nseg + 1, t1 - 1) + 1;
+  }
+  __syncthreads();
+  const int64_t i = t0 + threadIdx.x;
+  if (i >= t1) return;
+  const int64_t q0 = range[0];
+  const int64_t q = q0 + upper_bound(offsets + q0, range[1] - q0, i) - 1;
+  const int64_t a = __ldg(offsets + q), b = __ldg(offsets + q + 1), e = __ldg(null_start + q);
+  int64_t lo, hi;
+  if (i >= e) {  // a NULL key: its peers are the NULL tail [e, b)
+    lo = (flags & FB_FRAME_UNBOUNDED_START) ? a : e;
+    hi = b - 1;
+  } else {
+    const uint64_t k = __ldg((const unsigned long long*)keys + i);
+    if (flags & FB_FRAME_UNBOUNDED_START) lo = a;
+    else lo = range_search<false>(keys, cls, desc != 0, a, e, i, range_target(k, start, cls, desc != 0));
+    if (flags & FB_FRAME_UNBOUNDED_END) hi = b - 1;
+    else hi = range_search<true>(keys, cls, desc != 0, a, e, i, range_target(k, end, cls, desc != 0)) - 1;
+  }
+  out_lo[i] = lo;
+  out_hi[i] = hi;
+}
+
+// ---- aggregates over arbitrary row intervals: an aligned power-of-two block tree ----------------------
+// Level l >= 1 holds (op, count) of rows [m 2^l, (m + 1) 2^l) for m < nrows >> l, in scratch; level 0 is the
+// input.  Level l starts at node tree_off[l] of a column's nodes.
+constexpr int kTreeMaxLevels = 64;
+
+struct TreeLevels {
+  int64_t off[kTreeMaxLevels];
+  int64_t total;  // nodes of levels >= 1 per column
+  int levels;     // highest level with a node
+};
+
+TreeLevels tree_levels(int64_t nrows) {
+  TreeLevels L;
+  memset(&L, 0, sizeof(L));
+  int64_t acc = 0;
+  for (int l = 1; l < kTreeMaxLevels && (nrows >> l) > 0; ++l) {
+    L.off[l] = acc;
+    acc += nrows >> l;
+    L.levels = l;
+  }
+  L.total = acc;
+  return L;
+}
+
+__device__ __forceinline__ St tree_node(const ScanCols& a, int col, bool is_count, const TreeLevels& L,
+                                        const uint64_t* __restrict__ tv, const int64_t* __restrict__ tc, int level,
+                                        int64_t m) {
+  if (level == 0) {
+    const uint8_t* vm = a.valid[col];
+    const int c = vm == nullptr ? 1 : (__ldg(vm + m) != 0);
+    return St{c && !is_count ? __ldg((const unsigned long long*)a.vals[col] + m) : 0, c, 0};
+  }
+  const int64_t p = (int64_t)col * L.total + L.off[level] + m;
+  return St{is_count ? 0 : __ldg((const unsigned long long*)tv + p), __ldg((const long long*)tc + p), 0};
+}
+
+// one level of the tree from the one below, pairwise in a fixed order; blockIdx.y = column
+__global__ void __launch_bounds__(kThreads)
+fb_tree_level_kernel(const __grid_constant__ ScanCols a, const __grid_constant__ TreeLevels L, int level,
+                     int64_t nrows, uint64_t* __restrict__ tv, int64_t* __restrict__ tc) {
+  const int col = blockIdx.y;
+  const int op = a.op[col];
+  const bool is_count = op == FB_AGG_COUNT;
+  const int64_t nodes = nrows >> level;
+  for (int64_t m = (int64_t)blockIdx.x * kThreads + threadIdx.x; m < nodes; m += (int64_t)gridDim.x * kThreads) {
+    const St r = combine(op, tree_node(a, col, is_count, L, tv, tc, level - 1, 2 * m),
+                         tree_node(a, col, is_count, L, tv, tc, level - 1, 2 * m + 1));
+    const int64_t p = (int64_t)col * L.total + L.off[level] + m;
+    if (!is_count) tv[p] = r.c > 0 ? r.v : 0;
+    tc[p] = r.c;
+  }
+}
+
+// Per row, [lo, hi] clamped to [0, nrows) as its canonical decomposition into tree blocks (at most two per
+// level, O(log width) levels), combined left to right.
+__global__ void __launch_bounds__(kThreads)
+fb_tree_query_kernel(const __grid_constant__ ScanCols a, const __grid_constant__ TreeLevels L, int64_t nrows,
+                     const int64_t* __restrict__ d_lo, const int64_t* __restrict__ d_hi,
+                     const uint64_t* __restrict__ tv, const int64_t* __restrict__ tc) {
+  const int64_t i = (int64_t)blockIdx.x * kThreads + threadIdx.x;
+  if (i >= nrows) return;
+  int64_t lo = __ldg((const long long*)d_lo + i), hi = __ldg((const long long*)d_hi + i);
+  lo = lo < 0 ? 0 : lo;
+  hi = hi > nrows - 1 ? nrows - 1 : hi;
+  for (int col = 0; col < a.ncols; ++col) {
+    const int op = a.op[col];
+    const bool is_count = op == FB_AGG_COUNT;
+    St left{0, 0, 0}, right{0, 0, 0};
+    int64_t l = lo, r = hi + 1;  // [l, r) in blocks of the current level
+    for (int level = 0; l < r; ++level, l >>= 1, r >>= 1) {
+      if (l & 1) left = combine(op, left, tree_node(a, col, is_count, L, tv, tc, level, l++));
+      if (r & 1) right = combine(op, tree_node(a, col, is_count, L, tv, tc, level, --r), right);
+    }
+    const St res = combine(op, left, right);
+    if (a.out_vals[col] != nullptr) ((uint64_t*)a.out_vals[col])[i] = res.c > 0 ? res.v : 0;
+    if (a.out_count[col] != nullptr) a.out_count[col][i] = res.c;
+  }
+}
+
 // the column arrays of the C ABI -> ScanCols (checked)
 int scan_cols(int64_t nrows, int ncols, const int32_t* ops, const void* const* vals, const uint8_t* const* valid,
               void* const* out_vals, int64_t* const* out_count, ScanCols* a) {
@@ -652,6 +872,76 @@ extern "C" int fb_window_frame(int dev, void* stream, int64_t nrows, int64_t nse
   }
   fb_window_frame_combine_kernel<<<(unsigned)num_tiles(nrows), kThreads, 0, st>>>(
       nrows, nseg, d_offsets, a, f.start, f.end, f.flags, f.width, pv, pc, sv, sc);
+  FB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+extern "C" size_t fb_window_range_bounds_scratch_bytes(int64_t nseg) {
+  return nseg > 0 ? (size_t)nseg * sizeof(int64_t) : 0;
+}
+
+extern "C" int fb_window_range_bounds(int dev, void* stream, int64_t nrows, int64_t nseg, const int64_t* d_offsets,
+                                      const void* d_keys, const uint8_t* d_key_valid, int key_class, int descending,
+                                      uint64_t start, uint64_t end, int flags, int64_t* d_lo, int64_t* d_hi,
+                                      void* scratch, size_t scratch_bytes) {
+  FB_CHECK(nrows >= 0 && nseg >= 0, "negative row or segment count");
+  FB_CHECK((flags & ~(FB_FRAME_UNBOUNDED_START | FB_FRAME_UNBOUNDED_END)) == 0, "unknown frame flags %d", flags);
+  FB_CHECK(key_class == FB_RANGE_KEY_I64 || key_class == FB_RANGE_KEY_U64 || key_class == FB_RANGE_KEY_F64,
+           "unknown key class %d", key_class);
+  if (nrows == 0) return 0;
+  FB_CHECK(nseg >= 1 && d_offsets != nullptr, "%lld rows need at least one segment", (long long)nrows);
+  FB_CHECK(d_keys != nullptr && d_lo != nullptr && d_hi != nullptr, "NULL keys or outputs");
+  FB_CHECK(scratch != nullptr && scratch_bytes >= fb_window_range_bounds_scratch_bytes(nseg),
+           "scratch too small: %zu < %zu", scratch_bytes, fb_window_range_bounds_scratch_bytes(nseg));
+  const int64_t grid = (nrows + kRangeThreads - 1) / kRangeThreads;
+  FB_CHECK(grid < (1LL << 31), "too many rows");
+  FbDeviceGuard guard(dev);
+  FB_CHECK(guard.ok, "cannot select device %d", dev);
+  cudaStream_t st = (cudaStream_t)stream;
+  int64_t* null_start = (int64_t*)scratch;
+  fb_range_null_start_kernel<<<(unsigned)((nseg + kRangeThreads - 1) / kRangeThreads), kRangeThreads, 0, st>>>(
+      nseg, d_offsets, d_key_valid, null_start);
+  FB_CUDA(cudaGetLastError());
+  fb_range_bounds_kernel<<<(unsigned)grid, kRangeThreads, 0, st>>>(nrows, nseg, d_offsets, null_start,
+                                                                    (const uint64_t*)d_keys, key_class, descending,
+                                                                    start, end, flags, d_lo, d_hi);
+  FB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+extern "C" size_t fb_window_bounded_scratch_bytes(int64_t nrows, int ncols) {
+  if (nrows <= 0 || ncols <= 0) return 0;
+  return (size_t)tree_levels(nrows).total * 16 * (size_t)ncols;
+}
+
+extern "C" int fb_window_bounded(int dev, void* stream, int64_t nrows, const int64_t* d_lo, const int64_t* d_hi,
+                                 int ncols, const int32_t* ops, const void* const* vals, const uint8_t* const* valid,
+                                 void* const* out_vals, int64_t* const* out_count, void* scratch,
+                                 size_t scratch_bytes) {
+  FB_CHECK(nrows >= 0, "negative row count");
+  ScanCols a;
+  if (scan_cols(nrows, ncols, ops, vals, valid, out_vals, out_count, &a) != 0) return 1;
+  if (nrows == 0) return 0;
+  FB_CHECK(d_lo != nullptr && d_hi != nullptr, "NULL bounds");
+  const int64_t grid = (nrows + kThreads - 1) / kThreads;
+  FB_CHECK(grid < (1LL << 31), "too many rows");
+  const size_t need = fb_window_bounded_scratch_bytes(nrows, ncols);
+  FB_CHECK(need == 0 || (scratch != nullptr && scratch_bytes >= need), "scratch too small: %zu < %zu", scratch_bytes,
+           need);
+  FbDeviceGuard guard(dev);
+  FB_CHECK(guard.ok, "cannot select device %d", dev);
+  cudaStream_t st = (cudaStream_t)stream;
+  const TreeLevels L = tree_levels(nrows);
+  uint64_t* tv = (uint64_t*)scratch;
+  int64_t* tc = (int64_t*)(tv + (size_t)ncols * L.total);
+  const int64_t max_grid = 8 * (int64_t)fb_sm_count(dev);
+  for (int level = 1; level <= L.levels; ++level) {
+    const int64_t blocks = ((nrows >> level) + kThreads - 1) / kThreads;
+    const dim3 grid((unsigned)(blocks < max_grid ? blocks : max_grid), (unsigned)ncols);
+    fb_tree_level_kernel<<<grid, kThreads, 0, st>>>(a, L, level, nrows, tv, tc);
+    FB_CUDA(cudaGetLastError());
+  }
+  fb_tree_query_kernel<<<(unsigned)grid, kThreads, 0, st>>>(a, L, nrows, d_lo, d_hi, tv, tc);
   FB_CUDA(cudaGetLastError());
   return 0;
 }

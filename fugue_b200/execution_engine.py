@@ -146,6 +146,7 @@ class B200MapEngine:
                 t.logical_offsets = edf.native.logical_offsets if keyed else \
                     torch.tensor([0, t.num_rows], dtype=torch.int64, device=t.device)
                 t.logical_order = list(presort.keys())
+                t.logical_ascending = list(presort.values())  # RANGE frames search the presort key's direction
                 edf = B200DataFrame(t)
             cursor.set(lambda: edf.peek_array(), 0, 0)
             out = map_func(cursor, edf)

@@ -3,6 +3,7 @@
 torch is used here only as the owner of device memory and streams; every
 operation is a call into ``libfugue_b200.so``.
 """
+import struct
 from typing import Any, List, Optional, Sequence, Tuple
 
 import torch
@@ -468,6 +469,83 @@ def window_frame(offsets: torch.Tensor, nrows: int, start: Optional[int], end: O
         scratch = torch.empty(max(nb, 8), dtype=torch.uint8, device=dev)
         _lib.check(lib.fb_window_frame(
             dev.index, _stream_ptr(dev), nrows, nseg, offsets.data_ptr(), s, e, flags, len(batch),
+            _lib.i32_array([op for op, _, _ in batch]),
+            _lib.ptr_array([0 if v is None else v.data_ptr() for _, v, _ in batch]),
+            _lib.ptr_array([0 if m is None else m.data_ptr() for _, _, m in batch]),
+            _lib.ptr_array([0 if o is None else o.data_ptr() for o in outs]),
+            _lib.ptr_array([c.data_ptr() for c in cnts]), scratch.data_ptr(), scratch.numel()))
+        res.extend(zip(outs, cnts))
+    return res
+
+
+RANGE_KEY_I64 = 0   # FB_RANGE_KEY_*: how fb_window_range_bounds reads the 8-byte presort key
+RANGE_KEY_U64 = 1
+RANGE_KEY_F64 = 2
+
+
+def window_range_bounds(offsets: torch.Tensor, keys: torch.Tensor, valid: Optional[torch.Tensor], key_class: int,
+                        ascending: bool, start: Optional[Any], end: Optional[Any]) -> Tuple[torch.Tensor, torch.Tensor]:
+    """K9: ``RANGE BETWEEN start AND end`` over every segment ``[offsets[s], offsets[s + 1])``, each sorted by
+    one key (``keys``: 8-byte values of ``key_class``; ``valid``: uint8 validity with a float key's NaN rows
+    cleared, NULLs last).  Offsets are ints (``RANGE_KEY_I64`` / ``_U64``, within int64) or floats
+    (``RANGE_KEY_F64``), ``None`` unbounded.  Returns per row the first and last row of its frame (int64;
+    last < first: empty)."""
+    lib = _lib.load()
+    assert offsets.dtype == torch.int64 and offsets.is_cuda and offsets.is_contiguous()
+    dev = offsets.device
+    nseg = int(offsets.shape[0]) - 1
+    n = int(keys.shape[0])
+    assert keys.element_size() == 8 and keys.device == dev and keys.is_contiguous()
+    if valid is not None:
+        assert valid.dtype == torch.uint8 and valid.device == dev and valid.is_contiguous() and valid.shape[0] == n
+
+    def bits(b: Any) -> int:
+        if b is None:
+            return 0
+        if key_class == RANGE_KEY_F64:
+            return struct.unpack("<Q", struct.pack("<d", float(b)))[0]
+        assert -(1 << 63) <= b < (1 << 63), f"offset {b} outside int64"
+        return int(b) & ((1 << 64) - 1)
+
+    flags = (FRAME_UNBOUNDED_START if start is None else 0) | (FRAME_UNBOUNDED_END if end is None else 0)
+    lo = torch.empty(n, dtype=torch.int64, device=dev)
+    hi = torch.empty(n, dtype=torch.int64, device=dev)
+    nb = int(lib.fb_window_range_bounds_scratch_bytes(nseg))
+    scratch = torch.empty(max(nb, 8), dtype=torch.uint8, device=dev)
+    _lib.check(lib.fb_window_range_bounds(
+        dev.index, _stream_ptr(dev), n, nseg, offsets.data_ptr(), keys.data_ptr(),
+        0 if valid is None else valid.data_ptr(), key_class, 0 if ascending else 1, bits(start), bits(end), flags,
+        lo.data_ptr(), hi.data_ptr(), scratch.data_ptr(), scratch.numel()))
+    return lo, hi
+
+
+def window_bounded(lo: torch.Tensor, hi: torch.Tensor,
+                   columns: Sequence[Tuple[int, Optional[torch.Tensor], Optional[torch.Tensor]]]
+                   ) -> List[Tuple[Optional[torch.Tensor], torch.Tensor]]:
+    """K9: per row i, the op over the valid rows of ``[lo[i], hi[i]]`` (clamped to the table; hi < lo: empty)
+    and their count, 0 where the count is 0.  ``columns`` and the result are shaped as in
+    :func:`segmented_scan`; up to ``SCAN_MAX_COLS`` columns share one tree build and query."""
+    lib = _lib.load()
+    dev = lo.device
+    nrows = int(lo.shape[0])
+    for b_ in (lo, hi):
+        assert b_.dtype == torch.int64 and b_.is_cuda and b_.is_contiguous() and b_.shape[0] == nrows
+    res: List[Tuple[Optional[torch.Tensor], torch.Tensor]] = []
+    for b in range(0, len(columns), SCAN_MAX_COLS):
+        batch = columns[b:b + SCAN_MAX_COLS]
+        outs, cnts = [], []
+        for op, v, m in batch:
+            assert (v is None) == (op == AGG_COUNT)
+            if v is not None:
+                assert v.element_size() == 8 and v.device == dev and v.is_contiguous() and v.shape[0] == nrows
+            if m is not None:
+                assert m.dtype == torch.uint8 and m.device == dev and m.is_contiguous() and m.shape[0] == nrows
+            outs.append(None if v is None else torch.empty_like(v))
+            cnts.append(torch.empty(nrows, dtype=torch.int64, device=dev))
+        nb = int(lib.fb_window_bounded_scratch_bytes(nrows, len(batch)))
+        scratch = torch.empty(max(nb, 8), dtype=torch.uint8, device=dev)
+        _lib.check(lib.fb_window_bounded(
+            dev.index, _stream_ptr(dev), nrows, lo.data_ptr(), hi.data_ptr(), len(batch),
             _lib.i32_array([op for op, _, _ in batch]),
             _lib.ptr_array([0 if v is None else v.data_ptr() for _, v, _ in batch]),
             _lib.ptr_array([0 if m is None else m.data_ptr() for _, _, m in batch]),

@@ -101,6 +101,7 @@ class B200Table:
         #                                                      per distinct key tuple (logical partition)
         self.logical_order: Optional[List[str]] = None  # presort columns the rows of a logical partition are
         #                                                 sorted by (peers of RANK / DENSE_RANK are equal on all)
+        self.logical_ascending: Optional[List[bool]] = None  # their directions (NULLs last either way)
         # multi-GPU shuffle result (fugue_b200/dist.py): int64 [world, nown + 1] on the HOST; owned
         # partition j is the concatenation over source ranks s of rows
         # [segment_offsets[s, j], segment_offsets[s, j + 1]) - see compacted()

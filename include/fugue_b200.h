@@ -281,6 +281,37 @@ int fb_window_frame(int dev, void* stream, int64_t nrows, int64_t nseg, const in
                     const uint8_t* const* valid, void* const* out_vals, int64_t* const* out_count, void* scratch,
                     size_t scratch_bytes);
 
+/* K9  value frames: RANGE BETWEEN start AND end over the same segments, as two calls.
+ * fb_window_range_bounds writes, per row i, the first and last row d_lo[i] / d_hi[i] of its frame (int64;
+ * d_hi[i] < d_lo[i]: empty).  Every segment is sorted by one presort key, NULL keys last: d_keys holds the
+ * key as 8-byte values (int64 for FB_RANGE_KEY_I64, uint64 for FB_RANGE_KEY_U64, f64 for FB_RANGE_KEY_F64)
+ * and d_key_valid its validity (NULL: all valid; a float key's NaN rows must be cleared in it); -0.0 equals
+ * 0.0.  descending != 0: the keys descend.  start / end are the offsets as 8-byte patterns of the key
+ * class's type (int64 offsets for both integer classes, f64 offsets for FB_RANGE_KEY_F64).  For a non-NULL
+ * key k_i, row j with a non-NULL key k_j is in the frame when k_i + start <= k_j <= k_i + end (descending:
+ * k_i - end <= k_j <= k_i - start): exact integer sums (a sum past the type's range selects nothing on
+ * that side), one IEEE f64 addition for f64 keys.  A NULL key's frame is its NULL peers.  Either way
+ * FB_FRAME_UNBOUNDED_START / _END extend a side to the segment's first / last row.  Cost O(log distance)
+ * per row (a galloping search from the row).  Scratch: fb_window_range_bounds_scratch_bytes.
+ * fb_window_bounded writes, per column c and row i, the count of valid rows in [d_lo[i], d_hi[i]] clamped
+ * to [0, nrows) and ops[c] over them, 0 where the count is 0: the contract of fb_window_frame for any
+ * intervals (no monotonicity assumed).  An aligned power-of-two block tree (level l: op and count of rows
+ * [m 2^l, (m + 1) 2^l)) answers each interval from at most two blocks per level: O(log width) per row,
+ * bit-identical runs, f64 sums made of the frame's own values.  Scratch: fb_window_bounded_scratch_bytes
+ * (16 bytes per row and column). */
+#define FB_RANGE_KEY_I64 0
+#define FB_RANGE_KEY_U64 1
+#define FB_RANGE_KEY_F64 2
+size_t fb_window_range_bounds_scratch_bytes(int64_t nseg);
+int fb_window_range_bounds(int dev, void* stream, int64_t nrows, int64_t nseg, const int64_t* d_offsets,
+                           const void* d_keys, const uint8_t* d_key_valid, int key_class, int descending,
+                           uint64_t start, uint64_t end, int flags, int64_t* d_lo, int64_t* d_hi, void* scratch,
+                           size_t scratch_bytes);
+size_t fb_window_bounded_scratch_bytes(int64_t nrows, int ncols);
+int fb_window_bounded(int dev, void* stream, int64_t nrows, const int64_t* d_lo, const int64_t* d_hi, int ncols,
+                      const int32_t* ops, const void* const* vals, const uint8_t* const* valid, void* const* out_vals,
+                      int64_t* const* out_count, void* scratch, size_t scratch_bytes);
+
 /* ---------------------------------------------------------------------------
  * K7  hash equi-join on one 8-byte key (other key shapes are packed by the host layer)
  * Replaces: NativeExecutionEngine.join -> triad PandasUtils.join -> pd.merge

@@ -193,18 +193,41 @@ class B200MapEngine:
                 run(pdf, 0)
         elif len(pdf) > 0:
             offsets = edf.native.offsets.cpu().tolist()
+            by = _host_group_keys(edf.native, pdf, spec.partition_by)
             no = 0
             for p in range(len(offsets) - 1):
                 if offsets[p + 1] == offsets[p]:
                     continue
                 part = pdf.iloc[offsets[p]:offsets[p + 1]]
-                for _, sub in part.groupby(spec.partition_by, dropna=False, sort=True):
+                for _, sub in part.groupby([s.iloc[offsets[p]:offsets[p + 1]] for s in by], dropna=False, sort=True):
                     no += 1
                     run(sub, no)
         if not outs:
             return engine.to_df(ArrowDataFrame(None, output_schema))
         res = pd.concat(outs, ignore_index=True)
         return engine.to_df(PandasDataFrame(res, output_schema))
+
+
+_NULLABLE_INT = {pa.int8(): pd.Int8Dtype(), pa.int16(): pd.Int16Dtype(), pa.int32(): pd.Int32Dtype(),
+                 pa.int64(): pd.Int64Dtype(), pa.uint8(): pd.UInt8Dtype(), pa.uint16(): pd.UInt16Dtype(),
+                 pa.uint32(): pd.UInt32Dtype(), pa.uint64(): pd.UInt64Dtype()}
+
+
+def _host_group_keys(t: B200Table, pdf: pd.DataFrame, keys: List[str]) -> List[pd.Series]:
+    """What pandas groups the rows of a host callback by, so that its groups are the logical partitions (DESIGN
+    §7d).  pandas cannot group a float16 column: it groups a float64 copy.  pandas holds an integer column with
+    NULLs as float64, which merges values that differ beyond 2^53 (uint64 2^63 - 1 and 2^63): such a column groups
+    as a nullable integer.  The callback still gets the columns as ``pdf`` holds them."""
+    out = []
+    for k in keys:
+        tp = t.schema.types[t.schema.index_of_key(k)]
+        s = pdf[k]
+        if tp == pa.float16():
+            s = s.astype("float64")
+        elif pa.types.is_integer(tp) and s.dtype.kind == "f":
+            s = t.select([k]).to_arrow().column(k).to_pandas(types_mapper=_NULLABLE_INT.get)
+        out.append(s)
+    return out
 
 
 def decompose_aggs(agg_cols: List[Any]) -> Any:
@@ -395,10 +418,12 @@ class B200ExecutionEngine(EngineLifecycle):
         kidx = [t.schema.index_of_key(k) for k in keys]
         kcols = [t.columns[i] for i in kidx]
         kvalid = [t.valid[i] for i in kidx]
-        normalized = logical and any(c.dtype in (torch.float32, torch.float64) for c in kcols)
+        ktypes = [t.schema.types[i] for i in kidx]
+        normalized = logical and any(pa.types.is_floating(tp) for tp in ktypes)
         if normalized:
-            kvalid = [S.float_key_valid(c, v) if c.is_floating_point() else v for c, v in zip(kcols, kvalid)]
-            kcols = [S.float_key_bits(c) if c.is_floating_point() else c for c in kcols]
+            keyed = [S.float_key(c, tp, v) if pa.types.is_floating(tp) else (c, v)
+                     for c, tp, v in zip(kcols, ktypes, kvalid)]
+            kcols, kvalid = [c for c, _ in keyed], [v for _, v in keyed]
         elif t.offsets is not None and t.partition_keys == keys and t.num_partitions == num:
             return edf  # already partitioned this way
         if num > K.MAX_PARTITIONS:
@@ -581,24 +606,37 @@ class B200ExecutionEngine(EngineLifecycle):
         multi = len(keys) > 1
         kidx = [t.schema.index_of_key(k) for k in keys]
 
-        def key_bits64(c: torch.Tensor) -> torch.Tensor:
-            if c.is_floating_point():  # -0.0 groups with 0.0 (DESIGN §7d)
-                return S.float_key_bits(c).to(torch.int64)
-            return c if c.dtype == torch.int64 else c.to(torch.int64)
+        # float keys (DESIGN §7d): -0.0 groups with 0.0, and a NaN key is NULL, so it groups with the NULL keys
+        key_bits, key_valid = {}, {}
+        for i in kidx:
+            c, tp = t.columns[i], t.schema.types[i]
+            if pa.types.is_floating(tp):
+                c, key_valid[i] = S.float_key(c, tp, t.valid[i])
+            else:
+                key_valid[i] = t.valid[i]
+            key_bits[i] = c if c.dtype == torch.int64 else c.to(torch.int64)
 
-        # a NaN key is NULL: it groups with the NULL keys (DESIGN §7d)
-        key_valid = {i: S.float_key_valid(t.columns[i], t.valid[i]) if t.columns[i].is_floating_point()
-                     else t.valid[i] for i in kidx}
+        def key_column(raw: torch.Tensor, i: int) -> torch.Tensor:
+            """The stored key column of arrow type ``t.schema.types[i]`` from its int64 group key."""
+            tp, sd = t.schema.types[i], t.columns[i].dtype
+            if tp == pa.float16():
+                return narrow(raw.view(torch.float64), tp)
+            if sd == torch.float64:
+                return raw.view(torch.float64)
+            if sd == torch.float32:
+                return raw.to(torch.int32).view(torch.float32)
+            return raw if sd == torch.int64 else raw.to(sd)
+
         if len(keys) == 1:
             ki = kidx[0]
-            kcol, kvalid, ktype = t.columns[ki], key_valid[ki], t.schema.types[ki]
-            key64 = key_bits64(kcol)
+            kvalid, ktype = key_valid[ki], t.schema.types[ki]
+            key64 = key_bits[ki]
         elif multi:
             # several key columns: group on the 64-bit hash of the key tuple (same hash as the
             # partitioner) and carry MIN/MAX of every key column as hidden aggregates: a group whose
             # MIN != MAX (or that mixes NULL and non-NULL) is a hash collision -> error instead of a
             # silently merged group.  The key values of the output are the MINs.
-            kb = [key_bits64(t.columns[i]).contiguous() for i in kidx]
+            kb = [key_bits[i].contiguous() for i in kidx]
             key64 = K.row_hash64(kb, [key_valid[i] for i in kidx])
             kvalid, ktype = None, None
         else:
@@ -683,29 +721,14 @@ class B200ExecutionEngine(EngineLifecycle):
                 bad |= (gaggs[smin] != gaggs[smax]).any() if scnt is None else \
                     (((gaggs[scnt] > 0) & (gaggs[smin] != gaggs[smax])) |
                      ((gaggs[scnt] > 0) & (gaggs[scnt] != gaggs[rows_slot]))).any()
-                kc = t.columns[i]
-                raw = gaggs[smin]
-                if kc.dtype == torch.float64:
-                    out_k = raw.view(torch.float64)
-                elif kc.dtype == torch.float32:
-                    out_k = raw.to(torch.int32).view(torch.float32)
-                else:
-                    out_k = raw if kc.dtype == torch.int64 else raw.to(kc.dtype)
                 fields.append(pa.field(k, t.schema.types[i]))
-                cols.append(out_k.contiguous())
+                cols.append(key_column(gaggs[smin], i).contiguous())
                 valids.append(None if scnt is None else (gaggs[scnt] > 0).to(torch.uint8))
             assert_or_throw(not bool(bad), RuntimeError(
                 "64-bit hash collision between two distinct key tuples in a multi-column GROUP BY"))
         if len(keys) == 1:
-            kc = t.columns[ki]
-            if kc.dtype == torch.float64:
-                out_k = gkeys.view(torch.float64)
-            elif kc.dtype == torch.float32:
-                out_k = gkeys.to(torch.int32).view(torch.float32)
-            else:
-                out_k = gkeys if kc.dtype == torch.int64 else gkeys.to(kc.dtype)
             fields.append(pa.field(keys[0], ktype))
-            cols.append(out_k.contiguous())
+            cols.append(key_column(gkeys, ki).contiguous())
             valids.append(gvalid)
         dicts = {k: t.dictionaries[k] for k in keys if k in t.dictionaries}
         for name, kind, slot, tp, nn in plan:

@@ -14,7 +14,8 @@ import torch
 from . import kernels as K
 from .dataframe import B200DataFrame
 from .schema import Schema, SchemaError
-from .table import B200Table
+from .sort import float_key
+from .table import B200Table, widen
 
 _JOIN_TYPES = ["semi", "left_semi", "anti", "left_anti", "inner", "left_outer", "right_outer",
                "full_outer", "cross"]
@@ -58,19 +59,15 @@ def _key64(t1: B200Table, t2: B200Table, keys: List[str]):
     """One 8-byte surrogate key per row on both sides + validity (NULL in any key -> never matches).
     A NaN in a float key counts as NULL: it never matches, on either key path, as in the reference, where
     pandas holds NULL as NaN.  exact == False means the surrogate is a hash and matches must be verified."""
-    def norm(c: torch.Tensor) -> torch.Tensor:
-        if c.dtype in (torch.float32, torch.float64):
-            return torch.where(c == 0, torch.zeros_like(c), c)  # -0.0 == 0.0
-        return c
-
     def cols_of(t: B200Table, remap=None):
         out, val = [], None
         for k in keys:
             i = t.schema.index_of_key(k)
-            c = norm(t.columns[i])
-            if c.dtype in (torch.float32, torch.float64):
-                not_nan = (c == c).to(torch.uint8)
-                val = not_nan if val is None else val & not_nan
+            c, tp = t.columns[i], t.schema.types[i]
+            if pa.types.is_floating(tp):  # bits with -0.0 read as 0.0; a NaN clears the row's validity
+                c, not_nan = float_key(c, tp, None)
+                if not_nan is not None:
+                    val = not_nan if val is None else val & not_nan
             if remap is not None and k in remap:
                 m = remap[k]
                 c = m[c.long().clamp(min=0)]
@@ -93,11 +90,7 @@ def _key64(t1: B200Table, t2: B200Table, keys: List[str]):
     if len(keys) == 1 and c1[0].element_size() == 8:
         return c1[0].view(torch.int64), v1, c2[0].view(torch.int64), v2, True
     if len(keys) == 1:
-        def widen(c):
-            if c.dtype == torch.float32:
-                c = c.view(torch.int32)
-            return c.to(torch.int64)
-        return widen(c1[0]), v1, widen(c2[0]), v2, True
+        return c1[0].to(torch.int64), v1, c2[0].to(torch.int64), v2, True
     return K.row_hash64(c1), v1, K.row_hash64(c2), v2, False
 
 
@@ -112,6 +105,9 @@ def _verify(t1: B200Table, t2: B200Table, keys: List[str], li: torch.Tensor, ri:
             pos = pc.index_in(d2, value_set=d1).fill_null(-1)
             m = torch.from_numpy(pos.to_numpy(zero_copy_only=False).astype("int32")).to(li.device)
             b = m[b.long()]
+        tp = t1.schema[k].type
+        if pa.types.is_floating(tp):  # compare values: -0.0 == 0.0, also for float16 (stored as int16)
+            a, b = widen(a, tp), widen(b, tp)
         ok &= a == b
     return ok
 

@@ -47,6 +47,14 @@ def float_key_valid(c: torch.Tensor, v: Optional[torch.Tensor]) -> Optional[torc
     return None if bool(ok.all()) else ok.to(torch.uint8)
 
 
+def float_key(c: torch.Tensor, tp: pa.DataType,
+              v: Optional[torch.Tensor]) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
+    """(bits, validity) of a stored float key column of arrow type ``tp`` under §7d.  float16 (stored as int16) is
+    widened to float64 first, exactly, so its bits are int64; float32 / float64 keep their width."""
+    w = widen(c, tp) if tp == pa.float16() else c
+    return float_key_bits(w), float_key_valid(w, v)
+
+
 def _unsigned_order_key(t: B200Table, name: str, ascending: bool) -> torch.Tensor:
     """int64 tensor whose bit pattern, read as unsigned, orders like the column."""
     i = t.schema.index_of_key(name)
@@ -150,8 +158,7 @@ def group_starts(t: B200Table, keys: List[str]) -> torch.Tensor:
         i = t.schema.index_of_key(k)
         c, v = t.columns[i], t.valid[i]
         if pa.types.is_floating(t.schema.types[i]):
-            w = widen(c, t.schema.types[i]) if c.dtype == torch.int16 else c  # float16
-            c, v = float_key_bits(w), float_key_valid(w, v)
+            c, v = float_key(c, t.schema.types[i], v)
         if v is None:
             diff = c[1:] != c[:-1]
         else:

@@ -110,6 +110,9 @@ SIGNATURES = {
     "fb_window_bounded_scratch_bytes": (C.c_size_t, [C.c_int64, C.c_int]),
     "fb_window_bounded": (C.c_int, [C.c_int, _vp, C.c_int64, _vp, _vp, C.c_int, _i32p, _vpp, _vpp, _vpp, _vpp, _vp,
                                     C.c_size_t]),
+    "fb_quantile_scratch_bytes": (C.c_size_t, [C.c_int, C.c_int64, C.c_int64]),
+    "fb_segmented_quantile": (C.c_int, [C.c_int, _vp, C.c_int64, C.c_int64, _vp, _vp, _vp, C.c_int, C.c_int,
+                                        C.POINTER(C.c_double), _i32p, _vp, _vpp, _vp, C.c_size_t]),
 }
 
 

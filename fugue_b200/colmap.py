@@ -28,7 +28,7 @@ import pyarrow as pa
 import torch
 
 from . import kernels as K
-from .column import ColumnExpr, Kind, SelectColumns, col as _col, has_window, is_agg
+from .column import PERCENTILES, ColumnExpr, Kind, SelectColumns, col as _col, has_window, is_agg
 from .table import B200Table, narrow, widen
 
 
@@ -177,7 +177,7 @@ def _with_windows(t: B200Table, cols: List[ColumnExpr]) -> B200Table:
     by the evaluator (K8), running / partition aggregates and ranks by the segmented scan (K9), moving
     frames (``rows``) by the frame kernel, value frames (``range``) by the bounds kernel (or the peer groups)
     and the block tree, all with the same finishers, FIRST / LAST / partition values / LAG / LEAD by row
-    gathers."""
+    gathers, percentiles by the quantile kernel (K10), one call per argument column with all its q values."""
     from . import expr as X
     from . import sort as S
     from .schema import Schema
@@ -229,6 +229,7 @@ def _with_windows(t: B200Table, cols: List[ColumnExpr]) -> B200Table:
 
     # ---- scans: collected first, all run in one call per frame (None: the running scan)
     scans: Dict[Any, List[Any]] = {}
+    quantiles: Dict[str, List[Tuple[float, int]]] = {}  # argument column -> its (q, CONT | DISC) pairs
     finish: List[Any] = []     # per node: (fingerprint, fn(scan results) -> (column, validity, type, dictionary))
 
     def scan(op: int, v: Any, m: Any, frame: Any = None) -> Tuple[Any, int]:
@@ -240,6 +241,12 @@ def _with_windows(t: B200Table, cols: List[ColumnExpr]) -> B200Table:
         fn = bare.func
         if fn in ("LAG", "LEAD"):
             finish.append((uid, _offset_value(base, bare, arg_name, rows, seg_first, seg_last)))
+            continue
+        if fn in PERCENTILES:
+            name = arg_name[bare.arg.fingerprint()]
+            qs = quantiles.setdefault(name, [])
+            qs.append((bare.kwargs["q"], K.QUANTILE_CONT if fn == "PERCENTILE_CONT" else K.QUANTILE_DISC))
+            finish.append((uid, _percentile_value(base, name, len(qs) - 1, fn == "PERCENTILE_CONT", lengths, n)))
             continue
         if fn == "ROW_NUMBER":
             finish.append((uid, lambda r, rows=rows: (rows - seg_first() + 1, None, pa.int64(), None)))
@@ -342,6 +349,8 @@ def _with_windows(t: B200Table, cols: List[ColumnExpr]) -> B200Table:
         else:
             res = K.window_frame(off.contiguous(), n, frame[0], frame[1], spec)
         results.update(((frame, j), r) for j, r in enumerate(res))
+    for name, qs in quantiles.items():
+        results[("quantile", name)] = K.segmented_quantile(off.contiguous(), *quantile_input(base, name), qs)
     names, types, columns, valid = list(base.schema.names), list(base.schema.types), list(base.columns), list(base.valid)
     dicts = dict(base.dictionaries)
     window_names: Dict[str, str] = {}
@@ -358,6 +367,40 @@ def _with_windows(t: B200Table, cols: List[ColumnExpr]) -> B200Table:
     out = _WindowTable(Schema([pa.field(a, b) for a, b in zip(names, types)]), columns, valid, dicts)
     out.window_names = window_names
     return out
+
+
+def quantile_input(t: B200Table, name: str) -> Tuple[torch.Tensor, Optional[torch.Tensor], int]:
+    """Column ``name`` as the 8-byte values, validity and value class of the quantile kernel: floats as
+    float64, unsigned integers as uint64, strings as their dictionary rank, everything else as int64."""
+    from . import sort as S
+
+    i = t.schema.index_of_key(name)
+    c, m, tp = t.columns[i], t.valid[i], t.schema.types[i]
+    if name in t.dictionaries:
+        return S._unsigned_order_key(t, name, True), m, K.RANGE_KEY_U64
+    if pa.types.is_floating(tp):
+        return widen(c, tp).contiguous(), m, K.RANGE_KEY_F64
+    return widen(c, tp).contiguous(), m, K.RANGE_KEY_U64 if pa.types.is_unsigned_integer(tp) else K.RANGE_KEY_I64
+
+
+def _percentile_value(base: B200Table, name: str, j: int, cont: bool, lengths: torch.Tensor, n: int) -> Any:
+    """The finisher of a percentile node: its per-partition result repeated over the partition's rows; a
+    DISC result is the picked row's own value (any type), gathered."""
+    i = base.schema.index_of_key(name)
+    c, m, tp = base.columns[i], base.valid[i], base.schema.types[i]
+    if cont and (name in base.dictionaries or not (pa.types.is_integer(tp) or pa.types.is_floating(tp))):
+        raise NotImplementedError(f"PERCENTILE_CONT needs an integer or float column; {name} is {tp}")
+
+    def run(r: Any) -> Any:
+        count, outs = r[("quantile", name)]
+        has = torch.repeat_interleave(count > 0, lengths, output_size=n)
+        res = torch.repeat_interleave(outs[j], lengths, output_size=n)
+        if cont:
+            return res.contiguous(), has.to(torch.uint8), pa.float64(), None
+        (g,), (gv,) = K.gather_rows([c], [m], res.contiguous(), want_valid=True)
+        return g, gv, tp, base.dictionaries.get(name)
+
+    return run
 
 
 _TIME_UNIT_US = {"s": 1_000_000, "ms": 1_000, "us": 1}  # microseconds per unit ("ns": 1 / 1000)

@@ -6,8 +6,10 @@ from an expression is a function of ``(kind, head, args)``:
     NAMED     head = column name                     WILDCARD  ``*``
     LITERAL   head = python value (None = NULL)      UNARY     head in ``- ~ IS_NULL NOT_NULL``, one arg
     BINARY    head in ``+ - * / & | < > <= >= == !=``  CALL      head = function name (``COALESCE`` ...)
-    AGG       head in ``SUM COUNT AVG MIN MAX FIRST LAST``, one arg, optional DISTINCT
-    WINDOW    head in the AGG functions (one arg, kwargs ``running``, ``rows`` or ``range``), ``ROW_NUMBER RANK
+    AGG       head in ``SUM COUNT AVG MIN MAX FIRST LAST``, one arg, optional DISTINCT, or ``PERCENTILE_CONT
+              PERCENTILE_DISC``, one arg and kwarg ``q`` (MEDIAN is PERCENTILE_CONT at q = 0.5)
+    WINDOW    head in the AGG functions (one arg, kwargs ``running``, ``rows`` or ``range``; a percentile keeps
+              its ``q`` and covers the whole partition), ``ROW_NUMBER RANK
               DENSE_RANK`` (no arg) or ``LAG LEAD`` (one arg, kwargs ``n`` and ``default``): evaluated over the logical
               partitions of ``fa.transform`` (PartitionSpec keys, presort order) by a ``ColumnMap``
 
@@ -48,6 +50,7 @@ BOOL_OPS = frozenset(["&", "|", "<", ">", "<=", ">=", "==", "!="])
 ARITH_OPS = frozenset(["+", "-", "*", "/"])
 AGG_KEEPS_ARG_TYPE = frozenset(["MIN", "MAX", "FIRST", "LAST"])
 WINDOW_AGGS = frozenset(["SUM", "COUNT", "AVG", "MIN", "MAX", "FIRST", "LAST"])
+PERCENTILES = frozenset(["PERCENTILE_CONT", "PERCENTILE_DISC"])
 _RANKINGS = frozenset(["ROW_NUMBER", "RANK", "DENSE_RANK"])
 _RUNNING_FRAME = "ROWS BETWEEN UNBOUNDED PRECEDING AND CURRENT ROW"
 _LITERAL_TYPES = (int, bool, float, str)
@@ -199,6 +202,8 @@ class ColumnExpr:
             return tp if fits else None
         if k == Kind.AGG and self.head in AGG_KEEPS_ARG_TYPE:
             return self.args[0].infer_type(schema)
+        if k in (Kind.AGG, Kind.WINDOW) and self.head in PERCENTILES:
+            return pa.float64() if self.head == "PERCENTILE_CONT" else self.args[0].infer_type(schema)
         if k == Kind.WINDOW:
             if self.head in _RANKINGS or self.head == "COUNT":
                 return pa.int64()
@@ -271,10 +276,14 @@ class ColumnExpr:
             raise ValueError(f"{self} is not an aggregation: only an aggregation has an OVER form")
         if self.is_distinct:
             raise ValueError(f"{self}: DISTINCT aggregations have no window form")
-        if self.head not in WINDOW_AGGS:
+        if self.head not in WINDOW_AGGS and self.head not in PERCENTILES:
             raise ValueError(f"{self}: {self.head} has no window form")
         if not isinstance(running, bool):
             raise ValueError(f"running must be a bool, got {running!r}")
+        if self.head in PERCENTILES:
+            if running or rows is not None or range is not None:
+                raise ValueError(f"{self}: a percentile covers the whole partition; it takes no frame")
+            return ColumnExpr(Kind.WINDOW, self.head, self.args, self.kwargs, False, self.as_name, self.as_type)
         if range is not None:
             if running or rows is not None:
                 raise ValueError("over() takes one of running=True, rows and range")
@@ -373,6 +382,21 @@ def agg(func: str, arg: Any, as_name: str = "", arg_distinct: bool = False) -> C
     return ColumnExpr(Kind.AGG, func.upper(), [col(arg)], None, arg_distinct, as_name)
 
 
+def _percentile(func: str, c: Any, q: Any) -> ColumnExpr:
+    """``PERCENTILE_CONT / PERCENTILE_DISC(q) WITHIN GROUP (ORDER BY c)``; ``q`` an int or float in [0, 1]."""
+    if isinstance(q, bool) or not isinstance(q, (int, float)) or not 0 <= q <= 1:  # NaN fails the range test
+        raise ValueError(f"{func}: q must be an int or float in [0, 1], got {q!r}")
+    arg = col(c)
+    if arg.kind == Kind.WILDCARD or is_agg(arg) or has_window(arg):
+        raise ValueError(f"{func} needs a row-wise column expression, got {arg}")
+    return ColumnExpr(Kind.AGG, func, [arg], {"q": float(q)})
+
+
+def _within_group(e: ColumnExpr, show: Any) -> str:
+    """``PERCENTILE_CONT(q) WITHIN GROUP (ORDER BY arg)``: the SQL form of a percentile."""
+    return f"{e.head}({e.kwargs['q']!r}) WITHIN GROUP (ORDER BY {show(e.args[0])})"
+
+
 def is_agg(column: Any) -> bool:
     """True when the expression contains an aggregation anywhere."""
     if not isinstance(column, ColumnExpr):
@@ -395,6 +419,8 @@ def has_window(column: Any) -> bool:
 
 def _window_text(e: ColumnExpr, show: Any) -> str:
     """``FUNC(args) OVER (frame)`` of a WINDOW node; ``show`` renders one argument."""
+    if e.head in PERCENTILES:
+        return _within_group(e, show) + " OVER ()"
     parts = [show(x) for x in e.args]
     if e.head in ("LAG", "LEAD"):
         parts += [str(e.kwargs["n"]), _show_literal(e.kwargs["default"])]
@@ -515,6 +541,21 @@ class functions:
 
     mean = avg
     is_agg = staticmethod(is_agg)
+
+    @staticmethod
+    def percentile_cont(c: Any, q: Any) -> ColumnExpr:
+        """The q-quantile of the non-NULL values, interpolated linearly between the two nearest (float64)."""
+        return _percentile("PERCENTILE_CONT", c, q)
+
+    @staticmethod
+    def percentile_disc(c: Any, q: Any) -> ColumnExpr:
+        """The first value (in ascending order) whose cumulative distribution reaches q; keeps the type."""
+        return _percentile("PERCENTILE_DISC", c, q)
+
+    @staticmethod
+    def median(c: Any) -> ColumnExpr:
+        """``percentile_cont(c, 0.5)``: the same node."""
+        return _percentile("PERCENTILE_CONT", c, 0.5)
 
     @staticmethod
     def row_number() -> ColumnExpr:
@@ -644,6 +685,8 @@ def to_sql(expr: ColumnExpr, enable_cast: bool = True, nested: bool = False) -> 
                 "NOT_NULL": inner + " IS NOT NULL"}[expr.head]
     elif k == Kind.WINDOW:
         body = _window_text(expr, lambda x: to_sql(_operand(x), enable_cast))
+    elif k == Kind.AGG and expr.head in PERCENTILES:
+        body = _within_group(expr, lambda x: to_sql(x, enable_cast))
     elif k == Kind.BINARY:
         if expr.head not in BOOL_OPS and expr.head not in ARITH_OPS:
             raise NotImplementedError(expr)

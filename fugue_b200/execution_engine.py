@@ -580,12 +580,13 @@ class B200ExecutionEngine(EngineLifecycle):
 
     @staticmethod
     def _plain_aggs(agg_cols: List[Any]) -> bool:
-        """``SUM/COUNT/MIN/MAX/AVG`` of a named column (or ``*``) without casts: what the group-by
-        kernel takes directly (and what the distributed engine decomposes into partial / final)."""
+        """``SUM/COUNT/MIN/MAX/AVG/FIRST/LAST/PERCENTILE_*`` of a named column (or ``*``) without casts: what
+        ``_aggregate_named`` takes directly (and what the distributed engine decomposes into partial / final)."""
         from .column import ColumnExpr, Kind
 
         return all(isinstance(a, ColumnExpr) and a.kind == Kind.AGG and a.as_type is None and not a.is_distinct
-                   and a.func in ("SUM", "COUNT", "MIN", "MAX", "AVG", "FIRST", "LAST")
+                   and a.func in ("SUM", "COUNT", "MIN", "MAX", "AVG", "FIRST", "LAST", "PERCENTILE_CONT",
+                                  "PERCENTILE_DISC")
                    and a.arg.kind in (Kind.NAMED, Kind.WILDCARD) and a.arg.as_type is None
                    and not (a.func in ("FIRST", "LAST") and a.arg.kind == Kind.WILDCARD)
                    for a in agg_cols)
@@ -596,7 +597,10 @@ class B200ExecutionEngine(EngineLifecycle):
         import pyarrow as pa
 
         from . import sort as S
+        from .column import PERCENTILES
 
+        if any(a.func in PERCENTILES for a in agg_cols):
+            return self._aggregate_sorted(df, partition_spec, agg_cols)
         edf = self.to_df(df)
         t: B200Table = edf.native
         keys = [] if partition_spec is None else list(partition_spec.partition_by)
@@ -755,6 +759,66 @@ class B200ExecutionEngine(EngineLifecycle):
             valids.append(v)
         return B200DataFrame(B200Table(Schema(fields), cols, valids, dicts))
 
+    def _aggregate_sorted(self, df: Any, partition_spec: Optional[PartitionSpec],
+                          agg_cols: List[Any]) -> B200DataFrame:
+        """GROUP BY with a percentile among the aggregates: sort by the keys (stable, so FIRST / LAST keep their
+        input-order meaning), then every aggregate as its whole-partition window form over the groups (the
+        segmented scan, the quantile kernel K10), then the first row of every group."""
+        import pyarrow as pa
+
+        from collections import OrderedDict
+
+        from . import sort as S
+        from .colmap import _with_windows
+        from .column import Kind, col
+
+        t: B200Table = self.to_df(df).native
+        keys = [] if partition_spec is None else list(partition_spec.partition_by)
+        names = list(dict.fromkeys(keys + [a.arg.name for a in agg_cols if a.arg.kind != Kind.WILDCARD]))
+        sub = t.select(names)
+        sub = B200Table(sub.schema, sub.columns, sub.valid, sub.dictionaries)
+        n, dev = sub.num_rows, sub.device
+        if keys:
+            sub = S.take_rows(sub, S.argsort_rows(sub, OrderedDict((k, True) for k in keys)))
+            sub.logical_offsets = S.logical_offsets(sub, keys)
+        else:
+            sub.logical_offsets = torch.tensor([0, n], dtype=torch.int64, device=dev)
+        nodes = [a.alias("").over() for a in agg_cols]
+        fields: List[Any] = []
+        cols: List[Any] = []
+        valids: List[Any] = []
+        dicts: Dict[str, Any] = {}
+        if n == 0 and not keys:  # SQL: a global aggregate of an empty table is one row, NULL but for COUNT
+            for a, e in zip(agg_cols, nodes):
+                tp = e.infer_type(sub.schema) or pa.float64()
+                is_count = a.func == "COUNT"
+                fields.append(pa.field(a.output_name, tp))
+                cols.append(narrow(torch.zeros(1, dtype=torch.float64 if pa.types.is_floating(tp) else torch.int64,
+                                               device=dev), tp).contiguous())
+                valids.append(None if is_count else torch.zeros(1, dtype=torch.uint8, device=dev))
+                if a.func not in ("COUNT", "PERCENTILE_CONT") and a.arg.name in sub.dictionaries:
+                    dicts[a.output_name] = sub.dictionaries[a.arg.name]
+            return B200DataFrame(B200Table(Schema(fields), cols, valids, dicts))
+        w = _with_windows(sub, nodes)
+        first = sub.logical_offsets[:-1].contiguous()
+        picked = [col(k) for k in keys] + [w.window_column(e) for e in nodes]
+        src = [w.schema.index_of_key(c.name) for c in picked]
+        g, gv = K.gather_rows([w.columns[i] for i in src], [w.valid[i] for i in src], first, want_valid=False)
+        for j, (i, c, v) in enumerate(zip(src, g, gv)):
+            nm = w.schema.names[i]
+            tp = w.schema.types[i]
+            out = keys[j] if j < len(keys) else agg_cols[j - len(keys)].output_name
+            if j < len(keys) and pa.types.is_floating(tp):  # DESIGN §7d: -0.0 groups as 0.0, a NaN key is NULL
+                f = widen(c, tp)
+                v = S.float_key_valid(f, v)
+                c = narrow(torch.where(f == 0, torch.zeros_like(f), f), tp)
+            fields.append(pa.field(out, tp))
+            cols.append(c.contiguous())
+            valids.append(v)
+            if nm in w.dictionaries:
+                dicts[out] = w.dictionaries[nm]
+        return B200DataFrame(B200Table(Schema(fields), cols, valids, dicts))
+
     # ---- select / filter / assign (K8) ---------------------------------------------------
     def select(self, df: Any, cols: Any, where: Any = None, having: Any = None) -> B200DataFrame:
         """``ExecutionEngine.select`` (execution_engine.py:736-806): ``SELECT cols FROM df [WHERE ...]
@@ -763,7 +827,7 @@ class B200ExecutionEngine(EngineLifecycle):
         SQL text.  Pins: fugue_test/execution_suite.py:98-155."""
         from . import expr as X
         from . import relational as R
-        from .column import ColumnExpr, Kind, SelectColumns, agg as _agg, col, has_window, is_agg
+        from .column import PERCENTILES, ColumnExpr, Kind, SelectColumns, agg as _agg, col, has_window, is_agg
 
         for e in list(cols.all_cols) + [where, having]:
             assert_or_throw(not has_window(e), lambda: NotImplementedError(
@@ -816,8 +880,8 @@ class B200ExecutionEngine(EngineLifecycle):
             uid = bare.fingerprint()
             if uid in agg_col:
                 continue
-            assert_or_throw(a.func in ("SUM", "COUNT", "MIN", "MAX", "AVG", "FIRST", "LAST"),
-                            NotImplementedError(f"aggregation {a.func}"))
+            assert_or_throw(a.func in ("SUM", "COUNT", "MIN", "MAX", "AVG", "FIRST", "LAST", "PERCENTILE_CONT",
+                                       "PERCENTILE_DISC"), NotImplementedError(f"aggregation {a.func}"))
             assert_or_throw(not is_agg(a.arg), ValueError(f"nested aggregation {a}"))
             out = f"__fb_a{len(agg_col)}"
             agg_col[uid] = out
@@ -832,17 +896,20 @@ class B200ExecutionEngine(EngineLifecycle):
                 distinct_outs.append(out)
                 continue
             if a.arg.kind == Kind.WILDCARD:
-                named_aggs.append(_agg(a.func, col("*"), out))
+                arg = col("*")
             elif a.arg.kind == Kind.LITERAL:
-                nm = temp(a.arg.alias("").cast(a.arg.as_type), "l")
-                named_aggs.append(_agg(a.func, col(nm), out))
+                arg = col(temp(a.arg.alias("").cast(a.arg.as_type), "l"))
             else:
-                named_aggs.append(_agg(a.func, col(temp(a.arg, "v")), out))
+                arg = col(temp(a.arg, "v"))
+            # the same aggregation of the temporary column (a percentile keeps its q)
+            named_aggs.append(ColumnExpr(Kind.AGG, a.func, [arg], a.kwargs, False, out))
         if len(pre) == 0:  # e.g. SELECT COUNT(*) FROM t
             tmp = t
         else:
             tmp = X.project(t, pre)
         # (self.aggregate, not the local kernel wrapper: the distributed engine shuffles partials here)
+        assert_or_throw(distinct_on is None or not any(a.func in PERCENTILES for a in named_aggs),
+                        NotImplementedError("COUNT(DISTINCT ...) and a percentile in one SELECT"))
         if distinct_on is None:
             g = self.aggregate(B200DataFrame(tmp), PartitionSpec(by=key_names) if key_names else None,
                                named_aggs).native

@@ -3,6 +3,7 @@
 torch is used here only as the owner of device memory and streams; every
 operation is a call into ``libfugue_b200.so``.
 """
+import ctypes as C
 import struct
 from typing import Any, List, Optional, Sequence, Tuple
 
@@ -553,6 +554,47 @@ def window_bounded(lo: torch.Tensor, hi: torch.Tensor,
             _lib.ptr_array([c.data_ptr() for c in cnts]), scratch.data_ptr(), scratch.numel()))
         res.extend(zip(outs, cnts))
     return res
+
+
+QUANTILE_TILE_ROWS = 2048   # FB_QUANTILE_TILE_ROWS: longest segment of the one-pass shared-memory path
+QUANTILE_MAX_Q = 16
+QUANTILE_CONT = 0
+QUANTILE_DISC = 1
+
+
+def segmented_quantile(offsets: torch.Tensor, values: torch.Tensor, valid: Optional[torch.Tensor], value_class: int,
+                       quantiles: Sequence[Tuple[float, int]]) -> Tuple[torch.Tensor, List[torch.Tensor]]:
+    """K10: exact quantiles of every segment ``[offsets[s], offsets[s + 1])`` of one column (``values``: 8-byte
+    values of ``value_class``, a ``RANGE_KEY_*``; ``valid``: uint8 validity or None; f64 NaN is NULL too).
+    ``quantiles`` = ``(q, QUANTILE_CONT | QUANTILE_DISC)`` pairs; up to ``QUANTILE_MAX_Q`` share one call.
+    Returns (per segment the non-NULL count m, per pair a result per segment: f64 for CONT, 0 where m = 0;
+    for DISC the int64 row of the picked value, -1 where m = 0)."""
+    lib = _lib.load()
+    assert offsets.dtype == torch.int64 and offsets.is_cuda and offsets.is_contiguous()
+    dev = offsets.device
+    nseg = int(offsets.shape[0]) - 1
+    n = int(values.shape[0])
+    assert values.element_size() == 8 and values.device == dev and values.is_contiguous()
+    if valid is not None:
+        assert valid.dtype == torch.uint8 and valid.device == dev and valid.is_contiguous() and valid.shape[0] == n
+    count = torch.empty(nseg, dtype=torch.int64, device=dev)
+    outs = [torch.empty(nseg, dtype=torch.float64 if kind == QUANTILE_CONT else torch.int64, device=dev)
+            for _, kind in quantiles]
+    if nseg == 0 or not quantiles:
+        return count, outs
+    lengths = offsets[1:] - offsets[:-1]
+    long_rows = int(torch.where(lengths > QUANTILE_TILE_ROWS, lengths, 0).sum()) if n > QUANTILE_TILE_ROWS else 0
+    nb = int(lib.fb_quantile_scratch_bytes(dev.index, n, long_rows))
+    scratch = torch.empty(max(nb, 8), dtype=torch.uint8, device=dev)
+    for b in range(0, len(quantiles), QUANTILE_MAX_Q):
+        batch = quantiles[b:b + QUANTILE_MAX_Q]
+        qs = (C.c_double * len(batch))(*[float(q) for q, _ in batch])
+        _lib.check(lib.fb_segmented_quantile(
+            dev.index, _stream_ptr(dev), n, nseg, offsets.data_ptr(), values.data_ptr(),
+            0 if valid is None else valid.data_ptr(), value_class, len(batch), qs,
+            _lib.i32_array([kind for _, kind in batch]), count.data_ptr(),
+            _lib.ptr_array([o.data_ptr() for o in outs[b:b + QUANTILE_MAX_Q]]), scratch.data_ptr(), scratch.numel()))
+    return count, outs
 
 
 def exclusive_scan(counts: torch.Tensor) -> Tuple[torch.Tensor, int]:

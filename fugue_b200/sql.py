@@ -487,6 +487,32 @@ class _Parser:
                     self.fail(f"{fn}(DISTINCT ...)")
                 return functions.count_distinct(arg)
             return _AGG_FUNCS[fn](arg)
+        if fn == "MEDIAN":
+            arg = self.expr()
+            self.expect(")")
+            return functions.median(arg)
+        if fn in ("PERCENTILE_CONT", "PERCENTILE_DISC"):
+            # PERCENTILE_CONT(q) WITHIN GROUP (ORDER BY x [ASC]): consumed here, so that GROUP is not read as
+            # a GROUP BY clause and WITHIN not as an implicit alias
+            q = self._quantile_literal(fn)
+            self.expect(")")
+            if not self.kw("WITHIN", "GROUP"):
+                self.fail(f"{fn}(q) needs WITHIN GROUP (ORDER BY ...)")
+            self.expect("(")
+            if not self.kw("ORDER", "BY"):
+                self.fail(f"{fn} WITHIN GROUP needs ORDER BY")
+            arg = self.expr()
+            if self.kw("DESC"):
+                raise NotImplementedError(f"{fn} WITHIN GROUP (ORDER BY ... DESC) in: {self.sql}")
+            self.kw("ASC")
+            self.expect(")")
+            return functions.percentile_cont(arg, q) if fn == "PERCENTILE_CONT" else functions.percentile_disc(arg, q)
+        if fn in ("QUANTILE_CONT", "QUANTILE_DISC"):  # DuckDB's spelling: QUANTILE_CONT(x, q)
+            arg = self.expr()
+            self.expect(",")
+            q = self._quantile_literal(fn)
+            self.expect(")")
+            return functions.percentile_cont(arg, q) if fn == "QUANTILE_CONT" else functions.percentile_disc(arg, q)
         args: List[Any] = []
         if not self.op(")"):
             while True:
@@ -497,6 +523,13 @@ class _Parser:
         if fn == "COALESCE":
             return functions.coalesce(*args)
         return function(fn, *args)
+
+    def _quantile_literal(self, fn: str) -> Any:
+        kind, val = self.peek()
+        if kind != "num":
+            self.fail(f"{fn} needs a numeric literal q")
+        self.i += 1
+        return _number(val)
 
     # ---- select items / lists
     def item(self) -> ColumnExpr:

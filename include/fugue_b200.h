@@ -313,6 +313,38 @@ int fb_window_bounded(int dev, void* stream, int64_t nrows, const int64_t* d_lo,
                       int64_t* const* out_count, void* scratch, size_t scratch_bytes);
 
 /* ---------------------------------------------------------------------------
+ * K10 exact order statistics per segment: PERCENTILE_CONT / PERCENTILE_DISC / MEDIAN of one column over the
+ *     segments [d_offsets[s], d_offsets[s + 1]) of fb_segmented_scan (logical partitions, sorted groups)
+ * Replaces: a pandas function per logical partition (fugue/execution/native_execution_engine.py:156-164)
+ *           for groupby().quantile(q).
+ * d_vals holds 8-byte values of value_class (FB_RANGE_KEY_I64 / _U64 / _F64: narrower types widened by the
+ * host, strings as dictionary ranks), d_valid their validity (NULL: all valid).  NULL rows and f64 NaN are
+ * skipped; the non-NULL values of a segment are ordered ascending, -0.0 equal to 0.0, ties by row.  m is
+ * their number, written to d_count[s].  For each of the nq <= FB_QUANTILE_MAX_Q pairs (qs[j] in [0, 1],
+ * kinds[j]), outs[j] receives per segment:
+ *   FB_QUANTILE_CONT  f64: h = q (m - 1), lo = floor(h), frac = h - lo; x[lo] if frac == 0, else
+ *                     x[lo] + (x[lo + 1] - x[lo]) frac, every step one IEEE f64 op (values converted to f64 by
+ *                     their class, uint64 as unsigned); 0 where m = 0.
+ *   FB_QUANTILE_DISC  int64: the row at sorted position max(ceil(q m) - 1, 0) (q m one f64 multiply); -1
+ *                     where m = 0.  The caller gathers the value (fb_gather_rows), for any column type.
+ * Segments of at most FB_QUANTILE_TILE_ROWS rows are sorted in shared memory by the CTA whose window of that
+ * many rows they start in (the column is read once); longer segments are sorted by fb_radix_pass over their
+ * rows only, then picked.  The path depends on the segment length alone and both give the same results.
+ * qs, kinds and outs are HOST arrays.  Scratch: fb_quantile_scratch_bytes, where long_rows is the number of
+ * rows in segments longer than FB_QUANTILE_TILE_ROWS (an upper bound is fine).  With long segments the call
+ * synchronises `stream` twice (their number and their key range decide the radix passes).
+ * --------------------------------------------------------------------------- */
+#define FB_QUANTILE_MAX_Q 16
+#define FB_QUANTILE_TILE_ROWS 2048
+#define FB_QUANTILE_CONT 0
+#define FB_QUANTILE_DISC 1
+size_t fb_quantile_scratch_bytes(int dev, int64_t nrows, int64_t long_rows);
+int fb_segmented_quantile(int dev, void* stream, int64_t nrows, int64_t nseg, const int64_t* d_offsets,
+                          const void* d_vals, const uint8_t* d_valid, int value_class, int nq, const double* qs,
+                          const int32_t* kinds, int64_t* d_count, void* const* outs, void* scratch,
+                          size_t scratch_bytes);
+
+/* ---------------------------------------------------------------------------
  * K7  hash equi-join on one 8-byte key (other key shapes are packed by the host layer)
  * Replaces: NativeExecutionEngine.join -> triad PandasUtils.join -> pd.merge
  *             fugue/execution/native_execution_engine.py:230-241

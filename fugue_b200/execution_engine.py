@@ -472,8 +472,14 @@ class B200ExecutionEngine(EngineLifecycle):
         got = Schema([pa.field(n, u[6]) for n, u in zip(names, units)])
         assert_or_throw(got == output_schema, lambda: f"map output {got} mismatches given {output_schema}")
         kidx = [t.schema.index_of_key(k) for k in keys]
+        kcols, kvalid = [t.columns[i] for i in kidx], [t.valid[i] for i in kidx]
+        for j, i in enumerate(kidx):  # the same partitions as _repartition_logical: float keys under DESIGN §7d
+            if pa.types.is_floating(t.schema.types[i]):
+                from . import sort as S
+
+                kcols[j], kvalid[j] = S.float_key(kcols[j], t.schema.types[i], kvalid[j])
         scratch = self._pool.scratch(t.device, K.partition_scratch_bytes(t.device, t.num_rows, num))
-        plan = K.partition_plan([t.columns[i] for i in kidx], num, [t.valid[i] for i in kidx], scratch=scratch)
+        plan = K.partition_plan(kcols, num, kvalid, scratch=scratch)
         outs = K.partition_apply_map(plan, [u[:6] for u in units])
         outs = [o.view(torch.float64) if u[6] == pa.float64() else
                 (o.view(torch.int64) if o.dtype != torch.int64 and u[2] != K.MAP_COPY else o)

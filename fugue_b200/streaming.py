@@ -25,6 +25,7 @@ import pyarrow as pa
 import torch
 
 from . import kernels as K
+from . import sort as S
 from .dataframe import ArrowDataFrame, B200DataFrame, DataFrame
 from .partition import PartitionSpec
 from .schema import Schema
@@ -88,8 +89,14 @@ def streaming_transform(engine: Any, local_df: DataFrame, runner: Any, out_schem
             ev_in[c] = ev
     for k in keys:
         s_cmp.wait_event(ev_in[k])
+    # pass 1 hashes float keys as the logical hash partition of map_dataframe does (DESIGN §7d): -0.0 read as 0.0,
+    # NaN as NULL, float16 widened to float64; pass 2 moves the original columns
+    kcols, kvalid = [dcols[k] for k in keys], [None] * len(keys)
+    for i, k in enumerate(keys):
+        if pa.types.is_floating(schema[k].type):
+            kcols[i], kvalid[i] = S.float_key(dcols[k], schema[k].type, None)
     scratch = engine._pool.scratch(dev, K.partition_scratch_bytes(dev, n, num))
-    plan = K.partition_plan([dcols[k] for k in keys], num, scratch=scratch)
+    plan = K.partition_plan(kcols, num, kvalid, scratch=scratch)
     ev_out = {}
     for c in order:
         s_cmp.wait_event(ev_in[c])

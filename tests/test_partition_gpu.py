@@ -200,16 +200,84 @@ def test_full_size_properties_100m_rows():
     assert int((rid ^ (rid >> 7)).sum()) == int((rowid ^ (rowid >> 7)).sum())
 
 
-@pytest.mark.parametrize("env", [{}, {"FB_SCATTER": "swc"}, {"FB_DISABLE_TMA": "1"}, {"FB_WS_COLS": "8"},
-                                 {"FB_WS_COLS": "1"}])
-def test_all_scatter_kernel_paths_agree(env, monkeypatch):
-    """warp-specialised (default), single-role write-combining (v4) and generic kernels: same bits."""
-    for k, v in env.items():
-        monkeypatch.setenv(k, v)
+def _misaligned(a: np.ndarray):
+    """``a`` on the device at an address that is 8- but not 16-byte aligned (8-byte columns): a column of a
+    device table sliced at row 1."""
+    t = torch.empty(len(a) + 1, dtype=_to_dev(a[:1]).dtype, device=_dev())
+    t[1:].copy_(_to_dev(a))
+    assert t[1:].data_ptr() % 16 == 8 or a.dtype.itemsize < 8
+    return t[1:]
+
+
+def _check_scatter_route(route: str) -> None:
+    from fugue_b200 import api as fa
+    from fugue_b200 import kernels as K
+    from fugue_b200.dataframe import B200DataFrame
+    from fugue_b200.partition import PartitionSpec
+    from fugue_b200.table import B200Table
+
     rng = np.random.default_rng(23)
     n = 1_234_567
-    cols = [rng.integers(0, 1 << 16, n).astype("int64")] + \
-           [rng.integers(-(2**62), 2**62, n).astype("int64") for _ in range(4)] + \
-           [rng.standard_normal(n) for _ in range(5)]          # 10 columns: more than one launch
-    _check_partition(cols, [0], 256)
-    _check_partition(cols, [0, 5], 200)                           # two key columns, num not a power of two
+    key = rng.integers(0, 1 << 16, n).astype("int64")
+    c8 = [rng.integers(-(2**62), 2**62, n).astype("int64") for _ in range(4)] + \
+         [rng.standard_normal(n) for _ in range(5)]
+    if route.startswith("misaligned"):
+        # 8-byte columns at an 8-byte boundary take the generic kernel over all chunks (all-8-byte or mixed widths),
+        # next to 16-byte-aligned ones on the fast kernel
+        num = int(route.split("_")[-1])
+        mixed = "mixed" in route
+        cols = [key] + c8 + ([rng.integers(-2**31, 2**31, n).astype("int32"), rng.integers(0, 256, n).astype("uint8")]
+                             if mixed else [])
+        dcols = [_misaligned(c) if i % 2 == 0 or c.dtype.itemsize < 8 else _to_dev(c) for i, c in enumerate(cols)]
+        out, off = K.partition_columns(dcols, [0, 3], num)
+        exp, exp_off = hp.partition_table(cols, [0, 3], num)
+        assert np.array_equal(off.cpu().numpy(), exp_off)
+        for c, (a, b) in enumerate(zip(out, exp)):
+            assert np.array_equal(_bytes(a), b.view("u1")), f"column {c} differs"
+    elif route.startswith("cols_per_launch"):
+        per = int(route.split("_")[-1])
+        d = [_to_dev(c) for c in [key] + c8]                          # 10 aligned 8-byte columns
+        plan = K.partition_plan([d[0]], 256)
+        out = K.partition_apply(plan, d, cols_per_launch=per)
+        exp, exp_off = hp.partition_table([key] + c8, [0], 256)
+        assert np.array_equal(plan.offsets.cpu().numpy(), exp_off)
+        for c, (a, b) in enumerate(zip(out, exp)):
+            assert np.array_equal(_bytes(a), b.view("u1")), f"column {c} differs"
+    else:
+        # a device table sliced at row 1 through engine.repartition / fa.transform; the validity mask travels too
+        import pyarrow as pa
+
+        v = rng.random(n) < 0.9
+        tbl = pa.table({"k": key, "a": c8[0], "x": pa.array(c8[5], mask=~v),
+                        "i": rng.integers(0, 9, n).astype("int32")})
+        t = B200Table.from_arrow(tbl, _dev()).slice(1, n)
+        e = fa.make_execution_engine("b200")
+        spec = PartitionSpec(by="k", algo="hash", num=200)
+        assert t.columns[0].data_ptr() % 16 == 8 and t.columns[3].data_ptr() % 16 == 4
+
+        def identity(tb: B200Table) -> B200Table:
+            return tb
+
+        if route == "repartition_sliced":
+            got = e.repartition(B200DataFrame(t), spec).native
+        else:
+            got = fa.transform(B200DataFrame(t), identity, schema="*", partition=spec, engine=e, as_fugue=True).native
+            assert got.offsets is not None
+        cols = [c.cpu().numpy() for c in t.columns] + [t.valid[2].cpu().numpy()]
+        assert np.array_equal(cols[4], v[1:].astype("uint8"))
+        exp, exp_off = hp.partition_table(cols, [0], 200)
+        assert np.array_equal(got.offsets.cpu().numpy(), exp_off)
+        for c in range(4):
+            assert np.array_equal(_bytes(got.columns[c]), exp[c].view("u1")), f"column {c} differs"
+        assert np.array_equal(got.valid[2].cpu().numpy(), exp[4])
+        assert got.valid[0] is None and got.valid[1] is None and got.valid[3] is None
+
+
+@pytest.mark.parametrize("route", ["misaligned_all8_256", "misaligned_mixed_256", "misaligned_mixed_200",
+                                   "misaligned_all8_1000", "cols_per_launch_1", "cols_per_launch_8",
+                                   "repartition_sliced", "transform_sliced"])
+def test_scatter_routes_agree(route):
+    """Every route of pass 2: the fast kernel on 16-byte-aligned 8-byte columns (num <= 256) in groups of 1 and 8
+    columns per launch, and the generic kernel (all-8-byte or mixed widths) on the rest, also over a device table
+    sliced at row 1: the same bits as the oracle."""
+    _check_scatter_route(route)

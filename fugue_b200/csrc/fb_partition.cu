@@ -662,20 +662,36 @@ __device__ __forceinline__ void tma_load_1d(uint32_t dst_smem, const void* src, 
 //   warps 16-23  rankers  : place tile t+1: advance the write-combining state of every partition,
 //                           build the slot list of the tile
 //   warps 0-15   movers   : tile t: per column gather from the staged tile / carry, store whole
-//                           sector groups, save the new carry (in place: the per-column barrier
+//                           G-row groups, save the new carry (in place: the per-column barrier
 //                           separates the reads of the old carry from the writes of the new one)
 // Hand-off through mbarriers: slots_ready (rankers -> movers), slots_free (movers -> rankers, as
 // soon as the slot list sits in mover registers), flush_done at chunk ends, full/empty per ring
 // stage and per pid buffer.
 // Shared memory (one CTA per SM), T = 4096, E = num * (G - 1):
 //   ring[S][T] u64 | mbarriers | carry[ncols][E] u64 | slotinfo[T+E] u32 | wpos kcnt binfo
-//   bin_n wstart wdelta [nbp] u32 | scanw[64] | carryinfo[E] u16 | rank records [2][12800 B]
+//   wstart wdelta [nbp] u32 | scanw[64] | carryinfo[E] u16 | rank records [2][12800 B]
 // ---------------------------------------------------------------------------
 constexpr int kWsMoverWarps = 16, kWsRankWarps = 8;
 constexpr int kWsMovers = kWsMoverWarps * 32, kWsRankers = kWsRankWarps * 32;
 constexpr int kWsThreads = kWsMovers + kWsRankers + 128;  // + producer warpgroup (1 active warp)
-constexpr int kWsG = 4;  // rows per write-combined group (32 B); 8 (64 B) was slower: spills, 3 ring stages
+// Rows per write-combined group.  16 rows = 128 B = one whole L2 line per store event, so a line never waits
+// half-written in L2 for the next tile of its CTA, and DRAM gets it in one write-back.  H100 at 700 W, 100 M rows
+// x 8 columns in groups of 2: 5.31 ms at G = 4 (one sector), 5.18 at G = 8, 5.04 at G = 16 (MEASUREMENTS.md).
+constexpr int kWsG = 16;
+// Groups of other sizes use 4-row (32 B, one sector) groups: a single column per CTA is slower at G = 16, and the
+// G = 16 carry (30 KB per column at num = 256) of 3 or more columns leaves fewer than kWsMinStages ring stages.
+constexpr int kWsGWide = 4;
+constexpr int kWsMinStages = 3;
 constexpr int kWsRankItems = 16;  // rows per ranker thread per tile: tile = 256 x 16 = 4096 rows (2048: no faster)
+// Registers per thread of each role (setmaxnreg).  The launch gives every thread 65536 / 896 -> 72; the producer
+// warpgroup and the rankers hand theirs to the movers, whose G = 16 slot lists (16 slot rounds, 8 carry rounds) do
+// not fit 72.  128 x 24 + 256 x 64 + 512 x 88 = 896 x 72.
+constexpr uint32_t kWsProducerRegs = 24, kWsRankerRegs = 64, kWsMoverRegs = 88;
+static_assert(128 * kWsProducerRegs + kWsRankers * kWsRankerRegs + kWsMovers * kWsMoverRegs <= kWsThreads * 72,
+              "setmaxnreg: the roles take more registers than the launch gives the CTA");
+// Slot rounds a mover gathers before it stores them: bounds the values live at once (4 and 8 run alike; all 16
+// rounds at once spill)
+constexpr int kMoveBatch = 8;
 
 // The units of every column group of one launch.  Group k holds units [k * per_group, min(nunits,
 // (k + 1) * per_group)).  CTA b moves group b % ngroups over chunks b / ngroups, + S, + 2S, ... with
@@ -720,7 +736,7 @@ __host__ __device__ inline size_t ws_book_bytes(uint32_t num, int ncols) {
   size_t b = 64 * 8;                           // mbarriers
   b += (size_t)ncols * E * 8;                  // carry buffers (in place)
   b += (kT + E) * 4;                           // slotinfo
-  b += 6 * nbp * 4 + 64 * 4;                   // per-partition arrays + scanw
+  b += 5 * nbp * 4 + 64 * 4;                   // per-partition arrays + scanw
   b += ((E * 2 + 15) / 16) * 16;               // carryinfo
   b += 2 * (size_t)kMetaBytes + 128;           // rank records (+ alignment slack)
   return b;
@@ -731,6 +747,11 @@ __device__ __forceinline__ void mbar_arrive(uint32_t bar) {  // release.cta: pub
 }
 __device__ __forceinline__ void mover_sync() { asm volatile("bar.sync 1, %0;" ::"n"(kWsMovers) : "memory"); }
 __device__ __forceinline__ void ranker_sync() { asm volatile("bar.sync 2, %0;" ::"n"(kWsRankers) : "memory"); }
+// warpgroup-wide register reallocation (sm_90a; SASS: USETMAXREG)
+template <uint32_t N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <uint32_t N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 
 template <int kBits, int G, int kWsRankItems, bool kMap>
 __global__ void __launch_bounds__(kWsThreads, 1)
@@ -740,11 +761,12 @@ fb_scatter_ws_kernel(WsUnits units, uint32_t num, ChunkGeom g, int nstages,
                      const __grid_constant__ WsMap map) {
   constexpr uint32_t T = (uint32_t)kWsRankers * kWsRankItems;  // rows per tile
   static_assert(T == (uint32_t)kTile, "pass 1 ranks tiles of kTile rows");
+  // kcnt keeps the pending count (phantoms included) and the phantom count in 8 bits each
+  static_assert(G >= 2 && G <= 16 && (G & (G - 1)) == 0, "G must be a power of two <= 16");
   constexpr uint32_t GM = G - 1;
   constexpr uint32_t kStageBytes = T * 8;
   constexpr int kSlotRounds = ((int)T + (int)kSwcMaxNum * (G - 1) + kWsMovers - 1) / kWsMovers;
   constexpr int kEntryRoundsM = ((int)kSwcMaxNum * (G - 1) + kWsMovers - 1) / kWsMovers;
-  constexpr int kEntryRoundsR = ((int)kSwcMaxNum * (G - 1) + kWsRankers - 1) / kWsRankers;
   extern __shared__ __align__(128) uint64_t smem64[];
   const uint32_t nbp = nb_padded(num);
   const uint32_t E = num * GM;
@@ -760,8 +782,7 @@ fb_scatter_ws_kernel(WsUnits units, uint32_t num, ChunkGeom g, int nstages,
   uint32_t* wpos = slotinfo + T + E;
   uint32_t* kcnt = wpos + nbp;
   uint32_t* binfo = kcnt + nbp;
-  uint32_t* bin_n = binfo + nbp;
-  uint32_t* wstart = bin_n + nbp;
+  uint32_t* wstart = binfo + nbp;
   uint32_t* wdelta = wstart + nbp;
   uint32_t* scanw = wdelta + nbp;  // [8,16) written per ranker warp, [40] W
   uint16_t* carryinfo = (uint16_t*)(scanw + 64);
@@ -772,10 +793,6 @@ fb_scatter_ws_kernel(WsUnits units, uint32_t num, ChunkGeom g, int nstages,
   const uint32_t bar_pid_full = smem_u32(bars + 32), bar_pid_empty = smem_u32(bars + 34);
   const uint32_t bar_slots_ready = smem_u32(bars + 36), bar_slots_free = smem_u32(bars + 37);
   const uint32_t bar_flush_done = smem_u32(bars + 38);
-  // per column step: "all movers have read the old carry".  Two barriers used alternately: the wait
-  // for step k happens during step k+1, after this warp's arrival for step k+1, so a single barrier
-  // could run two phases ahead of a pending parity wait (deadlock); with two, at most one.
-  const uint32_t bar_carry_read = smem_u32(bars + 40);
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < nstages; ++s) {
@@ -789,14 +806,13 @@ fb_scatter_ws_kernel(WsUnits units, uint32_t num, ChunkGeom g, int nstages,
     mbar_init(bar_slots_ready, kWsRankWarps);
     mbar_init(bar_slots_free, kWsMoverWarps);
     mbar_init(bar_flush_done, kWsMoverWarps);
-    mbar_init(bar_carry_read, kWsMoverWarps);
-    mbar_init(bar_carry_read + 8, kWsMoverWarps);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
 
   if (warp >= kWsMoverWarps + kWsRankWarps) {
     // ============================ producer =============================================
+    setmaxnreg_dec<kWsProducerRegs>();
     if (warp == kWsMoverWarps + kWsRankWarps && lane == 0) {
       // the payload is read once: evict first.  A rank record is read by every group of its chunk: kept
       // in L2 for the sibling CTAs (H100 at 400 W, 100 M rows x 8 columns in 4 groups: records loaded
@@ -851,6 +867,7 @@ fb_scatter_ws_kernel(WsUnits units, uint32_t num, ChunkGeom g, int nstages,
 
   if (warp >= kWsMoverWarps) {
     // ============================ rankers (8 warps) ====================================
+    setmaxnreg_dec<kWsRankerRegs>();
     const unsigned rw = warp - kWsMoverWarps;          // ranker warp 0..7
     const unsigned rtid = threadIdx.x - kWsMovers;     // 0..255
     uint32_t seq = 0, cseq = 0;
@@ -869,19 +886,10 @@ fb_scatter_ws_kernel(WsUnits units, uint32_t num, ChunkGeom g, int nstages,
         const uint32_t pb = seq & 1, pph = (seq >> 1) & 1;
         mbar_wait(bar_pid_full + 8 * pb, pph);
         const uint8_t* __restrict__ rec = metabuf + pb * kMetaBytes;
-        // rows of this thread: r * 256 + rtid; packed (partition id << 16) | rank in tile
-        uint32_t pr[kWsRankItems];
-#pragma unroll
-        for (int r = 0; r < kWsRankItems; ++r) {
-          const uint32_t row = r * kWsRankers + rtid;
-          pr[r] = ((uint32_t)rec[row] << 16) | ((const uint16_t*)(rec + kMetaRank))[row];
-        }
         // ---- per partition (thread b < num): tile count, rows to write, new pending state
         const uint32_t b = rtid;
         uint32_t n = 0, w = 0, kold = 0, phold = 0, wp_old = 0;
         if (b < num) n = ((const uint16_t*)(rec + kMetaCnt))[b];
-        __syncwarp();
-        if (lane == 0) mbar_arrive_relaxed(bar_pid_empty + 8 * pb);  // the record is in registers
         if (b < num) {
           const uint32_t kc = kcnt[b];
           kold = kc & 0xFFu;
@@ -896,8 +904,7 @@ fb_scatter_ws_kernel(WsUnits units, uint32_t num, ChunkGeom g, int nstages,
           } else {
             kcnt[b] = (kold + n) | (phold << 8);
           }
-          binfo[b] = kold | (phold << 4) | (w << 8);
-          bin_n[b] = n;
+          binfo[b] = kold | (w << 8);
         }
         uint32_t xw = w;
 #pragma unroll
@@ -924,31 +931,31 @@ fb_scatter_ws_kernel(WsUnits units, uint32_t num, ChunkGeom g, int nstages,
         }
         if (rtid == kWsRankers - 1) scanw[40] = bw + w;  // W: slots to store this tile
         ranker_sync();  // C
-        // ---- every new row / old carry entry finds its place
+        // ---- every new row / old carry entry finds its place.  The rows of this thread (r * 256 + rtid) are read
+        //      from the record here, not kept in registers since the top of the tile: the producer fills the
+        //      other record buffer meanwhile, and needs this one only for the tile after next.
 #pragma unroll
         for (int r = 0; r < kWsRankItems; ++r) {
-          const uint32_t pb2 = pr[r] >> 16;
-          const uint32_t bi = binfo[pb2];
-          const uint32_t i = (bi & 0xFu) + (pr[r] & 0xFFFFu);
-          const uint32_t ww = bi >> 8;
           const uint32_t row = r * kWsRankers + rtid;
+          const uint32_t pb2 = rec[row];
+          const uint32_t bi = binfo[pb2];
+          const uint32_t i = (bi & 0xFFu) + ((const uint16_t*)(rec + kMetaRank))[row];
+          const uint32_t ww = bi >> 8;
           if (i < ww) slotinfo[wstart[pb2] + i] = (pb2 << 16) | row;
           else carryinfo[pb2 * GM + (i - ww)] = (uint16_t)row;
         }
+        __syncwarp();
+        if (lane == 0) mbar_arrive_relaxed(bar_pid_empty + 8 * pb);  // the record has been read
+        if (b < num) {  // the old carry entries of partition b
 #pragma unroll
-        for (int q = 0; q < kEntryRoundsR; ++q) {
-          const uint32_t e = q * kWsRankers + rtid;
-          if (e < E) {
-            const uint32_t eb = e / GM, i = e - eb * GM;
-            const uint32_t bi = binfo[eb];
-            const uint32_t ko = bi & 0xFu, po = (bi >> 4) & 0xFu, ww = bi >> 8;
-            const uint32_t nn = bin_n[eb];
-            const uint32_t desc = i < po ? 0xFFFFu : T + e;
-            if (i < ko) {
-              if (i < ww) slotinfo[wstart[eb] + i] = (eb << 16) | desc;
+          for (uint32_t i = 0; i < GM; ++i) {
+            const uint32_t e = b * GM + i;
+            const uint32_t desc = i < phold ? 0xFFFFu : T + e;
+            if (i < kold) {
+              if (i < w) slotinfo[bw + i] = (b << 16) | desc;
               else carryinfo[e] = (uint16_t)desc;
             }
-            if (ww + i >= ko + nn) carryinfo[e] = 0xFFFFu;
+            if (w + i >= kold + n) carryinfo[e] = 0xFFFFu;
           }
         }
         ranker_sync();  // D: the slot list of this tile is complete
@@ -959,7 +966,8 @@ fb_scatter_ws_kernel(WsUnits units, uint32_t num, ChunkGeom g, int nstages,
   }
 
   // ================================ movers (16 warps) ====================================
-  uint32_t s = 0, ph = 0, seq = 0, astep = 0, wstep = 0;
+  setmaxnreg_inc<kWsMoverRegs>();
+  uint32_t s = 0, ph = 0, seq = 0;
   for (int chunk = chunk_first; chunk < g.nchunks_full; chunk += chunk_step) {
     int64_t r0, r1;
     chunk_range(g, chunk, r0, r1);
@@ -978,95 +986,77 @@ fb_scatter_ws_kernel(WsUnits units, uint32_t num, ChunkGeom g, int nstages,
           dst[k] = wdelta[info >> 16] + j;
         }
       }
+      // New carry entries that come from the staged tile.  An entry carried over from an earlier tile keeps
+      // its place (its descriptor is T + e: a partition either writes all its pending rows or none), so it
+      // is neither read nor rewritten.
       uint32_t csrc[kEntryRoundsM];
 #pragma unroll
       for (int q = 0; q < kEntryRoundsM; ++q) {
         const uint32_t e = q * kWsMovers + threadIdx.x;
-        csrc[q] = e < E ? (uint32_t)carryinfo[e] : 0xFFFFu;
+        const uint32_t d = e < E ? (uint32_t)carryinfo[e] : 0xFFFFu;
+        csrc[q] = d < T ? d : 0xFFFFu;
       }
       __syncwarp();
       if (lane == 0) mbar_arrive(bar_slots_free);  // the slot list sits in registers now
 
-      // The new carry of column u is written one step late (while column u+1 moves): by then every
-      // mover has long finished reading the old carry of column u, so nobody waits at a barrier.
-      uint64_t cv_prev[kEntryRoundsM];
       for (int u = 0; u < ncols; ++u) {
         mbar_wait(bar_full + 8 * s, ph);
         const uint64_t* __restrict__ st = ring + (size_t)s * T;
         uint64_t* __restrict__ out = units.dst[u0 + u];
-        const uint64_t* __restrict__ cbuf = carry + (size_t)u * E;
-        uint64_t v[kSlotRounds], cv[kEntryRoundsM];
+        uint64_t* __restrict__ cbuf = carry + (size_t)u * E;
         uint32_t s2 = s;
         bool two = false;
+        const uint64_t* __restrict__ st2 = st;
+        int mode = 0;
+        uint64_t ma = 0, mb = 0, mc = 0;
         if constexpr (kMap) {
           // fused map (K4): rows taken from the staged tile(s) are mapped here; carry entries already are
           // output values
-          const int mode = map.mode[u0 + u];
+          mode = map.mode[u0 + u];
           two = map.src2[u0 + u] != nullptr;
-          const uint64_t* __restrict__ st2 = st;
           if (two) {
             s2 = s + 1 == (uint32_t)nstages ? 0 : s + 1;
             mbar_wait(bar_full + 8 * s2, s2 == 0 ? ph ^ 1 : ph);
             st2 = ring + (size_t)s2 * T;
           }
-          const uint64_t ma = map.a[u0 + u], mb = map.b[u0 + u], mc = map.c[u0 + u];
-#pragma unroll
-          for (int k = 0; k < kSlotRounds; ++k)
-            if (srcd[k] != 0xFFFFu)
-              v[k] = srcd[k] < T ? ws_apply_map(mode, two, st[srcd[k]], st2[srcd[k]], ma, mb, mc) : cbuf[srcd[k] - T];
-#pragma unroll
-          for (int q = 0; q < kEntryRoundsM; ++q)
-            if (csrc[q] != 0xFFFFu)
-              cv[q] = csrc[q] < T ? ws_apply_map(mode, two, st[csrc[q]], st2[csrc[q]], ma, mb, mc) : cbuf[csrc[q] - T];
-        } else {
-#pragma unroll
-          for (int k = 0; k < kSlotRounds; ++k)
-            if (srcd[k] != 0xFFFFu) v[k] = srcd[k] < T ? st[srcd[k]] : cbuf[srcd[k] - T];
-#pragma unroll
-          for (int q = 0; q < kEntryRoundsM; ++q)
-            if (csrc[q] != 0xFFFFu) cv[q] = csrc[q] < T ? st[csrc[q]] : cbuf[csrc[q] - T];
+          ma = map.a[u0 + u]; mb = map.b[u0 + u]; mc = map.c[u0 + u];
         }
+        auto staged = [&](uint32_t r) -> uint64_t {
+          if constexpr (kMap) return ws_apply_map(mode, two, st[r], st2[r], ma, mb, mc);
+          else return st[r];
+        };
+        // gather from the stage / old carry and store, kMoveBatch slot rounds at a time
 #pragma unroll
-        for (int k = 0; k < kSlotRounds; ++k)
-          if (srcd[k] != 0xFFFFu) out[dst[k]] = v[k];
-        // all my reads of the stage and of the old carry have completed (their values were
-        // consumed by the stores above / are in cv): release the stage, publish "carry read"
+        for (int k0 = 0; k0 < kSlotRounds; k0 += kMoveBatch) {
+          uint64_t v[kMoveBatch];
+#pragma unroll
+          for (int k = 0; k < kMoveBatch; ++k)
+            if (k0 + k < kSlotRounds && srcd[k0 + k] != 0xFFFFu)
+              v[k] = srcd[k0 + k] < T ? staged(srcd[k0 + k]) : cbuf[srcd[k0 + k] - T];
+#pragma unroll
+          for (int k = 0; k < kMoveBatch; ++k)
+            if (k0 + k < kSlotRounds && srcd[k0 + k] != 0xFFFFu) out[dst[k0 + k]] = v[k];
+        }
+        mover_sync();  // every mover has read the old carry of this column: it is overwritten in place
+#pragma unroll
+        for (int q = 0; q < kEntryRoundsM; ++q)
+          if (csrc[q] != 0xFFFFu) cbuf[q * kWsMovers + threadIdx.x] = staged(csrc[q]);
+        // all my reads of the stage have completed (their values were consumed by the stores above)
         __syncwarp();
         if (lane == 0) {
           mbar_arrive_relaxed(bar_empty + 8 * s);
           if (kMap && two) mbar_arrive_relaxed(bar_empty + 8 * s2);
-          mbar_arrive_relaxed(bar_carry_read + 8 * (astep & 1));
         }
-        ++astep;
         if (++s == (uint32_t)nstages) { s = 0; ph ^= 1; }
         if (kMap && two) {
           if (++s == (uint32_t)nstages) { s = 0; ph ^= 1; }
         }
-        if (u > 0) {  // write the previous column's new carry
-          mbar_wait(bar_carry_read + 8 * (wstep & 1), (wstep >> 1) & 1);
-          ++wstep;
-          uint64_t* __restrict__ pbuf = carry + (size_t)(u - 1) * E;
-#pragma unroll
-          for (int q = 0; q < kEntryRoundsM; ++q) {
-            const uint32_t e = q * kWsMovers + threadIdx.x;
-            if (csrc[q] != 0xFFFFu) pbuf[e] = cv_prev[q];
-          }
-        }
-#pragma unroll
-        for (int q = 0; q < kEntryRoundsM; ++q) cv_prev[q] = cv[q];
       }
-      {  // the last column's new carry
-        mbar_wait(bar_carry_read + 8 * (wstep & 1), (wstep >> 1) & 1);
-        ++wstep;
-        uint64_t* __restrict__ pbuf = carry + (size_t)(ncols - 1) * E;
-#pragma unroll
-        for (int q = 0; q < kEntryRoundsM; ++q) {
-          const uint32_t e = q * kWsMovers + threadIdx.x;
-          if (csrc[q] != 0xFFFFu) pbuf[e] = cv_prev[q];
-        }
-      }
+      // The new carry of column u is read in the next tile after the barrier of column u + 1 of this tile or
+      // of column 0 of the next one.  A single column has neither: order it here.
+      if (ncols == 1) mover_sync();
     }
-    // ---- chunk end: flush the pending rows (partial sector groups)
+    // ---- chunk end: flush the pending rows (partial groups)
     mover_sync();
     for (int u = 0; u < ncols; ++u) {
       uint64_t* __restrict__ out = units.dst[u0 + u];
@@ -1159,10 +1149,16 @@ cudaError_t ensure_smem_optin(int dev) {
   {
     int smem_max = 0;
     if (e == cudaSuccess) e = cudaDeviceGetAttribute(&smem_max, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
-    if (e == cudaSuccess) e = optin(fb_scatter_ws_kernel<4, kWsG, kWsRankItems, false>, (size_t)smem_max);
-    if (e == cudaSuccess) e = optin(fb_scatter_ws_kernel<8, kWsG, kWsRankItems, false>, (size_t)smem_max);
-    if (e == cudaSuccess) e = optin(fb_scatter_ws_kernel<4, kWsG, kWsRankItems, true>, (size_t)smem_max);
-    if (e == cudaSuccess) e = optin(fb_scatter_ws_kernel<8, kWsG, kWsRankItems, true>, (size_t)smem_max);
+#define FB_OPTIN_WS(G)                                                                                        \
+  do {                                                                                                        \
+    if (e == cudaSuccess) e = optin(fb_scatter_ws_kernel<4, G, kWsRankItems, false>, (size_t)smem_max);       \
+    if (e == cudaSuccess) e = optin(fb_scatter_ws_kernel<8, G, kWsRankItems, false>, (size_t)smem_max);       \
+    if (e == cudaSuccess) e = optin(fb_scatter_ws_kernel<4, G, kWsRankItems, true>, (size_t)smem_max);        \
+    if (e == cudaSuccess) e = optin(fb_scatter_ws_kernel<8, G, kWsRankItems, true>, (size_t)smem_max);        \
+  } while (0)
+    FB_OPTIN_WS(kWsG);
+    FB_OPTIN_WS(kWsGWide);
+#undef FB_OPTIN_WS
   }
   if (e == cudaSuccess) e = optin(fb_rank_kernel<true, 4, true>, kRankStageBytes);
   if (e == cudaSuccess) e = optin(fb_rank_kernel<true, 8, true>, kRankStageBytes);
@@ -1441,15 +1437,24 @@ static int apply_impl(int dev, void* stream, int64_t nrows, const FbKeys& k, boo
     const uint8_t* pid_plane = (const uint8_t*)scratch + l.pid_offset;  // rank records of pass 1
     // Column groups of at most 2, evenly sized.  Measured on H100 (100 M rows x 8 cols; MEASUREMENTS.md), one
     // launch per group at 700 W: 8 columns per group -> 6.54 ms, 4 -> 6.28, 3 -> 6.00, 2 -> 5.84, 1 -> 6.29; one
-    // launch at 400 W: 4 -> 6.25, 2 -> 5.56, 1 -> 5.88.  With more than 2 columns in flight per CTA, half-written
-    // lines no longer meet their other half in the 50 MB L2.
+    // launch at 400 W: 4 -> 6.25, 2 -> 5.56, 1 -> 5.88 (all with 4-row write groups: with more than 2 columns in
+    // flight per CTA, half-written lines no longer met their other half in the 50 MB L2).  With whole-line groups
+    // at 2 columns, one launch at 700 W: 2 -> 5.04 ms, against 5.39 for 1 column per group at G = 4.
     int ngroups = (nfast + 1) / 2;
     int per_group = (nfast + ngroups - 1) / ngroups;
     if (cols_per_launch_req >= 1 && cols_per_launch_req <= kSwcMaxCols) per_group = cols_per_launch_req;
     ngroups = (nfast + per_group - 1) / per_group;
-    const size_t book = ws_book_bytes<kWsG, kWsRankItems>(num_partitions, per_group);
     const size_t stage_bytes = (size_t)kWsRankers * kWsRankItems * 8;
-    int nstages = (int)(((size_t)smem_max - book) / stage_bytes);
+    auto stages_for = [&](size_t book) { return book < (size_t)smem_max ? (int)(((size_t)smem_max - book) / stage_bytes) : 0; };
+    // Whole-line groups (kWsG) for groups of 2 columns, if the ring keeps kWsMinStages stages next to their carry.
+    // H100 at 700 W, one launch, 100 M rows x 8 columns (MEASUREMENTS.md): 2 columns per group 5.31 ms at G = 4,
+    // 5.18 at G = 8, 5.04 at G = 16; 1 column per group 5.39 at G = 4, 6.03 at G = 16 (the rankers' longer
+    // per-tile work at G = 16 is no longer hidden behind the moves of a single column).
+    const bool lines = per_group == 2 &&
+                       stages_for(ws_book_bytes<kWsG, kWsRankItems>(num_partitions, per_group)) >= kWsMinStages;
+    const size_t book = lines ? ws_book_bytes<kWsG, kWsRankItems>(num_partitions, per_group)
+                              : ws_book_bytes<kWsGWide, kWsRankItems>(num_partitions, per_group);
+    int nstages = stages_for(book);
     if (nstages > 16) nstages = 16;
     FB_CHECK(nstages >= 2, "not enough shared memory for the TMA ring (%d stages)", nstages);
     const size_t tsmem = (size_t)nstages * stage_bytes + book;
@@ -1479,20 +1484,24 @@ static int apply_impl(int dev, void* stream, int64_t nrows, const FbKeys& k, boo
       }
       const int64_t ctas = avail < (int64_t)lg * g.nchunks_full ? avail : (int64_t)lg * g.nchunks_full;
       const int grid = (int)(ctas / lg) * lg;
-      if (maps != nullptr) {
-        if (bits == 4)
-          fb_scatter_ws_kernel<4, kWsG, kWsRankItems, true><<<grid, kWsThreads, tsmem, st>>>(
-              wu, num_partitions, g, nstages, pid_plane, (const uint32_t*)scratch, part_offsets, wm);
-        else
-          fb_scatter_ws_kernel<8, kWsG, kWsRankItems, true><<<grid, kWsThreads, tsmem, st>>>(
-              wu, num_partitions, g, nstages, pid_plane, (const uint32_t*)scratch, part_offsets, wm);
-      } else if (bits == 4) {
-        fb_scatter_ws_kernel<4, kWsG, kWsRankItems, false><<<grid, kWsThreads, tsmem, st>>>(
-            wu, num_partitions, g, nstages, pid_plane, (const uint32_t*)scratch, part_offsets, wm);
-      } else {
-        fb_scatter_ws_kernel<8, kWsG, kWsRankItems, false><<<grid, kWsThreads, tsmem, st>>>(
-            wu, num_partitions, g, nstages, pid_plane, (const uint32_t*)scratch, part_offsets, wm);
-      }
+#define FB_LAUNCH_WS(B, G, M)                                                                               \
+  fb_scatter_ws_kernel<B, G, kWsRankItems, M><<<grid, kWsThreads, tsmem, st>>>(                              \
+      wu, num_partitions, g, nstages, pid_plane, (const uint32_t*)scratch, part_offsets, wm)
+#define FB_LAUNCH_WS_G(G)                                                                                   \
+  do {                                                                                                      \
+    if (maps != nullptr) {                                                                                  \
+      if (bits == 4) FB_LAUNCH_WS(4, G, true);                                                              \
+      else FB_LAUNCH_WS(8, G, true);                                                                        \
+    } else if (bits == 4) {                                                                                 \
+      FB_LAUNCH_WS(4, G, false);                                                                            \
+    } else {                                                                                                \
+      FB_LAUNCH_WS(8, G, false);                                                                            \
+    }                                                                                                       \
+  } while (0)
+      if (lines) FB_LAUNCH_WS_G(kWsG);
+      else FB_LAUNCH_WS_G(kWsGWide);
+#undef FB_LAUNCH_WS_G
+#undef FB_LAUNCH_WS
       FB_CUDA(cudaGetLastError());
     }
     // the partial tail tile of the fast columns

@@ -113,6 +113,8 @@ SIGNATURES = {
     "fb_quantile_scratch_bytes": (C.c_size_t, [C.c_int, C.c_int64, C.c_int64]),
     "fb_segmented_quantile": (C.c_int, [C.c_int, _vp, C.c_int64, C.c_int64, _vp, _vp, _vp, C.c_int, C.c_int,
                                         C.POINTER(C.c_double), _i32p, _vp, _vpp, _vp, C.c_size_t]),
+    "fb_string_length": (C.c_int, [C.c_int, _vp, C.c_int64, _vp, _vp, _vp, _vp]),
+    "fb_string_like": (C.c_int, [C.c_int, _vp, C.c_int64, _vp, _vp, _vp, C.c_int, C.POINTER(C.c_int16), _vp, _vp]),
 }
 
 

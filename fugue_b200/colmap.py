@@ -290,7 +290,17 @@ def _with_windows(t: B200Table, cols: List[ColumnExpr]) -> B200Table:
             finish.append((uid, pick))
             continue
         if name in base.dictionaries:
-            raise NotImplementedError(f"{fn} on a string column: {bare}")
+            if fn not in ("MIN", "MAX"):
+                raise NotImplementedError(f"{fn} on a string column: {bare}")
+            rank, rm = S.string_ranks(base, name)  # MIN / MAX of the ranks, mapped back to codes
+            i = scan(K.AGG_MIN_I64 if fn == "MIN" else K.AGG_MAX_I64, rank, rm, frame)
+
+            def extreme_string(r: Any, i: Any = i, e: Any = at_end, tp: Any = tp, d: Any = base.dictionaries[name]) -> Any:
+                v, cnt = e(r[i][0]), e(r[i][1])
+                return S.codes_of_ranks(d, v), (cnt > 0).to(torch.uint8), tp, d
+
+            finish.append((uid, extreme_string))
+            continue
         is_f = pa.types.is_floating(tp)
         if fn in ("SUM", "AVG"):
             f64 = fn == "AVG" or is_f

@@ -6,6 +6,7 @@ from an expression is a function of ``(kind, head, args)``:
     NAMED     head = column name                     WILDCARD  ``*``
     LITERAL   head = python value (None = NULL)      UNARY     head in ``- ~ IS_NULL NOT_NULL``, one arg
     BINARY    head in ``+ - * / & | < > <= >= == !=``  CALL      head = function name (``COALESCE`` ...)
+              ``LIKE``: args (string, pattern literal[, escape literal]); ``LENGTH``: args (string,)
     AGG       head in ``SUM COUNT AVG MIN MAX FIRST LAST``, one arg, optional DISTINCT, or ``PERCENTILE_CONT
               PERCENTILE_DISC``, one arg and kwarg ``q`` (MEDIAN is PERCENTILE_CONT at q = 0.5)
     WINDOW    head in the AGG functions (one arg, kwargs ``running``, ``rows`` or ``range``; a percentile keeps
@@ -202,6 +203,8 @@ class ColumnExpr:
             return tp if fits else None
         if k == Kind.AGG and self.head in AGG_KEEPS_ARG_TYPE:
             return self.args[0].infer_type(schema)
+        if k == Kind.CALL and self.head in ("LIKE", "LENGTH"):
+            return pa.bool_() if self.head == "LIKE" else pa.int64()
         if k in (Kind.AGG, Kind.WINDOW) and self.head in PERCENTILES:
             return pa.float64() if self.head == "PERCENTILE_CONT" else self.args[0].infer_type(schema)
         if k == Kind.WINDOW:
@@ -260,6 +263,27 @@ class ColumnExpr:
 
     def __invert__(self) -> "ColumnExpr":
         return ColumnExpr(Kind.UNARY, "~", [self])
+
+    def like(self, pattern: Any, escape: Optional[str] = None) -> "ColumnExpr":
+        """SQL ``self LIKE pattern [ESCAPE escape]``: a case-sensitive match of the whole string, ``%`` any
+        sequence of characters, ``_`` exactly one character (code point).  No escape character unless one is
+        given; with ``escape``, it makes the next character of the pattern a literal."""
+        if isinstance(pattern, ColumnExpr) and pattern.kind == Kind.LITERAL and pattern.as_type is None:
+            pattern = pattern.value
+        if not isinstance(pattern, str):
+            raise NotImplementedError(f"LIKE needs a string literal pattern, got {pattern!r}")
+        if escape is not None:
+            if not isinstance(escape, str) or len(escape) != 1:
+                raise ValueError(f"ESCAPE takes exactly one character, got {escape!r}")
+            i = 0
+            while i < len(pattern):
+                if pattern[i] == escape:
+                    if i + 1 == len(pattern):
+                        raise ValueError(f"LIKE pattern {pattern!r} ends in the escape character {escape!r}")
+                    i += 1
+                i += 1
+        args = [self, lit(pattern)] + ([] if escape is None else [lit(escape)])
+        return ColumnExpr(Kind.CALL, "LIKE", args)
 
     def over(self, running: bool = False, rows: Optional[Tuple[Optional[int], Optional[int]]] = None,
              range: Optional[Tuple[Any, Any]] = None) -> "ColumnExpr":  # noqa: A002 - the SQL word
@@ -508,6 +532,11 @@ class functions:
         return function("COALESCE", *[_operand(x) for x in args])
 
     @staticmethod
+    def length(c: Any) -> ColumnExpr:
+        """SQL ``LENGTH(c)``: the number of characters (code points) of a string, int64."""
+        return ColumnExpr(Kind.CALL, "LENGTH", [col(c)])
+
+    @staticmethod
     def min(c: Any) -> ColumnExpr:  # noqa: A003
         return agg("MIN", c)
 
@@ -687,6 +716,12 @@ def to_sql(expr: ColumnExpr, enable_cast: bool = True, nested: bool = False) -> 
         body = _window_text(expr, lambda x: to_sql(_operand(x), enable_cast))
     elif k == Kind.AGG and expr.head in PERCENTILES:
         body = _within_group(expr, lambda x: to_sql(x, enable_cast))
+    elif k == Kind.CALL and expr.head == "LIKE":
+        body = to_sql(expr.args[0], enable_cast, True) + " LIKE " + to_sql(expr.args[1], enable_cast)
+        if len(expr.args) > 2:
+            body += " ESCAPE " + to_sql(expr.args[2], enable_cast)
+        if nested:
+            body = "(" + body + ")"
     elif k == Kind.BINARY:
         if expr.head not in BOOL_OPS and expr.head not in ARITH_OPS:
             raise NotImplementedError(expr)

@@ -95,6 +95,23 @@ __device__ __forceinline__ void store_f16(void* p, int64_t row0, int tid, int nk
   }
 }
 
+// FB_X_LOOKUP: acc <- table[acc] (8-byte entries) for the valid rows whose entry number is in [0, nent); every
+// other row is NULL
+__device__ __forceinline__ void lookup(const uint64_t* __restrict__ q, const uint8_t* m, uint64_t nent,
+                                       uint64_t (&acc)[kExprItems], unsigned& accv) {
+  unsigned nv = 0;
+#pragma unroll
+  for (int k = 0; k < kExprItems; ++k) {
+    const uint64_t e = acc[k];
+    acc[k] = 0;
+    if (((accv >> k) & 1u) && e < nent) {  // a NULL row's stored code means nothing: never an index
+      acc[k] = q[e];
+      if (m == nullptr || m[e] != 0) nv |= 1u << k;
+    }
+  }
+  accv = nv;
+}
+
 // one tile of kExprTile rows (kFull: no bounds checks; only the last tile of a table is partial)
 template <bool kFull>
 __device__ __forceinline__ void run_tile(const ExprProgram& P, int64_t row0, int nk, int tid, uint64_t* tmp_v,
@@ -112,7 +129,7 @@ __device__ __forceinline__ void run_tile(const ExprProgram& P, int64_t row0, int
       if (in.kind == FB_XK_IMM) {
 #pragma unroll
         for (int k = 0; k < kExprItems; ++k) b[k] = (uint64_t)in.imm;
-      } else if (in.kind == FB_XK_COL) {
+      } else if (in.kind == FB_XK_COL && in.op != FB_X_LOOKUP) {  // a lookup table is indexed by acc
         const void* p = P.col_ptr[in.b];
         switch (P.col_type[in.b]) {
           case FB_T_I8: load_col<int8_t, false, kFull>(p, row0, tid, nk, b); break;
@@ -234,6 +251,9 @@ __device__ __forceinline__ void run_tile(const ExprProgram& P, int64_t row0, int
         }
         case FB_X_COALESCE: FB_ROWS(if (!((accv >> k) & 1u)) acc[k] = b[k];) accv |= bv; break;
         case FB_X_RCOALESCE: FB_ROWS(if ((bv >> k) & 1u) acc[k] = b[k];) accv |= bv; break;
+        case FB_X_LOOKUP:
+          lookup((const uint64_t*)P.col_ptr[in.b], P.col_valid[in.b], (uint64_t)in.imm, acc, accv);
+          break;
         default: break;
       }
 #undef FB_BIN
@@ -288,7 +308,14 @@ extern "C" int fb_eval_expr(int dev, void* stream, int64_t nrows, int ncols, con
   }
   for (int i = 0; i < nins; ++i) {
     const fb_expr_ins& in = program[i];
-    FB_CHECK(in.op >= FB_X_MOV && in.op <= FB_X_RCOALESCE, "instruction %d: unknown op %d", i, in.op);
+    FB_CHECK(in.op >= FB_X_MOV && in.op <= FB_X_LOOKUP, "instruction %d: unknown op %d", i, in.op);
+    if (in.op == FB_X_LOOKUP) {
+      FB_CHECK(in.kind == FB_XK_COL, "instruction %d: FB_X_LOOKUP reads a column operand", i);
+      FB_CHECK(in.b >= 0 && in.b < ncols, "instruction %d: column %d out of range", i, in.b);
+      FB_CHECK(in.imm >= 0, "instruction %d: FB_X_LOOKUP table of %lld entries", i, (long long)in.imm);
+      FB_CHECK(col_types[in.b] == FB_T_I64 || col_types[in.b] == FB_T_F64,
+               "instruction %d: FB_X_LOOKUP reads a table of 8-byte values, not type %d", i, col_types[in.b]);
+    }
     FB_CHECK(in.kind >= FB_XK_NONE && in.kind <= FB_XK_NULL, "instruction %d: unknown operand kind %d", i, in.kind);
     if (in.op == FB_X_ST) {
       FB_CHECK(in.b >= 0 && in.b < FB_EXPR_NREGS, "instruction %d: temporary %d out of range", i, in.b);

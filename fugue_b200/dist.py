@@ -31,6 +31,7 @@ import numpy as np  # noqa: E402
 import torch  # noqa: E402
 import torch.distributed as dist  # noqa: E402
 
+from .column import Kind
 from .dataframe import B200DataFrame
 from .execution_engine import B200ExecutionEngine, assert_or_throw
 from .partition import PartitionSpec
@@ -611,6 +612,12 @@ class DistributedB200Engine(B200ExecutionEngine):
         rank; the result stays sharded.  SUM/COUNT/MIN/MAX decompose directly, AVG as SUM + COUNT."""
 
         keys = [] if partition_spec is None else list(partition_spec.partition_by)
+        if self._world > 1:
+            # MIN / MAX of a string column compare dictionary ranks, and every rank has its own dictionary
+            strs = self.to_df(df).native.dictionaries
+            assert_or_throw(not any(a.func in ("MIN", "MAX") and a.arg.kind == Kind.NAMED and a.arg.name in strs
+                                    for a in agg_cols if a.kind == Kind.AGG), lambda: NotImplementedError(
+                "MIN / MAX of a string column across GPUs: string dictionaries are per rank"))
         if self._world == 1 or not self._plain_aggs(agg_cols):
             # aggregations of expressions / expressions of aggregations: the base class evaluates the
             # row-wise parts locally and comes back here with plain FUNC(column) aggregations

@@ -691,7 +691,13 @@ class B200ExecutionEngine(EngineLifecycle):
                 plan.append((a.output_name, "pick", add(rowno, m, K.AGG_MIN_I64 if fn == "FIRST" else K.AGG_MAX_I64),
                              tp, (cnt, ci)))
                 continue
-            assert_or_throw(arg not in t.dictionaries, NotImplementedError(f"{fn} on a string column"))
+            if arg in t.dictionaries:  # MIN / MAX of strings: of the dictionary ranks, mapped back to codes
+                assert_or_throw(fn in ("MIN", "MAX"), NotImplementedError(f"{fn} on a string column"))
+                rank, rm = S.string_ranks(t, arg)
+                cnt = add(None, rm, K.AGG_COUNT)
+                plan.append((a.output_name, "string", add(rank, rm, K.AGG_MIN_I64 if fn == "MIN" else K.AGG_MAX_I64),
+                             tp, (cnt, arg)))
+                continue
             is_f = pa.types.is_floating(tp)
             c8 = widen(c, tp)
             # non-null count -> result validity.  A global aggregate (no keys) always carries it: over an
@@ -752,6 +758,13 @@ class B200ExecutionEngine(EngineLifecycle):
                 valids.append(has.to(torch.uint8))
                 if t.schema.names[ci] in t.dictionaries:
                     dicts[name] = t.dictionaries[t.schema.names[ci]]
+                continue
+            if kind == "string":
+                cnt, arg = nn
+                fields.append(pa.field(name, tp))
+                cols.append(S.codes_of_ranks(t.dictionaries[arg], raw))
+                valids.append((gaggs[cnt] > 0).to(torch.uint8))
+                dicts[name] = t.dictionaries[arg]
                 continue
             v = None if nn is None else (gaggs[nn] > 0).to(torch.uint8)
             if kind == "avg":

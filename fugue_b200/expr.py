@@ -10,6 +10,8 @@ Typing rules (the reference leaves them to the SQL engine; these are the pandas/
 comparisons / ``& | ~`` / ``IS NULL`` -> bool with SQL three-valued logic; an explicit ``cast`` wins.
 String columns are dictionary encoded: they can be passed through, tested for NULL and compared
 (``==`` / ``!=``) with a string literal; ``cast(str)`` of a numeric result builds a dictionary.
+``LIKE`` and ``LENGTH`` of a string column are computed once per dictionary entry (``strings.py``) and
+read per row through the entry's code (``FB_X_LOOKUP``), inside the same program.
 """
 import struct
 from typing import Any, Dict, List, Optional, Sequence, Tuple
@@ -18,6 +20,7 @@ import pyarrow as pa
 import torch
 
 from . import kernels as K
+from . import strings as ST
 from .column import ColumnExpr, Kind, lit as _lit
 from .schema import Schema
 from .table import B200Table, _storage_dtype, expr_type
@@ -62,7 +65,8 @@ class _Program:
     def __init__(self, table: B200Table):
         self.t = table
         self.ins: List[Tuple[int, int, int, int, int]] = []
-        self.cols: List[int] = []          # table column indices, in load order
+        self.cols: List[Any] = []          # table column indices / lookup-table keys, in load order
+        self.tables: Dict[Any, Tuple[torch.Tensor, Optional[torch.Tensor]]] = {}  # key -> per-entry table
         self.free = list(range(K.EXPR_NREGS - 1, -1, -1))
         self.outs: List[Tuple[torch.dtype, bool, int]] = []  # (dtype, want_valid, K8 type) per FB_X_OUT
 
@@ -80,7 +84,7 @@ class _Program:
             raise _OutOfResources("instructions")
         self.ins.append((op, kind, b, flags, imm))
 
-    def col_slot(self, ci: int) -> int:
+    def col_slot(self, ci: Any) -> int:
         if ci in self.cols:
             return self.cols.index(ci)
         if len(self.cols) >= K.EXPR_MAX_COLS:
@@ -209,6 +213,8 @@ class _Program:
         if e.kind == Kind.CALL:
             if e.func.upper() == "COALESCE":
                 return self._coalesce(e)
+            if e.func.upper() in ("LIKE", "LENGTH"):
+                return self._string_function(e, e.func.upper())
             raise NotImplementedError(f"function {e.func} has no device implementation")
         raise NotImplementedError(f"can't evaluate {e!r}")
 
@@ -281,6 +287,33 @@ class _Program:
                   (code if code is not None else -1) & ((1 << 64) - 1))
         return "b", t.valid[ci] is not None
 
+    def _string_function(self, e: ColumnExpr, fn: str) -> Tuple[str, bool]:
+        """``LIKE`` / ``LENGTH`` of a string column: the code, then its dictionary entry's result."""
+        t = self.t
+        s = e.args[0] if e.args else None
+        if not (isinstance(s, ColumnExpr) and s.kind == Kind.NAMED and s.as_type is None and s.name in t.schema
+                and _is_str(t.schema[s.name].type)):
+            raise NotImplementedError(f"{fn} needs a string column as its operand: {e}")
+        d = t.dictionaries[s.name]
+        if fn == "LIKE":
+            lits = e.args[1:]
+            if not (1 <= len(lits) <= 2 and all(a.kind == Kind.LITERAL and isinstance(a.value, str) for a in lits)):
+                raise NotImplementedError(f"LIKE needs a string literal pattern: {e}")
+            pattern, escape = lits[0].value, (lits[1].value if len(lits) > 1 else None)
+            key: Any = ("LIKE", s.name, pattern, escape)
+            if key not in self.tables:
+                self.tables[key] = ST.like_table(d, t.device, pattern, escape)
+        else:
+            if len(e.args) != 1:
+                raise ValueError(f"LENGTH takes one argument: {e}")
+            key = ("LENGTH", s.name)
+            if key not in self.tables:
+                self.tables[key] = ST.length_table(d, t.device)
+        ci = t.schema.index_of_key(s.name)
+        self.emit(K.X_MOV, K.XK_COL, self.col_slot(ci))
+        self.emit(K.X_LOOKUP, K.XK_COL, self.col_slot(key), 0, len(d))
+        return ("b" if fn == "LIKE" else "i"), t.valid[ci] is not None or self.tables[key][1] is not None
+
     def _coalesce(self, e: ColumnExpr) -> Tuple[str, bool]:
         args = [a if isinstance(a, ColumnExpr) else _lit(a) for a in e.args]
         if len(args) == 0:
@@ -331,14 +364,17 @@ class _Program:
         if e.kind == Kind.CALL and e.func.upper() == "COALESCE":
             cs = [self._static_cls(a if isinstance(a, ColumnExpr) else _lit(a)) for a in e.args]
             return "f" if "f" in cs else ("b" if "b" in cs and all(c in ("b", "n") for c in cs) else "i")
+        if e.kind == Kind.CALL and e.func.upper() == "LIKE":
+            return "b"
         return "i"
 
     def run(self) -> Tuple[List[torch.Tensor], List[Optional[torch.Tensor]]]:
         t = self.t
-        return K.eval_expr(t.num_rows, t.device, [t.columns[i] for i in self.cols],
-                           [t.valid[i] for i in self.cols], self.ins, [o[0] for o in self.outs],
-                           [o[1] for o in self.outs], col_types=[expr_type(t.schema.types[i]) for i in self.cols],
-                           out_types=[o[2] for o in self.outs])
+        cols = [t.columns[i] if isinstance(i, int) else self.tables[i][0] for i in self.cols]
+        valid = [t.valid[i] if isinstance(i, int) else self.tables[i][1] for i in self.cols]
+        types = [expr_type(t.schema.types[i]) if isinstance(i, int) else K.T_I64 for i in self.cols]
+        return K.eval_expr(t.num_rows, t.device, cols, valid, self.ins, [o[0] for o in self.outs],
+                           [o[1] for o in self.outs], col_types=types, out_types=[o[2] for o in self.outs])
 
 
 def _default_type(cls: str, e: ColumnExpr, schema: Schema) -> pa.DataType:

@@ -826,7 +826,7 @@ XF_B_I2F = 1
 (X_MOV, X_ST, X_OUT, X_I2F, X_F2I, X_NEG_I, X_NEG_F, X_NOT, X_IS_NULL, X_NOT_NULL, X_TOBOOL_I, X_TOBOOL_F,
  X_ADD_I, X_SUB_I, X_RSUB_I, X_MUL_I, X_ADD_F, X_SUB_F, X_RSUB_F, X_MUL_F, X_DIV_F, X_RDIV_F,
  X_LT_I, X_LE_I, X_GT_I, X_GE_I, X_EQ_I, X_NE_I, X_LT_F, X_LE_F, X_GT_F, X_GE_F, X_EQ_F, X_NE_F,
- X_AND, X_OR, X_COALESCE, X_RCOALESCE) = range(38)
+ X_AND, X_OR, X_COALESCE, X_RCOALESCE, X_LOOKUP) = range(39)
 
 # storage dtype of each K8 type: uint16 / uint32 / float16 live in the signed tensors of their width
 EXPR_STORAGE = {T_I8: torch.int8, T_I16: torch.int16, T_I32: torch.int32, T_I64: torch.int64, T_U8: torch.uint8,
@@ -867,8 +867,9 @@ def eval_expr(nrows: int, device: torch.device, cols: Sequence[torch.Tensor],
         prog[i].op, prog[i].kind, prog[i].b, prog[i].flags = op, kind, b, flags
         imm &= (1 << 64) - 1
         prog[i].imm = imm - (1 << 64) if imm >= (1 << 63) else imm
-    for c, tp in zip(cols, col_types):
-        assert c.is_cuda and c.is_contiguous() and c.shape[0] == nrows
+    tables = {b for op, kind, b, _, _ in program if op == X_LOOKUP}  # per-entry tables: any length
+    for j, (c, tp) in enumerate(zip(cols, col_types)):
+        assert c.is_cuda and c.is_contiguous() and (j in tables or c.shape[0] == nrows)
         assert c.element_size() == EXPR_STORAGE[tp].itemsize, f"{c.dtype} column can't hold K8 type {tp}"
     _lib.check(lib.fb_eval_expr(
         device.index, _stream_ptr(device), nrows, len(cols), _lib.ptr_array([c.data_ptr() for c in cols]),
@@ -878,3 +879,35 @@ def eval_expr(nrows: int, device: torch.device, cols: Sequence[torch.Tensor],
         _lib.ptr_array([o.data_ptr() for o in outs]),
         _lib.ptr_array([0 if v is None else v.data_ptr() for v in outv])))
     return outs, outv
+
+
+# ---- K11: string functions over a dictionary's entries ------------------------------------------
+LIKE_MAX_TOKENS, LIKE_ONE, LIKE_ANY = 1024, 256, 257
+
+
+def string_length(offsets: torch.Tensor, data: torch.Tensor, valid: Optional[torch.Tensor]) -> torch.Tensor:
+    """Code points of every entry of a device dictionary (int64 ``offsets`` of n + 1 entries, uint8 UTF-8
+    ``data``, uint8 ``valid`` or None); 0 for a NULL entry."""
+    lib = _lib.load()
+    dev = offsets.device
+    n = int(offsets.shape[0]) - 1
+    out = torch.empty(n, dtype=torch.int64, device=dev)
+    _lib.check(lib.fb_string_length(dev.index, _stream_ptr(dev), n, offsets.data_ptr(), data.data_ptr(),
+                                    0 if valid is None else valid.data_ptr(), out.data_ptr()))
+    return out
+
+
+def string_like(offsets: torch.Tensor, data: torch.Tensor, valid: Optional[torch.Tensor],
+                tokens: Sequence[int]) -> Tuple[torch.Tensor, torch.Tensor]:
+    """(match, validity) of every entry, uint8 each: the entries against a pattern compiled to ``tokens``
+    (literal bytes, ``LIKE_ONE`` for ``_``, ``LIKE_ANY`` for ``%``)."""
+    lib = _lib.load()
+    dev = offsets.device
+    n = int(offsets.shape[0]) - 1
+    out = torch.empty(n, dtype=torch.uint8, device=dev)
+    out_valid = torch.empty(n, dtype=torch.uint8, device=dev)
+    toks = (C.c_int16 * max(len(tokens), 1))(*tokens)
+    _lib.check(lib.fb_string_like(dev.index, _stream_ptr(dev), n, offsets.data_ptr(), data.data_ptr(),
+                                  0 if valid is None else valid.data_ptr(), len(tokens), toks, out.data_ptr(),
+                                  out_valid.data_ptr()))
+    return out, out_valid

@@ -55,13 +55,19 @@ def float_key(c: torch.Tensor, tp: pa.DataType,
     return float_key_bits(w), float_key_valid(w, v)
 
 
+def dictionary_order(d: pa.Array) -> np.ndarray:
+    """The entries of a string dictionary in code-point (UTF-8 byte) order, as their codes; NULL entries last.
+    The position of an entry's code here is its rank."""
+    return pc.sort_indices(d).to_numpy()
+
+
 def _unsigned_order_key(t: B200Table, name: str, ascending: bool) -> torch.Tensor:
     """int64 tensor whose bit pattern, read as unsigned, orders like the column."""
     i = t.schema.index_of_key(name)
     c, tp = t.columns[i], t.schema.types[i]
     if name in t.dictionaries:  # strings: rank of every dictionary entry in sorted order
         d = t.dictionaries[name]
-        order = pc.sort_indices(d).to_numpy()
+        order = dictionary_order(d)
         rank = np.empty(len(d), dtype=np.int64)
         rank[order] = np.arange(len(d), dtype=np.int64)
         r = torch.from_numpy(rank).to(c.device)
@@ -82,6 +88,31 @@ def _unsigned_order_key(t: B200Table, name: str, ascending: bool) -> torch.Tenso
     if not ascending:
         key = ~key
     return key.contiguous()
+
+
+def string_ranks(t: B200Table, name: str) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
+    """A string column as the rank of every row's dictionary entry (int64, see ``dictionary_order``) and its
+    validity: a NULL row or a row whose entry is NULL is not valid (None: every row is valid).  MIN / MAX of
+    the ranks are MIN / MAX of the strings in code-point order; ``codes_of_ranks`` maps them back."""
+    i = t.schema.index_of_key(name)
+    rank, v = _unsigned_order_key(t, name, True), t.valid[i]
+    d = t.dictionaries[name]
+    if d.null_count > 0:
+        ok = torch.from_numpy(d.is_valid().to_numpy(zero_copy_only=False).astype(np.uint8)).to(rank.device)
+        c = t.columns[i].long()
+        if v is not None:
+            c = torch.where(v.bool(), c, torch.zeros_like(c))  # a NULL row's stored code means nothing
+        hit = ok[c]
+        v = hit if v is None else v & hit
+    return rank, v
+
+
+def codes_of_ranks(d: pa.Array, ranks: torch.Tensor) -> torch.Tensor:
+    """The int32 codes of dictionary ``d`` whose ranks are ``ranks`` (the inverse of ``string_ranks``)."""
+    if len(d) == 0:
+        return torch.zeros(ranks.shape, dtype=torch.int32, device=ranks.device)
+    order = torch.from_numpy(dictionary_order(d).astype(np.int32)).to(ranks.device)
+    return order[ranks.clamp(0, len(d) - 1)].contiguous()
 
 
 def _radix_sort_pairs(key: torch.Tensor, idx: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:

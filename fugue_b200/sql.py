@@ -15,7 +15,8 @@ fugue/workflow/workflow.py:2109-2166) and ``ExecutionEngine.aggregate`` reaches 
              [USING (k, ...) | ON a.k = b.k [AND ...]]                        -> hash join kernels
 
 Expressions: + - * /, comparisons (= == != <> < <= > >=), AND / OR / NOT, IS [NOT] NULL, [NOT] IN (...),
-[NOT] BETWEEN, CAST(x AS type), COALESCE, literals, `quoted` and table-qualified names.
+[NOT] BETWEEN, x [NOT] LIKE 'pattern' [ESCAPE 'c'], CAST(x AS type), COALESCE, LENGTH, literals, `quoted` and
+table-qualified names.
 Anything else raises NotImplementedError (there is no host SQL fallback in this package).
 """
 import re
@@ -365,6 +366,10 @@ class _Parser:
                 e = ~self._in_or_between(e)
             elif self.at_kw("IN") or self.at_kw("BETWEEN"):
                 e = self._in_or_between(e)
+            elif self.kw("NOT", "LIKE"):
+                e = ~self._like(e)
+            elif self.kw("LIKE"):
+                e = self._like(e)
             else:
                 kind, val = self.peek()
                 if kind == "op" and val in ("=", "==", "!=", "<>", "<", "<=", ">", ">="):
@@ -374,6 +379,18 @@ class _Parser:
                          ">": e > r, ">=": e >= r}[val]
                 else:
                     return e
+
+    def _string_literal(self, what: str) -> str:
+        kind, val = self.peek()
+        if kind != "str":
+            raise NotImplementedError(f"{what} takes a string literal, got {val!r} in: {self.sql}")
+        self.i += 1
+        return _unquote(val)
+
+    def _like(self, e: ColumnExpr) -> ColumnExpr:
+        pattern = self._string_literal("LIKE")
+        escape = self._string_literal("ESCAPE") if self.kw("ESCAPE") else None
+        return e.like(pattern, escape)
 
     def _in_or_between(self, e: ColumnExpr) -> ColumnExpr:
         if self.kw("IN"):
@@ -431,8 +448,7 @@ class _Parser:
             return lit(_number(val))
         if kind == "str":
             self.i += 1
-            body = val[1:-1].replace("''", "'")
-            return lit(re.sub(r"\\(.)", r"\1", body))
+            return lit(_unquote(val))
         if kind == "op" and val == "(":
             self.i += 1
             e = self.expr()
@@ -548,6 +564,12 @@ class _Parser:
             self.i += 1  # implicit alias
             return e.alias(val[1:-1].replace("``", "`") if kind == "bq" else val)
         return e
+
+
+def _unquote(token: str) -> str:
+    """The value of a string literal token: quotes removed, '' and backslash escapes resolved."""
+    body = token[1:-1].replace("''", "'")
+    return re.sub(r"\\(.)", r"\1", body)
 
 
 def _number(text: str) -> Any:

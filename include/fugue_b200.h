@@ -453,6 +453,11 @@ int fb_join2_emit(int dev, void* stream, int64_t nprobe, const void* probe_keys,
  *   FB_X_AND / FB_X_OR: Kleene three-valued logic; FB_X_IS_NULL / FB_X_NOT_NULL / FB_X_COALESCE
  *   flags & FB_XF_B_I2F: convert operand B from int64 to float64 first
  *   FB_X_F2I: truncate toward zero; out of range saturates to INT64_MIN / INT64_MAX; NaN -> INT64_MIN
+ *   FB_X_LOOKUP acc <- B[acc]: B (FB_XK_COL, type FB_T_I64 or FB_T_F64) is a per-entry table of imm
+ *               8-byte values, not a per-row column; entry acc is read, and the table's validity (if any)
+ *               at the same entry.  A NULL accumulator, or an entry number outside [0, imm), gives
+ *               NULL and issues no load.  A dictionary-encoded string column is loaded with FB_X_MOV (its
+ *               int32 code) and mapped through a per-entry result table (fb_string_like / _length).
  * Column types: FB_T_U16 / FB_T_U32 load zero-extended, FB_T_F16 loads its IEEE half value exactly.
  * Stores keep the low bits of an integer (unsigned stores are the signed ones of the same width) and
  * round a float to nearest even (FB_T_F32, FB_T_F16).
@@ -475,7 +480,7 @@ enum fb_expr_op {
   FB_X_ADD_F = 16, FB_X_SUB_F = 17, FB_X_RSUB_F = 18, FB_X_MUL_F = 19, FB_X_DIV_F = 20, FB_X_RDIV_F = 21,
   FB_X_LT_I = 22, FB_X_LE_I = 23, FB_X_GT_I = 24, FB_X_GE_I = 25, FB_X_EQ_I = 26, FB_X_NE_I = 27,
   FB_X_LT_F = 28, FB_X_LE_F = 29, FB_X_GT_F = 30, FB_X_GE_F = 31, FB_X_EQ_F = 32, FB_X_NE_F = 33,
-  FB_X_AND = 34, FB_X_OR = 35, FB_X_COALESCE = 36, FB_X_RCOALESCE = 37
+  FB_X_AND = 34, FB_X_OR = 35, FB_X_COALESCE = 36, FB_X_RCOALESCE = 37, FB_X_LOOKUP = 38
 };
 typedef struct fb_expr_ins {
   int32_t op;    /* enum fb_expr_op */
@@ -488,6 +493,34 @@ int fb_eval_expr(int dev, void* stream, int64_t nrows, int ncols, const void* co
                  const int32_t* col_types, const uint8_t* const* col_valid, int nins,
                  const fb_expr_ins* program, int nouts, const int32_t* out_types, void* const* out_ptrs,
                  uint8_t* const* out_valid);
+
+/* ---------------------------------------------------------------------------
+ * K11 string functions, evaluated once per dictionary entry
+ * Replaces: the SQL engine's LIKE and LENGTH on a string column (fugue/column/sql.py:275-347 hands them
+ *           to qpd / pandas: Series.str.match / str.len, one Python string per row).
+ * A dictionary is the Arrow layout of a string array: entry i is the UTF-8 bytes
+ * data[offsets[i], offsets[i + 1]) (offsets: n + 1 int64), valid[i] == 0 marks a NULL entry (valid may be
+ * NULL: none).  The results are per entry; K8 maps every row's code to its entry's result (FB_X_LOOKUP).
+ *
+ * fb_string_length : out[i] = the number of code points of entry i (bytes that are not 10xxxxxx), int64;
+ *                    0 for a NULL entry.
+ * fb_string_like   : out[i] = 1 when entry i matches the pattern, else 0; out_valid[i] = valid[i] (1 when
+ *                    valid is NULL).  NULL entries give 0.  Case-sensitive, whole string.  The host compiles
+ *                    the pattern into `tokens` (ntokens <= FB_LIKE_MAX_TOKENS): a literal byte 0..255,
+ *                    FB_LIKE_ONE (`_`: exactly one code point) or FB_LIKE_ANY (`%`: any sequence, never two in
+ *                    a row).  The FB_LIKE_ANY tokens split the pattern into segments: the first is anchored at
+ *                    the start of the string, the last at its end, and each middle segment takes its leftmost
+ *                    match after the previous one (correct for LIKE without backtracking).  Matches start on
+ *                    code-point boundaries only.  tokens is a HOST array (copied into the launch).
+ * One thread per entry, grid-stride; the entries must be valid UTF-8 (Arrow strings are).
+ * --------------------------------------------------------------------------- */
+#define FB_LIKE_MAX_TOKENS 1024
+#define FB_LIKE_ONE 256
+#define FB_LIKE_ANY 257
+int fb_string_length(int dev, void* stream, int64_t n, const int64_t* offsets, const uint8_t* data,
+                     const uint8_t* valid, int64_t* out);
+int fb_string_like(int dev, void* stream, int64_t n, const int64_t* offsets, const uint8_t* data,
+                   const uint8_t* valid, int ntokens, const int16_t* tokens, uint8_t* out, uint8_t* out_valid);
 
 #ifdef __cplusplus
 }

@@ -7,8 +7,11 @@
 // Design (HBM-bound byte movement; no tensor-core work exists on this path):
 //   * the row range is cut into contiguous chunks of whole TILE-row tiles (at most
 //     2 x #SM of them) plus one tail chunk holding the final partial tile;
-//   * pass 1 (fb_hist_kernel)   : per-chunk histogram of partition ids (reads the
-//     key column(s) only: 8 B/row for the benchmark schema);
+//   * pass 1 (fb_rank_tile_kernel for num <= 256, fb_hist_kernel otherwise and for the
+//     tail chunk): per-chunk histogram of partition ids (reads the key column(s) only:
+//     8 B/row for the benchmark schema); for num <= 256 also one rank record per whole
+//     tile (partition id and stable rank of every row, rows per partition), each tile
+//     ranked by one warp;
 //   * scan  (fb_scan_*_kernel)  : exclusive prefix per partition over chunks, then
 //     over partitions -> part_offsets[num+1] and chunk bases;
 //   * pass 2, fast path (fb_scatter_tma_kernel; single 8-byte key, 8-byte columns):
@@ -110,15 +113,17 @@ __global__ void fb_row_hash_kernel(FbKeys keys, int64_t nrows, uint64_t* __restr
 // Warp-level "which lanes hold my value": kBits ballots instead of the hardware
 // MATCH instruction (MATCH.ANY is a slow multi-cycle warp instruction that caps the
 // whole kernel; ballots issue at full rate).  `m` starts as the mask of lanes
-// that take part.
+// that take part.  Bit b is moved to the sign bit so that the ballot's predicate
+// and the all-ones / all-zeros select come from one shift each: 5 SASS
+// instructions per bit, against 7 for `m &= bit ? bal : ~bal`.
 // ---------------------------------------------------------------------------
 template <int kBits>
 __device__ __forceinline__ unsigned match_lanes(uint32_t v, unsigned m) {
 #pragma unroll
   for (int b = 0; b < kBits; ++b) {
-    const bool bit = (v >> b) & 1u;
-    const unsigned bal = __ballot_sync(0xFFFFFFFFu, bit);
-    m &= bit ? bal : ~bal;
+    const int s = (int)(v << (31 - b)) >> 31;  // all ones if bit b of v is set, else 0
+    const unsigned bal = __ballot_sync(0xFFFFFFFFu, s < 0);
+    m &= ~(bal ^ (unsigned)s);
   }
   return m;
 }
@@ -173,118 +178,103 @@ fb_hist_kernel(FbKeys keys, FbDiv dv, uint32_t num, ChunkGeom g, int chunk0, uin
 //   [0, 4096)       uint8  partition id of every row
 //   [4096, 12288)   uint16 rank of the row among the rows of the same partition in this tile
 //   [12288, 12800)  uint16 rows per partition in this tile (256 entries)
-// Pass 2 loads one record per tile with a single TMA bulk copy.  This kernel runs at full occupancy
-// (2 x 1024 threads per SM); the same work done by the 8 ranker warps of the pass-2 CTA was the
-// bottleneck of 4-column launches.
+// Pass 2 loads one record per tile with a single TMA bulk copy.
+//
+// One warp ranks one whole tile: it walks the rows in order, 32 per round (row t0 + 32 i + lane), and
+// keeps 256 uint16 counters of its own in shared memory.  Per round the lanes of one partition find each
+// other with ballots, the lowest of them bumps the counter, and every lane's rank is the counter before
+// the bump plus the lanes of its partition below it.  The running counter is the exclusive prefix over
+// the earlier rows of the tile, so no block-wide prefix and no barrier is needed inside a tile.  The
+// tiles of chunk c are dealt to the warps of CTA c; one barrier at the end sums the warps' histograms.
 // ---------------------------------------------------------------------------
-constexpr int kRankBlock = 1024, kRankWarps = kRankBlock / 32, kRankItems = kTile / kRankBlock;
+constexpr int kRankBlock = 512, kRankWarps = kRankBlock / 32;
+constexpr int kRankRounds = kTile / 32;  // rounds of 32 rows per tile
+constexpr int kRankBatch = 8;            // rounds whose keys are loaded together, one batch ahead
 constexpr uint32_t kMetaRank = kTile, kMetaCnt = 3 * kTile, kMetaBytes = 3 * kTile + 512;
-static_assert(kRankItems * kRankBlock == kTile, "tile must be a multiple of the rank block");
+static_assert(kRankRounds % kRankBatch == 0, "a tile is a whole number of key batches");
 
-// kStaged (one 8-byte key without validity: hashed, or a radix digit): the keys of tile t+1 are copied
-// into shared memory (cp.async, one ring slot per row, each thread reads back only what it copied) while
-// tile t is ranked, so the key loads of the next tile overlap the barriers and the prefix of this one.
-// Dynamic shared memory: 2 x kTile uint64.
-constexpr size_t kRankStageBytes = 2 * (size_t)kTile * 8;
-
-__device__ __forceinline__ void cp_async8(void* dst_smem, const void* src) {
-  asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"((uint32_t)__cvta_generic_to_shared(dst_smem)),
-               "l"(src) : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-__device__ __forceinline__ void cp_async_wait_one() { asm volatile("cp.async.wait_group 1;" ::: "memory"); }
-
-// compute_pid of a row whose 8-byte key is `v`
+// compute_pid of a row whose 8-byte key is `v` (kStaged shapes: one 8-byte key without validity)
 template <bool kSingleU64>
 __device__ __forceinline__ uint32_t pid_of_key(const FbKeys& keys, const FbDiv& dv, uint64_t v) {
   if (kSingleU64) return fb_fastmod(fb_hash_single_u64(v), dv);
   return (uint32_t)(v >> keys.digit_shift) & (dv.d - 1);
 }
 
+// kStaged (one 8-byte key without validity: hashed, or a radix digit): the keys of the next batch of
+// rounds, in this tile or the warp's next one, are loaded into registers while this batch is ranked.
+// Other key shapes load in the loop (the loads of a batch are still issued together).
 template <bool kSingleU64, int kBits, bool kStaged>
 __global__ void __launch_bounds__(kRankBlock, 2)
-fb_rank_kernel(FbKeys keys, FbDiv dv, uint32_t num, ChunkGeom g, uint32_t* __restrict__ hist,
-               uint8_t* __restrict__ meta) {
-  __shared__ uint16_t s_cnt[kRankWarps * 256];
-  extern __shared__ __align__(16) unsigned long long s_keys[];  // kStaged: [2][kTile]
-  for (uint32_t i = threadIdx.x; i < (uint32_t)kRankWarps * 256; i += kRankBlock) s_cnt[i] = 0;
-  __syncthreads();
-  int64_t row0, row1;
-  chunk_range(g, (int)blockIdx.x, row0, row1);  // launched over the full chunks only
+fb_rank_tile_kernel(FbKeys keys, FbDiv dv, uint32_t num, ChunkGeom g, uint32_t* __restrict__ hist,
+                    uint8_t* __restrict__ meta) {
+  __shared__ __align__(16) uint16_t s_cnt[kRankWarps * 256];
+  __shared__ uint32_t s_hist[256];
   const unsigned lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const unsigned lt = fb_lanemask_lt();
   uint16_t* __restrict__ my = s_cnt + warp * 256;
-  uint32_t acc = 0;  // thread b < num: rows of partition b in this chunk
-  const unsigned long long* __restrict__ kp = (const unsigned long long*)keys.ptr[0];
-  const uint32_t my_row0 = warp * (32 * kRankItems) + lane;  // rows my_row0 + r * 32 of every tile
+  ((uint4*)my)[lane] = make_uint4(0, 0, 0, 0);
+  if (threadIdx.x < 256) s_hist[threadIdx.x] = 0;
+  __syncthreads();
+  int64_t row0, row1;
+  chunk_range(g, (int)blockIdx.x, row0, row1);  // launched over the full chunks only
+  constexpr int64_t kStride = (int64_t)kRankWarps * kTile;
+  uint32_t acc[8] = {0, 0, 0, 0, 0, 0, 0, 0};  // rows of partitions 8 lane .. 8 lane + 7 in this warp's tiles
+  const unsigned long long* __restrict__ kp = (const unsigned long long*)keys.ptr[0] + lane;
+  uint64_t kv[kRankBatch];
   if constexpr (kStaged) {
+    if (row0 + (int64_t)warp * kTile < row1) {
 #pragma unroll
-    for (int r = 0; r < kRankItems; ++r) cp_async8(s_keys + my_row0 + r * 32, kp + row0 + my_row0 + r * 32);
-    cp_async_commit();
+      for (int b = 0; b < kRankBatch; ++b) kv[b] = __ldg(kp + row0 + (int64_t)warp * kTile + b * 32);
+    }
   }
-  uint32_t stage = 0;
-  for (int64_t t0 = row0; t0 < row1; t0 += kTile) {
+  for (int64_t t0 = row0 + (int64_t)warp * kTile; t0 < row1; t0 += kStride) {
     uint8_t* __restrict__ rec = meta + (size_t)(t0 / kTile) * kMetaBytes;
-    uint32_t pid[kRankItems], pos[kRankItems];
-    if constexpr (kStaged) {
-      // the other slot was read back during the previous tile: refill it with the next tile's keys
-      if (t0 + kTile < row1) {
-        unsigned long long* nxt = s_keys + (stage ^ 1) * kTile;
+    uint8_t* __restrict__ rec_id = rec + lane;
+    uint16_t* __restrict__ rec_rank = (uint16_t*)(rec + kMetaRank) + lane;
+    for (int r0 = 0; r0 < kRankRounds; r0 += kRankBatch) {
+      uint32_t pid[kRankBatch];
+      if constexpr (kStaged) {
 #pragma unroll
-        for (int r = 0; r < kRankItems; ++r) cp_async8(nxt + my_row0 + r * 32, kp + t0 + kTile + my_row0 + r * 32);
+        for (int b = 0; b < kRankBatch; ++b) pid[b] = pid_of_key<kSingleU64>(keys, dv, kv[b]);
+        // next batch: the rest of this tile, then the first rows of this warp's next tile
+        const int64_t nxt = r0 + kRankBatch < kRankRounds ? t0 + (r0 + kRankBatch) * 32 : t0 + kStride;
+        if (nxt < row1) {
+#pragma unroll
+          for (int b = 0; b < kRankBatch; ++b) kv[b] = __ldg(kp + nxt + b * 32);
+        }
+      } else {
+#pragma unroll
+        for (int b = 0; b < kRankBatch; ++b)
+          pid[b] = compute_pid<kSingleU64>(keys, dv, t0 + (r0 + b) * 32 + (int64_t)lane);
       }
-      cp_async_commit();  // possibly empty: the group of this tile is then always the one before the last
-      cp_async_wait_one();
-      const unsigned long long* cur = s_keys + stage * kTile;
 #pragma unroll
-      for (int r = 0; r < kRankItems; ++r) pid[r] = pid_of_key<kSingleU64>(keys, dv, cur[my_row0 + r * 32]);
-      stage ^= 1;
-    } else {
-#pragma unroll
-      for (int r = 0; r < kRankItems; ++r) pid[r] = compute_pid<kSingleU64>(keys, dv, t0 + my_row0 + r * 32);
-    }
-    unsigned mm[kRankItems];
-#pragma unroll
-    for (int r = 0; r < kRankItems; ++r) mm[r] = match_lanes<kBits>(pid[r], 0xFFFFFFFFu);
-#pragma unroll
-    for (int r = 0; r < kRankItems; ++r) {
-      const unsigned m = mm[r];
-      const unsigned before = __popc(m & lt);
-      uint32_t old = 0;
-      if (before == 0) {
-        old = my[pid[r]];
-        my[pid[r]] = (uint16_t)(old + __popc(m));
+      for (int b = 0; b < kRankBatch; ++b) {
+        const uint32_t p = pid[b];
+        const unsigned m = match_lanes<kBits>(p, 0xFFFFFFFFu);
+        const unsigned before = __popc(m & lt);
+        const uint32_t old = my[p];
+        __syncwarp();  // every lane has read the counter before the lowest lane of its partition bumps it
+        if (before == 0) my[p] = (uint16_t)(old + __popc(m));
+        __syncwarp();  // the next round reads the bumped counters
+        rec_id[(r0 + b) * 32] = (uint8_t)p;
+        rec_rank[(r0 + b) * 32] = (uint16_t)(old + before);
       }
-      __syncwarp();
-      old = __shfl_sync(0xFFFFFFFFu, old, __ffs(m) - 1);
-      pos[r] = old + before;
     }
-    __syncthreads();
-    if (threadIdx.x < 256) {  // exclusive prefix over the warps, per partition
-      const uint32_t b = threadIdx.x;
-      uint32_t n = 0;
-#pragma unroll
-      for (int w = 0; w < kRankWarps; ++w) {
-        const uint32_t t = s_cnt[w * 256 + b];
-        s_cnt[w * 256 + b] = (uint16_t)n;
-        n += t;
-      }
-      acc += n;
-      ((uint16_t*)(rec + kMetaCnt))[b] = (uint16_t)n;
-    }
-    __syncthreads();
-#pragma unroll
-    for (int r = 0; r < kRankItems; ++r) {
-      const uint32_t idx = warp * (32 * kRankItems) + r * 32 + lane;
-      rec[idx] = (uint8_t)pid[r];
-      ((uint16_t*)(rec + kMetaRank))[idx] = (uint16_t)(pos[r] + my[pid[r]]);
-    }
-    __syncwarp();
-#pragma unroll
-    for (int i = 0; i < 4; ++i) ((uint32_t*)my)[i * 32 + lane] = 0;
+    // the counters are the tile's rows per partition: the record's count[256]; then reset them
+    const uint4 c = ((const uint4*)my)[lane];
+    ((uint4*)(rec + kMetaCnt))[lane] = c;
+    acc[0] += c.x & 0xFFFFu; acc[1] += c.x >> 16;
+    acc[2] += c.y & 0xFFFFu; acc[3] += c.y >> 16;
+    acc[4] += c.z & 0xFFFFu; acc[5] += c.z >> 16;
+    acc[6] += c.w & 0xFFFFu; acc[7] += c.w >> 16;
+    ((uint4*)my)[lane] = make_uint4(0, 0, 0, 0);
     __syncwarp();
   }
-  if (threadIdx.x < num) hist[(size_t)blockIdx.x * num + threadIdx.x] = acc;
+#pragma unroll
+  for (int i = 0; i < 8; ++i)
+    if (acc[i] != 0) atomicAdd(&s_hist[lane * 8 + i], acc[i]);
+  __syncthreads();
+  if (threadIdx.x < num) hist[(size_t)blockIdx.x * num + threadIdx.x] = s_hist[threadIdx.x];
 }
 
 // ---------------------------------------------------------------------------
@@ -1160,10 +1150,6 @@ cudaError_t ensure_smem_optin(int dev) {
     FB_OPTIN_WS(kWsGWide);
 #undef FB_OPTIN_WS
   }
-  if (e == cudaSuccess) e = optin(fb_rank_kernel<true, 4, true>, kRankStageBytes);
-  if (e == cudaSuccess) e = optin(fb_rank_kernel<true, 8, true>, kRankStageBytes);
-  if (e == cudaSuccess) e = optin(fb_rank_kernel<false, 4, true>, kRankStageBytes);
-  if (e == cudaSuccess) e = optin(fb_rank_kernel<false, 8, true>, kRankStageBytes);
   FB_OPTIN(true, 4); FB_OPTIN(true, 8); FB_OPTIN(true, 10);
   FB_OPTIN(false, 4); FB_OPTIN(false, 8); FB_OPTIN(false, 10);
 #undef FB_OPTIN
@@ -1280,14 +1266,13 @@ static int plan_impl(int dev, void* stream, int64_t nrows, const FbKeys& k, bool
   size_t smem = (size_t)kHistWarps * num_partitions * sizeof(uint32_t);
   FB_CUDA(ensure_smem_optin(dev));
   const int bits = bits_for(num_partitions);
-  // num <= 256: full tiles are ranked completely (fb_rank_kernel); the tail chunk and larger
+  // num <= 256: full tiles are ranked completely (fb_rank_tile_kernel); the tail chunk and larger
   // partition counts only need the histogram
   int hist_chunk0 = 0;
   if (num_partitions <= kSwcMaxNum && g.nchunks_full > 0) {
     uint8_t* meta = (uint8_t*)scratch + l.pid_offset;
-#define FB_LAUNCH_RANK(S, B, STAGED)                                                                  \
-  fb_rank_kernel<S, B, STAGED><<<g.nchunks_full, kRankBlock, STAGED ? kRankStageBytes : 0, st>>>( \
-      k, dv, num_partitions, g, hist, meta)
+#define FB_LAUNCH_RANK(S, B, STAGED) \
+  fb_rank_tile_kernel<S, B, STAGED><<<g.nchunks_full, kRankBlock, 0, st>>>(k, dv, num_partitions, g, hist, meta)
     if (single) {
       if (bits == 4) FB_LAUNCH_RANK(true, 4, true);
       else FB_LAUNCH_RANK(true, 8, true);

@@ -5,8 +5,10 @@ from an expression is a function of ``(kind, head, args)``:
 
     NAMED     head = column name                     WILDCARD  ``*``
     LITERAL   head = python value (None = NULL)      UNARY     head in ``- ~ IS_NULL NOT_NULL``, one arg
-    BINARY    head in ``+ - * / & | < > <= >= == !=``  CALL      head = function name (``COALESCE`` ...)
+    BINARY    head in ``+ - * / % & | < > <= >= == !=``  CALL    head = function name (``COALESCE`` ...)
               ``LIKE``: args (string, pattern literal[, escape literal]); ``LENGTH``: args (string,)
+              ``CASE``: args (cond1, value1, ..., condN, valueN, else), the ELSE always stored (NULL if absent);
+              ``NULLIF ABS FLOOR CEIL SQRT EXP LN LOG10 POWER GREATEST LEAST``; ``ROUND``: args (x, digits literal)
     AGG       head in ``SUM COUNT AVG MIN MAX FIRST LAST``, one arg, optional DISTINCT, or ``PERCENTILE_CONT
               PERCENTILE_DISC``, one arg and kwarg ``q`` (MEDIAN is PERCENTILE_CONT at q = 0.5)
     WINDOW    head in the AGG functions (one arg, kwargs ``running``, ``rows`` or ``range``; a percentile keeps
@@ -48,13 +50,15 @@ class Kind(enum.IntEnum):
 
 
 BOOL_OPS = frozenset(["&", "|", "<", ">", "<=", ">=", "==", "!="])
-ARITH_OPS = frozenset(["+", "-", "*", "/"])
+ARITH_OPS = frozenset(["+", "-", "*", "/", "%"])
 AGG_KEEPS_ARG_TYPE = frozenset(["MIN", "MAX", "FIRST", "LAST"])
 WINDOW_AGGS = frozenset(["SUM", "COUNT", "AVG", "MIN", "MAX", "FIRST", "LAST"])
 PERCENTILES = frozenset(["PERCENTILE_CONT", "PERCENTILE_DISC"])
 _RANKINGS = frozenset(["ROW_NUMBER", "RANK", "DENSE_RANK"])
 _RUNNING_FRAME = "ROWS BETWEEN UNBOUNDED PRECEDING AND CURRENT ROW"
 _LITERAL_TYPES = (int, bool, float, str)
+FLOAT_FUNCTIONS = frozenset(["SQRT", "EXP", "LN", "LOG10", "POWER", "POW"])  # always float64
+ROUND_MAX_DIGITS = 18
 
 
 def to_pa_datatype(obj: Any) -> pa.DataType:
@@ -205,6 +209,10 @@ class ColumnExpr:
             return self.args[0].infer_type(schema)
         if k == Kind.CALL and self.head in ("LIKE", "LENGTH"):
             return pa.bool_() if self.head == "LIKE" else pa.int64()
+        if k == Kind.CALL and self.head.upper() in FLOAT_FUNCTIONS:
+            return pa.float64()
+        if k == Kind.CALL and case_string_results(self) is not None:
+            return pa.string()
         if k in (Kind.AGG, Kind.WINDOW) and self.head in PERCENTILES:
             return pa.float64() if self.head == "PERCENTILE_CONT" else self.args[0].infer_type(schema)
         if k == Kind.WINDOW:
@@ -351,7 +359,8 @@ def _binary_method(op: str, swap: bool) -> Any:
     return method
 
 
-for _name, _op in (("add", "+"), ("sub", "-"), ("mul", "*"), ("truediv", "/"), ("and", "&"), ("or", "|")):
+for _name, _op in (("add", "+"), ("sub", "-"), ("mul", "*"), ("truediv", "/"), ("mod", "%"), ("and", "&"),
+                   ("or", "|")):
     setattr(ColumnExpr, f"__{_name}__", _binary_method(_op, False))
     setattr(ColumnExpr, f"__r{_name}__", _binary_method(_op, True))
 for _name, _op in (("lt", "<"), ("gt", ">"), ("le", "<="), ("ge", ">="), ("eq", "=="), ("ne", "!=")):
@@ -513,6 +522,38 @@ def _offset_fn(name: str, c: Any, n: Any, default: Any) -> ColumnExpr:
     return ColumnExpr(Kind.WINDOW, name, [arg], {"n": n, "default": default})
 
 
+def _result_args(e: ColumnExpr) -> List[Any]:
+    """The operands of a CASE / IF / IIF / NULLIF that can become its value."""
+    head = e.head.upper()
+    if head == "CASE":
+        return list(e.args[1::2]) + [e.args[-1]] if e.args else []
+    if head in ("IF", "IIF"):
+        return list(e.args[1:3])
+    return list(e.args[:1]) if head == "NULLIF" else []
+
+
+def case_string_results(e: Any) -> Optional[List[str]]:
+    """The distinct string literals (in order of appearance) of a CASE / IF / IIF / NULLIF whose every result is a
+    string literal or NULL, with at least one string; None for any other node."""
+    if not (isinstance(e, ColumnExpr) and e.kind == Kind.CALL and e.head.upper() in ("CASE", "IF", "IIF", "NULLIF")):
+        return None
+    out: List[str] = []
+    for r in _result_args(e):
+        r = _operand(r)
+        if r.kind != Kind.LITERAL or r.as_type is not None or not (r.value is None or isinstance(r.value, str)):
+            return None
+        if r.value is not None and r.value not in out:
+            out.append(r.value)
+    return out if out else None
+
+
+def _check_results(e: ColumnExpr) -> ColumnExpr:
+    lits = [r for r in _result_args(e) if r.kind == Kind.LITERAL and r.value is not None]
+    if any(isinstance(r.value, str) for r in lits) and not all(isinstance(r.value, str) for r in lits):
+        raise ValueError(f"{e.head} mixes string and numeric results: {e}")
+    return e
+
+
 def column_mentions(column: Any) -> Iterator[str]:
     """Names of the columns an expression reads."""
     if isinstance(column, ColumnExpr):
@@ -530,6 +571,83 @@ class functions:
     @staticmethod
     def coalesce(*args: Any) -> ColumnExpr:
         return function("COALESCE", *[_operand(x) for x in args])
+
+    @staticmethod
+    def case(branches: Sequence[Tuple[Any, Any]], else_: Any = None) -> ColumnExpr:
+        """SQL ``CASE WHEN cond THEN value ... ELSE else_ END``: the value of the first branch whose condition is
+        TRUE (NULL and FALSE fall through), else ``else_`` (NULL if not given).  The result is float64 if any branch
+        is a float, bool if all are bool or NULL, else int64; string literals (and NULL) give a string column."""
+        branches = list(branches)
+        if not branches:
+            raise ValueError("CASE needs at least one WHEN branch")
+        args: List[ColumnExpr] = []
+        for b in branches:
+            if not isinstance(b, tuple) or len(b) != 2:
+                raise ValueError(f"a CASE branch is a (condition, value) pair, got {b!r}")
+            args += [_operand(b[0]), _operand(b[1])]
+        return _check_results(ColumnExpr(Kind.CALL, "CASE", args + [_operand(else_)]))
+
+    @staticmethod
+    def nullif(a: Any, b: Any) -> ColumnExpr:
+        """SQL ``NULLIF(a, b)``: NULL where ``a = b`` is TRUE, else ``a``."""
+        return ColumnExpr(Kind.CALL, "NULLIF", [_operand(a), _operand(b)])
+
+    @staticmethod
+    def abs(c: Any) -> ColumnExpr:  # noqa: A003
+        """``|c|``; an integer wraps at INT64_MIN as unary ``-`` does."""
+        return ColumnExpr(Kind.CALL, "ABS", [_operand(c)])
+
+    @staticmethod
+    def floor(c: Any) -> ColumnExpr:
+        return ColumnExpr(Kind.CALL, "FLOOR", [_operand(c)])
+
+    @staticmethod
+    def ceil(c: Any) -> ColumnExpr:
+        return ColumnExpr(Kind.CALL, "CEIL", [_operand(c)])
+
+    @staticmethod
+    def round(c: Any, d: Any = 0) -> ColumnExpr:  # noqa: A003
+        """SQL ``ROUND(c, d)``: to ``d`` decimal digits (an int literal in [-18, 18]), half away from zero."""
+        if isinstance(d, ColumnExpr) and d.kind == Kind.LITERAL and d.as_type is None:
+            d = d.value
+        if isinstance(d, bool) or not isinstance(d, int) or not -ROUND_MAX_DIGITS <= d <= ROUND_MAX_DIGITS:
+            raise ValueError(f"ROUND takes an integer literal in [-{ROUND_MAX_DIGITS}, {ROUND_MAX_DIGITS}] as its "
+                             f"digits, got {d!r}")
+        return ColumnExpr(Kind.CALL, "ROUND", [_operand(c), lit(d)])
+
+    @staticmethod
+    def sqrt(c: Any) -> ColumnExpr:
+        return ColumnExpr(Kind.CALL, "SQRT", [_operand(c)])
+
+    @staticmethod
+    def exp(c: Any) -> ColumnExpr:
+        return ColumnExpr(Kind.CALL, "EXP", [_operand(c)])
+
+    @staticmethod
+    def ln(c: Any) -> ColumnExpr:
+        return ColumnExpr(Kind.CALL, "LN", [_operand(c)])
+
+    @staticmethod
+    def log10(c: Any) -> ColumnExpr:
+        return ColumnExpr(Kind.CALL, "LOG10", [_operand(c)])
+
+    @staticmethod
+    def power(a: Any, b: Any) -> ColumnExpr:
+        return ColumnExpr(Kind.CALL, "POWER", [_operand(a), _operand(b)])
+
+    @staticmethod
+    def greatest(*args: Any) -> ColumnExpr:
+        """The largest non-NULL argument (NULL only if all are NULL); floats in the order of aggregate MAX."""
+        if len(args) < 2:
+            raise ValueError("GREATEST needs at least two arguments")
+        return ColumnExpr(Kind.CALL, "GREATEST", [_operand(x) for x in args])
+
+    @staticmethod
+    def least(*args: Any) -> ColumnExpr:
+        """The smallest non-NULL argument (NULL only if all are NULL); floats in the order of aggregate MIN."""
+        if len(args) < 2:
+            raise ValueError("LEAST needs at least two arguments")
+        return ColumnExpr(Kind.CALL, "LEAST", [_operand(x) for x in args])
 
     @staticmethod
     def length(c: Any) -> ColumnExpr:
@@ -722,6 +840,10 @@ def to_sql(expr: ColumnExpr, enable_cast: bool = True, nested: bool = False) -> 
             body += " ESCAPE " + to_sql(expr.args[2], enable_cast)
         if nested:
             body = "(" + body + ")"
+    elif k == Kind.CALL and expr.head.upper() == "CASE" and len(expr.args) % 2 == 1:
+        a = expr.args
+        body = "CASE" + "".join(f" WHEN {to_sql(_operand(a[i]), enable_cast)} THEN {to_sql(_operand(a[i + 1]), enable_cast)}"
+                                for i in range(0, len(a) - 1, 2)) + f" ELSE {to_sql(_operand(a[-1]), enable_cast)} END"
     elif k == Kind.BINARY:
         if expr.head not in BOOL_OPS and expr.head not in ARITH_OPS:
             raise NotImplementedError(expr)

@@ -16,7 +16,10 @@
 //     so the switch is amortised; every output is written by its own FB_X_OUT instruction;
 //   * SQL NULL semantics: arithmetic and comparisons propagate NULL (validity bits are ANDed for
 //     all rows of the thread at once), AND / OR are Kleene three-valued, IS NULL / IS NOT NULL /
-//     COALESCE read the validity bits.
+//     COALESCE read the validity bits;
+//   * CASE runs without branching: every branch is computed for every row and FB_X_SEL keeps, per row,
+//     the value of the first branch whose condition is TRUE.  No op traps (x % 0 is NULL, not a fault),
+//     so computing a branch a row does not take is harmless.
 #include <mutex>
 
 #include <cuda_fp16.h>
@@ -112,6 +115,60 @@ __device__ __forceinline__ void lookup(const uint64_t* __restrict__ q, const uin
   accv = nv;
 }
 
+// ---- scalar functions (one row).  An integer is int64 and wraps; a float is float64.
+__device__ __forceinline__ bool mod_i(const uint64_t x, const uint64_t y, uint64_t& r) {  // false: NULL (y = 0)
+  const int64_t a = (int64_t)x, b = (int64_t)y;
+  r = (b == -1 || b == 0) ? 0 : (uint64_t)(a % b);  // INT64_MIN % -1 would trap: every x % -1 is 0
+  return b != 0;
+}
+
+// fmod is exact.  y = +-0.0 is NULL even for a NaN x; fmod(+-inf, y) is a domain error (NaN from non-NaN)
+__device__ __noinline__ double fn_fmod(double x, double y) { return fmod(x, y); }
+
+__device__ __forceinline__ bool mod_f(const uint64_t xb, const uint64_t yb, uint64_t& rb) {
+  const double x = as_f(xb), y = as_f(yb), r = fn_fmod(x, y);
+  rb = f_bits(r);
+  return y != 0.0 && !(isnan(r) && !isnan(x) && !isnan(y));
+}
+
+__device__ __forceinline__ double pow10_f(int e) {  // 10^e for e in [0, 18]: every one is exact in a double
+  double p = 1.0;
+  for (int i = 0; i < e; ++i) p *= 10.0;  // each product is an integer below 2^63 with at most 53 significant bits
+  return p;
+}
+
+// ROUND(x, d): d = 0 is C round; else DuckDB's round(x * 10^d) / 10^d, and x itself when the scaled value is not finite
+__device__ __forceinline__ double round_f(double x, int d) {
+  if (d == 0) return round(x);
+  const double p = pow10_f(d < 0 ? -d : d);
+  const double s = d > 0 ? x * p : x / p;
+  if (!isfinite(s)) return x;
+  return d > 0 ? round(s) / p : round(s) * p;
+}
+
+// ROUND(x, d) of an int64, d < 0: the nearest multiple of 10^-d, half away from zero; wraps like + - *
+__device__ __forceinline__ uint64_t round_i(uint64_t x, int d) {
+  int64_t p = 1;
+  for (int i = 0; i < -d; ++i) p *= 10;
+  const int64_t a = (int64_t)x, r = a % p;
+  uint64_t q = x - (uint64_t)r;
+  const uint64_t ar = (uint64_t)(r < 0 ? -r : r);
+  if (2 * ar >= (uint64_t)p) q += a < 0 ? (uint64_t)(-p) : (uint64_t)p;
+  return q;
+}
+
+// IEEE totalOrder as a signed key: -NaN < -inf < ... < -0.0 < +0.0 < ... < +inf < +NaN (aggregate MIN / MAX)
+__device__ __forceinline__ int64_t total_key(uint64_t b) {
+  const int64_t s = (int64_t)b;
+  return s >= 0 ? s : s ^ 0x7FFFFFFFFFFFFFFFll;
+}
+
+// the transcendental functions run out of line, once per row: inlined into the 8-row unrolled loop they cost registers
+__device__ __noinline__ double fn_exp(double x) { return exp(x); }
+__device__ __noinline__ double fn_ln(double x) { return log(x); }
+__device__ __noinline__ double fn_log10(double x) { return log10(x); }
+__device__ __noinline__ double fn_pow(double x, double y) { return pow(x, y); }
+
 // one tile of kExprTile rows (kFull: no bounds checks; only the last tile of a table is partial)
 template <bool kFull>
 __device__ __forceinline__ void run_tile(const ExprProgram& P, int64_t row0, int nk, int tid, uint64_t* tmp_v,
@@ -172,6 +229,12 @@ __device__ __forceinline__ void run_tile(const ExprProgram& P, int64_t row0, int
 #define FB_ROWS(...) _Pragma("unroll") for (int k = 0; k < kExprItems; ++k) { __VA_ARGS__ }
 #define FB_BIN(EXPR) FB_ROWS(const uint64_t x = acc[k], y = b[k]; acc[k] = (EXPR);) accv &= bv;
 #define FB_UN(EXPR) FB_ROWS(const uint64_t x = acc[k]; acc[k] = (EXPR);)
+// CHK: a binary op whose call is false where the row becomes NULL; FUN / FBIN: float functions under the domain rule
+#define FB_CHK(CALL) { unsigned ok = 0; FB_ROWS(if (CALL) ok |= 1u << k;) accv &= bv & ok; }
+#define FB_FUN(EXPR) { unsigned bad = 0; FB_ROWS(const double x = as_f(acc[k]); const double r = (EXPR); \
+                       acc[k] = f_bits(r); if (isnan(r) && !isnan(x)) bad |= 1u << k;) accv &= ~bad; }
+#define FB_FBIN(EXPR) { unsigned bad = 0; FB_ROWS(const double x = as_f(acc[k]), y = as_f(b[k]); const double r = (EXPR); \
+                        acc[k] = f_bits(r); if (isnan(r) && !isnan(x) && !isnan(y)) bad |= 1u << k;) accv &= bv & ~bad; }
       switch (in.op) {
         case FB_X_MOV: FB_ROWS(acc[k] = b[k];) accv = bv; break;
         case FB_X_ST: {
@@ -254,8 +317,52 @@ __device__ __forceinline__ void run_tile(const ExprProgram& P, int64_t row0, int
         case FB_X_LOOKUP:
           lookup((const uint64_t*)P.col_ptr[in.b], P.col_valid[in.b], (uint64_t)in.imm, acc, accv);
           break;
+        case FB_X_SEL: {  // acc <- temp[flags >> FB_XF_COND_SHIFT] is TRUE ? acc : B
+          const int cr = in.flags >> FB_XF_COND_SHIFT;
+          const uint64_t* c = tmp_v + (size_t)cr * kExprTile;
+          const unsigned cm = tmp_m[cr * kExprThreads + tid];
+          unsigned t = 0;
+          FB_ROWS(if (((cm >> k) & 1u) && c[k * kExprThreads + tid] != 0) t |= 1u << k; else acc[k] = b[k];)
+          accv = (accv & t) | (bv & ~t);
+          break;
+        }
+        case FB_X_MOD_I: FB_CHK(mod_i(acc[k], b[k], acc[k])) break;
+        case FB_X_RMOD_I: FB_CHK(mod_i(b[k], acc[k], acc[k])) break;
+        case FB_X_MOD_F: FB_CHK(mod_f(acc[k], b[k], acc[k])) break;
+        case FB_X_RMOD_F: FB_CHK(mod_f(b[k], acc[k], acc[k])) break;
+        case FB_X_ABS_I: FB_UN((int64_t)x < 0 ? 0 - x : x) break;
+        case FB_X_ABS_F: FB_UN(x & 0x7FFFFFFFFFFFFFFFull) break;
+        case FB_X_FLOOR_F: FB_UN(f_bits(floor(as_f(x)))) break;
+        case FB_X_CEIL_F: FB_UN(f_bits(ceil(as_f(x)))) break;
+        case FB_X_ROUND_F: FB_UN(f_bits(round_f(as_f(x), (int)in.imm))) break;
+        case FB_X_ROUND_I: FB_UN(round_i(x, (int)in.imm)) break;
+        case FB_X_SQRT: FB_FUN(sqrt(x)) break;
+        case FB_X_EXP: FB_FUN(fn_exp(x)) break;
+        case FB_X_LN: FB_FUN(fn_ln(x)) break;
+        case FB_X_LOG10: FB_FUN(fn_log10(x)) break;
+        case FB_X_POW: FB_FBIN(fn_pow(x, y)) break;
+        case FB_X_RPOW: FB_FBIN(fn_pow(y, x)) break;
+        case FB_X_GREATEST_I:
+          FB_ROWS(if (((bv >> k) & 1u) && (!((accv >> k) & 1u) || (int64_t)b[k] > (int64_t)acc[k])) acc[k] = b[k];)
+          accv |= bv;
+          break;
+        case FB_X_LEAST_I:
+          FB_ROWS(if (((bv >> k) & 1u) && (!((accv >> k) & 1u) || (int64_t)b[k] < (int64_t)acc[k])) acc[k] = b[k];)
+          accv |= bv;
+          break;
+        case FB_X_GREATEST_F:
+          FB_ROWS(if (((bv >> k) & 1u) && (!((accv >> k) & 1u) || total_key(b[k]) > total_key(acc[k]))) acc[k] = b[k];)
+          accv |= bv;
+          break;
+        case FB_X_LEAST_F:
+          FB_ROWS(if (((bv >> k) & 1u) && (!((accv >> k) & 1u) || total_key(b[k]) < total_key(acc[k]))) acc[k] = b[k];)
+          accv |= bv;
+          break;
         default: break;
       }
+#undef FB_FBIN
+#undef FB_FUN
+#undef FB_CHK
 #undef FB_BIN
 #undef FB_UN
 #undef FB_ROWS
@@ -308,7 +415,20 @@ extern "C" int fb_eval_expr(int dev, void* stream, int64_t nrows, int ncols, con
   }
   for (int i = 0; i < nins; ++i) {
     const fb_expr_ins& in = program[i];
-    FB_CHECK(in.op >= FB_X_MOV && in.op <= FB_X_LOOKUP, "instruction %d: unknown op %d", i, in.op);
+    FB_CHECK(in.op >= FB_X_MOV && in.op <= FB_X_LEAST_F, "instruction %d: unknown op %d", i, in.op);
+    const bool unary_fn = (in.op >= FB_X_ABS_I && in.op <= FB_X_LOG10);  // scalar functions of acc alone
+    if (unary_fn) FB_CHECK(in.kind == FB_XK_NONE, "instruction %d: op %d takes no operand", i, in.op);
+    if (in.op == FB_X_SEL)
+      FB_CHECK(in.flags >= 0 && (in.flags >> FB_XF_COND_SHIFT) < FB_EXPR_NREGS,
+               "instruction %d: FB_X_SEL condition temporary %d out of range", i, in.flags >> FB_XF_COND_SHIFT);
+    else if (in.op > FB_X_LOOKUP)
+      FB_CHECK((in.flags & ~FB_XF_B_I2F) == 0, "instruction %d: unknown flags %#x", i, in.flags);
+    if (in.op == FB_X_ROUND_F)
+      FB_CHECK(in.imm >= -FB_EXPR_ROUND_MAX_DIGITS && in.imm <= FB_EXPR_ROUND_MAX_DIGITS,
+               "instruction %d: FB_X_ROUND_F digits %lld out of range", i, (long long)in.imm);
+    if (in.op == FB_X_ROUND_I)
+      FB_CHECK(in.imm >= -FB_EXPR_ROUND_MAX_DIGITS && in.imm <= -1, "instruction %d: FB_X_ROUND_I digits %lld out of range",
+               i, (long long)in.imm);
     if (in.op == FB_X_LOOKUP) {
       FB_CHECK(in.kind == FB_XK_COL, "instruction %d: FB_X_LOOKUP reads a column operand", i);
       FB_CHECK(in.b >= 0 && in.b < ncols, "instruction %d: column %d out of range", i, in.b);
@@ -328,7 +448,7 @@ extern "C" int fb_eval_expr(int dev, void* stream, int64_t nrows, int ncols, con
     } else if (in.kind == FB_XK_COL) {
       FB_CHECK(in.b >= 0 && in.b < ncols, "instruction %d: column %d out of range", i, in.b);
     }
-    const bool binary = in.op == FB_X_MOV || in.op >= FB_X_ADD_I;
+    const bool binary = in.op == FB_X_MOV || (in.op >= FB_X_ADD_I && !unary_fn);
     FB_CHECK(!binary || in.kind != FB_XK_NONE, "instruction %d: op %d needs an operand", i, in.op);
     P.ins[i] = in;
   }

@@ -12,6 +12,10 @@ String columns are dictionary encoded: they can be passed through, tested for NU
 (``==`` / ``!=``) with a string literal; ``cast(str)`` of a numeric result builds a dictionary.
 ``LIKE`` and ``LENGTH`` of a string column are computed once per dictionary entry (``strings.py``) and
 read per row through the entry's code (``FB_X_LOOKUP``), inside the same program.
+``CASE`` runs without branching (every branch on every row, ``FB_X_SEL`` picks); its class, and that of
+``GREATEST`` / ``LEAST``, is COALESCE's rule.  ``%`` and ``ABS FLOOR CEIL ROUND`` keep the operand's class
+(int64 or float64), ``SQRT EXP LN LOG10 POWER`` are float64.  A CASE whose results are string literals is a
+whole output column only: ``project`` compiles it to int32 codes into a dictionary of those literals.
 """
 import struct
 from typing import Any, Dict, List, Optional, Sequence, Tuple
@@ -21,7 +25,7 @@ import torch
 
 from . import kernels as K
 from . import strings as ST
-from .column import ColumnExpr, Kind, lit as _lit
+from .column import FLOAT_FUNCTIONS, ROUND_MAX_DIGITS, ColumnExpr, Kind, case_string_results, lit as _lit
 from .schema import Schema
 from .table import B200Table, _storage_dtype, expr_type
 
@@ -48,19 +52,55 @@ class _OutOfResources(Exception):
     pass
 
 
+def _lower(e: ColumnExpr) -> Optional[ColumnExpr]:
+    """The canonical node of a function spelled another way (no alias, no cast), or None:
+    IF / IIF -> CASE, NULLIF(a, b) -> CASE WHEN a = b THEN NULL ELSE a END, IFNULL -> COALESCE, MOD -> %,
+    POW -> POWER, CEILING -> CEIL."""
+    if e.kind != Kind.CALL:
+        return None
+    fn = e.func.upper()
+    args = [a if isinstance(a, ColumnExpr) else _lit(a) for a in e.args]
+    if fn in ("IF", "IIF", "NULLIF", "MOD") and len(args) != (3 if fn in ("IF", "IIF") else 2):
+        raise ValueError(f"{fn} takes {3 if fn in ('IF', 'IIF') else 2} arguments: {e}")
+    if fn in ("IF", "IIF"):
+        return ColumnExpr(Kind.CALL, "CASE", args)
+    if fn == "NULLIF":
+        return ColumnExpr(Kind.CALL, "CASE", [ColumnExpr(Kind.BINARY, "==", args), _lit(None), args[0]])
+    if fn == "IFNULL":
+        return ColumnExpr(Kind.CALL, "COALESCE", args)
+    if fn == "MOD":
+        return ColumnExpr(Kind.BINARY, "%", args)
+    if fn in ("POW", "CEILING"):
+        return ColumnExpr(Kind.CALL, "POWER" if fn == "POW" else "CEIL", args)
+    if e.head != fn and fn in ("CASE", "COALESCE", "ABS", "FLOOR", "CEIL", "ROUND", "GREATEST", "LEAST") + \
+            tuple(FLOAT_FUNCTIONS):
+        return ColumnExpr(Kind.CALL, fn, args)  # function("abs", x) is ABS(x)
+    return None
+
+
+def _coalesce_cls(cs: Sequence[str]) -> str:
+    """COALESCE's result class: float64 if any is a float, bool if all are bool / NULL, else int64."""
+    return "f" if "f" in cs else ("b" if "b" in cs and all(c in ("b", "n") for c in cs) else "i")
+
+
 class _Program:
     """One ``fb_eval_expr`` launch.  Code generation for the accumulator machine: ``compile`` leaves the
     value of an expression in the accumulator; the right-hand side of an operator is used in place
     when it is a leaf (column / literal), otherwise the left value waits in a temporary."""
 
     _REVERSE = {"+": "+", "*": "*", "-": "r-", "/": "r/", "<": ">", "<=": ">=", ">": "<", ">=": "<=",
-                "==": "==", "!=": "!=", "&": "&", "|": "|"}
+                "==": "==", "!=": "!=", "&": "&", "|": "|", "%": "r%", "**": "r**"}
     _OPS = {  # (int opcode, float opcode)
         "+": (K.X_ADD_I, K.X_ADD_F), "-": (K.X_SUB_I, K.X_SUB_F), "r-": (K.X_RSUB_I, K.X_RSUB_F),
         "*": (K.X_MUL_I, K.X_MUL_F), "/": (None, K.X_DIV_F), "r/": (None, K.X_RDIV_F),
         "<": (K.X_LT_I, K.X_LT_F), "<=": (K.X_LE_I, K.X_LE_F), ">": (K.X_GT_I, K.X_GT_F),
         ">=": (K.X_GE_I, K.X_GE_F), "==": (K.X_EQ_I, K.X_EQ_F), "!=": (K.X_NE_I, K.X_NE_F),
+        "%": (K.X_MOD_I, K.X_MOD_F), "r%": (K.X_RMOD_I, K.X_RMOD_F),
+        "**": (None, K.X_POW), "r**": (None, K.X_RPOW),  # "**" is POWER(a, b), only inside the compiler
     }
+    _UNARY_FN = {"ABS": (K.X_ABS_I, K.X_ABS_F), "FLOOR": (None, K.X_FLOOR_F), "CEIL": (None, K.X_CEIL_F),
+                 "ROUND": (K.X_ROUND_I, K.X_ROUND_F), "SQRT": (None, K.X_SQRT), "EXP": (None, K.X_EXP),
+                 "LN": (None, K.X_LN), "LOG10": (None, K.X_LOG10)}
 
     def __init__(self, table: B200Table):
         self.t = table
@@ -130,14 +170,13 @@ class _Program:
                 return (K.XK_IMM, 0, _f64_bits(v), "f", False)
         return None
 
-    def _emit_with(self, op: int, leaf: Tuple[int, int, int, str, bool], ctx: str) -> None:
+    def _emit_with(self, op: int, leaf: Tuple[int, int, int, str, bool], ctx: str, flags: int = 0) -> None:
         """``acc <- acc op leaf`` with the leaf converted to the context class ('i', 'f' or 'b')."""
         kind, b, imm, cls, _ = leaf
-        flags = 0
         if kind == K.XK_COL:
             b = self.col_slot(b)
             if ctx == "f" and cls != "f":
-                flags = K.XF_B_I2F
+                flags |= K.XF_B_I2F
         elif kind == K.XK_IMM and ctx == "f" and cls != "f":
             v = imm - (1 << 64) if imm >= (1 << 63) else imm
             imm = _f64_bits(float(v))
@@ -211,10 +250,24 @@ class _Program:
         if e.kind == Kind.BINARY:
             return self._binary(e)
         if e.kind == Kind.CALL:
-            if e.func.upper() == "COALESCE":
+            low = _lower(e)
+            if low is not None:
+                return self._node(low)
+            fn = e.func.upper()
+            if fn == "COALESCE":
                 return self._coalesce(e)
-            if e.func.upper() in ("LIKE", "LENGTH"):
-                return self._string_function(e, e.func.upper())
+            if fn in ("LIKE", "LENGTH"):
+                return self._string_function(e, fn)
+            if fn == "CASE":
+                return self._case(e)
+            if fn in self._UNARY_FN:
+                return self._unary_function(e, fn)
+            if fn == "POWER":
+                if len(e.args) != 2:
+                    raise ValueError(f"POWER takes 2 arguments: {e}")
+                return self._binary(ColumnExpr(Kind.BINARY, "**", e.args))
+            if fn in ("GREATEST", "LEAST"):
+                return self._greatest(e, fn)
             raise NotImplementedError(f"function {e.func} has no device implementation")
         raise NotImplementedError(f"can't evaluate {e!r}")
 
@@ -229,7 +282,7 @@ class _Program:
         if "s" in (cl, cr):
             raise NotImplementedError(f"operator {op} on string operands: {e}")
         logical = op in ("&", "|")
-        ctx = "b" if logical else ("f" if (op == "/" or "f" in (cl, cr)) else "i")
+        ctx = "b" if logical else ("f" if (op in ("/", "**") or "f" in (cl, cr)) else "i")
         res = "b" if (logical or op in ("<", "<=", ">", ">=", "==", "!=")) else ctx
 
         def usable(leaf: Any) -> bool:  # a leaf whose class needs no instruction of its own in this context
@@ -241,17 +294,18 @@ class _Program:
             oi, of = self._OPS[o]
             return of if ctx == "f" else oi
 
+        makes_null = op in ("%", "**")  # x % 0 and a domain error of POWER are NULL whatever the operands
         lr, ll = self._leaf(e.right), self._leaf(e.left)
         if usable(lr):
             ca, na = self.compile(e.left)
             self._acc_to(ca, ctx)
             self._emit_with(code(op), lr, ctx)
-            return res, na or lr[4]
+            return res, na or lr[4] or makes_null
         if usable(ll):
             cb, nb = self.compile(e.right)
             self._acc_to(cb, ctx)
             self._emit_with(code(self._REVERSE[op]), ll, ctx)
-            return res, nb or ll[4]
+            return res, nb or ll[4] or makes_null
         ca, na = self.compile(e.left)
         self._acc_to(ca, ctx)
         tmp = self.alloc()
@@ -260,7 +314,7 @@ class _Program:
         self._acc_to(cb, ctx)
         self.emit(code(self._REVERSE[op]), K.XK_REG, tmp)
         self.release(tmp)
-        return res, na or nb
+        return res, na or nb or makes_null
 
     def _string_compare(self, e: ColumnExpr) -> Optional[Tuple[str, bool]]:
         """``strcol == 'lit'`` / ``!=``: compare dictionary codes."""
@@ -339,10 +393,119 @@ class _Program:
             nullable = nullable and n
         return want, nullable
 
+    def _case(self, e: ColumnExpr) -> Tuple[str, bool]:
+        """CASE WHEN c1 THEN v1 ... ELSE e END: the ELSE first, then the branches from last to first, each
+        ``acc <- c TRUE ? v : result so far`` (FB_X_SEL).  A leaf ELSE is read as the operand of the first select."""
+        args = [a if isinstance(a, ColumnExpr) else _lit(a) for a in e.args]
+        if len(args) < 3 or len(args) % 2 == 0:
+            raise ValueError(f"CASE needs (condition, value) pairs and an ELSE: {e}")
+        results = args[1::2] + [args[-1]]
+        probe = [self._static_cls(a) for a in results]
+        if "s" in probe:
+            raise NotImplementedError(f"CASE with string results outside a whole output column, or with string "
+                                      f"columns as results: {e}")
+        want = _coalesce_cls(probe)
+        pending = self._leaf(args[-1])
+        if pending is not None and (want != "b" or pending[3] in ("b", "n")):
+            nullable = pending[4]
+        else:
+            pending = None
+            cls, nullable = self.compile(args[-1])
+            self._acc_to(cls, want)
+        r = None
+        for i in range(len(args) // 2 - 1, -1, -1):
+            if pending is None:
+                if r is None:
+                    r = self.alloc()
+                self.emit(K.X_ST, K.XK_NONE, r)  # the result so far
+            cc, _ = self.compile(args[2 * i])
+            if cc == "s":
+                raise NotImplementedError(f"CASE condition {args[2 * i]} is a string: {e}")
+            self._acc_to(cc, "b")
+            c = self.alloc()
+            self.emit(K.X_ST, K.XK_NONE, c)
+            vc, vn = self.compile(args[2 * i + 1])
+            self._acc_to(vc, want)
+            if pending is not None:
+                self._emit_with(K.X_SEL, pending, want, c << K.XF_COND_SHIFT)
+                pending = None
+            else:
+                self.emit(K.X_SEL, K.XK_REG, r, c << K.XF_COND_SHIFT)
+            self.release(c)
+            nullable = nullable or vn
+        if r is not None:
+            self.release(r)
+        return want, nullable
+
+    def _unary_function(self, e: ColumnExpr, fn: str) -> Tuple[str, bool]:
+        """ABS FLOOR CEIL ROUND keep the class (bool counts as int64); SQRT EXP LN LOG10 give float64."""
+        nargs = len(e.args)
+        if not (nargs == 1 or (fn == "ROUND" and nargs == 2)):
+            raise ValueError(f"{fn} takes {'1 or 2 arguments' if fn == 'ROUND' else '1 argument'}: {e}")
+        d = 0
+        if nargs == 2:
+            dl = e.args[1]
+            d = dl.value if isinstance(dl, ColumnExpr) and dl.kind == Kind.LITERAL and dl.as_type is None else dl
+            if isinstance(d, bool) or not isinstance(d, int):
+                raise NotImplementedError(f"ROUND digits must be an integer literal: {e}")
+            if not -ROUND_MAX_DIGITS <= d <= ROUND_MAX_DIGITS:
+                raise ValueError(f"ROUND digits {d} outside [-{ROUND_MAX_DIGITS}, {ROUND_MAX_DIGITS}]: {e}")
+        arg = e.args[0] if isinstance(e.args[0], ColumnExpr) else _lit(e.args[0])
+        cls, nullable = self.compile(arg)
+        if cls == "s":
+            raise NotImplementedError(f"{fn} of a string: {e}")
+        opi, opf = self._UNARY_FN[fn]
+        if opi is None and fn not in ("FLOOR", "CEIL"):  # always float64; a domain error is NULL
+            if cls != "n":
+                self._acc_to(cls, "f")
+                self.emit(opf)
+            return "f", nullable if fn == "EXP" else True
+        if cls == "n":
+            return "n", True
+        if cls == "f":
+            self.emit(opf, imm=d & ((1 << 64) - 1))
+            return "f", nullable
+        if fn == "ABS":
+            self.emit(opi)
+        elif fn == "ROUND" and d < 0:
+            self.emit(opi, imm=d & ((1 << 64) - 1))
+        return "i", nullable
+
+    def _greatest(self, e: ColumnExpr, fn: str) -> Tuple[str, bool]:
+        """GREATEST / LEAST: NULL operands are skipped; NULL only if every operand is NULL."""
+        args = [a if isinstance(a, ColumnExpr) else _lit(a) for a in e.args]
+        if len(args) < 2:
+            raise ValueError(f"{fn} needs at least two arguments: {e}")
+        probe = [self._static_cls(a) for a in args]
+        if "s" in probe:
+            raise NotImplementedError(f"{fn} on strings: {e}")
+        want = _coalesce_cls(probe)
+        op = {("GREATEST", "f"): K.X_GREATEST_F, ("LEAST", "f"): K.X_LEAST_F}.get(
+            (fn, want), K.X_GREATEST_I if fn == "GREATEST" else K.X_LEAST_I)
+        cls, nullable = self.compile(args[0])
+        self._acc_to(cls, want)
+        for a in args[1:]:
+            leaf = self._leaf(a)
+            if leaf is not None and (want != "b" or leaf[3] in ("b", "n")):
+                self._emit_with(op, leaf, want)
+                nullable = nullable and leaf[4]
+                continue
+            tmp = self.alloc()
+            self.emit(K.X_ST, K.XK_NONE, tmp)
+            cls, n = self.compile(a)
+            self._acc_to(cls, want)
+            self.emit(op, K.XK_REG, tmp)  # symmetric: no reverse form
+            self.release(tmp)
+            nullable = nullable and n
+        return want, nullable
+
     def _static_cls(self, e: ColumnExpr) -> str:
         """Class an expression will evaluate to (without emitting code)."""
         if e.as_type is not None:
             return _cls_of(e.as_type)
+        low = _lower(e)
+        if low is not None:
+            return self._static_cls(low)
         if e.kind == Kind.NAMED:
             if e.name not in self.t.schema:
                 raise KeyError(f"column {e.name} is not in {self.t.schema}")
@@ -357,15 +520,24 @@ class _Program:
             c = self._static_cls(e.col)
             return "i" if c == "b" else c
         if e.kind == Kind.BINARY:
-            if e.op in ("+", "-", "*", "/"):
+            if e.op in ("+", "-", "*", "/", "%", "**"):
                 cs = (self._static_cls(e.left), self._static_cls(e.right))
-                return "f" if (e.op == "/" or "f" in cs) else "i"
+                return "f" if (e.op in ("/", "**") or "f" in cs) else "i"
             return "b"
         if e.kind == Kind.CALL and e.func.upper() == "COALESCE":
             cs = [self._static_cls(a if isinstance(a, ColumnExpr) else _lit(a)) for a in e.args]
             return "f" if "f" in cs else ("b" if "b" in cs and all(c in ("b", "n") for c in cs) else "i")
         if e.kind == Kind.CALL and e.func.upper() == "LIKE":
             return "b"
+        if e.kind == Kind.CALL and e.func.upper() in FLOAT_FUNCTIONS:
+            return "f"
+        if e.kind == Kind.CALL and e.func.upper() in ("CASE", "GREATEST", "LEAST"):
+            args = e.args[1::2] + e.args[-1:] if e.func.upper() == "CASE" else e.args
+            cs = [self._static_cls(a if isinstance(a, ColumnExpr) else _lit(a)) for a in args]
+            return "s" if "s" in cs else _coalesce_cls(cs)
+        if e.kind == Kind.CALL and e.func.upper() in ("ABS", "FLOOR", "CEIL", "ROUND") and e.args:
+            c = self._static_cls(e.args[0] if isinstance(e.args[0], ColumnExpr) else _lit(e.args[0]))
+            return "i" if c == "b" else c
         return "i"
 
     def run(self) -> Tuple[List[torch.Tensor], List[Optional[torch.Tensor]]]:
@@ -409,6 +581,7 @@ def project(t: B200Table, exprs: Sequence[ColumnExpr]) -> B200Table:
     out_valid: List[Any] = [None] * len(exprs)
     out_types: List[Any] = [None] * len(exprs)
     dicts: Dict[str, pa.Array] = {}
+    str_case: Dict[int, pa.Array] = {}  # output -> dictionary of a CASE with string-literal results
     pending: List[Tuple[int, ColumnExpr]] = []
     for i, e in enumerate(exprs):
         if e.kind == Kind.NAMED:
@@ -438,6 +611,12 @@ def project(t: B200Table, exprs: Sequence[ColumnExpr]) -> B200Table:
                     raise NotImplementedError(f"cast of string literal {e} to {tp}")
                 dicts[names[i]] = pa.array([e.value], type=pa.string())
             continue
+        strs = case_string_results(e)
+        if strs is not None:
+            if e.as_type is not None and not _is_str(e.as_type):
+                raise NotImplementedError(f"cast of a string CASE to {e.as_type}: {e}")
+            str_case[i] = pa.array(strs, type=pa.string())
+            e = _coded_case(e, strs)
         pending.append((i, e))
     # ---- computed columns: as many as fit into one launch at a time
     k = 0
@@ -448,6 +627,13 @@ def project(t: B200Table, exprs: Sequence[ColumnExpr]) -> B200Table:
             i, e = pending[k]
             mark = prog.mark()
             try:
+                if i in str_case:  # int32 codes into the literals' dictionary
+                    _, nullable = prog.compile(e, top=True)
+                    prog.output(torch.int32, nullable, K.T_I32)
+                    out_types[i] = pa.string()
+                    batch.append((i, e, "i"))
+                    k += 1
+                    continue
                 cls, nullable = prog.compile(e, top=True)
                 if cls == "n":  # a bare NULL-valued expression
                     cls = _cls_of(e.as_type) if e.as_type is not None and not _is_str(e.as_type) else "i"
@@ -469,11 +655,24 @@ def project(t: B200Table, exprs: Sequence[ColumnExpr]) -> B200Table:
             k += 1
         cols, valids = prog.run()
         for (i, e, cls), c, v in zip(batch, cols, valids):
-            if _is_str(out_types[i]):
+            if i in str_case:
+                dicts[names[i]] = str_case[i]
+            elif _is_str(out_types[i]):
                 c, dicts[names[i]] = _to_string_column(c, v, cls)
             out_cols[i], out_valid[i] = c, v
     schema = Schema([pa.field(nm, tp) for nm, tp in zip(names, out_types)])
     return B200Table(schema, out_cols, out_valid, dicts)
+
+
+def _coded_case(e: ColumnExpr, strs: List[str]) -> ColumnExpr:
+    """A CASE / IF / IIF / NULLIF with string-literal results as CASE with their codes in ``strs`` as results."""
+    low = _lower(e) or ColumnExpr(e.kind, e.head, e.args)
+    args = [a if isinstance(a, ColumnExpr) else _lit(a) for a in low.args]
+    code = {s: j for j, s in enumerate(strs)}
+    for j in list(range(1, len(args) - 1, 2)) + [len(args) - 1]:
+        if args[j].value is not None:
+            args[j] = _lit(code[args[j].value])
+    return ColumnExpr(Kind.CALL, "CASE", args, as_name=e.as_name)
 
 
 def predicate_mask(t: B200Table, condition: ColumnExpr) -> torch.Tensor:

@@ -823,10 +823,13 @@ EXPR_MAX_COLS, EXPR_MAX_OUTS, EXPR_MAX_INS, EXPR_NREGS = 16, 16, 96, 4
 T_I8, T_I16, T_I32, T_I64, T_U8, T_F32, T_F64, T_U16, T_U32, T_F16 = range(10)
 XK_NONE, XK_REG, XK_COL, XK_IMM, XK_NULL = range(5)
 XF_B_I2F = 1
+XF_COND_SHIFT = 8  # X_SEL: the condition's temporary is flags >> 8
 (X_MOV, X_ST, X_OUT, X_I2F, X_F2I, X_NEG_I, X_NEG_F, X_NOT, X_IS_NULL, X_NOT_NULL, X_TOBOOL_I, X_TOBOOL_F,
  X_ADD_I, X_SUB_I, X_RSUB_I, X_MUL_I, X_ADD_F, X_SUB_F, X_RSUB_F, X_MUL_F, X_DIV_F, X_RDIV_F,
  X_LT_I, X_LE_I, X_GT_I, X_GE_I, X_EQ_I, X_NE_I, X_LT_F, X_LE_F, X_GT_F, X_GE_F, X_EQ_F, X_NE_F,
- X_AND, X_OR, X_COALESCE, X_RCOALESCE, X_LOOKUP) = range(39)
+ X_AND, X_OR, X_COALESCE, X_RCOALESCE, X_LOOKUP,
+ X_SEL, X_MOD_I, X_RMOD_I, X_MOD_F, X_RMOD_F, X_ABS_I, X_ABS_F, X_FLOOR_F, X_CEIL_F, X_ROUND_F, X_ROUND_I,
+ X_SQRT, X_EXP, X_LN, X_LOG10, X_POW, X_RPOW, X_GREATEST_I, X_LEAST_I, X_GREATEST_F, X_LEAST_F) = range(60)
 
 # storage dtype of each K8 type: uint16 / uint32 / float16 live in the signed tensors of their width
 EXPR_STORAGE = {T_I8: torch.int8, T_I16: torch.int16, T_I32: torch.int32, T_I64: torch.int64, T_U8: torch.uint8,

@@ -14,9 +14,10 @@ fugue/workflow/workflow.py:2109-2166) and ``ExecutionEngine.aggregate`` reaches 
     SELECT * FROM a [INNER|LEFT|RIGHT|FULL [OUTER]|LEFT SEMI|LEFT ANTI|CROSS] JOIN b
              [USING (k, ...) | ON a.k = b.k [AND ...]]                        -> hash join kernels
 
-Expressions: + - * /, comparisons (= == != <> < <= > >=), AND / OR / NOT, IS [NOT] NULL, [NOT] IN (...),
-[NOT] BETWEEN, x [NOT] LIKE 'pattern' [ESCAPE 'c'], CAST(x AS type), COALESCE, LENGTH, literals, `quoted` and
-table-qualified names.
+Expressions: + - * / %, comparisons (= == != <> < <= > >=), AND / OR / NOT, IS [NOT] NULL, [NOT] IN (...),
+[NOT] BETWEEN, x [NOT] LIKE 'pattern' [ESCAPE 'c'], CAST(x AS type), CASE [x] WHEN .. THEN .. [ELSE ..] END,
+COALESCE, IFNULL, NULLIF, IF / IIF, MOD, ABS, FLOOR, CEIL / CEILING, ROUND, SQRT, EXP, LN, LOG10, POWER / POW,
+GREATEST, LEAST, LENGTH, literals, `quoted` and table-qualified names.
 Anything else raises NotImplementedError (there is no host SQL fallback in this package).
 """
 import re
@@ -277,12 +278,17 @@ _TOKEN = re.compile(r"""\s*(?:
   | (?P<str>'(?:[^'\\]|\\.|'')*')
   | (?P<bq>`(?:[^`]|``)*`)
   | (?P<id>[A-Za-z_]\w*)
-  | (?P<op><=|>=|<>|!=|==|=|<|>|\+|-|\*|/|\(|\)|,|\.)
+  | (?P<op><=|>=|<>|!=|==|=|<|>|\+|-|\*|/|%|\(|\)|,|\.)
 )""", re.X)
 
 _AGG_FUNCS = {"SUM": functions.sum, "COUNT": functions.count, "MIN": functions.min, "MAX": functions.max,
               "AVG": functions.avg, "MEAN": functions.avg, "FIRST": functions.first, "LAST": functions.last}
 _CLAUSES = ("WHERE", "GROUP", "HAVING", "ORDER", "LIMIT")
+_CASE_WORDS = ("WHEN", "THEN", "ELSE", "END")  # never a column name or an implicit alias
+_ONE_ARG = {"ABS": functions.abs, "FLOOR": functions.floor, "CEIL": functions.ceil, "CEILING": functions.ceil,
+            "SQRT": functions.sqrt, "EXP": functions.exp, "LN": functions.ln, "LOG10": functions.log10}
+_TWO_ARGS = {"NULLIF": functions.nullif, "IFNULL": functions.coalesce, "MOD": lambda a, b: a % b,
+             "POWER": functions.power, "POW": functions.power}
 
 
 def _tokenize(text: str, sql: str) -> List[Tuple[str, str]]:
@@ -427,6 +433,8 @@ class _Parser:
                 e = e * self.unary()
             elif self.op("/"):
                 e = e / self.unary()
+            elif self.op("%"):
+                e = e % self.unary()
             else:
                 return e
 
@@ -465,6 +473,10 @@ class _Parser:
             if up in ("TRUE", "FALSE"):
                 self.i += 1
                 return lit(up == "TRUE")
+            if up == "CASE":
+                return self._case()
+            if up in _CASE_WORDS:
+                self.fail(f"unexpected {up}")
             if up == "CAST" and self.peek(1) == ("op", "("):
                 self.i += 2
                 e = self.expr()
@@ -481,6 +493,21 @@ class _Parser:
             self.i += 1
             return self._maybe_qualified(val)
         return self.fail(f"unexpected token {val!r}")
+
+    def _case(self) -> ColumnExpr:
+        """``CASE WHEN c THEN v ... [ELSE e] END``, or ``CASE x WHEN a THEN v ...``, the searched form with ``x = a``."""
+        self.i += 1
+        subject = None if any(self.at_kw(w) for w in ("WHEN", "ELSE", "END")) else self.expr()
+        branches = []
+        while self.kw("WHEN"):
+            c = self.expr()
+            if not self.kw("THEN"):
+                self.fail("CASE WHEN without THEN")
+            branches.append((c if subject is None else subject == c, self.expr()))
+        else_ = self.expr() if self.kw("ELSE") else None
+        if not self.kw("END"):
+            self.fail("CASE without END")
+        return functions.case(branches, else_)
 
     def _maybe_qualified(self, name: str) -> ColumnExpr:
         if self.peek() == ("op", ".") and self.peek(1)[0] in ("id", "bq"):  # table.column
@@ -538,6 +565,21 @@ class _Parser:
             self.expect(")")
         if fn == "COALESCE":
             return functions.coalesce(*args)
+        want = 1 if fn in _ONE_ARG else 2 if fn in _TWO_ARGS else 3 if fn in ("IF", "IIF") else None
+        if want is not None and len(args) != want:
+            raise ValueError(f"{fn} takes {want} argument(s), got {len(args)} in: {self.sql}")
+        if fn in _ONE_ARG:
+            return _ONE_ARG[fn](args[0])
+        if fn in _TWO_ARGS:
+            return _TWO_ARGS[fn](args[0], args[1])
+        if fn in ("IF", "IIF"):
+            return functions.case([(args[0], args[1])], args[2])
+        if fn == "ROUND":
+            if len(args) not in (1, 2):
+                raise ValueError(f"ROUND takes 1 or 2 arguments, got {len(args)} in: {self.sql}")
+            return functions.round(args[0], args[1] if len(args) == 2 else 0)
+        if fn in ("GREATEST", "LEAST"):
+            return functions.greatest(*args) if fn == "GREATEST" else functions.least(*args)
         return function(fn, *args)
 
     def _quantile_literal(self, fn: str) -> Any:
@@ -560,7 +602,7 @@ class _Parser:
             self.i += 1
             return e.alias(val[1:-1].replace("``", "`") if kind == "bq" else val)
         kind, val = self.peek()
-        if kind == "bq" or (kind == "id" and val.upper() not in _CLAUSES + ("FROM",)):
+        if kind == "bq" or (kind == "id" and val.upper() not in _CLAUSES + _CASE_WORDS + ("FROM",)):
             self.i += 1  # implicit alias
             return e.alias(val[1:-1].replace("``", "`") if kind == "bq" else val)
         return e

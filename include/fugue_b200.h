@@ -458,6 +458,24 @@ int fb_join2_emit(int dev, void* stream, int64_t nprobe, const void* probe_keys,
  *               at the same entry.  A NULL accumulator, or an entry number outside [0, imm), gives
  *               NULL and issues no load.  A dictionary-encoded string column is loaded with FB_X_MOV (its
  *               int32 code) and mapped through a per-entry result table (fb_string_like / _length).
+ * Scalar functions (CASE / NULLIF / % / numeric functions).  Integer ops are on int64 and wrap; float ops on float64.
+ * Rule of these ops only: a NaN result from operands that are not NaN (a domain error) is NULL.
+ *   FB_X_SEL     acc <- temp[c] is TRUE ? acc : B, c = flags >> FB_XF_COND_SHIFT, a temporary in [0, FB_EXPR_NREGS)
+ *                holding a bool.  A NULL or FALSE condition takes B, with B's validity (CASE WHEN, branch by branch)
+ *   FB_X_MOD_I   acc <- acc % B, truncated (sign of acc); B = 0 gives NULL; INT64_MIN % -1 = 0 (FB_X_RMOD_I: B % acc)
+ *   FB_X_MOD_F   acc <- fmod(acc, B), exact; B = +-0.0 gives NULL, fmod(+-inf, y) is a domain error (FB_X_RMOD_F)
+ *   FB_X_ABS_I   acc <- |acc|, INT64_MIN stays INT64_MIN        FB_X_ABS_F   acc <- fabs(acc) (clears the sign bit)
+ *   FB_X_FLOOR_F / FB_X_CEIL_F   IEEE floor / ceil
+ *   FB_X_ROUND_F acc <- acc rounded to imm decimal digits (imm in [-18, 18]): imm = 0 is C round (half away from
+ *                zero); otherwise round(acc * 10^imm) / 10^imm (imm < 0: round(acc / 10^-imm) * 10^-imm), one IEEE
+ *                op per step, and acc itself when the scaled value is +-inf or NaN
+ *   FB_X_ROUND_I acc <- acc rounded to a multiple of 10^-imm, half away from zero (imm in [-18, -1]), wrapping
+ *   FB_X_SQRT / FB_X_EXP / FB_X_LN / FB_X_LOG10   sqrt (correctly rounded), exp, log, log10 of the float acc
+ *   FB_X_POW     acc <- pow(acc, B) (C99 Annex F special cases); FB_X_RPOW: pow(B, acc)
+ *   FB_X_GREATEST_I / FB_X_LEAST_I / FB_X_GREATEST_F / FB_X_LEAST_F   the larger / smaller of acc and B; a NULL
+ *                side is skipped, so the result is NULL only if both are; floats in IEEE totalOrder
+ *                (-NaN < -inf < ... < -0.0 < +0.0 < ... < +inf < +NaN), returning that operand's bits
+ *   The unary ops among these (ABS, FLOOR, CEIL, ROUND, SQRT, EXP, LN, LOG10) take no operand (FB_XK_NONE).
  * Column types: FB_T_U16 / FB_T_U32 load zero-extended, FB_T_F16 loads its IEEE half value exactly.
  * Stores keep the low bits of an integer (unsigned stores are the signed ones of the same width) and
  * round a float to nearest even (FB_T_F32, FB_T_F16).
@@ -472,6 +490,7 @@ enum fb_expr_type { FB_T_I8 = 0, FB_T_I16 = 1, FB_T_I32 = 2, FB_T_I64 = 3, FB_T_
                     FB_T_U16 = 7, FB_T_U32 = 8, FB_T_F16 = 9 };
 enum fb_expr_operand { FB_XK_NONE = 0, FB_XK_REG = 1, FB_XK_COL = 2, FB_XK_IMM = 3, FB_XK_NULL = 4 };
 #define FB_XF_B_I2F 1
+#define FB_XF_COND_SHIFT 8 /* FB_X_SEL: the condition's temporary sits in flags >> 8 */
 enum fb_expr_op {
   FB_X_MOV = 0, FB_X_ST = 1, FB_X_OUT = 2,
   FB_X_I2F = 3, FB_X_F2I = 4, FB_X_NEG_I = 5, FB_X_NEG_F = 6, FB_X_NOT = 7, FB_X_IS_NULL = 8,
@@ -480,8 +499,13 @@ enum fb_expr_op {
   FB_X_ADD_F = 16, FB_X_SUB_F = 17, FB_X_RSUB_F = 18, FB_X_MUL_F = 19, FB_X_DIV_F = 20, FB_X_RDIV_F = 21,
   FB_X_LT_I = 22, FB_X_LE_I = 23, FB_X_GT_I = 24, FB_X_GE_I = 25, FB_X_EQ_I = 26, FB_X_NE_I = 27,
   FB_X_LT_F = 28, FB_X_LE_F = 29, FB_X_GT_F = 30, FB_X_GE_F = 31, FB_X_EQ_F = 32, FB_X_NE_F = 33,
-  FB_X_AND = 34, FB_X_OR = 35, FB_X_COALESCE = 36, FB_X_RCOALESCE = 37, FB_X_LOOKUP = 38
+  FB_X_AND = 34, FB_X_OR = 35, FB_X_COALESCE = 36, FB_X_RCOALESCE = 37, FB_X_LOOKUP = 38,
+  FB_X_SEL = 39, FB_X_MOD_I = 40, FB_X_RMOD_I = 41, FB_X_MOD_F = 42, FB_X_RMOD_F = 43,
+  FB_X_ABS_I = 44, FB_X_ABS_F = 45, FB_X_FLOOR_F = 46, FB_X_CEIL_F = 47, FB_X_ROUND_F = 48, FB_X_ROUND_I = 49,
+  FB_X_SQRT = 50, FB_X_EXP = 51, FB_X_LN = 52, FB_X_LOG10 = 53, FB_X_POW = 54, FB_X_RPOW = 55,
+  FB_X_GREATEST_I = 56, FB_X_LEAST_I = 57, FB_X_GREATEST_F = 58, FB_X_LEAST_F = 59
 };
+#define FB_EXPR_ROUND_MAX_DIGITS 18
 typedef struct fb_expr_ins {
   int32_t op;    /* enum fb_expr_op */
   int32_t kind;  /* enum fb_expr_operand: what operand B is */

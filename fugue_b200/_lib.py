@@ -115,6 +115,11 @@ SIGNATURES = {
                                         C.POINTER(C.c_double), _i32p, _vp, _vpp, _vp, C.c_size_t]),
     "fb_string_length": (C.c_int, [C.c_int, _vp, C.c_int64, _vp, _vp, _vp, _vp]),
     "fb_string_like": (C.c_int, [C.c_int, _vp, C.c_int64, _vp, _vp, _vp, C.c_int, C.POINTER(C.c_int16), _vp, _vp]),
+    "fb_string_transform": (C.c_int, [C.c_int, _vp, C.c_int, C.c_int64, _vp, _vp, _vp, _vp, C.c_int64, C.c_int64,
+                                      C.c_int, C.c_int, C.c_char_p, C.c_int, C.c_char_p, C.c_int,
+                                      C.POINTER(C.c_int16), C.c_int, _vp, _vp, _vp, _vp]),
+    "fb_string_hash": (C.c_int, [C.c_int, _vp, C.c_int64, _vp, _vp, _vp, C.c_int, _vp]),
+    "fb_string_first_equal": (C.c_int, [C.c_int, _vp, C.c_int64, _vp, _vp, _vp, _vp, _vp, _vp]),
 }
 
 

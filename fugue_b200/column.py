@@ -5,10 +5,12 @@ from an expression is a function of ``(kind, head, args)``:
 
     NAMED     head = column name                     WILDCARD  ``*``
     LITERAL   head = python value (None = NULL)      UNARY     head in ``- ~ IS_NULL NOT_NULL``, one arg
-    BINARY    head in ``+ - * / % & | < > <= >= == !=``  CALL    head = function name (``COALESCE`` ...)
+    BINARY    head in ``+ - * / % & | < > <= >= == != ||``  CALL  head = function name (``COALESCE`` ...)
               ``LIKE``: args (string, pattern literal[, escape literal]); ``LENGTH``: args (string,)
               ``CASE``: args (cond1, value1, ..., condN, valueN, else), the ELSE always stored (NULL if absent);
               ``NULLIF ABS FLOOR CEIL SQRT EXP LN LOG10 POWER GREATEST LEAST``; ``ROUND``: args (x, digits literal)
+              ``UPPER LOWER``: args (string,); ``SUBSTR``: args (string, start[, length]); ``TRIM LTRIM RTRIM``:
+              args (string[, characters]); ``REPLACE``: args (string, from, to); ``CONCAT``: args (part, ...)
     AGG       head in ``SUM COUNT AVG MIN MAX FIRST LAST``, one arg, optional DISTINCT, or ``PERCENTILE_CONT
               PERCENTILE_DISC``, one arg and kwarg ``q`` (MEDIAN is PERCENTILE_CONT at q = 0.5)
     WINDOW    head in the AGG functions (one arg, kwargs ``running``, ``rows`` or ``range``; a percentile keeps
@@ -59,6 +61,8 @@ _RUNNING_FRAME = "ROWS BETWEEN UNBOUNDED PRECEDING AND CURRENT ROW"
 _LITERAL_TYPES = (int, bool, float, str)
 FLOAT_FUNCTIONS = frozenset(["SQRT", "EXP", "LN", "LOG10", "POWER", "POW"])  # always float64
 ROUND_MAX_DIGITS = 18
+# functions that build a string from one string expression and literals (SUBSTRING is SUBSTR); ``||`` too
+STRING_FUNCTIONS = frozenset(["UPPER", "LOWER", "SUBSTR", "SUBSTRING", "TRIM", "LTRIM", "RTRIM", "REPLACE", "CONCAT"])
 
 
 def to_pa_datatype(obj: Any) -> pa.DataType:
@@ -197,7 +201,7 @@ class ColumnExpr:
         if k == Kind.LITERAL:
             return None if self.head is None else to_pa_datatype(type(self.head))
         if k == Kind.BINARY:
-            return pa.bool_() if self.head in BOOL_OPS else None
+            return pa.bool_() if self.head in BOOL_OPS else (pa.string() if self.head == "||" else None)
         if k == Kind.UNARY and self.head in ("-", "~"):
             tp = self.args[0].infer_type(schema)
             if tp is None:
@@ -209,6 +213,8 @@ class ColumnExpr:
             return self.args[0].infer_type(schema)
         if k == Kind.CALL and self.head in ("LIKE", "LENGTH"):
             return pa.bool_() if self.head == "LIKE" else pa.int64()
+        if k == Kind.CALL and self.head.upper() in STRING_FUNCTIONS:
+            return pa.string()
         if k == Kind.CALL and self.head.upper() in FLOAT_FUNCTIONS:
             return pa.float64()
         if k == Kind.CALL and case_string_results(self) is not None:
@@ -532,6 +538,32 @@ def _result_args(e: ColumnExpr) -> List[Any]:
     return list(e.args[:1]) if head == "NULLIF" else []
 
 
+def is_string_build(e: Any) -> bool:
+    """True for a node that builds a string: a call of ``STRING_FUNCTIONS`` (any letter case) or ``||``."""
+    return isinstance(e, ColumnExpr) and ((e.kind == Kind.CALL and e.head.upper() in STRING_FUNCTIONS) or
+                                          (e.kind == Kind.BINARY and e.head == "||"))
+
+
+def _int_arg(fn: str, what: str, v: Any) -> ColumnExpr:
+    """An int literal argument (or NULL) of a string function."""
+    e = _operand(v)
+    if e.kind != Kind.LITERAL or e.as_type is not None:
+        raise NotImplementedError(f"{fn}: {what} must be an int literal, got {e}")
+    if e.value is not None and (isinstance(e.value, bool) or not isinstance(e.value, int)):
+        raise ValueError(f"{fn}: {what} must be an int literal or NULL, got {e.value!r}")
+    return e
+
+
+def _str_arg(fn: str, what: str, v: Any) -> ColumnExpr:
+    """A string literal argument (or NULL) of a string function."""
+    e = _operand(v)
+    if e.kind != Kind.LITERAL or e.as_type is not None:
+        raise NotImplementedError(f"{fn}: {what} must be a string literal, got {e}")
+    if e.value is not None and not isinstance(e.value, str):
+        raise ValueError(f"{fn}: {what} must be a string literal or NULL, got {e.value!r}")
+    return e
+
+
 def case_string_results(e: Any) -> Optional[List[str]]:
     """The distinct string literals (in order of appearance) of a CASE / IF / IIF / NULLIF whose every result is a
     string literal or NULL, with at least one string; None for any other node."""
@@ -653,6 +685,67 @@ class functions:
     def length(c: Any) -> ColumnExpr:
         """SQL ``LENGTH(c)``: the number of characters (code points) of a string, int64."""
         return ColumnExpr(Kind.CALL, "LENGTH", [col(c)])
+
+    @staticmethod
+    def upper(c: Any) -> ColumnExpr:
+        """SQL ``UPPER(c)``: every code point by its simple (one to one) Unicode upper-case mapping."""
+        return ColumnExpr(Kind.CALL, "UPPER", [col(c)])
+
+    @staticmethod
+    def lower(c: Any) -> ColumnExpr:
+        """SQL ``LOWER(c)``: every code point by its simple (one to one) Unicode lower-case mapping."""
+        return ColumnExpr(Kind.CALL, "LOWER", [col(c)])
+
+    @staticmethod
+    def substr(c: Any, start: Any, length: Any = None) -> ColumnExpr:
+        """SQLite ``SUBSTR(c, start[, length])`` in code points: 1-based; a negative start counts from the end;
+        a negative length takes the code points before start.  ``start`` / ``length`` are int literals; NULL
+        (``null()``) gives NULL, and ``length=None`` means no length."""
+        args = [col(c), _int_arg("SUBSTR", "start", start)]
+        if length is not None:
+            args.append(_int_arg("SUBSTR", "length", length))
+        return ColumnExpr(Kind.CALL, "SUBSTR", args)
+
+    @staticmethod
+    def _trim(fn: str, c: Any, chars: Any) -> ColumnExpr:
+        return ColumnExpr(Kind.CALL, fn, [col(c)] + ([] if chars is None else [_str_arg(fn, "characters", chars)]))
+
+    @staticmethod
+    def trim(c: Any, chars: Any = None) -> ColumnExpr:
+        """SQLite ``TRIM(c[, chars])``: removes the code points of ``chars`` (default: the space U+0020 only)
+        from both ends."""
+        return functions._trim("TRIM", c, chars)
+
+    @staticmethod
+    def ltrim(c: Any, chars: Any = None) -> ColumnExpr:
+        return functions._trim("LTRIM", c, chars)
+
+    @staticmethod
+    def rtrim(c: Any, chars: Any = None) -> ColumnExpr:
+        return functions._trim("RTRIM", c, chars)
+
+    @staticmethod
+    def replace(c: Any, from_: Any, to: Any) -> ColumnExpr:
+        """SQLite ``REPLACE(c, from_, to)``: every non-overlapping ``from_``, left to right, by ``to``; an empty
+        ``from_`` leaves ``c`` unchanged."""
+        return ColumnExpr(Kind.CALL, "REPLACE", [col(c), _str_arg("REPLACE", "from", from_), _str_arg("REPLACE", "to", to)])
+
+    @staticmethod
+    def concat(*parts: Any) -> ColumnExpr:
+        """SQLite ``CONCAT(a, ...)``: the parts joined; NULL parts are skipped (``CONCAT(NULL)`` is '')."""
+        if not parts:
+            raise ValueError("CONCAT needs at least one argument")
+        return ColumnExpr(Kind.CALL, "CONCAT", [_operand(x) for x in parts])
+
+    @staticmethod
+    def concat_strict(*parts: Any) -> ColumnExpr:
+        """SQL ``a || b || ...`` (left-nested): the parts joined, NULL if any part is NULL."""
+        if len(parts) < 2:
+            raise ValueError("|| needs at least two operands")
+        e = _operand(parts[0])
+        for x in parts[1:]:
+            e = binary("||", e, x)
+        return e
 
     @staticmethod
     def min(c: Any) -> ColumnExpr:  # noqa: A003
@@ -809,7 +902,7 @@ class SelectColumns:
 
 
 # ---- SQL text of a tree (error messages, INTEGRATION.md examples, the golden test) ------------------
-_SQL_OF_OP = {"&": " AND ", "|": " OR ", "==": "="}
+_SQL_OF_OP = {"&": " AND ", "|": " OR ", "==": "=", "||": " || "}
 
 
 def _quote(name: str) -> str:
@@ -845,7 +938,7 @@ def to_sql(expr: ColumnExpr, enable_cast: bool = True, nested: bool = False) -> 
         body = "CASE" + "".join(f" WHEN {to_sql(_operand(a[i]), enable_cast)} THEN {to_sql(_operand(a[i + 1]), enable_cast)}"
                                 for i in range(0, len(a) - 1, 2)) + f" ELSE {to_sql(_operand(a[-1]), enable_cast)} END"
     elif k == Kind.BINARY:
-        if expr.head not in BOOL_OPS and expr.head not in ARITH_OPS:
+        if expr.head not in BOOL_OPS and expr.head not in ARITH_OPS and expr.head != "||":
             raise NotImplementedError(expr)
         body = to_sql(expr.args[0], enable_cast, True) + _SQL_OF_OP.get(expr.head, expr.head) + \
             to_sql(expr.args[1], enable_cast, True)

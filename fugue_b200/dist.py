@@ -28,6 +28,7 @@ from typing import Any, Dict, List, Optional, Sequence, Tuple
 os.environ.setdefault("CUDA_DEVICE_MAX_CONNECTIONS", "32")
 
 import numpy as np  # noqa: E402
+import pyarrow as pa  # noqa: E402
 import torch  # noqa: E402
 import torch.distributed as dist  # noqa: E402
 
@@ -613,11 +614,19 @@ class DistributedB200Engine(B200ExecutionEngine):
 
         keys = [] if partition_spec is None else list(partition_spec.partition_by)
         if self._world > 1:
-            # MIN / MAX of a string column compare dictionary ranks, and every rank has its own dictionary
-            strs = self.to_df(df).native.dictionaries
-            assert_or_throw(not any(a.func in ("MIN", "MAX") and a.arg.kind == Kind.NAMED and a.arg.name in strs
-                                    for a in agg_cols if a.kind == Kind.AGG), lambda: NotImplementedError(
-                "MIN / MAX of a string column across GPUs: string dictionaries are per rank"))
+            # MIN / MAX of a string column or expression compare dictionary ranks, and every rank has its own
+            # dictionary
+            t = self.to_df(df).native
+
+            def is_str(a: Any) -> bool:
+                if a.kind == Kind.NAMED and a.name in t.dictionaries:
+                    return True
+                tp = a.infer_type(t.schema)
+                return tp is not None and (pa.types.is_string(tp) or pa.types.is_large_string(tp))
+
+            assert_or_throw(not any(a.func in ("MIN", "MAX") and is_str(a.arg) for a in agg_cols if a.kind == Kind.AGG),
+                            lambda: NotImplementedError("MIN / MAX of a string column or expression across GPUs: "
+                                                        "string dictionaries are per rank"))
         if self._world == 1 or not self._plain_aggs(agg_cols):
             # aggregations of expressions / expressions of aggregations: the base class evaluates the
             # row-wise parts locally and comes back here with plain FUNC(column) aggregations

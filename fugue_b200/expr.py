@@ -16,6 +16,10 @@ read per row through the entry's code (``FB_X_LOOKUP``), inside the same program
 ``GREATEST`` / ``LEAST``, is COALESCE's rule.  ``%`` and ``ABS FLOOR CEIL ROUND`` keep the operand's class
 (int64 or float64), ``SQRT EXP LN LOG10 POWER`` are float64.  A CASE whose results are string literals is a
 whole output column only: ``project`` compiles it to int32 codes into a dictionary of those literals.
+A string-building expression over one string column (``UPPER LOWER SUBSTR TRIM LTRIM RTRIM REPLACE CONCAT ||``)
+is evaluated over the dictionary (``strings.evaluate``); per row it is the code (``FB_X_MOV``) mapped to the
+result's code in a new dictionary (``FB_X_LOOKUP``).  It is a whole output column (``project``), or the
+operand of ``==`` / ``!=`` with a string literal, of ``IS [NOT] NULL``, of ``LIKE`` and of ``LENGTH``.
 """
 import struct
 from typing import Any, Dict, List, Optional, Sequence, Tuple
@@ -25,7 +29,8 @@ import torch
 
 from . import kernels as K
 from . import strings as ST
-from .column import FLOAT_FUNCTIONS, ROUND_MAX_DIGITS, ColumnExpr, Kind, case_string_results, lit as _lit
+from .column import (FLOAT_FUNCTIONS, ROUND_MAX_DIGITS, ColumnExpr, Kind, case_string_results, is_string_build,
+                     lit as _lit)
 from .schema import Schema
 from .table import B200Table, _storage_dtype, expr_type
 
@@ -218,6 +223,9 @@ class _Program:
         return cls, nullable
 
     def _node(self, e: ColumnExpr) -> Tuple[str, bool]:  # noqa: C901
+        if is_string_build(e):
+            raise NotImplementedError(f"{e} builds a string: it is a whole output column, or the operand of == / != "
+                                      f"with a string literal, IS NULL, LIKE or LENGTH")
         if e.kind == Kind.WILDCARD:
             raise ValueError("'*' can't be evaluated as a value")
         if e.kind == Kind.AGG:
@@ -231,6 +239,10 @@ class _Program:
             self._emit_with(K.X_MOV, leaf, leaf[3])
             return leaf[3], leaf[4]
         if e.kind == Kind.UNARY:
+            if e.op in ("IS_NULL", "NOT_NULL") and is_string_build(e.col):
+                self.string_codes(e.col)
+                self.emit(K.X_IS_NULL if e.op == "IS_NULL" else K.X_NOT_NULL)
+                return "b", False
             cls, nullable = self.compile(e.col)
             if e.op in ("IS_NULL", "NOT_NULL"):  # string columns are fine here: only validity is read
                 self.emit(K.X_IS_NULL if e.op == "IS_NULL" else K.X_NOT_NULL)
@@ -317,16 +329,24 @@ class _Program:
         return res, na or nb or makes_null
 
     def _string_compare(self, e: ColumnExpr) -> Optional[Tuple[str, bool]]:
-        """``strcol == 'lit'`` / ``!=``: compare dictionary codes."""
+        """``strcol == 'lit'`` / ``!=``: compare dictionary codes; a string expression's codes are those of its
+        new dictionary."""
         t = self.t
         sides = [e.left, e.right]
         named = [s.kind == Kind.NAMED and s.as_type is None and s.name in t.schema
                  and _is_str(t.schema[s.name].type) for s in sides]
+        built = [is_string_build(s) for s in sides]
         lits = [s.kind == Kind.LITERAL and isinstance(s.value, str) for s in sides]
-        if not (any(named) or any(lits)):
+        if not (any(named) or any(lits) or any(built)):
             return None
         if e.op not in ("==", "!="):
             raise NotImplementedError(f"operator {e.op} on strings (only == and != run on the device): {e}")
+        if (built[0] and lits[1]) or (built[1] and lits[0]):
+            s, lit_ = (sides[0], sides[1]) if built[0] else (sides[1], sides[0])
+            d, nullable = self.string_codes(s)
+            code = d.index(lit_.value).as_py() if len(d) > 0 else -1
+            self.emit(K.X_EQ_I if e.op == "==" else K.X_NE_I, K.XK_IMM, 0, 0, code & ((1 << 64) - 1))
+            return "b", nullable
         if named[0] and lits[1]:
             c, lit_ = sides[0], sides[1]
         elif named[1] and lits[0]:
@@ -341,10 +361,33 @@ class _Program:
                   (code if code is not None else -1) & ((1 << 64) - 1))
         return "b", t.valid[ci] is not None
 
+    def string_codes(self, s: ColumnExpr) -> Tuple[pa.Array, bool]:
+        """A string-building expression's int32 codes into the accumulator: the column's code, then the
+        result's code in the new dictionary (and, after a CONCAT, the code of a NULL row's result).  Returns
+        (the new dictionary, nullable)."""
+        t = self.t
+        if s.as_type is not None and not _is_str(s.as_type):
+            raise NotImplementedError(f"cast of a string expression to {s.as_type}: {s}")
+        name, steps = ST.string_chain(s, t.dictionaries)
+        r = ST.evaluate(t.dictionaries[name], t.device, steps)
+        key: Any = ("STR", name, steps)
+        self.tables[key] = (r.remap, r.remap_valid)
+        ci = t.schema.index_of_key(name)
+        self.emit(K.X_MOV, K.XK_COL, self.col_slot(ci))
+        self.emit(K.X_LOOKUP, K.XK_COL, self.col_slot(key), 0, len(t.dictionaries[name]))
+        row_null = t.valid[ci] is not None
+        if r.null_code is not None and row_null:
+            self.emit(K.X_COALESCE, K.XK_IMM, 0, 0, r.null_code)
+            row_null = False
+        return r.dictionary, row_null or r.remap_valid is not None
+
     def _string_function(self, e: ColumnExpr, fn: str) -> Tuple[str, bool]:
-        """``LIKE`` / ``LENGTH`` of a string column: the code, then its dictionary entry's result."""
+        """``LIKE`` / ``LENGTH`` of a string column: the code, then its dictionary entry's result.  Of a string
+        expression: its code in the new dictionary, then that entry's result."""
         t = self.t
         s = e.args[0] if e.args else None
+        if isinstance(s, ColumnExpr) and is_string_build(s):
+            return self._string_function_of_expr(e, fn, s)
         if not (isinstance(s, ColumnExpr) and s.kind == Kind.NAMED and s.as_type is None and s.name in t.schema
                 and _is_str(t.schema[s.name].type)):
             raise NotImplementedError(f"{fn} needs a string column as its operand: {e}")
@@ -367,6 +410,31 @@ class _Program:
         self.emit(K.X_MOV, K.XK_COL, self.col_slot(ci))
         self.emit(K.X_LOOKUP, K.XK_COL, self.col_slot(key), 0, len(d))
         return ("b" if fn == "LIKE" else "i"), t.valid[ci] is not None or self.tables[key][1] is not None
+
+    def _string_function_of_expr(self, e: ColumnExpr, fn: str, s: ColumnExpr) -> Tuple[str, bool]:
+        t = self.t
+        if fn == "LIKE":
+            lits = e.args[1:]
+            if not (1 <= len(lits) <= 2 and all(a.kind == Kind.LITERAL and isinstance(a.value, str) for a in lits)):
+                raise NotImplementedError(f"LIKE needs a string literal pattern: {e}")
+        elif len(e.args) != 1:
+            raise ValueError(f"LENGTH takes one argument: {e}")
+        d, nullable = self.string_codes(s)
+        name, steps = ST.string_chain(s, t.dictionaries)
+        if fn == "LIKE":
+            pattern, escape = lits[0].value, (lits[1].value if len(lits) > 1 else None)
+            key: Any = ("LIKE", ("STR", name, steps), pattern, escape)
+            if key not in self.tables:
+                self.tables[key] = ST.like_table(d, t.device, pattern, escape)
+        else:
+            key = ("LENGTH", ("STR", name, steps))
+            if key not in self.tables:
+                self.tables[key] = ST.length_table(d, t.device)
+        if len(d) == 0:  # every result is NULL: a one-entry table that is never read, for a real device pointer
+            self.tables[key] = (torch.zeros(1, dtype=torch.int64, device=t.device),
+                                torch.zeros(1, dtype=torch.uint8, device=t.device))
+        self.emit(K.X_LOOKUP, K.XK_COL, self.col_slot(key), 0, len(d))
+        return ("b" if fn == "LIKE" else "i"), nullable or self.tables[key][1] is not None
 
     def _coalesce(self, e: ColumnExpr) -> Tuple[str, bool]:
         args = [a if isinstance(a, ColumnExpr) else _lit(a) for a in e.args]
@@ -519,6 +587,8 @@ class _Program:
                 return "b"
             c = self._static_cls(e.col)
             return "i" if c == "b" else c
+        if is_string_build(e):
+            return "s"
         if e.kind == Kind.BINARY:
             if e.op in ("+", "-", "*", "/", "%", "**"):
                 cs = (self._static_cls(e.left), self._static_cls(e.right))
@@ -582,6 +652,7 @@ def project(t: B200Table, exprs: Sequence[ColumnExpr]) -> B200Table:
     out_types: List[Any] = [None] * len(exprs)
     dicts: Dict[str, pa.Array] = {}
     str_case: Dict[int, pa.Array] = {}  # output -> dictionary of a CASE with string-literal results
+    str_built: Dict[int, pa.Array] = {}  # output -> dictionary of a string-building expression
     pending: List[Tuple[int, ColumnExpr]] = []
     for i, e in enumerate(exprs):
         if e.kind == Kind.NAMED:
@@ -627,6 +698,13 @@ def project(t: B200Table, exprs: Sequence[ColumnExpr]) -> B200Table:
             i, e = pending[k]
             mark = prog.mark()
             try:
+                if is_string_build(e):  # int32 codes into the result's dictionary
+                    str_built[i], nullable = prog.string_codes(e)
+                    prog.output(torch.int32, nullable, K.T_I32)
+                    out_types[i] = pa.string()
+                    batch.append((i, e, "i"))
+                    k += 1
+                    continue
                 if i in str_case:  # int32 codes into the literals' dictionary
                     _, nullable = prog.compile(e, top=True)
                     prog.output(torch.int32, nullable, K.T_I32)
@@ -657,6 +735,8 @@ def project(t: B200Table, exprs: Sequence[ColumnExpr]) -> B200Table:
         for (i, e, cls), c, v in zip(batch, cols, valids):
             if i in str_case:
                 dicts[names[i]] = str_case[i]
+            elif i in str_built:
+                dicts[names[i]] = str_built[i]
             elif _is_str(out_types[i]):
                 c, dicts[names[i]] = _to_string_column(c, v, cls)
             out_cols[i], out_valid[i] = c, v

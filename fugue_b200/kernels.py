@@ -914,3 +914,61 @@ def string_like(offsets: torch.Tensor, data: torch.Tensor, valid: Optional[torch
                                   0 if valid is None else valid.data_ptr(), len(tokens), toks, out.data_ptr(),
                                   out_valid.data_ptr()))
     return out, out_valid
+
+
+# ---- K12: string-building functions over a dictionary's entries ---------------------------------
+STR_MAX_LITERAL, STR_MAX_TOKENS, STR_SELF = 256, 1024, 256
+(STR_COPY, STR_UPPER, STR_LOWER, STR_SUBSTR, STR_LTRIM, STR_RTRIM, STR_TRIM, STR_REPLACE, STR_FORMAT) = range(9)
+
+
+def string_transform(op: int, offsets: torch.Tensor, data: torch.Tensor, valid: Optional[torch.Tensor],
+                     src: Optional[torch.Tensor] = None, start: int = 0, length: Optional[int] = None,
+                     lits: Sequence[bytes] = (), tokens: Sequence[int] = (), null_is_empty: bool = False,
+                     out_offsets: Optional[torch.Tensor] = None, out_data: Optional[torch.Tensor] = None
+                     ) -> Tuple[Optional[torch.Tensor], Optional[torch.Tensor]]:
+    """One ``fb_string_transform`` call over the entries of a device dictionary (int64 ``offsets``, uint8
+    ``data`` and ``valid``), or over the entries ``src`` (int64) when given.  Without ``out_data`` it is the
+    measure call and returns (byte length int64, validity uint8) per output; with ``out_offsets`` /
+    ``out_data`` it fills the bytes and returns (None, None).  ``lits``: up to two literal arguments."""
+    lib = _lib.load()
+    dev = offsets.device
+    n = int(src.shape[0]) if src is not None else int(offsets.shape[0]) - 1
+    lit0, lit1 = (list(lits) + [b"", b""])[:2]
+    toks = (C.c_int16 * max(len(tokens), 1))(*tokens)
+    out_len = out_valid = None
+    if out_data is None:
+        out_len = torch.empty(n, dtype=torch.int64, device=dev)
+        out_valid = torch.empty(n, dtype=torch.uint8, device=dev)
+    _lib.check(lib.fb_string_transform(
+        dev.index, _stream_ptr(dev), op, n, offsets.data_ptr(), data.data_ptr(),
+        0 if valid is None else valid.data_ptr(), 0 if src is None else src.data_ptr(), start,
+        0 if length is None else length, int(length is not None), len(lit0), lit0, len(lit1), lit1, len(tokens),
+        toks, int(null_is_empty), 0 if out_len is None else out_len.data_ptr(),
+        0 if out_valid is None else out_valid.data_ptr(), 0 if out_offsets is None else out_offsets.data_ptr(),
+        0 if out_data is None else out_data.data_ptr()))
+    return out_len, out_valid
+
+
+def string_hash(offsets: torch.Tensor, data: torch.Tensor, valid: Optional[torch.Tensor], bits: int = 64
+                ) -> torch.Tensor:
+    """A 64-bit hash of every entry's bytes (its low ``bits`` kept), as int64; 0 for a NULL entry."""
+    lib = _lib.load()
+    dev = offsets.device
+    n = int(offsets.shape[0]) - 1
+    out = torch.empty(n, dtype=torch.int64, device=dev)
+    _lib.check(lib.fb_string_hash(dev.index, _stream_ptr(dev), n, offsets.data_ptr(), data.data_ptr(),
+                                  0 if valid is None else valid.data_ptr(), bits, out.data_ptr()))
+    return out
+
+
+def string_first_equal(offsets: torch.Tensor, data: torch.Tensor, valid: Optional[torch.Tensor],
+                       sorted_hash: torch.Tensor, sorted_idx: torch.Tensor) -> torch.Tensor:
+    """Per entry: the smallest entry id with equal bytes (int64), from the stably sorted (hash, entry) pairs."""
+    lib = _lib.load()
+    dev = offsets.device
+    n = int(offsets.shape[0]) - 1
+    out = torch.empty(n, dtype=torch.int64, device=dev)
+    _lib.check(lib.fb_string_first_equal(dev.index, _stream_ptr(dev), n, offsets.data_ptr(), data.data_ptr(),
+                                         0 if valid is None else valid.data_ptr(), sorted_hash.data_ptr(),
+                                         sorted_idx.data_ptr(), out.data_ptr()))
+    return out

@@ -17,7 +17,8 @@ fugue/workflow/workflow.py:2109-2166) and ``ExecutionEngine.aggregate`` reaches 
 Expressions: + - * / %, comparisons (= == != <> < <= > >=), AND / OR / NOT, IS [NOT] NULL, [NOT] IN (...),
 [NOT] BETWEEN, x [NOT] LIKE 'pattern' [ESCAPE 'c'], CAST(x AS type), CASE [x] WHEN .. THEN .. [ELSE ..] END,
 COALESCE, IFNULL, NULLIF, IF / IIF, MOD, ABS, FLOOR, CEIL / CEILING, ROUND, SQRT, EXP, LN, LOG10, POWER / POW,
-GREATEST, LEAST, LENGTH, literals, `quoted` and table-qualified names.
+GREATEST, LEAST, LENGTH, UPPER, LOWER, SUBSTR / SUBSTRING, TRIM, LTRIM, RTRIM, REPLACE, CONCAT, a || b, literals,
+`quoted` and table-qualified names.
 Anything else raises NotImplementedError (there is no host SQL fallback in this package).
 """
 import re
@@ -278,7 +279,7 @@ _TOKEN = re.compile(r"""\s*(?:
   | (?P<str>'(?:[^'\\]|\\.|'')*')
   | (?P<bq>`(?:[^`]|``)*`)
   | (?P<id>[A-Za-z_]\w*)
-  | (?P<op><=|>=|<>|!=|==|=|<|>|\+|-|\*|/|%|\(|\)|,|\.)
+  | (?P<op>\|\||<=|>=|<>|!=|==|=|<|>|\+|-|\*|/|%|\(|\)|,|\.)
 )""", re.X)
 
 _AGG_FUNCS = {"SUM": functions.sum, "COUNT": functions.count, "MIN": functions.min, "MAX": functions.max,
@@ -287,6 +288,11 @@ _CLAUSES = ("WHERE", "GROUP", "HAVING", "ORDER", "LIMIT")
 _CASE_WORDS = ("WHEN", "THEN", "ELSE", "END")  # never a column name or an implicit alias
 _ONE_ARG = {"ABS": functions.abs, "FLOOR": functions.floor, "CEIL": functions.ceil, "CEILING": functions.ceil,
             "SQRT": functions.sqrt, "EXP": functions.exp, "LN": functions.ln, "LOG10": functions.log10}
+_STRING_ARGS = {"UPPER": (1, 1), "LOWER": (1, 1), "SUBSTR": (2, 3), "SUBSTRING": (2, 3), "TRIM": (1, 2),
+                "LTRIM": (1, 2), "RTRIM": (1, 2), "REPLACE": (3, 3)}
+_STRING_BUILDERS = {"UPPER": functions.upper, "LOWER": functions.lower, "SUBSTR": functions.substr,
+                    "SUBSTRING": functions.substr, "TRIM": functions.trim, "LTRIM": functions.ltrim,
+                    "RTRIM": functions.rtrim, "REPLACE": functions.replace}
 _TWO_ARGS = {"NULLIF": functions.nullif, "IFNULL": functions.coalesce, "MOD": lambda a, b: a % b,
              "POWER": functions.power, "POW": functions.power}
 
@@ -306,7 +312,7 @@ def _tokenize(text: str, sql: str) -> List[Tuple[str, str]]:
 
 
 class _Parser:
-    """Recursive descent over the token list; precedence OR < AND < NOT < comparison < + - < * / < unary."""
+    """Recursive descent over the token list; precedence OR < AND < NOT < comparison < + - < * / < || < unary."""
 
     def __init__(self, tokens: List[Tuple[str, str]], sql: str):
         self.t = tokens
@@ -427,16 +433,23 @@ class _Parser:
                 return e
 
     def multiplicative(self) -> ColumnExpr:
-        e = self.unary()
+        e = self.concat()
         while True:
             if self.op("*"):
-                e = e * self.unary()
+                e = e * self.concat()
             elif self.op("/"):
-                e = e / self.unary()
+                e = e / self.concat()
             elif self.op("%"):
-                e = e % self.unary()
+                e = e % self.concat()
             else:
                 return e
+
+    def concat(self) -> ColumnExpr:
+        """``a || b``: tighter than ``*`` and left-associative, as in SQLite."""
+        e = self.unary()
+        while self.op("||"):
+            e = functions.concat_strict(e, self.unary())
+        return e
 
     def unary(self) -> ColumnExpr:
         if self.op("-"):
@@ -565,6 +578,14 @@ class _Parser:
             self.expect(")")
         if fn == "COALESCE":
             return functions.coalesce(*args)
+        if fn in _STRING_ARGS:
+            lo, hi = _STRING_ARGS[fn]
+            if not lo <= len(args) <= hi:
+                raise ValueError(f"{fn} takes {lo if lo == hi else f'{lo} to {hi}'} arguments, got {len(args)} in: "
+                                 f"{self.sql}")
+            return _STRING_BUILDERS[fn](*args)
+        if fn == "CONCAT":
+            return functions.concat(*args)
         want = 1 if fn in _ONE_ARG else 2 if fn in _TWO_ARGS else 3 if fn in ("IF", "IIF") else None
         if want is not None and len(args) != want:
             raise ValueError(f"{fn} takes {want} argument(s), got {len(args)} in: {self.sql}")

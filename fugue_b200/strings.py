@@ -1,4 +1,5 @@
-"""String functions on dictionary-encoded columns: ``LIKE`` and ``LENGTH``.
+"""String functions on dictionary-encoded columns: ``LIKE`` and ``LENGTH``, and the functions that build
+strings (``UPPER LOWER SUBSTR TRIM LTRIM RTRIM REPLACE CONCAT ||``).
 
 A string column is int32 codes on the device plus a dictionary (an Arrow ``string`` / ``large_string``
 array) on the host (``table.py``).  LIKE and LENGTH depend on the string alone, so they are evaluated once
@@ -9,18 +10,27 @@ The dictionary's Arrow layout (offsets widened to int64, the UTF-8 bytes, a vali
 uploaded once per dictionary object and device.  The copy hangs off the ``pa.Array`` through a weak
 reference: tables that share a dictionary object (``select``, ``rename``, filters, derived tables) share
 the copy, and it is freed with the dictionary.
+
+A string-building expression over one string column is a function of the entry too (K12, ``fb_strbuild.cu``):
+``string_chain`` reads it as the column and a chain of steps, ``evaluate`` runs the steps over the dictionary
+on the device (one measure and one write launch per step; intermediate dictionaries stay on the device),
+deduplicates the results and returns the new dictionary and the entry -> new code table the rows are mapped
+through (``FB_X_LOOKUP``).  Results are cached per (dictionary object, chain) the same way as uploads.
 """
 import weakref
-from typing import Any, Dict, List, Optional, Tuple
+from typing import Any, Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
 import pyarrow as pa
 import torch
 
 from . import kernels as K
+from .column import ColumnExpr, Kind, is_string_build, lit
 
-_CACHE: Dict[int, Tuple[Any, Dict[torch.device, "DeviceDictionary"]]] = {}
-uploads = 0  # dictionaries copied to a device so far (the cache's misses)
+_CACHE: Dict[int, Tuple[Any, Dict[Any, Any]]] = {}     # dictionary -> {device: DeviceDictionary}
+_DERIVED: Dict[int, Tuple[Any, Dict[Any, Any]]] = {}   # dictionary -> {(chain, device): StringResult}
+uploads = 0     # dictionaries copied to a device so far (the cache's misses)
+transforms = 0  # string expressions evaluated over a dictionary so far (the result cache's misses)
 
 
 class DeviceDictionary:
@@ -54,18 +64,23 @@ def _upload(d: pa.Array, device: torch.device) -> DeviceDictionary:
     return DeviceDictionary(torch.from_numpy(offs - lo).to(device), torch.from_numpy(data).to(device), valid)
 
 
-def device_dictionary(d: pa.Array, device: torch.device) -> DeviceDictionary:
-    """The device copy of dictionary ``d`` on ``device``: uploaded on first use, then cached on ``d``."""
+def _slot(cache: Dict[int, Tuple[Any, Dict[Any, Any]]], d: pa.Array) -> Dict[Any, Any]:
+    """The cache entry of dictionary object ``d``: dropped when ``d`` is freed."""
     key = id(d)
-    ent = _CACHE.get(key)
+    ent = cache.get(key)
     if ent is None or ent[0]() is not d:
         def drop(ref: Any, key: int = key) -> None:
-            if key in _CACHE and _CACHE[key][0] is ref:
-                del _CACHE[key]
+            if key in cache and cache[key][0] is ref:
+                del cache[key]
 
         ent = (weakref.ref(d, drop), {})
-        _CACHE[key] = ent
-    per_dev = ent[1]
+        cache[key] = ent
+    return ent[1]
+
+
+def device_dictionary(d: pa.Array, device: torch.device) -> DeviceDictionary:
+    """The device copy of dictionary ``d`` on ``device``: uploaded on first use, then cached on ``d``."""
+    per_dev = _slot(_CACHE, d)
     if device not in per_dev:
         per_dev[device] = _upload(d, device)
     return per_dev[device]
@@ -113,3 +128,233 @@ def length_table(d: pa.Array, device: torch.device) -> Tuple[torch.Tensor, Optio
     """Per entry of ``d``: its number of code points (int64), and the entry validity (None: no NULL)."""
     dd = device_dictionary(d, device)
     return K.string_length(dd.offsets, dd.data, dd.valid), dd.valid
+
+
+# ---- string-building functions ------------------------------------------------------------------------
+_ARITY = {"UPPER": (0, 0), "LOWER": (0, 0), "SUBSTR": (1, 2), "TRIM": (0, 1), "LTRIM": (0, 1), "RTRIM": (0, 1),
+          "REPLACE": (2, 2)}
+
+
+def _literal(fn: str, e: ColumnExpr, want: type) -> Any:
+    """The value of a literal argument: an int (no bool) or a string, or None for NULL."""
+    if e.kind != Kind.LITERAL or e.as_type is not None:
+        raise NotImplementedError(f"{fn} takes literal arguments after the string, got {e}")
+    v = e.value
+    if v is not None and (isinstance(v, bool) or not isinstance(v, want)):
+        raise ValueError(f"{fn}: {v!r} is not a {want.__name__} literal")
+    return v
+
+
+def _utf8(fn: str, v: str) -> bytes:
+    b = v.encode("utf-8")
+    if len(b) > K.STR_MAX_LITERAL:
+        raise NotImplementedError(f"{fn}: a literal of {len(b)} bytes; the device takes {K.STR_MAX_LITERAL}")
+    return b
+
+
+def _concat_parts(e: ColumnExpr) -> List[ColumnExpr]:
+    """The operands of a chain of ``||`` (no alias or cast inside), left to right."""
+    out: List[ColumnExpr] = []
+    for a in e.args:
+        if a.kind == Kind.BINARY and a.head == "||" and a.as_type is None and a.as_name == "":
+            out.extend(_concat_parts(a))
+        else:
+            out.append(a)
+    return out
+
+
+def string_chain(e: ColumnExpr, string_columns: Any) -> Tuple[str, Tuple[Any, ...]]:
+    """A string-building expression (``is_string_build``) as (its one string column, its steps), innermost
+    step first.  ``string_columns``: the names of the table's string columns.  A step is a hashable tuple:
+    ``("UPPER",)``, ``("LOWER",)``, ``("SUBSTR", start, length or None)``, ``("TRIM" / "LTRIM" / "RTRIM",
+    characters)``, ``("REPLACE", from, to)``, ``("FORMAT", tokens, null_is_empty)`` for CONCAT / ``||``, or
+    ``("NULL",)`` (a NULL literal argument: every result is NULL).  Literals are UTF-8 bytes.
+    Raises NotImplementedError for what the device does not evaluate (two different string operands, numbers
+    in a concatenation, a non-literal argument, no string column) and ValueError for a wrong argument count
+    or a literal of the wrong type."""
+
+    def operand(x: Any) -> Tuple[str, Tuple[Any, ...]]:
+        x = x if isinstance(x, ColumnExpr) else lit(x)
+        str_cast = x.as_type is None or pa.types.is_string(x.as_type) or pa.types.is_large_string(x.as_type)
+        if x.kind == Kind.NAMED and x.name in string_columns and str_cast:
+            return x.name, ()
+        if is_string_build(x) and str_cast:
+            return chain(x)
+        raise NotImplementedError(f"{e}: a string function needs a string expression over one string column, "
+                                  f"got {x}")
+
+    def chain(x: ColumnExpr) -> Tuple[str, Tuple[Any, ...]]:
+        fn = "||" if x.kind == Kind.BINARY else x.head.upper()
+        fn = "SUBSTR" if fn == "SUBSTRING" else fn
+        args = [a if isinstance(a, ColumnExpr) else lit(a) for a in x.args]
+        if fn in ("CONCAT", "||"):
+            parts = _concat_parts(x) if fn == "||" else args
+            if not parts:
+                raise ValueError(f"CONCAT needs at least one argument: {x}")
+            toks: List[int] = []
+            base: Any = None
+            null = False
+            for p in parts:
+                if p.kind == Kind.LITERAL and p.as_type is None:
+                    if p.value is None:
+                        null = True
+                    elif isinstance(p.value, str):
+                        toks.extend(p.value.encode("utf-8"))
+                    else:
+                        raise NotImplementedError(f"a number inside a concatenation: {x}")
+                    continue
+                fp = p.fingerprint()
+                if base is None:
+                    base = (fp, operand(p))
+                elif base[0] != fp:
+                    raise NotImplementedError(f"a concatenation of different string expressions (every operand "
+                                              f"that is not a literal must be the same): {x}")
+                toks.append(K.STR_SELF)
+            if base is None:
+                raise NotImplementedError(f"a concatenation of literals only (no string column): {x}")
+            if len(toks) > K.STR_MAX_TOKENS:
+                raise NotImplementedError(f"a concatenation of {len(toks)} tokens; the device takes {K.STR_MAX_TOKENS}")
+            name, steps = base[1]
+            step = ("NULL",) if (fn == "||" and null) else ("FORMAT", tuple(toks), fn == "CONCAT")
+            return name, steps + (step,)
+        if not args:
+            raise ValueError(f"{fn} needs a string argument: {x}")
+        lo, hi = _ARITY[fn]
+        rest = args[1:]
+        if not lo <= len(rest) <= hi:
+            n = f"{lo + 1}" if lo == hi else f"{lo + 1} to {hi + 1}"
+            raise ValueError(f"{fn} takes {n} arguments: {x}")
+        vals = [_literal(fn, a, int if fn == "SUBSTR" else str) for a in rest]
+        name, steps = operand(args[0])
+        if any(v is None for v in vals):
+            return name, steps + (("NULL",),)
+        if fn == "SUBSTR":
+            for v in vals:
+                if not -(1 << 62) <= v <= 1 << 62:
+                    raise NotImplementedError(f"SUBSTR: {v} is outside [-2^62, 2^62]")
+            step: Tuple[Any, ...] = ("SUBSTR", vals[0], vals[1] if len(vals) > 1 else None)
+        elif fn in ("TRIM", "LTRIM", "RTRIM"):
+            step = (fn, _utf8(fn, vals[0]) if vals else b" ")
+        elif fn == "REPLACE":
+            step = (fn, _utf8(fn, vals[0]), _utf8(fn, vals[1]))
+        else:
+            step = (fn,)
+        return name, steps + (step,)
+
+    return chain(e)
+
+
+class StringResult:
+    """A string expression evaluated over a dictionary: the new ``dictionary`` (distinct entries, in the order
+    of their first source entry), ``remap`` (int64: source entry -> new code; a per-entry table for
+    ``FB_X_LOOKUP``), ``remap_valid`` (uint8, 0 where the result is NULL; None: no NULL result) and
+    ``null_code``: the code of the result for a NULL row (None: NULL), which is not NULL only after a CONCAT."""
+
+    def __init__(self, dictionary: pa.Array, remap: torch.Tensor, remap_valid: Optional[torch.Tensor],
+                 null_code: Optional[int]):
+        self.dictionary, self.remap, self.remap_valid, self.null_code = dictionary, remap, remap_valid, null_code
+
+
+_STEP_OPS = {"UPPER": K.STR_UPPER, "LOWER": K.STR_LOWER, "SUBSTR": K.STR_SUBSTR, "TRIM": K.STR_TRIM,
+             "LTRIM": K.STR_LTRIM, "RTRIM": K.STR_RTRIM, "REPLACE": K.STR_REPLACE, "FORMAT": K.STR_FORMAT}
+
+
+def _step_args(step: Tuple[Any, ...]) -> Dict[str, Any]:
+    name = step[0]
+    if name == "SUBSTR":
+        return {"start": step[1], "length": step[2]}
+    if name in ("TRIM", "LTRIM", "RTRIM"):
+        return {"lits": [step[1]]}
+    if name == "REPLACE":
+        return {"lits": [step[1], step[2]]}
+    if name == "FORMAT":
+        return {"tokens": step[1], "null_is_empty": step[2]}
+    return {}
+
+
+def _scan(lengths: torch.Tensor) -> Tuple[torch.Tensor, int]:
+    """Offsets of outputs of ``lengths`` bytes (exclusive scan, n + 1 entries) and the total."""
+    offs = torch.zeros(int(lengths.shape[0]) + 1, dtype=torch.int64, device=lengths.device)
+    torch.cumsum(lengths, 0, out=offs[1:])
+    return offs, int(offs[-1].item())
+
+
+def apply_steps(offsets: torch.Tensor, data: torch.Tensor, valid: Optional[torch.Tensor], steps: Sequence[Any]
+                ) -> Tuple[torch.Tensor, torch.Tensor, Optional[torch.Tensor]]:
+    """The dictionary (offsets, data, validity) after ``steps``, entry for entry, on the device."""
+    for step in steps:
+        m = int(offsets.shape[0]) - 1
+        if step[0] == "NULL":
+            valid = torch.zeros(m, dtype=torch.uint8, device=offsets.device)
+            continue
+        op, kw = _STEP_OPS[step[0]], _step_args(step)
+        lengths, out_valid = K.string_transform(op, offsets, data, valid, **kw)
+        new_offsets, total = _scan(lengths)
+        new_data = torch.empty(max(total, 1), dtype=torch.uint8, device=offsets.device)
+        K.string_transform(op, offsets, data, valid, out_offsets=new_offsets, out_data=new_data, **kw)
+        offsets, data, valid = new_offsets, new_data, out_valid
+    return offsets, data, valid
+
+
+def dedup(offsets: torch.Tensor, data: torch.Tensor, valid: Optional[torch.Tensor], bits: int = 64
+          ) -> Tuple[pa.Array, torch.Tensor, Optional[torch.Tensor], DeviceDictionary]:
+    """Distinct non-NULL entries of a device dictionary, in the order of their first entry: (the new dictionary
+    as a ``pa.string()`` array, entry -> new code (int64, at least one element), its validity (None: no NULL
+    entry), the new dictionary's device copy).  Equal entries are found through a hash of ``bits`` bits, a
+    stable radix sort of the (hash, entry) pairs and a byte comparison inside each run of equal hashes."""
+    from .sort import _radix_sort_pairs
+
+    dev = offsets.device
+    m = int(offsets.shape[0]) - 1
+    if valid is not None and bool(valid.all().item()):
+        valid = None
+    ids = torch.arange(m, dtype=torch.int64, device=dev)
+    sh, si = _radix_sort_pairs(K.string_hash(offsets, data, valid, bits), ids.clone())  # sorts in place
+    canon = K.string_first_equal(offsets, data, valid, sh, si)
+    keep = canon == ids
+    if valid is not None:
+        keep &= valid.bool()
+    code = torch.cumsum(keep, 0) - 1
+    remap = code[canon] if m > 0 else torch.zeros(1, dtype=torch.int64, device=dev)
+    remap_valid = valid if m > 0 else torch.zeros(1, dtype=torch.uint8, device=dev)
+    kept = torch.nonzero(keep).squeeze(1)
+    k = int(kept.shape[0])
+    new_offsets, total = _scan(offsets[kept + 1] - offsets[kept])
+    if total > (1 << 31) - 1:
+        raise NotImplementedError(f"a string result of {total} bytes; a pa.string() dictionary holds 2^31 - 1")
+    new_data = torch.empty(max(total, 1), dtype=torch.uint8, device=dev)
+    K.string_transform(K.STR_COPY, offsets, data, None, src=kept, out_offsets=new_offsets, out_data=new_data)
+    host_offsets = new_offsets.cpu().numpy().astype(np.int32)
+    host_data = new_data[:total].cpu().numpy()
+    d = pa.Array.from_buffers(pa.string(), k, [None, pa.py_buffer(host_offsets), pa.py_buffer(host_data)])
+    return d, remap.contiguous(), remap_valid, DeviceDictionary(new_offsets, new_data, None)
+
+
+def _evaluate(d: pa.Array, device: torch.device, steps: Tuple[Any, ...]) -> StringResult:
+    global transforms
+    transforms += 1
+    dd = device_dictionary(d, device)
+    n = dd.size
+    offsets, data, valid = dd.offsets, dd.data, dd.valid
+    extra = any(s[0] == "FORMAT" and s[2] for s in steps)
+    if extra:  # one more entry, NULL: what a NULL row becomes (CONCAT skips NULL operands)
+        ones = torch.ones(n, dtype=torch.uint8, device=device)
+        offsets = torch.cat([offsets, offsets[-1:]])
+        valid = torch.cat([ones if valid is None else valid, torch.zeros(1, dtype=torch.uint8, device=device)])
+    offsets, data, valid = apply_steps(offsets, data, valid, steps)
+    new, remap, remap_valid, copy = dedup(offsets, data, valid)
+    _slot(_CACHE, new)[device] = copy  # the new dictionary's device copy: LIKE / LENGTH of it upload nothing
+    null_code = None
+    if extra and (remap_valid is None or bool(remap_valid[n].item())):
+        null_code = int(remap[n].item())
+    return StringResult(new, remap, remap_valid, null_code)
+
+
+def evaluate(d: pa.Array, device: torch.device, steps: Tuple[Any, ...]) -> StringResult:
+    """``steps`` (``string_chain``) over dictionary ``d`` on ``device``: computed on first use, then cached on
+    ``d``, so a repeated call launches nothing and returns the same ``StringResult`` (the same ``pa.Array``)."""
+    per = _slot(_DERIVED, d)
+    key = (steps, device)
+    if key not in per:
+        per[key] = _evaluate(d, device, steps)
+    return per[key]

@@ -546,6 +546,58 @@ int fb_string_length(int dev, void* stream, int64_t n, const int64_t* offsets, c
 int fb_string_like(int dev, void* stream, int64_t n, const int64_t* offsets, const uint8_t* data,
                    const uint8_t* valid, int ntokens, const int16_t* tokens, uint8_t* out, uint8_t* out_valid);
 
+/* ---------------------------------------------------------------------------
+ * K12 string-building functions, evaluated once per dictionary entry
+ * Replaces: the SQL engine's UPPER / LOWER / SUBSTR / TRIM / REPLACE / CONCAT / || on a string column
+ *           (one Python string per row in qpd / pandas).
+ * Dictionaries have the K11 layout.  A function of one string column is a function of its entry, so the
+ * host builds a new dictionary from the old one and maps every row's code through an entry -> new code table
+ * (K8: FB_X_MOV, FB_X_LOOKUP).
+ *
+ * fb_string_transform : one op over n outputs; output i reads entry src[i] (src: DEVICE int64, NULL: entry i).
+ *   Measure call (out_data == NULL): out_len[i] = the output's byte length (0 when NULL), out_valid[i] = 1
+ *   unless the output is NULL.  Write call: the bytes of output i go to out_data + out_offsets[i] (the host's
+ *   exclusive scan of out_len); out_len / out_valid are not read.  A NULL entry gives NULL except in
+ *   FB_STR_FORMAT with null_is_empty.  Ops (code points are UTF-8 sequences; other bytes pass unchanged):
+ *     FB_STR_COPY    the entry (a gather, with src)
+ *     FB_STR_UPPER / FB_STR_LOWER  simple case mapping, one code point to one (fb_casemap.inc, pyarrow's
+ *                    utf8_upper / utf8_lower)
+ *     FB_STR_SUBSTR  SQLite substr(s, start[, length]) in code points (has_length == 0: no length); start and
+ *                    length in [-2^62, 2^62]
+ *     FB_STR_LTRIM / FB_STR_RTRIM / FB_STR_TRIM  remove the code points of literal 0 from the start / end / both
+ *     FB_STR_REPLACE every non-overlapping match of literal 0, left to right, by literal 1; an empty literal 0
+ *                    leaves the entry unchanged
+ *     FB_STR_FORMAT  the tokens in order: a literal byte 0..255, or FB_STR_SELF for the entry's bytes.  A NULL
+ *                    entry gives NULL (||), or with null_is_empty adds no bytes (CONCAT)
+ *   Literals (at most FB_STR_MAX_LITERAL bytes each) and tokens (at most FB_STR_MAX_TOKENS) are HOST arrays,
+ *   copied into the launch.
+ * fb_string_hash        : out[i] = a 64-bit hash of entry i's bytes, keeping the low `bits` (1..64); 0 for a
+ *                         NULL entry.
+ * fb_string_first_equal : given the (hash, entry) pairs sorted by unsigned hash, stably (sorted_hash,
+ *                         sorted_idx; the entries 0..n-1 before the sort), canon[e] = the smallest entry id
+ *                         whose bytes equal entry e's (NULL entries are equal to each other only).  It finds
+ *                         the start of e's hash run by binary search and compares forward from there: one
+ *                         comparison per entry unless hashes collide.
+ * One thread per entry, grid-stride; UPPER / LOWER stage their table (about 12 KB) in shared memory.
+ * --------------------------------------------------------------------------- */
+#define FB_STR_MAX_LITERAL 256
+#define FB_STR_MAX_TOKENS 1024
+#define FB_STR_SELF 256
+enum fb_str_op {
+  FB_STR_COPY = 0, FB_STR_UPPER = 1, FB_STR_LOWER = 2, FB_STR_SUBSTR = 3, FB_STR_LTRIM = 4, FB_STR_RTRIM = 5,
+  FB_STR_TRIM = 6, FB_STR_REPLACE = 7, FB_STR_FORMAT = 8
+};
+int fb_string_transform(int dev, void* stream, int op, int64_t n, const int64_t* offsets, const uint8_t* data,
+                        const uint8_t* valid, const int64_t* src, int64_t start, int64_t length, int has_length,
+                        int nlit0, const uint8_t* lit0, int nlit1, const uint8_t* lit1, int ntokens,
+                        const int16_t* tokens, int null_is_empty, int64_t* out_len, uint8_t* out_valid,
+                        const int64_t* out_offsets, uint8_t* out_data);
+int fb_string_hash(int dev, void* stream, int64_t n, const int64_t* offsets, const uint8_t* data,
+                   const uint8_t* valid, int bits, uint64_t* out);
+int fb_string_first_equal(int dev, void* stream, int64_t n, const int64_t* offsets, const uint8_t* data,
+                          const uint8_t* valid, const uint64_t* sorted_hash, const int64_t* sorted_idx,
+                          int64_t* canon);
+
 #ifdef __cplusplus
 }
 #endif

@@ -28,7 +28,7 @@ import pyarrow as pa
 import torch
 
 from . import kernels as K
-from .column import PERCENTILES, ColumnExpr, Kind, SelectColumns, col as _col, has_window, is_agg
+from .column import PERCENTILES, VARIANCES, ColumnExpr, Kind, SelectColumns, col as _col, has_window, is_agg
 from .table import B200Table, narrow, widen
 
 
@@ -230,6 +230,7 @@ def _with_windows(t: B200Table, cols: List[ColumnExpr]) -> B200Table:
     # ---- scans: collected first, all run in one call per frame (None: the running scan)
     scans: Dict[Any, List[Any]] = {}
     quantiles: Dict[str, List[Tuple[float, int]]] = {}  # argument column -> its (q, CONT | DISC) pairs
+    moments: Dict[str, int] = {}  # argument column of a variance -> its column of the moments scan
     finish: List[Any] = []     # per node: (fingerprint, fn(scan results) -> (column, validity, type, dictionary))
 
     def scan(op: int, v: Any, m: Any, frame: Any = None) -> Tuple[Any, int]:
@@ -302,6 +303,18 @@ def _with_windows(t: B200Table, cols: List[ColumnExpr]) -> B200Table:
             finish.append((uid, extreme_string))
             continue
         is_f = pa.types.is_floating(tp)
+        if fn in VARIANCES:  # the moments scan; frames are rejected by over()
+            if not (pa.types.is_integer(tp) or is_f):
+                raise NotImplementedError(f"{fn} needs an integer or float column; {name} is {tp}")
+            j = moments.setdefault(name, len(moments))
+
+            def variance(r: Any, j: int = j, e: Any = at_end, fn: str = fn) -> Any:
+                cnt, m2 = r[("moments", j)]
+                v, vv = variance_of(fn, e(m2), e(cnt))
+                return v, vv, pa.float64(), None
+
+            finish.append((uid, variance))
+            continue
         if fn in ("SUM", "AVG"):
             f64 = fn == "AVG" or is_f
             v8 = widen(c, tp)
@@ -361,6 +374,13 @@ def _with_windows(t: B200Table, cols: List[ColumnExpr]) -> B200Table:
         results.update(((frame, j), r) for j, r in enumerate(res))
     for name, qs in quantiles.items():
         results[("quantile", name)] = K.segmented_quantile(off.contiguous(), *quantile_input(base, name), qs)
+    if moments:
+        mcols = []
+        for name in moments:
+            i = base.schema.index_of_key(name)
+            v = widen(base.columns[i], base.schema.types[i])
+            mcols.append(((v if v.dtype == torch.float64 else v.to(torch.float64)).contiguous(), base.valid[i]))
+        results.update((("moments", j), r) for j, r in enumerate(K.segmented_moments(off.contiguous(), n, mcols)))
     names, types, columns, valid = list(base.schema.names), list(base.schema.types), list(base.columns), list(base.valid)
     dicts = dict(base.dictionaries)
     window_names: Dict[str, str] = {}
@@ -377,6 +397,17 @@ def _with_windows(t: B200Table, cols: List[ColumnExpr]) -> B200Table:
     out = _WindowTable(Schema([pa.field(a, b) for a, b in zip(names, types)]), columns, valid, dicts)
     out.window_names = window_names
     return out
+
+
+def variance_of(fn: str, m2: torch.Tensor, count: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+    """``fn`` (a ``VARIANCES`` head) from M2 and the non-NULL count m: (float64 values, validity).  The sample
+    forms divide by m - 1 and are NULL when m < 2, the population forms divide by m and are NULL when m = 0."""
+    samp = fn in ("VAR_SAMP", "STDDEV_SAMP")
+    has = count > (1 if samp else 0)
+    v = m2 / torch.where(has, count - (1 if samp else 0), torch.ones_like(count)).to(torch.float64)
+    if fn.startswith("STDDEV"):
+        v = torch.sqrt(v)
+    return torch.where(has, v, torch.zeros_like(v)).contiguous(), has.to(torch.uint8)
 
 
 def quantile_input(t: B200Table, name: str) -> Tuple[torch.Tensor, Optional[torch.Tensor], int]:

@@ -11,10 +11,11 @@ from an expression is a function of ``(kind, head, args)``:
               ``NULLIF ABS FLOOR CEIL SQRT EXP LN LOG10 POWER GREATEST LEAST``; ``ROUND``: args (x, digits literal)
               ``UPPER LOWER``: args (string,); ``SUBSTR``: args (string, start[, length]); ``TRIM LTRIM RTRIM``:
               args (string[, characters]); ``REPLACE``: args (string, from, to); ``CONCAT``: args (part, ...)
-    AGG       head in ``SUM COUNT AVG MIN MAX FIRST LAST``, one arg, optional DISTINCT, or ``PERCENTILE_CONT
-              PERCENTILE_DISC``, one arg and kwarg ``q`` (MEDIAN is PERCENTILE_CONT at q = 0.5)
+    AGG       head in ``SUM COUNT AVG MIN MAX FIRST LAST VAR_SAMP VAR_POP STDDEV_SAMP STDDEV_POP``, one arg,
+              optional DISTINCT, or ``PERCENTILE_CONT PERCENTILE_DISC``, one arg and kwarg ``q`` (MEDIAN is
+              PERCENTILE_CONT at q = 0.5)
     WINDOW    head in the AGG functions (one arg, kwargs ``running``, ``rows`` or ``range``; a percentile keeps
-              its ``q`` and covers the whole partition), ``ROW_NUMBER RANK
+              its ``q`` and covers the whole partition; a variance takes ``running`` only), ``ROW_NUMBER RANK
               DENSE_RANK`` (no arg) or ``LAG LEAD`` (one arg, kwargs ``n`` and ``default``): evaluated over the logical
               partitions of ``fa.transform`` (PartitionSpec keys, presort order) by a ``ColumnMap``
 
@@ -56,6 +57,9 @@ ARITH_OPS = frozenset(["+", "-", "*", "/", "%"])
 AGG_KEEPS_ARG_TYPE = frozenset(["MIN", "MAX", "FIRST", "LAST"])
 WINDOW_AGGS = frozenset(["SUM", "COUNT", "AVG", "MIN", "MAX", "FIRST", "LAST"])
 PERCENTILES = frozenset(["PERCENTILE_CONT", "PERCENTILE_DISC"])
+# sample / population variance and standard deviation (float64); STDDEV and VARIANCE name the sample forms
+VARIANCES = frozenset(["VAR_SAMP", "VAR_POP", "STDDEV_SAMP", "STDDEV_POP"])
+_AGG_ALIASES = {"STDDEV": "STDDEV_SAMP", "VARIANCE": "VAR_SAMP"}
 _RANKINGS = frozenset(["ROW_NUMBER", "RANK", "DENSE_RANK"])
 _RUNNING_FRAME = "ROWS BETWEEN UNBOUNDED PRECEDING AND CURRENT ROW"
 _LITERAL_TYPES = (int, bool, float, str)
@@ -221,6 +225,8 @@ class ColumnExpr:
             return pa.string()
         if k in (Kind.AGG, Kind.WINDOW) and self.head in PERCENTILES:
             return pa.float64() if self.head == "PERCENTILE_CONT" else self.args[0].infer_type(schema)
+        if k in (Kind.AGG, Kind.WINDOW) and self.head in VARIANCES:
+            return pa.float64()
         if k == Kind.WINDOW:
             if self.head in _RANKINGS or self.head == "COUNT":
                 return pa.int64()
@@ -314,7 +320,7 @@ class ColumnExpr:
             raise ValueError(f"{self} is not an aggregation: only an aggregation has an OVER form")
         if self.is_distinct:
             raise ValueError(f"{self}: DISTINCT aggregations have no window form")
-        if self.head not in WINDOW_AGGS and self.head not in PERCENTILES:
+        if self.head not in WINDOW_AGGS and self.head not in PERCENTILES and self.head not in VARIANCES:
             raise ValueError(f"{self}: {self.head} has no window form")
         if not isinstance(running, bool):
             raise ValueError(f"running must be a bool, got {running!r}")
@@ -342,6 +348,9 @@ class ColumnExpr:
                 running, rows = True, None
             elif rows == (None, None):
                 rows = None
+        if self.head in VARIANCES and (rows is not None or range is not None):
+            raise NotImplementedError(f"{self}: {self.head} runs over the whole partition or running=True; "
+                                      "ROWS and RANGE frames are not supported")
         if is_agg(self.args[0]) or has_window(self.args[0]):
             raise ValueError(f"nested aggregation {self}")
         if self.head in ("FIRST", "LAST") and self.args[0].kind == Kind.WILDCARD:
@@ -417,8 +426,10 @@ def function(name: str, *args: Any, arg_distinct: bool = False, **kwargs: Any) -
 
 
 def agg(func: str, arg: Any, as_name: str = "", arg_distinct: bool = False) -> ColumnExpr:
-    """``FUNC([DISTINCT] arg)``: SUM / COUNT / AVG / MIN / MAX / FIRST / LAST."""
-    return ColumnExpr(Kind.AGG, func.upper(), [col(arg)], None, arg_distinct, as_name)
+    """``FUNC([DISTINCT] arg)``: SUM / COUNT / AVG / MIN / MAX / FIRST / LAST / VAR_SAMP / VAR_POP / STDDEV_SAMP /
+    STDDEV_POP (STDDEV and VARIANCE give the sample forms)."""
+    func = func.upper()
+    return ColumnExpr(Kind.AGG, _AGG_ALIASES.get(func, func), [col(arg)], None, arg_distinct, as_name)
 
 
 def _percentile(func: str, c: Any, q: Any) -> ColumnExpr:
@@ -781,6 +792,30 @@ class functions:
 
     mean = avg
     is_agg = staticmethod(is_agg)
+
+    @staticmethod
+    def var_samp(c: Any) -> ColumnExpr:
+        """Sample variance M2 / (m - 1) of the m non-NULL values (float64; NULL when m < 2)."""
+        return agg("VAR_SAMP", c)
+
+    variance = var_samp
+
+    @staticmethod
+    def var_pop(c: Any) -> ColumnExpr:
+        """Population variance M2 / m of the m non-NULL values (float64; NULL when m = 0)."""
+        return agg("VAR_POP", c)
+
+    @staticmethod
+    def stddev_samp(c: Any) -> ColumnExpr:
+        """sqrt(VAR_SAMP): pandas ``std()`` (ddof = 1)."""
+        return agg("STDDEV_SAMP", c)
+
+    stddev = stddev_samp
+
+    @staticmethod
+    def stddev_pop(c: Any) -> ColumnExpr:
+        """sqrt(VAR_POP): pandas ``std(ddof=0)``."""
+        return agg("STDDEV_POP", c)
 
     @staticmethod
     def percentile_cont(c: Any, q: Any) -> ColumnExpr:

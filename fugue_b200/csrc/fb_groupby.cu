@@ -20,6 +20,12 @@
 // cost one CAS per warp instead of 32.
 // Algorithmic bytes: 8 (key) + 8 per value column per row; the table traffic is random-access
 // (one 32 B sector per row when the table exceeds L2).
+//
+// Variance (FB_AGG_DEV_F64 / FB_AGG_DEV2_F64, DESIGN §7i): pass A (the kernels above, which leave these
+// accumulators at 0) completes SUM and COUNT of every group; pass B (fb_groupby_dev_kernel) reads the rows
+// again, finds each row's slot without inserting, and adds d = x - SUM / COUNT and d^2.  The host forms
+// M2 = DEV2 - DEV^2 / m: Chan, Golub & LeVeque's corrected two-pass, whose correction term cancels the
+// first-order error of the atomically summed mean.
 #include "fb_common.cuh"
 
 namespace {
@@ -35,6 +41,8 @@ enum : int32_t {
   kMaxI64 = FB_AGG_MAX_I64,
   kMinF64 = FB_AGG_MIN_F64,
   kMaxF64 = FB_AGG_MAX_F64,
+  kDevF64 = FB_AGG_DEV_F64,
+  kDev2F64 = FB_AGG_DEV2_F64,
 };
 
 struct AggSpec {
@@ -42,6 +50,19 @@ struct AggSpec {
   const uint8_t* valid[FB_MAX_AGGS];  // byte mask or NULL
   int32_t op[FB_MAX_AGGS];
   int32_t naggs;
+};
+
+// pass B: one entry per value column with deviations; a column also needs its SUM and COUNT, so at most
+// FB_MAX_AGGS / 3 columns fit in one call
+constexpr int kMaxDevCols = FB_MAX_AGGS / 3;
+struct DevCol {
+  const double* val;
+  const uint8_t* valid;
+  int32_t sum, cnt, dev, dev2;  // accumulator indices; dev / dev2 = -1 when not asked for
+};
+struct DevSpec {
+  DevCol col[kMaxDevCols];
+  int32_t ncols;
 };
 
 __host__ __device__ inline int slot_words(int naggs) { return (1 + naggs + 3) & ~3; }
@@ -310,6 +331,96 @@ void launch_lean(const uint64_t* keys, const uint8_t* key_valid, int64_t nrows, 
                                                      region_shift);
 }
 
+// ---------------------------------------------------------------------------------------------------
+// Pass B of the variance: the slot of `key` as pass A placed it, without inserting; -1 when absent (only after
+// an overflow, which the host retries).  kLean: fb_groupby_lean_kernel's layout (region = the partitioner hash's
+// low bits, slot from its bits 10..); otherwise find_or_insert's (region_shift < 0: the whole table).
+// ---------------------------------------------------------------------------------------------------
+template <bool kLean>
+__device__ __forceinline__ int64_t find_slot(const uint64_t* __restrict__ table, int words, int64_t mask,
+                                             uint64_t key, const FbDiv& dv, int64_t region_shift,
+                                             uint32_t parts_mask) {
+  int64_t base = 0, s;
+  if (kLean) {
+    const uint64_t h = fb_hash_single_u64(key);
+    base = (int64_t)((uint32_t)h & parts_mask) << region_shift;
+    s = (int64_t)((uint32_t)(h >> 10) & (uint32_t)mask);
+  } else {
+    uint64_t h = fb_fmix64(key);
+    if (region_shift >= 0) {
+      base = (int64_t)fb_fastmod(fb_hash_single_u64(key), dv) << region_shift;
+      h >>= 7;
+    }
+    s = (int64_t)(h & (uint64_t)mask);
+  }
+#pragma unroll 1
+  for (int probe = 0; probe < kMaxProbe; ++probe) {
+    const uint64_t cur = table[(base + s) * words];
+    if (cur == key) return base + s;
+    if (cur == kEmpty) return -1;
+    s = (s + 1) & mask;
+  }
+  return -1;
+}
+
+// Rows as fb_groupby_kernel walks them (part_off != nullptr: the rows of hash partitions [p0, p1)); per valid
+// value x of a deviation column, d = x - SUM / COUNT of the row's group is added into DEV and d * d into DEV2.
+template <bool kLean>
+__global__ void __launch_bounds__(256)
+fb_groupby_dev_kernel(const uint64_t* __restrict__ keys, const uint8_t* __restrict__ key_valid, int64_t nrows,
+                      uint64_t* __restrict__ table, int64_t capacity, int words, const DevSpec spec, FbDiv dv,
+                      int64_t region_shift, uint32_t parts_mask, const int64_t* __restrict__ part_off, int p0,
+                      int p1) {
+  const int64_t mask = region_shift >= 0 ? (((int64_t)1 << region_shift) - 1) : capacity - 1;
+  const unsigned lane = threadIdx.x & 31;
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  const int64_t row_lo = part_off != nullptr ? part_off[p0] : 0;
+  const int64_t row_hi = part_off != nullptr ? part_off[p1] : nrows;
+  const int64_t nround = (row_hi - row_lo + stride - 1) / stride;
+  for (int64_t it = 0; it < nround; ++it) {
+    const int64_t row = row_lo + it * stride + (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const bool ok = row < row_hi;
+    uint64_t key = 0;
+    int64_t s = -1;
+    bool special = false;
+    if (ok) {
+      key = keys[row];
+      if (key_valid != nullptr && key_valid[row] == 0) { s = capacity + 1; special = true; }  // NULL group
+      else if (key == kEmpty) { s = capacity; special = true; }                             // EMPTY-valued key
+    }
+    // the warp pre-merge of pass A: one read-only probe per distinct key per warp
+    const bool need = ok && !special;
+    const unsigned need_mask = __ballot_sync(0xFFFFFFFFu, need);
+    unsigned peers = need_mask;
+    if (need) {
+      const uint32_t h = (uint32_t)(fb_fmix64(key) >> 20);
+#pragma unroll
+      for (int b = 0; b < 6; ++b) {
+        const bool bit = (h >> b) & 1u;
+        const unsigned bal = __ballot_sync(need_mask, bit);
+        peers &= bit ? bal : ~bal;
+      }
+    }
+    const int leader = need ? (__ffs(peers) - 1) : (int)lane;
+    const uint64_t lkey = __shfl_sync(0xFFFFFFFFu, key, leader);
+    const bool follow = need && leader != (int)lane && lkey == key;
+    if (need && !follow) s = find_slot<kLean>(table, words, mask, key, dv, region_shift, parts_mask);
+    const int64_t ls = __shfl_sync(0xFFFFFFFFu, s, leader);
+    if (follow) s = ls;
+    if (!ok || s < 0) continue;
+    uint64_t* slot = table + s * words;
+#pragma unroll 1
+    for (int c = 0; c < spec.ncols; ++c) {
+      const DevCol& d = spec.col[c];
+      if (d.valid != nullptr && d.valid[row] == 0) continue;  // NULL value: skipped
+      const double mean = __longlong_as_double((long long)slot[1 + d.sum]) / (double)(long long)slot[1 + d.cnt];
+      const double dx = d.val[row] - mean;
+      if (d.dev >= 0) atomicAdd((double*)(slot + 1 + d.dev), dx);
+      if (d.dev2 >= 0) atomicAdd((double*)(slot + 1 + d.dev2), dx * dx);
+    }
+  }
+}
+
 __global__ void __launch_bounds__(256)
 fb_groupby_extract_kernel(const uint64_t* __restrict__ table, int64_t capacity, int words, AggSpec spec,
                           uint64_t* __restrict__ out_keys, uint8_t* __restrict__ out_key_valid,
@@ -342,18 +453,38 @@ fb_groupby_extract_kernel(const uint64_t* __restrict__ table, int64_t capacity, 
   }
 }
 
-int fill_spec(AggSpec& spec, int naggs, const void* const* val_ptrs, const uint8_t* const* val_valid,
+// also resolves every FB_AGG_DEV_F64 / FB_AGG_DEV2_F64 to the SUM and COUNT of its column (pass B's DevSpec)
+int fill_spec(AggSpec& spec, DevSpec& dev, int naggs, const void* const* val_ptrs, const uint8_t* const* val_valid,
               const int32_t* ops) {
   FB_CHECK(naggs >= 0 && naggs <= FB_MAX_AGGS, "naggs=%d out of range [0,%d]", naggs, FB_MAX_AGGS);
   memset(&spec, 0, sizeof(spec));
+  memset(&dev, 0, sizeof(dev));
   spec.naggs = naggs;
   for (int a = 0; a < naggs; ++a) {
-    FB_CHECK(ops[a] >= FB_AGG_SUM_F64 && ops[a] <= FB_AGG_MAX_F64, "unknown aggregate op %d", ops[a]);
+    FB_CHECK(ops[a] >= FB_AGG_SUM_F64 && ops[a] <= FB_AGG_DEV2_F64, "unknown aggregate op %d", ops[a]);
     FB_CHECK(ops[a] == FB_AGG_COUNT || (val_ptrs != nullptr && val_ptrs[a] != nullptr),
              "aggregate %d needs a value column", a);
     spec.op[a] = ops[a];
     spec.val[a] = val_ptrs ? (const uint64_t*)val_ptrs[a] : nullptr;
     spec.valid[a] = val_valid ? val_valid[a] : nullptr;
+  }
+  for (int a = 0; a < naggs; ++a) {
+    if (ops[a] != kDevF64 && ops[a] != kDev2F64) continue;
+    int sum = -1, cnt = -1;
+    for (int b = 0; b < naggs; ++b) {
+      if (sum < 0 && ops[b] == kSumF64 && spec.val[b] == spec.val[a] && spec.valid[b] == spec.valid[a]) sum = b;
+      if (cnt < 0 && ops[b] == kCount && spec.valid[b] == spec.valid[a]) cnt = b;
+    }
+    FB_CHECK(sum >= 0 && cnt >= 0, "aggregate %d (op %d) needs a SUM_F64 and a COUNT of the same column and validity",
+             a, ops[a]);
+    int c = 0;
+    while (c < dev.ncols && !(dev.col[c].val == (const double*)spec.val[a] && dev.col[c].valid == spec.valid[a])) ++c;
+    if (c == dev.ncols) {
+      FB_CHECK(c < kMaxDevCols, "more than %d value columns with deviations", kMaxDevCols);
+      dev.col[c] = DevCol{(const double*)spec.val[a], spec.valid[a], sum, cnt, -1, -1};
+      ++dev.ncols;
+    }
+    (ops[a] == kDevF64 ? dev.col[c].dev : dev.col[c].dev2) = a;
   }
   return 0;
 }
@@ -377,7 +508,8 @@ int fb_groupby_u64(int dev, void* stream, int64_t nrows, const void* keys, const
   FbDeviceGuard guard(dev);
   FB_CHECK(guard.ok, "cannot select device %d", dev);
   AggSpec spec;
-  if (int rc = fill_spec(spec, naggs, val_ptrs, val_valid, agg_ops)) return rc;
+  DevSpec devs;
+  if (int rc = fill_spec(spec, devs, naggs, val_ptrs, val_valid, agg_ops)) return rc;
   int64_t region_shift = -1;
   if (num_parts > 1) {
     FB_CHECK((num_parts & (num_parts - 1)) == 0 && (int64_t)num_parts * 2 <= capacity,
@@ -412,6 +544,10 @@ int fb_groupby_u64(int dev, void* stream, int64_t nrows, const void* keys, const
       fb_groupby_kernel<<<(unsigned)gb, 256, 0, st>>>((const uint64_t*)keys, key_valid, nrows, (uint64_t*)table,
                                                      capacity, words, spec, d_status, dv, region_shift,
                                                      d_part_offsets, (int)p0, (int)p1);
+      if (devs.ncols > 0)  // pass B of the batch while its regions are still in L2
+        fb_groupby_dev_kernel<false><<<(unsigned)gb, 256, 0, st>>>((const uint64_t*)keys, key_valid, nrows,
+                                                                  (uint64_t*)table, capacity, words, devs, dv,
+                                                                  region_shift, 0u, d_part_offsets, (int)p0, (int)p1);
     }
     FB_CUDA(cudaGetLastError());
     return 0;
@@ -430,12 +566,18 @@ int fb_groupby_u64(int dev, void* stream, int64_t nrows, const void* keys, const
       case 3: launch_lean<3>(k64, key_valid, nrows, t64, capacity, spec, d_status, num_parts, (int)region_shift, sms * 8, st); break;
       default: launch_lean<4>(k64, key_valid, nrows, t64, capacity, spec, d_status, num_parts, (int)region_shift, sms * 8, st); break;
     }
+    if (devs.ncols > 0)
+      fb_groupby_dev_kernel<true><<<sms * 8, 256, 0, st>>>(k64, key_valid, nrows, t64, capacity, words, devs, dv,
+                                                          region_shift, num_parts - 1, nullptr, 0, 0);
     FB_CUDA(cudaGetLastError());
     return 0;
   }
   if (nrows > 0) {
     fb_groupby_kernel<<<sms * 8, 256, 0, st>>>((const uint64_t*)keys, key_valid, nrows, (uint64_t*)table,
                                               capacity, words, spec, d_status, dv, region_shift, nullptr, 0, 0);
+    if (devs.ncols > 0)
+      fb_groupby_dev_kernel<false><<<sms * 8, 256, 0, st>>>((const uint64_t*)keys, key_valid, nrows, (uint64_t*)table,
+                                                           capacity, words, devs, dv, region_shift, 0u, nullptr, 0, 0);
     FB_CUDA(cudaGetLastError());
   }
   return 0;

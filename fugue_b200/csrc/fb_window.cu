@@ -114,22 +114,51 @@ __device__ __forceinline__ St shfl_down(const St& s, int d) {
   return r;
 }
 
+// (count, mean, M2, "a segment starts in here") of the valid values of a run of consecutive rows: the state of
+// fb_segmented_moments
+struct MSt {
+  int64_t c;
+  double mean, m2;
+  int32_t f;
+};
+
+// `a` followed by `b`: Chan, Golub & LeVeque's pairwise update; a run without a valid row takes no part
+__device__ __forceinline__ MSt combine(int, const MSt& a, const MSt& b) {
+  if (b.f) return b;
+  if (b.c == 0) return MSt{a.c, a.mean, a.m2, a.f};
+  if (a.c == 0) return MSt{b.c, b.mean, b.m2, a.f};
+  const int64_t n = a.c + b.c;
+  const double delta = b.mean - a.mean;
+  const double wb = (double)b.c * __drcp_rn((double)n);  // nb / n within 2 u; a division call spilled
+  return MSt{n, a.mean + delta * wb, a.m2 + b.m2 + delta * delta * (double)a.c * wb, a.f};
+}
+
+__device__ __forceinline__ MSt shfl_up(const MSt& s, int d) {
+  return MSt{(int64_t)__shfl_up_sync(0xFFFFFFFFu, (long long)s.c, d), __shfl_up_sync(0xFFFFFFFFu, s.mean, d),
+             __shfl_up_sync(0xFFFFFFFFu, s.m2, d), __shfl_up_sync(0xFFFFFFFFu, s.f, d)};
+}
+
+__device__ __forceinline__ MSt shfl_down(const MSt& s, int d) {
+  return MSt{(int64_t)__shfl_down_sync(0xFFFFFFFFu, (long long)s.c, d), __shfl_down_sync(0xFFFFFFFFu, s.mean, d),
+             __shfl_down_sync(0xFFFFFFFFu, s.m2, d), __shfl_down_sync(0xFFFFFFFFu, s.f, d)};
+}
+
 // Exclusive scan of one state per thread across the CTA, and the CTA total; fixed combination order.
-// kRev: the scan runs from the last thread to the first.
-template <int kWarps, bool kRev = false>
-__device__ __forceinline__ St block_exclusive(int op, const St& x, St* warp_tot, St* total) {
+// kRev: the scan runs from the last thread to the first.  S: St, or MSt (op unused).
+template <int kWarps, bool kRev = false, class S = St>
+__device__ __forceinline__ S block_exclusive(int op, const S& x, S* warp_tot, S* total) {
   const int lane = kRev ? 31 - (threadIdx.x & 31) : threadIdx.x & 31;
   const int w = kRev ? kWarps - 1 - (int)(threadIdx.x >> 5) : threadIdx.x >> 5;
-  St inc = x;
+  S inc = x;
 #pragma unroll
   for (int d = 1; d < 32; d <<= 1) {
-    const St o = kRev ? shfl_down(inc, d) : shfl_up(inc, d);
+    const S o = kRev ? shfl_down(inc, d) : shfl_up(inc, d);
     if (lane >= d) inc = combine(op, o, inc);
   }
-  const St ex = kRev ? shfl_down(inc, 1) : shfl_up(inc, 1);
+  const S ex = kRev ? shfl_down(inc, 1) : shfl_up(inc, 1);
   if (lane == 31) warp_tot[w] = inc;
   __syncthreads();
-  St pre{0, 0, 0}, tot{0, 0, 0};
+  S pre{}, tot{};
   for (int i = 0; i < kWarps; ++i) {
     if (i == w) pre = tot;
     tot = combine(op, tot, warp_tot[i]);
@@ -174,6 +203,38 @@ struct TileSmem {
   int64_t seg_range[2];
 };
 
+// Marks head[p - start] for every position p in [start, end) where a run restarts (see fb_segscan_tile_kernel);
+// seg_range is two int64 of shared memory.  The caller synchronises before reading head.
+template <bool kReverse, bool kBlocks>
+__device__ __forceinline__ void mark_heads(int64_t nrows, int64_t nseg, const int64_t* __restrict__ offsets,
+                                           int64_t start, int64_t end, int64_t block, uint8_t* head,
+                                           int64_t* seg_range) {
+  // ---- segment heads inside [start, end): offsets[s] for s in [segment of `start`, first offset >= end);
+  // reversed, offsets o in [nrows - end + 1, nrows - start] (row o - 1 ends a segment) at position nrows - o
+  for (int i = threadIdx.x; i < kTile; i += kThreads) head[i] = 0;
+  if (threadIdx.x == 0) {
+    if (kReverse) {
+      seg_range[0] = upper_bound(offsets, nseg + 1, nrows - end);
+      seg_range[1] = upper_bound(offsets, nseg + 1, nrows - start);
+    } else {
+      const int64_t s0 = upper_bound(offsets, nseg + 1, start) - 1;
+      seg_range[0] = s0 < 0 ? 0 : s0;
+      seg_range[1] = lower_bound(offsets, nseg + 1, end);
+    }
+  }
+  __syncthreads();
+  for (int64_t s = seg_range[0] + threadIdx.x; s < seg_range[1]; s += kThreads) {
+    const int64_t o = __ldg(offsets + s);
+    const int64_t p = kReverse ? nrows - o : o;
+    if (p >= start && p < end) head[p - start] = 1;
+  }
+  if (kBlocks) {  // multiples m of `block` with position (m, or nrows - m reversed) inside the tile
+    const int64_t lo = kReverse ? nrows - end + 1 : start, hi = kReverse ? nrows - start : end - 1;
+    for (int64_t m = first_multiple(lo, block) + threadIdx.x * block; m <= hi; m += kThreads * block)
+      head[(kReverse ? nrows - m : m) - start] = 1;
+  }
+}
+
 // kFinal = false: pass 1 (tile aggregates); true: pass 3 (outputs, from the carries of pass 2).
 // The scan runs over positions p; position p is row p, or row nrows - 1 - p when kReverse (then a run
 // restarts after every segment's last row).  block > 0 also restarts the runs at every row that is a
@@ -192,30 +253,7 @@ fb_segscan_tile_kernel(int64_t nrows, int64_t nseg, const int64_t* __restrict__ 
   // row of the tile's position i
   const int64_t row0 = kReverse ? nrows - 1 - start : start;
   auto row = [row0](int i) -> int64_t { return kReverse ? row0 - i : row0 + i; };
-  // ---- segment heads inside [start, end): offsets[s] for s in [segment of `start`, first offset >= end);
-  // reversed, offsets o in [nrows - end + 1, nrows - start] (row o - 1 ends a segment) at position nrows - o
-  for (int i = threadIdx.x; i < kTile; i += kThreads) sm.head[i] = 0;
-  if (threadIdx.x == 0) {
-    if (kReverse) {
-      sm.seg_range[0] = upper_bound(offsets, nseg + 1, nrows - end);
-      sm.seg_range[1] = upper_bound(offsets, nseg + 1, nrows - start);
-    } else {
-      const int64_t s0 = upper_bound(offsets, nseg + 1, start) - 1;
-      sm.seg_range[0] = s0 < 0 ? 0 : s0;
-      sm.seg_range[1] = lower_bound(offsets, nseg + 1, end);
-    }
-  }
-  __syncthreads();
-  for (int64_t s = sm.seg_range[0] + threadIdx.x; s < sm.seg_range[1]; s += kThreads) {
-    const int64_t o = __ldg(offsets + s);
-    const int64_t p = kReverse ? nrows - o : o;
-    if (p >= start && p < end) sm.head[p - start] = 1;
-  }
-  if (kBlocks) {  // multiples m of `block` with position (m, or nrows - m reversed) inside the tile
-    const int64_t lo = kReverse ? nrows - end + 1 : start, hi = kReverse ? nrows - start : end - 1;
-    for (int64_t m = first_multiple(lo, block) + threadIdx.x * block; m <= hi; m += kThreads * block)
-      sm.head[(kReverse ? nrows - m : m) - start] = 1;
-  }
+  mark_heads<kReverse, kBlocks>(nrows, nseg, offsets, start, end, block, sm.head, sm.seg_range);
   const int j0 = threadIdx.x * kItems;
   for (int col = 0; col < a.ncols; ++col) {
     const int op = a.op[col];
@@ -289,6 +327,112 @@ fb_segscan_carry_kernel(int64_t ntiles, const __grid_constant__ ScanCols a, uint
     tv[t] = run.v;
     tc[t] = run.c;
     run = combine(op, run, x);
+  }
+}
+
+// ---- segmented moments (fb_segmented_moments): the same three launches over MSt ----------------------
+struct MomentCols {
+  const double* vals[FB_SCAN_MAX_COLS];
+  const uint8_t* valid[FB_SCAN_MAX_COLS];
+  int64_t* out_count[FB_SCAN_MAX_COLS];
+  double* out_m2[FB_SCAN_MAX_COLS];
+  int32_t ncols;
+};
+
+struct MomentSmem {
+  double x[padded(kTile)];  // values in, running M2 out
+  int64_t c[padded(kTile)];
+  uint8_t valid[kTile];
+  uint8_t head[kTile];
+  MSt warp_tot[kThreads / 32];
+  int64_t seg_range[2];
+};
+
+// the state of one row: a valid value x enters as (1, x, x - x), so that a NaN or an infinity makes M2 NaN
+__device__ __forceinline__ MSt moment_of(const MomentSmem& sm, int j) {
+  const int c = sm.valid[j];
+  const double x = c ? sm.x[padded(j)] : 0.0;
+  return MSt{c, x, x - x, sm.head[j]};
+}
+
+// kFinal = false: pass 1 (tile states); true: pass 3 (running count and M2 per row, from the carries)
+template <bool kFinal>
+__global__ void __launch_bounds__(kThreads)
+fb_segmoments_tile_kernel(int64_t nrows, int64_t nseg, const int64_t* __restrict__ offsets,
+                          const __grid_constant__ MomentCols a, int64_t ntiles, int64_t* __restrict__ tile_c,
+                          double* __restrict__ tile_mean, double* __restrict__ tile_m2, int32_t* __restrict__ tile_f) {
+  __shared__ __align__(16) MomentSmem sm;
+  const int64_t tile = blockIdx.x;
+  const int64_t start = tile * kTile;
+  const int64_t end = start + kTile < nrows ? start + kTile : nrows;
+  const int nloc = (int)(end - start);
+  mark_heads<false, false>(nrows, nseg, offsets, start, end, 0, sm.head, sm.seg_range);
+  const int j0 = threadIdx.x * kItems;
+  for (int col = 0; col < a.ncols; ++col) {
+    const double* __restrict__ src = a.vals[col];
+    const uint8_t* __restrict__ vm = a.valid[col];
+    for (int i = threadIdx.x; i < kTile; i += kThreads) {
+      const bool in = i < nloc;
+      sm.x[padded(i)] = in ? __ldg(src + start + i) : 0.0;
+      sm.valid[i] = in ? (vm == nullptr ? 1 : (__ldg(vm + start + i) != 0)) : 0;
+    }
+    __syncthreads();
+    MSt acc{};
+#pragma unroll
+    for (int k = 0; k < kItems; ++k) acc = combine(0, acc, moment_of(sm, j0 + k));
+    MSt total;
+    const MSt pre = block_exclusive<kThreads / 32, false, MSt>(0, acc, sm.warp_tot, &total);
+    const int64_t t = col * ntiles + tile;
+    if (!kFinal) {
+      if (threadIdx.x == 0) {
+        tile_c[t] = total.c;
+        tile_mean[t] = total.mean;
+        tile_m2[t] = total.m2;
+        if (col == 0) tile_f[tile] = total.f;
+      }
+      continue;
+    }
+    MSt run = combine(0, MSt{tile_c[t], tile_mean[t], tile_m2[t], 0}, pre);
+#pragma unroll
+    for (int k = 0; k < kItems; ++k) {
+      const int j = j0 + k;
+      run = combine(0, run, moment_of(sm, j));
+      sm.x[padded(j)] = run.c > 0 ? run.m2 : 0.0;  // no valid row yet: 0, not whatever preceded the segment
+      sm.c[padded(j)] = run.c;
+    }
+    __syncthreads();
+    double* __restrict__ om = a.out_m2[col];
+    int64_t* __restrict__ oc = a.out_count[col];
+    for (int i = threadIdx.x; i < nloc; i += kThreads) {
+      if (om != nullptr) om[start + i] = sm.x[padded(i)];
+      if (oc != nullptr) oc[start + i] = sm.c[padded(i)];
+    }
+    __syncthreads();  // shared buffers are refilled by the next column
+  }
+}
+
+// pass 2: per column, the exclusive segmented scan of the tile states (in place: state -> carry)
+__global__ void __launch_bounds__(kCarryThreads)
+fb_segmoments_carry_kernel(int64_t ntiles, int64_t* __restrict__ tile_c, double* __restrict__ tile_mean,
+                           double* __restrict__ tile_m2, const int32_t* __restrict__ tile_f) {
+  __shared__ MSt warp_tot[kCarryThreads / 32];
+  const int64_t o = (int64_t)blockIdx.x * ntiles;
+  int64_t* tc = tile_c + o;
+  double* tm = tile_mean + o;
+  double* tq = tile_m2 + o;
+  const int64_t per = (ntiles + kCarryThreads - 1) / kCarryThreads;
+  const int64_t b = threadIdx.x * per;
+  const int64_t e = b + per < ntiles ? b + per : ntiles;
+  MSt acc{};
+  for (int64_t t = b; t < e; ++t) acc = combine(0, acc, MSt{tc[t], tm[t], tq[t], tile_f[t]});
+  MSt total;
+  MSt run = block_exclusive<kCarryThreads / 32, false, MSt>(0, acc, warp_tot, &total);
+  for (int64_t t = b; t < e; ++t) {
+    const MSt x{tc[t], tm[t], tq[t], tile_f[t]};
+    tc[t] = run.c;
+    tm[t] = run.mean;
+    tq[t] = run.m2;
+    run = combine(0, run, x);
   }
 }
 
@@ -801,6 +945,51 @@ extern "C" int fb_segmented_scan(int dev, void* stream, int64_t nrows, int64_t n
   FbDeviceGuard guard(dev);
   FB_CHECK(guard.ok, "cannot select device %d", dev);
   return run_scan((cudaStream_t)stream, false, 0, nrows, nseg, d_offsets, a, scratch);
+}
+
+extern "C" size_t fb_segmented_moments_scratch_bytes(int64_t nrows, int ncols) {
+  if (nrows <= 0 || ncols <= 0) return 0;
+  return (size_t)num_tiles(nrows) * (24 * (size_t)ncols + 4);
+}
+
+extern "C" int fb_segmented_moments(int dev, void* stream, int64_t nrows, int64_t nseg, const int64_t* d_offsets,
+                                    int ncols, const void* const* vals, const uint8_t* const* valid,
+                                    int64_t* const* out_count, void* const* out_m2, void* scratch,
+                                    size_t scratch_bytes) {
+  FB_CHECK(nrows >= 0 && nseg >= 0, "negative row or segment count");
+  FB_CHECK(ncols >= 1 && ncols <= FB_SCAN_MAX_COLS, "ncols=%d out of range [1,%d]", ncols, FB_SCAN_MAX_COLS);
+  MomentCols a;
+  memset(&a, 0, sizeof(a));
+  a.ncols = ncols;
+  for (int c = 0; c < ncols; ++c) {
+    a.vals[c] = vals != nullptr ? (const double*)vals[c] : nullptr;
+    a.valid[c] = valid != nullptr ? valid[c] : nullptr;
+    a.out_count[c] = out_count != nullptr ? out_count[c] : nullptr;
+    a.out_m2[c] = out_m2 != nullptr ? (double*)out_m2[c] : nullptr;
+    FB_CHECK(nrows == 0 || a.vals[c] != nullptr, "column %d needs a value column", c);
+  }
+  if (nrows == 0) return 0;
+  FB_CHECK(nseg >= 1 && d_offsets != nullptr, "%lld rows need at least one segment", (long long)nrows);
+  FB_CHECK(num_tiles(nrows) < (1LL << 31), "too many rows");
+  FB_CHECK(scratch != nullptr && scratch_bytes >= fb_segmented_moments_scratch_bytes(nrows, ncols),
+           "scratch too small: %zu < %zu", scratch_bytes, fb_segmented_moments_scratch_bytes(nrows, ncols));
+  FbDeviceGuard guard(dev);
+  FB_CHECK(guard.ok, "cannot select device %d", dev);
+  cudaStream_t st = (cudaStream_t)stream;
+  const int64_t ntiles = num_tiles(nrows);
+  int64_t* tile_c = (int64_t*)scratch;
+  double* tile_mean = (double*)(tile_c + ncols * ntiles);
+  double* tile_m2 = tile_mean + ncols * ntiles;
+  int32_t* tile_f = (int32_t*)(tile_m2 + ncols * ntiles);
+  fb_segmoments_tile_kernel<false><<<(unsigned)ntiles, kThreads, 0, st>>>(nrows, nseg, d_offsets, a, ntiles, tile_c,
+                                                                          tile_mean, tile_m2, tile_f);
+  FB_CUDA(cudaGetLastError());
+  fb_segmoments_carry_kernel<<<ncols, kCarryThreads, 0, st>>>(ntiles, tile_c, tile_mean, tile_m2, tile_f);
+  FB_CUDA(cudaGetLastError());
+  fb_segmoments_tile_kernel<true><<<(unsigned)ntiles, kThreads, 0, st>>>(nrows, nseg, d_offsets, a, ntiles, tile_c,
+                                                                         tile_mean, tile_m2, tile_f);
+  FB_CUDA(cudaGetLastError());
+  return 0;
 }
 
 extern "C" size_t fb_window_frame_scratch_bytes(int64_t nrows, int ncols, int64_t start, int64_t end, int flags) {

@@ -588,11 +588,11 @@ class B200ExecutionEngine(EngineLifecycle):
     def _plain_aggs(agg_cols: List[Any]) -> bool:
         """``SUM/COUNT/MIN/MAX/AVG/FIRST/LAST/PERCENTILE_*`` of a named column (or ``*``) without casts: what
         ``_aggregate_named`` takes directly (and what the distributed engine decomposes into partial / final)."""
-        from .column import ColumnExpr, Kind
+        from .column import VARIANCES, ColumnExpr, Kind
 
         return all(isinstance(a, ColumnExpr) and a.kind == Kind.AGG and a.as_type is None and not a.is_distinct
-                   and a.func in ("SUM", "COUNT", "MIN", "MAX", "AVG", "FIRST", "LAST", "PERCENTILE_CONT",
-                                  "PERCENTILE_DISC")
+                   and (a.func in ("SUM", "COUNT", "MIN", "MAX", "AVG", "FIRST", "LAST", "PERCENTILE_CONT",
+                                   "PERCENTILE_DISC") or a.func in VARIANCES)
                    and a.arg.kind in (Kind.NAMED, Kind.WILDCARD) and a.arg.as_type is None
                    and not (a.func in ("FIRST", "LAST") and a.arg.kind == Kind.WILDCARD)
                    for a in agg_cols)
@@ -603,7 +603,8 @@ class B200ExecutionEngine(EngineLifecycle):
         import pyarrow as pa
 
         from . import sort as S
-        from .column import PERCENTILES
+        from .colmap import variance_of
+        from .column import PERCENTILES, VARIANCES
 
         if any(a.func in PERCENTILES for a in agg_cols):
             return self._aggregate_sorted(df, partition_spec, agg_cols)
@@ -671,6 +672,7 @@ class B200ExecutionEngine(EngineLifecycle):
                                   add(None, m, K.AGG_COUNT) if m is not None else None))
             rows_slot = add(None, None, K.AGG_COUNT)
         rowno: Any = None
+        moments: Dict[str, Any] = {}  # argument column -> its (SUM, COUNT, DEV, DEV2) accumulators
         for a in agg_cols:
             fn, arg = a.func, a.arg.name
             if fn == "COUNT":
@@ -697,6 +699,17 @@ class B200ExecutionEngine(EngineLifecycle):
                 cnt = add(None, rm, K.AGG_COUNT)
                 plan.append((a.output_name, "string", add(rank, rm, K.AGG_MIN_I64 if fn == "MIN" else K.AGG_MAX_I64),
                              tp, (cnt, arg)))
+                continue
+            if fn in VARIANCES:
+                # one SUM, COUNT, DEV, DEV2 per column, shared by all its variances (DESIGN §7i)
+                assert_or_throw(pa.types.is_integer(tp) or pa.types.is_floating(tp),
+                                lambda: NotImplementedError(f"{fn}({arg}): {tp} is not a numeric type"))
+                if arg not in moments:
+                    cf = widen(c, tp)
+                    cf = (cf if cf.dtype == torch.float64 else cf.to(torch.float64)).contiguous()
+                    moments[arg] = (add(cf, m, K.AGG_SUM_F64), add(None, m, K.AGG_COUNT), add(cf, m, K.AGG_DEV_F64),
+                                    add(cf, m, K.AGG_DEV2_F64))
+                plan.append((a.output_name, "var", moments[arg], pa.float64(), fn))
                 continue
             is_f = pa.types.is_floating(tp)
             c8 = widen(c, tp)
@@ -748,6 +761,16 @@ class B200ExecutionEngine(EngineLifecycle):
             valids.append(gvalid)
         dicts = {k: t.dictionaries[k] for k in keys if k in t.dictionaries}
         for name, kind, slot, tp, nn in plan:
+            if kind == "var":
+                _, cnt, dev_, dev2 = slot
+                m_ = gaggs[cnt]
+                d = gaggs[dev_].view(torch.float64)
+                m2 = torch.clamp_min(gaggs[dev2].view(torch.float64) - d * d / m_.to(torch.float64), 0.0)
+                col, v = variance_of(nn, m2, m_)
+                fields.append(pa.field(name, tp))
+                cols.append(col)
+                valids.append(v)
+                continue
             raw = gaggs[slot]
             if kind == "pick":
                 cnt, ci = nn
@@ -846,7 +869,8 @@ class B200ExecutionEngine(EngineLifecycle):
         SQL text.  Pins: fugue_test/execution_suite.py:98-155."""
         from . import expr as X
         from . import relational as R
-        from .column import PERCENTILES, ColumnExpr, Kind, SelectColumns, agg as _agg, col, has_window, is_agg
+        from .column import (PERCENTILES, VARIANCES, ColumnExpr, Kind, SelectColumns, agg as _agg, col, has_window,
+                             is_agg)
 
         for e in list(cols.all_cols) + [where, having]:
             assert_or_throw(not has_window(e), lambda: NotImplementedError(
@@ -900,7 +924,8 @@ class B200ExecutionEngine(EngineLifecycle):
             if uid in agg_col:
                 continue
             assert_or_throw(a.func in ("SUM", "COUNT", "MIN", "MAX", "AVG", "FIRST", "LAST", "PERCENTILE_CONT",
-                                       "PERCENTILE_DISC"), NotImplementedError(f"aggregation {a.func}"))
+                                       "PERCENTILE_DISC") or a.func in VARIANCES,
+                            NotImplementedError(f"aggregation {a.func}"))
             assert_or_throw(not is_agg(a.arg), ValueError(f"nested aggregation {a}"))
             out = f"__fb_a{len(agg_col)}"
             agg_col[uid] = out

@@ -290,6 +290,9 @@ def unscramble64(k: torch.Tensor) -> torch.Tensor:
 
 
 AGG_SUM_F64, AGG_SUM_I64, AGG_COUNT, AGG_MIN_I64, AGG_MAX_I64, AGG_MIN_F64, AGG_MAX_F64 = range(7)
+# group-by only: deviations from the group mean (sum of d and of d * d, d = x - SUM / COUNT); each needs an
+# AGG_SUM_F64 of the same f64 column and validity and an AGG_COUNT of the same validity in the same call
+AGG_DEV_F64, AGG_DEV2_F64 = 7, 8
 MAX_AGGS = 16
 
 
@@ -428,6 +431,39 @@ def segmented_scan(offsets: torch.Tensor, nrows: int,
             _lib.ptr_array([0 if o is None else o.data_ptr() for o in outs]),
             _lib.ptr_array([c.data_ptr() for c in cnts]), scratch.data_ptr(), scratch.numel()))
         res.extend(zip(outs, cnts))
+    return res
+
+
+def segmented_moments(offsets: torch.Tensor, nrows: int,
+                      columns: Sequence[Tuple[torch.Tensor, Optional[torch.Tensor]]]
+                      ) -> List[Tuple[torch.Tensor, torch.Tensor]]:
+    """K9: running moments restarting at every segment ``[offsets[s], offsets[s + 1])``.  ``columns`` = one
+    ``(float64 values, validity or None)`` per column.  Returns per column ``(running count of the valid rows
+    (int64), running M2 = sum of (x - mean)^2 over them (float64, 0 where the count is 0))``; up to
+    ``SCAN_MAX_COLS`` columns share one launch sequence."""
+    lib = _lib.load()
+    assert offsets.dtype == torch.int64 and offsets.is_cuda and offsets.is_contiguous()
+    dev = offsets.device
+    nseg = int(offsets.shape[0]) - 1
+    res: List[Tuple[torch.Tensor, torch.Tensor]] = []
+    for b in range(0, len(columns), SCAN_MAX_COLS):
+        batch = columns[b:b + SCAN_MAX_COLS]
+        cnts, m2s = [], []
+        for v, m in batch:
+            assert v.dtype == torch.float64 and v.device == dev and v.is_contiguous() and v.shape[0] == nrows
+            if m is not None:
+                assert m.dtype == torch.uint8 and m.device == dev and m.is_contiguous() and m.shape[0] == nrows
+            cnts.append(torch.empty(nrows, dtype=torch.int64, device=dev))
+            m2s.append(torch.empty(nrows, dtype=torch.float64, device=dev))
+        nb = int(lib.fb_segmented_moments_scratch_bytes(nrows, len(batch)))
+        scratch = torch.empty(max(nb, 8), dtype=torch.uint8, device=dev)
+        _lib.check(lib.fb_segmented_moments(
+            dev.index, _stream_ptr(dev), nrows, nseg, offsets.data_ptr(), len(batch),
+            _lib.ptr_array([v.data_ptr() for v, _ in batch]),
+            _lib.ptr_array([0 if m is None else m.data_ptr() for _, m in batch]),
+            _lib.ptr_array([c.data_ptr() for c in cnts]), _lib.ptr_array([q.data_ptr() for q in m2s]),
+            scratch.data_ptr(), scratch.numel()))
+        res.extend(zip(cnts, m2s))
     return res
 
 

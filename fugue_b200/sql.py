@@ -10,7 +10,8 @@ fugue/workflow/workflow.py:2109-2166) and ``ExecutionEngine.aggregate`` reaches 
     SELECT [DISTINCT] <expr [AS a], ...> FROM t [WHERE <expr>] [GROUP BY <expr, ...>] [HAVING <expr>]
              [ORDER BY c [ASC|DESC], ...] [LIMIT n]
         -> parsed into column expressions (fugue_b200.column) and run by ``engine.select``: row-wise
-           parts in the device expression evaluator, SUM/COUNT/MIN/MAX/AVG in the hash group-by kernel
+           parts in the device expression evaluator, SUM/COUNT/MIN/MAX/AVG and VAR_SAMP / VARIANCE / VAR_POP /
+           STDDEV_SAMP / STDDEV / STDDEV_POP in the hash group-by kernel
     SELECT * FROM a [INNER|LEFT|RIGHT|FULL [OUTER]|LEFT SEMI|LEFT ANTI|CROSS] JOIN b
              [USING (k, ...) | ON a.k = b.k [AND ...]]                        -> hash join kernels
 
@@ -283,7 +284,9 @@ _TOKEN = re.compile(r"""\s*(?:
 )""", re.X)
 
 _AGG_FUNCS = {"SUM": functions.sum, "COUNT": functions.count, "MIN": functions.min, "MAX": functions.max,
-              "AVG": functions.avg, "MEAN": functions.avg, "FIRST": functions.first, "LAST": functions.last}
+              "AVG": functions.avg, "MEAN": functions.avg, "FIRST": functions.first, "LAST": functions.last,
+              "VAR_SAMP": functions.var_samp, "VARIANCE": functions.variance, "VAR_POP": functions.var_pop,
+              "STDDEV_SAMP": functions.stddev_samp, "STDDEV": functions.stddev, "STDDEV_POP": functions.stddev_pop}
 _CLAUSES = ("WHERE", "GROUP", "HAVING", "ORDER", "LIMIT")
 _CASE_WORDS = ("WHEN", "THEN", "ELSE", "END")  # never a column name or an implicit alias
 _ONE_ARG = {"ABS": functions.abs, "FLOOR": functions.floor, "CEIL": functions.ceil, "CEILING": functions.ceil,

@@ -218,6 +218,14 @@ int fb_pull_runs_tma(int dev, void* stream, int nruns, const void* const* src, v
  *                      (each 8 bytes per group, capacity + 2 entries allocated by the caller);
  *                      d_status[1] receives the number of groups.  d_out_aggs is a DEVICE array
  *                      of naggs device pointers.  Group order is unspecified.
+ *
+ * Deviations (the corrected two-pass variance, DESIGN §7i): FB_AGG_DEV_F64 and FB_AGG_DEV2_F64 read
+ * the f64 values of their column like FB_AGG_SUM_F64, and each needs, in the same call, an
+ * FB_AGG_SUM_F64 with the same value and validity pointers and an FB_AGG_COUNT with the same validity
+ * pointer (rejected otherwise).  After the other aggregates of a row's group are complete, the call adds
+ * d = x - SUM / COUNT of the row's group into DEV and d * d into DEV2, for every valid x.  With m = COUNT,
+ * M2 = sum over the group of (x - mean)^2 = max(0, DEV2 - DEV^2 / m).  A NaN or +-inf value makes DEV
+ * and DEV2 NaN.  fb_segmented_scan and the frame kernels reject both ops.
  * --------------------------------------------------------------------------- */
 #define FB_MAX_AGGS 16
 enum {
@@ -227,7 +235,9 @@ enum {
   FB_AGG_MIN_I64 = 3,
   FB_AGG_MAX_I64 = 4,
   FB_AGG_MIN_F64 = 5,
-  FB_AGG_MAX_F64 = 6
+  FB_AGG_MAX_F64 = 6,
+  FB_AGG_DEV_F64 = 7,
+  FB_AGG_DEV2_F64 = 8
 };
 size_t fb_groupby_table_bytes(int64_t capacity, int naggs);
 int fb_groupby_u64(int dev, void* stream, int64_t nrows, const void* keys, const uint8_t* key_valid,
@@ -260,6 +270,19 @@ size_t fb_segmented_scan_scratch_bytes(int64_t nrows, int ncols);
 int fb_segmented_scan(int dev, void* stream, int64_t nrows, int64_t nseg, const int64_t* d_offsets, int ncols,
                       const int32_t* ops, const void* const* vals, const uint8_t* const* valid,
                       void* const* out_vals, int64_t* const* out_count, void* scratch, size_t scratch_bytes);
+
+/* K9  segmented moments: over the same segments, per column c and row i, the valid rows of i's segment up to
+ * and including i (f64 values vals[c], mask valid[c] or NULL):
+ *   out_count[c][i]  their number m (int64)
+ *   out_m2[c][i]     M2 = sum of (x - mean)^2 over them (f64), 0 where m = 0; NaN once a NaN or +-inf is among them
+ * The state (n, mean, M2) is combined with Chan, Golub & LeVeque's pairwise update; a value enters as
+ * (1, x, x - x).  Same launch sequence and fixed combination order as fb_segmented_scan: bit-identical runs.
+ * vals, valid, out_count and out_m2 are HOST arrays of ncols <= FB_SCAN_MAX_COLS entries (an output may be
+ * NULL: not written); scratch: fb_segmented_moments_scratch_bytes. */
+size_t fb_segmented_moments_scratch_bytes(int64_t nrows, int ncols);
+int fb_segmented_moments(int dev, void* stream, int64_t nrows, int64_t nseg, const int64_t* d_offsets, int ncols,
+                         const void* const* vals, const uint8_t* const* valid, int64_t* const* out_count,
+                         void* const* out_m2, void* scratch, size_t scratch_bytes);
 
 /* K9  moving-window aggregate: ROWS BETWEEN start AND end over the same segments.  For row i of segment
  * [a, b) the frame is rows [max(a, i + start), min(b - 1, i + end)] (may be empty); a negative bound is

@@ -11,6 +11,8 @@ from an expression is a function of ``(kind, head, args)``:
               ``NULLIF ABS FLOOR CEIL SQRT EXP LN LOG10 POWER GREATEST LEAST``; ``ROUND``: args (x, digits literal)
               ``UPPER LOWER``: args (string,); ``SUBSTR``: args (string, start[, length]); ``TRIM LTRIM RTRIM``:
               args (string[, characters]); ``REPLACE``: args (string, from, to); ``CONCAT``: args (part, ...)
+              ``EXTRACT``: args (x,), kwarg ``field``; ``DATE_TRUNC``: args (x,), kwarg ``part``; ``DATEDIFF``: args
+              (a, b), kwarg ``part``; ``ADD_MONTHS``: args (x, n)
     AGG       head in ``SUM COUNT AVG MIN MAX FIRST LAST VAR_SAMP VAR_POP STDDEV_SAMP STDDEV_POP``, one arg,
               optional DISTINCT, or ``PERCENTILE_CONT PERCENTILE_DISC``, one arg and kwarg ``q`` (MEDIAN is
               PERCENTILE_CONT at q = 0.5)
@@ -62,7 +64,14 @@ VARIANCES = frozenset(["VAR_SAMP", "VAR_POP", "STDDEV_SAMP", "STDDEV_POP"])
 _AGG_ALIASES = {"STDDEV": "STDDEV_SAMP", "VARIANCE": "VAR_SAMP"}
 _RANKINGS = frozenset(["ROW_NUMBER", "RANK", "DENSE_RANK"])
 _RUNNING_FRAME = "ROWS BETWEEN UNBOUNDED PRECEDING AND CURRENT ROW"
-_LITERAL_TYPES = (int, bool, float, str)
+_LITERAL_TYPES = (int, bool, float, str, datetime.date, datetime.datetime, datetime.timedelta)
+TEMPORAL_LITERALS = (datetime.date, datetime.datetime, datetime.timedelta)
+# EXTRACT fields and DATE_TRUNC / DATEDIFF parts, in the order of the device's codes (``epoch`` has no code: it is
+# a division of the stored value)
+TIME_FIELDS = ("year", "month", "day", "hour", "minute", "second", "quarter", "dow", "isodow", "doy", "week",
+               "isoyear")
+TIME_PARTS = ("year", "quarter", "month", "week", "day", "hour", "minute", "second")
+TEMPORAL_FUNCTIONS = frozenset(["EXTRACT", "DATE_TRUNC", "DATEDIFF", "ADD_MONTHS"])
 FLOAT_FUNCTIONS = frozenset(["SQRT", "EXP", "LN", "LOG10", "POWER", "POW"])  # always float64
 ROUND_MAX_DIGITS = 18
 # functions that build a string from one string expression and literals (SUBSTRING is SUBSTR); ``||`` too
@@ -80,7 +89,7 @@ def to_pa_datatype(obj: Any) -> pa.DataType:
     if isinstance(obj, str):
         return parse_type(obj)
     table = {int: pa.int64(), float: pa.float64(), str: pa.string(), bool: pa.bool_(),
-             datetime.datetime: pa.timestamp("us"), datetime.date: pa.date32()}
+             datetime.datetime: pa.timestamp("us"), datetime.date: pa.date32(), datetime.timedelta: pa.duration("us")}
     if obj in table:
         return table[obj]
     raise TypeError(f"can't convert {obj!r} to a data type")
@@ -101,6 +110,12 @@ def _show_literal(v: Any) -> str:
         return "TRUE" if v else "FALSE"
     if isinstance(v, str):
         return "'" + v.replace("\\", "\\\\").replace("'", "\\'") + "'"
+    if isinstance(v, datetime.datetime):
+        return f"TIMESTAMP '{v.isoformat(sep=' ')}'"
+    if isinstance(v, datetime.date):
+        return f"DATE '{v.isoformat()}'"
+    if isinstance(v, datetime.timedelta):
+        return _interval_text(v)
     return str(v)
 
 
@@ -205,6 +220,12 @@ class ColumnExpr:
         if k == Kind.LITERAL:
             return None if self.head is None else to_pa_datatype(type(self.head))
         if k == Kind.BINARY:
+            if self.head in ("+", "-"):  # a date or timestamp moved by a day-time interval keeps its type
+                for x, d in ((self.args[0], self.args[1]), (self.args[1], self.args[0])):
+                    if d.kind == Kind.LITERAL and d.as_type is None and isinstance(d.head, datetime.timedelta) and \
+                            (self.head == "+" or d is self.args[1]):
+                        tp = x.infer_type(schema)
+                        return tp if tp is not None and pa.types.is_temporal(tp) else None
             return pa.bool_() if self.head in BOOL_OPS else (pa.string() if self.head == "||" else None)
         if k == Kind.UNARY and self.head in ("-", "~"):
             tp = self.args[0].infer_type(schema)
@@ -221,6 +242,10 @@ class ColumnExpr:
             return pa.string()
         if k == Kind.CALL and self.head.upper() in FLOAT_FUNCTIONS:
             return pa.float64()
+        if k == Kind.CALL and self.head.upper() in ("EXTRACT", "DATEDIFF"):
+            return pa.float64() if str(self.kwargs.get("field", "")).lower() == "epoch" else pa.int64()
+        if k == Kind.CALL and self.head.upper() in ("DATE_TRUNC", "ADD_MONTHS") and self.args:
+            return _operand(self.args[0]).infer_type(schema)
         if k == Kind.CALL and case_string_results(self) is not None:
             return pa.string()
         if k in (Kind.AGG, Kind.WINDOW) and self.head in PERCENTILES:
@@ -392,8 +417,12 @@ def _canon(v: Any) -> str:
 
 # ---- builders -------------------------------------------------------------------------------------
 def lit(obj: Any, alias: str = "") -> ColumnExpr:
+    """A literal: None (NULL), bool, int, float, str, ``datetime.date`` (date32), ``datetime.datetime`` (timestamp[us];
+    a naive one is UTC wall clock, an aware one is converted to UTC) or ``datetime.timedelta`` (duration[us])."""
     if not (obj is None or isinstance(obj, _LITERAL_TYPES)):
         raise NotImplementedError(f"{obj}, type: {type(obj)}")
+    if isinstance(obj, datetime.datetime) and obj.tzinfo is not None:
+        obj = obj.astimezone(datetime.timezone.utc).replace(tzinfo=None)
     return ColumnExpr(Kind.LITERAL, obj, as_name=alias)
 
 
@@ -494,13 +523,15 @@ def _frame_bound(b: Any, unbounded: str) -> str:
 
 
 def _interval_text(d: datetime.timedelta) -> str:
-    """A positive timedelta as an SQL day-time INTERVAL literal: ``INTERVAL '7' DAY`` for whole days, else
-    ``INTERVAL '1 02:03:04[.000005]' DAY TO SECOND``."""
+    """A timedelta as an SQL day-time INTERVAL literal: ``INTERVAL '7' DAY`` for whole days, else
+    ``INTERVAL '1 02:03:04[.000005]' DAY TO SECOND``; a negative one carries one leading ``-`` for the whole value."""
+    sign = "-" if d < datetime.timedelta(0) else ""
+    d = abs(d)
     if d.seconds == 0 and d.microseconds == 0:
-        return f"INTERVAL '{d.days}' DAY"
+        return f"INTERVAL '{sign}{d.days}' DAY"
     hms = f"{d.seconds // 3600:02d}:{d.seconds // 60 % 60:02d}:{d.seconds % 60:02d}"
     frac = f".{d.microseconds:06d}" if d.microseconds else ""
-    return f"INTERVAL '{d.days} {hms}{frac}' DAY TO SECOND"
+    return f"INTERVAL '{sign}{d.days} {hms}{frac}' DAY TO SECOND"
 
 
 def _range_frame(frame: Any) -> Tuple[Any, Any]:
@@ -759,6 +790,36 @@ class functions:
         return e
 
     @staticmethod
+    def extract(field: str, c: Any) -> ColumnExpr:
+        """SQL ``EXTRACT(field FROM c)`` of a date or UTC timestamp (proleptic Gregorian, floor semantics before
+        1970): ``year month day hour minute second`` (whole second 0-59) ``quarter dow`` (0 = Sunday) ``isodow``
+        (1 = Monday ... 7) ``doy week`` (ISO 8601) ``isoyear``, int64; ``epoch``: float64 seconds since 1970-01-01."""
+        field = _time_word("EXTRACT", "field", field, TIME_FIELDS + ("epoch",))
+        return ColumnExpr(Kind.CALL, "EXTRACT", [_operand(c)], {"field": field})
+
+    date_part = extract
+
+    @staticmethod
+    def date_trunc(part: str, c: Any) -> ColumnExpr:
+        """SQL ``DATE_TRUNC(part, c)``: the start of the ``year quarter month week`` (Monday) ``day hour minute
+        second`` that ``c`` lies in; keeps the type of ``c`` (a date stays a date)."""
+        return ColumnExpr(Kind.CALL, "DATE_TRUNC", [_operand(c)], {"part": _time_word("DATE_TRUNC", "part", part, TIME_PARTS)})
+
+    @staticmethod
+    def datediff(part: str, a: Any, b: Any) -> ColumnExpr:
+        """DuckDB's ``DATEDIFF(part, a, b)``: the number of ``part`` boundaries crossed from ``a`` to ``b`` (int64)."""
+        return ColumnExpr(Kind.CALL, "DATEDIFF", [_operand(a), _operand(b)],
+                          {"part": _time_word("DATEDIFF", "part", part, TIME_PARTS)})
+
+    @staticmethod
+    def add_months(c: Any, n: Any) -> ColumnExpr:
+        """``c + n`` calendar months (``n`` an int or an int64 expression): the day is clamped to the last day of the
+        target month (Jan 31 + 1 month = Feb 28 / 29), the time of day kept; Postgres, DuckDB, ``pandas.DateOffset``."""
+        if isinstance(n, bool) or (not isinstance(n, (int, ColumnExpr))):
+            raise ValueError(f"ADD_MONTHS: n must be an int or an integer expression, got {n!r}")
+        return ColumnExpr(Kind.CALL, "ADD_MONTHS", [_operand(c), _operand(n)])
+
+    @staticmethod
     def min(c: Any) -> ColumnExpr:  # noqa: A003
         return agg("MIN", c)
 
@@ -856,6 +917,18 @@ class functions:
     def lead(c: Any, n: int = 1, default: Any = None) -> ColumnExpr:
         """``c`` of the row ``n`` rows later in the same logical partition, else ``default``."""
         return _offset_fn("LEAD", c, n, default)
+
+
+def _time_word(fn: str, what: str, word: Any, known: Tuple[str, ...]) -> str:
+    if not isinstance(word, str) or word.lower() not in known:
+        raise ValueError(f"{fn}: unknown {what} {word!r}; one of {', '.join(known)}")
+    return word.lower()
+
+
+for _field in ("year", "month", "day", "hour", "minute", "second", "quarter"):
+    setattr(functions, _field, staticmethod(lambda c, _f=_field: functions.extract(_f, c)))
+for _name, _field in (("dayofweek", "dow"), ("dayofyear", "doy"), ("week", "week")):
+    setattr(functions, _name, staticmethod(lambda c, _f=_field: functions.extract(_f, c)))
 
 
 # ---- one SELECT list ------------------------------------------------------------------------------
@@ -968,6 +1041,11 @@ def to_sql(expr: ColumnExpr, enable_cast: bool = True, nested: bool = False) -> 
             body += " ESCAPE " + to_sql(expr.args[2], enable_cast)
         if nested:
             body = "(" + body + ")"
+    elif k == Kind.CALL and expr.head.upper() in ("EXTRACT", "DATE_TRUNC", "DATEDIFF") and \
+            isinstance(expr.kwargs.get("field" if expr.head.upper() == "EXTRACT" else "part"), str):
+        inner = ", ".join(to_sql(_operand(x), enable_cast) for x in expr.args)
+        body = f"EXTRACT({expr.kwargs['field']} FROM {inner})" if expr.head.upper() == "EXTRACT" else \
+            f"{expr.head.upper()}('{expr.kwargs['part']}', {inner})"
     elif k == Kind.CALL and expr.head.upper() == "CASE" and len(expr.args) % 2 == 1:
         a = expr.args
         body = "CASE" + "".join(f" WHEN {to_sql(_operand(a[i]), enable_cast)} THEN {to_sql(_operand(a[i + 1]), enable_cast)}"

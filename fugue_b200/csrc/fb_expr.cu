@@ -169,6 +169,177 @@ __device__ __noinline__ double fn_ln(double x) { return log(x); }
 __device__ __noinline__ double fn_log10(double x) { return log10(x); }
 __device__ __noinline__ double fn_pow(double x, double y) { return pow(x, y); }
 
+// ---- temporal ops (one row): proleptic Gregorian calendar, UTC, no leap seconds.  A value is an int64 count of
+// `unit`s since 1970-01-01 00:00.  Sums and products are taken on uint64 (they wrap, never overflow a signed type);
+// every division is by a positive compile-time constant and floors, so no instruction can trap.
+__device__ __forceinline__ int64_t wadd(int64_t a, int64_t b) { return (int64_t)((uint64_t)a + (uint64_t)b); }
+__device__ __forceinline__ int64_t wsub(int64_t a, int64_t b) { return (int64_t)((uint64_t)a - (uint64_t)b); }
+__device__ __forceinline__ int64_t wmul(int64_t a, int64_t b) { return (int64_t)((uint64_t)a * (uint64_t)b); }
+template <int64_t C>
+__device__ __forceinline__ int64_t fdiv(int64_t x) {  // floor(x / C)
+  const int64_t q = x / C;
+  return q - (int64_t)(x % C < 0);
+}
+
+__device__ __forceinline__ int64_t units_per_second(int unit) {
+  switch (unit) {
+    case FB_TU_MS: return 1000ll;
+    case FB_TU_US: return 1000000ll;
+    case FB_TU_NS: return 1000000000ll;
+    default: return 1ll;
+  }
+}
+
+// x -> whole days since the epoch and the second of that day (0 for a date)
+__device__ __forceinline__ void split_days(int64_t x, int unit, int64_t& days, int64_t& sod) {
+  int64_t s = x;
+  switch (unit) {
+    case FB_TU_DAY: days = x; sod = 0; return;
+    case FB_TU_MS: s = fdiv<1000ll>(x); break;
+    case FB_TU_US: s = fdiv<1000000ll>(x); break;
+    case FB_TU_NS: s = fdiv<1000000000ll>(x); break;
+    default: break;
+  }
+  days = fdiv<86400ll>(s);
+  sod = s - days * 86400ll;
+}
+
+__device__ __forceinline__ int64_t join_days(int64_t days, int64_t sod, int unit) {
+  if (unit == FB_TU_DAY) return days;
+  return wmul(wadd(wmul(days, 86400ll), sod), units_per_second(unit));
+}
+
+__device__ __forceinline__ bool is_leap(int64_t y) { return (y & 3) == 0 && (y % 100 != 0 || y % 400 == 0); }
+
+// days since the epoch -> year, month (1-12), day (1-31), day of the year (1-366): 400-year eras of 146 097 days,
+// years that start on March 1
+__device__ __forceinline__ void civil_from_days(int64_t days, int64_t& y, int& m, int& d, int& doy) {
+  const int64_t z = wadd(days, 719468ll);
+  const int64_t era = fdiv<146097ll>(z);
+  const int doe = (int)(z - era * 146097ll);                                    // [0, 146096]
+  const int yoe = (doe - doe / 1460 + doe / 36524 - doe / 146096) / 365;        // [0, 399]
+  const int doy_m = doe - (365 * yoe + yoe / 4 - yoe / 100);                    // [0, 365], from March 1
+  const int mp = (5 * doy_m + 2) / 153;                                         // [0, 11]
+  d = doy_m - (153 * mp + 2) / 5 + 1;
+  m = mp < 10 ? mp + 3 : mp - 9;
+  y = wadd(wadd((int64_t)yoe, wmul(era, 400ll)), (int64_t)(m <= 2));
+  doy = mp < 10 ? doy_m + 60 + (int)is_leap(y) : doy_m - 305;
+}
+
+__device__ __forceinline__ int64_t days_from_civil(int64_t y, int m, int d) {
+  y = wsub(y, (int64_t)(m <= 2));
+  const int64_t era = fdiv<400ll>(y);
+  const int yoe = (int)wsub(y, wmul(era, 400ll));                                // [0, 399]
+  const int doy_m = (153 * (m > 2 ? m - 3 : m + 9) + 2) / 5 + d - 1;
+  const int doe = yoe * 365 + yoe / 4 - yoe / 100 + doy_m;
+  return wsub(wadd(wmul(era, 146097ll), (int64_t)doe), 719468ll);
+}
+
+__device__ __forceinline__ int iso_weekday(int64_t days) {  // 1 = Monday ... 7 = Sunday; 1970-01-01 was a Thursday
+  const int64_t t = wadd(days, 3ll);
+  return (int)(t - fdiv<7ll>(t) * 7ll) + 1;
+}
+
+__device__ __forceinline__ uint64_t ts_part(int64_t x, int field, int unit) {
+  int64_t days, sod, y;
+  int m, d, doy;
+  split_days(x, unit, days, sod);
+  switch (field) {
+    case FB_TF_HOUR: return (uint64_t)(sod / 3600);
+    case FB_TF_MINUTE: return (uint64_t)(sod / 60 % 60);
+    case FB_TF_SECOND: return (uint64_t)(sod % 60);
+    case FB_TF_DOW: return (uint64_t)(iso_weekday(days) % 7);
+    case FB_TF_ISODOW: return (uint64_t)iso_weekday(days);
+    case FB_TF_WEEK:
+    case FB_TF_ISOYEAR: days = wadd(days, (int64_t)(4 - iso_weekday(days))); break;  // the Thursday of the ISO week
+    default: break;
+  }
+  civil_from_days(days, y, m, d, doy);
+  switch (field) {
+    case FB_TF_MONTH: return (uint64_t)m;
+    case FB_TF_DAY: return (uint64_t)d;
+    case FB_TF_QUARTER: return (uint64_t)((m - 1) / 3 + 1);
+    case FB_TF_DOY: return (uint64_t)doy;
+    case FB_TF_WEEK: return (uint64_t)((doy - 1) / 7 + 1);
+    default: return (uint64_t)y;  // FB_TF_YEAR, FB_TF_ISOYEAR
+  }
+}
+
+__device__ __forceinline__ uint64_t ts_trunc(int64_t x, int part, int unit) {
+  int64_t days, sod, y;
+  int m, d, doy;
+  split_days(x, unit, days, sod);
+  switch (part) {
+    case FB_TP_SECOND: break;
+    case FB_TP_MINUTE: sod -= sod % 60; break;
+    case FB_TP_HOUR: sod -= sod % 3600; break;
+    case FB_TP_DAY: sod = 0; break;
+    case FB_TP_WEEK: sod = 0; days = wsub(days, (int64_t)(iso_weekday(days) - 1)); break;
+    default:
+      civil_from_days(days, y, m, d, doy);
+      sod = 0;
+      days = days_from_civil(y, part == FB_TP_YEAR ? 1 : part == FB_TP_QUARTER ? (m - 1) / 3 * 3 + 1 : m, 1);
+      break;
+  }
+  return (uint64_t)join_days(days, sod, unit);
+}
+
+// whole parts since 1970-01-01 00:00 (weeks: since Monday 1969-12-29)
+__device__ __forceinline__ uint64_t ts_index(int64_t x, int part, int unit) {
+  int64_t days, sod, y;
+  int m, d, doy;
+  split_days(x, unit, days, sod);
+  switch (part) {
+    case FB_TP_SECOND: return (uint64_t)wadd(wmul(days, 86400ll), sod);
+    case FB_TP_MINUTE: return (uint64_t)wadd(wmul(days, 1440ll), sod / 60);
+    case FB_TP_HOUR: return (uint64_t)wadd(wmul(days, 24ll), sod / 3600);
+    case FB_TP_DAY: return (uint64_t)days;
+    case FB_TP_WEEK: return (uint64_t)fdiv<7ll>(wadd(days, 3ll));
+    default: break;
+  }
+  civil_from_days(days, y, m, d, doy);
+  y = wsub(y, 1970ll);
+  if (part == FB_TP_YEAR) return (uint64_t)y;
+  if (part == FB_TP_QUARTER) return (uint64_t)wadd(wmul(y, 4ll), (int64_t)((m - 1) / 3));
+  return (uint64_t)wadd(wmul(y, 12ll), (int64_t)(m - 1));
+}
+
+// x + n calendar months: the day of the month clamped to the target month's last day, the time of day kept
+__device__ __forceinline__ uint64_t ts_addmon(int64_t x, int64_t n, int unit) {
+  int64_t days, sod, y;
+  int m, d, doy;
+  split_days(x, unit, days, sod);
+  const int64_t sub = wsub(x, join_days(days, sod, unit));  // the fraction of a second, in units
+  civil_from_days(days, y, m, d, doy);
+  const int64_t mi = wadd(wadd(wmul(y, 12ll), (int64_t)(m - 1)), n);
+  const int64_t y2 = fdiv<12ll>(mi);
+  const int m2 = (int)(mi - y2 * 12ll) + 1;
+  const int last = m2 == 2 ? 28 + (int)is_leap(y2) : 30 + ((m2 + (m2 >> 3)) & 1);
+  return (uint64_t)wadd(join_days(days_from_civil(y2, m2, d < last ? d : last), sod, unit), sub);
+}
+
+__device__ __forceinline__ uint64_t mulsat_i(int64_t x, int64_t b) {  // b >= 1
+  const int64_t lo = wmul(x, b);
+  if (__mul64hi(x, b) != (lo >> 63)) return x < 0 ? 0x8000000000000000ull : 0x7FFFFFFFFFFFFFFFull;
+  return (uint64_t)lo;
+}
+
+__device__ __forceinline__ uint64_t floordiv_i(int64_t x, int64_t b) {  // b >= 1 (checked on the host)
+  const int64_t q = x / b;
+  return (uint64_t)(q - (int64_t)(x % b < 0));
+}
+
+// the temporal ops run out of line, once per row, like the transcendental functions below: the interpreter's switch
+// and its registers stay what they were.  `code`: field or part | unit << 8
+__device__ __noinline__ uint64_t fn_mulsat(uint64_t x, uint64_t b) { return mulsat_i((int64_t)x, (int64_t)b); }
+__device__ __noinline__ uint64_t fn_floordiv(uint64_t x, uint64_t b) { return floordiv_i((int64_t)x, (int64_t)b); }
+__device__ __noinline__ uint64_t fn_ts_part(uint64_t x, int code) { return ts_part((int64_t)x, code & 0xFF, code >> 8); }
+__device__ __noinline__ uint64_t fn_ts_trunc(uint64_t x, int code) { return ts_trunc((int64_t)x, code & 0xFF, code >> 8); }
+__device__ __noinline__ uint64_t fn_ts_index(uint64_t x, int code) { return ts_index((int64_t)x, code & 0xFF, code >> 8); }
+__device__ __noinline__ uint64_t fn_ts_addmon(uint64_t x, uint64_t n, int unit) {
+  return ts_addmon((int64_t)x, (int64_t)n, unit);
+}
+
 // one tile of kExprTile rows (kFull: no bounds checks; only the last tile of a table is partial)
 template <bool kFull>
 __device__ __forceinline__ void run_tile(const ExprProgram& P, int64_t row0, int nk, int tid, uint64_t* tmp_v,
@@ -358,6 +529,12 @@ __device__ __forceinline__ void run_tile(const ExprProgram& P, int64_t row0, int
           FB_ROWS(if (((bv >> k) & 1u) && (!((accv >> k) & 1u) || total_key(b[k]) < total_key(acc[k]))) acc[k] = b[k];)
           accv |= bv;
           break;
+        case FB_X_MULSAT_I: FB_BIN(fn_mulsat(x, y)) break;
+        case FB_X_FLOORDIV_I: FB_BIN(fn_floordiv(x, y)) break;
+        case FB_X_TS_PART: FB_UN(fn_ts_part(x, (int)in.imm)) break;
+        case FB_X_TS_TRUNC: FB_UN(fn_ts_trunc(x, (int)in.imm)) break;
+        case FB_X_TS_INDEX: FB_UN(fn_ts_index(x, (int)in.imm)) break;
+        case FB_X_TS_ADDMON: FB_BIN(fn_ts_addmon(x, y, in.flags >> FB_XF_UNIT_SHIFT)) break;
         default: break;
       }
 #undef FB_FBIN
@@ -415,10 +592,22 @@ extern "C" int fb_eval_expr(int dev, void* stream, int64_t nrows, int ncols, con
   }
   for (int i = 0; i < nins; ++i) {
     const fb_expr_ins& in = program[i];
-    FB_CHECK(in.op >= FB_X_MOV && in.op <= FB_X_LEAST_F, "instruction %d: unknown op %d", i, in.op);
-    const bool unary_fn = (in.op >= FB_X_ABS_I && in.op <= FB_X_LOG10);  // scalar functions of acc alone
+    FB_CHECK(in.op >= FB_X_MOV && in.op <= FB_X_TS_ADDMON, "instruction %d: unknown op %d", i, in.op);
+    const bool unary_fn = (in.op >= FB_X_ABS_I && in.op <= FB_X_LOG10) ||  // scalar functions of acc alone
+                          (in.op >= FB_X_TS_PART && in.op <= FB_X_TS_INDEX);
     if (unary_fn) FB_CHECK(in.kind == FB_XK_NONE, "instruction %d: op %d takes no operand", i, in.op);
-    if (in.op == FB_X_SEL)
+    if (in.op == FB_X_MULSAT_I || in.op == FB_X_FLOORDIV_I)
+      FB_CHECK(in.kind == FB_XK_IMM && in.imm >= 1, "instruction %d: op %d takes an immediate >= 1", i, in.op);
+    if (in.op >= FB_X_TS_PART && in.op <= FB_X_TS_INDEX) {
+      const int64_t nsel = in.op == FB_X_TS_PART ? (int64_t)FB_TF_COUNT : (int64_t)FB_TP_COUNT;
+      FB_CHECK(in.imm >= 0 && (in.imm & 0xFF) < nsel && (in.imm >> 8) < FB_TU_COUNT,
+               "instruction %d: op %d: field / part %lld or unit %lld out of range", i, in.op,
+               (long long)(in.imm & 0xFF), (long long)(in.imm >> 8));
+    }
+    if (in.op == FB_X_TS_ADDMON)
+      FB_CHECK(in.flags >= 0 && (in.flags & 0xFF) == 0 && (in.flags >> FB_XF_UNIT_SHIFT) < FB_TU_COUNT,
+               "instruction %d: FB_X_TS_ADDMON flags %#x: the unit in flags >> 8 is out of range", i, in.flags);
+    else if (in.op == FB_X_SEL)
       FB_CHECK(in.flags >= 0 && (in.flags >> FB_XF_COND_SHIFT) < FB_EXPR_NREGS,
                "instruction %d: FB_X_SEL condition temporary %d out of range", i, in.flags >> FB_XF_COND_SHIFT);
     else if (in.op > FB_X_LOOKUP)

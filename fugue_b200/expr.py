@@ -20,7 +20,12 @@ A string-building expression over one string column (``UPPER LOWER SUBSTR TRIM L
 is evaluated over the dictionary (``strings.evaluate``); per row it is the code (``FB_X_MOV``) mapped to the
 result's code in a new dictionary (``FB_X_LOOKUP``).  It is a whole output column (``project``), or the
 operand of ``==`` / ``!=`` with a string literal, of ``IS [NOT] NULL``, of ``LIKE`` and of ``LENGTH``.
+Dates and timestamps are int64 counts of their Arrow unit.  A temporal literal (``DATE '..'``, ``TIMESTAMP '..'``, an
+interval) is rescaled on the host to the unit of the temporal operand it meets and becomes a plain immediate; two
+temporal columns meet as their raw integers, and the unit-correct form is an explicit ``CAST`` between temporal types
+(``FB_X_MULSAT_I`` / ``FB_X_FLOORDIV_I``).  ``EXTRACT DATE_TRUNC DATEDIFF ADD_MONTHS`` are the ``FB_X_TS_*`` ops.
 """
+import datetime
 import struct
 from typing import Any, Dict, List, Optional, Sequence, Tuple
 
@@ -29,8 +34,8 @@ import torch
 
 from . import kernels as K
 from . import strings as ST
-from .column import (FLOAT_FUNCTIONS, ROUND_MAX_DIGITS, ColumnExpr, Kind, case_string_results, is_string_build,
-                     lit as _lit)
+from .column import (FLOAT_FUNCTIONS, ROUND_MAX_DIGITS, TEMPORAL_LITERALS, TIME_FIELDS, TIME_PARTS, ColumnExpr, Kind,
+                     case_string_results, is_string_build, lit as _lit)
 from .schema import Schema
 from .table import B200Table, _storage_dtype, expr_type
 
@@ -51,6 +56,60 @@ def _cls_of(tp: pa.DataType) -> str:
 
 def _f64_bits(v: float) -> int:
     return struct.unpack("<Q", struct.pack("<d", float(v)))[0]
+
+
+_I64_MIN, _I64_MAX = -(1 << 63), (1 << 63) - 1
+_EPOCH = datetime.datetime(1970, 1, 1)
+_US = datetime.timedelta(microseconds=1)
+# units of one microsecond as a fraction (numerator, denominator), by unit code (kernels.TU_*)
+_PER_US = {K.TU_DAY: (1, 86_400_000_000), K.TU_S: (1, 1_000_000), K.TU_MS: (1, 1000), K.TU_US: (1, 1), K.TU_NS: (1000, 1)}
+_UNIT_CODE = {"s": K.TU_S, "ms": K.TU_MS, "us": K.TU_US, "ns": K.TU_NS}
+
+
+def time_unit(tp: Optional[pa.DataType]) -> Optional[Tuple[str, int]]:
+    """``("point" | "span", unit code)`` of a date / timestamp / duration type, None for every other type."""
+    if tp is None:
+        return None
+    if pa.types.is_date32(tp):
+        return "point", K.TU_DAY
+    if pa.types.is_date64(tp):
+        return "point", K.TU_MS
+    if pa.types.is_timestamp(tp):
+        return "point", _UNIT_CODE[tp.unit]
+    if pa.types.is_duration(tp):
+        return "span", _UNIT_CODE[tp.unit]
+    return None
+
+
+def _literal_us(v: Any) -> int:
+    """A temporal literal as exact microseconds (since the epoch for a date or timestamp; a date is its midnight)."""
+    if isinstance(v, datetime.timedelta):
+        return v // _US
+    if not isinstance(v, datetime.datetime):
+        v = datetime.datetime(v.year, v.month, v.day)
+    return (v - _EPOCH) // _US
+
+
+def _natural_type(v: Any) -> pa.DataType:
+    return pa.duration("us") if isinstance(v, datetime.timedelta) else \
+        pa.timestamp("us") if isinstance(v, datetime.datetime) else pa.date32()
+
+
+def _is_temporal_literal(e: Any) -> bool:
+    return isinstance(e, ColumnExpr) and e.kind == Kind.LITERAL and e.as_type is None and \
+        isinstance(e.value, TEMPORAL_LITERALS)
+
+
+def _in_unit(v: Any, unit: int) -> Tuple[int, bool]:
+    """(floor of the literal in ``unit``, whether it is a whole number of them)."""
+    num, den = _PER_US[unit]
+    q, r = divmod(_literal_us(v) * num, den)
+    return q, r == 0
+
+
+def _const_predicate(x: ColumnExpr, truth: bool) -> ColumnExpr:
+    """``truth`` where ``x`` is not NULL, NULL elsewhere (Kleene: TRUE OR NULL, FALSE AND NULL)."""
+    return (x.not_null() | _lit(None)) if truth else (x.is_null() & _lit(None))
 
 
 class _OutOfResources(Exception):
@@ -173,6 +232,9 @@ class _Program:
                 return (K.XK_IMM, 0, v & ((1 << 64) - 1), "i", False)
             if isinstance(v, float):
                 return (K.XK_IMM, 0, _f64_bits(v), "f", False)
+            if isinstance(v, TEMPORAL_LITERALS):  # alone: in the unit of its own type (days / microseconds)
+                q, _ = _in_unit(v, time_unit(_natural_type(v))[1])
+                return (K.XK_IMM, 0, q & ((1 << 64) - 1), "i", False)
         return None
 
     def _emit_with(self, op: int, leaf: Tuple[int, int, int, str, bool], ctx: str, flags: int = 0) -> None:
@@ -218,9 +280,198 @@ class _Program:
             elif cls == "s":
                 raise NotImplementedError(f"cast of a string expression to {e.as_type}: {e}")
             elif cls != "n":
+                self._temporal_cast(e)
                 self._acc_to(cls, want)
                 cls = want
         return cls, nullable
+
+    # -- dates and timestamps
+    def _ttype(self, e: Any) -> Optional[pa.DataType]:
+        """The date / timestamp / duration type whose unit the value of ``e`` is counted in; None if it is not temporal
+        (a temporal literal alone has none: it takes the unit of the operand it meets)."""
+        if not isinstance(e, ColumnExpr):
+            return None
+        if e.as_type is not None:
+            return e.as_type if time_unit(e.as_type) else None
+        if e.kind == Kind.NAMED:
+            tp = self.t.schema[e.name].type if e.name in self.t.schema else None
+            return tp if time_unit(tp) else None
+        if e.kind == Kind.BINARY and e.op in ("+", "-"):
+            for x, d in ((e.left, e.right), (e.right, e.left)):
+                if _is_temporal_literal(d) and isinstance(d.value, datetime.timedelta) and (e.op == "+" or d is e.right):
+                    return self._ttype(x)
+            return None
+        if e.kind == Kind.CALL:
+            fn = e.func.upper()
+            if fn in ("DATE_TRUNC", "ADD_MONTHS"):
+                return self._operand_type(e.args[0]) if e.args else None
+            if fn in ("COALESCE", "IFNULL", "GREATEST", "LEAST", "CASE", "IF", "IIF", "NULLIF"):
+                args = e.args[1::2] + e.args[-1:] if fn == "CASE" else e.args[1:] if fn in ("IF", "IIF") else \
+                    e.args[:1] if fn == "NULLIF" else e.args
+                for a in args:
+                    tp = self._ttype(a)
+                    if tp is not None:
+                        return tp
+        return None
+
+    def _operand_type(self, e: Any) -> Optional[pa.DataType]:
+        """``_ttype``, and for a temporal literal the type of the literal itself."""
+        e = e if isinstance(e, ColumnExpr) else _lit(e)
+        return _natural_type(e.value) if _is_temporal_literal(e) else self._ttype(e)
+
+    def _temporal_cast(self, e: ColumnExpr) -> None:
+        """``CAST`` between two date / timestamp types or two durations: the accumulator rescaled to the target's unit.
+        To a finer unit the product saturates (it keeps its order against every value that fits); to a coarser one the
+        division floors (``CAST(ts AS date)`` is the calendar day, also before 1970)."""
+        dst, src = time_unit(e.as_type), time_unit(self._operand_type(e.cast(None)))
+        if dst is None or src is None or dst[0] != src[0] or dst[1] == src[1]:
+            return
+        (n1, d1), (n2, d2) = _PER_US[src[1]], _PER_US[dst[1]]
+        num, den = n2 * d1, d2 * n1  # target units per source unit
+        if num >= den:
+            self.emit(K.X_MULSAT_I, K.XK_IMM, 0, 0, num // den)
+        else:
+            self.emit(K.X_FLOORDIV_I, K.XK_IMM, 0, 0, den // num)
+
+    def _literal_for(self, v: Any, tp: pa.DataType, what: Any) -> ColumnExpr:
+        """A temporal literal as the int64 literal of its exact value in the unit of ``tp`` (clamped to int64)."""
+        kind, unit = time_unit(tp)
+        if (kind == "span") != isinstance(v, datetime.timedelta):
+            raise ValueError(f"{_lit(v)} can't stand for a value of type {tp}: {what}")
+        q, exact = _in_unit(v, unit)
+        if not exact:
+            raise ValueError(f"{_lit(v)} is not a whole number of the units of {tp}: {what}")
+        return _lit(min(max(q, _I64_MIN), _I64_MAX))
+
+    def _temporal_operands(self, e: ColumnExpr) -> ColumnExpr:  # noqa: C901
+        """The node with its temporal literals replaced by int64 literals in the unit of the temporal operand they
+        meet (comparison, ``+ -``, COALESCE, CASE result, GREATEST / LEAST), so that no device instruction is spent
+        on them.  Two literals fold on the host."""
+        if e.kind == Kind.BINARY and e.op in ("+", "-", "<", "<=", ">", ">=", "==", "!="):
+            a, b = _folded(e.left), _folded(e.right)
+            la, lb = _is_temporal_literal(a), _is_temporal_literal(b)
+            if not (la or lb):
+                return e
+            if la and lb:
+                return _fold(e.op, a.value, b.value, e)
+            x, l, lit_left = (b, a, True) if la else (a, b, False)
+            v = l.value
+            tp = self._ttype(x)
+            if tp is None:
+                raise ValueError(f"{l} meets an operand that is not a date, timestamp or duration: {e}")
+            kind, unit = time_unit(tp)
+            span = isinstance(v, datetime.timedelta)
+            if e.op in ("+", "-"):
+                if e.op == "+" and not span:
+                    raise ValueError(f"a date or timestamp can't be added to another: {e}")
+                if span and e.op == "-" and lit_left and kind == "point":
+                    raise ValueError(f"an interval minus a date or timestamp has no meaning: {e}")
+                q, exact = _in_unit(v, unit)
+                if not exact:
+                    raise ValueError(f"{l} is not a whole number of the units of {tp} (cast the operand first): {e}")
+                n = _lit(min(max(q, _I64_MIN), _I64_MAX))
+                return ColumnExpr(Kind.BINARY, e.op, [n, x] if lit_left else [x, n])
+            if span != (kind == "span"):
+                raise ValueError(f"{l} can't be compared with a value of type {tp}: {e}")
+            op = _Program._REVERSE[e.op] if lit_left else e.op  # x op literal
+            q, exact = _in_unit(v, unit)
+            if q > _I64_MAX or q < _I64_MIN:  # beyond every value of the unit
+                return _const_predicate(x, op in (("<", "<=", "!=") if q > _I64_MAX else (">", ">=", "!=")))
+            if not exact:
+                if op in ("==", "!="):
+                    return _const_predicate(x, op == "!=")
+                if op in (">=", "<"):  # x >= v <=> x >= ceil(v); x < v <=> x < ceil(v)
+                    if q == _I64_MAX:
+                        return _const_predicate(x, op == "<")
+                    q += 1
+            return ColumnExpr(Kind.BINARY, op, [x, _lit(q)])
+        if e.kind == Kind.CALL and e.func.upper() in ("COALESCE", "GREATEST", "LEAST", "CASE"):
+            args = [a if isinstance(a, ColumnExpr) else _lit(a) for a in e.args]
+            n = len(args)
+            results = [i for i in range(n) if e.func.upper() != "CASE" or i % 2 == 1 or i == n - 1]
+            if not any(_is_temporal_literal(args[i]) for i in results):
+                return e
+            tp = self._ttype(e)
+            if tp is None:
+                kinds = {isinstance(args[i].value, datetime.timedelta) for i in results if _is_temporal_literal(args[i])}
+                if len(kinds) > 1:
+                    raise ValueError(f"{e.func} mixes points in time and intervals: {e}")
+                tp = pa.duration("us") if True in kinds else pa.timestamp("us")  # literals only
+            for i in results:
+                if _is_temporal_literal(args[i]):
+                    args[i] = self._literal_for(args[i].value, tp, e)
+            return ColumnExpr(Kind.CALL, e.head, args, e.kwargs)
+        return e
+
+    def _calendar_unit(self, e: ColumnExpr, a: Any) -> int:
+        """The unit of a calendar function's date / timestamp operand; raises for what the device has no calendar for."""
+        tp = self._operand_type(a)
+        if tp is None:
+            at = a.infer_type(self.t.schema) if isinstance(a, ColumnExpr) else None
+            if at is not None and (pa.types.is_time(at) or pa.types.is_duration(at)):
+                raise NotImplementedError(f"{e.func} of a {at} value: {e}")
+            raise ValueError(f"{e.func} needs a date or timestamp operand, got {a}: {e}")
+        if time_unit(tp)[0] != "point":
+            raise NotImplementedError(f"{e.func} of a {tp} value: {e}")
+        if pa.types.is_timestamp(tp) and tp.tz is not None and tp.tz.upper() != "UTC":
+            raise NotImplementedError(f"{e.func} of a timestamp in time zone {tp.tz} (only UTC; there is no time-zone "
+                                      f"database on the device): {e}")
+        return time_unit(tp)[1]
+
+    def _temporal_function(self, e: ColumnExpr, fn: str) -> Tuple[str, bool]:
+        args = [a if isinstance(a, ColumnExpr) else _lit(a) for a in e.args]
+        if len(args) != (1 if fn in ("EXTRACT", "DATE_TRUNC") else 2):
+            raise ValueError(f"{fn} takes {1 if fn in ('EXTRACT', 'DATE_TRUNC') else 2} value argument(s): {e}")
+        word = e.kwargs.get("field" if fn == "EXTRACT" else "part")
+        if fn != "ADD_MONTHS":
+            known = TIME_FIELDS + ("epoch",) if fn == "EXTRACT" else TIME_PARTS
+            if not isinstance(word, str) or word.lower() not in known:
+                raise ValueError(f"{fn}: unknown {'field' if fn == 'EXTRACT' else 'part'} {word!r}: {e}")
+            word = word.lower()
+        unit = self._calendar_unit(e, args[0])
+        if fn == "DATEDIFF":
+            unit_b = self._calendar_unit(e, args[1])
+            code = TIME_PARTS.index(word)
+            ca, na = self.compile(args[0])
+            self.emit(K.X_TS_INDEX, imm=code | unit << 8)
+            tmp = self.alloc()
+            self.emit(K.X_ST, K.XK_NONE, tmp)
+            cb, nb = self.compile(args[1])
+            self.emit(K.X_TS_INDEX, imm=code | unit_b << 8)
+            self.emit(K.X_SUB_I, K.XK_REG, tmp)
+            self.release(tmp)
+            return "i", na or nb or "n" in (ca, cb)
+        if fn == "ADD_MONTHS":
+            cn = self._static_cls(args[1])
+            if cn not in ("i", "n"):
+                raise ValueError(f"ADD_MONTHS: the number of months must be an integer: {e}")
+            leaf = self._leaf(args[1])
+            if leaf is not None:
+                cls, nullable = self.compile(args[0])
+                self._emit_with(K.X_TS_ADDMON, leaf, "i", unit << K.XF_UNIT_SHIFT)
+                return "i", nullable or leaf[4]
+            _, nn = self.compile(args[1])
+            tmp = self.alloc()
+            self.emit(K.X_ST, K.XK_NONE, tmp)
+            cls, nullable = self.compile(args[0])
+            self.emit(K.X_TS_ADDMON, K.XK_REG, tmp, unit << K.XF_UNIT_SHIFT)
+            self.release(tmp)
+            return "i", nullable or nn
+        cls, nullable = self.compile(args[0])
+        if cls == "n":
+            return "n", True
+        if fn == "DATE_TRUNC":
+            self.emit(K.X_TS_TRUNC, imm=TIME_PARTS.index(word) | unit << 8)
+            return "i", nullable
+        if word == "epoch":  # one IEEE operation on the stored value
+            self.emit(K.X_I2F)
+            if unit == K.TU_DAY:
+                self.emit(K.X_MUL_F, K.XK_IMM, 0, 0, _f64_bits(86400.0))
+            else:
+                self.emit(K.X_DIV_F, K.XK_IMM, 0, 0, _f64_bits(float(_PER_US[K.TU_S][1] * _PER_US[unit][0] // _PER_US[unit][1])))
+            return "f", nullable
+        self.emit(K.X_TS_PART, imm=TIME_FIELDS.index(word) | unit << 8)
+        return "i", nullable
 
     def _node(self, e: ColumnExpr) -> Tuple[str, bool]:  # noqa: C901
         if is_string_build(e):
@@ -260,12 +511,16 @@ class _Program:
                 return "b", nullable
             raise NotImplementedError(f"unary operator {e.op}")
         if e.kind == Kind.BINARY:
-            return self._binary(e)
+            r = self._temporal_operands(e)
+            return self._binary(r) if r.kind == Kind.BINARY else self._node(r)
         if e.kind == Kind.CALL:
             low = _lower(e)
             if low is not None:
                 return self._node(low)
+            e = self._temporal_operands(e)
             fn = e.func.upper()
+            if fn in ("EXTRACT", "DATE_TRUNC", "DATEDIFF", "ADD_MONTHS"):
+                return self._temporal_function(e, fn)
             if fn == "COALESCE":
                 return self._coalesce(e)
             if fn in ("LIKE", "LENGTH"):
@@ -580,8 +835,8 @@ class _Program:
             return _cls_of(self.t.schema[e.name].type)
         if e.kind == Kind.LITERAL:
             v = e.value
-            return "n" if v is None else "b" if isinstance(v, bool) else "i" if isinstance(v, int) else \
-                "f" if isinstance(v, float) else "s"
+            return "n" if v is None else "b" if isinstance(v, bool) else \
+                "i" if isinstance(v, (int,) + TEMPORAL_LITERALS) else "f" if isinstance(v, float) else "s"
         if e.kind == Kind.UNARY:
             if e.op in ("IS_NULL", "NOT_NULL", "~"):
                 return "b"
@@ -601,6 +856,8 @@ class _Program:
             return "b"
         if e.kind == Kind.CALL and e.func.upper() in FLOAT_FUNCTIONS:
             return "f"
+        if e.kind == Kind.CALL and e.func.upper() == "EXTRACT" and str(e.kwargs.get("field", "")).lower() == "epoch":
+            return "f"
         if e.kind == Kind.CALL and e.func.upper() in ("CASE", "GREATEST", "LEAST"):
             args = e.args[1::2] + e.args[-1:] if e.func.upper() == "CASE" else e.args
             cs = [self._static_cls(a if isinstance(a, ColumnExpr) else _lit(a)) for a in args]
@@ -617,6 +874,34 @@ class _Program:
         types = [expr_type(t.schema.types[i]) if isinstance(i, int) else K.T_I64 for i in self.cols]
         return K.eval_expr(t.num_rows, t.device, cols, valid, self.ins, [o[0] for o in self.outs],
                            [o[1] for o in self.outs], col_types=types, out_types=[o[2] for o in self.outs])
+
+
+def _folded(e: ColumnExpr) -> ColumnExpr:
+    """``e``, or the literal it folds to when it is an operator between two temporal literals."""
+    if e.kind == Kind.BINARY and e.as_type is None and e.op in ("+", "-"):
+        a, b = _folded(e.left), _folded(e.right)
+        if _is_temporal_literal(a) and _is_temporal_literal(b):
+            return _fold(e.op, a.value, b.value, e)
+    return e
+
+
+def _fold(op: str, a: Any, b: Any, e: ColumnExpr) -> ColumnExpr:
+    """``a op b`` of two temporal literals, computed on the host."""
+    span_a, span_b = isinstance(a, datetime.timedelta), isinstance(b, datetime.timedelta)
+    if not span_a and not span_b:  # a date next to a timestamp is its midnight
+        a, b = _EPOCH + _literal_us(a) * _US, _EPOCH + _literal_us(b) * _US
+    elif span_a != span_b:
+        if op not in ("+", "-") or (op == "-" and span_a):
+            raise ValueError(f"operator {op} has no meaning between a point in time and an interval: {e}")
+        a = a if span_a else _EPOCH + _literal_us(a) * _US
+        b = b if span_b else _EPOCH + _literal_us(b) * _US
+    if op == "+" and not (span_a or span_b):
+        raise ValueError(f"a date or timestamp can't be added to another: {e}")
+    import operator
+
+    fn = {"+": operator.add, "-": operator.sub, "<": operator.lt, "<=": operator.le, ">": operator.gt,
+          ">=": operator.ge, "==": operator.eq, "!=": operator.ne}[op]
+    return _lit(fn(a, b))
 
 
 def _default_type(cls: str, e: ColumnExpr, schema: Schema) -> pa.DataType:

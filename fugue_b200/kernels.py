@@ -865,7 +865,13 @@ XF_COND_SHIFT = 8  # X_SEL: the condition's temporary is flags >> 8
  X_LT_I, X_LE_I, X_GT_I, X_GE_I, X_EQ_I, X_NE_I, X_LT_F, X_LE_F, X_GT_F, X_GE_F, X_EQ_F, X_NE_F,
  X_AND, X_OR, X_COALESCE, X_RCOALESCE, X_LOOKUP,
  X_SEL, X_MOD_I, X_RMOD_I, X_MOD_F, X_RMOD_F, X_ABS_I, X_ABS_F, X_FLOOR_F, X_CEIL_F, X_ROUND_F, X_ROUND_I,
- X_SQRT, X_EXP, X_LN, X_LOG10, X_POW, X_RPOW, X_GREATEST_I, X_LEAST_I, X_GREATEST_F, X_LEAST_F) = range(60)
+ X_SQRT, X_EXP, X_LN, X_LOG10, X_POW, X_RPOW, X_GREATEST_I, X_LEAST_I, X_GREATEST_F, X_LEAST_F,
+ X_MULSAT_I, X_FLOORDIV_I, X_TS_PART, X_TS_TRUNC, X_TS_INDEX, X_TS_ADDMON) = range(66)
+XF_UNIT_SHIFT = 8  # X_TS_ADDMON: the unit is flags >> 8; X_TS_PART / TRUNC / INDEX: imm = field or part | unit << 8
+TU_DAY, TU_S, TU_MS, TU_US, TU_NS = range(5)  # enum fb_time_unit: what one count of a temporal value is
+TIME_FIELDS = ("year", "month", "day", "hour", "minute", "second", "quarter", "dow", "isodow", "doy", "week",
+               "isoyear")  # enum fb_time_field, in order
+TIME_PARTS = ("year", "quarter", "month", "week", "day", "hour", "minute", "second")  # enum fb_time_part, in order
 
 # storage dtype of each K8 type: uint16 / uint32 / float16 live in the signed tensors of their width
 EXPR_STORAGE = {T_I8: torch.int8, T_I16: torch.int16, T_I32: torch.int32, T_I64: torch.int64, T_U8: torch.uint8,

@@ -18,10 +18,13 @@ fugue/workflow/workflow.py:2109-2166) and ``ExecutionEngine.aggregate`` reaches 
 Expressions: + - * / %, comparisons (= == != <> < <= > >=), AND / OR / NOT, IS [NOT] NULL, [NOT] IN (...),
 [NOT] BETWEEN, x [NOT] LIKE 'pattern' [ESCAPE 'c'], CAST(x AS type), CASE [x] WHEN .. THEN .. [ELSE ..] END,
 COALESCE, IFNULL, NULLIF, IF / IIF, MOD, ABS, FLOOR, CEIL / CEILING, ROUND, SQRT, EXP, LN, LOG10, POWER / POW,
-GREATEST, LEAST, LENGTH, UPPER, LOWER, SUBSTR / SUBSTRING, TRIM, LTRIM, RTRIM, REPLACE, CONCAT, a || b, literals,
-`quoted` and table-qualified names.
+GREATEST, LEAST, LENGTH, UPPER, LOWER, SUBSTR / SUBSTRING, TRIM, LTRIM, RTRIM, REPLACE, CONCAT, a || b,
+DATE '..' / TIMESTAMP '..' / INTERVAL '..' DAY | HOUR | MINUTE | SECOND | DAY TO SECOND literals, x + INTERVAL 'n' MONTH | YEAR,
+EXTRACT(field FROM x), DATE_PART, YEAR MONTH DAY HOUR MINUTE SECOND QUARTER DAYOFWEEK DAYOFYEAR WEEK, DATE_TRUNC,
+DATEDIFF, ADD_MONTHS, literals, `quoted` and table-qualified names.
 Anything else raises NotImplementedError (there is no host SQL fallback in this package).
 """
+import datetime
 import re
 from typing import Any, Dict, List, Tuple
 
@@ -157,10 +160,10 @@ class B200SQLEngine:
         sql = statement.construct() if isinstance(statement, StructuredRawSQL) else str(statement)
         sql = re.sub(r"\s+", " ", sql.strip().rstrip(";"))
         tables = {k: self._engine.to_df(v) for k, v in dfs.items()}
-        m = re.match(r"(?is)^SELECT (.+?) FROM (.+)$", sql)
-        if m is None:
+        cut = _top_level_from(sql)
+        if re.match(r"(?i)^SELECT ", sql) is None or cut is None:
             raise NotImplementedError(f"unsupported SQL: {sql}")
-        items, rest = m.group(1).strip(), m.group(2).strip()
+        items, rest = sql[len("SELECT "):cut[0]].strip(), sql[cut[1]:].strip()
         if re.search(r"(?i)\bJOIN\b", rest):
             return self._join(items, rest, tables, sql)
         return self._single(items, rest, tables, sql)
@@ -244,6 +247,29 @@ class B200SQLEngine:
         return self._engine.join(t1, t2, how=how, on=on)
 
 
+def _top_level_from(sql: str) -> Any:
+    """(start, end) of the first `` FROM `` outside parentheses and string literals (the one inside
+    ``EXTRACT(field FROM x)`` is not the clause), or None."""
+    depth, quote, i = 0, "", 0
+    while i < len(sql):
+        ch = sql[i]
+        if quote:
+            if ch == "\\" and quote == "'":
+                i += 1
+            elif ch == quote:
+                quote = ""
+        elif ch in "'`":
+            quote = ch
+        elif ch == "(":
+            depth += 1
+        elif ch == ")":
+            depth -= 1
+        elif depth == 0 and sql[i:i + 6].upper() == " FROM " and i > 0:
+            return i, i + 6
+        i += 1
+    return None
+
+
 def _split_commas(text: str) -> List[str]:
     out, depth, cur = [], 0, []
     for ch in text:
@@ -296,6 +322,9 @@ _STRING_ARGS = {"UPPER": (1, 1), "LOWER": (1, 1), "SUBSTR": (2, 3), "SUBSTRING":
 _STRING_BUILDERS = {"UPPER": functions.upper, "LOWER": functions.lower, "SUBSTR": functions.substr,
                     "SUBSTRING": functions.substr, "TRIM": functions.trim, "LTRIM": functions.ltrim,
                     "RTRIM": functions.rtrim, "REPLACE": functions.replace}
+_FIELD_FUNCS = {"YEAR": "year", "MONTH": "month", "DAY": "day", "HOUR": "hour", "MINUTE": "minute", "SECOND": "second",
+                "QUARTER": "quarter", "DAYOFWEEK": "dow", "DAYOFYEAR": "doy", "WEEK": "week"}
+_MONTHS = "INTERVAL_MONTHS"  # a calendar interval literal: only the operand of + / - next to a date or timestamp
 _TWO_ARGS = {"NULLIF": functions.nullif, "IFNULL": functions.coalesce, "MOD": lambda a, b: a % b,
              "POWER": functions.power, "POW": functions.power}
 
@@ -429,11 +458,19 @@ class _Parser:
         e = self.multiplicative()
         while True:
             if self.op("+"):
-                e = e + self.multiplicative()
+                e = self._plus(e, self.multiplicative(), 1)
             elif self.op("-"):
-                e = e - self.multiplicative()
+                e = self._plus(e, self.multiplicative(), -1)
             else:
                 return e
+
+    def _plus(self, a: ColumnExpr, b: ColumnExpr, sign: int) -> ColumnExpr:
+        """``a + b`` / ``a - b``; a calendar interval on the right (or, for ``+``, on the left) adds months."""
+        for x, iv in ((a, b), (b, a)):
+            if iv.kind == Kind.CALL and iv.head == _MONTHS and (iv is b or sign > 0) and \
+                    not (x.kind == Kind.CALL and x.head == _MONTHS):
+                return functions.add_months(x, sign * iv.args[0].value)
+        return a + b if sign > 0 else a - b
 
     def multiplicative(self) -> ColumnExpr:
         e = self.concat()
@@ -483,6 +520,8 @@ class _Parser:
             return self._maybe_qualified(val[1:-1].replace("``", "`"))
         if kind == "id":
             up = val.upper()
+            if up in ("DATE", "TIMESTAMP", "INTERVAL") and self.peek(1)[0] == "str":
+                return self._temporal_literal(up)
             if up == "NULL":
                 self.i += 1
                 return null()
@@ -509,6 +548,36 @@ class _Parser:
             self.i += 1
             return self._maybe_qualified(val)
         return self.fail(f"unexpected token {val!r}")
+
+    def _temporal_literal(self, word: str) -> ColumnExpr:
+        """``DATE '2024-01-31'``, ``TIMESTAMP '2024-01-31 12:00:00[.ffffff]'``, ``INTERVAL 'n' DAY | HOUR | MINUTE |
+        SECOND``, ``INTERVAL 'd hh:mm:ss[.f]' DAY TO SECOND``, ``INTERVAL 'n' MONTH | YEAR``."""
+        text = _unquote(self.peek(1)[1])
+        self.i += 2
+        shown = f"{word} '{text}'"
+        try:
+            if word == "DATE":
+                return lit(datetime.date.fromisoformat(text.strip()))
+            if word == "TIMESTAMP":
+                v = datetime.datetime.fromisoformat(text.strip())
+                return lit(v if isinstance(v, datetime.datetime) else datetime.datetime(v.year, v.month, v.day))
+            kind, unit = self.peek()
+            unit = unit.upper() if kind == "id" else ""
+            self.i += 1
+            if unit in ("MONTH", "YEAR"):
+                return function(_MONTHS, lit(int(text.strip()) * (12 if unit == "YEAR" else 1)))
+            if unit == "DAY" and self.kw("TO", "SECOND"):
+                m = re.fullmatch(r"\s*(-?)(\d+) (\d+):(\d+):(\d+)(?:\.(\d{1,6}))?\s*", text)
+                if m is None:
+                    raise ValueError("expected 'd hh:mm:ss[.ffffff]'")
+                d = datetime.timedelta(days=int(m.group(2)), hours=int(m.group(3)), minutes=int(m.group(4)),
+                                       seconds=int(m.group(5)), microseconds=int((m.group(6) or "0").ljust(6, "0")))
+                return lit(-d if m.group(1) else d)
+            if unit in ("DAY", "HOUR", "MINUTE", "SECOND"):
+                return lit(datetime.timedelta(**{unit.lower() + "s": int(text.strip())}))
+            raise ValueError(f"unknown interval unit {unit!r}")
+        except (ValueError, OverflowError) as ex:
+            raise ValueError(f"malformed literal {shown}: {ex} in: {self.sql}") from None
 
     def _case(self) -> ColumnExpr:
         """``CASE WHEN c THEN v ... [ELSE e] END``, or ``CASE x WHEN a THEN v ...``, the searched form with ``x = a``."""
@@ -572,6 +641,14 @@ class _Parser:
             q = self._quantile_literal(fn)
             self.expect(")")
             return functions.percentile_cont(arg, q) if fn == "QUANTILE_CONT" else functions.percentile_disc(arg, q)
+        if fn == "EXTRACT":  # EXTRACT(field FROM x)
+            kind, field = self.peek()
+            if kind not in ("id", "str") or not (self.peek(1)[0] == "id" and self.peek(1)[1].upper() == "FROM"):
+                self.fail("EXTRACT needs (field FROM value)")
+            self.i += 2
+            arg = self.expr()
+            self.expect(")")
+            return functions.extract(_unquote(field) if kind == "str" else field, arg)
         args: List[Any] = []
         if not self.op(")"):
             while True:
@@ -581,6 +658,8 @@ class _Parser:
             self.expect(")")
         if fn == "COALESCE":
             return functions.coalesce(*args)
+        if fn in _FIELD_FUNCS or fn in ("DATE_PART", "DATE_TRUNC", "DATEDIFF", "DATE_DIFF", "ADD_MONTHS"):
+            return self._temporal_call(fn, args)
         if fn in _STRING_ARGS:
             lo, hi = _STRING_ARGS[fn]
             if not lo <= len(args) <= hi:
@@ -605,6 +684,24 @@ class _Parser:
         if fn in ("GREATEST", "LEAST"):
             return functions.greatest(*args) if fn == "GREATEST" else functions.least(*args)
         return function(fn, *args)
+
+    def _temporal_call(self, fn: str, args: List[Any]) -> ColumnExpr:
+        want = 1 if fn in _FIELD_FUNCS else 3 if fn in ("DATEDIFF", "DATE_DIFF") else 2
+        if len(args) != want:
+            raise ValueError(f"{fn} takes {want} argument(s), got {len(args)} in: {self.sql}")
+        if fn in _FIELD_FUNCS:
+            return functions.extract(_FIELD_FUNCS[fn], args[0])
+        if fn == "ADD_MONTHS":
+            n = args[1]
+            return functions.add_months(args[0], n.value if n.kind == Kind.LITERAL and n.as_type is None else n)
+        word = args[0]
+        if word.kind != Kind.LITERAL or not isinstance(word.value, str):
+            raise ValueError(f"{fn} takes a string literal as its first argument, got {word} in: {self.sql}")
+        if fn == "DATE_PART":
+            return functions.extract(word.value, args[1])
+        if fn == "DATE_TRUNC":
+            return functions.date_trunc(word.value, args[1])
+        return functions.datediff(word.value, args[1], args[2])
 
     def _quantile_literal(self, fn: str) -> Any:
         kind, val = self.peek()

@@ -499,6 +499,21 @@ int fb_join2_emit(int dev, void* stream, int64_t nprobe, const void* probe_keys,
  *                side is skipped, so the result is NULL only if both are; floats in IEEE totalOrder
  *                (-NaN < -inf < ... < -0.0 < +0.0 < ... < +inf < +NaN), returning that operand's bits
  *   The unary ops among these (ABS, FLOOR, CEIL, ROUND, SQRT, EXP, LN, LOG10) take no operand (FB_XK_NONE).
+ * Temporal ops.  A value is an int64 count of a unit (enum fb_time_unit) since 1970-01-01 00:00 UTC; the calendar is
+ * the proleptic Gregorian one without leap seconds, every division floors (1969-12-31 23:59:59.5 has second 59), NULL
+ * propagates.  Exact for every int64 of FB_TU_NS and FB_TU_US, every int32 of FB_TU_DAY, and for FB_TU_MS / FB_TU_S
+ * where the year lies within the range of an int32 day count; elsewhere the result is unspecified, but nothing traps
+ * (sums and products wrap, every divisor is a positive constant).
+ *   FB_X_MULSAT_I   acc <- acc * B, saturated to INT64_MIN / INT64_MAX; B an immediate >= 1 (rescale to a finer unit)
+ *   FB_X_FLOORDIV_I acc <- floor(acc / B); B an immediate >= 1 (rescale to a coarser unit)
+ *   FB_X_TS_PART    acc <- field of acc; imm = fb_time_field | fb_time_unit << 8, no operand.  FB_TF_SECOND is the
+ *                   whole second 0-59; FB_TF_WEEK / FB_TF_ISOYEAR are those of the week's Thursday (ISO 8601)
+ *   FB_X_TS_TRUNC   acc <- acc truncated to the start of its part, in the same unit; imm = fb_time_part | unit << 8
+ *   FB_X_TS_INDEX   acc <- whole parts from 1970-01-01 00:00 to acc (weeks: from Monday 1969-12-29); same imm.
+ *                   DATEDIFF(part, a, b) is INDEX(b) - INDEX(a)
+ *   FB_X_TS_ADDMON  acc <- acc + B calendar months (B of any operand kind, int64): month index y * 12 + m - 1 + B with
+ *                   floor arithmetic, the day clamped to the last day of the target month, the time of day kept;
+ *                   the unit sits in flags >> FB_XF_UNIT_SHIFT
  * Column types: FB_T_U16 / FB_T_U32 load zero-extended, FB_T_F16 loads its IEEE half value exactly.
  * Stores keep the low bits of an integer (unsigned stores are the signed ones of the same width) and
  * round a float to nearest even (FB_T_F32, FB_T_F16).
@@ -526,9 +541,23 @@ enum fb_expr_op {
   FB_X_SEL = 39, FB_X_MOD_I = 40, FB_X_RMOD_I = 41, FB_X_MOD_F = 42, FB_X_RMOD_F = 43,
   FB_X_ABS_I = 44, FB_X_ABS_F = 45, FB_X_FLOOR_F = 46, FB_X_CEIL_F = 47, FB_X_ROUND_F = 48, FB_X_ROUND_I = 49,
   FB_X_SQRT = 50, FB_X_EXP = 51, FB_X_LN = 52, FB_X_LOG10 = 53, FB_X_POW = 54, FB_X_RPOW = 55,
-  FB_X_GREATEST_I = 56, FB_X_LEAST_I = 57, FB_X_GREATEST_F = 58, FB_X_LEAST_F = 59
+  FB_X_GREATEST_I = 56, FB_X_LEAST_I = 57, FB_X_GREATEST_F = 58, FB_X_LEAST_F = 59,
+  FB_X_MULSAT_I = 60, FB_X_FLOORDIV_I = 61, FB_X_TS_PART = 62, FB_X_TS_TRUNC = 63, FB_X_TS_INDEX = 64,
+  FB_X_TS_ADDMON = 65
 };
 #define FB_EXPR_ROUND_MAX_DIGITS 18
+#define FB_XF_UNIT_SHIFT 8 /* FB_X_TS_ADDMON: the unit sits in flags >> 8 (imm is free to hold operand B) */
+/* what one count of a temporal value is: date32 = days, date64 = milliseconds, timestamp[s|ms|us|ns] */
+enum fb_time_unit { FB_TU_DAY = 0, FB_TU_S = 1, FB_TU_MS = 2, FB_TU_US = 3, FB_TU_NS = 4, FB_TU_COUNT = 5 };
+enum fb_time_field {
+  FB_TF_YEAR = 0, FB_TF_MONTH = 1, FB_TF_DAY = 2, FB_TF_HOUR = 3, FB_TF_MINUTE = 4, FB_TF_SECOND = 5,
+  FB_TF_QUARTER = 6, FB_TF_DOW = 7 /* 0 = Sunday */, FB_TF_ISODOW = 8 /* 1 = Monday ... 7 */, FB_TF_DOY = 9,
+  FB_TF_WEEK = 10 /* ISO 8601 */, FB_TF_ISOYEAR = 11, FB_TF_COUNT = 12
+};
+enum fb_time_part {
+  FB_TP_YEAR = 0, FB_TP_QUARTER = 1, FB_TP_MONTH = 2, FB_TP_WEEK = 3 /* starts on Monday */, FB_TP_DAY = 4,
+  FB_TP_HOUR = 5, FB_TP_MINUTE = 6, FB_TP_SECOND = 7, FB_TP_COUNT = 8
+};
 typedef struct fb_expr_ins {
   int32_t op;    /* enum fb_expr_op */
   int32_t kind;  /* enum fb_expr_operand: what operand B is */

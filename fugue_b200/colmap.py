@@ -28,7 +28,8 @@ import pyarrow as pa
 import torch
 
 from . import kernels as K
-from .column import PERCENTILES, VARIANCES, ColumnExpr, Kind, SelectColumns, col as _col, has_window, is_agg
+from .column import (BIVARIATES, PERCENTILES, VARIANCES, ColumnExpr, Kind, SelectColumns, bivariate_xy, col as _col,
+                     has_window, is_agg)
 from .table import B200Table, narrow, widen
 
 
@@ -190,19 +191,19 @@ def _with_windows(t: B200Table, cols: List[ColumnExpr]) -> B200Table:
     pre = [_col(nm) for nm in t.schema.names]
     arg_name: Dict[str, str] = {}
     for bare in nodes.values():
-        if not bare.args or bare.arg.kind == Kind.WILDCARD:
-            continue
-        a = bare.arg
-        uid = a.fingerprint()
-        if uid in arg_name:
-            continue
-        if a.kind == Kind.NAMED and a.as_type is None:
-            if a.name not in t.schema:
-                raise KeyError(f"column {a.name} is not in {t.schema}")
-            arg_name[uid] = a.name
-        else:
-            arg_name[uid] = f"__fb_wa{len(arg_name)}"
-            pre.append(a.alias(arg_name[uid]))
+        for a in bare.args:
+            if a.kind == Kind.WILDCARD:
+                continue
+            uid = a.fingerprint()
+            if uid in arg_name:
+                continue
+            if a.kind == Kind.NAMED and a.as_type is None:
+                if a.name not in t.schema:
+                    raise KeyError(f"column {a.name} is not in {t.schema}")
+                arg_name[uid] = a.name
+            else:
+                arg_name[uid] = f"__fb_wa{len(arg_name)}"
+                pre.append(a.alias(arg_name[uid]))
     base = X.project(t, pre) if len(pre) > len(t.schema) else t
     # ---- segments: the logical partitions, one segment when the table has none
     off = t.logical_offsets
@@ -231,6 +232,7 @@ def _with_windows(t: B200Table, cols: List[ColumnExpr]) -> B200Table:
     scans: Dict[Any, List[Any]] = {}
     quantiles: Dict[str, List[Tuple[float, int]]] = {}  # argument column -> its (q, CONT | DISC) pairs
     moments: Dict[str, int] = {}  # argument column of a variance -> its column of the moments scan
+    comoments: Dict[Tuple[str, str], int] = {}  # (x, y) argument columns of a pair -> its pair of the co-moments scan
     finish: List[Any] = []     # per node: (fingerprint, fn(scan results) -> (column, validity, type, dictionary))
 
     def scan(op: int, v: Any, m: Any, frame: Any = None) -> Tuple[Any, int]:
@@ -268,6 +270,20 @@ def _with_windows(t: B200Table, cols: List[ColumnExpr]) -> B200Table:
         def at_end(x: torch.Tensor, whole: Any = whole) -> torch.Tensor:  # partition value: the scan at its last row
             return x if whole is None else x[whole()]
 
+        if fn in BIVARIATES:  # the co-moments scan, one pair per (x, y) shared by its functions; no frames
+            xy = tuple(arg_name[a.fingerprint()] for a in bivariate_xy(bare))
+            for nm in xy:
+                tp = base.schema.types[base.schema.index_of_key(nm)]
+                if not (pa.types.is_integer(tp) or pa.types.is_floating(tp)):
+                    raise NotImplementedError(f"{fn} needs integer or float columns; {nm} is {tp}")
+            j = comoments.setdefault(xy, len(comoments))
+
+            def bivariate(r: Any, j: int = j, e: Any = at_end, fn: str = fn) -> Any:
+                v, vv = bivariate_of(fn, *(e(x) for x in r[("comoments", j)]))
+                return v, vv, pa.int64() if fn == "REGR_COUNT" else pa.float64(), None
+
+            finish.append((uid, bivariate))
+            continue
         if bare.arg.kind == Kind.WILDCARD:  # COUNT(*)
             i = scan(K.AGG_COUNT, None, None, frame)
             finish.append((uid, lambda r, i=i, e=at_end: (e(r[i][1]), None, pa.int64(), None)))
@@ -381,6 +397,16 @@ def _with_windows(t: B200Table, cols: List[ColumnExpr]) -> B200Table:
             v = widen(base.columns[i], base.schema.types[i])
             mcols.append(((v if v.dtype == torch.float64 else v.to(torch.float64)).contiguous(), base.valid[i]))
         results.update((("moments", j), r) for j, r in enumerate(K.segmented_moments(off.contiguous(), n, mcols)))
+    if comoments:
+        pairs = []
+        for xy in comoments:
+            f64 = []
+            for nm in xy:
+                i = base.schema.index_of_key(nm)
+                v = widen(base.columns[i], base.schema.types[i])
+                f64 += [(v if v.dtype == torch.float64 else v.to(torch.float64)).contiguous(), base.valid[i]]
+            pairs.append(tuple(f64))
+        results.update((("comoments", j), r) for j, r in enumerate(K.segmented_comoments(off.contiguous(), n, pairs)))
     names, types, columns, valid = list(base.schema.names), list(base.schema.types), list(base.columns), list(base.valid)
     dicts = dict(base.dictionaries)
     window_names: Dict[str, str] = {}
@@ -407,6 +433,35 @@ def variance_of(fn: str, m2: torch.Tensor, count: torch.Tensor) -> Tuple[torch.T
     v = m2 / torch.where(has, count - (1 if samp else 0), torch.ones_like(count)).to(torch.float64)
     if fn.startswith("STDDEV"):
         v = torch.sqrt(v)
+    return torch.where(has, v, torch.zeros_like(v)).contiguous(), has.to(torch.uint8)
+
+
+def bivariate_of(fn: str, m: torch.Tensor, mx: torch.Tensor, my: torch.Tensor, sxx: torch.Tensor, syy: torch.Tensor,
+                 sxy: torch.Tensor) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
+    """``fn`` (a ``BIVARIATES`` head) from the pair count m, the means of x and y and Sxx, Syy, Sxy over the pair
+    rows: (values, validity or None).  REGR_COUNT is m (int64, never NULL); COVAR_SAMP is NULL when m < 2; every
+    other function is NULL when m = 0, and SLOPE / INTERCEPT / R2 also when Sxx = 0, CORR when Sxx = 0 or Syy = 0.
+    CORR is clamped to [-1, 1] and R2 to [0, 1] (1 when Syy = 0).  A NaN Sxx or Syy is not 0: the result is NaN."""
+    if fn == "REGR_COUNT":
+        return m.contiguous(), None
+    has = m > (1 if fn == "COVAR_SAMP" else 0)
+    mf = m.to(torch.float64)
+    if fn in ("COVAR_POP", "COVAR_SAMP"):
+        v = sxy / torch.where(has, mf - (1 if fn == "COVAR_SAMP" else 0), torch.ones_like(mf))
+    elif fn in ("REGR_AVGX", "REGR_AVGY", "REGR_SXX", "REGR_SYY", "REGR_SXY"):
+        v = {"REGR_AVGX": mx, "REGR_AVGY": my, "REGR_SXX": sxx, "REGR_SYY": syy, "REGR_SXY": sxy}[fn]
+    elif fn == "CORR":
+        has = has & (sxx != 0) & (syy != 0)
+        v = torch.clamp(sxy / (torch.sqrt(sxx) * torch.sqrt(syy)), -1.0, 1.0)
+    else:
+        has = has & (sxx != 0)
+        slope = sxy / sxx
+        if fn == "REGR_SLOPE":
+            v = slope
+        elif fn == "REGR_INTERCEPT":
+            v = my - slope * mx
+        else:  # REGR_R2
+            v = torch.where(syy == 0, torch.ones_like(syy), torch.clamp(sxy * sxy / (sxx * syy), 0.0, 1.0))
     return torch.where(has, v, torch.zeros_like(v)).contiguous(), has.to(torch.uint8)
 
 

@@ -15,9 +15,12 @@ from an expression is a function of ``(kind, head, args)``:
               (a, b), kwarg ``part``; ``ADD_MONTHS``: args (x, n)
     AGG       head in ``SUM COUNT AVG MIN MAX FIRST LAST VAR_SAMP VAR_POP STDDEV_SAMP STDDEV_POP``, one arg,
               optional DISTINCT, or ``PERCENTILE_CONT PERCENTILE_DISC``, one arg and kwarg ``q`` (MEDIAN is
-              PERCENTILE_CONT at q = 0.5)
-    WINDOW    head in the AGG functions (one arg, kwargs ``running``, ``rows`` or ``range``; a percentile keeps
-              its ``q`` and covers the whole partition; a variance takes ``running`` only), ``ROW_NUMBER RANK
+              PERCENTILE_CONT at q = 0.5), or ``CORR COVAR_POP COVAR_SAMP REGR_COUNT REGR_AVGX REGR_AVGY
+              REGR_SXX REGR_SYY REGR_SXY REGR_SLOPE REGR_INTERCEPT REGR_R2``, two args (a, b) as in SQL: the
+              REGR_* functions take the dependent variable y first, (y, x)
+    WINDOW    head in the AGG functions (their args, kwargs ``running``, ``rows`` or ``range``; a percentile keeps
+              its ``q`` and covers the whole partition; a variance or a two-argument aggregate takes ``running``
+              only), ``ROW_NUMBER RANK
               DENSE_RANK`` (no arg) or ``LAG LEAD`` (one arg, kwargs ``n`` and ``default``): evaluated over the logical
               partitions of ``fa.transform`` (PartitionSpec keys, presort order) by a ``ColumnMap``
 
@@ -62,6 +65,10 @@ PERCENTILES = frozenset(["PERCENTILE_CONT", "PERCENTILE_DISC"])
 # sample / population variance and standard deviation (float64); STDDEV and VARIANCE name the sample forms
 VARIANCES = frozenset(["VAR_SAMP", "VAR_POP", "STDDEV_SAMP", "STDDEV_POP"])
 _AGG_ALIASES = {"STDDEV": "STDDEV_SAMP", "VARIANCE": "VAR_SAMP"}
+# SQL:2003 binary set functions of two arguments (float64; REGR_COUNT int64); x is args[0] of CORR / COVAR_*,
+# args[1] of the REGR_* functions (see bivariate_xy)
+BIVARIATES = frozenset(["CORR", "COVAR_POP", "COVAR_SAMP", "REGR_COUNT", "REGR_AVGX", "REGR_AVGY", "REGR_SXX",
+                        "REGR_SYY", "REGR_SXY", "REGR_SLOPE", "REGR_INTERCEPT", "REGR_R2"])
 _RANKINGS = frozenset(["ROW_NUMBER", "RANK", "DENSE_RANK"])
 _RUNNING_FRAME = "ROWS BETWEEN UNBOUNDED PRECEDING AND CURRENT ROW"
 _LITERAL_TYPES = (int, bool, float, str, datetime.date, datetime.datetime, datetime.timedelta)
@@ -204,6 +211,8 @@ class ColumnExpr:
         an aggregation of a named column takes the column's name."""
         if self.kind == Kind.NAMED:
             return self.alias(self.head) if (self.as_name == "" and self.as_type is not None) else self
+        if self.kind in (Kind.AGG, Kind.WINDOW) and self.head in BIVARIATES:
+            return self  # two arguments: no implicit name
         if self.kind in (Kind.UNARY, Kind.AGG) and self.as_name == "":
             return self.alias(self.args[0].infer_alias().output_name)
         if self.kind == Kind.WINDOW and self.as_name == "" and self.args and self.args[0].kind != Kind.WILDCARD:
@@ -252,6 +261,8 @@ class ColumnExpr:
             return pa.float64() if self.head == "PERCENTILE_CONT" else self.args[0].infer_type(schema)
         if k in (Kind.AGG, Kind.WINDOW) and self.head in VARIANCES:
             return pa.float64()
+        if k in (Kind.AGG, Kind.WINDOW) and self.head in BIVARIATES:
+            return pa.int64() if self.head == "REGR_COUNT" else pa.float64()
         if k == Kind.WINDOW:
             if self.head in _RANKINGS or self.head == "COUNT":
                 return pa.int64()
@@ -345,7 +356,8 @@ class ColumnExpr:
             raise ValueError(f"{self} is not an aggregation: only an aggregation has an OVER form")
         if self.is_distinct:
             raise ValueError(f"{self}: DISTINCT aggregations have no window form")
-        if self.head not in WINDOW_AGGS and self.head not in PERCENTILES and self.head not in VARIANCES:
+        if self.head not in WINDOW_AGGS and self.head not in PERCENTILES and self.head not in VARIANCES and \
+                self.head not in BIVARIATES:
             raise ValueError(f"{self}: {self.head} has no window form")
         if not isinstance(running, bool):
             raise ValueError(f"running must be a bool, got {running!r}")
@@ -373,10 +385,10 @@ class ColumnExpr:
                 running, rows = True, None
             elif rows == (None, None):
                 rows = None
-        if self.head in VARIANCES and (rows is not None or range is not None):
+        if (self.head in VARIANCES or self.head in BIVARIATES) and (rows is not None or range is not None):
             raise NotImplementedError(f"{self}: {self.head} runs over the whole partition or running=True; "
                                       "ROWS and RANGE frames are not supported")
-        if is_agg(self.args[0]) or has_window(self.args[0]):
+        if any(is_agg(a) or has_window(a) for a in self.args):
             raise ValueError(f"nested aggregation {self}")
         if self.head in ("FIRST", "LAST") and self.args[0].kind == Kind.WILDCARD:
             raise ValueError(f"{self}: {self.head} needs a column")
@@ -459,6 +471,20 @@ def agg(func: str, arg: Any, as_name: str = "", arg_distinct: bool = False) -> C
     STDDEV_POP (STDDEV and VARIANCE give the sample forms)."""
     func = func.upper()
     return ColumnExpr(Kind.AGG, _AGG_ALIASES.get(func, func), [col(arg)], None, arg_distinct, as_name)
+
+
+def _bivariate(func: str, a: Any, b: Any) -> ColumnExpr:
+    """``FUNC(a, b)`` of ``BIVARIATES``: two row-wise column expressions (or column names)."""
+    args = [col(a), col(b)]
+    for x in args:
+        if x.kind == Kind.WILDCARD or is_agg(x) or has_window(x):
+            raise ValueError(f"{func} needs two row-wise column expressions, got {x}")
+    return ColumnExpr(Kind.AGG, func, args)
+
+
+def bivariate_xy(e: ColumnExpr) -> Tuple[ColumnExpr, ColumnExpr]:
+    """(x, y) of a ``BIVARIATES`` node: (a, b) of ``CORR / COVAR_*(a, b)``, (x, y) of ``REGR_*(y, x)``."""
+    return (e.args[1], e.args[0]) if e.head.startswith("REGR_") else (e.args[0], e.args[1])
 
 
 def _percentile(func: str, c: Any, q: Any) -> ColumnExpr:
@@ -877,6 +903,70 @@ class functions:
     def stddev_pop(c: Any) -> ColumnExpr:
         """sqrt(VAR_POP): pandas ``std(ddof=0)``."""
         return agg("STDDEV_POP", c)
+
+    # ---- two-argument aggregates (SQL:2003 binary set functions, DESIGN §7k).  Only the rows where both
+    # arguments are non-NULL take part; m is their number.  NaN and +-inf are values, not NULL.
+    @staticmethod
+    def corr(a: Any, b: Any) -> ColumnExpr:
+        """Pearson's correlation Sab / sqrt(Saa Sbb), clamped to [-1, 1] (float64; NULL when m = 0 or either
+        argument is constant over the pair rows)."""
+        return _bivariate("CORR", a, b)
+
+    @staticmethod
+    def covar_pop(a: Any, b: Any) -> ColumnExpr:
+        """Population covariance Sab / m (float64; NULL when m = 0)."""
+        return _bivariate("COVAR_POP", a, b)
+
+    @staticmethod
+    def covar_samp(a: Any, b: Any) -> ColumnExpr:
+        """Sample covariance Sab / (m - 1): pandas ``cov()`` (float64; NULL when m < 2)."""
+        return _bivariate("COVAR_SAMP", a, b)
+
+    @staticmethod
+    def regr_count(y: Any, x: Any) -> ColumnExpr:
+        """m, the number of rows where both are non-NULL (int64, never NULL)."""
+        return _bivariate("REGR_COUNT", y, x)
+
+    @staticmethod
+    def regr_avgx(y: Any, x: Any) -> ColumnExpr:
+        """The mean of x over the pair rows (float64; NULL when m = 0)."""
+        return _bivariate("REGR_AVGX", y, x)
+
+    @staticmethod
+    def regr_avgy(y: Any, x: Any) -> ColumnExpr:
+        """The mean of y over the pair rows (float64; NULL when m = 0)."""
+        return _bivariate("REGR_AVGY", y, x)
+
+    @staticmethod
+    def regr_sxx(y: Any, x: Any) -> ColumnExpr:
+        """Sxx = sum of (x - mean x)^2 over the pair rows (float64; NULL when m = 0)."""
+        return _bivariate("REGR_SXX", y, x)
+
+    @staticmethod
+    def regr_syy(y: Any, x: Any) -> ColumnExpr:
+        """Syy = sum of (y - mean y)^2 over the pair rows (float64; NULL when m = 0)."""
+        return _bivariate("REGR_SYY", y, x)
+
+    @staticmethod
+    def regr_sxy(y: Any, x: Any) -> ColumnExpr:
+        """Sxy = sum of (x - mean x)(y - mean y) over the pair rows (float64; NULL when m = 0)."""
+        return _bivariate("REGR_SXY", y, x)
+
+    @staticmethod
+    def regr_slope(y: Any, x: Any) -> ColumnExpr:
+        """The least-squares slope Sxy / Sxx of y on x (float64; NULL when m = 0 or Sxx = 0)."""
+        return _bivariate("REGR_SLOPE", y, x)
+
+    @staticmethod
+    def regr_intercept(y: Any, x: Any) -> ColumnExpr:
+        """The least-squares intercept mean y - slope * mean x (float64; NULL when m = 0 or Sxx = 0)."""
+        return _bivariate("REGR_INTERCEPT", y, x)
+
+    @staticmethod
+    def regr_r2(y: Any, x: Any) -> ColumnExpr:
+        """The coefficient of determination: 1 when Syy = 0, else Sxy^2 / (Sxx Syy) clamped to [0, 1] (float64;
+        NULL when m = 0 or Sxx = 0)."""
+        return _bivariate("REGR_R2", y, x)
 
     @staticmethod
     def percentile_cont(c: Any, q: Any) -> ColumnExpr:

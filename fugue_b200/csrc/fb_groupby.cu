@@ -26,6 +26,10 @@
 // again, finds each row's slot without inserting, and adds d = x - SUM / COUNT and d^2.  The host forms
 // M2 = DEV2 - DEV^2 / m: Chan, Golub & LeVeque's corrected two-pass, whose correction term cancels the
 // first-order error of the atomically summed mean.
+//
+// Covariance (FB_AGG_CODEV_F64, DESIGN §7k): pass B also adds dx * dy of a pair row into CODEV, with dx and dy the
+// row's deviations from its group's SUM / COUNT of x and of y; Sxy = CODEV - DEVx * DEVy / m is the same
+// correction applied to the cross sum.
 #include "fb_common.cuh"
 
 namespace {
@@ -43,6 +47,7 @@ enum : int32_t {
   kMaxF64 = FB_AGG_MAX_F64,
   kDevF64 = FB_AGG_DEV_F64,
   kDev2F64 = FB_AGG_DEV2_F64,
+  kCodevF64 = FB_AGG_CODEV_F64,
 };
 
 struct AggSpec {
@@ -60,9 +65,20 @@ struct DevCol {
   const uint8_t* valid;
   int32_t sum, cnt, dev, dev2;  // accumulator indices; dev / dev2 = -1 when not asked for
 };
+// a pair (x, y) with cross deviations: SUM of x, SUM of y, COUNT, CODEV and the DEV of y it is tied to, so at
+// most FB_MAX_AGGS / 5 pairs fit in one call
+constexpr int kMaxPairs = FB_MAX_AGGS / 5;
+struct PairCol {
+  const double* x;
+  const double* y;
+  const uint8_t* valid;  // the pair validity: both x and y present
+  int32_t sumx, sumy, cnt, codev;
+};
 struct DevSpec {
   DevCol col[kMaxDevCols];
   int32_t ncols;
+  PairCol pair[kMaxPairs];
+  int32_t npairs;
 };
 
 __host__ __device__ inline int slot_words(int naggs) { return (1 + naggs + 3) & ~3; }
@@ -115,6 +131,7 @@ __device__ __forceinline__ void apply_aggs(uint64_t* __restrict__ slot, const Ag
 #pragma unroll 1
   for (int a = 0; a < spec.naggs; ++a) {
     const int op = spec.op[a];
+    if (op >= kDevF64) continue;  // deviations: pass B
     if (spec.valid[a] != nullptr && spec.valid[a][row] == 0) continue;  // NULL value: skipped
     if (op == kCount) {
       atomicAdd((unsigned long long*)(slot + 1 + a), 1ULL);
@@ -418,6 +435,16 @@ fb_groupby_dev_kernel(const uint64_t* __restrict__ keys, const uint8_t* __restri
       if (d.dev >= 0) atomicAdd((double*)(slot + 1 + d.dev), dx);
       if (d.dev2 >= 0) atomicAdd((double*)(slot + 1 + d.dev2), dx * dx);
     }
+    if (kLean) continue;  // a pair's accumulators never fit the lean kernel
+#pragma unroll 1
+    for (int p = 0; p < spec.npairs; ++p) {
+      const PairCol& q = spec.pair[p];
+      if (q.valid != nullptr && q.valid[row] == 0) continue;  // not a pair row
+      const double m = (double)(long long)slot[1 + q.cnt];
+      const double mx = __longlong_as_double((long long)slot[1 + q.sumx]) / m;
+      const double my = __longlong_as_double((long long)slot[1 + q.sumy]) / m;
+      atomicAdd((double*)(slot + 1 + q.codev), (q.x[row] - mx) * (q.y[row] - my));
+    }
   }
 }
 
@@ -453,7 +480,8 @@ fb_groupby_extract_kernel(const uint64_t* __restrict__ table, int64_t capacity, 
   }
 }
 
-// also resolves every FB_AGG_DEV_F64 / FB_AGG_DEV2_F64 to the SUM and COUNT of its column (pass B's DevSpec)
+// also resolves every FB_AGG_DEV_F64 / FB_AGG_DEV2_F64 to the SUM and COUNT of its column, and every
+// FB_AGG_CODEV_F64 to its y (the DEV_F64 right after it) and the SUMs and COUNT of its pair (pass B's DevSpec)
 int fill_spec(AggSpec& spec, DevSpec& dev, int naggs, const void* const* val_ptrs, const uint8_t* const* val_valid,
               const int32_t* ops) {
   FB_CHECK(naggs >= 0 && naggs <= FB_MAX_AGGS, "naggs=%d out of range [0,%d]", naggs, FB_MAX_AGGS);
@@ -461,7 +489,7 @@ int fill_spec(AggSpec& spec, DevSpec& dev, int naggs, const void* const* val_ptr
   memset(&dev, 0, sizeof(dev));
   spec.naggs = naggs;
   for (int a = 0; a < naggs; ++a) {
-    FB_CHECK(ops[a] >= FB_AGG_SUM_F64 && ops[a] <= FB_AGG_DEV2_F64, "unknown aggregate op %d", ops[a]);
+    FB_CHECK(ops[a] >= FB_AGG_SUM_F64 && ops[a] <= FB_AGG_CODEV_F64, "unknown aggregate op %d", ops[a]);
     FB_CHECK(ops[a] == FB_AGG_COUNT || (val_ptrs != nullptr && val_ptrs[a] != nullptr),
              "aggregate %d needs a value column", a);
     spec.op[a] = ops[a];
@@ -477,14 +505,38 @@ int fill_spec(AggSpec& spec, DevSpec& dev, int naggs, const void* const* val_ptr
     }
     FB_CHECK(sum >= 0 && cnt >= 0, "aggregate %d (op %d) needs a SUM_F64 and a COUNT of the same column and validity",
              a, ops[a]);
+    // the entry of this column whose DEV (or DEV2) is still free: a second DEV of the same column and validity gets
+    // an entry of its own instead of taking the first one's place (which would leave that accumulator at 0)
+    const bool is_dev = ops[a] == kDevF64;
     int c = 0;
-    while (c < dev.ncols && !(dev.col[c].val == (const double*)spec.val[a] && dev.col[c].valid == spec.valid[a])) ++c;
+    while (c < dev.ncols && !(dev.col[c].val == (const double*)spec.val[a] && dev.col[c].valid == spec.valid[a] &&
+                              (is_dev ? dev.col[c].dev : dev.col[c].dev2) < 0))
+      ++c;
     if (c == dev.ncols) {
       FB_CHECK(c < kMaxDevCols, "more than %d value columns with deviations", kMaxDevCols);
       dev.col[c] = DevCol{(const double*)spec.val[a], spec.valid[a], sum, cnt, -1, -1};
       ++dev.ncols;
     }
-    (ops[a] == kDevF64 ? dev.col[c].dev : dev.col[c].dev2) = a;
+    (is_dev ? dev.col[c].dev : dev.col[c].dev2) = a;
+  }
+  for (int a = 0; a < naggs; ++a) {
+    if (ops[a] != kCodevF64) continue;
+    FB_CHECK(a + 1 < naggs && ops[a + 1] == kDevF64 && spec.valid[a + 1] == spec.valid[a],
+             "aggregate %d (CODEV) must be followed by the DEV_F64 of its y with the same validity", a);
+    const uint64_t* x = spec.val[a];
+    const uint64_t* y = spec.val[a + 1];
+    int sumx = -1, sumy = -1, cnt = -1;
+    for (int b = 0; b < naggs; ++b) {
+      if (ops[b] == kSumF64 && spec.valid[b] == spec.valid[a]) {
+        if (sumx < 0 && spec.val[b] == x) sumx = b;
+        if (sumy < 0 && spec.val[b] == y) sumy = b;
+      }
+      if (cnt < 0 && ops[b] == kCount && spec.valid[b] == spec.valid[a]) cnt = b;
+    }
+    FB_CHECK(sumx >= 0 && sumy >= 0 && cnt >= 0,
+             "aggregate %d (CODEV) needs a SUM_F64 of x, a SUM_F64 of y and a COUNT of the pair validity", a);
+    FB_CHECK(dev.npairs < kMaxPairs, "more than %d pairs with cross deviations", kMaxPairs);
+    dev.pair[dev.npairs++] = PairCol{(const double*)x, (const double*)y, spec.valid[a], sumx, sumy, cnt, a};
   }
   return 0;
 }
@@ -544,7 +596,7 @@ int fb_groupby_u64(int dev, void* stream, int64_t nrows, const void* keys, const
       fb_groupby_kernel<<<(unsigned)gb, 256, 0, st>>>((const uint64_t*)keys, key_valid, nrows, (uint64_t*)table,
                                                      capacity, words, spec, d_status, dv, region_shift,
                                                      d_part_offsets, (int)p0, (int)p1);
-      if (devs.ncols > 0)  // pass B of the batch while its regions are still in L2
+      if (devs.ncols + devs.npairs > 0)  // pass B of the batch while its regions are still in L2
         fb_groupby_dev_kernel<false><<<(unsigned)gb, 256, 0, st>>>((const uint64_t*)keys, key_valid, nrows,
                                                                   (uint64_t*)table, capacity, words, devs, dv,
                                                                   region_shift, 0u, d_part_offsets, (int)p0, (int)p1);
@@ -566,7 +618,7 @@ int fb_groupby_u64(int dev, void* stream, int64_t nrows, const void* keys, const
       case 3: launch_lean<3>(k64, key_valid, nrows, t64, capacity, spec, d_status, num_parts, (int)region_shift, sms * 8, st); break;
       default: launch_lean<4>(k64, key_valid, nrows, t64, capacity, spec, d_status, num_parts, (int)region_shift, sms * 8, st); break;
     }
-    if (devs.ncols > 0)
+    if (devs.ncols + devs.npairs > 0)
       fb_groupby_dev_kernel<true><<<sms * 8, 256, 0, st>>>(k64, key_valid, nrows, t64, capacity, words, devs, dv,
                                                           region_shift, num_parts - 1, nullptr, 0, 0);
     FB_CUDA(cudaGetLastError());
@@ -575,7 +627,7 @@ int fb_groupby_u64(int dev, void* stream, int64_t nrows, const void* keys, const
   if (nrows > 0) {
     fb_groupby_kernel<<<sms * 8, 256, 0, st>>>((const uint64_t*)keys, key_valid, nrows, (uint64_t*)table,
                                               capacity, words, spec, d_status, dv, region_shift, nullptr, 0, 0);
-    if (devs.ncols > 0)
+    if (devs.ncols + devs.npairs > 0)
       fb_groupby_dev_kernel<false><<<sms * 8, 256, 0, st>>>((const uint64_t*)keys, key_valid, nrows, (uint64_t*)table,
                                                            capacity, words, devs, dv, region_shift, 0u, nullptr, 0, 0);
     FB_CUDA(cudaGetLastError());

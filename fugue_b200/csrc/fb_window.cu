@@ -143,8 +143,48 @@ __device__ __forceinline__ MSt shfl_down(const MSt& s, int d) {
              __shfl_down_sync(0xFFFFFFFFu, s.m2, d), __shfl_down_sync(0xFFFFFFFFu, s.f, d)};
 }
 
+// (count, mean x, mean y, Sxx, Syy, Sxy, "a segment starts in here") of the pair rows of a run of consecutive
+// rows: the state of fb_segmented_comoments
+struct CSt {
+  int64_t c;
+  double mx, my, sxx, syy, sxy;
+  int32_t f;
+};
+
+// `a` followed by `b`: Chan's pairwise update with the cross term dx * dy * na * nb / n.  A non-finite mean
+// difference means a non-finite value (or an overflow): the mean is then the weighted sum of the two, which
+// gives +-inf or NaN as the sum of the values would, where the update form would give inf - inf = NaN.
+__device__ __forceinline__ CSt combine(int, const CSt& a, const CSt& b) {
+  if (b.f) return b;
+  if (b.c == 0) return CSt{a.c, a.mx, a.my, a.sxx, a.syy, a.sxy, a.f};
+  if (a.c == 0) return CSt{b.c, b.mx, b.my, b.sxx, b.syy, b.sxy, a.f};
+  const int64_t n = a.c + b.c;
+  const double dx = b.mx - a.mx, dy = b.my - a.my;
+  const double rn = __drcp_rn((double)n);
+  const double wb = (double)b.c * rn;  // nb / n within 2 u
+  const double na = (double)a.c, nb = (double)b.c;
+  const double mx = isfinite(dx) ? a.mx + dx * wb : (a.mx * na + b.mx * nb) * rn;
+  const double my = isfinite(dy) ? a.my + dy * wb : (a.my * na + b.my * nb) * rn;
+  return CSt{n, mx, my, a.sxx + b.sxx + dx * dx * na * wb, a.syy + b.syy + dy * dy * na * wb,
+             a.sxy + b.sxy + dx * dy * na * wb, a.f};
+}
+
+__device__ __forceinline__ CSt shfl_up(const CSt& s, int d) {
+  return CSt{(int64_t)__shfl_up_sync(0xFFFFFFFFu, (long long)s.c, d), __shfl_up_sync(0xFFFFFFFFu, s.mx, d),
+             __shfl_up_sync(0xFFFFFFFFu, s.my, d), __shfl_up_sync(0xFFFFFFFFu, s.sxx, d),
+             __shfl_up_sync(0xFFFFFFFFu, s.syy, d), __shfl_up_sync(0xFFFFFFFFu, s.sxy, d),
+             __shfl_up_sync(0xFFFFFFFFu, s.f, d)};
+}
+
+__device__ __forceinline__ CSt shfl_down(const CSt& s, int d) {
+  return CSt{(int64_t)__shfl_down_sync(0xFFFFFFFFu, (long long)s.c, d), __shfl_down_sync(0xFFFFFFFFu, s.mx, d),
+             __shfl_down_sync(0xFFFFFFFFu, s.my, d), __shfl_down_sync(0xFFFFFFFFu, s.sxx, d),
+             __shfl_down_sync(0xFFFFFFFFu, s.syy, d), __shfl_down_sync(0xFFFFFFFFu, s.sxy, d),
+             __shfl_down_sync(0xFFFFFFFFu, s.f, d)};
+}
+
 // Exclusive scan of one state per thread across the CTA, and the CTA total; fixed combination order.
-// kRev: the scan runs from the last thread to the first.  S: St, or MSt (op unused).
+// kRev: the scan runs from the last thread to the first.  S: St, or MSt / CSt (op unused).
 template <int kWarps, bool kRev = false, class S = St>
 __device__ __forceinline__ S block_exclusive(int op, const S& x, S* warp_tot, S* total) {
   const int lane = kRev ? 31 - (threadIdx.x & 31) : threadIdx.x & 31;
@@ -432,6 +472,137 @@ fb_segmoments_carry_kernel(int64_t ntiles, int64_t* __restrict__ tile_c, double*
     tc[t] = run.c;
     tm[t] = run.mean;
     tq[t] = run.m2;
+    run = combine(0, run, x);
+  }
+}
+
+// ---- segmented co-moments (fb_segmented_comoments): the same three launches over CSt --------------------
+struct CoCols {
+  const double* x[FB_SCAN_MAX_COLS];
+  const double* y[FB_SCAN_MAX_COLS];
+  const uint8_t* vx[FB_SCAN_MAX_COLS];
+  const uint8_t* vy[FB_SCAN_MAX_COLS];
+  int64_t* out_count[FB_SCAN_MAX_COLS];
+  double* out[5][FB_SCAN_MAX_COLS];  // mean x, mean y, Sxx, Syy, Sxy
+  int32_t ncols;
+};
+
+// the tile states of every pair, column-major (pair * ntiles + tile); f: one per tile
+struct CoTiles {
+  int64_t* c;
+  double* mx;
+  double* my;
+  double* sxx;
+  double* syy;
+  double* sxy;
+  int32_t* f;
+};
+
+struct CoSmem {
+  double x[padded(kTile)];
+  double y[padded(kTile)];
+  uint8_t valid[kTile];  // x and y both valid
+  uint8_t head[kTile];
+  CSt warp_tot[kThreads / 32];
+  int64_t seg_range[2];
+};
+
+// the state of one row: a pair enters as (1, x, y, z, z, z) with z = (x - x) * (y - y), +0 for finite x and y and
+// NaN otherwise, so that a NaN or an infinity on either side makes all three sums NaN
+__device__ __forceinline__ CSt comoment_of(const CoSmem& sm, int j) {
+  const int c = sm.valid[j];
+  const double x = c ? sm.x[padded(j)] : 0.0, y = c ? sm.y[padded(j)] : 0.0;
+  const double z = (x - x) * (y - y);
+  return CSt{c, x, y, z, z, z, sm.head[j]};
+}
+
+// kFinal = false: pass 1 (tile states); true: pass 3 (the running state per row, from the carries).  Pass 3
+// stores a thread's kItems consecutive rows straight from registers: six outputs per row do not fit the staging
+// buffers, and the stores of a warp still cover whole lines together.
+template <bool kFinal>
+__global__ void __launch_bounds__(kThreads)
+fb_segcomoments_tile_kernel(int64_t nrows, int64_t nseg, const int64_t* __restrict__ offsets,
+                            const __grid_constant__ CoCols a, int64_t ntiles, CoTiles ts) {
+  __shared__ __align__(16) CoSmem sm;
+  const int64_t tile = blockIdx.x;
+  const int64_t start = tile * kTile;
+  const int64_t end = start + kTile < nrows ? start + kTile : nrows;
+  const int nloc = (int)(end - start);
+  mark_heads<false, false>(nrows, nseg, offsets, start, end, 0, sm.head, sm.seg_range);
+  const int j0 = threadIdx.x * kItems;
+  for (int col = 0; col < a.ncols; ++col) {
+    const double* __restrict__ xs = a.x[col];
+    const double* __restrict__ ys = a.y[col];
+    const uint8_t* __restrict__ vx = a.vx[col];
+    const uint8_t* __restrict__ vy = a.vy[col];
+    for (int i = threadIdx.x; i < kTile; i += kThreads) {
+      const bool in = i < nloc;
+      sm.x[padded(i)] = in ? __ldg(xs + start + i) : 0.0;
+      sm.y[padded(i)] = in ? __ldg(ys + start + i) : 0.0;
+      sm.valid[i] = in && (vx == nullptr || __ldg(vx + start + i) != 0) && (vy == nullptr || __ldg(vy + start + i) != 0);
+    }
+    __syncthreads();
+    CSt acc{};
+#pragma unroll
+    for (int k = 0; k < kItems; ++k) acc = combine(0, acc, comoment_of(sm, j0 + k));
+    CSt total;
+    const CSt pre = block_exclusive<kThreads / 32, false, CSt>(0, acc, sm.warp_tot, &total);
+    const int64_t t = col * ntiles + tile;
+    if (!kFinal) {
+      if (threadIdx.x == 0) {
+        ts.c[t] = total.c;
+        ts.mx[t] = total.mx;
+        ts.my[t] = total.my;
+        ts.sxx[t] = total.sxx;
+        ts.syy[t] = total.syy;
+        ts.sxy[t] = total.sxy;
+        if (col == 0) ts.f[tile] = total.f;
+      }
+      continue;
+    }
+    CSt run = combine(0, CSt{ts.c[t], ts.mx[t], ts.my[t], ts.sxx[t], ts.syy[t], ts.sxy[t], 0}, pre);
+    int64_t* __restrict__ oc = a.out_count[col];
+#pragma unroll
+    for (int k = 0; k < kItems; ++k) {
+      const int j = j0 + k;
+      run = combine(0, run, comoment_of(sm, j));
+      if (j >= nloc) continue;
+      const bool any = run.c > 0;  // no pair row yet: 0, not whatever preceded the segment
+      const double v[5] = {run.mx, run.my, run.sxx, run.syy, run.sxy};
+      if (oc != nullptr) oc[start + j] = run.c;
+#pragma unroll
+      for (int o = 0; o < 5; ++o)
+        if (a.out[o][col] != nullptr) a.out[o][col][start + j] = any ? v[o] : 0.0;
+    }
+    __syncthreads();  // shared buffers are refilled by the next pair
+  }
+}
+
+// pass 2: per pair, the exclusive segmented scan of the tile states (in place: state -> carry).  Half the
+// threads of the other carry kernels: a CSt is twice an MSt, and 1024 threads leave 64 registers each.
+constexpr int kCoCarryThreads = 512;
+__global__ void __launch_bounds__(kCoCarryThreads, 1)
+fb_segcomoments_carry_kernel(int64_t ntiles, CoTiles ts) {
+  __shared__ CSt warp_tot[kCoCarryThreads / 32];
+  const int64_t o = (int64_t)blockIdx.x * ntiles;
+  const int64_t per = (ntiles + kCoCarryThreads - 1) / kCoCarryThreads;
+  const int64_t b = threadIdx.x * per;
+  const int64_t e = b + per < ntiles ? b + per : ntiles;
+  auto load = [&](int64_t t) {
+    return CSt{ts.c[o + t], ts.mx[o + t], ts.my[o + t], ts.sxx[o + t], ts.syy[o + t], ts.sxy[o + t], ts.f[t]};
+  };
+  CSt acc{};
+  for (int64_t t = b; t < e; ++t) acc = combine(0, acc, load(t));
+  CSt total;
+  CSt run = block_exclusive<kCoCarryThreads / 32, false, CSt>(0, acc, warp_tot, &total);
+  for (int64_t t = b; t < e; ++t) {
+    const CSt x = load(t);
+    ts.c[o + t] = run.c;
+    ts.mx[o + t] = run.mx;
+    ts.my[o + t] = run.my;
+    ts.sxx[o + t] = run.sxx;
+    ts.syy[o + t] = run.syy;
+    ts.sxy[o + t] = run.sxy;
     run = combine(0, run, x);
   }
 }
@@ -988,6 +1159,59 @@ extern "C" int fb_segmented_moments(int dev, void* stream, int64_t nrows, int64_
   FB_CUDA(cudaGetLastError());
   fb_segmoments_tile_kernel<true><<<(unsigned)ntiles, kThreads, 0, st>>>(nrows, nseg, d_offsets, a, ntiles, tile_c,
                                                                          tile_mean, tile_m2, tile_f);
+  FB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+extern "C" size_t fb_segmented_comoments_scratch_bytes(int64_t nrows, int npairs) {
+  if (nrows <= 0 || npairs <= 0) return 0;
+  return (size_t)num_tiles(nrows) * (48 * (size_t)npairs + 4);
+}
+
+extern "C" int fb_segmented_comoments(int dev, void* stream, int64_t nrows, int64_t nseg, const int64_t* d_offsets,
+                                      int npairs, const void* const* xs, const uint8_t* const* x_valid,
+                                      const void* const* ys, const uint8_t* const* y_valid, int64_t* const* out_count,
+                                      void* const* out_mean_x, void* const* out_mean_y, void* const* out_sxx,
+                                      void* const* out_syy, void* const* out_sxy, void* scratch,
+                                      size_t scratch_bytes) {
+  FB_CHECK(nrows >= 0 && nseg >= 0, "negative row or segment count");
+  FB_CHECK(npairs >= 1 && npairs <= FB_SCAN_MAX_COLS, "npairs=%d out of range [1,%d]", npairs, FB_SCAN_MAX_COLS);
+  CoCols a;
+  memset(&a, 0, sizeof(a));
+  a.ncols = npairs;
+  void* const* outs[5] = {out_mean_x, out_mean_y, out_sxx, out_syy, out_sxy};
+  for (int c = 0; c < npairs; ++c) {
+    a.x[c] = xs != nullptr ? (const double*)xs[c] : nullptr;
+    a.y[c] = ys != nullptr ? (const double*)ys[c] : nullptr;
+    a.vx[c] = x_valid != nullptr ? x_valid[c] : nullptr;
+    a.vy[c] = y_valid != nullptr ? y_valid[c] : nullptr;
+    a.out_count[c] = out_count != nullptr ? out_count[c] : nullptr;
+    for (int o = 0; o < 5; ++o) a.out[o][c] = outs[o] != nullptr ? (double*)outs[o][c] : nullptr;
+    FB_CHECK(nrows == 0 || (a.x[c] != nullptr && a.y[c] != nullptr), "pair %d needs an x and a y column", c);
+  }
+  if (nrows == 0) return 0;
+  FB_CHECK(nseg >= 1 && d_offsets != nullptr, "%lld rows need at least one segment", (long long)nrows);
+  FB_CHECK(num_tiles(nrows) < (1LL << 31), "too many rows");
+  FB_CHECK(scratch != nullptr && scratch_bytes >= fb_segmented_comoments_scratch_bytes(nrows, npairs),
+           "scratch too small: %zu < %zu", scratch_bytes, fb_segmented_comoments_scratch_bytes(nrows, npairs));
+  FbDeviceGuard guard(dev);
+  FB_CHECK(guard.ok, "cannot select device %d", dev);
+  cudaStream_t st = (cudaStream_t)stream;
+  const int64_t ntiles = num_tiles(nrows);
+  const int64_t nt = npairs * ntiles;
+  CoTiles ts;
+  ts.c = (int64_t*)scratch;
+  ts.mx = (double*)(ts.c + nt);
+  ts.my = ts.mx + nt;
+  ts.sxx = ts.my + nt;
+  ts.syy = ts.sxx + nt;
+  ts.sxy = ts.syy + nt;
+  ts.f = (int32_t*)(ts.sxy + nt);
+  fb_segcomoments_tile_kernel<false><<<(unsigned)ntiles, kThreads, 0, st>>>(nrows, nseg, d_offsets, a, ntiles, ts);
+  FB_CUDA(cudaGetLastError());
+  fb_segcomoments_carry_kernel<<<npairs, kCoCarryThreads, 0, st>>>(ntiles, ts);
+  FB_CUDA(cudaGetLastError());
+  fb_segcomoments_tile_kernel<true><<<(unsigned)ntiles, kThreads, 0, st>>>(nrows, nseg, d_offsets, a, ntiles, ts);
   FB_CUDA(cudaGetLastError());
   return 0;
 }

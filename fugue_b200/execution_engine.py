@@ -10,7 +10,8 @@ The arithmetic runs in ``libfugue_b200.so`` through ``fugue_b200.kernels``; ther
 no CPU implementation of the partition/join/aggregate steps in this package.
 """
 import logging
-from typing import Any, Callable, Dict, List, Optional
+import math
+from typing import Any, Callable, Dict, List, Optional, Tuple
 
 import pandas as pd
 import pyarrow as pa
@@ -259,6 +260,30 @@ def decompose_aggs(agg_cols: List[Any]) -> Any:
         else:
             raise NotImplementedError(f"{a.func} has no partial / final decomposition")
     return partial, final, post
+
+
+def _dev_key(v: torch.Tensor, m: Optional[torch.Tensor]) -> Tuple[int, int]:
+    return v.data_ptr(), 0 if m is None else m.data_ptr()
+
+
+def _deviations(devs: Dict[Tuple[int, int], Any], add: Any, v: torch.Tensor, m: Optional[torch.Tensor]) -> Any:
+    """The (SUM, COUNT, DEV, DEV2) accumulators of the f64 column ``v`` with validity ``m``, added once per call.  K6
+    resolves a DEV / DEV2 to its column by (value pointer, validity pointer), so a second set for the same pointers
+    would be ambiguous (DESIGN §7i, §7k)."""
+    k = _dev_key(v, m)
+    if k not in devs:
+        devs[k] = (add(v, m, K.AGG_SUM_F64), add(None, m, K.AGG_COUNT), add(v, m, K.AGG_DEV_F64),
+                   add(v, m, K.AGG_DEV2_F64))
+    return devs[k]
+
+
+def _f64_column(t: "B200Table", name: str, wide: Dict[str, torch.Tensor]) -> torch.Tensor:
+    """Column ``name`` of ``t`` widened to contiguous f64 as AVG reads it, once per call (``wide`` caches it)."""
+    if name not in wide:
+        i = t.schema.index_of_key(name)
+        v = widen(t.columns[i], t.schema.types[i])
+        wide[name] = (v if v.dtype == torch.float64 else v.to(torch.float64)).contiguous()
+    return wide[name]
 
 
 def finish_avgs(res: "B200DataFrame", post: List[Any], want: List[str]) -> "B200DataFrame":
@@ -586,16 +611,22 @@ class B200ExecutionEngine(EngineLifecycle):
 
     @staticmethod
     def _plain_aggs(agg_cols: List[Any]) -> bool:
-        """``SUM/COUNT/MIN/MAX/AVG/FIRST/LAST/PERCENTILE_*`` of a named column (or ``*``) without casts: what
-        ``_aggregate_named`` takes directly (and what the distributed engine decomposes into partial / final)."""
-        from .column import VARIANCES, ColumnExpr, Kind
+        """``SUM/COUNT/MIN/MAX/AVG/FIRST/LAST/PERCENTILE_*`` of a named column (or ``*``) without casts, and the
+        two-argument aggregates of two named columns: what ``_aggregate_named`` takes directly (and what the
+        distributed engine decomposes into partial / final)."""
+        from .column import BIVARIATES, VARIANCES, ColumnExpr, Kind
+
+        def one_arg(a: Any) -> bool:
+            return (a.func in ("SUM", "COUNT", "MIN", "MAX", "AVG", "FIRST", "LAST", "PERCENTILE_CONT",
+                               "PERCENTILE_DISC") or a.func in VARIANCES) \
+                and a.arg.kind in (Kind.NAMED, Kind.WILDCARD) and a.arg.as_type is None \
+                and not (a.func in ("FIRST", "LAST") and a.arg.kind == Kind.WILDCARD)
+
+        def two_args(a: Any) -> bool:
+            return a.func in BIVARIATES and all(x.kind == Kind.NAMED and x.as_type is None for x in a.args)
 
         return all(isinstance(a, ColumnExpr) and a.kind == Kind.AGG and a.as_type is None and not a.is_distinct
-                   and (a.func in ("SUM", "COUNT", "MIN", "MAX", "AVG", "FIRST", "LAST", "PERCENTILE_CONT",
-                                   "PERCENTILE_DISC") or a.func in VARIANCES)
-                   and a.arg.kind in (Kind.NAMED, Kind.WILDCARD) and a.arg.as_type is None
-                   and not (a.func in ("FIRST", "LAST") and a.arg.kind == Kind.WILDCARD)
-                   for a in agg_cols)
+                   and (two_args(a) or one_arg(a)) for a in agg_cols)
 
     def _aggregate_named(self, df: Any, partition_spec: Optional[PartitionSpec],
                          agg_cols: List[Any]) -> B200DataFrame:
@@ -603,8 +634,8 @@ class B200ExecutionEngine(EngineLifecycle):
         import pyarrow as pa
 
         from . import sort as S
-        from .colmap import variance_of
-        from .column import PERCENTILES, VARIANCES
+        from .colmap import bivariate_of, variance_of
+        from .column import BIVARIATES, PERCENTILES, VARIANCES, bivariate_xy
 
         if any(a.func in PERCENTILES for a in agg_cols):
             return self._aggregate_sorted(df, partition_spec, agg_cols)
@@ -672,8 +703,19 @@ class B200ExecutionEngine(EngineLifecycle):
                                   add(None, m, K.AGG_COUNT) if m is not None else None))
             rows_slot = add(None, None, K.AGG_COUNT)
         rowno: Any = None
-        moments: Dict[str, Any] = {}  # argument column -> its (SUM, COUNT, DEV, DEV2) accumulators
+        # (value pointer, validity pointer) -> its (SUM, COUNT, DEV, DEV2) accumulators, shared by every variance and
+        # pair of the call: K6 ties a DEV / DEV2 to its column by these two pointers, so each column needs one set
+        devs: Dict[Tuple[int, int], Any] = {}
+        wide: Dict[str, torch.Tensor] = {}  # argument column -> its f64 values, so that pointers repeat
+        pairs: Dict[Any, Any] = {}  # (x, y) argument columns -> the 12 accumulators of the pair
         for a in agg_cols:
+            if a.func in BIVARIATES:
+                xy = tuple(e.name for e in bivariate_xy(a))
+                if xy not in pairs:
+                    pairs[xy] = self._pair_accumulators(t, a, xy, add, devs, wide)
+                plan.append((a.output_name, "covar", pairs[xy], pa.int64() if a.func == "REGR_COUNT" else pa.float64(),
+                             a.func))
+                continue
             fn, arg = a.func, a.arg.name
             if fn == "COUNT":
                 if arg == "*":
@@ -704,12 +746,8 @@ class B200ExecutionEngine(EngineLifecycle):
                 # one SUM, COUNT, DEV, DEV2 per column, shared by all its variances (DESIGN §7i)
                 assert_or_throw(pa.types.is_integer(tp) or pa.types.is_floating(tp),
                                 lambda: NotImplementedError(f"{fn}({arg}): {tp} is not a numeric type"))
-                if arg not in moments:
-                    cf = widen(c, tp)
-                    cf = (cf if cf.dtype == torch.float64 else cf.to(torch.float64)).contiguous()
-                    moments[arg] = (add(cf, m, K.AGG_SUM_F64), add(None, m, K.AGG_COUNT), add(cf, m, K.AGG_DEV_F64),
-                                    add(cf, m, K.AGG_DEV2_F64))
-                plan.append((a.output_name, "var", moments[arg], pa.float64(), fn))
+                plan.append((a.output_name, "var", _deviations(devs, add, _f64_column(t, arg, wide), m), pa.float64(),
+                             fn))
                 continue
             is_f = pa.types.is_floating(tp)
             c8 = widen(c, tp)
@@ -729,6 +767,8 @@ class B200ExecutionEngine(EngineLifecycle):
                 plan.append((a.output_name, "avg", add(cf, m, K.AGG_SUM_F64), pa.float64(), cnt))
             else:
                 raise NotImplementedError(f"aggregation {fn}")
+        if len(ops) > K.MAX_AGGS and pairs:  # more than one kernel call holds: the sorted route has no such limit
+            return self._aggregate_sorted(df, partition_spec, agg_cols)
         assert_or_throw(len(ops) <= K.MAX_AGGS, NotImplementedError(
             f"{len(ops)} accumulators needed, one kernel call handles {K.MAX_AGGS}"))
         shuffled = getattr(t, "global_num_partitions", None) is not None and len(keys) > 0
@@ -761,6 +801,12 @@ class B200ExecutionEngine(EngineLifecycle):
             valids.append(gvalid)
         dicts = {k: t.dictionaries[k] for k in keys if k in t.dictionaries}
         for name, kind, slot, tp, nn in plan:
+            if kind == "covar":
+                col, v = bivariate_of(nn, *self._pair_moments(gaggs, slot))
+                fields.append(pa.field(name, tp))
+                cols.append(col)
+                valids.append(v)
+                continue
             if kind == "var":
                 _, cnt, dev_, dev2 = slot
                 m_ = gaggs[cnt]
@@ -801,6 +847,71 @@ class B200ExecutionEngine(EngineLifecycle):
             valids.append(v)
         return B200DataFrame(B200Table(Schema(fields), cols, valids, dicts))
 
+    @staticmethod
+    def _pair_accumulators(t: B200Table, a: Any, xy: Tuple[str, str], add: Any, devs: Dict[Tuple[int, int], Any],
+                           wide: Dict[str, torch.Tensor]) -> Tuple[int, ...]:
+        """The 12 accumulators of the pair of columns ``xy`` (DESIGN §7k): SUM x, SUM y, COUNT, DEV x, DEV2 x,
+        CODEV, DEV y, DEV2 y, MIN x, MAX x, MIN y, MAX y, all over ONE pair validity tensor, so that the kernel's
+        pointer ties survive the radix partition of ``K.groupby_u64``.  ``devs`` / ``wide``: the call's
+        deviation sets and f64 columns (see ``_deviations``): x and y share their SUM, DEV2 (and x its DEV) with a
+        variance of the same column and validity.  The DEV of y always follows the CODEV, so it is a second DEV of y
+        when a set for y came first; K6 gives it sums of its own."""
+        import pyarrow as pa
+
+        f64, masks = [], []
+        for nm in xy:
+            tp = t.schema.types[t.schema.index_of_key(nm)]
+            assert_or_throw(nm not in t.dictionaries and (pa.types.is_integer(tp) or pa.types.is_floating(tp)),
+                            lambda: NotImplementedError(f"{a.func}: {nm} is {tp}, not a numeric type"))
+            f64.append(_f64_column(t, nm, wide))
+            masks.append(t.valid[t.schema.index_of_key(nm)])
+        x, y = f64
+        mx, my = masks
+        p = mx if my is None else (my if mx is None else (mx & my).contiguous())
+        kx, ky = _dev_key(x, p), _dev_key(y, p)
+        sy: Any = None
+        if kx in devs:
+            sx, cnt, dx, d2x = devs[kx]
+        else:  # SUM x, SUM y and COUNT first, so that pass B reads the three from one sector of the slot
+            sx = add(x, p, K.AGG_SUM_F64)
+            if ky not in devs and ky != kx:
+                sy = add(y, p, K.AGG_SUM_F64)
+            cnt = add(None, p, K.AGG_COUNT)
+            dx, d2x = add(x, p, K.AGG_DEV_F64), add(x, p, K.AGG_DEV2_F64)
+            devs[kx] = (sx, cnt, dx, d2x)
+        codev = add(x, p, K.AGG_CODEV_F64)
+        dy = add(y, p, K.AGG_DEV_F64)  # the DEV of y right after the CODEV: the tie K6 reads
+        if ky in devs:  # (x, x), or a variance of y came first: a second DEV of y gets its own sums
+            sy, _, _, d2y = devs[ky]
+        else:
+            d2y = add(y, p, K.AGG_DEV2_F64)
+            if sy is None:
+                sy = add(y, p, K.AGG_SUM_F64)
+            devs[ky] = (sy, cnt, dy, d2y)
+        return (sx, sy, cnt, dx, d2x, codev, dy, d2y,
+                add(x, p, K.AGG_MIN_F64), add(x, p, K.AGG_MAX_F64), add(y, p, K.AGG_MIN_F64), add(y, p, K.AGG_MAX_F64))
+
+    @staticmethod
+    def _pair_moments(gaggs: List[torch.Tensor], slots: Tuple[int, ...]) -> Tuple[torch.Tensor, ...]:
+        """(m, mean x, mean y, Sxx, Syy, Sxy) per group from a pair's accumulators: the corrected two-pass
+        DEV2 - DEV^2 / m (clamped at 0) and CODEV - DEVx DEVy / m.  A column whose MIN equals its MAX is constant:
+        its S is exactly 0 and so is Sxy (the mean summed with atomics is not exactly the constant).  A NaN or
+        +-inf on either side (a MIN or MAX that is not finite) makes all three NaN."""
+        sx, sy, cnt, dx, d2x, cod, dy, d2y, mnx, mxx, mny, mxy = (gaggs[i] for i in slots)
+        f = [q.view(torch.float64) for q in (sx, sy, dx, d2x, cod, dy, d2y, mnx, mxx, mny, mxy)]
+        sx, sy, dx, d2x, cod, dy, d2y, mnx, mxx, mny, mxy = f
+        m = cnt
+        mf = m.to(torch.float64)
+        zero = torch.zeros_like(mf)
+        cx, cy = mnx == mxx, mny == mxy
+        sxx = torch.where(cx, zero, torch.clamp_min(d2x - dx * dx / mf, 0.0))
+        syy = torch.where(cy, zero, torch.clamp_min(d2y - dy * dy / mf, 0.0))
+        sxy = torch.where(cx | cy, zero, cod - dx * dy / mf)
+        finite = torch.isfinite(mnx) & torch.isfinite(mxx) & torch.isfinite(mny) & torch.isfinite(mxy)
+        nan = torch.full_like(mf, math.nan)
+        return (m, sx / mf, sy / mf, torch.where(finite, sxx, nan), torch.where(finite, syy, nan),
+                torch.where(finite, sxy, nan))
+
     def _aggregate_sorted(self, df: Any, partition_spec: Optional[PartitionSpec],
                           agg_cols: List[Any]) -> B200DataFrame:
         """GROUP BY with a percentile among the aggregates: sort by the keys (stable, so FIRST / LAST keep their
@@ -816,7 +927,7 @@ class B200ExecutionEngine(EngineLifecycle):
 
         t: B200Table = self.to_df(df).native
         keys = [] if partition_spec is None else list(partition_spec.partition_by)
-        names = list(dict.fromkeys(keys + [a.arg.name for a in agg_cols if a.arg.kind != Kind.WILDCARD]))
+        names = list(dict.fromkeys(keys + [x.name for a in agg_cols for x in a.args if x.kind != Kind.WILDCARD]))
         sub = t.select(names)
         sub = B200Table(sub.schema, sub.columns, sub.valid, sub.dictionaries)
         n, dev = sub.num_rows, sub.device
@@ -833,12 +944,12 @@ class B200ExecutionEngine(EngineLifecycle):
         if n == 0 and not keys:  # SQL: a global aggregate of an empty table is one row, NULL but for COUNT
             for a, e in zip(agg_cols, nodes):
                 tp = e.infer_type(sub.schema) or pa.float64()
-                is_count = a.func == "COUNT"
+                is_count = a.func in ("COUNT", "REGR_COUNT")
                 fields.append(pa.field(a.output_name, tp))
                 cols.append(narrow(torch.zeros(1, dtype=torch.float64 if pa.types.is_floating(tp) else torch.int64,
                                                device=dev), tp).contiguous())
                 valids.append(None if is_count else torch.zeros(1, dtype=torch.uint8, device=dev))
-                if a.func not in ("COUNT", "PERCENTILE_CONT") and a.arg.name in sub.dictionaries:
+                if len(a.args) == 1 and a.func not in ("COUNT", "PERCENTILE_CONT") and a.arg.name in sub.dictionaries:
                     dicts[a.output_name] = sub.dictionaries[a.arg.name]
             return B200DataFrame(B200Table(Schema(fields), cols, valids, dicts))
         w = _with_windows(sub, nodes)
@@ -869,8 +980,8 @@ class B200ExecutionEngine(EngineLifecycle):
         SQL text.  Pins: fugue_test/execution_suite.py:98-155."""
         from . import expr as X
         from . import relational as R
-        from .column import (PERCENTILES, VARIANCES, ColumnExpr, Kind, SelectColumns, agg as _agg, col, has_window,
-                             is_agg)
+        from .column import (BIVARIATES, PERCENTILES, VARIANCES, ColumnExpr, Kind, SelectColumns, agg as _agg, col,
+                             has_window, is_agg)
 
         for e in list(cols.all_cols) + [where, having]:
             assert_or_throw(not has_window(e), lambda: NotImplementedError(
@@ -924,9 +1035,9 @@ class B200ExecutionEngine(EngineLifecycle):
             if uid in agg_col:
                 continue
             assert_or_throw(a.func in ("SUM", "COUNT", "MIN", "MAX", "AVG", "FIRST", "LAST", "PERCENTILE_CONT",
-                                       "PERCENTILE_DISC") or a.func in VARIANCES,
+                                       "PERCENTILE_DISC") or a.func in VARIANCES or a.func in BIVARIATES,
                             NotImplementedError(f"aggregation {a.func}"))
-            assert_or_throw(not is_agg(a.arg), ValueError(f"nested aggregation {a}"))
+            assert_or_throw(not any(is_agg(x) for x in a.args), ValueError(f"nested aggregation {a}"))
             out = f"__fb_a{len(agg_col)}"
             agg_col[uid] = out
             if a.is_distinct:
@@ -939,14 +1050,18 @@ class B200ExecutionEngine(EngineLifecycle):
                 distinct_on = (dn, a.arg.kind == Kind.WILDCARD)
                 distinct_outs.append(out)
                 continue
-            if a.arg.kind == Kind.WILDCARD:
-                arg = col("*")
-            elif a.arg.kind == Kind.LITERAL:
-                arg = col(temp(a.arg.alias("").cast(a.arg.as_type), "l"))
-            else:
-                arg = col(temp(a.arg, "v"))
-            # the same aggregation of the temporary column (a percentile keeps its q)
-            named_aggs.append(ColumnExpr(Kind.AGG, a.func, [arg], a.kwargs, False, out))
+            args = []
+            for x in a.args:
+                if x.kind == Kind.WILDCARD:
+                    args.append(col("*"))
+                elif x.kind == Kind.LITERAL:
+                    args.append(col(temp(x.alias("").cast(x.as_type), "l")))
+                else:
+                    args.append(col(temp(x, "v")))
+            # the same aggregation of the temporary columns (a percentile keeps its q)
+            named_aggs.append(ColumnExpr(Kind.AGG, a.func, args, a.kwargs, False, out))
+        assert_or_throw(distinct_on is None or not any(a.func in BIVARIATES for a in named_aggs), NotImplementedError(
+            "COUNT(DISTINCT ...) and a two-argument aggregate in one SELECT: the family has no partial / final form"))
         if len(pre) == 0:  # e.g. SELECT COUNT(*) FROM t
             tmp = t
         else:

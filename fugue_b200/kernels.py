@@ -293,6 +293,10 @@ AGG_SUM_F64, AGG_SUM_I64, AGG_COUNT, AGG_MIN_I64, AGG_MAX_I64, AGG_MIN_F64, AGG_
 # group-by only: deviations from the group mean (sum of d and of d * d, d = x - SUM / COUNT); each needs an
 # AGG_SUM_F64 of the same f64 column and validity and an AGG_COUNT of the same validity in the same call
 AGG_DEV_F64, AGG_DEV2_F64 = 7, 8
+# group-by only: cross deviations of a pair (sum of dx * dy over the rows where the pair validity is set).  An
+# AGG_CODEV_F64 names x and the pair validity; the AGG_DEV_F64 right after it names y with the same validity, and
+# the call needs AGG_SUM_F64 of x and of y and an AGG_COUNT, all of that same validity tensor
+AGG_CODEV_F64 = 9
 MAX_AGGS = 16
 
 
@@ -464,6 +468,44 @@ def segmented_moments(offsets: torch.Tensor, nrows: int,
             _lib.ptr_array([c.data_ptr() for c in cnts]), _lib.ptr_array([q.data_ptr() for q in m2s]),
             scratch.data_ptr(), scratch.numel()))
         res.extend(zip(cnts, m2s))
+    return res
+
+
+def segmented_comoments(offsets: torch.Tensor, nrows: int,
+                        pairs: Sequence[Tuple[torch.Tensor, Optional[torch.Tensor], torch.Tensor, Optional[torch.Tensor]]]
+                        ) -> List[Tuple[torch.Tensor, ...]]:
+    """K9: running co-moments restarting at every segment ``[offsets[s], offsets[s + 1])``.  ``pairs`` = one
+    ``(float64 x, validity of x or None, float64 y, validity of y or None)`` per pair; the kernel takes the rows
+    where both are valid.  Returns per pair ``(count (int64), mean x, mean y, Sxx, Syy, Sxy)`` of those rows up to
+    each row (float64, 0 where the count is 0); up to ``SCAN_MAX_COLS`` pairs share one launch sequence."""
+    lib = _lib.load()
+    assert offsets.dtype == torch.int64 and offsets.is_cuda and offsets.is_contiguous()
+    dev = offsets.device
+    nseg = int(offsets.shape[0]) - 1
+    res: List[Tuple[torch.Tensor, ...]] = []
+    for b in range(0, len(pairs), SCAN_MAX_COLS):
+        batch = pairs[b:b + SCAN_MAX_COLS]
+        outs = []
+        for x, mx, y, my in batch:
+            for v in (x, y):
+                assert v.dtype == torch.float64 and v.device == dev and v.is_contiguous() and v.shape[0] == nrows
+            for m in (mx, my):
+                if m is not None:
+                    assert m.dtype == torch.uint8 and m.device == dev and m.is_contiguous() and m.shape[0] == nrows
+            outs.append((torch.empty(nrows, dtype=torch.int64, device=dev),)
+                        + tuple(torch.empty(nrows, dtype=torch.float64, device=dev) for _ in range(5)))
+        nb = int(lib.fb_segmented_comoments_scratch_bytes(nrows, len(batch)))
+        scratch = torch.empty(max(nb, 8), dtype=torch.uint8, device=dev)
+
+        def ptrs(ts: Sequence[Optional[torch.Tensor]]) -> Any:
+            return _lib.ptr_array([0 if t is None else t.data_ptr() for t in ts])
+
+        _lib.check(lib.fb_segmented_comoments(
+            dev.index, _stream_ptr(dev), nrows, nseg, offsets.data_ptr(), len(batch),
+            ptrs([p[0] for p in batch]), ptrs([p[1] for p in batch]), ptrs([p[2] for p in batch]),
+            ptrs([p[3] for p in batch]), *[ptrs([o[i] for o in outs]) for i in range(6)],
+            scratch.data_ptr(), scratch.numel()))
+        res.extend(outs)
     return res
 
 

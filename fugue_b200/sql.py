@@ -11,7 +11,7 @@ fugue/workflow/workflow.py:2109-2166) and ``ExecutionEngine.aggregate`` reaches 
              [ORDER BY c [ASC|DESC], ...] [LIMIT n]
         -> parsed into column expressions (fugue_b200.column) and run by ``engine.select``: row-wise
            parts in the device expression evaluator, SUM/COUNT/MIN/MAX/AVG and VAR_SAMP / VARIANCE / VAR_POP /
-           STDDEV_SAMP / STDDEV / STDDEV_POP in the hash group-by kernel
+           STDDEV_SAMP / STDDEV / STDDEV_POP and CORR / COVAR_POP / COVAR_SAMP / REGR_* in the hash group-by kernel
     SELECT * FROM a [INNER|LEFT|RIGHT|FULL [OUTER]|LEFT SEMI|LEFT ANTI|CROSS] JOIN b
              [USING (k, ...) | ON a.k = b.k [AND ...]]                        -> hash join kernels
 
@@ -28,7 +28,7 @@ import datetime
 import re
 from typing import Any, Dict, List, Tuple
 
-from .column import ColumnExpr, Kind, SelectColumns, all_cols, col, function, functions, is_agg, lit, null
+from .column import BIVARIATES, ColumnExpr, Kind, SelectColumns, all_cols, col, function, functions, is_agg, lit, null
 from .dataframe import DataFrame
 
 _AGG = r"(SUM|COUNT|MIN|MAX|AVG|MEAN)\s*\(\s*(\*|[A-Za-z_][\w]*)\s*\)"
@@ -313,6 +313,8 @@ _AGG_FUNCS = {"SUM": functions.sum, "COUNT": functions.count, "MIN": functions.m
               "AVG": functions.avg, "MEAN": functions.avg, "FIRST": functions.first, "LAST": functions.last,
               "VAR_SAMP": functions.var_samp, "VARIANCE": functions.variance, "VAR_POP": functions.var_pop,
               "STDDEV_SAMP": functions.stddev_samp, "STDDEV": functions.stddev, "STDDEV_POP": functions.stddev_pop}
+# CORR(a, b), COVAR_POP / COVAR_SAMP(a, b), REGR_*(y, x): two arguments, in SQL's order
+_BIVARIATE_FUNCS = {name: getattr(functions, name.lower()) for name in BIVARIATES}
 _CLAUSES = ("WHERE", "GROUP", "HAVING", "ORDER", "LIMIT")
 _CASE_WORDS = ("WHEN", "THEN", "ELSE", "END")  # never a column name or an implicit alias
 _ONE_ARG = {"ABS": functions.abs, "FLOOR": functions.floor, "CEIL": functions.ceil, "CEILING": functions.ceil,
@@ -615,6 +617,14 @@ class _Parser:
                     self.fail(f"{fn}(DISTINCT ...)")
                 return functions.count_distinct(arg)
             return _AGG_FUNCS[fn](arg)
+        if fn in _BIVARIATE_FUNCS:
+            if self.kw("DISTINCT"):
+                self.fail(f"{fn}(DISTINCT ...)")
+            a = self.expr()
+            self.expect(",")
+            b = self.expr()
+            self.expect(")")
+            return _BIVARIATE_FUNCS[fn](a, b)
         if fn == "MEDIAN":
             arg = self.expr()
             self.expect(")")

@@ -225,7 +225,16 @@ int fb_pull_runs_tma(int dev, void* stream, int nruns, const void* const* src, v
  * pointer (rejected otherwise).  After the other aggregates of a row's group are complete, the call adds
  * d = x - SUM / COUNT of the row's group into DEV and d * d into DEV2, for every valid x.  With m = COUNT,
  * M2 = sum over the group of (x - mean)^2 = max(0, DEV2 - DEV^2 / m).  A NaN or +-inf value makes DEV
- * and DEV2 NaN.  fb_segmented_scan and the frame kernels reject both ops.
+ * and DEV2 NaN.  Several DEV (or DEV2) accumulators of the same column and validity each receive the full sum.
+ * fb_segmented_scan and the frame kernels reject both ops.
+ *
+ * Cross deviations (covariance and regression, DESIGN §7k): an FB_AGG_CODEV_F64 accumulator at index a names
+ * x through val_ptrs[a] and the pair validity p through val_valid[a].  Its y is the value column of accumulator
+ * a + 1, which must be an FB_AGG_DEV_F64 with the same validity pointer p.  The call must also hold an
+ * FB_AGG_SUM_F64 of (x, p), an FB_AGG_SUM_F64 of (y, p) and an FB_AGG_COUNT of p (rejected otherwise).  For every
+ * row where p is set, the call adds dx * dy into CODEV, with dx = x - SUM(x) / COUNT and dy = y - SUM(y) / COUNT
+ * of the row's group.  With m = COUNT, DEVx and DEVy the deviation sums of x and y over the same rows,
+ * Sxy = sum over the group of (x - mean x)(y - mean y) = CODEV - DEVx * DEVy / m.
  * --------------------------------------------------------------------------- */
 #define FB_MAX_AGGS 16
 enum {
@@ -237,7 +246,8 @@ enum {
   FB_AGG_MIN_F64 = 5,
   FB_AGG_MAX_F64 = 6,
   FB_AGG_DEV_F64 = 7,
-  FB_AGG_DEV2_F64 = 8
+  FB_AGG_DEV2_F64 = 8,
+  FB_AGG_CODEV_F64 = 9
 };
 size_t fb_groupby_table_bytes(int64_t capacity, int naggs);
 int fb_groupby_u64(int dev, void* stream, int64_t nrows, const void* keys, const uint8_t* key_valid,
@@ -283,6 +293,26 @@ size_t fb_segmented_moments_scratch_bytes(int64_t nrows, int ncols);
 int fb_segmented_moments(int dev, void* stream, int64_t nrows, int64_t nseg, const int64_t* d_offsets, int ncols,
                          const void* const* vals, const uint8_t* const* valid, int64_t* const* out_count,
                          void* const* out_m2, void* scratch, size_t scratch_bytes);
+
+/* K9  segmented co-moments: over the same segments, per pair c and row i, the rows of i's segment up to and
+ * including i where both x and y are valid (f64 values xs[c] / ys[c], masks x_valid[c] / y_valid[c] or NULL,
+ * ANDed by the kernel):
+ *   out_count[c][i]               their number m (int64)
+ *   out_mean_x[c][i], out_mean_y  the means of x and y over them (f64)
+ *   out_sxx[c][i], out_syy, out_sxy  Sxx = sum of (x - mean x)^2, Syy likewise, Sxy = sum of (x - mean x)(y - mean y)
+ * All f64 outputs are 0 where m = 0.  A NaN or +-inf in x or y of a pair row makes Sxx, Syy and Sxy NaN from that
+ * row on; a mean then becomes what the sum of its values over m gives (+-inf, or NaN).  The state (n, mean x,
+ * mean y, Sxx, Syy, Sxy) is combined with Chan's pairwise update, whose cross term is dx * dy * na * nb / n; a
+ * pair enters as (1, x, y, z, z, z) with z = (x - x) * (y - y).  Same launch sequence and fixed combination order
+ * as fb_segmented_scan: bit-identical runs.  Every pointer argument but d_offsets and scratch is a HOST array of
+ * npairs <= FB_SCAN_MAX_COLS entries; an output may be NULL (not written); scratch:
+ * fb_segmented_comoments_scratch_bytes. */
+size_t fb_segmented_comoments_scratch_bytes(int64_t nrows, int npairs);
+int fb_segmented_comoments(int dev, void* stream, int64_t nrows, int64_t nseg, const int64_t* d_offsets, int npairs,
+                           const void* const* xs, const uint8_t* const* x_valid, const void* const* ys,
+                           const uint8_t* const* y_valid, int64_t* const* out_count, void* const* out_mean_x,
+                           void* const* out_mean_y, void* const* out_sxx, void* const* out_syy,
+                           void* const* out_sxy, void* scratch, size_t scratch_bytes);
 
 /* K9  moving-window aggregate: ROWS BETWEEN start AND end over the same segments.  For row i of segment
  * [a, b) the frame is rows [max(a, i + start), min(b - 1, i + end)] (may be empty); a negative bound is

@@ -27,9 +27,11 @@ from typing import Any, Dict, List, Optional, Tuple
 import pyarrow as pa
 import torch
 
+from . import aggregates as A
 from . import kernels as K
-from .column import (BIVARIATES, PERCENTILES, VARIANCES, ColumnExpr, Kind, SelectColumns, bivariate_xy, col as _col,
-                     has_window, is_agg)
+from .aggregates import bivariate_of
+from .column import (AGGREGATES, PERCENTILES, ColumnExpr, Kind, SelectColumns, bivariate_xy, col as _col, has_window,
+                     is_agg, result_type)
 from .table import B200Table, narrow, widen
 
 
@@ -270,95 +272,50 @@ def _with_windows(t: B200Table, cols: List[ColumnExpr]) -> B200Table:
         def at_end(x: torch.Tensor, whole: Any = whole) -> torch.Tensor:  # partition value: the scan at its last row
             return x if whole is None else x[whole()]
 
-        if fn in BIVARIATES:  # the co-moments scan, one pair per (x, y) shared by its functions; no frames
+        family = AGGREGATES[fn].family
+        if family == "bivariate":  # the co-moments scan, one pair per (x, y) shared by its functions; no frames
             xy = tuple(arg_name[a.fingerprint()] for a in bivariate_xy(bare))
             for nm in xy:
-                tp = base.schema.types[base.schema.index_of_key(nm)]
-                if not (pa.types.is_integer(tp) or pa.types.is_floating(tp)):
-                    raise NotImplementedError(f"{fn} needs integer or float columns; {nm} is {tp}")
+                A.check_argument(fn, nm, base.schema.types[base.schema.index_of_key(nm)], nm in base.dictionaries)
             j = comoments.setdefault(xy, len(comoments))
-
-            def bivariate(r: Any, j: int = j, e: Any = at_end, fn: str = fn) -> Any:
-                v, vv = bivariate_of(fn, *(e(x) for x in r[("comoments", j)]))
-                return v, vv, pa.int64() if fn == "REGR_COUNT" else pa.float64(), None
-
-            finish.append((uid, bivariate))
+            finish.append((uid, lambda r, j=j, e=at_end, fn=fn: (
+                *bivariate_of(fn, *(e(x) for x in r[("comoments", j)])), result_type(fn, None), None)))
             continue
-        if bare.arg.kind == Kind.WILDCARD:  # COUNT(*)
-            i = scan(K.AGG_COUNT, None, None, frame)
-            finish.append((uid, lambda r, i=i, e=at_end: (e(r[i][1]), None, pa.int64(), None)))
+        if fn == "COUNT" or bare.arg.kind == Kind.WILDCARD:  # COUNT(x), COUNT(*)
+            m = None if bare.arg.kind == Kind.WILDCARD else base.valid[base.schema.index_of_key(
+                arg_name[bare.arg.fingerprint()])]
+            i = scan(K.AGG_COUNT, None, m, frame)
+            finish.append((uid, lambda r, i=i, e=at_end: (*A.finish_basic("COUNT", None, e(r[i][1]), None), None)))
             continue
         name = arg_name[bare.arg.fingerprint()]
         ci = base.schema.index_of_key(name)
-        c, m, tp = base.columns[ci], base.valid[ci], base.schema.types[ci]
-        if fn == "COUNT":
-            i = scan(K.AGG_COUNT, None, m, frame)
-            finish.append((uid, lambda r, i=i, e=at_end: (e(r[i][1]), None, pa.int64(), None)))
-            continue
-        if fn in ("FIRST", "LAST"):
+        c, m, tp, d = base.columns[ci], base.valid[ci], base.schema.types[ci], base.dictionaries.get(name)
+        A.check_argument(fn, name, tp, d is not None)
+        if family == "pick":
             # first / last valid row so far: MIN / MAX of the row number over the valid rows, then a gather
-            i = scan(K.AGG_MIN_I64 if fn == "FIRST" else K.AGG_MAX_I64, rows, m, frame)
+            i = scan(*A.reduce_input(fn, rows, pa.int64()), m, frame)
 
-            def pick(r: Any, i: Any = i, e: Any = at_end, c: Any = c, m: Any = m, tp: Any = tp, name: str = name) -> Any:
+            def pick(r: Any, i: Any = i, e: Any = at_end, c: Any = c, m: Any = m, tp: Any = tp, d: Any = d) -> Any:
                 idx = torch.where(e(r[i][1]) > 0, e(r[i][0]), torch.full_like(rows, -1))
                 (g,), (gv,) = K.gather_rows([c], [m], idx.contiguous(), want_valid=True)
-                return g, gv, tp, base.dictionaries.get(name)
+                return g, gv, tp, d
 
             finish.append((uid, pick))
             continue
-        if name in base.dictionaries:
-            if fn not in ("MIN", "MAX"):
-                raise NotImplementedError(f"{fn} on a string column: {bare}")
-            rank, rm = S.string_ranks(base, name)  # MIN / MAX of the ranks, mapped back to codes
-            i = scan(K.AGG_MIN_I64 if fn == "MIN" else K.AGG_MAX_I64, rank, rm, frame)
-
-            def extreme_string(r: Any, i: Any = i, e: Any = at_end, tp: Any = tp, d: Any = base.dictionaries[name]) -> Any:
-                v, cnt = e(r[i][0]), e(r[i][1])
-                return S.codes_of_ranks(d, v), (cnt > 0).to(torch.uint8), tp, d
-
-            finish.append((uid, extreme_string))
+        if d is not None:  # MIN / MAX of the ranks, mapped back to codes
+            rank, rm = S.string_ranks(base, name)
+            i = scan(*A.reduce_input(fn, rank, pa.int64()), rm, frame)
+            finish.append((uid, lambda r, i=i, e=at_end, d=d, tp=tp: A.finish_string(e(r[i][0]), e(r[i][1]), d, tp)))
             continue
-        is_f = pa.types.is_floating(tp)
-        if fn in VARIANCES:  # the moments scan; frames are rejected by over()
-            if not (pa.types.is_integer(tp) or is_f):
-                raise NotImplementedError(f"{fn} needs an integer or float column; {name} is {tp}")
+        if family == "variance":  # the moments scan; frames are rejected by over()
             j = moments.setdefault(name, len(moments))
-
-            def variance(r: Any, j: int = j, e: Any = at_end, fn: str = fn) -> Any:
-                cnt, m2 = r[("moments", j)]
-                v, vv = variance_of(fn, e(m2), e(cnt))
-                return v, vv, pa.float64(), None
-
-            finish.append((uid, variance))
+            finish.append((uid, lambda r, j=j, e=at_end, fn=fn: (
+                *A.variance_of(fn, e(r[("moments", j)][1]), e(r[("moments", j)][0])), pa.float64(), None)))
             continue
-        if fn in ("SUM", "AVG"):
-            f64 = fn == "AVG" or is_f
-            v8 = widen(c, tp)
-            v8 = (v8.to(torch.float64) if f64 else v8).contiguous()
-            i = scan(K.AGG_SUM_F64 if f64 else K.AGG_SUM_I64, v8, m, frame)
-            out_tp = pa.float64() if f64 else pa.int64()
+        i = scan(*A.reduce_input(fn, c, tp), m, frame)
+        finish.append((uid, lambda r, i=i, e=at_end, fn=fn, tp=tp: (
+            *A.finish_basic(fn, e(r[i][0]), e(r[i][1]), tp), None)))
 
-            def total(r: Any, i: Any = i, e: Any = at_end, avg: bool = fn == "AVG", out_tp: Any = out_tp) -> Any:
-                v, cnt = e(r[i][0]), e(r[i][1])
-                if avg:
-                    v = v / cnt.to(torch.float64)
-                return v.contiguous(), (cnt > 0).to(torch.uint8), out_tp, None
-
-            finish.append((uid, total))
-            continue
-        if fn in ("MIN", "MAX"):
-            v8 = widen(c, tp).contiguous()
-            op = {("MIN", True): K.AGG_MIN_F64, ("MAX", True): K.AGG_MAX_F64,
-                  ("MIN", False): K.AGG_MIN_I64, ("MAX", False): K.AGG_MAX_I64}[(fn, is_f)]
-            i = scan(op, v8, m, frame)
-
-            def extreme(r: Any, i: Any = i, e: Any = at_end, tp: Any = tp) -> Any:
-                v, cnt = e(r[i][0]), e(r[i][1])
-                return narrow(v, tp).contiguous(), (cnt > 0).to(torch.uint8), tp, None
-
-            finish.append((uid, extreme))
-            continue
-        raise NotImplementedError(f"window function {fn}")  # pragma: no cover - builders admit no other
     def range_bounds(cls: Optional[int], start: Any, end: Any) -> Tuple[torch.Tensor, torch.Tensor]:
         """First and last row of every row's RANGE frame."""
         if cls is not None:  # an offset: a search over the one presort key
@@ -390,22 +347,15 @@ def _with_windows(t: B200Table, cols: List[ColumnExpr]) -> B200Table:
         results.update(((frame, j), r) for j, r in enumerate(res))
     for name, qs in quantiles.items():
         results[("quantile", name)] = K.segmented_quantile(off.contiguous(), *quantile_input(base, name), qs)
+
+    def f64_valid(name: str) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
+        return A.f64_values(base, name), base.valid[base.schema.index_of_key(name)]
+
     if moments:
-        mcols = []
-        for name in moments:
-            i = base.schema.index_of_key(name)
-            v = widen(base.columns[i], base.schema.types[i])
-            mcols.append(((v if v.dtype == torch.float64 else v.to(torch.float64)).contiguous(), base.valid[i]))
+        mcols = [f64_valid(name) for name in moments]
         results.update((("moments", j), r) for j, r in enumerate(K.segmented_moments(off.contiguous(), n, mcols)))
     if comoments:
-        pairs = []
-        for xy in comoments:
-            f64 = []
-            for nm in xy:
-                i = base.schema.index_of_key(nm)
-                v = widen(base.columns[i], base.schema.types[i])
-                f64 += [(v if v.dtype == torch.float64 else v.to(torch.float64)).contiguous(), base.valid[i]]
-            pairs.append(tuple(f64))
+        pairs = [f64_valid(x) + f64_valid(y) for x, y in comoments]
         results.update((("comoments", j), r) for j, r in enumerate(K.segmented_comoments(off.contiguous(), n, pairs)))
     names, types, columns, valid = list(base.schema.names), list(base.schema.types), list(base.columns), list(base.valid)
     dicts = dict(base.dictionaries)
@@ -423,46 +373,6 @@ def _with_windows(t: B200Table, cols: List[ColumnExpr]) -> B200Table:
     out = _WindowTable(Schema([pa.field(a, b) for a, b in zip(names, types)]), columns, valid, dicts)
     out.window_names = window_names
     return out
-
-
-def variance_of(fn: str, m2: torch.Tensor, count: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
-    """``fn`` (a ``VARIANCES`` head) from M2 and the non-NULL count m: (float64 values, validity).  The sample
-    forms divide by m - 1 and are NULL when m < 2, the population forms divide by m and are NULL when m = 0."""
-    samp = fn in ("VAR_SAMP", "STDDEV_SAMP")
-    has = count > (1 if samp else 0)
-    v = m2 / torch.where(has, count - (1 if samp else 0), torch.ones_like(count)).to(torch.float64)
-    if fn.startswith("STDDEV"):
-        v = torch.sqrt(v)
-    return torch.where(has, v, torch.zeros_like(v)).contiguous(), has.to(torch.uint8)
-
-
-def bivariate_of(fn: str, m: torch.Tensor, mx: torch.Tensor, my: torch.Tensor, sxx: torch.Tensor, syy: torch.Tensor,
-                 sxy: torch.Tensor) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
-    """``fn`` (a ``BIVARIATES`` head) from the pair count m, the means of x and y and Sxx, Syy, Sxy over the pair
-    rows: (values, validity or None).  REGR_COUNT is m (int64, never NULL); COVAR_SAMP is NULL when m < 2; every
-    other function is NULL when m = 0, and SLOPE / INTERCEPT / R2 also when Sxx = 0, CORR when Sxx = 0 or Syy = 0.
-    CORR is clamped to [-1, 1] and R2 to [0, 1] (1 when Syy = 0).  A NaN Sxx or Syy is not 0: the result is NaN."""
-    if fn == "REGR_COUNT":
-        return m.contiguous(), None
-    has = m > (1 if fn == "COVAR_SAMP" else 0)
-    mf = m.to(torch.float64)
-    if fn in ("COVAR_POP", "COVAR_SAMP"):
-        v = sxy / torch.where(has, mf - (1 if fn == "COVAR_SAMP" else 0), torch.ones_like(mf))
-    elif fn in ("REGR_AVGX", "REGR_AVGY", "REGR_SXX", "REGR_SYY", "REGR_SXY"):
-        v = {"REGR_AVGX": mx, "REGR_AVGY": my, "REGR_SXX": sxx, "REGR_SYY": syy, "REGR_SXY": sxy}[fn]
-    elif fn == "CORR":
-        has = has & (sxx != 0) & (syy != 0)
-        v = torch.clamp(sxy / (torch.sqrt(sxx) * torch.sqrt(syy)), -1.0, 1.0)
-    else:
-        has = has & (sxx != 0)
-        slope = sxy / sxx
-        if fn == "REGR_SLOPE":
-            v = slope
-        elif fn == "REGR_INTERCEPT":
-            v = my - slope * mx
-        else:  # REGR_R2
-            v = torch.where(syy == 0, torch.ones_like(syy), torch.clamp(sxy * sxy / (sxx * syy), 0.0, 1.0))
-    return torch.where(has, v, torch.zeros_like(v)).contiguous(), has.to(torch.uint8)
 
 
 def quantile_input(t: B200Table, name: str) -> Tuple[torch.Tensor, Optional[torch.Tensor], int]:

@@ -39,7 +39,7 @@ import datetime
 import enum
 import hashlib
 import math
-from typing import Any, Dict, Iterable, Iterator, List, Optional, Sequence, Tuple
+from typing import Any, Dict, Iterable, Iterator, List, NamedTuple, Optional, Sequence, Tuple
 
 import pyarrow as pa
 
@@ -59,16 +59,38 @@ class Kind(enum.IntEnum):
 
 BOOL_OPS = frozenset(["&", "|", "<", ">", "<=", ">=", "==", "!="])
 ARITH_OPS = frozenset(["+", "-", "*", "/", "%"])
-AGG_KEEPS_ARG_TYPE = frozenset(["MIN", "MAX", "FIRST", "LAST"])
-WINDOW_AGGS = frozenset(["SUM", "COUNT", "AVG", "MIN", "MAX", "FIRST", "LAST"])
-PERCENTILES = frozenset(["PERCENTILE_CONT", "PERCENTILE_DISC"])
-# sample / population variance and standard deviation (float64); STDDEV and VARIANCE name the sample forms
-VARIANCES = frozenset(["VAR_SAMP", "VAR_POP", "STDDEV_SAMP", "STDDEV_POP"])
+
+
+class Aggregate(NamedTuple):
+    """What the engine knows of one aggregate head.  ``family``: ``basic`` (SUM COUNT AVG MIN MAX), ``pick`` (FIRST
+    LAST), ``percentile``, ``variance`` or ``bivariate``.  ``result``: ``int64``, ``float64``, ``arg`` (the argument's
+    type) or ``sum`` (int64, float64 for a float argument).  ``frames``, what ``over()`` takes: ``any`` frame,
+    ``running`` (the whole partition or running=True only) or ``none`` (the whole partition only)."""
+    family: str
+    result: str
+    frames: str
+
+
+# every aggregate head (STDDEV and VARIANCE name the sample forms); all of them have a window form.  The variances
+# and the SQL:2003 binary set functions are float64 but REGR_COUNT; x is args[0] of CORR / COVAR_*, args[1] of the
+# REGR_* functions (see bivariate_xy)
+AGGREGATES: Dict[str, Aggregate] = {
+    "SUM": Aggregate("basic", "sum", "any"), "COUNT": Aggregate("basic", "int64", "any"),
+    "AVG": Aggregate("basic", "float64", "any"), "MIN": Aggregate("basic", "arg", "any"),
+    "MAX": Aggregate("basic", "arg", "any"), "FIRST": Aggregate("pick", "arg", "any"),
+    "LAST": Aggregate("pick", "arg", "any"),
+    "PERCENTILE_CONT": Aggregate("percentile", "float64", "none"),
+    "PERCENTILE_DISC": Aggregate("percentile", "arg", "none"),
+    **{h: Aggregate("variance", "float64", "running") for h in ("VAR_SAMP", "VAR_POP", "STDDEV_SAMP", "STDDEV_POP")},
+    "REGR_COUNT": Aggregate("bivariate", "int64", "running"),
+    **{h: Aggregate("bivariate", "float64", "running")
+       for h in ("CORR", "COVAR_POP", "COVAR_SAMP", "REGR_AVGX", "REGR_AVGY", "REGR_SXX", "REGR_SYY", "REGR_SXY",
+                 "REGR_SLOPE", "REGR_INTERCEPT", "REGR_R2")},
+}
+PERCENTILES = frozenset(h for h, a in AGGREGATES.items() if a.family == "percentile")
+VARIANCES = frozenset(h for h, a in AGGREGATES.items() if a.family == "variance")
+BIVARIATES = frozenset(h for h, a in AGGREGATES.items() if a.family == "bivariate")
 _AGG_ALIASES = {"STDDEV": "STDDEV_SAMP", "VARIANCE": "VAR_SAMP"}
-# SQL:2003 binary set functions of two arguments (float64; REGR_COUNT int64); x is args[0] of CORR / COVAR_*,
-# args[1] of the REGR_* functions (see bivariate_xy)
-BIVARIATES = frozenset(["CORR", "COVAR_POP", "COVAR_SAMP", "REGR_COUNT", "REGR_AVGX", "REGR_AVGY", "REGR_SXX",
-                        "REGR_SYY", "REGR_SXY", "REGR_SLOPE", "REGR_INTERCEPT", "REGR_R2"])
 _RANKINGS = frozenset(["ROW_NUMBER", "RANK", "DENSE_RANK"])
 _RUNNING_FRAME = "ROWS BETWEEN UNBOUNDED PRECEDING AND CURRENT ROW"
 _LITERAL_TYPES = (int, bool, float, str, datetime.date, datetime.datetime, datetime.timedelta)
@@ -83,6 +105,17 @@ FLOAT_FUNCTIONS = frozenset(["SQRT", "EXP", "LN", "LOG10", "POWER", "POW"])  # a
 ROUND_MAX_DIGITS = 18
 # functions that build a string from one string expression and literals (SUBSTRING is SUBSTR); ``||`` too
 STRING_FUNCTIONS = frozenset(["UPPER", "LOWER", "SUBSTR", "SUBSTRING", "TRIM", "LTRIM", "RTRIM", "REPLACE", "CONCAT"])
+
+
+def result_type(head: str, arg_type: Optional[pa.DataType]) -> Optional[pa.DataType]:
+    """The type of aggregate ``head`` of an argument of type ``arg_type`` (None: unknown, and so is a result that
+    depends on it)."""
+    rule = AGGREGATES[head].result
+    if rule in ("int64", "float64"):
+        return pa.type_for_alias(rule)
+    if rule == "arg" or arg_type is None:
+        return arg_type
+    return pa.float64() if pa.types.is_floating(arg_type) else pa.int64()
 
 
 def to_pa_datatype(obj: Any) -> pa.DataType:
@@ -243,8 +276,11 @@ class ColumnExpr:
             fits = (pa.types.is_signed_integer(tp) or pa.types.is_floating(tp)) if self.head == "-" \
                 else pa.types.is_boolean(tp)
             return tp if fits else None
-        if k == Kind.AGG and self.head in AGG_KEEPS_ARG_TYPE:
-            return self.args[0].infer_type(schema)
+        if k in (Kind.AGG, Kind.WINDOW) and self.head in AGGREGATES:
+            a = AGGREGATES[self.head]
+            if k == Kind.AGG and a.family == "basic" and a.result != "arg":
+                return None  # SUM / COUNT / AVG: select() keeps the type the group-by gives them
+            return result_type(self.head, self.args[0].infer_type(schema))
         if k == Kind.CALL and self.head in ("LIKE", "LENGTH"):
             return pa.bool_() if self.head == "LIKE" else pa.int64()
         if k == Kind.CALL and self.head.upper() in STRING_FUNCTIONS:
@@ -257,21 +293,8 @@ class ColumnExpr:
             return _operand(self.args[0]).infer_type(schema)
         if k == Kind.CALL and case_string_results(self) is not None:
             return pa.string()
-        if k in (Kind.AGG, Kind.WINDOW) and self.head in PERCENTILES:
-            return pa.float64() if self.head == "PERCENTILE_CONT" else self.args[0].infer_type(schema)
-        if k in (Kind.AGG, Kind.WINDOW) and self.head in VARIANCES:
-            return pa.float64()
-        if k in (Kind.AGG, Kind.WINDOW) and self.head in BIVARIATES:
-            return pa.int64() if self.head == "REGR_COUNT" else pa.float64()
         if k == Kind.WINDOW:
-            if self.head in _RANKINGS or self.head == "COUNT":
-                return pa.int64()
-            if self.head == "AVG":
-                return pa.float64()
-            tp = self.args[0].infer_type(schema)
-            if self.head == "SUM" and tp is not None:
-                return pa.float64() if pa.types.is_floating(tp) else pa.int64()
-            return tp  # SUM of an unknown type: None; MIN MAX FIRST LAST LAG LEAD keep the argument's type
+            return pa.int64() if self.head in _RANKINGS else self.args[0].infer_type(schema)  # LAG LEAD: the arg's
         return None
 
     # ---- text -------------------------------------------------------------------------------------
@@ -356,12 +379,12 @@ class ColumnExpr:
             raise ValueError(f"{self} is not an aggregation: only an aggregation has an OVER form")
         if self.is_distinct:
             raise ValueError(f"{self}: DISTINCT aggregations have no window form")
-        if self.head not in WINDOW_AGGS and self.head not in PERCENTILES and self.head not in VARIANCES and \
-                self.head not in BIVARIATES:
+        a = AGGREGATES.get(self.head)
+        if a is None:
             raise ValueError(f"{self}: {self.head} has no window form")
         if not isinstance(running, bool):
             raise ValueError(f"running must be a bool, got {running!r}")
-        if self.head in PERCENTILES:
+        if a.frames == "none":
             if running or rows is not None or range is not None:
                 raise ValueError(f"{self}: a percentile covers the whole partition; it takes no frame")
             return ColumnExpr(Kind.WINDOW, self.head, self.args, self.kwargs, False, self.as_name, self.as_type)
@@ -385,12 +408,12 @@ class ColumnExpr:
                 running, rows = True, None
             elif rows == (None, None):
                 rows = None
-        if (self.head in VARIANCES or self.head in BIVARIATES) and (rows is not None or range is not None):
+        if a.frames == "running" and (rows is not None or range is not None):
             raise NotImplementedError(f"{self}: {self.head} runs over the whole partition or running=True; "
                                       "ROWS and RANGE frames are not supported")
         if any(is_agg(a) or has_window(a) for a in self.args):
             raise ValueError(f"nested aggregation {self}")
-        if self.head in ("FIRST", "LAST") and self.args[0].kind == Kind.WILDCARD:
+        if a.family == "pick" and self.args[0].kind == Kind.WILDCARD:
             raise ValueError(f"{self}: {self.head} needs a column")
         if range is not None:
             kwargs: Dict[str, Any] = {"range": range}

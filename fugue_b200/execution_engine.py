@@ -10,13 +10,13 @@ The arithmetic runs in ``libfugue_b200.so`` through ``fugue_b200.kernels``; ther
 no CPU implementation of the partition/join/aggregate steps in this package.
 """
 import logging
-import math
 from typing import Any, Callable, Dict, List, Optional, Tuple
 
 import pandas as pd
 import pyarrow as pa
 import torch
 
+from . import aggregates as A
 from . import kernels as K
 from .dataframe import (ArrowDataFrame, B200DataFrame, DataFrame, LocalDataFrame, PandasDataFrame,
                         as_fugue_df)
@@ -275,15 +275,6 @@ def _deviations(devs: Dict[Tuple[int, int], Any], add: Any, v: torch.Tensor, m: 
         devs[k] = (add(v, m, K.AGG_SUM_F64), add(None, m, K.AGG_COUNT), add(v, m, K.AGG_DEV_F64),
                    add(v, m, K.AGG_DEV2_F64))
     return devs[k]
-
-
-def _f64_column(t: "B200Table", name: str, wide: Dict[str, torch.Tensor]) -> torch.Tensor:
-    """Column ``name`` of ``t`` widened to contiguous f64 as AVG reads it, once per call (``wide`` caches it)."""
-    if name not in wide:
-        i = t.schema.index_of_key(name)
-        v = widen(t.columns[i], t.schema.types[i])
-        wide[name] = (v if v.dtype == torch.float64 else v.to(torch.float64)).contiguous()
-    return wide[name]
 
 
 def finish_avgs(res: "B200DataFrame", post: List[Any], want: List[str]) -> "B200DataFrame":
@@ -611,31 +602,28 @@ class B200ExecutionEngine(EngineLifecycle):
 
     @staticmethod
     def _plain_aggs(agg_cols: List[Any]) -> bool:
-        """``SUM/COUNT/MIN/MAX/AVG/FIRST/LAST/PERCENTILE_*`` of a named column (or ``*``) without casts, and the
-        two-argument aggregates of two named columns: what ``_aggregate_named`` takes directly (and what the
-        distributed engine decomposes into partial / final)."""
-        from .column import BIVARIATES, VARIANCES, ColumnExpr, Kind
+        """Aggregates of named columns (or ``*``, but for FIRST / LAST) without casts: what ``_aggregate_named``
+        takes directly (and what the distributed engine decomposes into partial / final)."""
+        from .column import AGGREGATES, ColumnExpr, Kind
 
-        def one_arg(a: Any) -> bool:
-            return (a.func in ("SUM", "COUNT", "MIN", "MAX", "AVG", "FIRST", "LAST", "PERCENTILE_CONT",
-                               "PERCENTILE_DISC") or a.func in VARIANCES) \
-                and a.arg.kind in (Kind.NAMED, Kind.WILDCARD) and a.arg.as_type is None \
-                and not (a.func in ("FIRST", "LAST") and a.arg.kind == Kind.WILDCARD)
-
-        def two_args(a: Any) -> bool:
-            return a.func in BIVARIATES and all(x.kind == Kind.NAMED and x.as_type is None for x in a.args)
+        def plain(a: Any) -> bool:
+            family = AGGREGATES[a.func].family
+            if family == "bivariate":
+                return all(x.kind == Kind.NAMED and x.as_type is None for x in a.args)
+            return a.arg.kind in (Kind.NAMED, Kind.WILDCARD) and a.arg.as_type is None \
+                and not (family == "pick" and a.arg.kind == Kind.WILDCARD)
 
         return all(isinstance(a, ColumnExpr) and a.kind == Kind.AGG and a.as_type is None and not a.is_distinct
-                   and (two_args(a) or one_arg(a)) for a in agg_cols)
+                   and a.func in AGGREGATES and plain(a) for a in agg_cols)
 
     def _aggregate_named(self, df: Any, partition_spec: Optional[PartitionSpec],
                          agg_cols: List[Any]) -> B200DataFrame:
-        """GROUP BY on named key columns with ``SUM/COUNT/MIN/MAX/AVG`` of named columns."""
+        """GROUP BY on named key columns with the aggregates ``_plain_aggs`` takes: one K6 call, then one finisher
+        per aggregate (``aggregates.py``)."""
         import pyarrow as pa
 
         from . import sort as S
-        from .colmap import bivariate_of, variance_of
-        from .column import BIVARIATES, PERCENTILES, VARIANCES, bivariate_xy
+        from .column import AGGREGATES, PERCENTILES, bivariate_xy, result_type
 
         if any(a.func in PERCENTILES for a in agg_cols):
             return self._aggregate_sorted(df, partition_spec, agg_cols)
@@ -687,7 +675,7 @@ class B200ExecutionEngine(EngineLifecycle):
         vals: List[Any] = []
         vvalid: List[Any] = []
         ops: List[int] = []
-        plan: List[Any] = []  # (name, kind, slots..., out_type)
+        finish: List[Any] = []  # per aggregate: fn(K6 results) -> (column, validity, type, dictionary)
 
         def add(v: Any, m: Any, op: int) -> int:
             vals.append(v)
@@ -709,64 +697,59 @@ class B200ExecutionEngine(EngineLifecycle):
         wide: Dict[str, torch.Tensor] = {}  # argument column -> its f64 values, so that pointers repeat
         pairs: Dict[Any, Any] = {}  # (x, y) argument columns -> the 12 accumulators of the pair
         for a in agg_cols:
-            if a.func in BIVARIATES:
+            fn, family = a.func, AGGREGATES[a.func].family
+            if family == "bivariate":
                 xy = tuple(e.name for e in bivariate_xy(a))
                 if xy not in pairs:
                     pairs[xy] = self._pair_accumulators(t, a, xy, add, devs, wide)
-                plan.append((a.output_name, "covar", pairs[xy], pa.int64() if a.func == "REGR_COUNT" else pa.float64(),
-                             a.func))
+                finish.append(lambda g, s=pairs[xy], fn=fn: (*A.bivariate_of(fn, *self._pair_moments(g, s)),
+                                                             result_type(fn, None), None))
                 continue
-            fn, arg = a.func, a.arg.name
+            arg = a.arg.name
             if fn == "COUNT":
-                if arg == "*":
-                    plan.append((a.output_name, "plain", add(None, None, K.AGG_COUNT), pa.int64(), None))
-                else:
-                    ci = t.schema.index_of_key(arg)
-                    plan.append((a.output_name, "plain", add(None, t.valid[ci], K.AGG_COUNT), pa.int64(), None))
+                s = add(None, None if arg == "*" else t.valid[t.schema.index_of_key(arg)], K.AGG_COUNT)
+                finish.append(lambda g, s=s: (*A.finish_basic("COUNT", None, g[s], None), None))
                 continue
             ci = t.schema.index_of_key(arg)
-            c, m, tp = t.columns[ci], t.valid[ci], t.schema.types[ci]
-            if fn in ("FIRST", "LAST"):
+            c, m, tp, d = t.columns[ci], t.valid[ci], t.schema.types[ci], t.dictionaries.get(arg)
+            A.check_argument(fn, arg, tp, d is not None)
+            if family == "pick":
                 # first / last non-NULL value in input row order: MIN / MAX of the row number over the
                 # rows where the value is not NULL, then one gather (works for every column type)
                 if rowno is None:
                     rowno = torch.arange(n, dtype=torch.int64, device=dev)
                 cnt = add(None, m, K.AGG_COUNT)
-                plan.append((a.output_name, "pick", add(rowno, m, K.AGG_MIN_I64 if fn == "FIRST" else K.AGG_MAX_I64),
-                             tp, (cnt, ci)))
+                op, v = A.reduce_input(fn, rowno, pa.int64())
+                s = add(v, m, op)
+
+                def pick(g: Any, s: int = s, cnt: int = cnt, c: Any = c, tp: Any = tp, d: Any = d) -> Any:
+                    has = g[cnt] > 0
+                    idx = torch.where(has, g[s], torch.zeros_like(g[s]))
+                    return (c[idx].contiguous() if n > 0 else c[:0]), has.to(torch.uint8), tp, d
+
+                finish.append(pick)
                 continue
-            if arg in t.dictionaries:  # MIN / MAX of strings: of the dictionary ranks, mapped back to codes
-                assert_or_throw(fn in ("MIN", "MAX"), NotImplementedError(f"{fn} on a string column"))
+            if d is not None:  # MIN / MAX of strings: of the dictionary ranks, mapped back to codes
                 rank, rm = S.string_ranks(t, arg)
                 cnt = add(None, rm, K.AGG_COUNT)
-                plan.append((a.output_name, "string", add(rank, rm, K.AGG_MIN_I64 if fn == "MIN" else K.AGG_MAX_I64),
-                             tp, (cnt, arg)))
+                op, v = A.reduce_input(fn, rank, pa.int64())
+                s = add(v, rm, op)
+                finish.append(lambda g, s=s, cnt=cnt, d=d, tp=tp: A.finish_string(g[s], g[cnt], d, tp))
                 continue
-            if fn in VARIANCES:
+            if family == "variance":
                 # one SUM, COUNT, DEV, DEV2 per column, shared by all its variances (DESIGN §7i)
-                assert_or_throw(pa.types.is_integer(tp) or pa.types.is_floating(tp),
-                                lambda: NotImplementedError(f"{fn}({arg}): {tp} is not a numeric type"))
-                plan.append((a.output_name, "var", _deviations(devs, add, _f64_column(t, arg, wide), m), pa.float64(),
-                             fn))
+                _, cnt, d1, d2 = _deviations(devs, add, A.f64_values(t, arg, wide), m)
+                finish.append(lambda g, fn=fn, cnt=cnt, d1=d1, d2=d2: (
+                    *A.variance_of(fn, A.m2_of(g[d1].view(torch.float64), g[d2].view(torch.float64),
+                                               g[cnt].to(torch.float64)), g[cnt]), pa.float64(), None))
                 continue
-            is_f = pa.types.is_floating(tp)
-            c8 = widen(c, tp)
             # non-null count -> result validity.  A global aggregate (no keys) always carries it: over an
             # empty input (or an empty shard of a multi-GPU aggregate) SUM / MIN / MAX are NULL, not 0
-            nn = add(None, m, K.AGG_COUNT) if (m is not None or len(keys) == 0) else None
-            if fn == "SUM":
-                plan.append((a.output_name, "plain", add(c8, m, K.AGG_SUM_F64 if is_f else K.AGG_SUM_I64),
-                             pa.float64() if is_f else pa.int64(), nn))
-            elif fn in ("MIN", "MAX"):
-                op = {("MIN", True): K.AGG_MIN_F64, ("MAX", True): K.AGG_MAX_F64,
-                      ("MIN", False): K.AGG_MIN_I64, ("MAX", False): K.AGG_MAX_I64}[(fn, is_f)]
-                plan.append((a.output_name, "plain", add(c8, m, op), tp, nn))
-            elif fn == "AVG":
-                cf = c8 if is_f else c8.to(torch.float64)
-                cnt = nn if nn is not None else add(None, None, K.AGG_COUNT)
-                plan.append((a.output_name, "avg", add(cf, m, K.AGG_SUM_F64), pa.float64(), cnt))
-            else:
-                raise NotImplementedError(f"aggregation {fn}")
+            nn = add(None, m, K.AGG_COUNT) if (m is not None or len(keys) == 0 or A.divides_by_count(fn)) else None
+            op, v = A.reduce_input(fn, c, tp)
+            s = add(v, m, op)
+            finish.append(lambda g, fn=fn, s=s, nn=nn, tp=tp, f64=v.dtype == torch.float64: (*A.finish_basic(
+                fn, g[s].view(torch.float64) if f64 else g[s], None if nn is None else g[nn], tp), None))
         if len(ops) > K.MAX_AGGS and pairs:  # more than one kernel call holds: the sorted route has no such limit
             return self._aggregate_sorted(df, partition_spec, agg_cols)
         assert_or_throw(len(ops) <= K.MAX_AGGS, NotImplementedError(
@@ -783,8 +766,6 @@ class B200ExecutionEngine(EngineLifecycle):
         # ---- assemble the output table
         fields, cols, valids = [], [], []
         if multi:
-            from .table import _storage_dtype
-
             bad = torch.zeros((), dtype=torch.bool, device=dev)
             for k, i, (smin, smax, scnt) in zip(keys, kidx, key_slots):
                 bad |= (gaggs[smin] != gaggs[smax]).any() if scnt is None else \
@@ -800,52 +781,16 @@ class B200ExecutionEngine(EngineLifecycle):
             cols.append(key_column(gkeys, ki).contiguous())
             valids.append(gvalid)
         dicts = {k: t.dictionaries[k] for k in keys if k in t.dictionaries}
-        for name, kind, slot, tp, nn in plan:
-            if kind == "covar":
-                col, v = bivariate_of(nn, *self._pair_moments(gaggs, slot))
-                fields.append(pa.field(name, tp))
-                cols.append(col)
-                valids.append(v)
-                continue
-            if kind == "var":
-                _, cnt, dev_, dev2 = slot
-                m_ = gaggs[cnt]
-                d = gaggs[dev_].view(torch.float64)
-                m2 = torch.clamp_min(gaggs[dev2].view(torch.float64) - d * d / m_.to(torch.float64), 0.0)
-                col, v = variance_of(nn, m2, m_)
-                fields.append(pa.field(name, tp))
-                cols.append(col)
-                valids.append(v)
-                continue
-            raw = gaggs[slot]
-            if kind == "pick":
-                cnt, ci = nn
-                has = gaggs[cnt] > 0
-                idx = torch.where(has, raw, torch.zeros_like(raw))
-                fields.append(pa.field(name, tp))
-                cols.append(t.columns[ci][idx].contiguous() if n > 0 else t.columns[ci][:0])
-                valids.append(has.to(torch.uint8))
-                if t.schema.names[ci] in t.dictionaries:
-                    dicts[name] = t.dictionaries[t.schema.names[ci]]
-                continue
-            if kind == "string":
-                cnt, arg = nn
-                fields.append(pa.field(name, tp))
-                cols.append(S.codes_of_ranks(t.dictionaries[arg], raw))
-                valids.append((gaggs[cnt] > 0).to(torch.uint8))
-                dicts[name] = t.dictionaries[arg]
-                continue
-            v = None if nn is None else (gaggs[nn] > 0).to(torch.uint8)
-            if kind == "avg":
-                cnt = gaggs[nn].to(torch.float64)
-                col = raw.view(torch.float64) / cnt
-                v = (gaggs[nn] > 0).to(torch.uint8)
-            else:
-                col = narrow(raw.view(torch.float64) if pa.types.is_floating(tp) else raw, tp)
-            fields.append(pa.field(name, tp))
-            cols.append(col.contiguous())
+        for a, fin in zip(agg_cols, finish):
+            col, v, tp, d = fin(gaggs)
+            fields.append(pa.field(a.output_name, tp))
+            cols.append(col)
             valids.append(v)
+            if d is not None:
+                dicts[a.output_name] = d
         return B200DataFrame(B200Table(Schema(fields), cols, valids, dicts))
+
+    _pair_moments = staticmethod(A.pair_moments)  # (m, x̄, ȳ, Sxx, Syy, Sxy) from the 12 accumulators of a pair
 
     @staticmethod
     def _pair_accumulators(t: B200Table, a: Any, xy: Tuple[str, str], add: Any, devs: Dict[Tuple[int, int], Any],
@@ -856,15 +801,12 @@ class B200ExecutionEngine(EngineLifecycle):
         deviation sets and f64 columns (see ``_deviations``): x and y share their SUM, DEV2 (and x its DEV) with a
         variance of the same column and validity.  The DEV of y always follows the CODEV, so it is a second DEV of y
         when a set for y came first; K6 gives it sums of its own."""
-        import pyarrow as pa
-
         f64, masks = [], []
         for nm in xy:
-            tp = t.schema.types[t.schema.index_of_key(nm)]
-            assert_or_throw(nm not in t.dictionaries and (pa.types.is_integer(tp) or pa.types.is_floating(tp)),
-                            lambda: NotImplementedError(f"{a.func}: {nm} is {tp}, not a numeric type"))
-            f64.append(_f64_column(t, nm, wide))
-            masks.append(t.valid[t.schema.index_of_key(nm)])
+            i = t.schema.index_of_key(nm)
+            A.check_argument(a.func, nm, t.schema.types[i], nm in t.dictionaries)
+            f64.append(A.f64_values(t, nm, wide))
+            masks.append(t.valid[i])
         x, y = f64
         mx, my = masks
         p = mx if my is None else (my if mx is None else (mx & my).contiguous())
@@ -891,27 +833,6 @@ class B200ExecutionEngine(EngineLifecycle):
         return (sx, sy, cnt, dx, d2x, codev, dy, d2y,
                 add(x, p, K.AGG_MIN_F64), add(x, p, K.AGG_MAX_F64), add(y, p, K.AGG_MIN_F64), add(y, p, K.AGG_MAX_F64))
 
-    @staticmethod
-    def _pair_moments(gaggs: List[torch.Tensor], slots: Tuple[int, ...]) -> Tuple[torch.Tensor, ...]:
-        """(m, mean x, mean y, Sxx, Syy, Sxy) per group from a pair's accumulators: the corrected two-pass
-        DEV2 - DEV^2 / m (clamped at 0) and CODEV - DEVx DEVy / m.  A column whose MIN equals its MAX is constant:
-        its S is exactly 0 and so is Sxy (the mean summed with atomics is not exactly the constant).  A NaN or
-        +-inf on either side (a MIN or MAX that is not finite) makes all three NaN."""
-        sx, sy, cnt, dx, d2x, cod, dy, d2y, mnx, mxx, mny, mxy = (gaggs[i] for i in slots)
-        f = [q.view(torch.float64) for q in (sx, sy, dx, d2x, cod, dy, d2y, mnx, mxx, mny, mxy)]
-        sx, sy, dx, d2x, cod, dy, d2y, mnx, mxx, mny, mxy = f
-        m = cnt
-        mf = m.to(torch.float64)
-        zero = torch.zeros_like(mf)
-        cx, cy = mnx == mxx, mny == mxy
-        sxx = torch.where(cx, zero, torch.clamp_min(d2x - dx * dx / mf, 0.0))
-        syy = torch.where(cy, zero, torch.clamp_min(d2y - dy * dy / mf, 0.0))
-        sxy = torch.where(cx | cy, zero, cod - dx * dy / mf)
-        finite = torch.isfinite(mnx) & torch.isfinite(mxx) & torch.isfinite(mny) & torch.isfinite(mxy)
-        nan = torch.full_like(mf, math.nan)
-        return (m, sx / mf, sy / mf, torch.where(finite, sxx, nan), torch.where(finite, syy, nan),
-                torch.where(finite, sxy, nan))
-
     def _aggregate_sorted(self, df: Any, partition_spec: Optional[PartitionSpec],
                           agg_cols: List[Any]) -> B200DataFrame:
         """GROUP BY with a percentile among the aggregates: sort by the keys (stable, so FIRST / LAST keep their
@@ -923,7 +844,7 @@ class B200ExecutionEngine(EngineLifecycle):
 
         from . import sort as S
         from .colmap import _with_windows
-        from .column import Kind, col
+        from .column import AGGREGATES, Kind, col
 
         t: B200Table = self.to_df(df).native
         keys = [] if partition_spec is None else list(partition_spec.partition_by)
@@ -944,12 +865,12 @@ class B200ExecutionEngine(EngineLifecycle):
         if n == 0 and not keys:  # SQL: a global aggregate of an empty table is one row, NULL but for COUNT
             for a, e in zip(agg_cols, nodes):
                 tp = e.infer_type(sub.schema) or pa.float64()
-                is_count = a.func in ("COUNT", "REGR_COUNT")
+                is_count = AGGREGATES[a.func].result == "int64"
                 fields.append(pa.field(a.output_name, tp))
                 cols.append(narrow(torch.zeros(1, dtype=torch.float64 if pa.types.is_floating(tp) else torch.int64,
                                                device=dev), tp).contiguous())
                 valids.append(None if is_count else torch.zeros(1, dtype=torch.uint8, device=dev))
-                if len(a.args) == 1 and a.func not in ("COUNT", "PERCENTILE_CONT") and a.arg.name in sub.dictionaries:
+                if len(a.args) == 1 and a.arg.name in sub.dictionaries and tp == sub.schema[a.arg.name].type:
                     dicts[a.output_name] = sub.dictionaries[a.arg.name]
             return B200DataFrame(B200Table(Schema(fields), cols, valids, dicts))
         w = _with_windows(sub, nodes)
@@ -980,7 +901,7 @@ class B200ExecutionEngine(EngineLifecycle):
         SQL text.  Pins: fugue_test/execution_suite.py:98-155."""
         from . import expr as X
         from . import relational as R
-        from .column import (BIVARIATES, PERCENTILES, VARIANCES, ColumnExpr, Kind, SelectColumns, agg as _agg, col,
+        from .column import (AGGREGATES, BIVARIATES, PERCENTILES, ColumnExpr, Kind, SelectColumns, agg as _agg, col,
                              has_window, is_agg)
 
         for e in list(cols.all_cols) + [where, having]:
@@ -1034,9 +955,7 @@ class B200ExecutionEngine(EngineLifecycle):
             uid = bare.fingerprint()
             if uid in agg_col:
                 continue
-            assert_or_throw(a.func in ("SUM", "COUNT", "MIN", "MAX", "AVG", "FIRST", "LAST", "PERCENTILE_CONT",
-                                       "PERCENTILE_DISC") or a.func in VARIANCES or a.func in BIVARIATES,
-                            NotImplementedError(f"aggregation {a.func}"))
+            assert_or_throw(a.func in AGGREGATES, NotImplementedError(f"aggregation {a.func}"))
             assert_or_throw(not any(is_agg(x) for x in a.args), ValueError(f"nested aggregation {a}"))
             out = f"__fb_a{len(agg_col)}"
             agg_col[uid] = out

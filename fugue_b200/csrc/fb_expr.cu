@@ -24,7 +24,7 @@
 
 #include <cuda_fp16.h>
 
-#include "fb_common.cuh"
+#include "fb_calendar.cuh"
 
 namespace {
 
@@ -169,18 +169,8 @@ __device__ __noinline__ double fn_ln(double x) { return log(x); }
 __device__ __noinline__ double fn_log10(double x) { return log10(x); }
 __device__ __noinline__ double fn_pow(double x, double y) { return pow(x, y); }
 
-// ---- temporal ops (one row): proleptic Gregorian calendar, UTC, no leap seconds.  A value is an int64 count of
-// `unit`s since 1970-01-01 00:00.  Sums and products are taken on uint64 (they wrap, never overflow a signed type);
-// every division is by a positive compile-time constant and floors, so no instruction can trap.
-__device__ __forceinline__ int64_t wadd(int64_t a, int64_t b) { return (int64_t)((uint64_t)a + (uint64_t)b); }
-__device__ __forceinline__ int64_t wsub(int64_t a, int64_t b) { return (int64_t)((uint64_t)a - (uint64_t)b); }
-__device__ __forceinline__ int64_t wmul(int64_t a, int64_t b) { return (int64_t)((uint64_t)a * (uint64_t)b); }
-template <int64_t C>
-__device__ __forceinline__ int64_t fdiv(int64_t x) {  // floor(x / C)
-  const int64_t q = x / C;
-  return q - (int64_t)(x % C < 0);
-}
-
+// ---- temporal ops (one row): proleptic Gregorian calendar (fb_calendar.cuh), UTC, no leap seconds.  A value is an
+// int64 count of `unit`s since 1970-01-01 00:00.
 __device__ __forceinline__ int64_t units_per_second(int unit) {
   switch (unit) {
     case FB_TU_MS: return 1000ll;
@@ -209,8 +199,6 @@ __device__ __forceinline__ int64_t join_days(int64_t days, int64_t sod, int unit
   return wmul(wadd(wmul(days, 86400ll), sod), units_per_second(unit));
 }
 
-__device__ __forceinline__ bool is_leap(int64_t y) { return (y & 3) == 0 && (y % 100 != 0 || y % 400 == 0); }
-
 // days since the epoch -> year, month (1-12), day (1-31), day of the year (1-366): 400-year eras of 146 097 days,
 // years that start on March 1
 __device__ __forceinline__ void civil_from_days(int64_t days, int64_t& y, int& m, int& d, int& doy) {
@@ -224,15 +212,6 @@ __device__ __forceinline__ void civil_from_days(int64_t days, int64_t& y, int& m
   m = mp < 10 ? mp + 3 : mp - 9;
   y = wadd(wadd((int64_t)yoe, wmul(era, 400ll)), (int64_t)(m <= 2));
   doy = mp < 10 ? doy_m + 60 + (int)is_leap(y) : doy_m - 305;
-}
-
-__device__ __forceinline__ int64_t days_from_civil(int64_t y, int m, int d) {
-  y = wsub(y, (int64_t)(m <= 2));
-  const int64_t era = fdiv<400ll>(y);
-  const int yoe = (int)wsub(y, wmul(era, 400ll));                                // [0, 399]
-  const int doy_m = (153 * (m > 2 ? m - 3 : m + 9) + 2) / 5 + d - 1;
-  const int doe = yoe * 365 + yoe / 4 - yoe / 100 + doy_m;
-  return wsub(wadd(wmul(era, 146097ll), (int64_t)doe), 719468ll);
 }
 
 __device__ __forceinline__ int iso_weekday(int64_t days) {  // 1 = Monday ... 7 = Sunday; 1970-01-01 was a Thursday

@@ -467,18 +467,26 @@ class B200DataFrame(DataFrame):
         return B200DataFrame(self._table.select(columns))
 
     def alter_columns(self, columns: Any) -> DataFrame:
-        """Casts run on the device (one fb_eval_expr program); strings <-> numbers go through the host."""
+        """Casts run on the device (one fb_eval_expr program), casts from strings to numbers, bools, dates and
+        timestamps included (K13); casts to strings and to the types the device does not parse to go through the
+        host."""
         new = self._altered_schema(columns)
         if new is None:
             return self
         from . import expr as X
         from .column import col
+        from .strings import StringParseError
 
         try:
             exprs = [col(n) if tp == self._schema[n].type else col(n).cast(tp) for n, tp in zip(new.names, new.types)]
             return B200DataFrame(X.project(self._table, exprs))
         except NotImplementedError:
-            return B200DataFrame(super().alter_columns(columns).as_arrow())
+            from .table import B200Table
+
+            host = super().alter_columns(columns).as_arrow()
+            return B200DataFrame(B200Table.from_arrow(host, self._table.device))
+        except StringParseError as e:  # a string that does not parse, as the host path reports it
+            raise FugueDataFrameOperationError(str(e)) from e
 
     def rename(self, columns: Dict[str, str]) -> DataFrame:
         try:

@@ -24,6 +24,10 @@ Dates and timestamps are int64 counts of their Arrow unit.  A temporal literal (
 interval) is rescaled on the host to the unit of the temporal operand it meets and becomes a plain immediate; two
 temporal columns meet as their raw integers, and the unit-correct form is an explicit ``CAST`` between temporal types
 (``FB_X_MULSAT_I`` / ``FB_X_FLOORDIV_I``).  ``EXTRACT DATE_TRUNC DATEDIFF ADD_MONTHS`` are the ``FB_X_TS_*`` ops.
+A ``CAST`` of a string column, or of a string-building expression, to a number, bool, date or timestamp is Arrow's
+``cast(safe=False)`` of the entry: every entry is parsed once (``strings.parse_table``, K13) and each row reads its
+entry's value (``FB_X_LOOKUP``); the result has the target's class and, for a date or timestamp, its unit.  A string
+that does not parse raises ValueError when a valid row refers to it.  A cast string literal is cast on the host.
 """
 import datetime
 import struct
@@ -110,6 +114,28 @@ def _in_unit(v: Any, unit: int) -> Tuple[int, bool]:
 def _const_predicate(x: ColumnExpr, truth: bool) -> ColumnExpr:
     """``truth`` where ``x`` is not NULL, NULL elsewhere (Kleene: TRUE OR NULL, FALSE AND NULL)."""
     return (x.not_null() | _lit(None)) if truth else (x.is_null() & _lit(None))
+
+
+def string_literal_cast(e: ColumnExpr) -> ColumnExpr:
+    """``CAST('text' AS tp)`` folded on the host by Arrow's cast: a literal of the value's class that keeps the cast
+    (a date or timestamp is its count of the type's unit) and the alias.  ValueError when the text does not parse,
+    NotImplementedError for a target the device does not parse to."""
+    import pyarrow.compute as pc
+
+    tp = e.as_type
+    ST.parse_target(tp)
+    try:
+        v = pc.cast(pa.array([e.value], type=pa.string()), tp, safe=False)
+    except (pa.ArrowInvalid, pa.ArrowNotImplementedError):
+        raise ST.parse_error(e.value, tp) from None
+    if pa.types.is_date32(tp):
+        py: Any = v.view(pa.int32())[0].as_py()
+    elif pa.types.is_date64(tp) or pa.types.is_timestamp(tp):
+        py = v.view(pa.int64())[0].as_py()
+    else:
+        py = v[0].as_py()
+    out = _lit(py).cast(tp)
+    return out.alias(e.as_name) if e.as_name != "" else out
 
 
 class _OutOfResources(Exception):
@@ -271,6 +297,11 @@ class _Program:
 
     # -- compilation: value ends up in the accumulator; returns (class, nullable)
     def compile(self, e: ColumnExpr, top: bool = False) -> Tuple[str, bool]:
+        if e.as_type is not None and not _is_str(e.as_type):
+            if e.kind == Kind.LITERAL and isinstance(e.value, str):
+                return self.compile(string_literal_cast(e))
+            if self._is_string_operand(e.cast(None)):
+                return self._parse_cast(e)
         cls, nullable = self._node(e)
         if e.as_type is not None:
             want = _cls_of(e.as_type)
@@ -284,6 +315,42 @@ class _Program:
                 self._acc_to(cls, want)
                 cls = want
         return cls, nullable
+
+    # -- casts from strings
+    def _is_string_operand(self, x: ColumnExpr) -> bool:
+        """A string column or a string-building expression (what a cast can parse)."""
+        if x.kind == Kind.NAMED:
+            return x.as_type is None and x.name in self.t.schema and _is_str(self.t.schema[x.name].type)
+        return is_string_build(x) and (x.as_type is None or _is_str(x.as_type))
+
+    def _parse_cast(self, e: ColumnExpr) -> Tuple[str, bool]:
+        """``CAST(s AS tp)``: the entry's code, then ``FB_X_LOOKUP`` into the dictionary's parse table.  Raises
+        ValueError when a valid row refers to an entry that does not parse."""
+        t, tp, x = self.t, e.as_type, e.cast(None)
+        ST.parse_target(tp)  # NotImplementedError before anything runs for a target the device does not parse to
+        if x.kind == Kind.NAMED:
+            d = t.dictionaries[x.name]
+            ci = t.schema.index_of_key(x.name)
+            r = ST.parse_table(d, t.device, tp)
+            ST.check_referenced(r, d, tp, t.columns[ci], t.valid[ci])
+            key: Any = ("PARSE", x.name, tp)
+            self.emit(K.X_MOV, K.XK_COL, self.col_slot(ci))
+            row_null = t.valid[ci] is not None
+        else:
+            name, steps = ST.string_chain(x, t.dictionaries)
+            src = ST.evaluate(t.dictionaries[name], t.device, steps)
+            d, row_null = self.string_codes(x)
+            r = ST.parse_table(d, t.device, tp)
+            ci = t.schema.index_of_key(name)
+            ST.check_referenced(r, d, tp, t.columns[ci], t.valid[ci], src.remap, src.remap_valid, src.null_code)
+            key = ("PARSE", ("STR", name, steps), tp)
+        values, valid = r.values, r.valid
+        if len(d) == 0:  # every row is NULL: a one-entry table that is never read, for a real device pointer
+            values = torch.zeros(1, dtype=torch.int64, device=t.device)
+            valid = torch.zeros(1, dtype=torch.uint8, device=t.device)
+        self.tables[key] = (values, valid)
+        self.emit(K.X_LOOKUP, K.XK_COL, self.col_slot(key), 0, len(d))
+        return _cls_of(tp), row_null or valid is not None
 
     # -- dates and timestamps
     def _ttype(self, e: Any) -> Optional[pa.DataType]:
@@ -590,8 +657,9 @@ class _Program:
         sides = [e.left, e.right]
         named = [s.kind == Kind.NAMED and s.as_type is None and s.name in t.schema
                  and _is_str(t.schema[s.name].type) for s in sides]
-        built = [is_string_build(s) for s in sides]
-        lits = [s.kind == Kind.LITERAL and isinstance(s.value, str) for s in sides]
+        built = [is_string_build(s) and (s.as_type is None or _is_str(s.as_type)) for s in sides]
+        lits = [s.kind == Kind.LITERAL and isinstance(s.value, str) and (s.as_type is None or _is_str(s.as_type))
+                for s in sides]
         if not (any(named) or any(lits) or any(built)):
             return None
         if e.op not in ("==", "!="):
@@ -950,8 +1018,10 @@ def project(t: B200Table, exprs: Sequence[ColumnExpr]) -> B200Table:
                 if e.name in t.dictionaries:
                     dicts[names[i]] = t.dictionaries[e.name]
                 continue
-            if _is_str(tp):
+            if _is_str(tp) and _is_str(e.as_type):
                 raise NotImplementedError(f"cast of string column {e.name} to {e.as_type}")
+        if e.kind == Kind.LITERAL and isinstance(e.value, str) and e.as_type is not None and not _is_str(e.as_type):
+            e = string_literal_cast(e)
         if e.kind == Kind.LITERAL and (isinstance(e.value, str) or e.value is None):
             tp = e.as_type or (pa.string() if isinstance(e.value, str) else None)
             if tp is None:
@@ -963,8 +1033,6 @@ def project(t: B200Table, exprs: Sequence[ColumnExpr]) -> B200Table:
                 if _is_str(tp):
                     dicts[names[i]] = pa.array([], type=pa.string())
             else:
-                if not _is_str(tp):
-                    raise NotImplementedError(f"cast of string literal {e} to {tp}")
                 dicts[names[i]] = pa.array([e.value], type=pa.string())
             continue
         strs = case_string_results(e)
@@ -983,7 +1051,7 @@ def project(t: B200Table, exprs: Sequence[ColumnExpr]) -> B200Table:
             i, e = pending[k]
             mark = prog.mark()
             try:
-                if is_string_build(e):  # int32 codes into the result's dictionary
+                if is_string_build(e) and (e.as_type is None or _is_str(e.as_type)):  # codes into the result's dictionary
                     str_built[i], nullable = prog.string_codes(e)
                     prog.output(torch.int32, nullable, K.T_I32)
                     out_types[i] = pa.string()

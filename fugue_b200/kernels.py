@@ -7,6 +7,7 @@ import ctypes as C
 import struct
 from typing import Any, List, Optional, Sequence, Tuple
 
+import numpy as np
 import torch
 
 from . import _lib
@@ -1056,3 +1057,48 @@ def string_first_equal(offsets: torch.Tensor, data: torch.Tensor, valid: Optiona
                                          0 if valid is None else valid.data_ptr(), sorted_hash.data_ptr(),
                                          sorted_idx.data_ptr(), out.data_ptr()))
     return out
+
+
+# ---- K13: string casts over a dictionary's entries ----------------------------------------------
+(PARSE_I8, PARSE_I16, PARSE_I32, PARSE_I64, PARSE_U8, PARSE_U16, PARSE_U32, PARSE_U64, PARSE_F32, PARSE_F64,
+ PARSE_BOOL, PARSE_DATE32, PARSE_DATE64) = range(13)
+PARSE_TS, PARSE_TS_ZONED = 16, 8  # PARSE_TS + TU_S .. TU_NS (+ PARSE_TS_ZONED)
+PARSE_OK, PARSE_NULL, PARSE_INVALID, PARSE_UNDECIDED = range(4)
+
+
+def string_parse(offsets: torch.Tensor, data: torch.Tensor, valid: Optional[torch.Tensor], target: int
+                 ) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor, Optional[int]]:
+    """Every entry of a device dictionary parsed to ``target`` (a ``PARSE_*`` code): (value int64, validity uint8,
+    status uint8 per entry, the smallest entry whose status is ``PARSE_INVALID`` / ``PARSE_UNDECIDED`` or None).
+    The last one is the only value read back to the host."""
+    lib = _lib.load()
+    dev = offsets.device
+    n = int(offsets.shape[0]) - 1
+    out = torch.empty(max(n, 1), dtype=torch.int64, device=dev)
+    out_valid = torch.empty(max(n, 1), dtype=torch.uint8, device=dev)
+    status = torch.empty(max(n, 1), dtype=torch.uint8, device=dev)
+    first_bad = torch.empty(1, dtype=torch.int64, device=dev)
+    _lib.check(lib.fb_string_parse(dev.index, _stream_ptr(dev), n, offsets.data_ptr(), data.data_ptr(),
+                                   0 if valid is None else valid.data_ptr(), target, out.data_ptr(),
+                                   out_valid.data_ptr(), status.data_ptr(), first_bad.data_ptr()))
+    bad = int(first_bad.item())  # UINT64_MAX reads as -1
+    return out[:n], out_valid[:n], status[:n], (None if bad < 0 else bad)
+
+
+def string_parse_host(offsets: np.ndarray, data: np.ndarray, valid: Optional[np.ndarray], target: int
+                      ) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+    """``string_parse`` on the CPU over host arrays (int64 ``offsets``, uint8 ``data`` / ``valid``), by the same
+    parse routines: (value int64, validity uint8, status uint8)."""
+    lib = _lib.load()
+    n = int(offsets.shape[0]) - 1
+    offsets = np.ascontiguousarray(offsets, dtype=np.int64)
+    data = np.ascontiguousarray(data, dtype=np.uint8) if len(data) else np.zeros(1, dtype=np.uint8)
+    out = np.empty(max(n, 1), dtype=np.int64)
+    out_valid = np.empty(max(n, 1), dtype=np.uint8)
+    status = np.empty(max(n, 1), dtype=np.uint8)
+    if valid is not None:
+        valid = np.ascontiguousarray(valid, dtype=np.uint8)
+    _lib.check(lib.fb_debug_string_parse_host(n, offsets.ctypes.data, data.ctypes.data,
+                                              0 if valid is None else valid.ctypes.data, target, out.ctypes.data,
+                                              out_valid.ctypes.data, status.ctypes.data))
+    return out[:n], out_valid[:n], status[:n]

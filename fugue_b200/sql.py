@@ -28,6 +28,8 @@ import datetime
 import re
 from typing import Any, Dict, List, Tuple
 
+import pyarrow as pa
+
 from .column import BIVARIATES, ColumnExpr, Kind, SelectColumns, all_cols, col, function, functions, is_agg, lit, null
 from .dataframe import DataFrame
 
@@ -331,6 +333,27 @@ _TWO_ARGS = {"NULLIF": functions.nullif, "IFNULL": functions.coalesce, "MOD": la
              "POWER": functions.power, "POW": functions.power}
 
 
+# SQL type names inside CAST(... AS type), as schema types; every other name is read by the schema grammar
+_SQL_TYPES = {("bigint",): "long", ("integer",): "int", ("int",): "int", ("smallint",): "short", ("tinyint",): "byte",
+              ("real",): "float", ("double",): "double", ("double", "precision"): "double", ("varchar",): "str",
+              ("text",): "str", ("boolean",): "bool", ("date",): "date", ("timestamp",): "datetime"}
+
+
+def _cast_type(toks: List[Tuple[str, str]]) -> Any:
+    """The type of ``CAST(x AS <toks>)``: a SQL type name, ``timestamp(unit[, time zone])`` or a schema type
+    expression (``long``, ``timestamp(ns,UTC)``, ...)."""
+    words = tuple(v.lower() for _, v in toks)
+    if words in _SQL_TYPES:
+        return _SQL_TYPES[words]
+    if len(words) >= 4 and words[:2] == ("timestamp", "(") and words[-1] == ")":
+        inner = toks[2:-1]
+        cut = next((i for i, t in enumerate(inner) if t == ("op", ",")), len(inner))
+        unit = "".join(v for _, v in inner[:cut]).lower()
+        tz = "".join(_unquote(v) if k == "str" else v for k, v in inner[cut + 1:]) or None
+        return pa.timestamp(unit, tz)
+    return "".join(v for _, v in toks).lower()
+
+
 def _tokenize(text: str, sql: str) -> List[Tuple[str, str]]:
     out: List[Tuple[str, str]] = []
     pos = 0
@@ -539,12 +562,14 @@ class _Parser:
                 e = self.expr()
                 if not self.kw("AS"):
                     self.fail("CAST without AS")
-                tp = []
-                while self.peek() != ("op", ")") and self.peek()[0] != "end":
-                    tp.append(self.peek()[1])
+                tp: List[Tuple[str, str]] = []
+                depth = 0
+                while self.peek()[0] != "end" and (depth > 0 or self.peek() != ("op", ")")):
+                    depth += {"(": 1, ")": -1}.get(self.peek()[1], 0) if self.peek()[0] == "op" else 0
+                    tp.append(self.peek())
                     self.i += 1
                 self.expect(")")
-                return e.cast("".join(tp).lower())
+                return e.cast(_cast_type(tp))
             if self.peek(1) == ("op", "("):
                 return self._call(up)
             self.i += 1

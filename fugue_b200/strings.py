@@ -16,6 +16,13 @@ A string-building expression over one string column is a function of the entry t
 on the device (one measure and one write launch per step; intermediate dictionaries stay on the device),
 deduplicates the results and returns the new dictionary and the entry -> new code table the rows are mapped
 through (``FB_X_LOOKUP``).  Results are cached per (dictionary object, chain) the same way as uploads.
+
+A cast of a string to a number, bool, date or timestamp is a function of the entry as well (K13,
+``fb_strparse.cu``): ``parse_table`` parses every entry once and returns the per-entry table ``FB_X_LOOKUP`` reads,
+cached per (dictionary object, device, target type).  The parse is Arrow's ``cast(safe=False)`` of the entry; the
+few floats of more than 19 significant digits the device leaves undecided are re-parsed by pyarrow on the host
+(``parse_fallbacks`` counts them).  An entry that does not parse is an error only when a valid row of the table
+being evaluated refers to it (``check_referenced``).
 """
 import weakref
 from typing import Any, Dict, List, Optional, Sequence, Tuple
@@ -31,6 +38,8 @@ _CACHE: Dict[int, Tuple[Any, Dict[Any, Any]]] = {}     # dictionary -> {device: 
 _DERIVED: Dict[int, Tuple[Any, Dict[Any, Any]]] = {}   # dictionary -> {(chain, device): StringResult}
 uploads = 0     # dictionaries copied to a device so far (the cache's misses)
 transforms = 0  # string expressions evaluated over a dictionary so far (the result cache's misses)
+parses = 0      # dictionaries parsed to a type so far (the parse cache's misses)
+parse_fallbacks = 0  # entries re-parsed on the host because the device left them undecided
 
 
 class DeviceDictionary:
@@ -358,3 +367,121 @@ def evaluate(d: pa.Array, device: torch.device, steps: Tuple[Any, ...]) -> Strin
     if key not in per:
         per[key] = _evaluate(d, device, steps)
     return per[key]
+
+
+# ---- casts from strings (K13) -------------------------------------------------------------------------
+_INT_TARGETS = {8: (K.PARSE_I8, K.PARSE_U8), 16: (K.PARSE_I16, K.PARSE_U16), 32: (K.PARSE_I32, K.PARSE_U32),
+                64: (K.PARSE_I64, K.PARSE_U64)}
+_TS_UNITS = {"s": K.TU_S, "ms": K.TU_MS, "us": K.TU_US, "ns": K.TU_NS}
+
+
+def parse_target(tp: pa.DataType) -> int:
+    """The ``fb_string_parse`` target of a cast from a string to ``tp``; NotImplementedError for a type the device
+    does not parse to (float16, decimal, binary, nested, time, duration ...)."""
+    if pa.types.is_integer(tp):
+        return _INT_TARGETS[tp.bit_width][pa.types.is_unsigned_integer(tp)]
+    if pa.types.is_float32(tp) or pa.types.is_float64(tp):
+        return K.PARSE_F32 if pa.types.is_float32(tp) else K.PARSE_F64
+    if pa.types.is_boolean(tp):
+        return K.PARSE_BOOL
+    if pa.types.is_date32(tp) or pa.types.is_date64(tp):
+        return K.PARSE_DATE32 if pa.types.is_date32(tp) else K.PARSE_DATE64
+    if pa.types.is_timestamp(tp):
+        return K.PARSE_TS + _TS_UNITS[tp.unit] + (K.PARSE_TS_ZONED if tp.tz is not None else 0)
+    raise NotImplementedError(f"cast of a string to {tp} has no device implementation")
+
+
+class StringParseError(ValueError):
+    """A string a valid row refers to does not parse as the cast's target type (worded as Arrow words it)."""
+
+
+def parse_error(entry: Any, tp: pa.DataType) -> StringParseError:
+    return StringParseError(f"Failed to parse string: '{entry}' as a scalar of type {tp}")
+
+
+class ParseResult:
+    """A dictionary parsed to one type: ``values`` (int64 per entry, the 8-byte words ``FB_X_LOOKUP`` reads),
+    ``valid`` (uint8, 0 for a NULL entry or one that does not parse; None: every entry parsed) and ``bad`` (int64
+    device tensor of the entries that do not parse, None if there is none)."""
+
+    def __init__(self, values: torch.Tensor, valid: Optional[torch.Tensor], bad: Optional[torch.Tensor]):
+        self.values, self.valid, self.bad = values, valid, bad
+
+
+def _parse(d: pa.Array, device: torch.device, tp: pa.DataType) -> ParseResult:
+    global parses, parse_fallbacks
+    target = parse_target(tp)
+    parses += 1
+    dd = device_dictionary(d, device)
+    values, valid, status, first_bad = K.string_parse(dd.offsets, dd.data, dd.valid, target)
+    bad = None
+    if first_bad is not None:
+        undecided = torch.nonzero(status == K.PARSE_UNDECIDED).squeeze(1).cpu().tolist()
+        if undecided:
+            import pyarrow.compute as pc
+
+            parse_fallbacks += len(undecided)
+            for i in undecided:  # a float of more than 19 significant digits: pyarrow rounds it
+                try:
+                    v = pc.cast(d[i:i + 1], tp, safe=False)
+                except (pa.ArrowInvalid, pa.ArrowNotImplementedError):
+                    status[i] = K.PARSE_INVALID
+                    continue
+                word = v.cast(pa.float64()).to_numpy(zero_copy_only=False).view(np.int64)[0]
+                values[i] = int(word)
+                valid[i] = 1
+                status[i] = K.PARSE_OK
+        idx = torch.nonzero(status == K.PARSE_INVALID).squeeze(1)
+        bad = idx if int(idx.shape[0]) > 0 else None
+    if dd.valid is None and bad is None:
+        valid = None
+    return ParseResult(values, valid, bad)
+
+
+def parse_table(d: pa.Array, device: torch.device, tp: pa.DataType) -> ParseResult:
+    """Every entry of dictionary ``d`` cast to ``tp`` on ``device``: parsed on first use, then cached on ``d``, so
+    a repeated call launches nothing and reads nothing back."""
+    per = _slot(_DERIVED, d)
+    key = (("PARSE", tp), device)
+    if key not in per:
+        per[key] = _parse(d, device, tp)
+    return per[key]
+
+
+def check_referenced(r: ParseResult, d: pa.Array, tp: pa.DataType, codes: torch.Tensor,
+                     code_valid: Optional[torch.Tensor], remap: Optional[torch.Tensor] = None,
+                     remap_valid: Optional[torch.Tensor] = None, null_code: Optional[int] = None) -> None:
+    """Raise the parse error of the first row that refers to an entry of ``d`` that does not parse.  ``codes`` /
+    ``code_valid``: the rows' codes; with ``remap`` they are codes of a source dictionary whose entry ``e`` is entry
+    ``remap[e]`` of ``d`` (``remap_valid``: 0 where it is NULL), and a NULL row is entry ``null_code`` (None: NULL).
+    Costs nothing when every entry parsed."""
+    if r.bad is None:
+        return
+    dev = codes.device
+    bad = torch.zeros(len(d), dtype=torch.bool, device=dev)
+    bad[r.bad] = True
+    if remap is not None:
+        src = bad[remap.clamp(0, max(len(d) - 1, 0))]
+        if remap_valid is not None:
+            src &= remap_valid.bool()
+        src_of = remap
+    else:
+        src, src_of = bad, None
+    c = codes.long()
+    inside = (c >= 0) & (c < int(src.shape[0]))
+    hit = src[c.clamp(0, max(int(src.shape[0]) - 1, 0))] & inside
+    if code_valid is not None:
+        hit &= code_valid.bool()
+        if null_code is not None and bool(bad[null_code].item()):
+            hit |= ~code_valid.bool()
+    rows = torch.nonzero(hit)
+    if int(rows.shape[0]) == 0:
+        return
+    row = int(rows[0, 0].item())
+    if code_valid is not None and not bool(code_valid[row].item()):
+        entry = null_code
+    else:
+        entry = int(c[row].item())
+        if src_of is not None:
+            entry = int(src_of[entry].item())
+    raise parse_error(d[entry].as_py(), tp)

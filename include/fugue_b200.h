@@ -680,6 +680,42 @@ int fb_string_first_equal(int dev, void* stream, int64_t n, const int64_t* offse
                           const uint8_t* valid, const uint64_t* sorted_hash, const int64_t* sorted_idx,
                           int64_t* canon);
 
+/* ---------------------------------------------------------------------------
+ * K13 string casts, evaluated once per dictionary entry
+ * Replaces: Arrow's cast(string -> type, safe=False) on the host, which a string column's CAST needed (a copy of
+ *           the table to the host and back).
+ * Dictionaries have the K11 layout.  Entry i parses to what Arrow's cast(safe=False) of the one string gives
+ * (DESIGN.md section 7l):
+ *   FB_PARSE_I8 .. FB_PARSE_U64  decimal with an optional '-' (unsigned: none), in the target's range; or 0x / 0X
+ *                                and 1 to 2 * bytes hex digits, read as two's complement of the width
+ *   FB_PARSE_F32 / FB_PARSE_F64  [+-] digits [. digits] [(e|E) [+-] digits], or [+-] inf / infinity / nan /
+ *                                nan(chars) in any case; correctly rounded to the target
+ *   FB_PARSE_BOOL                true / false in any case, 1, 0
+ *   FB_PARSE_DATE32 / _DATE64    YYYY-MM-DD, a valid day of the proleptic Gregorian calendar
+ *   FB_PARSE_TS + unit (FB_TU_S .. FB_TU_NS), + FB_PARSE_TS_ZONED when the target has a time zone:
+ *                                YYYY-MM-DD[(T| )HH[:MM[:SS[.f]]]], at most as many fraction digits as the unit
+ *                                holds; zoned targets require Z / +-HH / +-HHMM / +-HH:MM after the time and store
+ *                                the UTC instant, others refuse an offset; the value must fit int64 in the unit.
+ * fb_string_parse : out[i] = the value as one 8-byte word (an integer in the target's storage units; float64
+ *                   bits for F64, and the float64 widening of the float32 for F32), out_valid[i] = 1 when it
+ *                   parsed, status[i] = FB_PARSE_OK / _NULL (a NULL entry) / _INVALID / _UNDECIDED (a float of
+ *                   more than 19 significant digits whose truncation does not decide the rounding).  first_bad
+ *                   (one DEVICE uint64) = the smallest i whose status is INVALID or UNDECIDED, or UINT64_MAX.
+ * fb_debug_string_parse_host : the same over HOST arrays, on the CPU (no first_bad).
+ * One thread per entry, grid-stride.
+ * --------------------------------------------------------------------------- */
+enum fb_parse_target {
+  FB_PARSE_I8 = 0, FB_PARSE_I16 = 1, FB_PARSE_I32 = 2, FB_PARSE_I64 = 3, FB_PARSE_U8 = 4, FB_PARSE_U16 = 5,
+  FB_PARSE_U32 = 6, FB_PARSE_U64 = 7, FB_PARSE_F32 = 8, FB_PARSE_F64 = 9, FB_PARSE_BOOL = 10, FB_PARSE_DATE32 = 11,
+  FB_PARSE_DATE64 = 12, FB_PARSE_TS = 16, FB_PARSE_TS_ZONED = 8
+};
+enum fb_parse_status { FB_PARSE_OK = 0, FB_PARSE_NULL = 1, FB_PARSE_INVALID = 2, FB_PARSE_UNDECIDED = 3 };
+int fb_string_parse(int dev, void* stream, int64_t n, const int64_t* offsets, const uint8_t* data,
+                    const uint8_t* valid, int target, uint64_t* out, uint8_t* out_valid, uint8_t* status,
+                    uint64_t* first_bad);
+int fb_debug_string_parse_host(int64_t n, const int64_t* offsets, const uint8_t* data, const uint8_t* valid,
+                               int target, uint64_t* out, uint8_t* out_valid, uint8_t* status);
+
 #ifdef __cplusplus
 }
 #endif

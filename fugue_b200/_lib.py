@@ -107,6 +107,9 @@ SIGNATURES = {
     "fb_segmented_comoments_scratch_bytes": (C.c_size_t, [C.c_int64, C.c_int]),
     "fb_segmented_comoments": (C.c_int, [C.c_int, _vp, C.c_int64, C.c_int64, _vp, C.c_int, _vpp, _vpp, _vpp, _vpp,
                                          _vpp, _vpp, _vpp, _vpp, _vpp, _vpp, _vp, C.c_size_t]),
+    "fb_segmented_shape_moments_scratch_bytes": (C.c_size_t, [C.c_int64, C.c_int]),
+    "fb_segmented_shape_moments": (C.c_int, [C.c_int, _vp, C.c_int64, C.c_int64, _vp, C.c_int, _vpp, _vpp, _vpp,
+                                             _vpp, _vpp, _vpp, _vp, C.c_size_t]),
     "fb_window_frame_scratch_bytes": (C.c_size_t, [C.c_int64, C.c_int, C.c_int64, C.c_int64, C.c_int]),
     "fb_window_frame": (C.c_int, [C.c_int, _vp, C.c_int64, C.c_int64, _vp, C.c_int64, C.c_int64, C.c_int, C.c_int,
                                   _i32p, _vpp, _vpp, _vpp, _vpp, _vp, C.c_size_t]),

@@ -25,8 +25,9 @@ _OPS = {("SUM", False): K.AGG_SUM_I64, ("SUM", True): K.AGG_SUM_F64, ("AVG", Tru
 
 def check_argument(fn: str, name: str, tp: pa.DataType, is_dictionary: bool) -> None:
     """Reject an argument column ``name`` of arrow type ``tp`` that ``fn`` does not take: the variances and the
-    two-argument functions need integer or float columns, and a string column takes no SUM or AVG."""
-    if AGGREGATES[fn].family in ("variance", "bivariate"):
+    shape statistics and the two-argument functions need integer or float columns, and a string column takes no SUM
+    or AVG."""
+    if AGGREGATES[fn].family in ("variance", "shape", "bivariate"):
         if is_dictionary or not (pa.types.is_integer(tp) or pa.types.is_floating(tp)):
             raise NotImplementedError(f"{fn} needs integer or float columns; {name} is {tp}")
     elif is_dictionary and fn in ("SUM", "AVG"):
@@ -92,6 +93,50 @@ def variance_of(fn: str, m2: torch.Tensor, count: torch.Tensor) -> Tuple[torch.T
     v = m2 / torch.where(has, count - (1 if samp else 0), torch.ones_like(count)).to(torch.float64)
     if fn.startswith("STDDEV"):
         v = torch.sqrt(v)
+    return torch.where(has, v, torch.zeros_like(v)).contiguous(), has.to(torch.uint8)
+
+
+def shape_moments(gaggs: Sequence[torch.Tensor], slots: Tuple[int, ...]) -> Tuple[torch.Tensor, ...]:
+    """(m, M2, M3, M4) per group from the K6 accumulators ``slots`` of a column: SUM, COUNT, DEV, DEV2, DEV3, DEV4,
+    MIN, MAX.  DEV .. DEV4 are the sums of d^k, d = x - c, about the atomically summed mean c; with delta = DEV / m
+    the central sums are exactly M2 = DEV2 - m delta^2, M3 = DEV3 - 3 delta DEV2 + 2 m delta^3 and
+    M4 = DEV4 - 4 delta DEV3 + 6 delta^2 DEV2 - 3 m delta^4 (M2 and M4 clamped at 0).  A column whose MIN equals its
+    MAX is constant: all three are exactly 0.  A MIN or MAX that is not finite (a NaN or +-inf) makes all three NaN."""
+    _, m, d1, d2, d3, d4, mn, mx = (gaggs[i] for i in slots)
+    d1, d2, d3, d4, mn, mx = (q.view(torch.float64) for q in (d1, d2, d3, d4, mn, mx))
+    mf = m.to(torch.float64)
+    delta = d1 / mf
+    dd = delta * delta
+    m2 = torch.clamp_min(d2 - mf * dd, 0.0)
+    m3 = d3 - 3.0 * delta * d2 + 2.0 * mf * dd * delta
+    m4 = torch.clamp_min(d4 - 4.0 * delta * d3 + 6.0 * dd * d2 - 3.0 * mf * dd * dd, 0.0)
+    const = mn == mx
+    finite = torch.isfinite(mn) & torch.isfinite(mx)
+    zero, nan = torch.zeros_like(mf), torch.full_like(mf, math.nan)
+    return (m, *(torch.where(finite, torch.where(const, zero, v), nan) for v in (m2, m3, m4)))
+
+
+def shape_of(fn: str, m: torch.Tensor, m2: torch.Tensor, m3: torch.Tensor,
+             m4: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+    """``fn`` (a ``SHAPES`` head) from the non-NULL count m and the central sums M2, M3, M4: (float64 values,
+    validity).  SKEWNESS (pandas ``skew()``) is NULL when m < 3, KURTOSIS (pandas ``kurt()``, excess) when m < 4, the
+    population forms when m = 0.  M2 = 0 (a constant column) gives 0; a NaN M2 gives NaN."""
+    need = {"SKEWNESS": 3, "KURTOSIS": 4}.get(fn, 1)
+    has = m >= need
+    mf = torch.where(has, m, torch.full_like(m, need)).to(torch.float64)
+    flat = m2 == 0
+    s2 = torch.where(flat, torch.ones_like(m2), m2)
+    if fn.startswith("SKEWNESS"):
+        w = mf * torch.sqrt(mf - 1.0) / (mf - 2.0) if fn == "SKEWNESS" else torch.sqrt(mf)
+        v = w * m3 / (s2 * torch.sqrt(s2))
+    else:
+        g = mf * m4 / (s2 * s2)
+        if fn == "KURTOSIS":
+            den = (mf - 2.0) * (mf - 3.0)
+            v = ((mf + 1.0) * (mf - 1.0) * g - 3.0 * (mf - 1.0) * (mf - 1.0)) / den
+        else:
+            v = g - 3.0
+    v = torch.where(flat, torch.zeros_like(v), v)
     return torch.where(has, v, torch.zeros_like(v)).contiguous(), has.to(torch.uint8)
 
 

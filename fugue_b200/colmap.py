@@ -234,6 +234,7 @@ def _with_windows(t: B200Table, cols: List[ColumnExpr]) -> B200Table:
     scans: Dict[Any, List[Any]] = {}
     quantiles: Dict[str, List[Tuple[float, int]]] = {}  # argument column -> its (q, CONT | DISC) pairs
     moments: Dict[str, int] = {}  # argument column of a variance -> its column of the moments scan
+    shapes: Dict[str, int] = {}  # argument column of a skewness or kurtosis -> its column of the shape-moments scan
     comoments: Dict[Tuple[str, str], int] = {}  # (x, y) argument columns of a pair -> its pair of the co-moments scan
     finish: List[Any] = []     # per node: (fingerprint, fn(scan results) -> (column, validity, type, dictionary))
 
@@ -312,6 +313,11 @@ def _with_windows(t: B200Table, cols: List[ColumnExpr]) -> B200Table:
             finish.append((uid, lambda r, j=j, e=at_end, fn=fn: (
                 *A.variance_of(fn, e(r[("moments", j)][1]), e(r[("moments", j)][0])), pa.float64(), None)))
             continue
+        if family == "shape":  # the shape-moments scan; frames are rejected by over()
+            j = shapes.setdefault(name, len(shapes))
+            finish.append((uid, lambda r, j=j, e=at_end, fn=fn: (
+                *A.shape_of(fn, *(e(x) for x in r[("shape", j)])), pa.float64(), None)))
+            continue
         i = scan(*A.reduce_input(fn, c, tp), m, frame)
         finish.append((uid, lambda r, i=i, e=at_end, fn=fn, tp=tp: (
             *A.finish_basic(fn, e(r[i][0]), e(r[i][1]), tp), None)))
@@ -354,6 +360,9 @@ def _with_windows(t: B200Table, cols: List[ColumnExpr]) -> B200Table:
     if moments:
         mcols = [f64_valid(name) for name in moments]
         results.update((("moments", j), r) for j, r in enumerate(K.segmented_moments(off.contiguous(), n, mcols)))
+    if shapes:
+        scols = [f64_valid(name) for name in shapes]
+        results.update((("shape", j), r) for j, r in enumerate(K.segmented_shape_moments(off.contiguous(), n, scols)))
     if comoments:
         pairs = [f64_valid(x) + f64_valid(y) for x, y in comoments]
         results.update((("comoments", j), r) for j, r in enumerate(K.segmented_comoments(off.contiguous(), n, pairs)))

@@ -13,13 +13,13 @@ from an expression is a function of ``(kind, head, args)``:
               args (string[, characters]); ``REPLACE``: args (string, from, to); ``CONCAT``: args (part, ...)
               ``EXTRACT``: args (x,), kwarg ``field``; ``DATE_TRUNC``: args (x,), kwarg ``part``; ``DATEDIFF``: args
               (a, b), kwarg ``part``; ``ADD_MONTHS``: args (x, n)
-    AGG       head in ``SUM COUNT AVG MIN MAX FIRST LAST VAR_SAMP VAR_POP STDDEV_SAMP STDDEV_POP``, one arg,
-              optional DISTINCT, or ``PERCENTILE_CONT PERCENTILE_DISC``, one arg and kwarg ``q`` (MEDIAN is
+    AGG       head in ``SUM COUNT AVG MIN MAX FIRST LAST VAR_SAMP VAR_POP STDDEV_SAMP STDDEV_POP SKEWNESS
+              SKEWNESS_POP KURTOSIS KURTOSIS_POP``, one arg, optional DISTINCT, or ``PERCENTILE_CONT PERCENTILE_DISC``, one arg and kwarg ``q`` (MEDIAN is
               PERCENTILE_CONT at q = 0.5), or ``CORR COVAR_POP COVAR_SAMP REGR_COUNT REGR_AVGX REGR_AVGY
               REGR_SXX REGR_SYY REGR_SXY REGR_SLOPE REGR_INTERCEPT REGR_R2``, two args (a, b) as in SQL: the
               REGR_* functions take the dependent variable y first, (y, x)
     WINDOW    head in the AGG functions (their args, kwargs ``running``, ``rows`` or ``range``; a percentile keeps
-              its ``q`` and covers the whole partition; a variance or a two-argument aggregate takes ``running``
+              its ``q`` and covers the whole partition; a variance, a shape statistic or a two-argument aggregate takes ``running``
               only), ``ROW_NUMBER RANK
               DENSE_RANK`` (no arg) or ``LAG LEAD`` (one arg, kwargs ``n`` and ``default``): evaluated over the logical
               partitions of ``fa.transform`` (PartitionSpec keys, presort order) by a ``ColumnMap``
@@ -63,7 +63,7 @@ ARITH_OPS = frozenset(["+", "-", "*", "/", "%"])
 
 class Aggregate(NamedTuple):
     """What the engine knows of one aggregate head.  ``family``: ``basic`` (SUM COUNT AVG MIN MAX), ``pick`` (FIRST
-    LAST), ``percentile``, ``variance`` or ``bivariate``.  ``result``: ``int64``, ``float64``, ``arg`` (the argument's
+    LAST), ``percentile``, ``variance``, ``shape`` (skewness and kurtosis) or ``bivariate``.  ``result``: ``int64``, ``float64``, ``arg`` (the argument's
     type) or ``sum`` (int64, float64 for a float argument).  ``frames``, what ``over()`` takes: ``any`` frame,
     ``running`` (the whole partition or running=True only) or ``none`` (the whole partition only)."""
     family: str
@@ -71,8 +71,9 @@ class Aggregate(NamedTuple):
     frames: str
 
 
-# every aggregate head (STDDEV and VARIANCE name the sample forms); all of them have a window form.  The variances
-# and the SQL:2003 binary set functions are float64 but REGR_COUNT; x is args[0] of CORR / COVAR_*, args[1] of the
+# every aggregate head (STDDEV and VARIANCE name the sample forms, SKEW and KURT the bias-corrected shape statistics);
+# all of them have a window form.  The variances, the shape statistics and the SQL:2003 binary set functions are
+# float64 but REGR_COUNT; x is args[0] of CORR / COVAR_*, args[1] of the
 # REGR_* functions (see bivariate_xy)
 AGGREGATES: Dict[str, Aggregate] = {
     "SUM": Aggregate("basic", "sum", "any"), "COUNT": Aggregate("basic", "int64", "any"),
@@ -82,6 +83,7 @@ AGGREGATES: Dict[str, Aggregate] = {
     "PERCENTILE_CONT": Aggregate("percentile", "float64", "none"),
     "PERCENTILE_DISC": Aggregate("percentile", "arg", "none"),
     **{h: Aggregate("variance", "float64", "running") for h in ("VAR_SAMP", "VAR_POP", "STDDEV_SAMP", "STDDEV_POP")},
+    **{h: Aggregate("shape", "float64", "running") for h in ("SKEWNESS", "SKEWNESS_POP", "KURTOSIS", "KURTOSIS_POP")},
     "REGR_COUNT": Aggregate("bivariate", "int64", "running"),
     **{h: Aggregate("bivariate", "float64", "running")
        for h in ("CORR", "COVAR_POP", "COVAR_SAMP", "REGR_AVGX", "REGR_AVGY", "REGR_SXX", "REGR_SYY", "REGR_SXY",
@@ -89,8 +91,9 @@ AGGREGATES: Dict[str, Aggregate] = {
 }
 PERCENTILES = frozenset(h for h, a in AGGREGATES.items() if a.family == "percentile")
 VARIANCES = frozenset(h for h, a in AGGREGATES.items() if a.family == "variance")
+SHAPES = frozenset(h for h, a in AGGREGATES.items() if a.family == "shape")
 BIVARIATES = frozenset(h for h, a in AGGREGATES.items() if a.family == "bivariate")
-_AGG_ALIASES = {"STDDEV": "STDDEV_SAMP", "VARIANCE": "VAR_SAMP"}
+_AGG_ALIASES = {"STDDEV": "STDDEV_SAMP", "VARIANCE": "VAR_SAMP", "SKEW": "SKEWNESS", "KURT": "KURTOSIS"}
 _RANKINGS = frozenset(["ROW_NUMBER", "RANK", "DENSE_RANK"])
 _RUNNING_FRAME = "ROWS BETWEEN UNBOUNDED PRECEDING AND CURRENT ROW"
 _LITERAL_TYPES = (int, bool, float, str, datetime.date, datetime.datetime, datetime.timedelta)
@@ -491,7 +494,8 @@ def function(name: str, *args: Any, arg_distinct: bool = False, **kwargs: Any) -
 
 def agg(func: str, arg: Any, as_name: str = "", arg_distinct: bool = False) -> ColumnExpr:
     """``FUNC([DISTINCT] arg)``: SUM / COUNT / AVG / MIN / MAX / FIRST / LAST / VAR_SAMP / VAR_POP / STDDEV_SAMP /
-    STDDEV_POP (STDDEV and VARIANCE give the sample forms)."""
+    STDDEV_POP / SKEWNESS / SKEWNESS_POP / KURTOSIS / KURTOSIS_POP (STDDEV and VARIANCE give the sample forms, SKEW
+    and KURT the bias-corrected ones)."""
     func = func.upper()
     return ColumnExpr(Kind.AGG, _AGG_ALIASES.get(func, func), [col(arg)], None, arg_distinct, as_name)
 
@@ -926,6 +930,34 @@ class functions:
     def stddev_pop(c: Any) -> ColumnExpr:
         """sqrt(VAR_POP): pandas ``std(ddof=0)``."""
         return agg("STDDEV_POP", c)
+
+    # ---- shape statistics (DESIGN §7m) of the m non-NULL values, from their central sums Mk = sum of (x - mean)^k.
+    # NaN and +-inf are values: one makes the result NaN.  A constant column gives 0.
+    @staticmethod
+    def skewness(c: Any) -> ColumnExpr:
+        """Bias-corrected skewness G1 = m sqrt(m - 1) / (m - 2) * M3 / M2^1.5: pandas ``skew()`` (float64; NULL when
+        m < 3)."""
+        return agg("SKEWNESS", c)
+
+    skew = skewness
+
+    @staticmethod
+    def skewness_pop(c: Any) -> ColumnExpr:
+        """Population skewness g1 = sqrt(m) * M3 / M2^1.5 (float64; NULL when m = 0)."""
+        return agg("SKEWNESS_POP", c)
+
+    @staticmethod
+    def kurtosis(c: Any) -> ColumnExpr:
+        """Bias-corrected excess kurtosis G2 = m (m + 1) (m - 1) M4 / ((m - 2)(m - 3) M2^2) - 3 (m - 1)^2 /
+        ((m - 2)(m - 3)): pandas ``kurt()`` (float64; NULL when m < 4)."""
+        return agg("KURTOSIS", c)
+
+    kurt = kurtosis
+
+    @staticmethod
+    def kurtosis_pop(c: Any) -> ColumnExpr:
+        """Population excess kurtosis g2 = m M4 / M2^2 - 3: DuckDB ``kurtosis_pop`` (float64; NULL when m = 0)."""
+        return agg("KURTOSIS_POP", c)
 
     # ---- two-argument aggregates (SQL:2003 binary set functions, DESIGN §7k).  Only the rows where both
     # arguments are non-NULL take part; m is their number.  NaN and +-inf are values, not NULL.

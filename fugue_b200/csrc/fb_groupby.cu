@@ -30,6 +30,11 @@
 // Covariance (FB_AGG_CODEV_F64, DESIGN §7k): pass B also adds dx * dy of a pair row into CODEV, with dx and dy the
 // row's deviations from its group's SUM / COUNT of x and of y; Sxy = CODEV - DEVx * DEVy / m is the same
 // correction applied to the cross sum.
+//
+// Skewness and kurtosis (FB_AGG_DEV3_F64 / FB_AGG_DEV4_F64, DESIGN §7m): pass B also adds d^3 and d^4 with the same d.
+// The host takes the central sums M2, M3, M4 about the exact mean from the four sums about SUM / COUNT.  Only the
+// fb_groupby_dev_kernel instantiations with kShape carry the two extra atomics, so a call with variances alone runs
+// the same code as before.
 #include "fb_common.cuh"
 
 namespace {
@@ -48,6 +53,8 @@ enum : int32_t {
   kDevF64 = FB_AGG_DEV_F64,
   kDev2F64 = FB_AGG_DEV2_F64,
   kCodevF64 = FB_AGG_CODEV_F64,
+  kDev3F64 = FB_AGG_DEV3_F64,
+  kDev4F64 = FB_AGG_DEV4_F64,
 };
 
 struct AggSpec {
@@ -63,7 +70,7 @@ constexpr int kMaxDevCols = FB_MAX_AGGS / 3;
 struct DevCol {
   const double* val;
   const uint8_t* valid;
-  int32_t sum, cnt, dev, dev2;  // accumulator indices; dev / dev2 = -1 when not asked for
+  int32_t sum, cnt, dev, dev2, dev3, dev4;  // accumulator indices; dev .. dev4 = -1 when not asked for
 };
 // a pair (x, y) with cross deviations: SUM of x, SUM of y, COUNT, CODEV and the DEV of y it is tied to, so at
 // most FB_MAX_AGGS / 5 pairs fit in one call
@@ -381,8 +388,9 @@ __device__ __forceinline__ int64_t find_slot(const uint64_t* __restrict__ table,
 }
 
 // Rows as fb_groupby_kernel walks them (part_off != nullptr: the rows of hash partitions [p0, p1)); per valid
-// value x of a deviation column, d = x - SUM / COUNT of the row's group is added into DEV and d * d into DEV2.
-template <bool kLean>
+// value x of a deviation column, d = x - SUM / COUNT of the row's group is added into DEV and d * d into DEV2, and
+// with kShape d^3 into DEV3 and d^4 into DEV4.
+template <bool kLean, bool kShape>
 __global__ void __launch_bounds__(256)
 fb_groupby_dev_kernel(const uint64_t* __restrict__ keys, const uint8_t* __restrict__ key_valid, int64_t nrows,
                       uint64_t* __restrict__ table, int64_t capacity, int words, const DevSpec spec, FbDiv dv,
@@ -434,6 +442,11 @@ fb_groupby_dev_kernel(const uint64_t* __restrict__ keys, const uint8_t* __restri
       const double dx = d.val[row] - mean;
       if (d.dev >= 0) atomicAdd((double*)(slot + 1 + d.dev), dx);
       if (d.dev2 >= 0) atomicAdd((double*)(slot + 1 + d.dev2), dx * dx);
+      if (kShape) {
+        const double d2 = dx * dx;
+        if (d.dev3 >= 0) atomicAdd((double*)(slot + 1 + d.dev3), d2 * dx);
+        if (d.dev4 >= 0) atomicAdd((double*)(slot + 1 + d.dev4), d2 * d2);
+      }
     }
     if (kLean) continue;  // a pair's accumulators never fit the lean kernel
 #pragma unroll 1
@@ -480,7 +493,22 @@ fb_groupby_extract_kernel(const uint64_t* __restrict__ table, int64_t capacity, 
   }
 }
 
-// also resolves every FB_AGG_DEV_F64 / FB_AGG_DEV2_F64 to the SUM and COUNT of its column, and every
+// pass B with the instantiation the spec needs: the d^3 / d^4 atomics only when a column asks for them
+template <bool kLean>
+void launch_dev(const DevSpec& devs, unsigned grid, cudaStream_t st, const uint64_t* keys, const uint8_t* key_valid,
+                int64_t nrows, uint64_t* table, int64_t capacity, int words, const FbDiv& dv, int64_t region_shift,
+                uint32_t parts_mask, const int64_t* part_off, int p0, int p1) {
+  bool shape = false;
+  for (int c = 0; c < devs.ncols; ++c) shape = shape || devs.col[c].dev3 >= 0 || devs.col[c].dev4 >= 0;
+  if (shape)
+    fb_groupby_dev_kernel<kLean, true><<<grid, 256, 0, st>>>(keys, key_valid, nrows, table, capacity, words, devs, dv,
+                                                             region_shift, parts_mask, part_off, p0, p1);
+  else
+    fb_groupby_dev_kernel<kLean, false><<<grid, 256, 0, st>>>(keys, key_valid, nrows, table, capacity, words, devs, dv,
+                                                              region_shift, parts_mask, part_off, p0, p1);
+}
+
+// also resolves every FB_AGG_DEV_F64 .. FB_AGG_DEV4_F64 to the SUM and COUNT of its column, and every
 // FB_AGG_CODEV_F64 to its y (the DEV_F64 right after it) and the SUMs and COUNT of its pair (pass B's DevSpec)
 int fill_spec(AggSpec& spec, DevSpec& dev, int naggs, const void* const* val_ptrs, const uint8_t* const* val_valid,
               const int32_t* ops) {
@@ -489,7 +517,7 @@ int fill_spec(AggSpec& spec, DevSpec& dev, int naggs, const void* const* val_ptr
   memset(&dev, 0, sizeof(dev));
   spec.naggs = naggs;
   for (int a = 0; a < naggs; ++a) {
-    FB_CHECK(ops[a] >= FB_AGG_SUM_F64 && ops[a] <= FB_AGG_CODEV_F64, "unknown aggregate op %d", ops[a]);
+    FB_CHECK(ops[a] >= FB_AGG_SUM_F64 && ops[a] <= FB_AGG_DEV4_F64, "unknown aggregate op %d", ops[a]);
     FB_CHECK(ops[a] == FB_AGG_COUNT || (val_ptrs != nullptr && val_ptrs[a] != nullptr),
              "aggregate %d needs a value column", a);
     spec.op[a] = ops[a];
@@ -497,7 +525,12 @@ int fill_spec(AggSpec& spec, DevSpec& dev, int naggs, const void* const* val_ptr
     spec.valid[a] = val_valid ? val_valid[a] : nullptr;
   }
   for (int a = 0; a < naggs; ++a) {
-    if (ops[a] != kDevF64 && ops[a] != kDev2F64) continue;
+    int32_t DevCol::*const field = ops[a] == kDevF64    ? &DevCol::dev
+                                   : ops[a] == kDev2F64 ? &DevCol::dev2
+                                   : ops[a] == kDev3F64 ? &DevCol::dev3
+                                   : ops[a] == kDev4F64 ? &DevCol::dev4
+                                                        : nullptr;
+    if (field == nullptr) continue;
     int sum = -1, cnt = -1;
     for (int b = 0; b < naggs; ++b) {
       if (sum < 0 && ops[b] == kSumF64 && spec.val[b] == spec.val[a] && spec.valid[b] == spec.valid[a]) sum = b;
@@ -505,19 +538,19 @@ int fill_spec(AggSpec& spec, DevSpec& dev, int naggs, const void* const* val_ptr
     }
     FB_CHECK(sum >= 0 && cnt >= 0, "aggregate %d (op %d) needs a SUM_F64 and a COUNT of the same column and validity",
              a, ops[a]);
-    // the entry of this column whose DEV (or DEV2) is still free: a second DEV of the same column and validity gets
-    // an entry of its own instead of taking the first one's place (which would leave that accumulator at 0)
-    const bool is_dev = ops[a] == kDevF64;
+    // the entry of this column whose DEV (or DEV2, DEV3, DEV4) is still free: a second DEV of the same column and
+    // validity gets an entry of its own instead of taking the first one's place (which would leave that accumulator
+    // at 0)
     int c = 0;
     while (c < dev.ncols && !(dev.col[c].val == (const double*)spec.val[a] && dev.col[c].valid == spec.valid[a] &&
-                              (is_dev ? dev.col[c].dev : dev.col[c].dev2) < 0))
+                              dev.col[c].*field < 0))
       ++c;
     if (c == dev.ncols) {
       FB_CHECK(c < kMaxDevCols, "more than %d value columns with deviations", kMaxDevCols);
-      dev.col[c] = DevCol{(const double*)spec.val[a], spec.valid[a], sum, cnt, -1, -1};
+      dev.col[c] = DevCol{(const double*)spec.val[a], spec.valid[a], sum, cnt, -1, -1, -1, -1};
       ++dev.ncols;
     }
-    (is_dev ? dev.col[c].dev : dev.col[c].dev2) = a;
+    dev.col[c].*field = a;
   }
   for (int a = 0; a < naggs; ++a) {
     if (ops[a] != kCodevF64) continue;
@@ -597,9 +630,8 @@ int fb_groupby_u64(int dev, void* stream, int64_t nrows, const void* keys, const
                                                      capacity, words, spec, d_status, dv, region_shift,
                                                      d_part_offsets, (int)p0, (int)p1);
       if (devs.ncols + devs.npairs > 0)  // pass B of the batch while its regions are still in L2
-        fb_groupby_dev_kernel<false><<<(unsigned)gb, 256, 0, st>>>((const uint64_t*)keys, key_valid, nrows,
-                                                                  (uint64_t*)table, capacity, words, devs, dv,
-                                                                  region_shift, 0u, d_part_offsets, (int)p0, (int)p1);
+        launch_dev<false>(devs, (unsigned)gb, st, (const uint64_t*)keys, key_valid, nrows, (uint64_t*)table, capacity,
+                          words, dv, region_shift, 0u, d_part_offsets, (int)p0, (int)p1);
     }
     FB_CUDA(cudaGetLastError());
     return 0;
@@ -619,8 +651,8 @@ int fb_groupby_u64(int dev, void* stream, int64_t nrows, const void* keys, const
       default: launch_lean<4>(k64, key_valid, nrows, t64, capacity, spec, d_status, num_parts, (int)region_shift, sms * 8, st); break;
     }
     if (devs.ncols + devs.npairs > 0)
-      fb_groupby_dev_kernel<true><<<sms * 8, 256, 0, st>>>(k64, key_valid, nrows, t64, capacity, words, devs, dv,
-                                                          region_shift, num_parts - 1, nullptr, 0, 0);
+      launch_dev<true>(devs, sms * 8, st, k64, key_valid, nrows, t64, capacity, words, dv, region_shift, num_parts - 1,
+                       nullptr, 0, 0);
     FB_CUDA(cudaGetLastError());
     return 0;
   }
@@ -628,8 +660,8 @@ int fb_groupby_u64(int dev, void* stream, int64_t nrows, const void* keys, const
     fb_groupby_kernel<<<sms * 8, 256, 0, st>>>((const uint64_t*)keys, key_valid, nrows, (uint64_t*)table,
                                               capacity, words, spec, d_status, dv, region_shift, nullptr, 0, 0);
     if (devs.ncols + devs.npairs > 0)
-      fb_groupby_dev_kernel<false><<<sms * 8, 256, 0, st>>>((const uint64_t*)keys, key_valid, nrows, (uint64_t*)table,
-                                                           capacity, words, devs, dv, region_shift, 0u, nullptr, 0, 0);
+      launch_dev<false>(devs, sms * 8, st, (const uint64_t*)keys, key_valid, nrows, (uint64_t*)table, capacity, words,
+                        dv, region_shift, 0u, nullptr, 0, 0);
     FB_CUDA(cudaGetLastError());
   }
   return 0;

@@ -183,8 +183,48 @@ __device__ __forceinline__ CSt shfl_down(const CSt& s, int d) {
              __shfl_down_sync(0xFFFFFFFFu, s.f, d)};
 }
 
+// (count, mean, M2, M3, M4, "a segment starts in here") of the valid values of a run of consecutive rows: the state
+// of fb_segmented_shape_moments
+struct SSt {
+  int64_t c;
+  double mean, m2, m3, m4;
+  int32_t f;
+};
+
+// `a` followed by `b`: Pebay's pairwise update of the third and fourth central sums beside Chan's M2, written in the
+// weights wa = na / n, wb = nb / n.  Every right-hand side reads the old sums.  Equal values give delta = 0 exactly,
+// so a constant run keeps M2 = M3 = M4 = 0; a run without a valid row takes no part.
+__device__ __forceinline__ SSt combine(int, const SSt& a, const SSt& b) {
+  if (b.f) return b;
+  if (b.c == 0) return SSt{a.c, a.mean, a.m2, a.m3, a.m4, a.f};
+  if (a.c == 0) return SSt{b.c, b.mean, b.m2, b.m3, b.m4, a.f};
+  const int64_t n = a.c + b.c;
+  const double rn = __drcp_rn((double)n);
+  const double wa = (double)a.c * rn, wb = (double)b.c * rn;  // na / n, nb / n within 2 u
+  const double d = b.mean - a.mean;
+  const double d2 = d * d;
+  const double t2 = d2 * (double)a.c * wb;  // d^2 na nb / n
+  return SSt{n, a.mean + d * wb, a.m2 + b.m2 + t2,
+             a.m3 + b.m3 + t2 * d * (wa - wb) + 3.0 * d * (wa * b.m2 - wb * a.m2),
+             a.m4 + b.m4 + t2 * d2 * (wa * wa - wa * wb + wb * wb) + 6.0 * d2 * (wa * wa * b.m2 + wb * wb * a.m2) +
+                 4.0 * d * (wa * b.m3 - wb * a.m3),
+             a.f};
+}
+
+__device__ __forceinline__ SSt shfl_up(const SSt& s, int d) {
+  return SSt{(int64_t)__shfl_up_sync(0xFFFFFFFFu, (long long)s.c, d), __shfl_up_sync(0xFFFFFFFFu, s.mean, d),
+             __shfl_up_sync(0xFFFFFFFFu, s.m2, d), __shfl_up_sync(0xFFFFFFFFu, s.m3, d),
+             __shfl_up_sync(0xFFFFFFFFu, s.m4, d), __shfl_up_sync(0xFFFFFFFFu, s.f, d)};
+}
+
+__device__ __forceinline__ SSt shfl_down(const SSt& s, int d) {
+  return SSt{(int64_t)__shfl_down_sync(0xFFFFFFFFu, (long long)s.c, d), __shfl_down_sync(0xFFFFFFFFu, s.mean, d),
+             __shfl_down_sync(0xFFFFFFFFu, s.m2, d), __shfl_down_sync(0xFFFFFFFFu, s.m3, d),
+             __shfl_down_sync(0xFFFFFFFFu, s.m4, d), __shfl_down_sync(0xFFFFFFFFu, s.f, d)};
+}
+
 // Exclusive scan of one state per thread across the CTA, and the CTA total; fixed combination order.
-// kRev: the scan runs from the last thread to the first.  S: St, or MSt / CSt (op unused).
+// kRev: the scan runs from the last thread to the first.  S: St, or MSt / CSt / SSt (op unused).
 template <int kWarps, bool kRev = false, class S = St>
 __device__ __forceinline__ S block_exclusive(int op, const S& x, S* warp_tot, S* total) {
   const int lane = kRev ? 31 - (threadIdx.x & 31) : threadIdx.x & 31;
@@ -603,6 +643,127 @@ fb_segcomoments_carry_kernel(int64_t ntiles, CoTiles ts) {
     ts.sxx[o + t] = run.sxx;
     ts.syy[o + t] = run.syy;
     ts.sxy[o + t] = run.sxy;
+    run = combine(0, run, x);
+  }
+}
+
+// ---- segmented shape moments (fb_segmented_shape_moments): the same three launches over SSt ------------------
+struct ShapeCols {
+  const double* vals[FB_SCAN_MAX_COLS];
+  const uint8_t* valid[FB_SCAN_MAX_COLS];
+  int64_t* out_count[FB_SCAN_MAX_COLS];
+  double* out[3][FB_SCAN_MAX_COLS];  // M2, M3, M4
+  int32_t ncols;
+};
+
+// the tile states of every column, column-major (column * ntiles + tile); f: one per tile
+struct ShapeTiles {
+  int64_t* c;
+  double* mean;
+  double* m2;
+  double* m3;
+  double* m4;
+  int32_t* f;
+};
+
+struct ShapeSmem {
+  double x[padded(kTile)];
+  uint8_t valid[kTile];
+  uint8_t head[kTile];
+  SSt warp_tot[kThreads / 32];
+  int64_t seg_range[2];
+};
+
+// the state of one row: a valid value x enters as (1, x, z, z, z) with z = x - x, +0 for a finite x and NaN
+// otherwise, so that a NaN or an infinity makes M2, M3 and M4 NaN
+__device__ __forceinline__ SSt shape_of(const ShapeSmem& sm, int j) {
+  const int c = sm.valid[j];
+  const double x = c ? sm.x[padded(j)] : 0.0;
+  const double z = x - x;
+  return SSt{c, x, z, z, z, sm.head[j]};
+}
+
+// kFinal = false: pass 1 (tile states); true: pass 3 (the running count, M2, M3 and M4 per row, from the carries).
+// Pass 3 stores a thread's kItems consecutive rows straight from registers, as the co-moments scan does.
+template <bool kFinal>
+__global__ void __launch_bounds__(kThreads)
+fb_segshape_tile_kernel(int64_t nrows, int64_t nseg, const int64_t* __restrict__ offsets,
+                        const __grid_constant__ ShapeCols a, int64_t ntiles, ShapeTiles ts) {
+  __shared__ __align__(16) ShapeSmem sm;
+  const int64_t tile = blockIdx.x;
+  const int64_t start = tile * kTile;
+  const int64_t end = start + kTile < nrows ? start + kTile : nrows;
+  const int nloc = (int)(end - start);
+  mark_heads<false, false>(nrows, nseg, offsets, start, end, 0, sm.head, sm.seg_range);
+  const int j0 = threadIdx.x * kItems;
+  for (int col = 0; col < a.ncols; ++col) {
+    const double* __restrict__ src = a.vals[col];
+    const uint8_t* __restrict__ vm = a.valid[col];
+    for (int i = threadIdx.x; i < kTile; i += kThreads) {
+      const bool in = i < nloc;
+      sm.x[padded(i)] = in ? __ldg(src + start + i) : 0.0;
+      sm.valid[i] = in ? (vm == nullptr ? 1 : (__ldg(vm + start + i) != 0)) : 0;
+    }
+    __syncthreads();
+    SSt acc{};
+#pragma unroll
+    for (int k = 0; k < kItems; ++k) acc = combine(0, acc, shape_of(sm, j0 + k));
+    SSt total;
+    const SSt pre = block_exclusive<kThreads / 32, false, SSt>(0, acc, sm.warp_tot, &total);
+    const int64_t t = col * ntiles + tile;
+    if (!kFinal) {
+      if (threadIdx.x == 0) {
+        ts.c[t] = total.c;
+        ts.mean[t] = total.mean;
+        ts.m2[t] = total.m2;
+        ts.m3[t] = total.m3;
+        ts.m4[t] = total.m4;
+        if (col == 0) ts.f[tile] = total.f;
+      }
+      continue;
+    }
+    SSt run = combine(0, SSt{ts.c[t], ts.mean[t], ts.m2[t], ts.m3[t], ts.m4[t], 0}, pre);
+    int64_t* __restrict__ oc = a.out_count[col];
+#pragma unroll
+    for (int k = 0; k < kItems; ++k) {
+      const int j = j0 + k;
+      run = combine(0, run, shape_of(sm, j));
+      if (j >= nloc) continue;
+      const bool any = run.c > 0;  // no valid row yet: 0, not whatever preceded the segment
+      const double v[3] = {run.m2, run.m3, run.m4};
+      if (oc != nullptr) oc[start + j] = run.c;
+#pragma unroll
+      for (int o = 0; o < 3; ++o)
+        if (a.out[o][col] != nullptr) a.out[o][col][start + j] = any ? v[o] : 0.0;
+    }
+    __syncthreads();  // shared buffers are refilled by the next column
+  }
+}
+
+// pass 2: per column, the exclusive segmented scan of the tile states (in place: state -> carry).  An SSt is
+// five 8-byte words and a flag, near a CSt, so the carry kernel runs the co-moments carry's 512 threads.
+constexpr int kShapeCarryThreads = 512;
+__global__ void __launch_bounds__(kShapeCarryThreads, 1)
+fb_segshape_carry_kernel(int64_t ntiles, ShapeTiles ts) {
+  __shared__ SSt warp_tot[kShapeCarryThreads / 32];
+  const int64_t o = (int64_t)blockIdx.x * ntiles;
+  const int64_t per = (ntiles + kShapeCarryThreads - 1) / kShapeCarryThreads;
+  const int64_t b = threadIdx.x * per;
+  const int64_t e = b + per < ntiles ? b + per : ntiles;
+  auto load = [&](int64_t t) {
+    return SSt{ts.c[o + t], ts.mean[o + t], ts.m2[o + t], ts.m3[o + t], ts.m4[o + t], ts.f[t]};
+  };
+  SSt acc{};
+  for (int64_t t = b; t < e; ++t) acc = combine(0, acc, load(t));
+  SSt total;
+  SSt run = block_exclusive<kShapeCarryThreads / 32, false, SSt>(0, acc, warp_tot, &total);
+  for (int64_t t = b; t < e; ++t) {
+    const SSt x = load(t);
+    ts.c[o + t] = run.c;
+    ts.mean[o + t] = run.mean;
+    ts.m2[o + t] = run.m2;
+    ts.m3[o + t] = run.m3;
+    ts.m4[o + t] = run.m4;
     run = combine(0, run, x);
   }
 }
@@ -1212,6 +1373,54 @@ extern "C" int fb_segmented_comoments(int dev, void* stream, int64_t nrows, int6
   fb_segcomoments_carry_kernel<<<npairs, kCoCarryThreads, 0, st>>>(ntiles, ts);
   FB_CUDA(cudaGetLastError());
   fb_segcomoments_tile_kernel<true><<<(unsigned)ntiles, kThreads, 0, st>>>(nrows, nseg, d_offsets, a, ntiles, ts);
+  FB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+extern "C" size_t fb_segmented_shape_moments_scratch_bytes(int64_t nrows, int ncols) {
+  if (nrows <= 0 || ncols <= 0) return 0;
+  return (size_t)num_tiles(nrows) * (40 * (size_t)ncols + 4);
+}
+
+extern "C" int fb_segmented_shape_moments(int dev, void* stream, int64_t nrows, int64_t nseg, const int64_t* d_offsets,
+                                          int ncols, const void* const* vals, const uint8_t* const* valid,
+                                          int64_t* const* out_count, void* const* out_m2, void* const* out_m3,
+                                          void* const* out_m4, void* scratch, size_t scratch_bytes) {
+  FB_CHECK(nrows >= 0 && nseg >= 0, "negative row or segment count");
+  FB_CHECK(ncols >= 1 && ncols <= FB_SCAN_MAX_COLS, "ncols=%d out of range [1,%d]", ncols, FB_SCAN_MAX_COLS);
+  ShapeCols a;
+  memset(&a, 0, sizeof(a));
+  a.ncols = ncols;
+  void* const* outs[3] = {out_m2, out_m3, out_m4};
+  for (int c = 0; c < ncols; ++c) {
+    a.vals[c] = vals != nullptr ? (const double*)vals[c] : nullptr;
+    a.valid[c] = valid != nullptr ? valid[c] : nullptr;
+    a.out_count[c] = out_count != nullptr ? out_count[c] : nullptr;
+    for (int o = 0; o < 3; ++o) a.out[o][c] = outs[o] != nullptr ? (double*)outs[o][c] : nullptr;
+    FB_CHECK(nrows == 0 || a.vals[c] != nullptr, "column %d needs a value column", c);
+  }
+  if (nrows == 0) return 0;
+  FB_CHECK(nseg >= 1 && d_offsets != nullptr, "%lld rows need at least one segment", (long long)nrows);
+  FB_CHECK(num_tiles(nrows) < (1LL << 31), "too many rows");
+  FB_CHECK(scratch != nullptr && scratch_bytes >= fb_segmented_shape_moments_scratch_bytes(nrows, ncols),
+           "scratch too small: %zu < %zu", scratch_bytes, fb_segmented_shape_moments_scratch_bytes(nrows, ncols));
+  FbDeviceGuard guard(dev);
+  FB_CHECK(guard.ok, "cannot select device %d", dev);
+  cudaStream_t st = (cudaStream_t)stream;
+  const int64_t ntiles = num_tiles(nrows);
+  const int64_t nt = ncols * ntiles;
+  ShapeTiles ts;
+  ts.c = (int64_t*)scratch;
+  ts.mean = (double*)(ts.c + nt);
+  ts.m2 = ts.mean + nt;
+  ts.m3 = ts.m2 + nt;
+  ts.m4 = ts.m3 + nt;
+  ts.f = (int32_t*)(ts.m4 + nt);
+  fb_segshape_tile_kernel<false><<<(unsigned)ntiles, kThreads, 0, st>>>(nrows, nseg, d_offsets, a, ntiles, ts);
+  FB_CUDA(cudaGetLastError());
+  fb_segshape_carry_kernel<<<ncols, kShapeCarryThreads, 0, st>>>(ntiles, ts);
+  FB_CUDA(cudaGetLastError());
+  fb_segshape_tile_kernel<true><<<(unsigned)ntiles, kThreads, 0, st>>>(nrows, nseg, d_offsets, a, ntiles, ts);
   FB_CUDA(cudaGetLastError());
   return 0;
 }

@@ -266,14 +266,19 @@ def _dev_key(v: torch.Tensor, m: Optional[torch.Tensor]) -> Tuple[int, int]:
     return v.data_ptr(), 0 if m is None else m.data_ptr()
 
 
-def _deviations(devs: Dict[Tuple[int, int], Any], add: Any, v: torch.Tensor, m: Optional[torch.Tensor]) -> Any:
-    """The (SUM, COUNT, DEV, DEV2) accumulators of the f64 column ``v`` with validity ``m``, added once per call.  K6
-    resolves a DEV / DEV2 to its column by (value pointer, validity pointer), so a second set for the same pointers
-    would be ambiguous (DESIGN §7i, §7k)."""
+def _deviations(devs: Dict[Tuple[int, int], Any], add: Any, v: torch.Tensor, m: Optional[torch.Tensor],
+                shape: bool = False) -> Any:
+    """The (SUM, COUNT, DEV, DEV2) accumulators of the f64 column ``v`` with validity ``m``, added once per call, and
+    with ``shape`` also its (DEV3, DEV4, MIN, MAX) for skewness and kurtosis, added once when a shape statistic first
+    asks.  K6 resolves a DEV .. DEV4 to its column by (value pointer, validity pointer), so a second set for the same
+    pointers would be ambiguous (DESIGN §7i, §7k, §7m)."""
     k = _dev_key(v, m)
     if k not in devs:
         devs[k] = (add(v, m, K.AGG_SUM_F64), add(None, m, K.AGG_COUNT), add(v, m, K.AGG_DEV_F64),
                    add(v, m, K.AGG_DEV2_F64))
+    if shape and len(devs[k]) == 4:
+        devs[k] += (add(v, m, K.AGG_DEV3_F64), add(v, m, K.AGG_DEV4_F64), add(v, m, K.AGG_MIN_F64),
+                    add(v, m, K.AGG_MAX_F64))
     return devs[k]
 
 
@@ -691,8 +696,9 @@ class B200ExecutionEngine(EngineLifecycle):
                                   add(None, m, K.AGG_COUNT) if m is not None else None))
             rows_slot = add(None, None, K.AGG_COUNT)
         rowno: Any = None
-        # (value pointer, validity pointer) -> its (SUM, COUNT, DEV, DEV2) accumulators, shared by every variance and
-        # pair of the call: K6 ties a DEV / DEV2 to its column by these two pointers, so each column needs one set
+        # (value pointer, validity pointer) -> its (SUM, COUNT, DEV, DEV2[, DEV3, DEV4, MIN, MAX]) accumulators, shared
+        # by every variance, shape statistic and pair of the call: K6 ties a DEV .. DEV4 to its column by these two
+        # pointers, so each column needs one set
         devs: Dict[Tuple[int, int], Any] = {}
         wide: Dict[str, torch.Tensor] = {}  # argument column -> its f64 values, so that pointers repeat
         pairs: Dict[Any, Any] = {}  # (x, y) argument columns -> the 12 accumulators of the pair
@@ -736,9 +742,14 @@ class B200ExecutionEngine(EngineLifecycle):
                 s = add(v, rm, op)
                 finish.append(lambda g, s=s, cnt=cnt, d=d, tp=tp: A.finish_string(g[s], g[cnt], d, tp))
                 continue
+            if family == "shape":
+                # the column's variance set and DEV3, DEV4, MIN, MAX, shared by all its shape statistics (DESIGN §7m)
+                s = _deviations(devs, add, A.f64_values(t, arg, wide), m, shape=True)
+                finish.append(lambda g, fn=fn, s=s: (*A.shape_of(fn, *A.shape_moments(g, s)), pa.float64(), None))
+                continue
             if family == "variance":
                 # one SUM, COUNT, DEV, DEV2 per column, shared by all its variances (DESIGN §7i)
-                _, cnt, d1, d2 = _deviations(devs, add, A.f64_values(t, arg, wide), m)
+                _, cnt, d1, d2 = _deviations(devs, add, A.f64_values(t, arg, wide), m)[:4]
                 finish.append(lambda g, fn=fn, cnt=cnt, d1=d1, d2=d2: (
                     *A.variance_of(fn, A.m2_of(g[d1].view(torch.float64), g[d2].view(torch.float64),
                                                g[cnt].to(torch.float64)), g[cnt]), pa.float64(), None))
@@ -750,7 +761,8 @@ class B200ExecutionEngine(EngineLifecycle):
             s = add(v, m, op)
             finish.append(lambda g, fn=fn, s=s, nn=nn, tp=tp, f64=v.dtype == torch.float64: (*A.finish_basic(
                 fn, g[s].view(torch.float64) if f64 else g[s], None if nn is None else g[nn], tp), None))
-        if len(ops) > K.MAX_AGGS and pairs:  # more than one kernel call holds: the sorted route has no such limit
+        if len(ops) > K.MAX_AGGS and (pairs or any(len(s) > 4 for s in devs.values())):
+            # more than one kernel call holds: the sorted route has no such limit
             return self._aggregate_sorted(df, partition_spec, agg_cols)
         assert_or_throw(len(ops) <= K.MAX_AGGS, NotImplementedError(
             f"{len(ops)} accumulators needed, one kernel call handles {K.MAX_AGGS}"))
@@ -813,7 +825,7 @@ class B200ExecutionEngine(EngineLifecycle):
         kx, ky = _dev_key(x, p), _dev_key(y, p)
         sy: Any = None
         if kx in devs:
-            sx, cnt, dx, d2x = devs[kx]
+            sx, cnt, dx, d2x = devs[kx][:4]
         else:  # SUM x, SUM y and COUNT first, so that pass B reads the three from one sector of the slot
             sx = add(x, p, K.AGG_SUM_F64)
             if ky not in devs and ky != kx:
@@ -824,7 +836,7 @@ class B200ExecutionEngine(EngineLifecycle):
         codev = add(x, p, K.AGG_CODEV_F64)
         dy = add(y, p, K.AGG_DEV_F64)  # the DEV of y right after the CODEV: the tie K6 reads
         if ky in devs:  # (x, x), or a variance of y came first: a second DEV of y gets its own sums
-            sy, _, _, d2y = devs[ky]
+            sy, _, _, d2y = devs[ky][:4]
         else:
             d2y = add(y, p, K.AGG_DEV2_F64)
             if sy is None:

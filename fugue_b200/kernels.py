@@ -298,6 +298,8 @@ AGG_DEV_F64, AGG_DEV2_F64 = 7, 8
 # AGG_CODEV_F64 names x and the pair validity; the AGG_DEV_F64 right after it names y with the same validity, and
 # the call needs AGG_SUM_F64 of x and of y and an AGG_COUNT, all of that same validity tensor
 AGG_CODEV_F64 = 9
+# group-by only: sums of d^3 and d^4, tied like AGG_DEV2_F64 to the AGG_SUM_F64 and AGG_COUNT of their column
+AGG_DEV3_F64, AGG_DEV4_F64 = 10, 11
 MAX_AGGS = 16
 
 
@@ -469,6 +471,39 @@ def segmented_moments(offsets: torch.Tensor, nrows: int,
             _lib.ptr_array([c.data_ptr() for c in cnts]), _lib.ptr_array([q.data_ptr() for q in m2s]),
             scratch.data_ptr(), scratch.numel()))
         res.extend(zip(cnts, m2s))
+    return res
+
+
+def segmented_shape_moments(offsets: torch.Tensor, nrows: int,
+                            columns: Sequence[Tuple[torch.Tensor, Optional[torch.Tensor]]]
+                            ) -> List[Tuple[torch.Tensor, torch.Tensor, torch.Tensor, torch.Tensor]]:
+    """K9: running shape moments restarting at every segment ``[offsets[s], offsets[s + 1])``.  ``columns`` = one
+    ``(float64 values, validity or None)`` per column.  Returns per column ``(running count of the valid rows (int64),
+    M2, M3, M4)``, Mk = sum of (x - mean)^k over them (float64, 0 where the count is 0); up to ``SCAN_MAX_COLS``
+    columns share one launch sequence."""
+    lib = _lib.load()
+    assert offsets.dtype == torch.int64 and offsets.is_cuda and offsets.is_contiguous()
+    dev = offsets.device
+    nseg = int(offsets.shape[0]) - 1
+    res: List[Tuple[torch.Tensor, torch.Tensor, torch.Tensor, torch.Tensor]] = []
+    for b in range(0, len(columns), SCAN_MAX_COLS):
+        batch = columns[b:b + SCAN_MAX_COLS]
+        outs = []
+        for v, m in batch:
+            assert v.dtype == torch.float64 and v.device == dev and v.is_contiguous() and v.shape[0] == nrows
+            if m is not None:
+                assert m.dtype == torch.uint8 and m.device == dev and m.is_contiguous() and m.shape[0] == nrows
+            outs.append((torch.empty(nrows, dtype=torch.int64, device=dev),)
+                        + tuple(torch.empty(nrows, dtype=torch.float64, device=dev) for _ in range(3)))
+        nb = int(lib.fb_segmented_shape_moments_scratch_bytes(nrows, len(batch)))
+        scratch = torch.empty(max(nb, 8), dtype=torch.uint8, device=dev)
+        _lib.check(lib.fb_segmented_shape_moments(
+            dev.index, _stream_ptr(dev), nrows, nseg, offsets.data_ptr(), len(batch),
+            _lib.ptr_array([v.data_ptr() for v, _ in batch]),
+            _lib.ptr_array([0 if m is None else m.data_ptr() for _, m in batch]),
+            *[_lib.ptr_array([o[i].data_ptr() for o in outs]) for i in range(4)],
+            scratch.data_ptr(), scratch.numel()))
+        res.extend(outs)
     return res
 
 

@@ -11,7 +11,8 @@ fugue/workflow/workflow.py:2109-2166) and ``ExecutionEngine.aggregate`` reaches 
              [ORDER BY c [ASC|DESC], ...] [LIMIT n]
         -> parsed into column expressions (fugue_b200.column) and run by ``engine.select``: row-wise
            parts in the device expression evaluator, SUM/COUNT/MIN/MAX/AVG and VAR_SAMP / VARIANCE / VAR_POP /
-           STDDEV_SAMP / STDDEV / STDDEV_POP and CORR / COVAR_POP / COVAR_SAMP / REGR_* in the hash group-by kernel
+           STDDEV_SAMP / STDDEV / STDDEV_POP, SKEWNESS / SKEW / SKEWNESS_POP / KURTOSIS / KURT / KURTOSIS_POP and
+           CORR / COVAR_POP / COVAR_SAMP / REGR_* in the hash group-by kernel
     SELECT * FROM a [INNER|LEFT|RIGHT|FULL [OUTER]|LEFT SEMI|LEFT ANTI|CROSS] JOIN b
              [USING (k, ...) | ON a.k = b.k [AND ...]]                        -> hash join kernels
 
@@ -314,7 +315,9 @@ _TOKEN = re.compile(r"""\s*(?:
 _AGG_FUNCS = {"SUM": functions.sum, "COUNT": functions.count, "MIN": functions.min, "MAX": functions.max,
               "AVG": functions.avg, "MEAN": functions.avg, "FIRST": functions.first, "LAST": functions.last,
               "VAR_SAMP": functions.var_samp, "VARIANCE": functions.variance, "VAR_POP": functions.var_pop,
-              "STDDEV_SAMP": functions.stddev_samp, "STDDEV": functions.stddev, "STDDEV_POP": functions.stddev_pop}
+              "STDDEV_SAMP": functions.stddev_samp, "STDDEV": functions.stddev, "STDDEV_POP": functions.stddev_pop,
+              "SKEWNESS": functions.skewness, "SKEW": functions.skew, "SKEWNESS_POP": functions.skewness_pop,
+              "KURTOSIS": functions.kurtosis, "KURT": functions.kurt, "KURTOSIS_POP": functions.kurtosis_pop}
 # CORR(a, b), COVAR_POP / COVAR_SAMP(a, b), REGR_*(y, x): two arguments, in SQL's order
 _BIVARIATE_FUNCS = {name: getattr(functions, name.lower()) for name in BIVARIATES}
 _CLAUSES = ("WHERE", "GROUP", "HAVING", "ORDER", "LIMIT")

@@ -235,6 +235,12 @@ int fb_pull_runs_tma(int dev, void* stream, int nruns, const void* const* src, v
  * row where p is set, the call adds dx * dy into CODEV, with dx = x - SUM(x) / COUNT and dy = y - SUM(y) / COUNT
  * of the row's group.  With m = COUNT, DEVx and DEVy the deviation sums of x and y over the same rows,
  * Sxy = sum over the group of (x - mean x)(y - mean y) = CODEV - DEVx * DEVy / m.
+ *
+ * Higher deviations (skewness and kurtosis, DESIGN §7m): FB_AGG_DEV3_F64 and FB_AGG_DEV4_F64 are tied like
+ * FB_AGG_DEV2_F64 to an FB_AGG_SUM_F64 of the same value and validity pointers and an FB_AGG_COUNT of the same
+ * validity pointer (rejected otherwise), and receive d^3 and d^4 with the same d.  With delta = DEV / m the central
+ * sums follow exactly: M2 = DEV2 - m delta^2, M3 = DEV3 - 3 delta DEV2 + 2 m delta^3,
+ * M4 = DEV4 - 4 delta DEV3 + 6 delta^2 DEV2 - 3 m delta^4.  A NaN or +-inf value makes them NaN.
  * --------------------------------------------------------------------------- */
 #define FB_MAX_AGGS 16
 enum {
@@ -247,7 +253,9 @@ enum {
   FB_AGG_MAX_F64 = 6,
   FB_AGG_DEV_F64 = 7,
   FB_AGG_DEV2_F64 = 8,
-  FB_AGG_CODEV_F64 = 9
+  FB_AGG_CODEV_F64 = 9,
+  FB_AGG_DEV3_F64 = 10,
+  FB_AGG_DEV4_F64 = 11
 };
 size_t fb_groupby_table_bytes(int64_t capacity, int naggs);
 int fb_groupby_u64(int dev, void* stream, int64_t nrows, const void* keys, const uint8_t* key_valid,
@@ -313,6 +321,21 @@ int fb_segmented_comoments(int dev, void* stream, int64_t nrows, int64_t nseg, c
                            const uint8_t* const* y_valid, int64_t* const* out_count, void* const* out_mean_x,
                            void* const* out_mean_y, void* const* out_sxx, void* const* out_syy,
                            void* const* out_sxy, void* scratch, size_t scratch_bytes);
+
+/* K9  segmented shape moments: over the same segments, per column c and row i, the valid rows of i's segment up to
+ * and including i (f64 values vals[c], mask valid[c] or NULL):
+ *   out_count[c][i]                 their number m (int64)
+ *   out_m2[c][i], out_m3, out_m4    Mk = sum of (x - mean)^k over them (f64), 0 where m = 0; NaN once a NaN or +-inf
+ *                                   is among them
+ * The state (n, mean, M2, M3, M4) is combined with Pebay's pairwise update; a value enters as (1, x, z, z, z) with
+ * z = x - x.  Same launch sequence and fixed combination order as fb_segmented_scan: bit-identical runs.  vals,
+ * valid and the outputs are HOST arrays of ncols <= FB_SCAN_MAX_COLS entries (an output may be NULL: not written);
+ * scratch: fb_segmented_shape_moments_scratch_bytes. */
+size_t fb_segmented_shape_moments_scratch_bytes(int64_t nrows, int ncols);
+int fb_segmented_shape_moments(int dev, void* stream, int64_t nrows, int64_t nseg, const int64_t* d_offsets, int ncols,
+                               const void* const* vals, const uint8_t* const* valid, int64_t* const* out_count,
+                               void* const* out_m2, void* const* out_m3, void* const* out_m4, void* scratch,
+                               size_t scratch_bytes);
 
 /* K9  moving-window aggregate: ROWS BETWEEN start AND end over the same segments.  For row i of segment
  * [a, b) the frame is rows [max(a, i + start), min(b - 1, i + end)] (may be empty); a negative bound is

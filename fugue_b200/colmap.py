@@ -236,6 +236,7 @@ def _with_windows(t: B200Table, cols: List[ColumnExpr]) -> B200Table:
     moments: Dict[str, int] = {}  # argument column of a variance -> its column of the moments scan
     shapes: Dict[str, int] = {}  # argument column of a skewness or kurtosis -> its column of the shape-moments scan
     comoments: Dict[Tuple[str, str], int] = {}  # (x, y) argument columns of a pair -> its pair of the co-moments scan
+    pair_sums: Dict[Tuple[str, str], Tuple[Any, Any]] = {}  # (x, y) -> the running SUM scans of x and y over the pair
     finish: List[Any] = []     # per node: (fingerprint, fn(scan results) -> (column, validity, type, dictionary))
 
     def scan(op: int, v: Any, m: Any, frame: Any = None) -> Tuple[Any, int]:
@@ -278,9 +279,20 @@ def _with_windows(t: B200Table, cols: List[ColumnExpr]) -> B200Table:
             xy = tuple(arg_name[a.fingerprint()] for a in bivariate_xy(bare))
             for nm in xy:
                 A.check_argument(fn, nm, base.schema.types[base.schema.index_of_key(nm)], nm in base.dictionaries)
-            j = comoments.setdefault(xy, len(comoments))
-            finish.append((uid, lambda r, j=j, e=at_end, fn=fn: (
-                *bivariate_of(fn, *(e(x) for x in r[("comoments", j)])), result_type(fn, None), None)))
+            if xy not in comoments:
+                comoments[xy] = len(comoments)
+                # the means follow AVG, as on the hash route: each side's float64 SUM over the pair rows, over their
+                # count (the scan's running means stay finite where that sum overflows)
+                vx, vy = (base.valid[base.schema.index_of_key(nm)] for nm in xy)
+                p = vx if vy is None else (vy if vx is None else (vx & vy).contiguous())
+                pair_sums[xy] = tuple(scan(K.AGG_SUM_F64, A.f64_values(base, nm), p) for nm in xy)
+
+            def pair(r: Any, j: int = comoments[xy], sums: Any = pair_sums[xy], e: Any = at_end, fn: str = fn) -> Any:
+                m, _, _, sxx, syy, sxy = (e(x) for x in r[("comoments", j)])
+                mx, my = (e(r[s][0]) / m.to(torch.float64) for s in sums)
+                return (*bivariate_of(fn, m, mx, my, sxx, syy, sxy), result_type(fn, None), None)
+
+            finish.append((uid, pair))
             continue
         if fn == "COUNT" or bare.arg.kind == Kind.WILDCARD:  # COUNT(x), COUNT(*)
             m = None if bare.arg.kind == Kind.WILDCARD else base.valid[base.schema.index_of_key(

@@ -52,12 +52,43 @@ def expr_type(tp: pa.DataType) -> int:
     return special.get(tp, _EXPR_TYPE_OF_STORAGE[_storage_dtype(tp)])
 
 
+# (mantissa bits, exponent mask) of float16 and float32: where a NaN's sign and payload sit
+_NAN_LAYOUT = {torch.float16: (10, 0x7C00), torch.float32: (23, 0x7F800000)}
+
+
+def _nan_bits_to_f64(x: torch.Tensor, raw: torch.Tensor, small: torch.dtype) -> torch.Tensor:
+    """``x`` (float64 from the device conversion of ``raw``, the float16 / float32 bits as int64) with every NaN
+    replaced by the float64 NaN of the same sign and payload: the device conversion makes them all one NaN."""
+    mbits, emask = _NAN_LAYOUT[small]
+    width = 16 if small == torch.float16 else 32
+    raw = raw & ((1 << width) - 1)
+    nan = ((raw & emask) == emask) & ((raw & ((1 << mbits) - 1)) != 0)
+    bits = (0x7FF << 52) | ((raw & ((1 << mbits) - 1)) << (52 - mbits))
+    bits = torch.where((raw >> (width - 1)) == 1, bits + (-(1 << 63)), bits)  # the sign bit
+    return torch.where(nan, bits, x.view(torch.int64)).view(torch.float64)
+
+
+def _nan_bits_from_f64(v: torch.Tensor, small: torch.dtype) -> torch.Tensor:
+    """``v`` (float64) converted to ``small`` with every NaN keeping its sign and the top bits of its payload (a
+    payload that loses all its bits keeps the lowest one, so that it stays a NaN), as the storage integers."""
+    mbits, emask = _NAN_LAYOUT[small]
+    width = 16 if small == torch.float16 else 32
+    store = torch.int16 if small == torch.float16 else torch.int32
+    b = v.view(torch.int64)
+    mant = (b >> (52 - mbits)) & ((1 << mbits) - 1)
+    bits = (((b >> 63) & 1) << (width - 1)) | emask | torch.where(mant == 0, torch.ones_like(mant), mant)
+    bits = torch.where(bits >= (1 << (width - 1)), bits - (1 << width), bits)  # as the signed storage integer
+    return torch.where(torch.isnan(v), bits.to(store), v.to(small).view(store))
+
+
 def widen(c: torch.Tensor, tp: pa.DataType) -> torch.Tensor:
     """A stored column as its canonical 64-bit value: float64 for float types, int64 for the rest.
-    uint16 / uint32 zero-extend, float16 is decoded from its int16 storage (exactly); uint64 values
-    >= 2**63 stay int64 bit patterns.  Returns ``c`` itself when it already is that."""
+    uint16 / uint32 zero-extend, float16 is decoded from its int16 storage (exactly, a NaN's sign and payload
+    too); uint64 values >= 2**63 stay int64 bit patterns.  Returns ``c`` itself when it already is that."""
     if tp == pa.float16():
-        return c.view(torch.float16).to(torch.float64)
+        return _nan_bits_to_f64(c.view(torch.float16).to(torch.float64), c.to(torch.int64), torch.float16)
+    if tp == pa.float32():
+        return _nan_bits_to_f64(c.to(torch.float64), c.view(torch.int32).to(torch.int64), torch.float32)
     if pa.types.is_floating(tp):
         return c.to(torch.float64)
     if tp == pa.uint16():
@@ -73,7 +104,9 @@ def narrow(v: torch.Tensor, tp: pa.DataType) -> torch.Tensor:
     if v.dtype == sd:
         return v
     if tp == pa.float16():
-        return v.to(torch.float16).view(torch.int16)
+        return _nan_bits_from_f64(v.to(torch.float64), torch.float16)
+    if tp == pa.float32():
+        return _nan_bits_from_f64(v.to(torch.float64), torch.float32).view(torch.float32)
     return v.to(sd)
 
 

@@ -131,6 +131,8 @@ SIGNATURES = {
     "fb_string_first_equal": (C.c_int, [C.c_int, _vp, C.c_int64, _vp, _vp, _vp, _vp, _vp, _vp]),
     "fb_string_parse": (C.c_int, [C.c_int, _vp, C.c_int64, _vp, _vp, _vp, C.c_int, _vp, _vp, _vp, _vp]),
     "fb_debug_string_parse_host": (C.c_int, [C.c_int64, _vp, _vp, _vp, C.c_int, _vp, _vp, _vp]),
+    "fb_value_format": (C.c_int, [C.c_int, _vp, C.c_int64, _vp, _vp, C.c_int, _vp, _vp, _vp]),
+    "fb_debug_value_format_host": (C.c_int, [C.c_int64, _vp, _vp, C.c_int, _vp, _vp, _vp]),
 }
 
 

@@ -468,8 +468,9 @@ class B200DataFrame(DataFrame):
 
     def alter_columns(self, columns: Any) -> DataFrame:
         """Casts run on the device (one fb_eval_expr program), casts from strings to numbers, bools, dates and
-        timestamps included (K13); casts to strings and to the types the device does not parse to go through the
-        host."""
+        timestamps included (K13), and casts of those to strings (K14: the text the host frames write, formatted once
+        per distinct value).  Casts to the types the device does not parse to, and to strings from types it does not
+        format (a timestamp in a time zone other than UTC, decimal ...), go through the host."""
         new = self._altered_schema(columns)
         if new is None:
             return self

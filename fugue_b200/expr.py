@@ -9,7 +9,9 @@ Typing rules (the reference leaves them to the SQL engine; these are the pandas/
 ``+ - *`` on integers -> int64, with any float -> float64; ``/`` -> float64 (true division);
 comparisons / ``& | ~`` / ``IS NULL`` -> bool with SQL three-valued logic; an explicit ``cast`` wins.
 String columns are dictionary encoded: they can be passed through, tested for NULL and compared
-(``==`` / ``!=``) with a string literal; ``cast(str)`` of a numeric result builds a dictionary.
+(``==`` / ``!=``) with a string literal.  ``CAST(x AS STRING)`` of a number, bool, date or timestamp formats every
+distinct value once (``strings.format_values``, K14) into a dictionary column; inside an expression it becomes a
+temporary column of a wider table first (``_string_casts``), which every string consumer takes as a string column.
 ``LIKE`` and ``LENGTH`` of a string column are computed once per dictionary entry (``strings.py``) and
 read per row through the entry's code (``FB_X_LOOKUP``), inside the same program.
 ``CASE`` runs without branching (every branch on every row, ``FB_X_SEL`` picks); its class, and that of
@@ -39,7 +41,7 @@ import torch
 from . import kernels as K
 from . import strings as ST
 from .column import (FLOAT_FUNCTIONS, ROUND_MAX_DIGITS, TEMPORAL_LITERALS, TIME_FIELDS, TIME_PARTS, ColumnExpr, Kind,
-                     case_string_results, is_string_build, lit as _lit)
+                     case_string_results, col as _col, is_string_build, lit as _lit)
 from .schema import Schema
 from .table import B200Table, _storage_dtype, expr_type
 
@@ -979,25 +981,56 @@ def _default_type(cls: str, e: ColumnExpr, schema: Schema) -> pa.DataType:
     return {"i": pa.int64(), "f": pa.float64(), "b": pa.bool_()}.get(cls, pa.int64())
 
 
-def _format_values(vals: torch.Tensor, tp_from: str) -> List[str]:
-    host = vals.cpu().tolist()
-    if tp_from == "b":
-        return ["true" if v else "false" for v in host]
-    return [str(v) for v in host]
+def _format_source(e: ColumnExpr, cls: str, schema: Schema) -> pa.DataType:
+    """The arrow type whose text ``CAST(x AS STRING)`` writes: ``x``'s inferred type, or the storage type of the
+    class K8 computed it in."""
+    tp = e.cast(None).infer_type(schema)
+    if tp is None or _cls_of(tp) != cls:
+        return {"i": pa.int64(), "f": pa.float64(), "b": pa.bool_()}[cls]
+    return tp
 
 
-def _to_string_column(col: torch.Tensor, valid: Optional[torch.Tensor], cls: str
-                      ) -> Tuple[torch.Tensor, pa.Array]:
-    """``CAST(x AS str)``: dictionary = the distinct values, formatted on the host."""
-    if col.numel() == 0:
-        return torch.empty(0, dtype=torch.int32, device=col.device), pa.array([], type=pa.string())
-    src = col if valid is None else torch.where(valid.bool(), col, torch.zeros_like(col))
-    uniq, inv = torch.unique(src, return_inverse=True)
-    return inv.to(torch.int32).contiguous(), pa.array(_format_values(uniq, cls), type=pa.string())
+_STR_CAST = "__str_cast_"
+
+
+def _string_casts(t: B200Table, exprs: Sequence[ColumnExpr], top: bool) -> Tuple[B200Table, List[ColumnExpr]]:
+    """Every ``CAST(x AS STRING)`` of a value ``x`` that is not a whole output column (``top``: the expressions
+    themselves are) evaluated into a dictionary column of a wider table, and the trees rewritten to read it: every
+    string consumer (==, LIKE, LENGTH, the string-building functions, casts back) then takes it as a string column.
+    Equal casts share one column."""
+    prog = _Program(t)
+    found: Dict[str, Tuple[str, ColumnExpr]] = {}
+
+    def visit(e: Any, is_top: bool) -> Any:
+        if not isinstance(e, ColumnExpr):
+            return e
+        if not is_top and e.as_type is not None and _is_str(e.as_type) and                 e.kind in (Kind.NAMED, Kind.UNARY, Kind.BINARY, Kind.CALL) and                 prog._static_cls(e.cast(None)) not in ("s", "n"):
+            bare = e.alias("")
+            fp = bare.fingerprint()
+            if fp not in found:
+                found[fp] = (f"{_STR_CAST}{len(found)}", bare)
+            out = _col(found[fp][0])
+            return out.alias(e.as_name) if e.as_name != "" else out
+        if e.has_args:
+            return ColumnExpr(e.kind, e.head, [visit(a, False) for a in e.args],
+                              {k: visit(v, False) for k, v in e.kwargs.items()}, e.is_distinct, e.as_name, e.as_type)
+        return e
+
+    new = [visit(e, top) for e in exprs]
+    if not found:
+        return t, list(exprs)
+    if any(n.startswith(_STR_CAST) for n in t.schema.names):
+        raise NotImplementedError(f"a column name starting with {_STR_CAST} next to a cast to string")
+    extra = project(t, [b.alias(name) for name, b in found.values()])
+    fields = [pa.field(n, tp) for n, tp in zip(t.schema.names + extra.schema.names, t.schema.types + extra.schema.types)]
+    wide = B200Table(Schema(fields), t.columns + extra.columns, t.valid + extra.valid,
+                     {**t.dictionaries, **extra.dictionaries}, t.offsets, t.partition_keys)
+    return wide, new
 
 
 def project(t: B200Table, exprs: Sequence[ColumnExpr]) -> B200Table:
     """Evaluate a SELECT list (no aggregations, wildcards already expanded, every column named)."""
+    t, exprs = _string_casts(t, exprs, True)
     n, dev = t.num_rows, t.device
     names = [e.output_name for e in exprs]
     out_cols: List[Any] = [None] * len(exprs)
@@ -1006,6 +1039,7 @@ def project(t: B200Table, exprs: Sequence[ColumnExpr]) -> B200Table:
     dicts: Dict[str, pa.Array] = {}
     str_case: Dict[int, pa.Array] = {}  # output -> dictionary of a CASE with string-literal results
     str_built: Dict[int, pa.Array] = {}  # output -> dictionary of a string-building expression
+    formatted: Dict[int, pa.DataType] = {}  # output -> the type a cast to string formats (K14)
     pending: List[Tuple[int, ColumnExpr]] = []
     for i, e in enumerate(exprs):
         if e.kind == Kind.NAMED:
@@ -1073,6 +1107,9 @@ def project(t: B200Table, exprs: Sequence[ColumnExpr]) -> B200Table:
                     store_tp = {"i": pa.int64(), "f": pa.float64(), "b": pa.bool_()}[cls]
                     if not _is_str(tp):
                         tp = store_tp  # an inferred type of another class than the computed value
+                    else:
+                        formatted[i] = _format_source(e, cls, t.schema)
+                        ST.format_kind(formatted[i])  # NotImplementedError before anything runs
                 else:
                     store_tp = tp
                 prog.output(_storage_dtype(store_tp), nullable, expr_type(store_tp))
@@ -1090,8 +1127,8 @@ def project(t: B200Table, exprs: Sequence[ColumnExpr]) -> B200Table:
                 dicts[names[i]] = str_case[i]
             elif i in str_built:
                 dicts[names[i]] = str_built[i]
-            elif _is_str(out_types[i]):
-                c, dicts[names[i]] = _to_string_column(c, v, cls)
+            elif i in formatted:
+                c, v, dicts[names[i]] = ST.format_values(c, v, formatted[i], dev)
             out_cols[i], out_valid[i] = c, v
     schema = Schema([pa.field(nm, tp) for nm, tp in zip(names, out_types)])
     return B200Table(schema, out_cols, out_valid, dicts)
@@ -1110,6 +1147,7 @@ def _coded_case(e: ColumnExpr, strs: List[str]) -> ColumnExpr:
 
 def predicate_mask(t: B200Table, condition: ColumnExpr) -> torch.Tensor:
     """uint8 mask: 1 where ``condition`` is TRUE (NULL counts as FALSE, like SQL WHERE)."""
+    t, (condition,) = _string_casts(t, [condition], False)
     prog = _Program(t)
     try:
         cls, _ = prog.compile(condition.alias("") if condition.as_name else condition)

@@ -1137,3 +1137,48 @@ def string_parse_host(offsets: np.ndarray, data: np.ndarray, valid: Optional[np.
                                               0 if valid is None else valid.ctypes.data, target, out.ctypes.data,
                                               out_valid.ctypes.data, status.ctypes.data))
     return out[:n], out_valid[:n], status[:n]
+
+
+# ---- K14: casts to string, one text per value ----------------------------------------------------
+FMT_I64, FMT_U64, FMT_BOOL, FMT_F64, FMT_DATE32, FMT_DATE64 = range(6)
+FMT_TS, FMT_TS_FRAC = 8, 16  # FMT_TS + TU_S .. TU_NS (+ FMT_TS_FRAC: the unit's fraction digits on every value)
+
+
+def value_format(values: torch.Tensor, valid: Optional[torch.Tensor], kind: int) -> Tuple[torch.Tensor, torch.Tensor]:
+    """The text of every value (one 8-byte word each: an int64 / uint64 / float64 bit pattern / date or timestamp
+    count, ``kind`` a ``FMT_*`` code) on the device: (offsets int64, n + 1 entries; UTF-8 bytes uint8, at least one
+    byte).  A value whose ``valid`` byte is 0 gets no bytes."""
+    from .strings import _scan
+
+    lib = _lib.load()
+    dev = values.device
+    n = int(values.shape[0])
+    values = values.contiguous()
+    vp = 0 if valid is None else valid.contiguous().data_ptr()
+    lengths = torch.empty(n, dtype=torch.int64, device=dev)
+    _lib.check(lib.fb_value_format(dev.index, _stream_ptr(dev), n, values.data_ptr(), vp, kind, lengths.data_ptr(),
+                                   0, 0))
+    offsets, total = _scan(lengths)
+    data = torch.empty(max(total, 1), dtype=torch.uint8, device=dev)
+    _lib.check(lib.fb_value_format(dev.index, _stream_ptr(dev), n, values.data_ptr(), vp, kind, 0,
+                                   offsets.data_ptr(), data.data_ptr()))
+    return offsets, data
+
+
+def value_format_host(values: np.ndarray, valid: Optional[np.ndarray], kind: int) -> Tuple[np.ndarray, np.ndarray]:
+    """``value_format`` on the CPU over host arrays (8-byte ``values``, uint8 ``valid``), by the same format
+    routines: (offsets int64, UTF-8 bytes uint8)."""
+    lib = _lib.load()
+    n = int(values.shape[0])
+    values = np.ascontiguousarray(values).view(np.uint64)
+    if valid is not None:
+        valid = np.ascontiguousarray(valid, dtype=np.uint8)
+    vp = 0 if valid is None else valid.ctypes.data
+    lengths = np.zeros(max(n, 1), dtype=np.int64)
+    _lib.check(lib.fb_debug_value_format_host(n, values.ctypes.data, vp, kind, lengths.ctypes.data, 0, 0))
+    offsets = np.zeros(n + 1, dtype=np.int64)
+    np.cumsum(lengths[:n], out=offsets[1:])
+    data = np.zeros(max(int(offsets[-1]), 1), dtype=np.uint8)
+    _lib.check(lib.fb_debug_value_format_host(n, values.ctypes.data, vp, kind, 0, offsets.ctypes.data,
+                                              data.ctypes.data))
+    return offsets, data

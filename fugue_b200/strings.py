@@ -23,6 +23,9 @@ cached per (dictionary object, device, target type).  The parse is Arrow's ``cas
 few floats of more than 19 significant digits the device leaves undecided are re-parsed by pyarrow on the host
 (``parse_fallbacks`` counts them).  An entry that does not parse is an error only when a valid row of the table
 being evaluated refers to it (``check_referenced``).
+
+A cast of a number, bool, date or timestamp to a string goes the other way (K14, ``fb_format.cu``): ``format_values``
+finds the distinct values on the device, formats each once there and returns the codes into the new dictionary.
 """
 import weakref
 from typing import Any, Dict, List, Optional, Sequence, Tuple
@@ -485,3 +488,78 @@ def check_referenced(r: ParseResult, d: pa.Array, tp: pa.DataType, codes: torch.
         if src_of is not None:
             entry = int(src_of[entry].item())
     raise parse_error(d[entry].as_py(), tp)
+
+
+# ---- casts to strings (K14) ---------------------------------------------------------------------------
+formats = 0  # columns whose distinct values were formatted to a dictionary so far
+_DAY_MS = 86_400_000
+_DAY_RANGE = (-12_687_428, 11_248_737)  # the days Arrow writes as a date (years -32767 .. 32767), fb_format.cuh
+
+
+def format_kind(tp: pa.DataType) -> int:
+    """The ``fb_value_format`` kind of a cast from ``tp`` to string; NotImplementedError for a type the device does
+    not format (decimal, time, duration, nested, a timestamp in a time zone other than UTC ...)."""
+    if pa.types.is_boolean(tp):
+        return K.FMT_BOOL
+    if pa.types.is_integer(tp):
+        return K.FMT_U64 if tp == pa.uint64() else K.FMT_I64
+    if pa.types.is_floating(tp):
+        return K.FMT_F64
+    if pa.types.is_date32(tp) or pa.types.is_date64(tp):
+        return K.FMT_DATE32 if pa.types.is_date32(tp) else K.FMT_DATE64
+    if pa.types.is_timestamp(tp):
+        if tp.tz is not None and tp.tz.upper() != "UTC":
+            raise NotImplementedError(f"cast of a timestamp in time zone {tp.tz} to string (only UTC; there is no "
+                                      f"time-zone database on the device)")
+        return K.FMT_TS + _TS_UNITS[tp.unit]
+    raise NotImplementedError(f"cast of {tp} to string has no device implementation")
+
+
+def _format_keys(values: torch.Tensor, tp: pa.DataType) -> torch.Tensor:
+    """The int64 word whose text is the value's: a float64's bits with every NaN one pattern (-0.0 stays apart from
+    0.0), a bool as 0 / 1, a date64 in range truncated to its day (the day Arrow writes), the value otherwise."""
+    if values.dtype.is_floating_point:
+        v = values.to(torch.float64)
+        return torch.where(torch.isnan(v), torch.full_like(v, float("nan")), v).view(torch.int64)
+    k = values.to(torch.int64)
+    if pa.types.is_boolean(tp):
+        return (k != 0).to(torch.int64)
+    if pa.types.is_date64(tp):
+        floor_day = torch.div(k, _DAY_MS, rounding_mode="floor")
+        inside = (floor_day >= _DAY_RANGE[0]) & (floor_day <= _DAY_RANGE[1])
+        return torch.where(inside, torch.div(k, _DAY_MS, rounding_mode="trunc") * _DAY_MS, k)
+    return k
+
+
+def format_values(values: torch.Tensor, valid: Optional[torch.Tensor], tp: pa.DataType, device: torch.device
+                  ) -> Tuple[torch.Tensor, Optional[torch.Tensor], pa.Array]:
+    """``CAST(x AS STRING)`` of a column of arrow type ``tp`` (``values``: its storage, or the 64-bit value K8
+    computed for it): (int32 codes, the validity, a ``pa.string()`` dictionary of distinct entries).  The distinct
+    values are found on the device over 8-byte keys the text is a function of (``_format_keys``), formatted there
+    (K14) and copied to the host once; the dictionary's device copy is registered, so string functions of the result
+    upload nothing.  A timestamp column has the unit's fraction digits on every row iff a valid value has a fraction
+    of a second."""
+    global formats
+    kind = format_kind(tp)
+    n = int(values.shape[0])
+    if n == 0:
+        return torch.empty(0, dtype=torch.int32, device=device), valid, pa.array([], type=pa.string())
+    keys = _format_keys(values, tp)
+    if valid is not None:
+        keys = torch.where(valid.bool(), keys, torch.zeros_like(keys))
+    uniq, inv = torch.unique(keys, return_inverse=True)
+    if kind >= K.FMT_TS and (kind & 7) != K.TU_S:
+        per = {K.TU_MS: 1000, K.TU_US: 1_000_000, K.TU_NS: 1_000_000_000}[kind & 7]
+        if bool((torch.remainder(uniq, per) != 0).any().item()):  # a NULL row's key is 0: a whole second
+            kind |= K.FMT_TS_FRAC
+    formats += 1
+    offsets, data = K.value_format(uniq, None, kind)
+    total = int(offsets[-1].item())
+    if total > (1 << 31) - 1:
+        raise NotImplementedError(f"a string result of {total} bytes; a pa.string() dictionary holds 2^31 - 1")
+    k = int(uniq.shape[0])
+    host_offsets = offsets.cpu().numpy().astype(np.int32)
+    host_data = data[:total].cpu().numpy()
+    d = pa.Array.from_buffers(pa.string(), k, [None, pa.py_buffer(host_offsets), pa.py_buffer(host_data)])
+    _slot(_CACHE, d)[device] = DeviceDictionary(offsets, data, None)
+    return inv.to(torch.int32).contiguous(), valid, d

@@ -739,6 +739,38 @@ int fb_string_parse(int dev, void* stream, int64_t n, const int64_t* offsets, co
 int fb_debug_string_parse_host(int64_t n, const int64_t* offsets, const uint8_t* data, const uint8_t* valid,
                                int target, uint64_t* out, uint8_t* out_valid, uint8_t* status);
 
+/* ---------------------------------------------------------------------------
+ * K14 casts to string, evaluated once per distinct value
+ * Replaces: Python's str() of every distinct value on the host, which a CAST(x AS STRING) needed.
+ * Value i is one 8-byte word (values: DEVICE) of a kind; its text is what the host frames write for the cast
+ * (DESIGN.md section 7n):
+ *   FB_FMT_I64 / FB_FMT_U64   decimal (every integer width, widened)
+ *   FB_FMT_BOOL               true / false (any non-zero word is true)
+ *   FB_FMT_F64                float64 bits as CPython's repr(): the shortest digits that read back to the value
+ *                             (Ryu), fixed notation iff the exponent of the first digit is in [-4, 16), else
+ *                             1e+16 / 1.5e-05; nan, inf, -inf, -0.0
+ *   FB_FMT_DATE32             days since 1970-01-01 as Arrow's cast: [-]YYYY-MM-DD, years -32767 .. 32767, else
+ *                             "<value out of range: n>"
+ *   FB_FMT_DATE64             milliseconds: the range holds the floor day, the text is the day truncated toward 0
+ *                             (Arrow's cast; n: the milliseconds)
+ *   FB_FMT_TS + unit (FB_TU_S .. FB_TU_NS), + FB_FMT_TS_FRAC for the unit's 3 / 6 / 9 fraction digits (not with
+ *                             FB_TU_S): Arrow's strftime "%Y-%m-%d %H:%M:%S" of the count, floor semantics before
+ *                             1970, with its 32-bit day and 16-bit year arithmetic far from the epoch
+ * fb_value_format : measure call (out_data == NULL): out_len[i] = value i's byte length (0 where valid[i] == 0).
+ *                   Write call: its bytes go to out_data + out_offsets[i] (the host's exclusive scan of out_len);
+ *                   out_len is not read.  valid: DEVICE uint8 per value, or NULL.
+ * fb_debug_value_format_host : the same over HOST arrays, on the CPU.
+ * One thread per value, grid-stride.
+ * --------------------------------------------------------------------------- */
+enum fb_format_kind {
+  FB_FMT_I64 = 0, FB_FMT_U64 = 1, FB_FMT_BOOL = 2, FB_FMT_F64 = 3, FB_FMT_DATE32 = 4, FB_FMT_DATE64 = 5,
+  FB_FMT_TS = 8, FB_FMT_TS_FRAC = 16
+};
+int fb_value_format(int dev, void* stream, int64_t n, const uint64_t* values, const uint8_t* valid, int kind,
+                    int64_t* out_len, const int64_t* out_offsets, uint8_t* out_data);
+int fb_debug_value_format_host(int64_t n, const uint64_t* values, const uint8_t* valid, int kind, int64_t* out_len,
+                               const int64_t* out_offsets, uint8_t* out_data);
+
 #ifdef __cplusplus
 }
 #endif

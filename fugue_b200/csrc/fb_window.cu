@@ -45,7 +45,6 @@ namespace {
 constexpr int kThreads = 256;
 constexpr int kItems = 8;                  // consecutive rows per thread
 constexpr int kTile = kThreads * kItems;   // rows per CTA
-constexpr int kCarryThreads = 1024;
 
 // one 8-byte pad word per kItems words: a thread reading its kItems consecutive rows from shared memory
 // and a warp storing striped rows both hit distinct banks
@@ -61,11 +60,18 @@ struct ScanCols {
   int32_t ncols;
 };
 
-// (value, count of valid rows, "a segment starts in here") of a run of consecutive rows
+// Every scan state is kWords 8-byte words and the flag f, "a segment starts in here".  zip(a, b, g) calls g on each
+// word of a with the same word of b, in order (a and b may be one state); shuffles and the tile states in scratch
+// go through it.
+
+// (value, count of valid rows, f) of a run of consecutive rows
 struct St {
   uint64_t v;
   int64_t c;
   int32_t f;
+  static constexpr int kWords = 2;
+  template <class A, class B, class G>
+  __device__ __forceinline__ static void zip(A& a, B& b, G&& g) { g(a.v, b.v); g(a.c, b.c); }
 };
 
 // IEEE totalOrder as a signed integer order: -NaN < -inf < ... < -0.0 < +0.0 < ... < +inf < +NaN
@@ -98,28 +104,15 @@ __device__ __forceinline__ St combine(int op, const St& a, const St& b) {
   return r;
 }
 
-__device__ __forceinline__ St shfl_up(const St& s, int d) {
-  St r;
-  r.v = __shfl_up_sync(0xFFFFFFFFu, (unsigned long long)s.v, d);
-  r.c = __shfl_up_sync(0xFFFFFFFFu, (long long)s.c, d);
-  r.f = __shfl_up_sync(0xFFFFFFFFu, s.f, d);
-  return r;
-}
-
-__device__ __forceinline__ St shfl_down(const St& s, int d) {
-  St r;
-  r.v = __shfl_down_sync(0xFFFFFFFFu, (unsigned long long)s.v, d);
-  r.c = __shfl_down_sync(0xFFFFFFFFu, (long long)s.c, d);
-  r.f = __shfl_down_sync(0xFFFFFFFFu, s.f, d);
-  return r;
-}
-
 // (count, mean, M2, "a segment starts in here") of the valid values of a run of consecutive rows: the state of
 // fb_segmented_moments
 struct MSt {
   int64_t c;
   double mean, m2;
   int32_t f;
+  static constexpr int kWords = 3;
+  template <class A, class B, class G>
+  __device__ __forceinline__ static void zip(A& a, B& b, G&& g) { g(a.c, b.c); g(a.mean, b.mean); g(a.m2, b.m2); }
 };
 
 // `a` followed by `b`: Chan, Golub & LeVeque's pairwise update; a run without a valid row takes no part
@@ -133,22 +126,18 @@ __device__ __forceinline__ MSt combine(int, const MSt& a, const MSt& b) {
   return MSt{n, a.mean + delta * wb, a.m2 + b.m2 + delta * delta * (double)a.c * wb, a.f};
 }
 
-__device__ __forceinline__ MSt shfl_up(const MSt& s, int d) {
-  return MSt{(int64_t)__shfl_up_sync(0xFFFFFFFFu, (long long)s.c, d), __shfl_up_sync(0xFFFFFFFFu, s.mean, d),
-             __shfl_up_sync(0xFFFFFFFFu, s.m2, d), __shfl_up_sync(0xFFFFFFFFu, s.f, d)};
-}
-
-__device__ __forceinline__ MSt shfl_down(const MSt& s, int d) {
-  return MSt{(int64_t)__shfl_down_sync(0xFFFFFFFFu, (long long)s.c, d), __shfl_down_sync(0xFFFFFFFFu, s.mean, d),
-             __shfl_down_sync(0xFFFFFFFFu, s.m2, d), __shfl_down_sync(0xFFFFFFFFu, s.f, d)};
-}
-
 // (count, mean x, mean y, Sxx, Syy, Sxy, "a segment starts in here") of the pair rows of a run of consecutive
 // rows: the state of fb_segmented_comoments
 struct CSt {
   int64_t c;
   double mx, my, sxx, syy, sxy;
   int32_t f;
+  static constexpr int kWords = 6;
+  template <class A, class B, class G>
+  __device__ __forceinline__ static void zip(A& a, B& b, G&& g) {
+    g(a.c, b.c); g(a.mx, b.mx); g(a.my, b.my);
+    g(a.sxx, b.sxx); g(a.syy, b.syy); g(a.sxy, b.sxy);
+  }
 };
 
 // `a` followed by `b`: Chan's pairwise update with the cross term dx * dy * na * nb / n.  A non-finite mean
@@ -169,26 +158,18 @@ __device__ __forceinline__ CSt combine(int, const CSt& a, const CSt& b) {
              a.sxy + b.sxy + dx * dy * na * wb, a.f};
 }
 
-__device__ __forceinline__ CSt shfl_up(const CSt& s, int d) {
-  return CSt{(int64_t)__shfl_up_sync(0xFFFFFFFFu, (long long)s.c, d), __shfl_up_sync(0xFFFFFFFFu, s.mx, d),
-             __shfl_up_sync(0xFFFFFFFFu, s.my, d), __shfl_up_sync(0xFFFFFFFFu, s.sxx, d),
-             __shfl_up_sync(0xFFFFFFFFu, s.syy, d), __shfl_up_sync(0xFFFFFFFFu, s.sxy, d),
-             __shfl_up_sync(0xFFFFFFFFu, s.f, d)};
-}
-
-__device__ __forceinline__ CSt shfl_down(const CSt& s, int d) {
-  return CSt{(int64_t)__shfl_down_sync(0xFFFFFFFFu, (long long)s.c, d), __shfl_down_sync(0xFFFFFFFFu, s.mx, d),
-             __shfl_down_sync(0xFFFFFFFFu, s.my, d), __shfl_down_sync(0xFFFFFFFFu, s.sxx, d),
-             __shfl_down_sync(0xFFFFFFFFu, s.syy, d), __shfl_down_sync(0xFFFFFFFFu, s.sxy, d),
-             __shfl_down_sync(0xFFFFFFFFu, s.f, d)};
-}
-
 // (count, mean, M2, M3, M4, "a segment starts in here") of the valid values of a run of consecutive rows: the state
 // of fb_segmented_shape_moments
 struct SSt {
   int64_t c;
   double mean, m2, m3, m4;
   int32_t f;
+  static constexpr int kWords = 5;
+  template <class A, class B, class G>
+  __device__ __forceinline__ static void zip(A& a, B& b, G&& g) {
+    g(a.c, b.c); g(a.mean, b.mean); g(a.m2, b.m2);
+    g(a.m3, b.m3); g(a.m4, b.m4);
+  }
 };
 
 // `a` followed by `b`: Pebay's pairwise update of the third and fourth central sums beside Chan's M2, written in the
@@ -211,16 +192,20 @@ __device__ __forceinline__ SSt combine(int, const SSt& a, const SSt& b) {
              a.f};
 }
 
-__device__ __forceinline__ SSt shfl_up(const SSt& s, int d) {
-  return SSt{(int64_t)__shfl_up_sync(0xFFFFFFFFu, (long long)s.c, d), __shfl_up_sync(0xFFFFFFFFu, s.mean, d),
-             __shfl_up_sync(0xFFFFFFFFu, s.m2, d), __shfl_up_sync(0xFFFFFFFFu, s.m3, d),
-             __shfl_up_sync(0xFFFFFFFFu, s.m4, d), __shfl_up_sync(0xFFFFFFFFu, s.f, d)};
+template <class S>
+__device__ __forceinline__ S shfl_up(const S& s, int d) {
+  S r;
+  S::zip(r, s, [d](auto& w, const auto& x) { w = __shfl_up_sync(0xFFFFFFFFu, x, d); });
+  r.f = __shfl_up_sync(0xFFFFFFFFu, s.f, d);
+  return r;
 }
 
-__device__ __forceinline__ SSt shfl_down(const SSt& s, int d) {
-  return SSt{(int64_t)__shfl_down_sync(0xFFFFFFFFu, (long long)s.c, d), __shfl_down_sync(0xFFFFFFFFu, s.mean, d),
-             __shfl_down_sync(0xFFFFFFFFu, s.m2, d), __shfl_down_sync(0xFFFFFFFFu, s.m3, d),
-             __shfl_down_sync(0xFFFFFFFFu, s.m4, d), __shfl_down_sync(0xFFFFFFFFu, s.f, d)};
+template <class S>
+__device__ __forceinline__ S shfl_down(const S& s, int d) {
+  S r;
+  S::zip(r, s, [d](auto& w, const auto& x) { w = __shfl_down_sync(0xFFFFFFFFu, x, d); });
+  r.f = __shfl_down_sync(0xFFFFFFFFu, s.f, d);
+  return r;
 }
 
 // Exclusive scan of one state per thread across the CTA, and the CTA total; fixed combination order.
@@ -274,15 +259,6 @@ __device__ __forceinline__ int64_t first_multiple(int64_t x, int64_t b) {
   return q * b;
 }
 
-struct TileSmem {
-  uint64_t v[padded(kTile)];
-  int64_t c[padded(kTile)];
-  uint8_t valid[kTile];
-  uint8_t head[kTile];
-  St warp_tot[kThreads / 32];
-  int64_t seg_range[2];
-};
-
 // Marks head[p - start] for every position p in [start, end) where a run restarts (see fb_segscan_tile_kernel);
 // seg_range is two int64 of shared memory.  The caller synchronises before reading head.
 template <bool kReverse, bool kBlocks>
@@ -315,17 +291,176 @@ __device__ __forceinline__ void mark_heads(int64_t nrows, int64_t nseg, const in
   }
 }
 
-// kFinal = false: pass 1 (tile aggregates); true: pass 3 (outputs, from the carries of pass 2).
+// ---- the segmented scans: one tile kernel, one carry kernel and one launch sequence over a scan's traits ----
+// A scan's traits give its State (with combine, its 8-byte words and the flag f), its Cols, the kInputs input
+// columns a tile stages, the state of one row (entry), its kOut output words (out), the carry CTA size and how
+// pass 3 stores:
+//   - kStaged: the one output word and the count go through shared memory, then striped (coalesced) stores;
+//   - otherwise a thread stores its kItems consecutive rows straight from registers: several outputs per row do
+//     not fit the staging buffers, and the stores of a warp still cover whole lines together.
+// kFrames: the scan also runs reversed and restarts at block bounds (P and S of fb_window_frame).
+
+// the columns of an f64 statistics scan: x (and y for pairs) with their validity, the count and up to five words out
+struct StatCols {
+  const double* in[2][FB_SCAN_MAX_COLS];      // x, y
+  const uint8_t* valid[2][FB_SCAN_MAX_COLS];  // of x, of y (NULL: every row valid)
+  int64_t* out_count[FB_SCAN_MAX_COLS];
+  double* out[5][FB_SCAN_MAX_COLS];
+  int32_t ncols;
+};
+
+// a column's op (0 for the f64 families), input k, its validity and output word o
+__device__ __forceinline__ int col_op(const ScanCols& a, int col) { return a.op[col]; }
+__device__ __forceinline__ int col_op(const StatCols&, int) { return 0; }
+__device__ __forceinline__ const uint64_t* col_input(const ScanCols& a, int col, int) {
+  return (const uint64_t*)a.vals[col];
+}
+__device__ __forceinline__ const uint64_t* col_input(const StatCols& a, int col, int k) {
+  return (const uint64_t*)a.in[k][col];
+}
+__device__ __forceinline__ const uint8_t* col_valid(const ScanCols& a, int col, int) { return a.valid[col]; }
+__device__ __forceinline__ const uint8_t* col_valid(const StatCols& a, int col, int k) { return a.valid[k][col]; }
+__device__ __forceinline__ uint64_t* col_output(const ScanCols& a, int col, int) { return (uint64_t*)a.out_vals[col]; }
+__device__ __forceinline__ uint64_t* col_output(const StatCols& a, int col, int o) { return (uint64_t*)a.out[o][col]; }
+
+__device__ __forceinline__ double f64_of(uint64_t b) { return __longlong_as_double((long long)b); }
+__device__ __forceinline__ uint64_t f64_bits(double x) { return (uint64_t)__double_as_longlong(x); }
+
+// SUM / MIN / MAX / COUNT (fb_segmented_scan, and P / S of fb_window_frame)
+struct OpScan {
+  using State = St;
+  using Cols = ScanCols;
+  static constexpr int kInputs = 1, kOut = 1, kCarryThreads = 1024;
+  static constexpr bool kStaged = true, kFrames = true;
+  template <class Sm>
+  __device__ __forceinline__ static St entry(int op, const Sm& sm, int j) {
+    const int c = sm.valid[j];
+    return St{c && op != FB_AGG_COUNT ? sm.buf[0][padded(j)] : 0, c, sm.head[j]};
+  }
+  __device__ __forceinline__ static uint64_t out(const St& s, int) { return s.v; }
+};
+
+// running count and M2 (fb_segmented_moments)
+struct MomentScan {
+  using State = MSt;
+  using Cols = StatCols;
+  static constexpr int kInputs = 1, kOut = 1, kCarryThreads = 1024;
+  static constexpr bool kStaged = true, kFrames = false;
+  // a valid value x enters as (1, x, x - x), so that a NaN or an infinity makes M2 NaN
+  template <class Sm>
+  __device__ __forceinline__ static MSt entry(int, const Sm& sm, int j) {
+    const int c = sm.valid[j];
+    const double x = c ? f64_of(sm.buf[0][padded(j)]) : 0.0;
+    return MSt{c, x, x - x, sm.head[j]};
+  }
+  __device__ __forceinline__ static uint64_t out(const MSt& s, int) { return f64_bits(s.m2); }
+};
+
+// running count, mean x, mean y, Sxx, Syy and Sxy of the rows where x and y are both valid (fb_segmented_comoments)
+struct CoMomentScan {
+  using State = CSt;
+  using Cols = StatCols;
+  // half the threads of the other carry kernels: a CSt is twice an MSt, and 1024 threads leave 64 registers each
+  static constexpr int kInputs = 2, kOut = 5, kCarryThreads = 512;
+  static constexpr bool kStaged = false, kFrames = false;
+  // a pair enters as (1, x, y, z, z, z) with z = (x - x) * (y - y), +0 for finite x and y and NaN otherwise, so
+  // that a NaN or an infinity on either side makes all three sums NaN
+  template <class Sm>
+  __device__ __forceinline__ static CSt entry(int, const Sm& sm, int j) {
+    const int c = sm.valid[j];
+    const double x = c ? f64_of(sm.buf[0][padded(j)]) : 0.0, y = c ? f64_of(sm.buf[1][padded(j)]) : 0.0;
+    const double z = (x - x) * (y - y);
+    return CSt{c, x, y, z, z, z, sm.head[j]};
+  }
+  __device__ __forceinline__ static uint64_t out(const CSt& s, int o) {
+    const double v[5] = {s.mx, s.my, s.sxx, s.syy, s.sxy};
+    return f64_bits(v[o]);
+  }
+};
+
+// running count, M2, M3 and M4 (fb_segmented_shape_moments)
+struct ShapeScan {
+  using State = SSt;
+  using Cols = StatCols;
+  // an SSt is five 8-byte words and a flag, near a CSt, so the carry runs the co-moments carry's 512 threads
+  static constexpr int kInputs = 1, kOut = 3, kCarryThreads = 512;
+  static constexpr bool kStaged = false, kFrames = false;
+  // a valid value x enters as (1, x, z, z, z) with z = x - x, +0 for a finite x and NaN otherwise, so that a NaN or
+  // an infinity makes M2, M3 and M4 NaN
+  template <class Sm>
+  __device__ __forceinline__ static SSt entry(int, const Sm& sm, int j) {
+    const int c = sm.valid[j];
+    const double x = c ? f64_of(sm.buf[0][padded(j)]) : 0.0;
+    const double z = x - x;
+    return SSt{c, x, z, z, z, sm.head[j]};
+  }
+  __device__ __forceinline__ static uint64_t out(const SSt& s, int o) {
+    const double v[3] = {s.m2, s.m3, s.m4};
+    return f64_bits(v[o]);
+  }
+};
+
+// A tile's rows in shared memory: buf[0, kInputs) the staged input columns; a kStaged scan writes its output word
+// over buf[0] and its count into buf[kInputs] in pass 3.
+template <class T>
+struct TileSmem {
+  uint64_t buf[T::kInputs + (T::kStaged ? 1 : 0)][padded(kTile)];
+  uint8_t valid[kTile];  // every input of the row valid
+  uint8_t head[kTile];
+  typename T::State warp_tot[kThreads / 32];
+  int64_t seg_range[2];
+};
+
+// The tile states in scratch, a struct of arrays: w[k][i] is word k of state i = column * tiles + tile (one array
+// of columns x tiles per word), then f[tile], one flag per tile.
+template <class S>
+struct TileStates {
+  uint64_t* w[S::kWords];
+  int32_t* f;
+};
+
+template <class S>
+TileStates<S> tile_states(void* scratch, int64_t nt) {
+  TileStates<S> ts;
+  for (int k = 0; k < S::kWords; ++k) ts.w[k] = (uint64_t*)scratch + k * nt;
+  ts.f = (int32_t*)((uint64_t*)scratch + S::kWords * nt);
+  return ts;
+}
+
+template <class S>
+__device__ __forceinline__ S load_state(const TileStates<S>& ts, int64_t i, int32_t f) {
+  S s;
+  int k = 0;
+  S::zip(s, s, [&](auto& x, auto&) {
+    const uint64_t b = ts.w[k++][i];
+    memcpy(&x, &b, 8);
+  });
+  s.f = f;
+  return s;
+}
+
+template <class S>
+__device__ __forceinline__ void store_state(const TileStates<S>& ts, int64_t i, S s) {
+  int k = 0;
+  S::zip(s, s, [&](auto& x, auto&) {
+    uint64_t b;
+    memcpy(&b, &x, 8);
+    ts.w[k++][i] = b;
+  });
+}
+
+// kFinal = false: pass 1 (tile states); true: pass 3 (outputs, from the carries of pass 2).
 // The scan runs over positions p; position p is row p, or row nrows - 1 - p when kReverse (then a run
 // restarts after every segment's last row).  block > 0 also restarts the runs at every row that is a
 // multiple of `block` (kReverse: every row r with r + 1 a multiple of `block`); only with kBlocks, so that the
 // plain scan compiles without it.
-template <bool kFinal, bool kReverse = false, bool kBlocks = false>
+template <class T, bool kFinal, bool kReverse = false, bool kBlocks = false>
 __global__ void __launch_bounds__(kThreads)
 fb_segscan_tile_kernel(int64_t nrows, int64_t nseg, const int64_t* __restrict__ offsets,
-                       const __grid_constant__ ScanCols a, int64_t ntiles, uint64_t* __restrict__ tile_v,
-                       int64_t* __restrict__ tile_c, int32_t* __restrict__ tile_f, int64_t block = 0) {
-  __shared__ __align__(16) TileSmem sm;
+                       const __grid_constant__ typename T::Cols a, int64_t ntiles,
+                       const TileStates<typename T::State> ts, int64_t block) {
+  using S = typename T::State;
+  __shared__ __align__(16) TileSmem<T> sm;
   const int64_t tile = blockIdx.x;
   const int64_t start = tile * kTile;
   const int64_t end = start + kTile < nrows ? start + kTile : nrows;
@@ -336,439 +471,140 @@ fb_segscan_tile_kernel(int64_t nrows, int64_t nseg, const int64_t* __restrict__ 
   mark_heads<kReverse, kBlocks>(nrows, nseg, offsets, start, end, block, sm.head, sm.seg_range);
   const int j0 = threadIdx.x * kItems;
   for (int col = 0; col < a.ncols; ++col) {
-    const int op = a.op[col];
+    const int op = col_op(a, col);
+    const uint64_t* src[T::kInputs];
+    const uint8_t* vm[T::kInputs];
+#pragma unroll
+    for (int k = 0; k < T::kInputs; ++k) {
+      src[k] = col_input(a, col, k);
+      vm[k] = col_valid(a, col, k);
+    }
+    // striped (coalesced) loads into shared memory; rows past the end are invalid.  They read the tile's first row
+    // instead, so that every load stays in bounds and none waits on a branch.  A COUNT scan reads no values.
     const bool is_count = op == FB_AGG_COUNT;
-    const uint64_t* __restrict__ src = (const uint64_t*)a.vals[col];
-    const uint8_t* __restrict__ vm = a.valid[col];
-    // striped (coalesced) loads into shared memory; rows past the end are invalid
     for (int i = threadIdx.x; i < kTile; i += kThreads) {
       const bool in = i < nloc;
-      if (!is_count) sm.v[padded(i)] = in ? __ldg((const unsigned long long*)src + row(i)) : 0;
-      sm.valid[i] = in ? (vm == nullptr ? 1 : (__ldg(vm + row(i)) != 0)) : 0;
+      const int64_t r = row(in ? i : 0);
+#pragma unroll
+      for (int k = 0; k < T::kInputs; ++k)
+        if (!is_count) sm.buf[k][padded(i)] = in ? __ldg((const unsigned long long*)src[k] + r) : 0;
+      bool ok = true;
+#pragma unroll
+      for (int k = 0; k < T::kInputs; ++k) ok = ok && (vm[k] == nullptr || __ldg(vm[k] + r) != 0);
+      sm.valid[i] = in ? ok : 0;
     }
     __syncthreads();
-    St acc{0, 0, 0};
+    S acc{};
 #pragma unroll
-    for (int k = 0; k < kItems; ++k) {
-      const int j = j0 + k;
-      const int c = sm.valid[j];
-      const St x{c && !is_count ? sm.v[padded(j)] : 0, c, sm.head[j]};
-      acc = combine(op, acc, x);
-    }
-    St total;
-    const St pre = block_exclusive<kThreads / 32>(op, acc, sm.warp_tot, &total);
-    if (!kFinal) {
-      if (threadIdx.x == 0) {
-        tile_v[col * ntiles + tile] = total.v;
-        tile_c[col * ntiles + tile] = total.c;
-        if (col == 0) tile_f[tile] = total.f;
-      }
-      continue;
-    }
-    St run = combine(op, St{tile_v[col * ntiles + tile], tile_c[col * ntiles + tile], 0}, pre);
-#pragma unroll
-    for (int k = 0; k < kItems; ++k) {
-      const int j = j0 + k;
-      const int c = sm.valid[j];
-      const St x{c && !is_count ? sm.v[padded(j)] : 0, c, sm.head[j]};
-      run = combine(op, run, x);
-      sm.v[padded(j)] = run.c > 0 ? run.v : 0;  // no valid row yet: 0, not whatever preceded the segment
-      sm.c[padded(j)] = run.c;
-    }
-    __syncthreads();
-    uint64_t* __restrict__ ov = (uint64_t*)a.out_vals[col];
-    int64_t* __restrict__ oc = a.out_count[col];
-    for (int i = threadIdx.x; i < nloc; i += kThreads) {
-      if (ov != nullptr) ov[row(i)] = sm.v[padded(i)];
-      if (oc != nullptr) oc[row(i)] = sm.c[padded(i)];
-    }
-    __syncthreads();  // shared buffers are refilled by the next column
-  }
-}
-
-// pass 2: per column, the exclusive segmented scan of the tile aggregates (in place: aggregate -> carry)
-__global__ void __launch_bounds__(kCarryThreads)
-fb_segscan_carry_kernel(int64_t ntiles, const __grid_constant__ ScanCols a, uint64_t* __restrict__ tile_v,
-                        int64_t* __restrict__ tile_c, const int32_t* __restrict__ tile_f) {
-  __shared__ St warp_tot[kCarryThreads / 32];
-  const int col = blockIdx.x;
-  const int op = a.op[col];
-  uint64_t* tv = tile_v + col * ntiles;
-  int64_t* tc = tile_c + col * ntiles;
-  const int64_t per = (ntiles + kCarryThreads - 1) / kCarryThreads;
-  const int64_t b = threadIdx.x * per;
-  const int64_t e = b + per < ntiles ? b + per : ntiles;
-  St acc{0, 0, 0};
-  for (int64_t t = b; t < e; ++t) acc = combine(op, acc, St{tv[t], tc[t], tile_f[t]});
-  St total;
-  St run = block_exclusive<kCarryThreads / 32>(op, acc, warp_tot, &total);
-  for (int64_t t = b; t < e; ++t) {
-    const St x{tv[t], tc[t], tile_f[t]};
-    tv[t] = run.v;
-    tc[t] = run.c;
-    run = combine(op, run, x);
-  }
-}
-
-// ---- segmented moments (fb_segmented_moments): the same three launches over MSt ----------------------
-struct MomentCols {
-  const double* vals[FB_SCAN_MAX_COLS];
-  const uint8_t* valid[FB_SCAN_MAX_COLS];
-  int64_t* out_count[FB_SCAN_MAX_COLS];
-  double* out_m2[FB_SCAN_MAX_COLS];
-  int32_t ncols;
-};
-
-struct MomentSmem {
-  double x[padded(kTile)];  // values in, running M2 out
-  int64_t c[padded(kTile)];
-  uint8_t valid[kTile];
-  uint8_t head[kTile];
-  MSt warp_tot[kThreads / 32];
-  int64_t seg_range[2];
-};
-
-// the state of one row: a valid value x enters as (1, x, x - x), so that a NaN or an infinity makes M2 NaN
-__device__ __forceinline__ MSt moment_of(const MomentSmem& sm, int j) {
-  const int c = sm.valid[j];
-  const double x = c ? sm.x[padded(j)] : 0.0;
-  return MSt{c, x, x - x, sm.head[j]};
-}
-
-// kFinal = false: pass 1 (tile states); true: pass 3 (running count and M2 per row, from the carries)
-template <bool kFinal>
-__global__ void __launch_bounds__(kThreads)
-fb_segmoments_tile_kernel(int64_t nrows, int64_t nseg, const int64_t* __restrict__ offsets,
-                          const __grid_constant__ MomentCols a, int64_t ntiles, int64_t* __restrict__ tile_c,
-                          double* __restrict__ tile_mean, double* __restrict__ tile_m2, int32_t* __restrict__ tile_f) {
-  __shared__ __align__(16) MomentSmem sm;
-  const int64_t tile = blockIdx.x;
-  const int64_t start = tile * kTile;
-  const int64_t end = start + kTile < nrows ? start + kTile : nrows;
-  const int nloc = (int)(end - start);
-  mark_heads<false, false>(nrows, nseg, offsets, start, end, 0, sm.head, sm.seg_range);
-  const int j0 = threadIdx.x * kItems;
-  for (int col = 0; col < a.ncols; ++col) {
-    const double* __restrict__ src = a.vals[col];
-    const uint8_t* __restrict__ vm = a.valid[col];
-    for (int i = threadIdx.x; i < kTile; i += kThreads) {
-      const bool in = i < nloc;
-      sm.x[padded(i)] = in ? __ldg(src + start + i) : 0.0;
-      sm.valid[i] = in ? (vm == nullptr ? 1 : (__ldg(vm + start + i) != 0)) : 0;
-    }
-    __syncthreads();
-    MSt acc{};
-#pragma unroll
-    for (int k = 0; k < kItems; ++k) acc = combine(0, acc, moment_of(sm, j0 + k));
-    MSt total;
-    const MSt pre = block_exclusive<kThreads / 32, false, MSt>(0, acc, sm.warp_tot, &total);
+    for (int k = 0; k < kItems; ++k) acc = combine(op, acc, T::entry(op, sm, j0 + k));
+    S total;
+    const S pre = block_exclusive<kThreads / 32, false, S>(op, acc, sm.warp_tot, &total);
     const int64_t t = col * ntiles + tile;
     if (!kFinal) {
       if (threadIdx.x == 0) {
-        tile_c[t] = total.c;
-        tile_mean[t] = total.mean;
-        tile_m2[t] = total.m2;
-        if (col == 0) tile_f[tile] = total.f;
+        store_state(ts, t, total);
+        if (col == 0) ts.f[tile] = total.f;
       }
       continue;
     }
-    MSt run = combine(0, MSt{tile_c[t], tile_mean[t], tile_m2[t], 0}, pre);
+    S run = combine(op, load_state(ts, t, 0), pre);
+    if constexpr (T::kStaged) {
+      static_assert(T::kOut == 1, "a staged scan has one output word");
 #pragma unroll
-    for (int k = 0; k < kItems; ++k) {
-      const int j = j0 + k;
-      run = combine(0, run, moment_of(sm, j));
-      sm.x[padded(j)] = run.c > 0 ? run.m2 : 0.0;  // no valid row yet: 0, not whatever preceded the segment
-      sm.c[padded(j)] = run.c;
-    }
-    __syncthreads();
-    double* __restrict__ om = a.out_m2[col];
-    int64_t* __restrict__ oc = a.out_count[col];
-    for (int i = threadIdx.x; i < nloc; i += kThreads) {
-      if (om != nullptr) om[start + i] = sm.x[padded(i)];
-      if (oc != nullptr) oc[start + i] = sm.c[padded(i)];
+      for (int k = 0; k < kItems; ++k) {
+        const int j = j0 + k;
+        run = combine(op, run, T::entry(op, sm, j));
+        sm.buf[0][padded(j)] = run.c > 0 ? T::out(run, 0) : 0;  // no valid row yet: 0, not whatever preceded the segment
+        sm.buf[T::kInputs][padded(j)] = (uint64_t)run.c;
+      }
+      __syncthreads();
+      uint64_t* __restrict__ ov = col_output(a, col, 0);
+      int64_t* __restrict__ oc = a.out_count[col];
+      for (int i = threadIdx.x; i < nloc; i += kThreads) {
+        if (ov != nullptr) ov[row(i)] = sm.buf[0][padded(i)];
+        if (oc != nullptr) oc[row(i)] = (int64_t)sm.buf[T::kInputs][padded(i)];
+      }
+    } else {
+      int64_t* __restrict__ oc = a.out_count[col];
+#pragma unroll
+      for (int k = 0; k < kItems; ++k) {
+        const int j = j0 + k;
+        run = combine(op, run, T::entry(op, sm, j));
+        if (j >= nloc) continue;
+        const bool any = run.c > 0;  // no valid row yet: 0, not whatever preceded the segment
+        if (oc != nullptr) oc[row(j)] = run.c;
+#pragma unroll
+        for (int o = 0; o < T::kOut; ++o) {
+          uint64_t* __restrict__ ov = col_output(a, col, o);
+          if (ov != nullptr) ov[row(j)] = any ? T::out(run, o) : 0;
+        }
+      }
     }
     __syncthreads();  // shared buffers are refilled by the next column
   }
 }
 
 // pass 2: per column, the exclusive segmented scan of the tile states (in place: state -> carry)
-__global__ void __launch_bounds__(kCarryThreads)
-fb_segmoments_carry_kernel(int64_t ntiles, int64_t* __restrict__ tile_c, double* __restrict__ tile_mean,
-                           double* __restrict__ tile_m2, const int32_t* __restrict__ tile_f) {
-  __shared__ MSt warp_tot[kCarryThreads / 32];
-  const int64_t o = (int64_t)blockIdx.x * ntiles;
-  int64_t* tc = tile_c + o;
-  double* tm = tile_mean + o;
-  double* tq = tile_m2 + o;
-  const int64_t per = (ntiles + kCarryThreads - 1) / kCarryThreads;
+template <class T>
+__global__ void __launch_bounds__(T::kCarryThreads, 1)
+fb_segscan_carry_kernel(int64_t ntiles, const __grid_constant__ typename T::Cols a,
+                        const TileStates<typename T::State> ts) {
+  using S = typename T::State;
+  __shared__ S warp_tot[T::kCarryThreads / 32];
+  const int col = blockIdx.x;
+  const int op = col_op(a, col);
+  const int64_t o = (int64_t)col * ntiles;
+  const int64_t per = (ntiles + T::kCarryThreads - 1) / T::kCarryThreads;
   const int64_t b = threadIdx.x * per;
   const int64_t e = b + per < ntiles ? b + per : ntiles;
-  MSt acc{};
-  for (int64_t t = b; t < e; ++t) acc = combine(0, acc, MSt{tc[t], tm[t], tq[t], tile_f[t]});
-  MSt total;
-  MSt run = block_exclusive<kCarryThreads / 32, false, MSt>(0, acc, warp_tot, &total);
+  S acc{};
+  for (int64_t t = b; t < e; ++t) acc = combine(op, acc, load_state(ts, o + t, ts.f[t]));
+  S total;
+  S run = block_exclusive<T::kCarryThreads / 32, false, S>(op, acc, warp_tot, &total);
   for (int64_t t = b; t < e; ++t) {
-    const MSt x{tc[t], tm[t], tq[t], tile_f[t]};
-    tc[t] = run.c;
-    tm[t] = run.mean;
-    tq[t] = run.m2;
-    run = combine(0, run, x);
-  }
-}
-
-// ---- segmented co-moments (fb_segmented_comoments): the same three launches over CSt --------------------
-struct CoCols {
-  const double* x[FB_SCAN_MAX_COLS];
-  const double* y[FB_SCAN_MAX_COLS];
-  const uint8_t* vx[FB_SCAN_MAX_COLS];
-  const uint8_t* vy[FB_SCAN_MAX_COLS];
-  int64_t* out_count[FB_SCAN_MAX_COLS];
-  double* out[5][FB_SCAN_MAX_COLS];  // mean x, mean y, Sxx, Syy, Sxy
-  int32_t ncols;
-};
-
-// the tile states of every pair, column-major (pair * ntiles + tile); f: one per tile
-struct CoTiles {
-  int64_t* c;
-  double* mx;
-  double* my;
-  double* sxx;
-  double* syy;
-  double* sxy;
-  int32_t* f;
-};
-
-struct CoSmem {
-  double x[padded(kTile)];
-  double y[padded(kTile)];
-  uint8_t valid[kTile];  // x and y both valid
-  uint8_t head[kTile];
-  CSt warp_tot[kThreads / 32];
-  int64_t seg_range[2];
-};
-
-// the state of one row: a pair enters as (1, x, y, z, z, z) with z = (x - x) * (y - y), +0 for finite x and y and
-// NaN otherwise, so that a NaN or an infinity on either side makes all three sums NaN
-__device__ __forceinline__ CSt comoment_of(const CoSmem& sm, int j) {
-  const int c = sm.valid[j];
-  const double x = c ? sm.x[padded(j)] : 0.0, y = c ? sm.y[padded(j)] : 0.0;
-  const double z = (x - x) * (y - y);
-  return CSt{c, x, y, z, z, z, sm.head[j]};
-}
-
-// kFinal = false: pass 1 (tile states); true: pass 3 (the running state per row, from the carries).  Pass 3
-// stores a thread's kItems consecutive rows straight from registers: six outputs per row do not fit the staging
-// buffers, and the stores of a warp still cover whole lines together.
-template <bool kFinal>
-__global__ void __launch_bounds__(kThreads)
-fb_segcomoments_tile_kernel(int64_t nrows, int64_t nseg, const int64_t* __restrict__ offsets,
-                            const __grid_constant__ CoCols a, int64_t ntiles, CoTiles ts) {
-  __shared__ __align__(16) CoSmem sm;
-  const int64_t tile = blockIdx.x;
-  const int64_t start = tile * kTile;
-  const int64_t end = start + kTile < nrows ? start + kTile : nrows;
-  const int nloc = (int)(end - start);
-  mark_heads<false, false>(nrows, nseg, offsets, start, end, 0, sm.head, sm.seg_range);
-  const int j0 = threadIdx.x * kItems;
-  for (int col = 0; col < a.ncols; ++col) {
-    const double* __restrict__ xs = a.x[col];
-    const double* __restrict__ ys = a.y[col];
-    const uint8_t* __restrict__ vx = a.vx[col];
-    const uint8_t* __restrict__ vy = a.vy[col];
-    for (int i = threadIdx.x; i < kTile; i += kThreads) {
-      const bool in = i < nloc;
-      sm.x[padded(i)] = in ? __ldg(xs + start + i) : 0.0;
-      sm.y[padded(i)] = in ? __ldg(ys + start + i) : 0.0;
-      sm.valid[i] = in && (vx == nullptr || __ldg(vx + start + i) != 0) && (vy == nullptr || __ldg(vy + start + i) != 0);
-    }
-    __syncthreads();
-    CSt acc{};
-#pragma unroll
-    for (int k = 0; k < kItems; ++k) acc = combine(0, acc, comoment_of(sm, j0 + k));
-    CSt total;
-    const CSt pre = block_exclusive<kThreads / 32, false, CSt>(0, acc, sm.warp_tot, &total);
-    const int64_t t = col * ntiles + tile;
-    if (!kFinal) {
-      if (threadIdx.x == 0) {
-        ts.c[t] = total.c;
-        ts.mx[t] = total.mx;
-        ts.my[t] = total.my;
-        ts.sxx[t] = total.sxx;
-        ts.syy[t] = total.syy;
-        ts.sxy[t] = total.sxy;
-        if (col == 0) ts.f[tile] = total.f;
-      }
-      continue;
-    }
-    CSt run = combine(0, CSt{ts.c[t], ts.mx[t], ts.my[t], ts.sxx[t], ts.syy[t], ts.sxy[t], 0}, pre);
-    int64_t* __restrict__ oc = a.out_count[col];
-#pragma unroll
-    for (int k = 0; k < kItems; ++k) {
-      const int j = j0 + k;
-      run = combine(0, run, comoment_of(sm, j));
-      if (j >= nloc) continue;
-      const bool any = run.c > 0;  // no pair row yet: 0, not whatever preceded the segment
-      const double v[5] = {run.mx, run.my, run.sxx, run.syy, run.sxy};
-      if (oc != nullptr) oc[start + j] = run.c;
-#pragma unroll
-      for (int o = 0; o < 5; ++o)
-        if (a.out[o][col] != nullptr) a.out[o][col][start + j] = any ? v[o] : 0.0;
-    }
-    __syncthreads();  // shared buffers are refilled by the next pair
-  }
-}
-
-// pass 2: per pair, the exclusive segmented scan of the tile states (in place: state -> carry).  Half the
-// threads of the other carry kernels: a CSt is twice an MSt, and 1024 threads leave 64 registers each.
-constexpr int kCoCarryThreads = 512;
-__global__ void __launch_bounds__(kCoCarryThreads, 1)
-fb_segcomoments_carry_kernel(int64_t ntiles, CoTiles ts) {
-  __shared__ CSt warp_tot[kCoCarryThreads / 32];
-  const int64_t o = (int64_t)blockIdx.x * ntiles;
-  const int64_t per = (ntiles + kCoCarryThreads - 1) / kCoCarryThreads;
-  const int64_t b = threadIdx.x * per;
-  const int64_t e = b + per < ntiles ? b + per : ntiles;
-  auto load = [&](int64_t t) {
-    return CSt{ts.c[o + t], ts.mx[o + t], ts.my[o + t], ts.sxx[o + t], ts.syy[o + t], ts.sxy[o + t], ts.f[t]};
-  };
-  CSt acc{};
-  for (int64_t t = b; t < e; ++t) acc = combine(0, acc, load(t));
-  CSt total;
-  CSt run = block_exclusive<kCoCarryThreads / 32, false, CSt>(0, acc, warp_tot, &total);
-  for (int64_t t = b; t < e; ++t) {
-    const CSt x = load(t);
-    ts.c[o + t] = run.c;
-    ts.mx[o + t] = run.mx;
-    ts.my[o + t] = run.my;
-    ts.sxx[o + t] = run.sxx;
-    ts.syy[o + t] = run.syy;
-    ts.sxy[o + t] = run.sxy;
-    run = combine(0, run, x);
-  }
-}
-
-// ---- segmented shape moments (fb_segmented_shape_moments): the same three launches over SSt ------------------
-struct ShapeCols {
-  const double* vals[FB_SCAN_MAX_COLS];
-  const uint8_t* valid[FB_SCAN_MAX_COLS];
-  int64_t* out_count[FB_SCAN_MAX_COLS];
-  double* out[3][FB_SCAN_MAX_COLS];  // M2, M3, M4
-  int32_t ncols;
-};
-
-// the tile states of every column, column-major (column * ntiles + tile); f: one per tile
-struct ShapeTiles {
-  int64_t* c;
-  double* mean;
-  double* m2;
-  double* m3;
-  double* m4;
-  int32_t* f;
-};
-
-struct ShapeSmem {
-  double x[padded(kTile)];
-  uint8_t valid[kTile];
-  uint8_t head[kTile];
-  SSt warp_tot[kThreads / 32];
-  int64_t seg_range[2];
-};
-
-// the state of one row: a valid value x enters as (1, x, z, z, z) with z = x - x, +0 for a finite x and NaN
-// otherwise, so that a NaN or an infinity makes M2, M3 and M4 NaN
-__device__ __forceinline__ SSt shape_of(const ShapeSmem& sm, int j) {
-  const int c = sm.valid[j];
-  const double x = c ? sm.x[padded(j)] : 0.0;
-  const double z = x - x;
-  return SSt{c, x, z, z, z, sm.head[j]};
-}
-
-// kFinal = false: pass 1 (tile states); true: pass 3 (the running count, M2, M3 and M4 per row, from the carries).
-// Pass 3 stores a thread's kItems consecutive rows straight from registers, as the co-moments scan does.
-template <bool kFinal>
-__global__ void __launch_bounds__(kThreads)
-fb_segshape_tile_kernel(int64_t nrows, int64_t nseg, const int64_t* __restrict__ offsets,
-                        const __grid_constant__ ShapeCols a, int64_t ntiles, ShapeTiles ts) {
-  __shared__ __align__(16) ShapeSmem sm;
-  const int64_t tile = blockIdx.x;
-  const int64_t start = tile * kTile;
-  const int64_t end = start + kTile < nrows ? start + kTile : nrows;
-  const int nloc = (int)(end - start);
-  mark_heads<false, false>(nrows, nseg, offsets, start, end, 0, sm.head, sm.seg_range);
-  const int j0 = threadIdx.x * kItems;
-  for (int col = 0; col < a.ncols; ++col) {
-    const double* __restrict__ src = a.vals[col];
-    const uint8_t* __restrict__ vm = a.valid[col];
-    for (int i = threadIdx.x; i < kTile; i += kThreads) {
-      const bool in = i < nloc;
-      sm.x[padded(i)] = in ? __ldg(src + start + i) : 0.0;
-      sm.valid[i] = in ? (vm == nullptr ? 1 : (__ldg(vm + start + i) != 0)) : 0;
-    }
-    __syncthreads();
-    SSt acc{};
-#pragma unroll
-    for (int k = 0; k < kItems; ++k) acc = combine(0, acc, shape_of(sm, j0 + k));
-    SSt total;
-    const SSt pre = block_exclusive<kThreads / 32, false, SSt>(0, acc, sm.warp_tot, &total);
-    const int64_t t = col * ntiles + tile;
-    if (!kFinal) {
-      if (threadIdx.x == 0) {
-        ts.c[t] = total.c;
-        ts.mean[t] = total.mean;
-        ts.m2[t] = total.m2;
-        ts.m3[t] = total.m3;
-        ts.m4[t] = total.m4;
-        if (col == 0) ts.f[tile] = total.f;
-      }
-      continue;
-    }
-    SSt run = combine(0, SSt{ts.c[t], ts.mean[t], ts.m2[t], ts.m3[t], ts.m4[t], 0}, pre);
-    int64_t* __restrict__ oc = a.out_count[col];
-#pragma unroll
-    for (int k = 0; k < kItems; ++k) {
-      const int j = j0 + k;
-      run = combine(0, run, shape_of(sm, j));
-      if (j >= nloc) continue;
-      const bool any = run.c > 0;  // no valid row yet: 0, not whatever preceded the segment
-      const double v[3] = {run.m2, run.m3, run.m4};
-      if (oc != nullptr) oc[start + j] = run.c;
-#pragma unroll
-      for (int o = 0; o < 3; ++o)
-        if (a.out[o][col] != nullptr) a.out[o][col][start + j] = any ? v[o] : 0.0;
-    }
-    __syncthreads();  // shared buffers are refilled by the next column
-  }
-}
-
-// pass 2: per column, the exclusive segmented scan of the tile states (in place: state -> carry).  An SSt is
-// five 8-byte words and a flag, near a CSt, so the carry kernel runs the co-moments carry's 512 threads.
-constexpr int kShapeCarryThreads = 512;
-__global__ void __launch_bounds__(kShapeCarryThreads, 1)
-fb_segshape_carry_kernel(int64_t ntiles, ShapeTiles ts) {
-  __shared__ SSt warp_tot[kShapeCarryThreads / 32];
-  const int64_t o = (int64_t)blockIdx.x * ntiles;
-  const int64_t per = (ntiles + kShapeCarryThreads - 1) / kShapeCarryThreads;
-  const int64_t b = threadIdx.x * per;
-  const int64_t e = b + per < ntiles ? b + per : ntiles;
-  auto load = [&](int64_t t) {
-    return SSt{ts.c[o + t], ts.mean[o + t], ts.m2[o + t], ts.m3[o + t], ts.m4[o + t], ts.f[t]};
-  };
-  SSt acc{};
-  for (int64_t t = b; t < e; ++t) acc = combine(0, acc, load(t));
-  SSt total;
-  SSt run = block_exclusive<kShapeCarryThreads / 32, false, SSt>(0, acc, warp_tot, &total);
-  for (int64_t t = b; t < e; ++t) {
-    const SSt x = load(t);
-    ts.c[o + t] = run.c;
-    ts.mean[o + t] = run.mean;
-    ts.m2[o + t] = run.m2;
-    ts.m3[o + t] = run.m3;
-    ts.m4[o + t] = run.m4;
-    run = combine(0, run, x);
+    const S x = load_state(ts, o + t, ts.f[t]);
+    store_state(ts, o + t, run);
+    run = combine(op, run, x);
   }
 }
 
 int64_t num_tiles(int64_t nrows) { return (nrows + kTile - 1) / kTile; }
+
+template <class T>
+size_t segscan_scratch_bytes(int64_t nrows, int ncols) {
+  if (nrows <= 0 || ncols <= 0) return 0;
+  return (size_t)num_tiles(nrows) * (8 * T::State::kWords * (size_t)ncols + 4);
+}
+
+template <class T, bool kReverse = false, bool kBlocks = false>
+int launch_segscan(cudaStream_t st, int64_t block, int64_t nrows, int64_t nseg, const int64_t* offsets,
+                   const typename T::Cols& a, void* scratch) {
+  const int64_t ntiles = num_tiles(nrows);
+  const TileStates<typename T::State> ts = tile_states<typename T::State>(scratch, a.ncols * ntiles);
+  const unsigned grid = (unsigned)ntiles;
+  fb_segscan_tile_kernel<T, false, kReverse, kBlocks><<<grid, kThreads, 0, st>>>(nrows, nseg, offsets, a, ntiles,
+                                                                                  ts, block);
+  FB_CUDA(cudaGetLastError());
+  fb_segscan_carry_kernel<T><<<a.ncols, T::kCarryThreads, 0, st>>>(ntiles, a, ts);
+  FB_CUDA(cudaGetLastError());
+  fb_segscan_tile_kernel<T, true, kReverse, kBlocks><<<grid, kThreads, 0, st>>>(nrows, nseg, offsets, a, ntiles,
+                                                                                 ts, block);
+  FB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// one inclusive scan of every column into its outputs; with T::kFrames, reversed (S) and / or restarting at blocks
+// of `block` rows (block > 0)
+template <class T>
+int run_segscan(cudaStream_t st, bool reverse, int64_t block, int64_t nrows, int64_t nseg, const int64_t* offsets,
+                const typename T::Cols& a, void* scratch) {
+  if constexpr (T::kFrames) {
+    if (reverse && block > 0) return launch_segscan<T, true, true>(st, block, nrows, nseg, offsets, a, scratch);
+    if (reverse) return launch_segscan<T, true>(st, block, nrows, nseg, offsets, a, scratch);
+    if (block > 0) return launch_segscan<T, false, true>(st, block, nrows, nseg, offsets, a, scratch);
+  }
+  return launch_segscan<T>(st, block, nrows, nseg, offsets, a, scratch);
+}
 
 // ---- moving frames -------------------------------------------------------------------------------
 constexpr int kFrameThreads = 256;
@@ -985,44 +821,7 @@ size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
 size_t frame_scratch(int64_t nrows, int ncols, const Frame& f) {
   if (nrows <= 0 || ncols <= 0 || f.tile) return 0;
   const int sides = f.flags == 0 ? 2 : 1;
-  return align256(fb_segmented_scan_scratch_bytes(nrows, ncols)) + (size_t)sides * 16 * ncols * (size_t)nrows;
-}
-
-// one inclusive scan (P, or S when reverse) of every column into out_vals / out_count, blocks of `block` rows
-int run_scan(cudaStream_t st, bool reverse, int64_t block, int64_t nrows, int64_t nseg, const int64_t* offsets,
-             const ScanCols& a, void* tiles) {
-  const int64_t ntiles = num_tiles(nrows);
-  uint64_t* tile_v = (uint64_t*)tiles;
-  int64_t* tile_c = (int64_t*)(tile_v + a.ncols * ntiles);
-  int32_t* tile_f = (int32_t*)(tile_c + a.ncols * ntiles);
-  const unsigned grid = (unsigned)ntiles;
-  if (reverse && block > 0)
-    fb_segscan_tile_kernel<false, true, true><<<grid, kThreads, 0, st>>>(nrows, nseg, offsets, a, ntiles, tile_v,
-                                                                         tile_c, tile_f, block);
-  else if (reverse)
-    fb_segscan_tile_kernel<false, true><<<grid, kThreads, 0, st>>>(nrows, nseg, offsets, a, ntiles, tile_v, tile_c,
-                                                                   tile_f);
-  else if (block > 0)
-    fb_segscan_tile_kernel<false, false, true><<<grid, kThreads, 0, st>>>(nrows, nseg, offsets, a, ntiles, tile_v,
-                                                                          tile_c, tile_f, block);
-  else
-    fb_segscan_tile_kernel<false><<<grid, kThreads, 0, st>>>(nrows, nseg, offsets, a, ntiles, tile_v, tile_c, tile_f);
-  FB_CUDA(cudaGetLastError());
-  fb_segscan_carry_kernel<<<a.ncols, kCarryThreads, 0, st>>>(ntiles, a, tile_v, tile_c, tile_f);
-  FB_CUDA(cudaGetLastError());
-  if (reverse && block > 0)
-    fb_segscan_tile_kernel<true, true, true><<<grid, kThreads, 0, st>>>(nrows, nseg, offsets, a, ntiles, tile_v,
-                                                                        tile_c, tile_f, block);
-  else if (reverse)
-    fb_segscan_tile_kernel<true, true><<<grid, kThreads, 0, st>>>(nrows, nseg, offsets, a, ntiles, tile_v, tile_c,
-                                                                  tile_f);
-  else if (block > 0)
-    fb_segscan_tile_kernel<true, false, true><<<grid, kThreads, 0, st>>>(nrows, nseg, offsets, a, ntiles, tile_v,
-                                                                         tile_c, tile_f, block);
-  else
-    fb_segscan_tile_kernel<true><<<grid, kThreads, 0, st>>>(nrows, nseg, offsets, a, ntiles, tile_v, tile_c, tile_f);
-  FB_CUDA(cudaGetLastError());
-  return 0;
+  return align256(segscan_scratch_bytes<OpScan>(nrows, ncols)) + (size_t)sides * 16 * ncols * (size_t)nrows;
 }
 
 // ---- value frames (RANGE BETWEEN) ----------------------------------------------------------------
@@ -1255,78 +1054,80 @@ int scan_cols(int64_t nrows, int ncols, const int32_t* ops, const void* const* v
   return 0;
 }
 
+// The host arrays of an f64 statistics entry -> StatCols: `nin` inputs with their validity, the count and `nout`
+// words out (any array may be NULL: every entry NULL)
+void stat_cols(StatCols& a, int nin, const void* const* const* in, const uint8_t* const* const* valid,
+               int64_t* const* out_count, int nout, void* const* const* out) {
+  for (int c = 0; c < a.ncols; ++c) {
+    for (int k = 0; k < nin; ++k) {
+      a.in[k][c] = in[k] != nullptr ? (const double*)in[k][c] : nullptr;
+      a.valid[k][c] = valid[k] != nullptr ? valid[k][c] : nullptr;
+    }
+    a.out_count[c] = out_count != nullptr ? out_count[c] : nullptr;
+    for (int o = 0; o < nout; ++o) a.out[o][c] = out[o] != nullptr ? (double*)out[o][c] : nullptr;
+  }
+}
+
+// What every segmented scan entry shares: the checks of the counts, `fill` (the columns, checked: nonzero is an
+// error), the checks of segments and scratch, the device, then the scan.  `what` names ncols in its error.
+template <class T, class Fill>
+int segscan_entry(int dev, void* stream, int64_t nrows, int64_t nseg, const int64_t* d_offsets, int ncols,
+                  const char* what, void* scratch, size_t scratch_bytes, Fill fill) {
+  FB_CHECK(nrows >= 0 && nseg >= 0, "negative row or segment count");
+  FB_CHECK(ncols >= 1 && ncols <= FB_SCAN_MAX_COLS, "%s=%d out of range [1,%d]", what, ncols, FB_SCAN_MAX_COLS);
+  typename T::Cols a;
+  memset(&a, 0, sizeof(a));
+  a.ncols = ncols;
+  if (fill(a) != 0) return 1;
+  if (nrows == 0) return 0;
+  FB_CHECK(nseg >= 1 && d_offsets != nullptr, "%lld rows need at least one segment", (long long)nrows);
+  FB_CHECK(num_tiles(nrows) < (1LL << 31), "too many rows");
+  const size_t need = segscan_scratch_bytes<T>(nrows, ncols);
+  FB_CHECK(scratch != nullptr && scratch_bytes >= need, "scratch too small: %zu < %zu", scratch_bytes, need);
+  FbDeviceGuard guard(dev);
+  FB_CHECK(guard.ok, "cannot select device %d", dev);
+  return run_segscan<T>((cudaStream_t)stream, false, 0, nrows, nseg, d_offsets, a, scratch);
+}
+
 }  // namespace
 
 extern "C" size_t fb_segmented_scan_scratch_bytes(int64_t nrows, int ncols) {
-  if (nrows <= 0 || ncols <= 0) return 0;
-  return (size_t)num_tiles(nrows) * (16 * (size_t)ncols + 4);
+  return segscan_scratch_bytes<OpScan>(nrows, ncols);
 }
 
 extern "C" int fb_segmented_scan(int dev, void* stream, int64_t nrows, int64_t nseg, const int64_t* d_offsets,
                                  int ncols, const int32_t* ops, const void* const* vals,
                                  const uint8_t* const* valid, void* const* out_vals, int64_t* const* out_count,
                                  void* scratch, size_t scratch_bytes) {
-  FB_CHECK(nrows >= 0 && nseg >= 0, "negative row or segment count");
-  ScanCols a;
-  if (scan_cols(nrows, ncols, ops, vals, valid, out_vals, out_count, &a) != 0) return 1;
-  if (nrows == 0) return 0;
-  FB_CHECK(nseg >= 1 && d_offsets != nullptr, "%lld rows need at least one segment", (long long)nrows);
-  FB_CHECK(num_tiles(nrows) < (1LL << 31), "too many rows");
-  FB_CHECK(scratch != nullptr && scratch_bytes >= fb_segmented_scan_scratch_bytes(nrows, ncols),
-           "scratch too small: %zu < %zu", scratch_bytes, fb_segmented_scan_scratch_bytes(nrows, ncols));
-  FbDeviceGuard guard(dev);
-  FB_CHECK(guard.ok, "cannot select device %d", dev);
-  return run_scan((cudaStream_t)stream, false, 0, nrows, nseg, d_offsets, a, scratch);
+  return segscan_entry<OpScan>(dev, stream, nrows, nseg, d_offsets, ncols, "ncols", scratch, scratch_bytes,
+                               [&](ScanCols& a) {
+                                 return scan_cols(nrows, ncols, ops, vals, valid, out_vals, out_count, &a);
+                               });
 }
 
 extern "C" size_t fb_segmented_moments_scratch_bytes(int64_t nrows, int ncols) {
-  if (nrows <= 0 || ncols <= 0) return 0;
-  return (size_t)num_tiles(nrows) * (24 * (size_t)ncols + 4);
+  return segscan_scratch_bytes<MomentScan>(nrows, ncols);
 }
 
 extern "C" int fb_segmented_moments(int dev, void* stream, int64_t nrows, int64_t nseg, const int64_t* d_offsets,
                                     int ncols, const void* const* vals, const uint8_t* const* valid,
                                     int64_t* const* out_count, void* const* out_m2, void* scratch,
                                     size_t scratch_bytes) {
-  FB_CHECK(nrows >= 0 && nseg >= 0, "negative row or segment count");
-  FB_CHECK(ncols >= 1 && ncols <= FB_SCAN_MAX_COLS, "ncols=%d out of range [1,%d]", ncols, FB_SCAN_MAX_COLS);
-  MomentCols a;
-  memset(&a, 0, sizeof(a));
-  a.ncols = ncols;
-  for (int c = 0; c < ncols; ++c) {
-    a.vals[c] = vals != nullptr ? (const double*)vals[c] : nullptr;
-    a.valid[c] = valid != nullptr ? valid[c] : nullptr;
-    a.out_count[c] = out_count != nullptr ? out_count[c] : nullptr;
-    a.out_m2[c] = out_m2 != nullptr ? (double*)out_m2[c] : nullptr;
-    FB_CHECK(nrows == 0 || a.vals[c] != nullptr, "column %d needs a value column", c);
-  }
-  if (nrows == 0) return 0;
-  FB_CHECK(nseg >= 1 && d_offsets != nullptr, "%lld rows need at least one segment", (long long)nrows);
-  FB_CHECK(num_tiles(nrows) < (1LL << 31), "too many rows");
-  FB_CHECK(scratch != nullptr && scratch_bytes >= fb_segmented_moments_scratch_bytes(nrows, ncols),
-           "scratch too small: %zu < %zu", scratch_bytes, fb_segmented_moments_scratch_bytes(nrows, ncols));
-  FbDeviceGuard guard(dev);
-  FB_CHECK(guard.ok, "cannot select device %d", dev);
-  cudaStream_t st = (cudaStream_t)stream;
-  const int64_t ntiles = num_tiles(nrows);
-  int64_t* tile_c = (int64_t*)scratch;
-  double* tile_mean = (double*)(tile_c + ncols * ntiles);
-  double* tile_m2 = tile_mean + ncols * ntiles;
-  int32_t* tile_f = (int32_t*)(tile_m2 + ncols * ntiles);
-  fb_segmoments_tile_kernel<false><<<(unsigned)ntiles, kThreads, 0, st>>>(nrows, nseg, d_offsets, a, ntiles, tile_c,
-                                                                          tile_mean, tile_m2, tile_f);
-  FB_CUDA(cudaGetLastError());
-  fb_segmoments_carry_kernel<<<ncols, kCarryThreads, 0, st>>>(ntiles, tile_c, tile_mean, tile_m2, tile_f);
-  FB_CUDA(cudaGetLastError());
-  fb_segmoments_tile_kernel<true><<<(unsigned)ntiles, kThreads, 0, st>>>(nrows, nseg, d_offsets, a, ntiles, tile_c,
-                                                                         tile_mean, tile_m2, tile_f);
-  FB_CUDA(cudaGetLastError());
-  return 0;
+  return segscan_entry<MomentScan>(dev, stream, nrows, nseg, d_offsets, ncols, "ncols", scratch, scratch_bytes,
+                                   [&](StatCols& a) {
+                                     const void* const* in[1] = {vals};
+                                     const uint8_t* const* vin[1] = {valid};
+                                     void* const* out[1] = {out_m2};
+                                     stat_cols(a, 1, in, vin, out_count, 1, out);
+                                     for (int c = 0; c < ncols; ++c)
+                                       FB_CHECK(nrows == 0 || a.in[0][c] != nullptr,
+                                                "column %d needs a value column", c);
+                                     return 0;
+                                   });
 }
 
 extern "C" size_t fb_segmented_comoments_scratch_bytes(int64_t nrows, int npairs) {
-  if (nrows <= 0 || npairs <= 0) return 0;
-  return (size_t)num_tiles(nrows) * (48 * (size_t)npairs + 4);
+  return segscan_scratch_bytes<CoMomentScan>(nrows, npairs);
 }
 
 extern "C" int fb_segmented_comoments(int dev, void* stream, int64_t nrows, int64_t nseg, const int64_t* d_offsets,
@@ -1335,94 +1136,38 @@ extern "C" int fb_segmented_comoments(int dev, void* stream, int64_t nrows, int6
                                       void* const* out_mean_x, void* const* out_mean_y, void* const* out_sxx,
                                       void* const* out_syy, void* const* out_sxy, void* scratch,
                                       size_t scratch_bytes) {
-  FB_CHECK(nrows >= 0 && nseg >= 0, "negative row or segment count");
-  FB_CHECK(npairs >= 1 && npairs <= FB_SCAN_MAX_COLS, "npairs=%d out of range [1,%d]", npairs, FB_SCAN_MAX_COLS);
-  CoCols a;
-  memset(&a, 0, sizeof(a));
-  a.ncols = npairs;
-  void* const* outs[5] = {out_mean_x, out_mean_y, out_sxx, out_syy, out_sxy};
-  for (int c = 0; c < npairs; ++c) {
-    a.x[c] = xs != nullptr ? (const double*)xs[c] : nullptr;
-    a.y[c] = ys != nullptr ? (const double*)ys[c] : nullptr;
-    a.vx[c] = x_valid != nullptr ? x_valid[c] : nullptr;
-    a.vy[c] = y_valid != nullptr ? y_valid[c] : nullptr;
-    a.out_count[c] = out_count != nullptr ? out_count[c] : nullptr;
-    for (int o = 0; o < 5; ++o) a.out[o][c] = outs[o] != nullptr ? (double*)outs[o][c] : nullptr;
-    FB_CHECK(nrows == 0 || (a.x[c] != nullptr && a.y[c] != nullptr), "pair %d needs an x and a y column", c);
-  }
-  if (nrows == 0) return 0;
-  FB_CHECK(nseg >= 1 && d_offsets != nullptr, "%lld rows need at least one segment", (long long)nrows);
-  FB_CHECK(num_tiles(nrows) < (1LL << 31), "too many rows");
-  FB_CHECK(scratch != nullptr && scratch_bytes >= fb_segmented_comoments_scratch_bytes(nrows, npairs),
-           "scratch too small: %zu < %zu", scratch_bytes, fb_segmented_comoments_scratch_bytes(nrows, npairs));
-  FbDeviceGuard guard(dev);
-  FB_CHECK(guard.ok, "cannot select device %d", dev);
-  cudaStream_t st = (cudaStream_t)stream;
-  const int64_t ntiles = num_tiles(nrows);
-  const int64_t nt = npairs * ntiles;
-  CoTiles ts;
-  ts.c = (int64_t*)scratch;
-  ts.mx = (double*)(ts.c + nt);
-  ts.my = ts.mx + nt;
-  ts.sxx = ts.my + nt;
-  ts.syy = ts.sxx + nt;
-  ts.sxy = ts.syy + nt;
-  ts.f = (int32_t*)(ts.sxy + nt);
-  fb_segcomoments_tile_kernel<false><<<(unsigned)ntiles, kThreads, 0, st>>>(nrows, nseg, d_offsets, a, ntiles, ts);
-  FB_CUDA(cudaGetLastError());
-  fb_segcomoments_carry_kernel<<<npairs, kCoCarryThreads, 0, st>>>(ntiles, ts);
-  FB_CUDA(cudaGetLastError());
-  fb_segcomoments_tile_kernel<true><<<(unsigned)ntiles, kThreads, 0, st>>>(nrows, nseg, d_offsets, a, ntiles, ts);
-  FB_CUDA(cudaGetLastError());
-  return 0;
+  return segscan_entry<CoMomentScan>(dev, stream, nrows, nseg, d_offsets, npairs, "npairs", scratch, scratch_bytes,
+                                     [&](StatCols& a) {
+                                       const void* const* in[2] = {xs, ys};
+                                       const uint8_t* const* vin[2] = {x_valid, y_valid};
+                                       void* const* out[5] = {out_mean_x, out_mean_y, out_sxx, out_syy, out_sxy};
+                                       stat_cols(a, 2, in, vin, out_count, 5, out);
+                                       for (int c = 0; c < npairs; ++c)
+                                         FB_CHECK(nrows == 0 || (a.in[0][c] != nullptr && a.in[1][c] != nullptr),
+                                                  "pair %d needs an x and a y column", c);
+                                       return 0;
+                                     });
 }
 
 extern "C" size_t fb_segmented_shape_moments_scratch_bytes(int64_t nrows, int ncols) {
-  if (nrows <= 0 || ncols <= 0) return 0;
-  return (size_t)num_tiles(nrows) * (40 * (size_t)ncols + 4);
+  return segscan_scratch_bytes<ShapeScan>(nrows, ncols);
 }
 
 extern "C" int fb_segmented_shape_moments(int dev, void* stream, int64_t nrows, int64_t nseg, const int64_t* d_offsets,
                                           int ncols, const void* const* vals, const uint8_t* const* valid,
                                           int64_t* const* out_count, void* const* out_m2, void* const* out_m3,
                                           void* const* out_m4, void* scratch, size_t scratch_bytes) {
-  FB_CHECK(nrows >= 0 && nseg >= 0, "negative row or segment count");
-  FB_CHECK(ncols >= 1 && ncols <= FB_SCAN_MAX_COLS, "ncols=%d out of range [1,%d]", ncols, FB_SCAN_MAX_COLS);
-  ShapeCols a;
-  memset(&a, 0, sizeof(a));
-  a.ncols = ncols;
-  void* const* outs[3] = {out_m2, out_m3, out_m4};
-  for (int c = 0; c < ncols; ++c) {
-    a.vals[c] = vals != nullptr ? (const double*)vals[c] : nullptr;
-    a.valid[c] = valid != nullptr ? valid[c] : nullptr;
-    a.out_count[c] = out_count != nullptr ? out_count[c] : nullptr;
-    for (int o = 0; o < 3; ++o) a.out[o][c] = outs[o] != nullptr ? (double*)outs[o][c] : nullptr;
-    FB_CHECK(nrows == 0 || a.vals[c] != nullptr, "column %d needs a value column", c);
-  }
-  if (nrows == 0) return 0;
-  FB_CHECK(nseg >= 1 && d_offsets != nullptr, "%lld rows need at least one segment", (long long)nrows);
-  FB_CHECK(num_tiles(nrows) < (1LL << 31), "too many rows");
-  FB_CHECK(scratch != nullptr && scratch_bytes >= fb_segmented_shape_moments_scratch_bytes(nrows, ncols),
-           "scratch too small: %zu < %zu", scratch_bytes, fb_segmented_shape_moments_scratch_bytes(nrows, ncols));
-  FbDeviceGuard guard(dev);
-  FB_CHECK(guard.ok, "cannot select device %d", dev);
-  cudaStream_t st = (cudaStream_t)stream;
-  const int64_t ntiles = num_tiles(nrows);
-  const int64_t nt = ncols * ntiles;
-  ShapeTiles ts;
-  ts.c = (int64_t*)scratch;
-  ts.mean = (double*)(ts.c + nt);
-  ts.m2 = ts.mean + nt;
-  ts.m3 = ts.m2 + nt;
-  ts.m4 = ts.m3 + nt;
-  ts.f = (int32_t*)(ts.m4 + nt);
-  fb_segshape_tile_kernel<false><<<(unsigned)ntiles, kThreads, 0, st>>>(nrows, nseg, d_offsets, a, ntiles, ts);
-  FB_CUDA(cudaGetLastError());
-  fb_segshape_carry_kernel<<<ncols, kShapeCarryThreads, 0, st>>>(ntiles, ts);
-  FB_CUDA(cudaGetLastError());
-  fb_segshape_tile_kernel<true><<<(unsigned)ntiles, kThreads, 0, st>>>(nrows, nseg, d_offsets, a, ntiles, ts);
-  FB_CUDA(cudaGetLastError());
-  return 0;
+  return segscan_entry<ShapeScan>(dev, stream, nrows, nseg, d_offsets, ncols, "ncols", scratch, scratch_bytes,
+                                  [&](StatCols& a) {
+                                    const void* const* in[1] = {vals};
+                                    const uint8_t* const* vin[1] = {valid};
+                                    void* const* out[3] = {out_m2, out_m3, out_m4};
+                                    stat_cols(a, 1, in, vin, out_count, 3, out);
+                                    for (int c = 0; c < ncols; ++c)
+                                      FB_CHECK(nrows == 0 || a.in[0][c] != nullptr, "column %d needs a value column",
+                                               c);
+                                    return 0;
+                                  });
 }
 
 extern "C" size_t fb_window_frame_scratch_bytes(int64_t nrows, int ncols, int64_t start, int64_t end, int flags) {
@@ -1471,7 +1216,7 @@ extern "C" int fb_window_frame(int dev, void* stream, int64_t nrows, int64_t nse
   const bool need_p = f.flags != FB_FRAME_UNBOUNDED_END;                 // bounded, (None, e), (None, None)
   const bool need_s = f.flags == 0 || f.flags == FB_FRAME_UNBOUNDED_END;  // bounded, (s, None)
   char* tiles = (char*)scratch;
-  char* sides = tiles + align256(fb_segmented_scan_scratch_bytes(nrows, ncols));
+  char* sides = tiles + align256(segscan_scratch_bytes<OpScan>(nrows, ncols));
   const size_t side = (size_t)ncols * (size_t)nrows;
   uint64_t* pv = need_p ? (uint64_t*)sides : nullptr;
   int64_t* pc = need_p ? (int64_t*)(pv + side) : nullptr;
@@ -1483,14 +1228,14 @@ extern "C" int fb_window_frame(int dev, void* stream, int64_t nrows, int64_t nse
       b.out_vals[c] = pv + c * nrows;
       b.out_count[c] = pc + c * nrows;
     }
-    if (run_scan(st, false, f.width, nrows, nseg, d_offsets, b, tiles) != 0) return 2;
+    if (run_segscan<OpScan>(st, false, f.width, nrows, nseg, d_offsets, b, tiles) != 0) return 2;
   }
   if (need_s) {
     for (int c = 0; c < ncols; ++c) {
       b.out_vals[c] = sv + c * nrows;
       b.out_count[c] = sc + c * nrows;
     }
-    if (run_scan(st, true, f.width, nrows, nseg, d_offsets, b, tiles) != 0) return 2;
+    if (run_segscan<OpScan>(st, true, f.width, nrows, nseg, d_offsets, b, tiles) != 0) return 2;
   }
   fb_window_frame_combine_kernel<<<(unsigned)num_tiles(nrows), kThreads, 0, st>>>(
       nrows, nseg, d_offsets, a, f.start, f.end, f.flags, f.width, pv, pc, sv, sc);

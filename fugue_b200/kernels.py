@@ -405,6 +405,73 @@ def groupby_u64(keys: torch.Tensor, key_valid: Optional[torch.Tensor],
 SCAN_MAX_COLS = 8
 
 
+def _segments(offsets: torch.Tensor) -> Tuple[torch.device, int]:
+    assert offsets.dtype == torch.int64 and offsets.is_cuda and offsets.is_contiguous()
+    return offsets.device, int(offsets.shape[0]) - 1
+
+
+def _check_rows(t: Optional[torch.Tensor], dev: torch.device, nrows: int, dtype: Optional[torch.dtype] = None) -> None:
+    """``t`` is None or a contiguous column of ``nrows`` values on ``dev``: of ``dtype``, or of any 8-byte type."""
+    if t is not None:
+        assert (t.element_size() == 8 if dtype is None else t.dtype == dtype)
+        assert t.device == dev and t.is_contiguous() and t.shape[0] == nrows
+
+
+def _ptrs(ts: Sequence[Optional[torch.Tensor]]) -> Any:
+    return _lib.ptr_array([0 if t is None else t.data_ptr() for t in ts])
+
+
+def _batched(items: Sequence[Any], dev: torch.device, outputs: Any, scratch_bytes: Any, launch: Any) -> List[Any]:
+    """Runs ``items`` ``SCAN_MAX_COLS`` at a time: per batch, ``outputs(*item)`` allocates each item's output tensors,
+    ``scratch_bytes(n)`` sizes the scratch of n items, and ``launch(batch, outs, scratch)`` calls the kernel with
+    ``outs[k]``, the pointer array of every item's k-th output.  Returns the outputs per item."""
+    res: List[Any] = []
+    for b in range(0, len(items), SCAN_MAX_COLS):
+        batch = items[b:b + SCAN_MAX_COLS]
+        outs = [outputs(*it) for it in batch]
+        nb = int(scratch_bytes(len(batch)))
+        scratch = torch.empty(max(nb, 8), dtype=torch.uint8, device=dev)
+        _lib.check(launch(batch, [_ptrs(o) for o in zip(*outs)], scratch))
+        res.extend(outs)
+    return res
+
+
+def _op_batched(columns: Sequence[Tuple[int, Optional[torch.Tensor], Optional[torch.Tensor]]], nrows: int,
+                dev: torch.device, scratch_bytes: Any, launch: Any) -> List[Tuple[Optional[torch.Tensor], torch.Tensor]]:
+    """:func:`_batched` over ``(op, values or None, validity or None)`` columns with ``(values, count)`` outputs:
+    ``launch(n, ops, vals, valid, out_vals, out_count, scratch, scratch_bytes)``."""
+
+    def outputs(op: int, v: Optional[torch.Tensor], m: Optional[torch.Tensor]) -> Tuple[Optional[torch.Tensor], torch.Tensor]:
+        assert (v is None) == (op == AGG_COUNT)
+        _check_rows(v, dev, nrows)
+        _check_rows(m, dev, nrows, torch.uint8)
+        return None if v is None else torch.empty_like(v), torch.empty(nrows, dtype=torch.int64, device=dev)
+
+    return _batched(columns, dev, outputs, scratch_bytes, lambda batch, outs, scratch: launch(
+        len(batch), _lib.i32_array([op for op, _, _ in batch]), _ptrs([v for _, v, _ in batch]),
+        _ptrs([m for _, _, m in batch]), *outs, scratch.data_ptr(), scratch.numel()))
+
+
+def _stat_outputs(dev: torch.device, nrows: int, nf64: int) -> Tuple[torch.Tensor, ...]:
+    return (torch.empty(nrows, dtype=torch.int64, device=dev),) + tuple(
+        torch.empty(nrows, dtype=torch.float64, device=dev) for _ in range(nf64))
+
+
+def _value_batched(columns: Sequence[Tuple[torch.Tensor, Optional[torch.Tensor]]], nrows: int, dev: torch.device,
+                   nf64: int, scratch_bytes: Any, launch: Any) -> List[Tuple[torch.Tensor, ...]]:
+    """:func:`_batched` over ``(float64 values, validity or None)`` columns with a count and ``nf64`` float64 outputs:
+    ``launch(n, vals, valid, out_count, *outs, scratch, scratch_bytes)``."""
+
+    def outputs(v: torch.Tensor, m: Optional[torch.Tensor]) -> Tuple[torch.Tensor, ...]:
+        _check_rows(v, dev, nrows, torch.float64)
+        _check_rows(m, dev, nrows, torch.uint8)
+        return _stat_outputs(dev, nrows, nf64)
+
+    return _batched(columns, dev, outputs, scratch_bytes, lambda batch, outs, scratch: launch(
+        len(batch), _ptrs([v for v, _ in batch]), _ptrs([m for _, m in batch]), *outs, scratch.data_ptr(),
+        scratch.numel()))
+
+
 def segmented_scan(offsets: torch.Tensor, nrows: int,
                    columns: Sequence[Tuple[int, Optional[torch.Tensor], Optional[torch.Tensor]]]
                    ) -> List[Tuple[Optional[torch.Tensor], torch.Tensor]]:
@@ -413,32 +480,10 @@ def segmented_scan(offsets: torch.Tensor, nrows: int,
     ``AGG_COUNT``).  Returns per scan ``(running op over the valid rows or None for COUNT, running count of
     the valid rows)``; up to ``SCAN_MAX_COLS`` scans share one launch sequence."""
     lib = _lib.load()
-    assert offsets.dtype == torch.int64 and offsets.is_cuda and offsets.is_contiguous()
-    dev = offsets.device
-    nseg = int(offsets.shape[0]) - 1
-    res: List[Tuple[Optional[torch.Tensor], torch.Tensor]] = []
-    for b in range(0, len(columns), SCAN_MAX_COLS):
-        batch = columns[b:b + SCAN_MAX_COLS]
-        outs, cnts = [], []
-        for op, v, m in batch:
-            assert (v is None) == (op == AGG_COUNT)
-            if v is not None:
-                assert v.element_size() == 8 and v.device == dev and v.is_contiguous() and v.shape[0] == nrows
-            if m is not None:
-                assert m.dtype == torch.uint8 and m.device == dev and m.is_contiguous() and m.shape[0] == nrows
-            outs.append(None if v is None else torch.empty_like(v))
-            cnts.append(torch.empty(nrows, dtype=torch.int64, device=dev))
-        nb = int(lib.fb_segmented_scan_scratch_bytes(nrows, len(batch)))
-        scratch = torch.empty(max(nb, 8), dtype=torch.uint8, device=dev)
-        _lib.check(lib.fb_segmented_scan(
-            dev.index, _stream_ptr(dev), nrows, nseg, offsets.data_ptr(), len(batch),
-            _lib.i32_array([op for op, _, _ in batch]),
-            _lib.ptr_array([0 if v is None else v.data_ptr() for _, v, _ in batch]),
-            _lib.ptr_array([0 if m is None else m.data_ptr() for _, _, m in batch]),
-            _lib.ptr_array([0 if o is None else o.data_ptr() for o in outs]),
-            _lib.ptr_array([c.data_ptr() for c in cnts]), scratch.data_ptr(), scratch.numel()))
-        res.extend(zip(outs, cnts))
-    return res
+    dev, nseg = _segments(offsets)
+    return _op_batched(columns, nrows, dev, lambda n: lib.fb_segmented_scan_scratch_bytes(nrows, n),
+                       lambda *args: lib.fb_segmented_scan(dev.index, _stream_ptr(dev), nrows, nseg,
+                                                           offsets.data_ptr(), *args))
 
 
 def segmented_moments(offsets: torch.Tensor, nrows: int,
@@ -449,29 +494,10 @@ def segmented_moments(offsets: torch.Tensor, nrows: int,
     (int64), running M2 = sum of (x - mean)^2 over them (float64, 0 where the count is 0))``; up to
     ``SCAN_MAX_COLS`` columns share one launch sequence."""
     lib = _lib.load()
-    assert offsets.dtype == torch.int64 and offsets.is_cuda and offsets.is_contiguous()
-    dev = offsets.device
-    nseg = int(offsets.shape[0]) - 1
-    res: List[Tuple[torch.Tensor, torch.Tensor]] = []
-    for b in range(0, len(columns), SCAN_MAX_COLS):
-        batch = columns[b:b + SCAN_MAX_COLS]
-        cnts, m2s = [], []
-        for v, m in batch:
-            assert v.dtype == torch.float64 and v.device == dev and v.is_contiguous() and v.shape[0] == nrows
-            if m is not None:
-                assert m.dtype == torch.uint8 and m.device == dev and m.is_contiguous() and m.shape[0] == nrows
-            cnts.append(torch.empty(nrows, dtype=torch.int64, device=dev))
-            m2s.append(torch.empty(nrows, dtype=torch.float64, device=dev))
-        nb = int(lib.fb_segmented_moments_scratch_bytes(nrows, len(batch)))
-        scratch = torch.empty(max(nb, 8), dtype=torch.uint8, device=dev)
-        _lib.check(lib.fb_segmented_moments(
-            dev.index, _stream_ptr(dev), nrows, nseg, offsets.data_ptr(), len(batch),
-            _lib.ptr_array([v.data_ptr() for v, _ in batch]),
-            _lib.ptr_array([0 if m is None else m.data_ptr() for _, m in batch]),
-            _lib.ptr_array([c.data_ptr() for c in cnts]), _lib.ptr_array([q.data_ptr() for q in m2s]),
-            scratch.data_ptr(), scratch.numel()))
-        res.extend(zip(cnts, m2s))
-    return res
+    dev, nseg = _segments(offsets)
+    return _value_batched(columns, nrows, dev, 1, lambda n: lib.fb_segmented_moments_scratch_bytes(nrows, n),
+                          lambda *args: lib.fb_segmented_moments(dev.index, _stream_ptr(dev), nrows, nseg,
+                                                                 offsets.data_ptr(), *args))
 
 
 def segmented_shape_moments(offsets: torch.Tensor, nrows: int,
@@ -482,29 +508,10 @@ def segmented_shape_moments(offsets: torch.Tensor, nrows: int,
     M2, M3, M4)``, Mk = sum of (x - mean)^k over them (float64, 0 where the count is 0); up to ``SCAN_MAX_COLS``
     columns share one launch sequence."""
     lib = _lib.load()
-    assert offsets.dtype == torch.int64 and offsets.is_cuda and offsets.is_contiguous()
-    dev = offsets.device
-    nseg = int(offsets.shape[0]) - 1
-    res: List[Tuple[torch.Tensor, torch.Tensor, torch.Tensor, torch.Tensor]] = []
-    for b in range(0, len(columns), SCAN_MAX_COLS):
-        batch = columns[b:b + SCAN_MAX_COLS]
-        outs = []
-        for v, m in batch:
-            assert v.dtype == torch.float64 and v.device == dev and v.is_contiguous() and v.shape[0] == nrows
-            if m is not None:
-                assert m.dtype == torch.uint8 and m.device == dev and m.is_contiguous() and m.shape[0] == nrows
-            outs.append((torch.empty(nrows, dtype=torch.int64, device=dev),)
-                        + tuple(torch.empty(nrows, dtype=torch.float64, device=dev) for _ in range(3)))
-        nb = int(lib.fb_segmented_shape_moments_scratch_bytes(nrows, len(batch)))
-        scratch = torch.empty(max(nb, 8), dtype=torch.uint8, device=dev)
-        _lib.check(lib.fb_segmented_shape_moments(
-            dev.index, _stream_ptr(dev), nrows, nseg, offsets.data_ptr(), len(batch),
-            _lib.ptr_array([v.data_ptr() for v, _ in batch]),
-            _lib.ptr_array([0 if m is None else m.data_ptr() for _, m in batch]),
-            *[_lib.ptr_array([o[i].data_ptr() for o in outs]) for i in range(4)],
-            scratch.data_ptr(), scratch.numel()))
-        res.extend(outs)
-    return res
+    dev, nseg = _segments(offsets)
+    return _value_batched(columns, nrows, dev, 3, lambda n: lib.fb_segmented_shape_moments_scratch_bytes(nrows, n),
+                          lambda *args: lib.fb_segmented_shape_moments(dev.index, _stream_ptr(dev), nrows, nseg,
+                                                                       offsets.data_ptr(), *args))
 
 
 def segmented_comoments(offsets: torch.Tensor, nrows: int,
@@ -515,34 +522,21 @@ def segmented_comoments(offsets: torch.Tensor, nrows: int,
     where both are valid.  Returns per pair ``(count (int64), mean x, mean y, Sxx, Syy, Sxy)`` of those rows up to
     each row (float64, 0 where the count is 0); up to ``SCAN_MAX_COLS`` pairs share one launch sequence."""
     lib = _lib.load()
-    assert offsets.dtype == torch.int64 and offsets.is_cuda and offsets.is_contiguous()
-    dev = offsets.device
-    nseg = int(offsets.shape[0]) - 1
-    res: List[Tuple[torch.Tensor, ...]] = []
-    for b in range(0, len(pairs), SCAN_MAX_COLS):
-        batch = pairs[b:b + SCAN_MAX_COLS]
-        outs = []
-        for x, mx, y, my in batch:
-            for v in (x, y):
-                assert v.dtype == torch.float64 and v.device == dev and v.is_contiguous() and v.shape[0] == nrows
-            for m in (mx, my):
-                if m is not None:
-                    assert m.dtype == torch.uint8 and m.device == dev and m.is_contiguous() and m.shape[0] == nrows
-            outs.append((torch.empty(nrows, dtype=torch.int64, device=dev),)
-                        + tuple(torch.empty(nrows, dtype=torch.float64, device=dev) for _ in range(5)))
-        nb = int(lib.fb_segmented_comoments_scratch_bytes(nrows, len(batch)))
-        scratch = torch.empty(max(nb, 8), dtype=torch.uint8, device=dev)
+    dev, nseg = _segments(offsets)
 
-        def ptrs(ts: Sequence[Optional[torch.Tensor]]) -> Any:
-            return _lib.ptr_array([0 if t is None else t.data_ptr() for t in ts])
+    def outputs(x: torch.Tensor, mx: Optional[torch.Tensor], y: torch.Tensor,
+                my: Optional[torch.Tensor]) -> Tuple[torch.Tensor, ...]:
+        for v in (x, y):
+            _check_rows(v, dev, nrows, torch.float64)
+        for m in (mx, my):
+            _check_rows(m, dev, nrows, torch.uint8)
+        return _stat_outputs(dev, nrows, 5)
 
-        _lib.check(lib.fb_segmented_comoments(
-            dev.index, _stream_ptr(dev), nrows, nseg, offsets.data_ptr(), len(batch),
-            ptrs([p[0] for p in batch]), ptrs([p[1] for p in batch]), ptrs([p[2] for p in batch]),
-            ptrs([p[3] for p in batch]), *[ptrs([o[i] for o in outs]) for i in range(6)],
-            scratch.data_ptr(), scratch.numel()))
-        res.extend(outs)
-    return res
+    return _batched(pairs, dev, outputs, lambda n: lib.fb_segmented_comoments_scratch_bytes(nrows, n),
+                    lambda batch, outs, scratch: lib.fb_segmented_comoments(
+                        dev.index, _stream_ptr(dev), nrows, nseg, offsets.data_ptr(), len(batch),
+                        *[_ptrs([p[i] for p in batch]) for i in range(4)], *outs, scratch.data_ptr(),
+                        scratch.numel()))
 
 
 FRAME_TILE_MAX_WIDTH = 1024   # FB_FRAME_TILE_MAX_WIDTH: widest frame of the one-pass kernel
@@ -558,9 +552,7 @@ def window_frame(offsets: torch.Tensor, nrows: int, start: Optional[int], end: O
     their count, 0 where the count is 0.  ``columns`` and the result are shaped as in
     :func:`segmented_scan`; up to ``SCAN_MAX_COLS`` columns share one launch sequence."""
     lib = _lib.load()
-    assert offsets.dtype == torch.int64 and offsets.is_cuda and offsets.is_contiguous()
-    dev = offsets.device
-    nseg = int(offsets.shape[0]) - 1
+    dev, nseg = _segments(offsets)
     # a bound past every segment is unbounded: exact, as no segment is longer than the table
     if start is not None and start <= -nrows:
         start = None
@@ -568,29 +560,9 @@ def window_frame(offsets: torch.Tensor, nrows: int, start: Optional[int], end: O
         end = None
     flags = (FRAME_UNBOUNDED_START if start is None else 0) | (FRAME_UNBOUNDED_END if end is None else 0)
     s, e = (0 if start is None else start), (0 if end is None else end)
-    res: List[Tuple[Optional[torch.Tensor], torch.Tensor]] = []
-    for b in range(0, len(columns), SCAN_MAX_COLS):
-        batch = columns[b:b + SCAN_MAX_COLS]
-        outs, cnts = [], []
-        for op, v, m in batch:
-            assert (v is None) == (op == AGG_COUNT)
-            if v is not None:
-                assert v.element_size() == 8 and v.device == dev and v.is_contiguous() and v.shape[0] == nrows
-            if m is not None:
-                assert m.dtype == torch.uint8 and m.device == dev and m.is_contiguous() and m.shape[0] == nrows
-            outs.append(None if v is None else torch.empty_like(v))
-            cnts.append(torch.empty(nrows, dtype=torch.int64, device=dev))
-        nb = int(lib.fb_window_frame_scratch_bytes(nrows, len(batch), s, e, flags))
-        scratch = torch.empty(max(nb, 8), dtype=torch.uint8, device=dev)
-        _lib.check(lib.fb_window_frame(
-            dev.index, _stream_ptr(dev), nrows, nseg, offsets.data_ptr(), s, e, flags, len(batch),
-            _lib.i32_array([op for op, _, _ in batch]),
-            _lib.ptr_array([0 if v is None else v.data_ptr() for _, v, _ in batch]),
-            _lib.ptr_array([0 if m is None else m.data_ptr() for _, _, m in batch]),
-            _lib.ptr_array([0 if o is None else o.data_ptr() for o in outs]),
-            _lib.ptr_array([c.data_ptr() for c in cnts]), scratch.data_ptr(), scratch.numel()))
-        res.extend(zip(outs, cnts))
-    return res
+    return _op_batched(columns, nrows, dev, lambda n: lib.fb_window_frame_scratch_bytes(nrows, n, s, e, flags),
+                       lambda *args: lib.fb_window_frame(dev.index, _stream_ptr(dev), nrows, nseg, offsets.data_ptr(),
+                                                         s, e, flags, *args))
 
 
 RANGE_KEY_I64 = 0   # FB_RANGE_KEY_*: how fb_window_range_bounds reads the 8-byte presort key
@@ -645,29 +617,9 @@ def window_bounded(lo: torch.Tensor, hi: torch.Tensor,
     nrows = int(lo.shape[0])
     for b_ in (lo, hi):
         assert b_.dtype == torch.int64 and b_.is_cuda and b_.is_contiguous() and b_.shape[0] == nrows
-    res: List[Tuple[Optional[torch.Tensor], torch.Tensor]] = []
-    for b in range(0, len(columns), SCAN_MAX_COLS):
-        batch = columns[b:b + SCAN_MAX_COLS]
-        outs, cnts = [], []
-        for op, v, m in batch:
-            assert (v is None) == (op == AGG_COUNT)
-            if v is not None:
-                assert v.element_size() == 8 and v.device == dev and v.is_contiguous() and v.shape[0] == nrows
-            if m is not None:
-                assert m.dtype == torch.uint8 and m.device == dev and m.is_contiguous() and m.shape[0] == nrows
-            outs.append(None if v is None else torch.empty_like(v))
-            cnts.append(torch.empty(nrows, dtype=torch.int64, device=dev))
-        nb = int(lib.fb_window_bounded_scratch_bytes(nrows, len(batch)))
-        scratch = torch.empty(max(nb, 8), dtype=torch.uint8, device=dev)
-        _lib.check(lib.fb_window_bounded(
-            dev.index, _stream_ptr(dev), nrows, lo.data_ptr(), hi.data_ptr(), len(batch),
-            _lib.i32_array([op for op, _, _ in batch]),
-            _lib.ptr_array([0 if v is None else v.data_ptr() for _, v, _ in batch]),
-            _lib.ptr_array([0 if m is None else m.data_ptr() for _, _, m in batch]),
-            _lib.ptr_array([0 if o is None else o.data_ptr() for o in outs]),
-            _lib.ptr_array([c.data_ptr() for c in cnts]), scratch.data_ptr(), scratch.numel()))
-        res.extend(zip(outs, cnts))
-    return res
+    return _op_batched(columns, nrows, dev, lambda n: lib.fb_window_bounded_scratch_bytes(nrows, n),
+                       lambda *args: lib.fb_window_bounded(dev.index, _stream_ptr(dev), nrows, lo.data_ptr(),
+                                                           hi.data_ptr(), *args))
 
 
 QUANTILE_TILE_ROWS = 2048   # FB_QUANTILE_TILE_ROWS: longest segment of the one-pass shared-memory path

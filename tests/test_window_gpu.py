@@ -25,7 +25,7 @@ from oracle import window as W
 DEV = torch.device("cuda", 0)
 OPS = {"SUM_I64": K.AGG_SUM_I64, "SUM_F64": K.AGG_SUM_F64, "MIN_I64": K.AGG_MIN_I64, "MAX_I64": K.AGG_MAX_I64,
        "MIN_F64": K.AGG_MIN_F64, "MAX_F64": K.AGG_MAX_F64, "COUNT": K.AGG_COUNT}
-TILE = 2048  # rows per CTA of fb_segscan_tile_kernel; 1024 * TILE rows fill one pass of the carry kernel
+TILE = 2048  # rows per CTA of fb_segscan_tile_kernel<OpScan, ...>; 1024 * TILE rows fill one pass of the carry kernel
 
 
 def _offsets(n: int, shape: str, rng) -> np.ndarray:

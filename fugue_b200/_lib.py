@@ -34,6 +34,22 @@ class MapUnit(C.Structure):
                 ("b", C.c_uint64), ("c", C.c_uint64)]
 
 
+REGEX_MAX_STATES, REGEX_MAX_RANGES, REGEX_MAX_SLOTS, REGEX_MAX_REWRITE = 64, 512, 8, 512
+REGEX_MAX_CLOSURES = 2 * (REGEX_MAX_STATES + 2)
+REGEX_MAX_ENTRIES = REGEX_MAX_CLOSURES * (REGEX_MAX_STATES + 1)
+
+
+class RegexProgram(C.Structure):
+    """``fb_regex_program`` of include/fugue_b200.h (K15)."""
+    _fields_ = [("npos", C.c_int32), ("nranges", C.c_int32), ("nslots", C.c_int32), ("op", C.c_int32),
+                ("group_pair", C.c_int32), ("nrewrite", C.c_int32), ("restart", C.c_int32), ("reserved", C.c_int32),
+                ("ascii", C.c_uint64 * 128), ("range_mask", C.c_uint64 * REGEX_MAX_RANGES),
+                ("range_lo", C.c_uint32 * REGEX_MAX_RANGES), ("cl_mask", C.c_uint64 * REGEX_MAX_CLOSURES),
+                ("cl_accept", C.c_uint8 * REGEX_MAX_CLOSURES), ("cl_off", C.c_uint16 * (REGEX_MAX_CLOSURES + 1)),
+                ("ent_target", C.c_uint8 * REGEX_MAX_ENTRIES), ("ent_save", C.c_uint8 * REGEX_MAX_ENTRIES),
+                ("rewrite", C.c_int16 * REGEX_MAX_REWRITE)]
+
+
 _vp = C.c_void_p
 _i32p = C.POINTER(C.c_int32)
 _vpp = C.POINTER(C.c_void_p)
@@ -133,6 +149,9 @@ SIGNATURES = {
     "fb_debug_string_parse_host": (C.c_int, [C.c_int64, _vp, _vp, _vp, C.c_int, _vp, _vp, _vp]),
     "fb_value_format": (C.c_int, [C.c_int, _vp, C.c_int64, _vp, _vp, C.c_int, _vp, _vp, _vp]),
     "fb_debug_value_format_host": (C.c_int, [C.c_int64, _vp, _vp, C.c_int, _vp, _vp, _vp]),
+    "fb_regex_match": (C.c_int, [C.c_int, _vp, C.c_int64, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "fb_regex_transform": (C.c_int, [C.c_int, _vp, C.c_int64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "fb_debug_regex_host": (C.c_int, [C.c_int64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
 }
 
 

@@ -107,7 +107,11 @@ TEMPORAL_FUNCTIONS = frozenset(["EXTRACT", "DATE_TRUNC", "DATEDIFF", "ADD_MONTHS
 FLOAT_FUNCTIONS = frozenset(["SQRT", "EXP", "LN", "LOG10", "POWER", "POW"])  # always float64
 ROUND_MAX_DIGITS = 18
 # functions that build a string from one string expression and literals (SUBSTRING is SUBSTR); ``||`` too
-STRING_FUNCTIONS = frozenset(["UPPER", "LOWER", "SUBSTR", "SUBSTRING", "TRIM", "LTRIM", "RTRIM", "REPLACE", "CONCAT"])
+STRING_FUNCTIONS = frozenset(["UPPER", "LOWER", "SUBSTR", "SUBSTRING", "TRIM", "LTRIM", "RTRIM", "REPLACE", "CONCAT",
+                              "REGEXP_EXTRACT", "REGEXP_REPLACE"])
+# regular-expression tests of one string expression: bool
+REGEX_PREDICATES = frozenset(["REGEXP_MATCHES", "REGEXP_FULL_MATCH"])
+REGEX_FUNCTIONS = REGEX_PREDICATES | {"REGEXP_EXTRACT", "REGEXP_REPLACE"}
 
 
 def result_type(head: str, arg_type: Optional[pa.DataType]) -> Optional[pa.DataType]:
@@ -286,6 +290,8 @@ class ColumnExpr:
             return result_type(self.head, self.args[0].infer_type(schema))
         if k == Kind.CALL and self.head in ("LIKE", "LENGTH"):
             return pa.bool_() if self.head == "LIKE" else pa.int64()
+        if k == Kind.CALL and self.head.upper() in REGEX_PREDICATES:
+            return pa.bool_()
         if k == Kind.CALL and self.head.upper() in STRING_FUNCTIONS:
             return pa.string()
         if k == Kind.CALL and self.head.upper() in FLOAT_FUNCTIONS:
@@ -366,6 +372,10 @@ class ColumnExpr:
                 i += 1
         args = [self, lit(pattern)] + ([] if escape is None else [lit(escape)])
         return ColumnExpr(Kind.CALL, "LIKE", args)
+
+    def rlike(self, pattern: Any) -> "ColumnExpr":
+        """SQL ``self RLIKE pattern``: ``functions.regexp_matches(self, pattern)``."""
+        return functions.regexp_matches(self, pattern)
 
     def over(self, running: bool = False, rows: Optional[Tuple[Optional[int], Optional[int]]] = None,
              range: Optional[Tuple[Any, Any]] = None) -> "ColumnExpr":  # noqa: A002 - the SQL word
@@ -826,6 +836,63 @@ class functions:
         return ColumnExpr(Kind.CALL, "REPLACE", [col(c), _str_arg("REPLACE", "from", from_), _str_arg("REPLACE", "to", to)])
 
     @staticmethod
+    def regexp_matches(c: Any, pattern: Any) -> ColumnExpr:
+        """DuckDB ``REGEXP_MATCHES(c, pattern)``: whether the regular expression matches somewhere in the string
+        (RE2 semantics, the subset of ``fugue_b200.regex``).  ``pattern`` is a string literal; NULL gives NULL."""
+        from . import regex
+
+        p = _str_arg("REGEXP_MATCHES", "pattern", pattern)
+        if p.value is not None:
+            regex.parse(p.value)
+        return ColumnExpr(Kind.CALL, "REGEXP_MATCHES", [col(c), p])
+
+    @staticmethod
+    def regexp_full_match(c: Any, pattern: Any) -> ColumnExpr:
+        """DuckDB ``REGEXP_FULL_MATCH(c, pattern)``: whether the regular expression matches the whole string."""
+        from . import regex
+
+        p = _str_arg("REGEXP_FULL_MATCH", "pattern", pattern)
+        if p.value is not None:
+            regex.parse(p.value)
+        return ColumnExpr(Kind.CALL, "REGEXP_FULL_MATCH", [col(c), p])
+
+    @staticmethod
+    def regexp_extract(c: Any, pattern: Any, group: Any = 0) -> ColumnExpr:
+        """DuckDB ``REGEXP_EXTRACT(c, pattern[, group])``: the text of group ``group`` (0, the default: the whole
+        match) of the leftmost match; '' when nothing matches or the group took no part.  A group above the
+        pattern's group count is a ValueError."""
+        from . import regex
+
+        p = _str_arg("REGEXP_EXTRACT", "pattern", pattern)
+        g = _int_arg("REGEXP_EXTRACT", "group", group)
+        if p.value is not None:
+            regex.parse(p.value)
+            if g.value is not None:
+                regex.check_group(p.value, g.value)
+        return ColumnExpr(Kind.CALL, "REGEXP_EXTRACT", [col(c), p] + ([] if g.value == 0 else [g]))
+
+    @staticmethod
+    def regexp_replace(c: Any, pattern: Any, rewrite: Any, options: Any = None) -> ColumnExpr:
+        """DuckDB ``REGEXP_REPLACE(c, pattern, rewrite[, options])``: the first match replaced by ``rewrite``, or
+        every non-overlapping match with ``options='g'``.  In ``rewrite``, ``\\0`` .. ``\\9`` are groups and
+        ``\\\\`` is a backslash."""
+        from . import regex
+
+        p = _str_arg("REGEXP_REPLACE", "pattern", pattern)
+        r = _str_arg("REGEXP_REPLACE", "rewrite", rewrite)
+        args = [col(c), p, r]
+        if options is not None:
+            o = _str_arg("REGEXP_REPLACE", "options", options)
+            if o.value is not None:
+                regex.replace_options(o.value)
+            args.append(o)
+        if p.value is not None:
+            regex.parse(p.value)
+            if r.value is not None:
+                regex.rewrite_tokens(p.value, r.value)
+        return ColumnExpr(Kind.CALL, "REGEXP_REPLACE", args)
+
+    @staticmethod
     def concat(*parts: Any) -> ColumnExpr:
         """SQLite ``CONCAT(a, ...)``: the parts joined; NULL parts are skipped (``CONCAT(NULL)`` is '')."""
         if not parts:
@@ -1186,6 +1253,12 @@ def to_sql(expr: ColumnExpr, enable_cast: bool = True, nested: bool = False) -> 
             body += " ESCAPE " + to_sql(expr.args[2], enable_cast)
         if nested:
             body = "(" + body + ")"
+    elif k == Kind.CALL and expr.head.upper() in REGEX_FUNCTIONS:
+        # the SQL parser reads a regular expression's string literals as written: only '' is a quote
+        parts = [to_sql(expr.args[0], enable_cast)] + [
+            "'" + x.value.replace("'", "''") + "'" if x.kind == Kind.LITERAL and isinstance(x.value, str)
+            and x.as_type is None else to_sql(_operand(x), enable_cast) for x in expr.args[1:]]
+        body = f"{expr.head.upper()}({','.join(parts)})"
     elif k == Kind.CALL and expr.head.upper() in ("EXTRACT", "DATE_TRUNC", "DATEDIFF") and \
             isinstance(expr.kwargs.get("field" if expr.head.upper() == "EXTRACT" else "part"), str):
         inner = ", ".join(to_sql(_operand(x), enable_cast) for x in expr.args)

@@ -40,7 +40,7 @@ import torch
 
 from . import kernels as K
 from . import strings as ST
-from .column import (FLOAT_FUNCTIONS, ROUND_MAX_DIGITS, TEMPORAL_LITERALS, TIME_FIELDS, TIME_PARTS, ColumnExpr, Kind,
+from .column import (FLOAT_FUNCTIONS, REGEX_PREDICATES, ROUND_MAX_DIGITS, TEMPORAL_LITERALS, TIME_FIELDS, TIME_PARTS, ColumnExpr, Kind,
                      case_string_results, col as _col, is_string_build, lit as _lit)
 from .schema import Schema
 from .table import B200Table, _storage_dtype, expr_type
@@ -142,6 +142,16 @@ def string_literal_cast(e: ColumnExpr) -> ColumnExpr:
 
 class _OutOfResources(Exception):
     pass
+
+
+def _regex_pattern(e: ColumnExpr, fn: str) -> Optional[str]:
+    """The pattern of REGEXP_MATCHES / REGEXP_FULL_MATCH (None: a NULL literal, so the result is NULL)."""
+    if len(e.args) != 2:
+        raise ValueError(f"{fn} takes 2 arguments: {e}")
+    p = e.args[1]
+    if p.kind != Kind.LITERAL or p.as_type is not None or not (p.value is None or isinstance(p.value, str)):
+        raise NotImplementedError(f"{fn} needs a string literal pattern: {e}")
+    return p.value
 
 
 def _lower(e: ColumnExpr) -> Optional[ColumnExpr]:
@@ -592,7 +602,7 @@ class _Program:
                 return self._temporal_function(e, fn)
             if fn == "COALESCE":
                 return self._coalesce(e)
-            if fn in ("LIKE", "LENGTH"):
+            if fn in ("LIKE", "LENGTH") or fn in REGEX_PREDICATES:
                 return self._string_function(e, fn)
             if fn == "CASE":
                 return self._case(e)
@@ -717,12 +727,19 @@ class _Program:
                 and _is_str(t.schema[s.name].type)):
             raise NotImplementedError(f"{fn} needs a string column as its operand: {e}")
         d = t.dictionaries[s.name]
-        if fn == "LIKE":
+        if fn in REGEX_PREDICATES:
+            pattern = _regex_pattern(e, fn)
+            if pattern is None:
+                return self._node(_lit(None))
+            key: Any = ("REGEX", s.name, pattern, fn == "REGEXP_FULL_MATCH")
+            if key not in self.tables:
+                self.tables[key] = ST.regex_table(d, t.device, pattern, key[3])
+        elif fn == "LIKE":
             lits = e.args[1:]
             if not (1 <= len(lits) <= 2 and all(a.kind == Kind.LITERAL and isinstance(a.value, str) for a in lits)):
                 raise NotImplementedError(f"LIKE needs a string literal pattern: {e}")
             pattern, escape = lits[0].value, (lits[1].value if len(lits) > 1 else None)
-            key: Any = ("LIKE", s.name, pattern, escape)
+            key = ("LIKE", s.name, pattern, escape)
             if key not in self.tables:
                 self.tables[key] = ST.like_table(d, t.device, pattern, escape)
         else:
@@ -734,11 +751,15 @@ class _Program:
         ci = t.schema.index_of_key(s.name)
         self.emit(K.X_MOV, K.XK_COL, self.col_slot(ci))
         self.emit(K.X_LOOKUP, K.XK_COL, self.col_slot(key), 0, len(d))
-        return ("b" if fn == "LIKE" else "i"), t.valid[ci] is not None or self.tables[key][1] is not None
+        return ("i" if fn == "LENGTH" else "b"), t.valid[ci] is not None or self.tables[key][1] is not None
 
     def _string_function_of_expr(self, e: ColumnExpr, fn: str, s: ColumnExpr) -> Tuple[str, bool]:
         t = self.t
-        if fn == "LIKE":
+        if fn in REGEX_PREDICATES:
+            pattern = _regex_pattern(e, fn)
+            if pattern is None:
+                return self._node(_lit(None))
+        elif fn == "LIKE":
             lits = e.args[1:]
             if not (1 <= len(lits) <= 2 and all(a.kind == Kind.LITERAL and isinstance(a.value, str) for a in lits)):
                 raise NotImplementedError(f"LIKE needs a string literal pattern: {e}")
@@ -746,9 +767,13 @@ class _Program:
             raise ValueError(f"LENGTH takes one argument: {e}")
         d, nullable = self.string_codes(s)
         name, steps = ST.string_chain(s, t.dictionaries)
-        if fn == "LIKE":
+        if fn in REGEX_PREDICATES:
+            key: Any = ("REGEX", ("STR", name, steps), pattern, fn == "REGEXP_FULL_MATCH")
+            if key not in self.tables:
+                self.tables[key] = ST.regex_table(d, t.device, pattern, key[3])
+        elif fn == "LIKE":
             pattern, escape = lits[0].value, (lits[1].value if len(lits) > 1 else None)
-            key: Any = ("LIKE", ("STR", name, steps), pattern, escape)
+            key = ("LIKE", ("STR", name, steps), pattern, escape)
             if key not in self.tables:
                 self.tables[key] = ST.like_table(d, t.device, pattern, escape)
         else:
@@ -759,7 +784,7 @@ class _Program:
             self.tables[key] = (torch.zeros(1, dtype=torch.int64, device=t.device),
                                 torch.zeros(1, dtype=torch.uint8, device=t.device))
         self.emit(K.X_LOOKUP, K.XK_COL, self.col_slot(key), 0, len(d))
-        return ("b" if fn == "LIKE" else "i"), nullable or self.tables[key][1] is not None
+        return ("i" if fn == "LENGTH" else "b"), nullable or self.tables[key][1] is not None
 
     def _coalesce(self, e: ColumnExpr) -> Tuple[str, bool]:
         args = [a if isinstance(a, ColumnExpr) else _lit(a) for a in e.args]
@@ -922,7 +947,7 @@ class _Program:
         if e.kind == Kind.CALL and e.func.upper() == "COALESCE":
             cs = [self._static_cls(a if isinstance(a, ColumnExpr) else _lit(a)) for a in e.args]
             return "f" if "f" in cs else ("b" if "b" in cs and all(c in ("b", "n") for c in cs) else "i")
-        if e.kind == Kind.CALL and e.func.upper() == "LIKE":
+        if e.kind == Kind.CALL and (e.func.upper() == "LIKE" or e.func.upper() in REGEX_PREDICATES):
             return "b"
         if e.kind == Kind.CALL and e.func.upper() in FLOAT_FUNCTIONS:
             return "f"

@@ -1046,6 +1046,70 @@ def string_first_equal(offsets: torch.Tensor, data: torch.Tensor, valid: Optiona
     return out
 
 
+# ---- K15: regular expressions over a dictionary's entries ---------------------------------------
+def _program_on(prog: Any, dev: torch.device) -> torch.Tensor:
+    return torch.frombuffer(bytearray(bytes(prog)), dtype=torch.uint8).to(dev)
+
+
+def regex_match(offsets: torch.Tensor, data: torch.Tensor, valid: Optional[torch.Tensor], prog: Any
+                ) -> Tuple[torch.Tensor, torch.Tensor]:
+    """(match, validity) of every entry, uint8 each, for a ``regex.match_program``."""
+    lib = _lib.load()
+    dev = offsets.device
+    n = int(offsets.shape[0]) - 1
+    out = torch.empty(n, dtype=torch.uint8, device=dev)
+    out_valid = torch.empty(n, dtype=torch.uint8, device=dev)
+    dprog = _program_on(prog, dev)
+    _lib.check(lib.fb_regex_match(dev.index, _stream_ptr(dev), n, offsets.data_ptr(), data.data_ptr(),
+                                  0 if valid is None else valid.data_ptr(), C.addressof(prog), dprog.data_ptr(),
+                                  out.data_ptr(), out_valid.data_ptr()))
+    return out, out_valid
+
+
+def regex_transform(offsets: torch.Tensor, data: torch.Tensor, valid: Optional[torch.Tensor], prog: Any,
+                    out_offsets: Optional[torch.Tensor] = None, out_data: Optional[torch.Tensor] = None
+                    ) -> Tuple[Optional[torch.Tensor], Optional[torch.Tensor]]:
+    """One ``fb_regex_transform`` call (``regex.extract_program`` / ``replace_program``) with the measure / write
+    contract of ``string_transform``."""
+    lib = _lib.load()
+    dev = offsets.device
+    n = int(offsets.shape[0]) - 1
+    out_len = out_valid = None
+    if out_data is None:
+        out_len = torch.empty(n, dtype=torch.int64, device=dev)
+        out_valid = torch.empty(n, dtype=torch.uint8, device=dev)
+    dprog = _program_on(prog, dev)
+    _lib.check(lib.fb_regex_transform(
+        dev.index, _stream_ptr(dev), n, offsets.data_ptr(), data.data_ptr(), 0 if valid is None else valid.data_ptr(),
+        C.addressof(prog), dprog.data_ptr(), 0 if out_len is None else out_len.data_ptr(),
+        0 if out_valid is None else out_valid.data_ptr(), 0 if out_offsets is None else out_offsets.data_ptr(),
+        0 if out_data is None else out_data.data_ptr()))
+    return out_len, out_valid
+
+
+def regex_host(offsets: np.ndarray, data: np.ndarray, valid: Optional[np.ndarray], prog: Any
+               ) -> Tuple[np.ndarray, np.ndarray, Optional[np.ndarray]]:
+    """Either regex call on the CPU over host arrays (int64 ``offsets``, uint8 ``data`` / ``valid``), by the same
+    per-entry code as the kernels: (0 / 1 match or byte length per entry (int64), validity, result offsets and
+    bytes as one (offsets, data) pair, None for a match program)."""
+    lib = _lib.load()
+    n = int(offsets.shape[0]) - 1
+    data = data if data.size else np.zeros(1, dtype=np.uint8)
+    out = np.zeros(max(n, 1), dtype=np.int64)
+    out_valid = np.zeros(max(n, 1), dtype=np.uint8)
+    vp = 0 if valid is None else valid.ctypes.data
+    _lib.check(lib.fb_debug_regex_host(n, offsets.ctypes.data, data.ctypes.data, vp, C.addressof(prog),
+                                       out.ctypes.data, out_valid.ctypes.data, 0, 0))
+    if prog.op == 0:
+        return out[:n], out_valid[:n], None
+    offs = np.zeros(n + 1, dtype=np.int64)
+    np.cumsum(out[:n], out=offs[1:])
+    buf = np.zeros(max(int(offs[-1]), 1), dtype=np.uint8)
+    _lib.check(lib.fb_debug_regex_host(n, offsets.ctypes.data, data.ctypes.data, vp, C.addressof(prog),
+                                       0, 0, offs.ctypes.data, buf.ctypes.data))
+    return out[:n], out_valid[:n], (offs, buf)
+
+
 # ---- K13: string casts over a dictionary's entries ----------------------------------------------
 (PARSE_I8, PARSE_I16, PARSE_I32, PARSE_I64, PARSE_U8, PARSE_U16, PARSE_U32, PARSE_U64, PARSE_F32, PARSE_F64,
  PARSE_BOOL, PARSE_DATE32, PARSE_DATE64) = range(13)

@@ -23,6 +23,8 @@ GREATEST, LEAST, LENGTH, UPPER, LOWER, SUBSTR / SUBSTRING, TRIM, LTRIM, RTRIM, R
 DATE '..' / TIMESTAMP '..' / INTERVAL '..' DAY | HOUR | MINUTE | SECOND | DAY TO SECOND literals, x + INTERVAL 'n' MONTH | YEAR,
 EXTRACT(field FROM x), DATE_PART, YEAR MONTH DAY HOUR MINUTE SECOND QUARTER DAYOFWEEK DAYOFYEAR WEEK, DATE_TRUNC,
 DATEDIFF, ADD_MONTHS, literals, `quoted` and table-qualified names.
+Regular expressions: x [NOT] RLIKE 'p', REGEXP_MATCHES / REGEXP_LIKE, REGEXP_FULL_MATCH, REGEXP_EXTRACT,
+REGEXP_REPLACE; their string literals are read as written (a backslash is a backslash, '' a quote).
 Anything else raises NotImplementedError (there is no host SQL fallback in this package).
 """
 import datetime
@@ -331,6 +333,7 @@ _STRING_BUILDERS = {"UPPER": functions.upper, "LOWER": functions.lower, "SUBSTR"
                     "RTRIM": functions.rtrim, "REPLACE": functions.replace}
 _FIELD_FUNCS = {"YEAR": "year", "MONTH": "month", "DAY": "day", "HOUR": "hour", "MINUTE": "minute", "SECOND": "second",
                 "QUARTER": "quarter", "DAYOFWEEK": "dow", "DAYOFYEAR": "doy", "WEEK": "week"}
+_REGEX_CALLS = ("REGEXP_MATCHES", "REGEXP_LIKE", "REGEXP_FULL_MATCH", "REGEXP_EXTRACT", "REGEXP_REPLACE")
 _MONTHS = "INTERVAL_MONTHS"  # a calendar interval literal: only the operand of + / - next to a date or timestamp
 _TWO_ARGS = {"NULLIF": functions.nullif, "IFNULL": functions.coalesce, "MOD": lambda a, b: a % b,
              "POWER": functions.power, "POW": functions.power}
@@ -438,6 +441,12 @@ class _Parser:
                 e = ~self._in_or_between(e)
             elif self.at_kw("IN") or self.at_kw("BETWEEN"):
                 e = self._in_or_between(e)
+            elif self.at_kw("RLIKE") and self.peek(1)[0] == "str":
+                self.i += 1
+                e = e.rlike(self._raw_string())
+            elif self.at_kw("NOT") and self.peek(1)[1].upper() == "RLIKE" and self.peek(2)[0] == "str":
+                self.i += 2
+                e = ~e.rlike(self._raw_string())
             elif self.kw("NOT", "LIKE"):
                 e = ~self._like(e)
             elif self.kw("LIKE"):
@@ -458,6 +467,33 @@ class _Parser:
             raise NotImplementedError(f"{what} takes a string literal, got {val!r} in: {self.sql}")
         self.i += 1
         return _unquote(val)
+
+    def _raw_string(self) -> str:
+        """A string literal as written, for a regular expression: only '' is resolved (to a quote), so a backslash
+        stays a backslash, as in DuckDB and Postgres."""
+        val = self.peek()[1]
+        self.i += 1
+        return val[1:-1].replace("''", "'")
+
+    def _regex_call(self, fn: str) -> ColumnExpr:
+        """``REGEXP_MATCHES / REGEXP_LIKE / REGEXP_FULL_MATCH / REGEXP_EXTRACT / REGEXP_REPLACE(s, 'p', ...)``; the
+        string literal arguments are read as written (``_raw_string``)."""
+        self.i += 2  # name (
+        args: List[Any] = [self.expr()]
+        while self.op(","):
+            args.append(self._raw_string() if self.peek()[0] == "str" else self.expr())
+        self.expect(")")
+        want = {"REGEXP_EXTRACT": (2, 3), "REGEXP_REPLACE": (3, 4)}.get(fn, (2, 2))
+        if not want[0] <= len(args) <= want[1]:
+            raise ValueError(f"{fn} takes {want[0] if want[0] == want[1] else f'{want[0]} to {want[1]}'} arguments, "
+                             f"got {len(args)} in: {self.sql}")
+        if fn in ("REGEXP_MATCHES", "REGEXP_LIKE"):
+            return functions.regexp_matches(*args)
+        if fn == "REGEXP_FULL_MATCH":
+            return functions.regexp_full_match(*args)
+        if fn == "REGEXP_EXTRACT":
+            return functions.regexp_extract(*args)
+        return functions.regexp_replace(*args)
 
     def _like(self, e: ColumnExpr) -> ColumnExpr:
         pattern = self._string_literal("LIKE")
@@ -573,6 +609,8 @@ class _Parser:
                     self.i += 1
                 self.expect(")")
                 return e.cast(_cast_type(tp))
+            if self.peek(1) == ("op", "(") and up in _REGEX_CALLS:
+                return self._regex_call(up)
             if self.peek(1) == ("op", "("):
                 return self._call(up)
             self.i += 1

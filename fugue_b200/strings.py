@@ -17,6 +17,9 @@ on the device (one measure and one write launch per step; intermediate dictionar
 deduplicates the results and returns the new dictionary and the entry -> new code table the rows are mapped
 through (``FB_X_LOOKUP``).  Results are cached per (dictionary object, chain) the same way as uploads.
 
+REGEXP_MATCHES / REGEXP_FULL_MATCH are per-entry tables as LIKE is (``regex_table``), and REGEXP_EXTRACT /
+REGEXP_REPLACE are chain steps (K15, ``fb_regex.cu``, compiled by ``regex.py``).
+
 A cast of a string to a number, bool, date or timestamp is a function of the entry as well (K13,
 ``fb_strparse.cu``): ``parse_table`` parses every entry once and returns the per-entry table ``FB_X_LOOKUP`` reads,
 cached per (dictionary object, device, target type).  The parse is Arrow's ``cast(safe=False)`` of the entry; the
@@ -35,6 +38,7 @@ import pyarrow as pa
 import torch
 
 from . import kernels as K
+from . import regex as R
 from .column import ColumnExpr, Kind, is_string_build, lit
 
 _CACHE: Dict[int, Tuple[Any, Dict[Any, Any]]] = {}     # dictionary -> {device: DeviceDictionary}
@@ -136,6 +140,26 @@ def like_table(d: pa.Array, device: torch.device, pattern: str, escape: Optional
     return out.to(torch.int64), (out_valid if dd.valid is not None else None)
 
 
+regex_matches = 0  # dictionaries tested against a regular expression so far (the regex cache's misses)
+
+
+def regex_table(d: pa.Array, device: torch.device, pattern: str, full: bool
+                ) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
+    """Per entry of ``d``: 1 where the regular expression ``pattern`` matches somewhere in it (``full``: matches
+    all of it), as the int64 table ``FB_X_LOOKUP`` reads, and the entry validity (None: no NULL entry).  Computed
+    on first use (K15), then cached on ``d``, so a repeated call launches nothing."""
+    global regex_matches
+    per = _slot(_DERIVED, d)
+    key = (("REGEX", pattern, full), device)
+    if key not in per:
+        prog = R.match_program(pattern, full)
+        regex_matches += 1
+        dd = device_dictionary(d, device)
+        out, out_valid = K.regex_match(dd.offsets, dd.data, dd.valid, prog)
+        per[key] = (out.to(torch.int64), out_valid if dd.valid is not None else None)
+    return per[key]
+
+
 def length_table(d: pa.Array, device: torch.device) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
     """Per entry of ``d``: its number of code points (int64), and the entry validity (None: no NULL)."""
     dd = device_dictionary(d, device)
@@ -144,7 +168,8 @@ def length_table(d: pa.Array, device: torch.device) -> Tuple[torch.Tensor, Optio
 
 # ---- string-building functions ------------------------------------------------------------------------
 _ARITY = {"UPPER": (0, 0), "LOWER": (0, 0), "SUBSTR": (1, 2), "TRIM": (0, 1), "LTRIM": (0, 1), "RTRIM": (0, 1),
-          "REPLACE": (2, 2)}
+          "REPLACE": (2, 2), "REGEXP_EXTRACT": (1, 2), "REGEXP_REPLACE": (2, 3)}
+_ARG_TYPES = {"SUBSTR": (int, int), "REGEXP_EXTRACT": (str, int)}  # literal types after the string; else str
 
 
 def _literal(fn: str, e: ColumnExpr, want: type) -> Any:
@@ -180,7 +205,8 @@ def string_chain(e: ColumnExpr, string_columns: Any) -> Tuple[str, Tuple[Any, ..
     step first.  ``string_columns``: the names of the table's string columns.  A step is a hashable tuple:
     ``("UPPER",)``, ``("LOWER",)``, ``("SUBSTR", start, length or None)``, ``("TRIM" / "LTRIM" / "RTRIM",
     characters)``, ``("REPLACE", from, to)``, ``("FORMAT", tokens, null_is_empty)`` for CONCAT / ``||``, or
-    ``("NULL",)`` (a NULL literal argument: every result is NULL).  Literals are UTF-8 bytes.
+    ``("REGEXP_EXTRACT", pattern, group)``, ``("REGEXP_REPLACE", pattern, rewrite, global)`` or ``("NULL",)`` (a
+    NULL literal argument: every result is NULL).  Literals are UTF-8 bytes; regular expressions stay ``str``.
     Raises NotImplementedError for what the device does not evaluate (two different string operands, numbers
     in a concatenation, a non-literal argument, no string column) and ValueError for a wrong argument count
     or a literal of the wrong type."""
@@ -236,7 +262,7 @@ def string_chain(e: ColumnExpr, string_columns: Any) -> Tuple[str, Tuple[Any, ..
         if not lo <= len(rest) <= hi:
             n = f"{lo + 1}" if lo == hi else f"{lo + 1} to {hi + 1}"
             raise ValueError(f"{fn} takes {n} arguments: {x}")
-        vals = [_literal(fn, a, int if fn == "SUBSTR" else str) for a in rest]
+        vals = [_literal(fn, a, _ARG_TYPES.get(fn, (str, str, str))[i]) for i, a in enumerate(rest)]
         name, steps = operand(args[0])
         if any(v is None for v in vals):
             return name, steps + (("NULL",),)
@@ -249,6 +275,13 @@ def string_chain(e: ColumnExpr, string_columns: Any) -> Tuple[str, Tuple[Any, ..
             step = (fn, _utf8(fn, vals[0]) if vals else b" ")
         elif fn == "REPLACE":
             step = (fn, _utf8(fn, vals[0]), _utf8(fn, vals[1]))
+        elif fn == "REGEXP_EXTRACT":
+            group = vals[1] if len(vals) > 1 else 0
+            R.extract_program(vals[0], group)  # the pattern's and the group's errors, before anything runs
+            step = (fn, vals[0], group)
+        elif fn == "REGEXP_REPLACE":
+            step = (fn, vals[0], vals[1], R.replace_options(vals[2] if len(vals) > 2 else None))
+            R.replace_program(*step[1:])
         else:
             step = (fn,)
         return name, steps + (step,)
@@ -298,6 +331,14 @@ def apply_steps(offsets: torch.Tensor, data: torch.Tensor, valid: Optional[torch
         m = int(offsets.shape[0]) - 1
         if step[0] == "NULL":
             valid = torch.zeros(m, dtype=torch.uint8, device=offsets.device)
+            continue
+        if step[0] in ("REGEXP_EXTRACT", "REGEXP_REPLACE"):
+            prog = R.extract_program(*step[1:]) if step[0] == "REGEXP_EXTRACT" else R.replace_program(*step[1:])
+            lengths, out_valid = K.regex_transform(offsets, data, valid, prog)
+            new_offsets, total = _scan(lengths)
+            new_data = torch.empty(max(total, 1), dtype=torch.uint8, device=offsets.device)
+            K.regex_transform(offsets, data, valid, prog, out_offsets=new_offsets, out_data=new_data)
+            offsets, data, valid = new_offsets, new_data, out_valid
             continue
         op, kw = _STEP_OPS[step[0]], _step_args(step)
         lengths, out_valid = K.string_transform(op, offsets, data, valid, **kw)

@@ -771,6 +771,72 @@ int fb_value_format(int dev, void* stream, int64_t n, const uint64_t* values, co
 int fb_debug_value_format_host(int64_t n, const uint64_t* values, const uint8_t* valid, int kind, int64_t* out_len,
                                const int64_t* out_offsets, uint8_t* out_data);
 
+/* ---------------------------------------------------------------------------
+ * K15 regular expressions, evaluated once per dictionary entry
+ * Replaces: pandas str.contains / str.extract / str.replace(regex=True) and DuckDB's regexp_matches /
+ *           regexp_extract / regexp_replace, which ran one Python string per row on the host.
+ * Dictionaries have the K11 layout.  The host (fugue_b200/regex.py) compiles a pattern of the RE2 subset into a
+ * position automaton: every instruction that consumes a code point is a position (at most FB_REGEX_MAX_STATES).
+ * A closure is the list of positions, in leftmost-first priority order, that the empty-width part of the program
+ * reaches from one point, with the capture slots set on the way (a bit per slot the call tracks) and the match
+ * target FB_REGEX_MAX_STATES.  Closure 2 * r + at_end: row r < FB_REGEX_MAX_STATES follows position r, row
+ * FB_REGEX_MAX_STATES starts a match away from the start of the text, row FB_REGEX_MAX_STATES + 1 at its start;
+ * at_end = 1 where the point is the end of the text ($ and \z hold only there, ^ and \A only at byte 0).
+ *   ascii[b]          positions that accept the ASCII byte b
+ *   range_lo / _mask  code points >= 128: range r is [range_lo[r], range_lo[r + 1]) (the last reaches U+10FFFF),
+ *                     range_lo[0] == 128, strictly increasing; range_mask[r] the positions that accept it
+ *   cl_mask / _accept the closure's positions as a bit set / 1 when it reaches the match
+ *   cl_off / ent_*    the closure's entries ent_*[cl_off[c], cl_off[c + 1]) in priority order
+ *   restart           1 when a match may start away from the start of the text (a search keeps starting them)
+ *   rewrite           REGEXP_REPLACE: a byte 0..255, or FB_REGEX_GROUP + k for the text of slots 2k, 2k + 1
+ *   group_pair        REGEXP_EXTRACT: the slot pair k whose text is the result
+ * fb_regex_match     : out[i] = 1 when the pattern matches somewhere in entry i (the host anchors a full match
+ *                      with \A(?:p)\z), else 0; out_valid[i] = valid[i].  A bit-parallel Thompson machine: the
+ *                      live positions are one 64-bit word; per code point it ORs the closures of the live positions
+ *                      that accept it and the start closure, and stops at the first accept.
+ * fb_regex_transform : the K12 measure / write contract of fb_string_transform (no src).  op FB_REGEX_EXTRACT:
+ *                      slot pair group_pair of the leftmost-first match, '' when there is none or it is unset.
+ *                      FB_REGEX_REPLACE: the first match replaced by the rewrite; FB_REGEX_REPLACE_ALL: every
+ *                      match left to right, where an empty match right after the previous match is skipped
+ *                      (RE2's GlobalReplace).  A Pike VM over the same closures: threads in priority order, one per
+ *                      position, each with nslots (<= FB_REGEX_MAX_SLOTS) int32 slots; entries of at most 2^31 - 1
+ *                      bytes.  A NULL entry gives NULL.
+ * fb_debug_regex_host : either call over HOST arrays, on the CPU, by the same per-entry code; for a program of op
+ *                      FB_REGEX_MATCH, out_len[i] = the 0 / 1 result and out_valid[i] the validity.
+ * prog: a HOST struct (checked); dprog: its bytes on the device.  One thread per entry, grid-stride; the match
+ * kernel stages ascii, cl_mask and cl_accept in shared memory.
+ * --------------------------------------------------------------------------- */
+#define FB_REGEX_MAX_STATES 64
+#define FB_REGEX_MAX_RANGES 512
+#define FB_REGEX_MAX_CLOSURES (2 * (FB_REGEX_MAX_STATES + 2))
+#define FB_REGEX_MAX_ENTRIES (FB_REGEX_MAX_CLOSURES * (FB_REGEX_MAX_STATES + 1))
+#define FB_REGEX_MAX_SLOTS 8
+#define FB_REGEX_MAX_REWRITE 512
+#define FB_REGEX_GROUP 256
+enum fb_regex_op { FB_REGEX_MATCH = 0, FB_REGEX_EXTRACT = 1, FB_REGEX_REPLACE = 2, FB_REGEX_REPLACE_ALL = 3 };
+typedef struct {
+  int32_t npos, nranges, nslots, op;
+  int32_t group_pair, nrewrite, restart, reserved;
+  uint64_t ascii[128];
+  uint64_t range_mask[FB_REGEX_MAX_RANGES];
+  uint32_t range_lo[FB_REGEX_MAX_RANGES];
+  uint64_t cl_mask[FB_REGEX_MAX_CLOSURES];
+  uint8_t cl_accept[FB_REGEX_MAX_CLOSURES];
+  uint16_t cl_off[FB_REGEX_MAX_CLOSURES + 1];
+  uint8_t ent_target[FB_REGEX_MAX_ENTRIES];
+  uint8_t ent_save[FB_REGEX_MAX_ENTRIES];
+  int16_t rewrite[FB_REGEX_MAX_REWRITE];
+} fb_regex_program;
+int fb_regex_match(int dev, void* stream, int64_t n, const int64_t* offsets, const uint8_t* data,
+                   const uint8_t* valid, const fb_regex_program* prog, const fb_regex_program* dprog, uint8_t* out,
+                   uint8_t* out_valid);
+int fb_regex_transform(int dev, void* stream, int64_t n, const int64_t* offsets, const uint8_t* data,
+                       const uint8_t* valid, const fb_regex_program* prog, const fb_regex_program* dprog,
+                       int64_t* out_len, uint8_t* out_valid, const int64_t* out_offsets, uint8_t* out_data);
+int fb_debug_regex_host(int64_t n, const int64_t* offsets, const uint8_t* data, const uint8_t* valid,
+                        const fb_regex_program* prog, int64_t* out_len, uint8_t* out_valid, const int64_t* out_offsets,
+                        uint8_t* out_data);
+
 #ifdef __cplusplus
 }
 #endif

@@ -578,7 +578,7 @@ fb_scatter_kernel(FbKeys keys, FbDiv dv, uint32_t num, ChunkGeom g, int chunk0,
 // partition keeps its last (< G) rows per column in a shared-memory carry buffer and
 // only whole G-row groups (G * 8 B = one or more full sectors) are stored; the
 // carried rows are prepended to the partition's rows of the next tile.  Partial
-// stores happen only at chunk heads/tails (2 per partition per column per chunk).
+// stores happen only at the two ends of a CTA's run of chunks (ws_chunk_run).
 //
 // Shared memory (dynamic, one CTA per SM), T = kTile, E = num * (G - 1):
 //   ring[S][T] uint64          S x 32 KB stages filled by cp.async.bulk (TMA)
@@ -589,7 +589,7 @@ fb_scatter_kernel(FbKeys keys, FbDiv dv, uint32_t num, ChunkGeom g, int chunk0,
 //   per-partition uint32 arrays: wpos, kcnt, binfo, bin_start, wstart, wdelta
 //   cnt[kWarps][nbp] uint16, scanw[64] uint32, mbarriers
 // Source descriptor: [0, T) row of the staged tile; [T, T + E) old carry entry;
-// 0xFFFF nothing (phantom row at a chunk head / unused carry entry).
+// 0xFFFF nothing (phantom row at the head of a run / unused carry entry).
 // ---------------------------------------------------------------------------
 constexpr int kSwcMaxCols = 8;             // payload columns per launch (carry buffers in smem)
 constexpr uint32_t kSwcMaxNum = 256;
@@ -620,9 +620,9 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
       "}\n" ::"r"(bar), "r"(parity)
       : "memory");
 }
-__device__ __forceinline__ uint64_t l2_policy_evict_first() {
+__device__ __forceinline__ uint64_t l2_policy_evict_normal() {
   uint64_t pol;
-  asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
+  asm volatile("createpolicy.fractional.L2::evict_normal.b64 %0, 1.0;" : "=l"(pol));
   return pol;
 }
 __device__ __forceinline__ uint64_t l2_policy_evict_last() {
@@ -655,8 +655,7 @@ __device__ __forceinline__ void tma_load_1d(uint32_t dst_smem, const void* src, 
 //                           G-row groups, save the new carry (in place: the per-column barrier
 //                           separates the reads of the old carry from the writes of the new one)
 // Hand-off through mbarriers: slots_ready (rankers -> movers), slots_free (movers -> rankers, as
-// soon as the slot list sits in mover registers), flush_done at chunk ends, full/empty per ring
-// stage and per pid buffer.
+// soon as the slot list sits in mover registers), full/empty per ring stage and per pid buffer.
 // Shared memory (one CTA per SM), T = 4096, E = num * (G - 1):
 //   ring[S][T] u64 | mbarriers | carry[ncols][E] u64 | slotinfo[T+E] u32 | wpos kcnt binfo
 //   wstart wdelta [nbp] u32 | scanw[64] | carryinfo[E] u16 | rank records [2][12800 B]
@@ -684,9 +683,9 @@ static_assert(128 * kWsProducerRegs + kWsRankers * kWsRankerRegs + kWsMovers * k
 constexpr int kMoveBatch = 8;
 
 // The units of every column group of one launch.  Group k holds units [k * per_group, min(nunits,
-// (k + 1) * per_group)).  CTA b moves group b % ngroups over chunks b / ngroups, + S, + 2S, ... with
-// S = gridDim.x / ngroups, so the ngroups CTAs of one chunk run side by side on the same tile sequence
-// and every rank record is fetched from HBM about once (the siblings find it in L2).
+// (k + 1) * per_group)).  CTA b moves group b % ngroups over the run of consecutive chunks ws_chunk_run gives
+// index b / ngroups of S = gridDim.x / ngroups, so the ngroups CTAs of one run go side by side on the same tile
+// sequence and every rank record is fetched from HBM about once (the siblings find it in L2).
 struct WsUnits {
   const uint64_t* src[FB_MAX_COLS];
   uint64_t* dst[FB_MAX_COLS];
@@ -694,6 +693,18 @@ struct WsUnits {
   int32_t per_group;  // <= kSwcMaxCols: carry buffers in shared memory
   int32_t ngroups;
 };
+
+// Rows [r0, r1) of the chunks [i * n / S, (i + 1) * n / S) of the n = g.nchunks_full full chunks.  The chunks
+// of a run are consecutive, so where partition p's rows of chunk c end in the output, its rows of chunk c + 1
+// begin: a CTA places the whole run as one sequence of tiles, and its write-combining state (cursor, pending
+// rows) runs on across the chunk boundaries.  Only the two ends of a run store partial groups.
+__device__ __forceinline__ void ws_chunk_run(const ChunkGeom& g, int i, int S, int& c0, int64_t& r0, int64_t& r1) {
+  c0 = (int)((int64_t)i * g.nchunks_full / S);
+  const int c1 = (int)((int64_t)(i + 1) * g.nchunks_full / S);
+  int64_t unused;
+  chunk_range(g, c0, r0, unused);
+  chunk_range(g, c1 - 1, unused, r1);
+}
 
 // K4, the fused map epilogue: output unit u is not a copy of src[u] but an affine function of one or
 // two staged input tiles, computed by the movers right after the gather and before the store:
@@ -760,9 +771,11 @@ fb_scatter_ws_kernel(WsUnits units, uint32_t num, ChunkGeom g, int nstages,
   extern __shared__ __align__(128) uint64_t smem64[];
   const uint32_t nbp = nb_padded(num);
   const uint32_t E = num * GM;
-  // this CTA's column group (units u0 .. u0 + ncols) and chunk sequence (chunk_first, + chunk_step, ...)
+  // this CTA's column group (units u0 .. u0 + ncols) and run of tiles [row0, row1), chunk0 its first chunk
   const int grp = (int)blockIdx.x % units.ngroups;
-  const int chunk_first = (int)blockIdx.x / units.ngroups, chunk_step = (int)gridDim.x / units.ngroups;
+  int chunk0;
+  int64_t row0, row1;
+  ws_chunk_run(g, (int)blockIdx.x / units.ngroups, (int)gridDim.x / units.ngroups, chunk0, row0, row1);
   const int u0 = grp * units.per_group;
   const int ncols = min(units.per_group, units.nunits - u0);
   uint64_t* ring = smem64;
@@ -782,7 +795,6 @@ fb_scatter_ws_kernel(WsUnits units, uint32_t num, ChunkGeom g, int nstages,
   const uint32_t bar_full = smem_u32(bars), bar_empty = smem_u32(bars + 16);
   const uint32_t bar_pid_full = smem_u32(bars + 32), bar_pid_empty = smem_u32(bars + 34);
   const uint32_t bar_slots_ready = smem_u32(bars + 36), bar_slots_free = smem_u32(bars + 37);
-  const uint32_t bar_flush_done = smem_u32(bars + 38);
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < nstages; ++s) {
@@ -795,7 +807,6 @@ fb_scatter_ws_kernel(WsUnits units, uint32_t num, ChunkGeom g, int nstages,
     }
     mbar_init(bar_slots_ready, kWsRankWarps);
     mbar_init(bar_slots_free, kWsMoverWarps);
-    mbar_init(bar_flush_done, kWsMoverWarps);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
@@ -804,36 +815,23 @@ fb_scatter_ws_kernel(WsUnits units, uint32_t num, ChunkGeom g, int nstages,
     // ============================ producer =============================================
     setmaxnreg_dec<kWsProducerRegs>();
     if (warp == kWsMoverWarps + kWsRankWarps && lane == 0) {
-      // the payload is read once: evict first.  A rank record is read by every group of its chunk: kept
-      // in L2 for the sibling CTAs (H100 at 400 W, 100 M rows x 8 columns in 4 groups: records loaded
-      // evict_first 5.94 ms, evict_normal 5.77, evict_last 5.59; MEASUREMENTS.md)
-      const uint64_t pol = l2_policy_evict_first(), meta_pol = l2_policy_evict_last();
+      // A rank record is read by every group of its chunk: kept in L2 for the sibling CTAs (H100 at 400 W,
+      // 100 M rows x 8 columns in 4 groups: records loaded evict_first 5.94 ms, evict_normal 5.77, evict_last
+      // 5.59).  The payload is read once, yet evict_normal beats evict_first (H100 at 700 W, same table:
+      // 4.90 ms against 4.98; MEASUREMENTS.md)
+      const uint64_t pol = l2_policy_evict_normal(), meta_pol = l2_policy_evict_last();
       const uint32_t ring_s = smem_u32(ring), meta_s = smem_u32(metabuf);
       uint32_t s = 0, ph = 0, seq = 0;
-      // pids of the very first tile
-      int chunk = chunk_first;
-      int64_t r0 = 0, r1 = 0, t0 = 0;
-      bool have = chunk < g.nchunks_full;
-      if (have) { chunk_range(g, chunk, r0, r1); t0 = r0; }
-      auto load_pid = [&](int64_t row0, uint32_t q) {
+      auto load_pid = [&](int64_t t, uint32_t q) {
         const uint32_t b = q & 1, pp = (q >> 1) & 1;
         mbar_wait(bar_pid_empty + 8 * b, pp ^ 1);
         mbar_expect_tx(bar_pid_full + 8 * b, kMetaBytes);
-        tma_load_1d(meta_s + b * kMetaBytes, meta + (size_t)(row0 / T) * kMetaBytes, kMetaBytes,
+        tma_load_1d(meta_s + b * kMetaBytes, meta + (size_t)(t / T) * kMetaBytes, kMetaBytes,
                     bar_pid_full + 8 * b, meta_pol);
       };
-      if (have) load_pid(t0, 0);
-      while (have) {
-        // next tile of this CTA's sequence (for the pid look-ahead)
-        int nchunk = chunk;
-        int64_t nr0 = r0, nr1 = r1, nt0 = t0 + T;
-        bool nhave = true;
-        if (nt0 >= r1) {
-          nchunk = chunk + chunk_step;
-          nhave = nchunk < g.nchunks_full;
-          if (nhave) { chunk_range(g, nchunk, nr0, nr1); nt0 = nr0; }
-        }
-        if (nhave) load_pid(nt0, seq + 1);
+      load_pid(row0, 0);  // the record of the first tile
+      for (int64_t t0 = row0; t0 < row1; t0 += T, ++seq) {
+        if (t0 + T < row1) load_pid(t0 + T, seq + 1);  // look-ahead: the next tile's record
         for (int u = u0; u < u0 + ncols; ++u) {
           mbar_wait(bar_empty + 8 * s, ph ^ 1);
           mbar_expect_tx(bar_full + 8 * s, kStageBytes);
@@ -848,8 +846,6 @@ fb_scatter_ws_kernel(WsUnits units, uint32_t num, ChunkGeom g, int nstages,
             }
           }
         }
-        chunk = nchunk; r0 = nr0; r1 = nr1; t0 = nt0; have = nhave;
-        ++seq;
       }
     }
     return;
@@ -860,97 +856,91 @@ fb_scatter_ws_kernel(WsUnits units, uint32_t num, ChunkGeom g, int nstages,
     setmaxnreg_dec<kWsRankerRegs>();
     const unsigned rw = warp - kWsMoverWarps;          // ranker warp 0..7
     const unsigned rtid = threadIdx.x - kWsMovers;     // 0..255
-    uint32_t seq = 0, cseq = 0;
-    for (int chunk = chunk_first; chunk < g.nchunks_full; chunk += chunk_step, ++cseq) {
-      int64_t r0, r1;
-      chunk_range(g, chunk, r0, r1);
-      if (cseq > 0) mbar_wait(bar_flush_done, (cseq - 1) & 1);  // movers flushed the previous chunk
-      ranker_sync();
-      for (uint32_t b = rtid; b < nbp; b += kWsRankers) {
-        const uint32_t p0 = b < num ? (uint32_t)part_offsets[b] + chunk_base[(size_t)chunk * num + b] : 0u;
-        wpos[b] = p0 & ~GM;
-        kcnt[b] = (p0 & GM) | ((p0 & GM) << 8);
+    for (uint32_t b = rtid; b < nbp; b += kWsRankers) {
+      const uint32_t p0 = b < num ? (uint32_t)part_offsets[b] + chunk_base[(size_t)chunk0 * num + b] : 0u;
+      wpos[b] = p0 & ~GM;
+      kcnt[b] = (p0 & GM) | ((p0 & GM) << 8);
+    }
+    ranker_sync();
+    uint32_t seq = 0;
+    for (int64_t t0 = row0; t0 < row1; t0 += T, ++seq) {
+      const uint32_t pb = seq & 1, pph = (seq >> 1) & 1;
+      mbar_wait(bar_pid_full + 8 * pb, pph);
+      const uint8_t* __restrict__ rec = metabuf + pb * kMetaBytes;
+      // ---- per partition (thread b < num): tile count, rows to write, new pending state
+      const uint32_t b = rtid;
+      uint32_t n = 0, w = 0, kold = 0, phold = 0, wp_old = 0;
+      if (b < num) n = ((const uint16_t*)(rec + kMetaCnt))[b];
+      if (b < num) {
+        const uint32_t kc = kcnt[b];
+        kold = kc & 0xFFu;
+        phold = kc >> 8;
+        wp_old = wpos[b];
+        const uint32_t end = wp_old + kold + n;
+        const uint32_t aend = end & ~GM;
+        if (aend > wp_old) {
+          w = aend - wp_old;
+          wpos[b] = aend;
+          kcnt[b] = end - aend;  // phantoms are consumed by the first write
+        } else {
+          kcnt[b] = (kold + n) | (phold << 8);
+        }
+        binfo[b] = kold | (w << 8);
       }
-      ranker_sync();
-      for (int64_t t0 = r0; t0 < r1; t0 += T, ++seq) {
-        const uint32_t pb = seq & 1, pph = (seq >> 1) & 1;
-        mbar_wait(bar_pid_full + 8 * pb, pph);
-        const uint8_t* __restrict__ rec = metabuf + pb * kMetaBytes;
-        // ---- per partition (thread b < num): tile count, rows to write, new pending state
-        const uint32_t b = rtid;
-        uint32_t n = 0, w = 0, kold = 0, phold = 0, wp_old = 0;
-        if (b < num) n = ((const uint16_t*)(rec + kMetaCnt))[b];
-        if (b < num) {
-          const uint32_t kc = kcnt[b];
-          kold = kc & 0xFFu;
-          phold = kc >> 8;
-          wp_old = wpos[b];
-          const uint32_t end = wp_old + kold + n;
-          const uint32_t aend = end & ~GM;
-          if (aend > wp_old) {
-            w = aend - wp_old;
-            wpos[b] = aend;
-            kcnt[b] = end - aend;  // phantoms are consumed by the first write
-          } else {
-            kcnt[b] = (kold + n) | (phold << 8);
-          }
-          binfo[b] = kold | (w << 8);
-        }
-        uint32_t xw = w;
+      uint32_t xw = w;
 #pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-          const uint32_t yw = __shfl_up_sync(0xFFFFFFFFu, xw, o);
-          if (lane >= (unsigned)o) xw += yw;
-        }
-        if (lane == 31) scanw[8 + rw] = xw;
-        ranker_sync();  // B
-        uint32_t bw = xw - w;
-        {
-          const uint32_t tw = lane < kWsRankWarps ? scanw[8 + lane] : 0;
-#pragma unroll
-          for (int wi = 0; wi < kWsRankWarps; ++wi) {
-            const uint32_t vw = __shfl_sync(0xFFFFFFFFu, tw, wi);
-            if ((unsigned)wi < rw) bw += vw;
-          }
-        }
-        // ---- hand-off arrays may be rewritten once the movers hold the previous slot list
-        if (seq > 0) mbar_wait(bar_slots_free, (seq - 1) & 1);
-        if (b < num) {
-          wstart[b] = bw;
-          wdelta[b] = wp_old - bw;  // slot j lands at output row wdelta + j
-        }
-        if (rtid == kWsRankers - 1) scanw[40] = bw + w;  // W: slots to store this tile
-        ranker_sync();  // C
-        // ---- every new row / old carry entry finds its place.  The rows of this thread (r * 256 + rtid) are read
-        //      from the record here, not kept in registers since the top of the tile: the producer fills the
-        //      other record buffer meanwhile, and needs this one only for the tile after next.
-#pragma unroll
-        for (int r = 0; r < kWsRankItems; ++r) {
-          const uint32_t row = r * kWsRankers + rtid;
-          const uint32_t pb2 = rec[row];
-          const uint32_t bi = binfo[pb2];
-          const uint32_t i = (bi & 0xFFu) + ((const uint16_t*)(rec + kMetaRank))[row];
-          const uint32_t ww = bi >> 8;
-          if (i < ww) slotinfo[wstart[pb2] + i] = (pb2 << 16) | row;
-          else carryinfo[pb2 * GM + (i - ww)] = (uint16_t)row;
-        }
-        __syncwarp();
-        if (lane == 0) mbar_arrive_relaxed(bar_pid_empty + 8 * pb);  // the record has been read
-        if (b < num) {  // the old carry entries of partition b
-#pragma unroll
-          for (uint32_t i = 0; i < GM; ++i) {
-            const uint32_t e = b * GM + i;
-            const uint32_t desc = i < phold ? 0xFFFFu : T + e;
-            if (i < kold) {
-              if (i < w) slotinfo[bw + i] = (b << 16) | desc;
-              else carryinfo[e] = (uint16_t)desc;
-            }
-            if (w + i >= kold + n) carryinfo[e] = 0xFFFFu;
-          }
-        }
-        ranker_sync();  // D: the slot list of this tile is complete
-        if (lane == 0) mbar_arrive(bar_slots_ready);
+      for (int o = 1; o < 32; o <<= 1) {
+        const uint32_t yw = __shfl_up_sync(0xFFFFFFFFu, xw, o);
+        if (lane >= (unsigned)o) xw += yw;
       }
+      if (lane == 31) scanw[8 + rw] = xw;
+      ranker_sync();  // B
+      uint32_t bw = xw - w;
+      {
+        const uint32_t tw = lane < kWsRankWarps ? scanw[8 + lane] : 0;
+#pragma unroll
+        for (int wi = 0; wi < kWsRankWarps; ++wi) {
+          const uint32_t vw = __shfl_sync(0xFFFFFFFFu, tw, wi);
+          if ((unsigned)wi < rw) bw += vw;
+        }
+      }
+      // ---- hand-off arrays may be rewritten once the movers hold the previous slot list
+      if (seq > 0) mbar_wait(bar_slots_free, (seq - 1) & 1);
+      if (b < num) {
+        wstart[b] = bw;
+        wdelta[b] = wp_old - bw;  // slot j lands at output row wdelta + j
+      }
+      if (rtid == kWsRankers - 1) scanw[40] = bw + w;  // W: slots to store this tile
+      ranker_sync();  // C
+      // ---- every new row / old carry entry finds its place.  The rows of this thread (r * 256 + rtid) are read
+      //      from the record here, not kept in registers since the top of the tile: the producer fills the
+      //      other record buffer meanwhile, and needs this one only for the tile after next.
+#pragma unroll
+      for (int r = 0; r < kWsRankItems; ++r) {
+        const uint32_t row = r * kWsRankers + rtid;
+        const uint32_t pb2 = rec[row];
+        const uint32_t bi = binfo[pb2];
+        const uint32_t i = (bi & 0xFFu) + ((const uint16_t*)(rec + kMetaRank))[row];
+        const uint32_t ww = bi >> 8;
+        if (i < ww) slotinfo[wstart[pb2] + i] = (pb2 << 16) | row;
+        else carryinfo[pb2 * GM + (i - ww)] = (uint16_t)row;
+      }
+      __syncwarp();
+      if (lane == 0) mbar_arrive_relaxed(bar_pid_empty + 8 * pb);  // the record has been read
+      if (b < num) {  // the old carry entries of partition b
+#pragma unroll
+        for (uint32_t i = 0; i < GM; ++i) {
+          const uint32_t e = b * GM + i;
+          const uint32_t desc = i < phold ? 0xFFFFu : T + e;
+          if (i < kold) {
+            if (i < w) slotinfo[bw + i] = (b << 16) | desc;
+            else carryinfo[e] = (uint16_t)desc;
+          }
+          if (w + i >= kold + n) carryinfo[e] = 0xFFFFu;
+        }
+      }
+      ranker_sync();  // D: the slot list of this tile is complete
+      if (lane == 0) mbar_arrive(bar_slots_ready);
     }
     return;
   }
@@ -958,111 +948,105 @@ fb_scatter_ws_kernel(WsUnits units, uint32_t num, ChunkGeom g, int nstages,
   // ================================ movers (16 warps) ====================================
   setmaxnreg_inc<kWsMoverRegs>();
   uint32_t s = 0, ph = 0, seq = 0;
-  for (int chunk = chunk_first; chunk < g.nchunks_full; chunk += chunk_step) {
-    int64_t r0, r1;
-    chunk_range(g, chunk, r0, r1);
-    for (int64_t t0 = r0; t0 < r1; t0 += T, ++seq) {
-      mbar_wait(bar_slots_ready, seq & 1);
-      const uint32_t W = scanw[40];
-      uint32_t srcd[kSlotRounds], dst[kSlotRounds];
+  for (int64_t t0 = row0; t0 < row1; t0 += T, ++seq) {
+    mbar_wait(bar_slots_ready, seq & 1);
+    const uint32_t W = scanw[40];
+    uint32_t srcd[kSlotRounds], dst[kSlotRounds];
 #pragma unroll
-      for (int k = 0; k < kSlotRounds; ++k) {
-        const uint32_t j = k * kWsMovers + threadIdx.x;
-        srcd[k] = 0xFFFFu;
-        dst[k] = 0;
-        if (j < W) {
-          const uint32_t info = slotinfo[j];
-          srcd[k] = info & 0xFFFFu;
-          dst[k] = wdelta[info >> 16] + j;
-        }
+    for (int k = 0; k < kSlotRounds; ++k) {
+      const uint32_t j = k * kWsMovers + threadIdx.x;
+      srcd[k] = 0xFFFFu;
+      dst[k] = 0;
+      if (j < W) {
+        const uint32_t info = slotinfo[j];
+        srcd[k] = info & 0xFFFFu;
+        dst[k] = wdelta[info >> 16] + j;
       }
-      // New carry entries that come from the staged tile.  An entry carried over from an earlier tile keeps
-      // its place (its descriptor is T + e: a partition either writes all its pending rows or none), so it
-      // is neither read nor rewritten.
-      uint32_t csrc[kEntryRoundsM];
-#pragma unroll
-      for (int q = 0; q < kEntryRoundsM; ++q) {
-        const uint32_t e = q * kWsMovers + threadIdx.x;
-        const uint32_t d = e < E ? (uint32_t)carryinfo[e] : 0xFFFFu;
-        csrc[q] = d < T ? d : 0xFFFFu;
-      }
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_slots_free);  // the slot list sits in registers now
-
-      for (int u = 0; u < ncols; ++u) {
-        mbar_wait(bar_full + 8 * s, ph);
-        const uint64_t* __restrict__ st = ring + (size_t)s * T;
-        uint64_t* __restrict__ out = units.dst[u0 + u];
-        uint64_t* __restrict__ cbuf = carry + (size_t)u * E;
-        uint32_t s2 = s;
-        bool two = false;
-        const uint64_t* __restrict__ st2 = st;
-        int mode = 0;
-        uint64_t ma = 0, mb = 0, mc = 0;
-        if constexpr (kMap) {
-          // fused map (K4): rows taken from the staged tile(s) are mapped here; carry entries already are
-          // output values
-          mode = map.mode[u0 + u];
-          two = map.src2[u0 + u] != nullptr;
-          if (two) {
-            s2 = s + 1 == (uint32_t)nstages ? 0 : s + 1;
-            mbar_wait(bar_full + 8 * s2, s2 == 0 ? ph ^ 1 : ph);
-            st2 = ring + (size_t)s2 * T;
-          }
-          ma = map.a[u0 + u]; mb = map.b[u0 + u]; mc = map.c[u0 + u];
-        }
-        auto staged = [&](uint32_t r) -> uint64_t {
-          if constexpr (kMap) return ws_apply_map(mode, two, st[r], st2[r], ma, mb, mc);
-          else return st[r];
-        };
-        // gather from the stage / old carry and store, kMoveBatch slot rounds at a time
-#pragma unroll
-        for (int k0 = 0; k0 < kSlotRounds; k0 += kMoveBatch) {
-          uint64_t v[kMoveBatch];
-#pragma unroll
-          for (int k = 0; k < kMoveBatch; ++k)
-            if (k0 + k < kSlotRounds && srcd[k0 + k] != 0xFFFFu)
-              v[k] = srcd[k0 + k] < T ? staged(srcd[k0 + k]) : cbuf[srcd[k0 + k] - T];
-#pragma unroll
-          for (int k = 0; k < kMoveBatch; ++k)
-            if (k0 + k < kSlotRounds && srcd[k0 + k] != 0xFFFFu) out[dst[k0 + k]] = v[k];
-        }
-        mover_sync();  // every mover has read the old carry of this column: it is overwritten in place
-#pragma unroll
-        for (int q = 0; q < kEntryRoundsM; ++q)
-          if (csrc[q] != 0xFFFFu) cbuf[q * kWsMovers + threadIdx.x] = staged(csrc[q]);
-        // all my reads of the stage have completed (their values were consumed by the stores above)
-        __syncwarp();
-        if (lane == 0) {
-          mbar_arrive_relaxed(bar_empty + 8 * s);
-          if (kMap && two) mbar_arrive_relaxed(bar_empty + 8 * s2);
-        }
-        if (++s == (uint32_t)nstages) { s = 0; ph ^= 1; }
-        if (kMap && two) {
-          if (++s == (uint32_t)nstages) { s = 0; ph ^= 1; }
-        }
-      }
-      // The new carry of column u is read in the next tile after the barrier of column u + 1 of this tile or
-      // of column 0 of the next one.  A single column has neither: order it here.
-      if (ncols == 1) mover_sync();
     }
-    // ---- chunk end: flush the pending rows (partial groups)
-    mover_sync();
-    for (int u = 0; u < ncols; ++u) {
-      uint64_t* __restrict__ out = units.dst[u0 + u];
-      const uint64_t* __restrict__ cbuf = carry + (size_t)u * E;
+    // New carry entries that come from the staged tile.  An entry carried over from an earlier tile keeps
+    // its place (its descriptor is T + e: a partition either writes all its pending rows or none), so it
+    // is neither read nor rewritten.
+    uint32_t csrc[kEntryRoundsM];
 #pragma unroll
-      for (int q = 0; q < kEntryRoundsM; ++q) {
-        const uint32_t e = q * kWsMovers + threadIdx.x;
-        if (e < E) {
-          const uint32_t b = e / GM, i = e - b * GM;
-          const uint32_t kc = kcnt[b];
-          if (i < (kc & 0xFFu) && i >= (kc >> 8)) out[wpos[b] + i] = cbuf[e];
-        }
-      }
+    for (int q = 0; q < kEntryRoundsM; ++q) {
+      const uint32_t e = q * kWsMovers + threadIdx.x;
+      const uint32_t d = e < E ? (uint32_t)carryinfo[e] : 0xFFFFu;
+      csrc[q] = d < T ? d : 0xFFFFu;
     }
     __syncwarp();
-    if (lane == 0) mbar_arrive(bar_flush_done);  // rankers may start the next chunk
+    if (lane == 0) mbar_arrive(bar_slots_free);  // the slot list sits in registers now
+
+    for (int u = 0; u < ncols; ++u) {
+      mbar_wait(bar_full + 8 * s, ph);
+      const uint64_t* __restrict__ st = ring + (size_t)s * T;
+      uint64_t* __restrict__ out = units.dst[u0 + u];
+      uint64_t* __restrict__ cbuf = carry + (size_t)u * E;
+      uint32_t s2 = s;
+      bool two = false;
+      const uint64_t* __restrict__ st2 = st;
+      int mode = 0;
+      uint64_t ma = 0, mb = 0, mc = 0;
+      if constexpr (kMap) {
+        // fused map (K4): rows taken from the staged tile(s) are mapped here; carry entries already are
+        // output values
+        mode = map.mode[u0 + u];
+        two = map.src2[u0 + u] != nullptr;
+        if (two) {
+          s2 = s + 1 == (uint32_t)nstages ? 0 : s + 1;
+          mbar_wait(bar_full + 8 * s2, s2 == 0 ? ph ^ 1 : ph);
+          st2 = ring + (size_t)s2 * T;
+        }
+        ma = map.a[u0 + u]; mb = map.b[u0 + u]; mc = map.c[u0 + u];
+      }
+      auto staged = [&](uint32_t r) -> uint64_t {
+        if constexpr (kMap) return ws_apply_map(mode, two, st[r], st2[r], ma, mb, mc);
+        else return st[r];
+      };
+      // gather from the stage / old carry and store, kMoveBatch slot rounds at a time
+#pragma unroll
+      for (int k0 = 0; k0 < kSlotRounds; k0 += kMoveBatch) {
+        uint64_t v[kMoveBatch];
+#pragma unroll
+        for (int k = 0; k < kMoveBatch; ++k)
+          if (k0 + k < kSlotRounds && srcd[k0 + k] != 0xFFFFu)
+            v[k] = srcd[k0 + k] < T ? staged(srcd[k0 + k]) : cbuf[srcd[k0 + k] - T];
+#pragma unroll
+        for (int k = 0; k < kMoveBatch; ++k)
+          if (k0 + k < kSlotRounds && srcd[k0 + k] != 0xFFFFu) out[dst[k0 + k]] = v[k];
+      }
+      mover_sync();  // every mover has read the old carry of this column: it is overwritten in place
+#pragma unroll
+      for (int q = 0; q < kEntryRoundsM; ++q)
+        if (csrc[q] != 0xFFFFu) cbuf[q * kWsMovers + threadIdx.x] = staged(csrc[q]);
+      // all my reads of the stage have completed (their values were consumed by the stores above)
+      __syncwarp();
+      if (lane == 0) {
+        mbar_arrive_relaxed(bar_empty + 8 * s);
+        if (kMap && two) mbar_arrive_relaxed(bar_empty + 8 * s2);
+      }
+      if (++s == (uint32_t)nstages) { s = 0; ph ^= 1; }
+      if (kMap && two) {
+        if (++s == (uint32_t)nstages) { s = 0; ph ^= 1; }
+      }
+    }
+    // The new carry of column u is read in the next tile after the barrier of column u + 1 of this tile or
+    // of column 0 of the next one.  A single column has neither: order it here.
+    if (ncols == 1) mover_sync();
+  }
+  // ---- end of the run: flush the pending rows (partial groups)
+  mover_sync();
+  for (int u = 0; u < ncols; ++u) {
+    uint64_t* __restrict__ out = units.dst[u0 + u];
+    const uint64_t* __restrict__ cbuf = carry + (size_t)u * E;
+#pragma unroll
+    for (int q = 0; q < kEntryRoundsM; ++q) {
+      const uint32_t e = q * kWsMovers + threadIdx.x;
+      if (e < E) {
+        const uint32_t b = e / GM, i = e - b * GM;
+        const uint32_t kc = kcnt[b];
+        if (i < (kc & 0xFFu) && i >= (kc >> 8)) out[wpos[b] + i] = cbuf[e];
+      }
+    }
   }
 }
 

@@ -103,15 +103,49 @@ TEMPORAL_LITERALS = (datetime.date, datetime.datetime, datetime.timedelta)
 TIME_FIELDS = ("year", "month", "day", "hour", "minute", "second", "quarter", "dow", "isodow", "doy", "week",
                "isoyear")
 TIME_PARTS = ("year", "quarter", "month", "week", "day", "hour", "minute", "second")
-TEMPORAL_FUNCTIONS = frozenset(["EXTRACT", "DATE_TRUNC", "DATEDIFF", "ADD_MONTHS"])
-FLOAT_FUNCTIONS = frozenset(["SQRT", "EXP", "LN", "LOG10", "POWER", "POW"])  # always float64
 ROUND_MAX_DIGITS = 18
-# functions that build a string from one string expression and literals (SUBSTRING is SUBSTR); ``||`` too
-STRING_FUNCTIONS = frozenset(["UPPER", "LOWER", "SUBSTR", "SUBSTRING", "TRIM", "LTRIM", "RTRIM", "REPLACE", "CONCAT",
-                              "REGEXP_EXTRACT", "REGEXP_REPLACE"])
+
+
+class Scalar(NamedTuple):
+    """What the engine knows of one scalar function head.  ``family``: ``conditional``, ``numeric``, ``string``,
+    ``regex`` or ``temporal``.  ``arity``: the least and the most arguments (None: no limit).  ``literals``: the
+    Python types of the arguments after the first; each must be a literal of its type or NULL.  ``result``: ``bool``,
+    ``int64``, ``float64``, ``string`` (it builds a string from one string expression), ``extract`` (float64 for the
+    ``epoch`` field, else int64), ``operand`` (the type of args[0]), ``case`` (string when every result is a string
+    literal or NULL) or None (the evaluator decides)."""
+    family: str
+    arity: Tuple[int, Optional[int]]
+    literals: Tuple[type, ...] = ()
+    result: Optional[str] = None
+
+
+# every scalar function head the device evaluates, in its canonical spelling.  NULLIF runs as a CASE and MOD as
+# ``%``; EXTRACT, DATE_TRUNC and DATEDIFF take their field or part as a keyword argument
+SCALARS: Dict[str, Scalar] = {
+    "CASE": Scalar("conditional", (3, None), result="case"), "NULLIF": Scalar("conditional", (2, 2), result="case"),
+    "COALESCE": Scalar("conditional", (1, None)), "GREATEST": Scalar("conditional", (2, None)),
+    "LEAST": Scalar("conditional", (2, None)),
+    **{h: Scalar("numeric", (1, 1)) for h in ("ABS", "FLOOR", "CEIL")},
+    "ROUND": Scalar("numeric", (1, 2), (int,)), "MOD": Scalar("numeric", (2, 2)),
+    **{h: Scalar("numeric", (1, 1), result="float64") for h in ("SQRT", "EXP", "LN", "LOG10")},
+    "POWER": Scalar("numeric", (2, 2), result="float64"),
+    "LIKE": Scalar("string", (2, 3), result="bool"), "LENGTH": Scalar("string", (1, 1), result="int64"),
+    **{h: Scalar("string", (1, 1), result="string") for h in ("UPPER", "LOWER")},
+    "SUBSTR": Scalar("string", (2, 3), (int, int), "string"),
+    **{h: Scalar("string", (1, 2), (str,), "string") for h in ("TRIM", "LTRIM", "RTRIM")},
+    "REPLACE": Scalar("string", (3, 3), (str, str), "string"), "CONCAT": Scalar("string", (1, None), result="string"),
+    **{h: Scalar("regex", (2, 2), result="bool") for h in ("REGEXP_MATCHES", "REGEXP_FULL_MATCH")},
+    "REGEXP_EXTRACT": Scalar("regex", (2, 3), (str, int), "string"),
+    "REGEXP_REPLACE": Scalar("regex", (3, 4), (str, str, str), "string"),
+    "EXTRACT": Scalar("temporal", (1, 1), result="extract"), "DATE_TRUNC": Scalar("temporal", (1, 1), result="operand"),
+    "DATEDIFF": Scalar("temporal", (2, 2), result="int64"), "ADD_MONTHS": Scalar("temporal", (2, 2), result="operand"),
+}
+# other spellings: (canonical head, the arity they allow; None: the head's)
+SCALAR_ALIASES: Dict[str, Tuple[str, Optional[Tuple[int, Optional[int]]]]] = {
+    "IFNULL": ("COALESCE", (2, 2)), "IF": ("CASE", (3, 3)), "IIF": ("CASE", (3, 3)), "POW": ("POWER", None),
+    "CEILING": ("CEIL", None), "SUBSTRING": ("SUBSTR", None), "REGEXP_LIKE": ("REGEXP_MATCHES", None)}
 # regular-expression tests of one string expression: bool
-REGEX_PREDICATES = frozenset(["REGEXP_MATCHES", "REGEXP_FULL_MATCH"])
-REGEX_FUNCTIONS = REGEX_PREDICATES | {"REGEXP_EXTRACT", "REGEXP_REPLACE"}
+REGEX_PREDICATES = frozenset(h for h, s in SCALARS.items() if s.family == "regex" and s.result == "bool")
 
 
 def result_type(head: str, arg_type: Optional[pa.DataType]) -> Optional[pa.DataType]:
@@ -288,20 +322,15 @@ class ColumnExpr:
             if k == Kind.AGG and a.family == "basic" and a.result != "arg":
                 return None  # SUM / COUNT / AVG: select() keeps the type the group-by gives them
             return result_type(self.head, self.args[0].infer_type(schema))
-        if k == Kind.CALL and self.head in ("LIKE", "LENGTH"):
-            return pa.bool_() if self.head == "LIKE" else pa.int64()
-        if k == Kind.CALL and self.head.upper() in REGEX_PREDICATES:
-            return pa.bool_()
-        if k == Kind.CALL and self.head.upper() in STRING_FUNCTIONS:
-            return pa.string()
-        if k == Kind.CALL and self.head.upper() in FLOAT_FUNCTIONS:
-            return pa.float64()
-        if k == Kind.CALL and self.head.upper() in ("EXTRACT", "DATEDIFF"):
-            return pa.float64() if str(self.kwargs.get("field", "")).lower() == "epoch" else pa.int64()
-        if k == Kind.CALL and self.head.upper() in ("DATE_TRUNC", "ADD_MONTHS") and self.args:
-            return _operand(self.args[0]).infer_type(schema)
-        if k == Kind.CALL and case_string_results(self) is not None:
-            return pa.string()
+        if k == Kind.CALL and scalar_head(self.head) is not None:
+            rule = scalar_head(self.head)[1].result
+            if rule == "extract":
+                return pa.float64() if str(self.kwargs.get("field", "")).lower() == "epoch" else pa.int64()
+            if rule == "operand":
+                return _operand(self.args[0]).infer_type(schema) if self.args else None
+            if rule == "case":
+                return pa.string() if case_string_results(self) is not None else None
+            return None if rule is None else pa.type_for_alias(rule)
         if k == Kind.WINDOW:
             return pa.int64() if self.head in _RANKINGS else self.args[0].infer_type(schema)  # LAG LEAD: the arg's
         return None
@@ -633,30 +662,69 @@ def _offset_fn(name: str, c: Any, n: Any, default: Any) -> ColumnExpr:
     return ColumnExpr(Kind.WINDOW, name, [arg], {"n": n, "default": default})
 
 
-def _result_args(e: ColumnExpr) -> List[Any]:
-    """The operands of a CASE / IF / IIF / NULLIF that can become its value."""
-    head = e.head.upper()
+def scalar_head(name: str) -> Optional[Tuple[str, Scalar]]:
+    """The canonical head of scalar function ``name`` (any letter case, any spelling) and its catalogue entry, with
+    the narrower arity of an alias; None for a name that is not in ``SCALARS``."""
+    up = name.upper()
+    if up in SCALAR_ALIASES:
+        head, arity = SCALAR_ALIASES[up]
+        return head, SCALARS[head] if arity is None else SCALARS[head]._replace(arity=arity)
+    return (up, SCALARS[up]) if up in SCALARS else None
+
+
+def check_arity(name: str, n: int) -> str:
+    """The canonical head of ``SCALARS`` function ``name``; ValueError unless it takes ``n`` arguments."""
+    head, s = scalar_head(name)
+    lo, hi = s.arity
+    if n < lo or (hi is not None and n > hi):
+        want = str(lo) if lo == hi else f"at least {lo}" if hi is None else f"{lo} to {hi}"
+        raise ValueError(f"{name.upper()} takes {want} argument(s), got {n}")
+    return head
+
+
+def check_call(name: str, args: Sequence[Any]) -> Tuple[str, List[ColumnExpr]]:
+    """The canonical head and the argument nodes of a call of ``SCALARS`` function ``name``, checked against its
+    entry: a wrong number of arguments or a literal of the wrong type raises ValueError, an argument that must be a
+    literal and is not raises NotImplementedError."""
+    head = check_arity(name, len(args))
+    nodes = [_operand(a) for a in args]
+    for i, (e, tp) in enumerate(zip(nodes[1:], SCALARS[head].literals)):
+        if e.kind != Kind.LITERAL or e.as_type is not None:
+            raise NotImplementedError(f"{head}: argument {i + 2} must be a {tp.__name__} literal, got {e}")
+        if e.value is not None and (isinstance(e.value, bool) or not isinstance(e.value, tp)):
+            raise ValueError(f"{head}: argument {i + 2} must be a {tp.__name__} literal or NULL, got {e.value!r}")
+    return head, nodes
+
+
+def _call(name: str, *args: Any) -> ColumnExpr:
+    head, nodes = check_call(name, args)
+    return ColumnExpr(Kind.CALL, head, nodes)
+
+
+def round_digits(d: Any) -> int:
+    """The digits of ROUND: an int literal in [-ROUND_MAX_DIGITS, ROUND_MAX_DIGITS], else ValueError."""
+    v = d.value if isinstance(d, ColumnExpr) and d.kind == Kind.LITERAL and d.as_type is None else d
+    if isinstance(v, bool) or not isinstance(v, int) or not -ROUND_MAX_DIGITS <= v <= ROUND_MAX_DIGITS:
+        raise ValueError(f"ROUND takes an integer literal in [-{ROUND_MAX_DIGITS}, {ROUND_MAX_DIGITS}] as its "
+                         f"digits, got {d!r}")
+    return v
+
+
+def result_args(e: ColumnExpr) -> List[Any]:
+    """The operands of a ``conditional`` call that can become its value: the THEN values and the ELSE of a CASE, the
+    first argument of NULLIF, every argument of COALESCE / GREATEST / LEAST."""
+    head = scalar_head(e.head)[0]
     if head == "CASE":
         return list(e.args[1::2]) + [e.args[-1]] if e.args else []
-    if head in ("IF", "IIF"):
-        return list(e.args[1:3])
-    return list(e.args[:1]) if head == "NULLIF" else []
+    return list(e.args[:1]) if head == "NULLIF" else list(e.args)
 
 
 def is_string_build(e: Any) -> bool:
-    """True for a node that builds a string: a call of ``STRING_FUNCTIONS`` (any letter case) or ``||``."""
-    return isinstance(e, ColumnExpr) and ((e.kind == Kind.CALL and e.head.upper() in STRING_FUNCTIONS) or
-                                          (e.kind == Kind.BINARY and e.head == "||"))
-
-
-def _int_arg(fn: str, what: str, v: Any) -> ColumnExpr:
-    """An int literal argument (or NULL) of a string function."""
-    e = _operand(v)
-    if e.kind != Kind.LITERAL or e.as_type is not None:
-        raise NotImplementedError(f"{fn}: {what} must be an int literal, got {e}")
-    if e.value is not None and (isinstance(e.value, bool) or not isinstance(e.value, int)):
-        raise ValueError(f"{fn}: {what} must be an int literal or NULL, got {e.value!r}")
-    return e
+    """True for a node that builds a string: a call whose ``SCALARS`` result is ``string`` or ``||``."""
+    if isinstance(e, ColumnExpr) and e.kind == Kind.BINARY:
+        return e.head == "||"
+    s = scalar_head(e.head) if isinstance(e, ColumnExpr) and e.kind == Kind.CALL else None
+    return s is not None and s[1].result == "string"
 
 
 def _str_arg(fn: str, what: str, v: Any) -> ColumnExpr:
@@ -672,10 +740,11 @@ def _str_arg(fn: str, what: str, v: Any) -> ColumnExpr:
 def case_string_results(e: Any) -> Optional[List[str]]:
     """The distinct string literals (in order of appearance) of a CASE / IF / IIF / NULLIF whose every result is a
     string literal or NULL, with at least one string; None for any other node."""
-    if not (isinstance(e, ColumnExpr) and e.kind == Kind.CALL and e.head.upper() in ("CASE", "IF", "IIF", "NULLIF")):
+    s = scalar_head(e.head) if isinstance(e, ColumnExpr) and e.kind == Kind.CALL else None
+    if s is None or s[1].result != "case":
         return None
     out: List[str] = []
-    for r in _result_args(e):
+    for r in result_args(e):
         r = _operand(r)
         if r.kind != Kind.LITERAL or r.as_type is not None or not (r.value is None or isinstance(r.value, str)):
             return None
@@ -685,7 +754,7 @@ def case_string_results(e: Any) -> Optional[List[str]]:
 
 
 def _check_results(e: ColumnExpr) -> ColumnExpr:
-    lits = [r for r in _result_args(e) if r.kind == Kind.LITERAL and r.value is not None]
+    lits = [r for r in result_args(e) if r.kind == Kind.LITERAL and r.value is not None]
     if any(isinstance(r.value, str) for r in lits) and not all(isinstance(r.value, str) for r in lits):
         raise ValueError(f"{e.head} mixes string and numeric results: {e}")
     return e
@@ -707,7 +776,7 @@ class functions:
 
     @staticmethod
     def coalesce(*args: Any) -> ColumnExpr:
-        return function("COALESCE", *[_operand(x) for x in args])
+        return _call("COALESCE", *args)
 
     @staticmethod
     def case(branches: Sequence[Tuple[Any, Any]], else_: Any = None) -> ColumnExpr:
@@ -717,123 +786,107 @@ class functions:
         branches = list(branches)
         if not branches:
             raise ValueError("CASE needs at least one WHEN branch")
-        args: List[ColumnExpr] = []
+        args: List[Any] = []
         for b in branches:
             if not isinstance(b, tuple) or len(b) != 2:
                 raise ValueError(f"a CASE branch is a (condition, value) pair, got {b!r}")
-            args += [_operand(b[0]), _operand(b[1])]
-        return _check_results(ColumnExpr(Kind.CALL, "CASE", args + [_operand(else_)]))
+            args += list(b)
+        return _check_results(_call("CASE", *args, else_))
 
     @staticmethod
     def nullif(a: Any, b: Any) -> ColumnExpr:
         """SQL ``NULLIF(a, b)``: NULL where ``a = b`` is TRUE, else ``a``."""
-        return ColumnExpr(Kind.CALL, "NULLIF", [_operand(a), _operand(b)])
+        return _call("NULLIF", a, b)
 
     @staticmethod
     def abs(c: Any) -> ColumnExpr:  # noqa: A003
         """``|c|``; an integer wraps at INT64_MIN as unary ``-`` does."""
-        return ColumnExpr(Kind.CALL, "ABS", [_operand(c)])
+        return _call("ABS", c)
 
     @staticmethod
     def floor(c: Any) -> ColumnExpr:
-        return ColumnExpr(Kind.CALL, "FLOOR", [_operand(c)])
+        return _call("FLOOR", c)
 
     @staticmethod
     def ceil(c: Any) -> ColumnExpr:
-        return ColumnExpr(Kind.CALL, "CEIL", [_operand(c)])
+        return _call("CEIL", c)
 
     @staticmethod
     def round(c: Any, d: Any = 0) -> ColumnExpr:  # noqa: A003
         """SQL ``ROUND(c, d)``: to ``d`` decimal digits (an int literal in [-18, 18]), half away from zero."""
-        if isinstance(d, ColumnExpr) and d.kind == Kind.LITERAL and d.as_type is None:
-            d = d.value
-        if isinstance(d, bool) or not isinstance(d, int) or not -ROUND_MAX_DIGITS <= d <= ROUND_MAX_DIGITS:
-            raise ValueError(f"ROUND takes an integer literal in [-{ROUND_MAX_DIGITS}, {ROUND_MAX_DIGITS}] as its "
-                             f"digits, got {d!r}")
-        return ColumnExpr(Kind.CALL, "ROUND", [_operand(c), lit(d)])
+        return _call("ROUND", c, round_digits(d))
 
     @staticmethod
     def sqrt(c: Any) -> ColumnExpr:
-        return ColumnExpr(Kind.CALL, "SQRT", [_operand(c)])
+        return _call("SQRT", c)
 
     @staticmethod
     def exp(c: Any) -> ColumnExpr:
-        return ColumnExpr(Kind.CALL, "EXP", [_operand(c)])
+        return _call("EXP", c)
 
     @staticmethod
     def ln(c: Any) -> ColumnExpr:
-        return ColumnExpr(Kind.CALL, "LN", [_operand(c)])
+        return _call("LN", c)
 
     @staticmethod
     def log10(c: Any) -> ColumnExpr:
-        return ColumnExpr(Kind.CALL, "LOG10", [_operand(c)])
+        return _call("LOG10", c)
 
     @staticmethod
     def power(a: Any, b: Any) -> ColumnExpr:
-        return ColumnExpr(Kind.CALL, "POWER", [_operand(a), _operand(b)])
+        return _call("POWER", a, b)
 
     @staticmethod
     def greatest(*args: Any) -> ColumnExpr:
         """The largest non-NULL argument (NULL only if all are NULL); floats in the order of aggregate MAX."""
-        if len(args) < 2:
-            raise ValueError("GREATEST needs at least two arguments")
-        return ColumnExpr(Kind.CALL, "GREATEST", [_operand(x) for x in args])
+        return _call("GREATEST", *args)
 
     @staticmethod
     def least(*args: Any) -> ColumnExpr:
         """The smallest non-NULL argument (NULL only if all are NULL); floats in the order of aggregate MIN."""
-        if len(args) < 2:
-            raise ValueError("LEAST needs at least two arguments")
-        return ColumnExpr(Kind.CALL, "LEAST", [_operand(x) for x in args])
+        return _call("LEAST", *args)
 
     @staticmethod
     def length(c: Any) -> ColumnExpr:
         """SQL ``LENGTH(c)``: the number of characters (code points) of a string, int64."""
-        return ColumnExpr(Kind.CALL, "LENGTH", [col(c)])
+        return _call("LENGTH", col(c))
 
     @staticmethod
     def upper(c: Any) -> ColumnExpr:
         """SQL ``UPPER(c)``: every code point by its simple (one to one) Unicode upper-case mapping."""
-        return ColumnExpr(Kind.CALL, "UPPER", [col(c)])
+        return _call("UPPER", col(c))
 
     @staticmethod
     def lower(c: Any) -> ColumnExpr:
         """SQL ``LOWER(c)``: every code point by its simple (one to one) Unicode lower-case mapping."""
-        return ColumnExpr(Kind.CALL, "LOWER", [col(c)])
+        return _call("LOWER", col(c))
 
     @staticmethod
     def substr(c: Any, start: Any, length: Any = None) -> ColumnExpr:
         """SQLite ``SUBSTR(c, start[, length])`` in code points: 1-based; a negative start counts from the end;
         a negative length takes the code points before start.  ``start`` / ``length`` are int literals; NULL
         (``null()``) gives NULL, and ``length=None`` means no length."""
-        args = [col(c), _int_arg("SUBSTR", "start", start)]
-        if length is not None:
-            args.append(_int_arg("SUBSTR", "length", length))
-        return ColumnExpr(Kind.CALL, "SUBSTR", args)
-
-    @staticmethod
-    def _trim(fn: str, c: Any, chars: Any) -> ColumnExpr:
-        return ColumnExpr(Kind.CALL, fn, [col(c)] + ([] if chars is None else [_str_arg(fn, "characters", chars)]))
+        return _call("SUBSTR", col(c), start, *([] if length is None else [length]))
 
     @staticmethod
     def trim(c: Any, chars: Any = None) -> ColumnExpr:
         """SQLite ``TRIM(c[, chars])``: removes the code points of ``chars`` (default: the space U+0020 only)
         from both ends."""
-        return functions._trim("TRIM", c, chars)
+        return _call("TRIM", col(c), *([] if chars is None else [chars]))
 
     @staticmethod
     def ltrim(c: Any, chars: Any = None) -> ColumnExpr:
-        return functions._trim("LTRIM", c, chars)
+        return _call("LTRIM", col(c), *([] if chars is None else [chars]))
 
     @staticmethod
     def rtrim(c: Any, chars: Any = None) -> ColumnExpr:
-        return functions._trim("RTRIM", c, chars)
+        return _call("RTRIM", col(c), *([] if chars is None else [chars]))
 
     @staticmethod
     def replace(c: Any, from_: Any, to: Any) -> ColumnExpr:
         """SQLite ``REPLACE(c, from_, to)``: every non-overlapping ``from_``, left to right, by ``to``; an empty
         ``from_`` leaves ``c`` unchanged."""
-        return ColumnExpr(Kind.CALL, "REPLACE", [col(c), _str_arg("REPLACE", "from", from_), _str_arg("REPLACE", "to", to)])
+        return _call("REPLACE", col(c), from_, to)
 
     @staticmethod
     def regexp_matches(c: Any, pattern: Any) -> ColumnExpr:
@@ -844,7 +897,7 @@ class functions:
         p = _str_arg("REGEXP_MATCHES", "pattern", pattern)
         if p.value is not None:
             regex.parse(p.value)
-        return ColumnExpr(Kind.CALL, "REGEXP_MATCHES", [col(c), p])
+        return _call("REGEXP_MATCHES", col(c), p)
 
     @staticmethod
     def regexp_full_match(c: Any, pattern: Any) -> ColumnExpr:
@@ -854,7 +907,7 @@ class functions:
         p = _str_arg("REGEXP_FULL_MATCH", "pattern", pattern)
         if p.value is not None:
             regex.parse(p.value)
-        return ColumnExpr(Kind.CALL, "REGEXP_FULL_MATCH", [col(c), p])
+        return _call("REGEXP_FULL_MATCH", col(c), p)
 
     @staticmethod
     def regexp_extract(c: Any, pattern: Any, group: Any = 0) -> ColumnExpr:
@@ -863,13 +916,12 @@ class functions:
         pattern's group count is a ValueError."""
         from . import regex
 
-        p = _str_arg("REGEXP_EXTRACT", "pattern", pattern)
-        g = _int_arg("REGEXP_EXTRACT", "group", group)
+        _, (s, p, g) = check_call("REGEXP_EXTRACT", [col(c), pattern, group])
         if p.value is not None:
             regex.parse(p.value)
             if g.value is not None:
                 regex.check_group(p.value, g.value)
-        return ColumnExpr(Kind.CALL, "REGEXP_EXTRACT", [col(c), p] + ([] if g.value == 0 else [g]))
+        return ColumnExpr(Kind.CALL, "REGEXP_EXTRACT", [s, p] + ([] if g.value == 0 else [g]))
 
     @staticmethod
     def regexp_replace(c: Any, pattern: Any, rewrite: Any, options: Any = None) -> ColumnExpr:
@@ -878,26 +930,20 @@ class functions:
         ``\\\\`` is a backslash."""
         from . import regex
 
-        p = _str_arg("REGEXP_REPLACE", "pattern", pattern)
-        r = _str_arg("REGEXP_REPLACE", "rewrite", rewrite)
-        args = [col(c), p, r]
-        if options is not None:
-            o = _str_arg("REGEXP_REPLACE", "options", options)
-            if o.value is not None:
-                regex.replace_options(o.value)
-            args.append(o)
+        e = _call("REGEXP_REPLACE", col(c), pattern, rewrite, *([] if options is None else [options]))
+        p, r, o = e.args[1], e.args[2], e.args[3] if len(e.args) > 3 else None
+        if o is not None and o.value is not None:
+            regex.replace_options(o.value)
         if p.value is not None:
             regex.parse(p.value)
             if r.value is not None:
                 regex.rewrite_tokens(p.value, r.value)
-        return ColumnExpr(Kind.CALL, "REGEXP_REPLACE", args)
+        return e
 
     @staticmethod
     def concat(*parts: Any) -> ColumnExpr:
         """SQLite ``CONCAT(a, ...)``: the parts joined; NULL parts are skipped (``CONCAT(NULL)`` is '')."""
-        if not parts:
-            raise ValueError("CONCAT needs at least one argument")
-        return ColumnExpr(Kind.CALL, "CONCAT", [_operand(x) for x in parts])
+        return _call("CONCAT", *parts)
 
     @staticmethod
     def concat_strict(*parts: Any) -> ColumnExpr:
@@ -937,7 +983,7 @@ class functions:
         target month (Jan 31 + 1 month = Feb 28 / 29), the time of day kept; Postgres, DuckDB, ``pandas.DateOffset``."""
         if isinstance(n, bool) or (not isinstance(n, (int, ColumnExpr))):
             raise ValueError(f"ADD_MONTHS: n must be an int or an integer expression, got {n!r}")
-        return ColumnExpr(Kind.CALL, "ADD_MONTHS", [_operand(c), _operand(n)])
+        return _call("ADD_MONTHS", c, n)
 
     @staticmethod
     def min(c: Any) -> ColumnExpr:  # noqa: A003
@@ -1253,7 +1299,7 @@ def to_sql(expr: ColumnExpr, enable_cast: bool = True, nested: bool = False) -> 
             body += " ESCAPE " + to_sql(expr.args[2], enable_cast)
         if nested:
             body = "(" + body + ")"
-    elif k == Kind.CALL and expr.head.upper() in REGEX_FUNCTIONS:
+    elif k == Kind.CALL and expr.head.upper() in SCALARS and SCALARS[expr.head.upper()].family == "regex":
         # the SQL parser reads a regular expression's string literals as written: only '' is a quote
         parts = [to_sql(expr.args[0], enable_cast)] + [
             "'" + x.value.replace("'", "''") + "'" if x.kind == Kind.LITERAL and isinstance(x.value, str)

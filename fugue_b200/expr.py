@@ -40,8 +40,9 @@ import torch
 
 from . import kernels as K
 from . import strings as ST
-from .column import (FLOAT_FUNCTIONS, REGEX_PREDICATES, ROUND_MAX_DIGITS, TEMPORAL_LITERALS, TIME_FIELDS, TIME_PARTS, ColumnExpr, Kind,
-                     case_string_results, col as _col, is_string_build, lit as _lit)
+from .column import (REGEX_PREDICATES, TEMPORAL_LITERALS, TIME_FIELDS, TIME_PARTS, ColumnExpr, Kind, Scalar,
+                     case_string_results, check_call, col as _col, is_string_build, lit as _lit, result_args, round_digits,
+                     scalar_head)
 from .schema import Schema
 from .table import B200Table, _storage_dtype, expr_type
 
@@ -146,38 +147,34 @@ class _OutOfResources(Exception):
 
 def _regex_pattern(e: ColumnExpr, fn: str) -> Optional[str]:
     """The pattern of REGEXP_MATCHES / REGEXP_FULL_MATCH (None: a NULL literal, so the result is NULL)."""
-    if len(e.args) != 2:
-        raise ValueError(f"{fn} takes 2 arguments: {e}")
     p = e.args[1]
     if p.kind != Kind.LITERAL or p.as_type is not None or not (p.value is None or isinstance(p.value, str)):
         raise NotImplementedError(f"{fn} needs a string literal pattern: {e}")
     return p.value
 
 
-def _lower(e: ColumnExpr) -> Optional[ColumnExpr]:
-    """The canonical node of a function spelled another way (no alias, no cast), or None:
-    IF / IIF -> CASE, NULLIF(a, b) -> CASE WHEN a = b THEN NULL ELSE a END, IFNULL -> COALESCE, MOD -> %,
-    POW -> POWER, CEILING -> CEIL."""
-    if e.kind != Kind.CALL:
-        return None
-    fn = e.func.upper()
-    args = [a if isinstance(a, ColumnExpr) else _lit(a) for a in e.args]
-    if fn in ("IF", "IIF", "NULLIF", "MOD") and len(args) != (3 if fn in ("IF", "IIF") else 2):
-        raise ValueError(f"{fn} takes {3 if fn in ('IF', 'IIF') else 2} arguments: {e}")
-    if fn in ("IF", "IIF"):
-        return ColumnExpr(Kind.CALL, "CASE", args)
-    if fn == "NULLIF":
+def _like_pattern(e: ColumnExpr) -> Tuple[str, Optional[str]]:
+    """The pattern and the escape character (None: none) of a LIKE."""
+    if not all(a.kind == Kind.LITERAL and isinstance(a.value, str) for a in e.args[1:]):
+        raise NotImplementedError(f"LIKE needs a string literal pattern: {e}")
+    return e.args[1].value, (e.args[2].value if len(e.args) > 2 else None)
+
+
+def _scalar(e: Any) -> Tuple[Optional[str], Optional[Scalar]]:
+    """The canonical head and ``SCALARS`` entry of a call, (None, None) for any other node."""
+    s = scalar_head(e.func) if isinstance(e, ColumnExpr) and e.kind == Kind.CALL else None
+    return s if s is not None else (None, None)
+
+
+def _canonical(e: ColumnExpr) -> ColumnExpr:
+    """A call of a ``SCALARS`` function, its arguments checked (``check_call``), in its canonical spelling (no alias,
+    no cast); NULLIF(a, b) as CASE WHEN a = b THEN NULL ELSE a END and MOD(a, b) as a % b."""
+    head, args = check_call(e.func, e.args)
+    if head == "NULLIF":
         return ColumnExpr(Kind.CALL, "CASE", [ColumnExpr(Kind.BINARY, "==", args), _lit(None), args[0]])
-    if fn == "IFNULL":
-        return ColumnExpr(Kind.CALL, "COALESCE", args)
-    if fn == "MOD":
+    if head == "MOD":
         return ColumnExpr(Kind.BINARY, "%", args)
-    if fn in ("POW", "CEILING"):
-        return ColumnExpr(Kind.CALL, "POWER" if fn == "POW" else "CEIL", args)
-    if e.head != fn and fn in ("CASE", "COALESCE", "ABS", "FLOOR", "CEIL", "ROUND", "GREATEST", "LEAST") + \
-            tuple(FLOAT_FUNCTIONS):
-        return ColumnExpr(Kind.CALL, fn, args)  # function("abs", x) is ABS(x)
-    return None
+    return ColumnExpr(Kind.CALL, head, args, e.kwargs)
 
 
 def _coalesce_cls(cs: Sequence[str]) -> str:
@@ -380,17 +377,14 @@ class _Program:
                 if _is_temporal_literal(d) and isinstance(d.value, datetime.timedelta) and (e.op == "+" or d is e.right):
                     return self._ttype(x)
             return None
-        if e.kind == Kind.CALL:
-            fn = e.func.upper()
-            if fn in ("DATE_TRUNC", "ADD_MONTHS"):
-                return self._operand_type(e.args[0]) if e.args else None
-            if fn in ("COALESCE", "IFNULL", "GREATEST", "LEAST", "CASE", "IF", "IIF", "NULLIF"):
-                args = e.args[1::2] + e.args[-1:] if fn == "CASE" else e.args[1:] if fn in ("IF", "IIF") else \
-                    e.args[:1] if fn == "NULLIF" else e.args
-                for a in args:
-                    tp = self._ttype(a)
-                    if tp is not None:
-                        return tp
+        s = _scalar(e)[1]
+        if s is not None and s.result == "operand":
+            return self._operand_type(e.args[0]) if e.args else None
+        if s is not None and s.family == "conditional":
+            for a in result_args(e):
+                tp = self._ttype(a)
+                if tp is not None:
+                    return tp
         return None
 
     def _operand_type(self, e: Any) -> Optional[pa.DataType]:
@@ -464,10 +458,10 @@ class _Program:
                         return _const_predicate(x, op == "<")
                     q += 1
             return ColumnExpr(Kind.BINARY, op, [x, _lit(q)])
-        if e.kind == Kind.CALL and e.func.upper() in ("COALESCE", "GREATEST", "LEAST", "CASE"):
-            args = [a if isinstance(a, ColumnExpr) else _lit(a) for a in e.args]
+        if e.kind == Kind.CALL and _scalar(e)[1].family == "conditional":
+            args = list(e.args)
             n = len(args)
-            results = [i for i in range(n) if e.func.upper() != "CASE" or i % 2 == 1 or i == n - 1]
+            results = [i for i in range(n) if e.head != "CASE" or i % 2 == 1 or i == n - 1]
             if not any(_is_temporal_literal(args[i]) for i in results):
                 return e
             tp = self._ttype(e)
@@ -498,9 +492,7 @@ class _Program:
         return time_unit(tp)[1]
 
     def _temporal_function(self, e: ColumnExpr, fn: str) -> Tuple[str, bool]:
-        args = [a if isinstance(a, ColumnExpr) else _lit(a) for a in e.args]
-        if len(args) != (1 if fn in ("EXTRACT", "DATE_TRUNC") else 2):
-            raise ValueError(f"{fn} takes {1 if fn in ('EXTRACT', 'DATE_TRUNC') else 2} value argument(s): {e}")
+        args = e.args
         word = e.kwargs.get("field" if fn == "EXTRACT" else "part")
         if fn != "ADD_MONTHS":
             known = TIME_FIELDS + ("epoch",) if fn == "EXTRACT" else TIME_PARTS
@@ -593,28 +585,24 @@ class _Program:
             r = self._temporal_operands(e)
             return self._binary(r) if r.kind == Kind.BINARY else self._node(r)
         if e.kind == Kind.CALL:
-            low = _lower(e)
-            if low is not None:
-                return self._node(low)
+            if _scalar(e)[0] is None:
+                raise NotImplementedError(f"function {e.func} has no device implementation")
+            e = _canonical(e)
+            if e.kind != Kind.CALL:
+                return self._node(e)
             e = self._temporal_operands(e)
-            fn = e.func.upper()
-            if fn in ("EXTRACT", "DATE_TRUNC", "DATEDIFF", "ADD_MONTHS"):
+            fn, s = _scalar(e)
+            if s.family == "temporal":
                 return self._temporal_function(e, fn)
+            if s.family in ("string", "regex"):  # the string-building ones were refused above
+                return self._string_function(e, fn)
+            if fn == "POWER":
+                return self._binary(ColumnExpr(Kind.BINARY, "**", e.args))
+            if s.family == "numeric":
+                return self._unary_function(e, fn)
             if fn == "COALESCE":
                 return self._coalesce(e)
-            if fn in ("LIKE", "LENGTH") or fn in REGEX_PREDICATES:
-                return self._string_function(e, fn)
-            if fn == "CASE":
-                return self._case(e)
-            if fn in self._UNARY_FN:
-                return self._unary_function(e, fn)
-            if fn == "POWER":
-                if len(e.args) != 2:
-                    raise ValueError(f"POWER takes 2 arguments: {e}")
-                return self._binary(ColumnExpr(Kind.BINARY, "**", e.args))
-            if fn in ("GREATEST", "LEAST"):
-                return self._greatest(e, fn)
-            raise NotImplementedError(f"function {e.func} has no device implementation")
+            return self._case(e) if fn == "CASE" else self._greatest(e, fn)
         raise NotImplementedError(f"can't evaluate {e!r}")
 
     def _binary(self, e: ColumnExpr) -> Tuple[str, bool]:
@@ -735,16 +723,11 @@ class _Program:
             if key not in self.tables:
                 self.tables[key] = ST.regex_table(d, t.device, pattern, key[3])
         elif fn == "LIKE":
-            lits = e.args[1:]
-            if not (1 <= len(lits) <= 2 and all(a.kind == Kind.LITERAL and isinstance(a.value, str) for a in lits)):
-                raise NotImplementedError(f"LIKE needs a string literal pattern: {e}")
-            pattern, escape = lits[0].value, (lits[1].value if len(lits) > 1 else None)
+            pattern, escape = _like_pattern(e)
             key = ("LIKE", s.name, pattern, escape)
             if key not in self.tables:
                 self.tables[key] = ST.like_table(d, t.device, pattern, escape)
         else:
-            if len(e.args) != 1:
-                raise ValueError(f"LENGTH takes one argument: {e}")
             key = ("LENGTH", s.name)
             if key not in self.tables:
                 self.tables[key] = ST.length_table(d, t.device)
@@ -760,11 +743,7 @@ class _Program:
             if pattern is None:
                 return self._node(_lit(None))
         elif fn == "LIKE":
-            lits = e.args[1:]
-            if not (1 <= len(lits) <= 2 and all(a.kind == Kind.LITERAL and isinstance(a.value, str) for a in lits)):
-                raise NotImplementedError(f"LIKE needs a string literal pattern: {e}")
-        elif len(e.args) != 1:
-            raise ValueError(f"LENGTH takes one argument: {e}")
+            pattern, escape = _like_pattern(e)
         d, nullable = self.string_codes(s)
         name, steps = ST.string_chain(s, t.dictionaries)
         if fn in REGEX_PREDICATES:
@@ -772,7 +751,6 @@ class _Program:
             if key not in self.tables:
                 self.tables[key] = ST.regex_table(d, t.device, pattern, key[3])
         elif fn == "LIKE":
-            pattern, escape = lits[0].value, (lits[1].value if len(lits) > 1 else None)
             key = ("LIKE", ("STR", name, steps), pattern, escape)
             if key not in self.tables:
                 self.tables[key] = ST.like_table(d, t.device, pattern, escape)
@@ -787,9 +765,7 @@ class _Program:
         return ("i" if fn == "LENGTH" else "b"), nullable or self.tables[key][1] is not None
 
     def _coalesce(self, e: ColumnExpr) -> Tuple[str, bool]:
-        args = [a if isinstance(a, ColumnExpr) else _lit(a) for a in e.args]
-        if len(args) == 0:
-            raise ValueError("COALESCE needs arguments")
+        args = e.args
         probe = [self._static_cls(a) for a in args]
         if "s" in probe:
             raise NotImplementedError(f"COALESCE on strings: {e}")
@@ -814,8 +790,8 @@ class _Program:
     def _case(self, e: ColumnExpr) -> Tuple[str, bool]:
         """CASE WHEN c1 THEN v1 ... ELSE e END: the ELSE first, then the branches from last to first, each
         ``acc <- c TRUE ? v : result so far`` (FB_X_SEL).  A leaf ELSE is read as the operand of the first select."""
-        args = [a if isinstance(a, ColumnExpr) else _lit(a) for a in e.args]
-        if len(args) < 3 or len(args) % 2 == 0:
+        args = list(e.args)
+        if len(args) % 2 == 0:
             raise ValueError(f"CASE needs (condition, value) pairs and an ELSE: {e}")
         results = args[1::2] + [args[-1]]
         probe = [self._static_cls(a) for a in results]
@@ -857,19 +833,8 @@ class _Program:
 
     def _unary_function(self, e: ColumnExpr, fn: str) -> Tuple[str, bool]:
         """ABS FLOOR CEIL ROUND keep the class (bool counts as int64); SQRT EXP LN LOG10 give float64."""
-        nargs = len(e.args)
-        if not (nargs == 1 or (fn == "ROUND" and nargs == 2)):
-            raise ValueError(f"{fn} takes {'1 or 2 arguments' if fn == 'ROUND' else '1 argument'}: {e}")
-        d = 0
-        if nargs == 2:
-            dl = e.args[1]
-            d = dl.value if isinstance(dl, ColumnExpr) and dl.kind == Kind.LITERAL and dl.as_type is None else dl
-            if isinstance(d, bool) or not isinstance(d, int):
-                raise NotImplementedError(f"ROUND digits must be an integer literal: {e}")
-            if not -ROUND_MAX_DIGITS <= d <= ROUND_MAX_DIGITS:
-                raise ValueError(f"ROUND digits {d} outside [-{ROUND_MAX_DIGITS}, {ROUND_MAX_DIGITS}]: {e}")
-        arg = e.args[0] if isinstance(e.args[0], ColumnExpr) else _lit(e.args[0])
-        cls, nullable = self.compile(arg)
+        d = round_digits(e.args[1]) if len(e.args) == 2 else 0
+        cls, nullable = self.compile(e.args[0])
         if cls == "s":
             raise NotImplementedError(f"{fn} of a string: {e}")
         opi, opf = self._UNARY_FN[fn]
@@ -891,9 +856,7 @@ class _Program:
 
     def _greatest(self, e: ColumnExpr, fn: str) -> Tuple[str, bool]:
         """GREATEST / LEAST: NULL operands are skipped; NULL only if every operand is NULL."""
-        args = [a if isinstance(a, ColumnExpr) else _lit(a) for a in e.args]
-        if len(args) < 2:
-            raise ValueError(f"{fn} needs at least two arguments: {e}")
+        args = e.args
         probe = [self._static_cls(a) for a in args]
         if "s" in probe:
             raise NotImplementedError(f"{fn} on strings: {e}")
@@ -921,9 +884,6 @@ class _Program:
         """Class an expression will evaluate to (without emitting code)."""
         if e.as_type is not None:
             return _cls_of(e.as_type)
-        low = _lower(e)
-        if low is not None:
-            return self._static_cls(low)
         if e.kind == Kind.NAMED:
             if e.name not in self.t.schema:
                 raise KeyError(f"column {e.name} is not in {self.t.schema}")
@@ -939,26 +899,25 @@ class _Program:
             return "i" if c == "b" else c
         if is_string_build(e):
             return "s"
+        if _scalar(e)[0] is not None:
+            e = _canonical(e)
         if e.kind == Kind.BINARY:
             if e.op in ("+", "-", "*", "/", "%", "**"):
                 cs = (self._static_cls(e.left), self._static_cls(e.right))
                 return "f" if (e.op in ("/", "**") or "f" in cs) else "i"
             return "b"
-        if e.kind == Kind.CALL and e.func.upper() == "COALESCE":
-            cs = [self._static_cls(a if isinstance(a, ColumnExpr) else _lit(a)) for a in e.args]
-            return "f" if "f" in cs else ("b" if "b" in cs and all(c in ("b", "n") for c in cs) else "i")
-        if e.kind == Kind.CALL and (e.func.upper() == "LIKE" or e.func.upper() in REGEX_PREDICATES):
-            return "b"
-        if e.kind == Kind.CALL and e.func.upper() in FLOAT_FUNCTIONS:
-            return "f"
-        if e.kind == Kind.CALL and e.func.upper() == "EXTRACT" and str(e.kwargs.get("field", "")).lower() == "epoch":
-            return "f"
-        if e.kind == Kind.CALL and e.func.upper() in ("CASE", "GREATEST", "LEAST"):
-            args = e.args[1::2] + e.args[-1:] if e.func.upper() == "CASE" else e.args
-            cs = [self._static_cls(a if isinstance(a, ColumnExpr) else _lit(a)) for a in args]
+        s = _scalar(e)[1]
+        if s is None:
+            return "i"
+        if s.result in ("bool", "float64"):
+            return s.result[0]
+        if s.result == "extract":
+            return "f" if str(e.kwargs.get("field", "")).lower() == "epoch" else "i"
+        if s.family == "conditional":
+            cs = [self._static_cls(a) for a in result_args(e)]
             return "s" if "s" in cs else _coalesce_cls(cs)
-        if e.kind == Kind.CALL and e.func.upper() in ("ABS", "FLOOR", "CEIL", "ROUND") and e.args:
-            c = self._static_cls(e.args[0] if isinstance(e.args[0], ColumnExpr) else _lit(e.args[0]))
+        if s.family == "numeric":  # ABS FLOOR CEIL ROUND keep the class
+            c = self._static_cls(e.args[0])
             return "i" if c == "b" else c
         return "i"
 
@@ -1161,8 +1120,7 @@ def project(t: B200Table, exprs: Sequence[ColumnExpr]) -> B200Table:
 
 def _coded_case(e: ColumnExpr, strs: List[str]) -> ColumnExpr:
     """A CASE / IF / IIF / NULLIF with string-literal results as CASE with their codes in ``strs`` as results."""
-    low = _lower(e) or ColumnExpr(e.kind, e.head, e.args)
-    args = [a if isinstance(a, ColumnExpr) else _lit(a) for a in low.args]
+    args = list(_canonical(e).args)
     code = {s: j for j, s in enumerate(strs)}
     for j in list(range(1, len(args) - 1, 2)) + [len(args) - 1]:
         if args[j].value is not None:

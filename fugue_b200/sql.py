@@ -33,7 +33,8 @@ from typing import Any, Dict, List, Tuple
 
 import pyarrow as pa
 
-from .column import BIVARIATES, ColumnExpr, Kind, SelectColumns, all_cols, col, function, functions, is_agg, lit, null
+from .column import (BIVARIATES, ColumnExpr, Kind, SelectColumns, all_cols, check_arity, col, function, functions, is_agg,
+                     lit, null, scalar_head)
 from .dataframe import DataFrame
 
 _AGG = r"(SUM|COUNT|MIN|MAX|AVG|MEAN)\s*\(\s*(\*|[A-Za-z_][\w]*)\s*\)"
@@ -324,19 +325,14 @@ _AGG_FUNCS = {"SUM": functions.sum, "COUNT": functions.count, "MIN": functions.m
 _BIVARIATE_FUNCS = {name: getattr(functions, name.lower()) for name in BIVARIATES}
 _CLAUSES = ("WHERE", "GROUP", "HAVING", "ORDER", "LIMIT")
 _CASE_WORDS = ("WHEN", "THEN", "ELSE", "END")  # never a column name or an implicit alias
-_ONE_ARG = {"ABS": functions.abs, "FLOOR": functions.floor, "CEIL": functions.ceil, "CEILING": functions.ceil,
-            "SQRT": functions.sqrt, "EXP": functions.exp, "LN": functions.ln, "LOG10": functions.log10}
-_STRING_ARGS = {"UPPER": (1, 1), "LOWER": (1, 1), "SUBSTR": (2, 3), "SUBSTRING": (2, 3), "TRIM": (1, 2),
-                "LTRIM": (1, 2), "RTRIM": (1, 2), "REPLACE": (3, 3)}
-_STRING_BUILDERS = {"UPPER": functions.upper, "LOWER": functions.lower, "SUBSTR": functions.substr,
-                    "SUBSTRING": functions.substr, "TRIM": functions.trim, "LTRIM": functions.ltrim,
-                    "RTRIM": functions.rtrim, "REPLACE": functions.replace}
 _FIELD_FUNCS = {"YEAR": "year", "MONTH": "month", "DAY": "day", "HOUR": "hour", "MINUTE": "minute", "SECOND": "second",
                 "QUARTER": "quarter", "DAYOFWEEK": "dow", "DAYOFYEAR": "doy", "WEEK": "week"}
-_REGEX_CALLS = ("REGEXP_MATCHES", "REGEXP_LIKE", "REGEXP_FULL_MATCH", "REGEXP_EXTRACT", "REGEXP_REPLACE")
 _MONTHS = "INTERVAL_MONTHS"  # a calendar interval literal: only the operand of + / - next to a date or timestamp
-_TWO_ARGS = {"NULLIF": functions.nullif, "IFNULL": functions.coalesce, "MOD": lambda a, b: a % b,
-             "POWER": functions.power, "POW": functions.power}
+# the trees of the column.SCALARS heads that are not the ``functions`` builder of the same name (CASE: IF / IIF)
+_SCALAR_FORMS = {"CASE": lambda c, v, e: functions.case([(c, v)], e), "MOD": lambda a, b: a % b,
+                 "LIKE": lambda *args: function("LIKE", *args),
+                 "ADD_MONTHS": lambda x, n: functions.add_months(x, n.value if n.kind == Kind.LITERAL and
+                                                                 n.as_type is None else n)}
 
 
 # SQL type names inside CAST(... AS type), as schema types; every other name is read by the schema grammar
@@ -475,26 +471,6 @@ class _Parser:
         self.i += 1
         return val[1:-1].replace("''", "'")
 
-    def _regex_call(self, fn: str) -> ColumnExpr:
-        """``REGEXP_MATCHES / REGEXP_LIKE / REGEXP_FULL_MATCH / REGEXP_EXTRACT / REGEXP_REPLACE(s, 'p', ...)``; the
-        string literal arguments are read as written (``_raw_string``)."""
-        self.i += 2  # name (
-        args: List[Any] = [self.expr()]
-        while self.op(","):
-            args.append(self._raw_string() if self.peek()[0] == "str" else self.expr())
-        self.expect(")")
-        want = {"REGEXP_EXTRACT": (2, 3), "REGEXP_REPLACE": (3, 4)}.get(fn, (2, 2))
-        if not want[0] <= len(args) <= want[1]:
-            raise ValueError(f"{fn} takes {want[0] if want[0] == want[1] else f'{want[0]} to {want[1]}'} arguments, "
-                             f"got {len(args)} in: {self.sql}")
-        if fn in ("REGEXP_MATCHES", "REGEXP_LIKE"):
-            return functions.regexp_matches(*args)
-        if fn == "REGEXP_FULL_MATCH":
-            return functions.regexp_full_match(*args)
-        if fn == "REGEXP_EXTRACT":
-            return functions.regexp_extract(*args)
-        return functions.regexp_replace(*args)
-
     def _like(self, e: ColumnExpr) -> ColumnExpr:
         pattern = self._string_literal("LIKE")
         escape = self._string_literal("ESCAPE") if self.kw("ESCAPE") else None
@@ -609,8 +585,6 @@ class _Parser:
                     self.i += 1
                 self.expect(")")
                 return e.cast(_cast_type(tp))
-            if self.peek(1) == ("op", "(") and up in _REGEX_CALLS:
-                return self._regex_call(up)
             if self.peek(1) == ("op", "("):
                 return self._call(up)
             self.i += 1
@@ -725,51 +699,31 @@ class _Parser:
             arg = self.expr()
             self.expect(")")
             return functions.extract(_unquote(field) if kind == "str" else field, arg)
+        # a regular expression's string literals (after the string it tests) are read as written
+        scalar = scalar_head(fn)
+        raw = scalar is not None and scalar[1].family == "regex"
         args: List[Any] = []
         if not self.op(")"):
             while True:
-                args.append(self.expr())
+                args.append(self._raw_string() if raw and args and self.peek()[0] == "str" else self.expr())
                 if not self.op(","):
                     break
             self.expect(")")
-        if fn == "COALESCE":
-            return functions.coalesce(*args)
-        if fn in _FIELD_FUNCS or fn in ("DATE_PART", "DATE_TRUNC", "DATEDIFF", "DATE_DIFF", "ADD_MONTHS"):
+        if fn in _FIELD_FUNCS or fn in ("DATE_PART", "DATE_TRUNC", "DATEDIFF", "DATE_DIFF"):
             return self._temporal_call(fn, args)
-        if fn in _STRING_ARGS:
-            lo, hi = _STRING_ARGS[fn]
-            if not lo <= len(args) <= hi:
-                raise ValueError(f"{fn} takes {lo if lo == hi else f'{lo} to {hi}'} arguments, got {len(args)} in: "
-                                 f"{self.sql}")
-            return _STRING_BUILDERS[fn](*args)
-        if fn == "CONCAT":
-            return functions.concat(*args)
-        want = 1 if fn in _ONE_ARG else 2 if fn in _TWO_ARGS else 3 if fn in ("IF", "IIF") else None
-        if want is not None and len(args) != want:
-            raise ValueError(f"{fn} takes {want} argument(s), got {len(args)} in: {self.sql}")
-        if fn in _ONE_ARG:
-            return _ONE_ARG[fn](args[0])
-        if fn in _TWO_ARGS:
-            return _TWO_ARGS[fn](args[0], args[1])
-        if fn in ("IF", "IIF"):
-            return functions.case([(args[0], args[1])], args[2])
-        if fn == "ROUND":
-            if len(args) not in (1, 2):
-                raise ValueError(f"ROUND takes 1 or 2 arguments, got {len(args)} in: {self.sql}")
-            return functions.round(args[0], args[1] if len(args) == 2 else 0)
-        if fn in ("GREATEST", "LEAST"):
-            return functions.greatest(*args) if fn == "GREATEST" else functions.least(*args)
-        return function(fn, *args)
+        if scalar is None:
+            return function(fn, *args)
+        head = check_arity(fn, len(args))  # the builder checks the rest
+        return (_SCALAR_FORMS.get(head) or getattr(functions, head.lower()))(*args)
 
     def _temporal_call(self, fn: str, args: List[Any]) -> ColumnExpr:
+        """The SQL forms that pass a field or a part as an argument: YEAR(x) ..., DATE_PART('f', x), DATE_TRUNC('p',
+        x), DATEDIFF / DATE_DIFF('p', a, b)."""
         want = 1 if fn in _FIELD_FUNCS else 3 if fn in ("DATEDIFF", "DATE_DIFF") else 2
         if len(args) != want:
             raise ValueError(f"{fn} takes {want} argument(s), got {len(args)} in: {self.sql}")
         if fn in _FIELD_FUNCS:
             return functions.extract(_FIELD_FUNCS[fn], args[0])
-        if fn == "ADD_MONTHS":
-            n = args[1]
-            return functions.add_months(args[0], n.value if n.kind == Kind.LITERAL and n.as_type is None else n)
         word = args[0]
         if word.kind != Kind.LITERAL or not isinstance(word.value, str):
             raise ValueError(f"{fn} takes a string literal as its first argument, got {word} in: {self.sql}")

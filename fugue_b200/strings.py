@@ -39,7 +39,7 @@ import torch
 
 from . import kernels as K
 from . import regex as R
-from .column import ColumnExpr, Kind, is_string_build, lit
+from .column import ColumnExpr, Kind, check_call, is_string_build, lit
 
 _CACHE: Dict[int, Tuple[Any, Dict[Any, Any]]] = {}     # dictionary -> {device: DeviceDictionary}
 _DERIVED: Dict[int, Tuple[Any, Dict[Any, Any]]] = {}   # dictionary -> {(chain, device): StringResult}
@@ -167,21 +167,6 @@ def length_table(d: pa.Array, device: torch.device) -> Tuple[torch.Tensor, Optio
 
 
 # ---- string-building functions ------------------------------------------------------------------------
-_ARITY = {"UPPER": (0, 0), "LOWER": (0, 0), "SUBSTR": (1, 2), "TRIM": (0, 1), "LTRIM": (0, 1), "RTRIM": (0, 1),
-          "REPLACE": (2, 2), "REGEXP_EXTRACT": (1, 2), "REGEXP_REPLACE": (2, 3)}
-_ARG_TYPES = {"SUBSTR": (int, int), "REGEXP_EXTRACT": (str, int)}  # literal types after the string; else str
-
-
-def _literal(fn: str, e: ColumnExpr, want: type) -> Any:
-    """The value of a literal argument: an int (no bool) or a string, or None for NULL."""
-    if e.kind != Kind.LITERAL or e.as_type is not None:
-        raise NotImplementedError(f"{fn} takes literal arguments after the string, got {e}")
-    v = e.value
-    if v is not None and (isinstance(v, bool) or not isinstance(v, want)):
-        raise ValueError(f"{fn}: {v!r} is not a {want.__name__} literal")
-    return v
-
-
 def _utf8(fn: str, v: str) -> bytes:
     b = v.encode("utf-8")
     if len(b) > K.STR_MAX_LITERAL:
@@ -222,13 +207,9 @@ def string_chain(e: ColumnExpr, string_columns: Any) -> Tuple[str, Tuple[Any, ..
                                   f"got {x}")
 
     def chain(x: ColumnExpr) -> Tuple[str, Tuple[Any, ...]]:
-        fn = "||" if x.kind == Kind.BINARY else x.head.upper()
-        fn = "SUBSTR" if fn == "SUBSTRING" else fn
-        args = [a if isinstance(a, ColumnExpr) else lit(a) for a in x.args]
+        fn, args = ("||", list(x.args)) if x.kind == Kind.BINARY else check_call(x.head, x.args)
         if fn in ("CONCAT", "||"):
             parts = _concat_parts(x) if fn == "||" else args
-            if not parts:
-                raise ValueError(f"CONCAT needs at least one argument: {x}")
             toks: List[int] = []
             base: Any = None
             null = False
@@ -255,14 +236,7 @@ def string_chain(e: ColumnExpr, string_columns: Any) -> Tuple[str, Tuple[Any, ..
             name, steps = base[1]
             step = ("NULL",) if (fn == "||" and null) else ("FORMAT", tuple(toks), fn == "CONCAT")
             return name, steps + (step,)
-        if not args:
-            raise ValueError(f"{fn} needs a string argument: {x}")
-        lo, hi = _ARITY[fn]
-        rest = args[1:]
-        if not lo <= len(rest) <= hi:
-            n = f"{lo + 1}" if lo == hi else f"{lo + 1} to {hi + 1}"
-            raise ValueError(f"{fn} takes {n} arguments: {x}")
-        vals = [_literal(fn, a, _ARG_TYPES.get(fn, (str, str, str))[i]) for i, a in enumerate(rest)]
+        vals = [a.value for a in args[1:]]  # literals of the types column.SCALARS gives
         name, steps = operand(args[0])
         if any(v is None for v in vals):
             return name, steps + (("NULL",),)

@@ -145,7 +145,13 @@ def sums_bound(values: Sequence[float], route: str) -> Tuple[float, float, float
         e = 2 * m * U * X
         return tuple((k + 1) * (m + 4) * U * b(k, e) * 1.01 for k in (2, 3, 4))  # type: ignore[return-value]
     assert route == "scan", route
-    return tuple(4 * (m + 4) * U * (b(k) + k * X * b(k - 1)) * 1.01 for k in (2, 3, 4))  # type: ignore[return-value]
+    return scan_bound(m, X, [b(k) for k in (1, 2, 3, 4)])
+
+
+def scan_bound(m: Any, X: Any, b: Sequence[Any]) -> Tuple[Any, Any, Any]:
+    """The ``"scan"`` bounds of ``sums_bound`` from m, X and b = (B_1, B_2, B_3, B_4); any upper bounds on X and the
+    B_k give sound (looser) bounds.  Plain arithmetic, so numpy arrays of rows work as well as floats."""
+    return tuple(4 * (m + 4) * U * (b[k - 1] + k * X * b[k - 2]) * 1.01 for k in (2, 3, 4))  # type: ignore
 
 
 def result_bound(fn: str, values: Sequence[float], route: str) -> float:
@@ -153,8 +159,13 @@ def result_bound(fn: str, values: Sequence[float], route: str) -> float:
     statistic over the box of central sums within ``sums_bound``, plus eight roundings of the finishing formula.
     Infinite when the box reaches M2 <= 0 (the data is too close to constant for the algorithm to say)."""
     m, *exact = central_sums(values)
-    e2, e3, e4 = (float(q) for q in exact)
-    d2, d3, d4 = sums_bound(values, route)
+    return box_bound(fn, m, [float(q) for q in exact], sums_bound(values, route))
+
+
+def box_bound(fn: str, m: int, exact: Sequence[float], bounds: Sequence[float]) -> float:
+    """``result_bound`` from m, the exact (M2, M3, M4) rounded to float and the bounds on them."""
+    e2, e3, e4 = exact
+    d2, d3, d4 = bounds
     if e2 == 0 and d2 == 0:
         return 0.0
     if e2 - d2 <= 0:

@@ -74,11 +74,17 @@ def check_result(fn: str, got: Optional[float], vals: List[Optional[float]], sca
     if math.isnan(want):
         assert math.isnan(got)
         return
-    div = len(vals) - 1 if fn.endswith("_SAMP") else len(vals)
-    var = float(OM.exact_m2(vals) / div)
-    tol = m2_tol(vals, scan) / div + 2 * U * var
+    check_finite_result(fn, got, len(vals), OM.exact_m2(vals), m2_tol(vals, scan))
+
+
+def check_finite_result(fn: str, got: float, m: int, m2: Fraction, m2_bound: float) -> None:
+    """``check_result`` of m finite values (at least the function's minimum count) from their exact M2 and the
+    bound on the computed M2."""
+    div = m - 1 if fn.endswith("_SAMP") else m
+    var = float(m2 / div)
+    tol = m2_bound / div + 2 * U * var
     g = got * got if fn.startswith("STDDEV") else got
-    assert abs(g - var) <= tol + (4 * U * var if fn.startswith("STDDEV") else 0), (fn, len(vals), got, want)
+    assert abs(g - var) <= tol + (4 * U * var if fn.startswith("STDDEV") else 0), (fn, m, got, var)
 
 
 # ---- K6 kernel paths ---------------------------------------------------------------------------------

@@ -566,17 +566,21 @@ def raw_sql(*statements: Any, engine: Any = None, engine_conf: Any = None, as_fu
             as_local: bool = False) -> Any:
     """``fa.raw_sql`` (fugue/sql/api.py): strings and dataframes interleaved, e.g.
     ``fa.raw_sql("SELECT key, SUM(v0) AS s, COUNT(*) AS c FROM", df, "GROUP BY key")``."""
-    from .column import has_window
+    from .column import ColumnExpr, has_bare_window, to_sql
     from .sql import StructuredRawSQL
 
-    e = make_execution_engine(engine, engine_conf, infer_by=[s for s in statements if not isinstance(s, str)])
+    e = make_execution_engine(engine, engine_conf, infer_by=[s for s in statements
+                                                             if not isinstance(s, (str, ColumnExpr))])
     dfs: Dict[str, Any] = {}
     pieces = []
     for s in statements:
-        assert_or_throw(not has_window(s), lambda: NotImplementedError(
-            f"{s}: window functions are not part of the SQL dialect; use them in a ColumnMap of fa.transform"))
+        assert_or_throw(not has_bare_window(s), lambda: NotImplementedError(
+            f"{s}: a window function without PARTITION BY / ORDER BY has no SQL form; give it "
+            "over(partition_by=.., order_by=..), or use it in a ColumnMap of fa.transform"))
         if isinstance(s, str):
             pieces.append((False, s))
+        elif isinstance(s, ColumnExpr):  # an expression piece: its SQL text
+            pieces.append((False, to_sql(s)))
         else:
             name = f"_{len(dfs)}"
             dfs[name] = e.to_df(s)

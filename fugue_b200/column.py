@@ -95,6 +95,7 @@ SHAPES = frozenset(h for h, a in AGGREGATES.items() if a.family == "shape")
 BIVARIATES = frozenset(h for h, a in AGGREGATES.items() if a.family == "bivariate")
 _AGG_ALIASES = {"STDDEV": "STDDEV_SAMP", "VARIANCE": "VAR_SAMP", "SKEW": "SKEWNESS", "KURT": "KURTOSIS"}
 _RANKINGS = frozenset(["ROW_NUMBER", "RANK", "DENSE_RANK"])
+_SPEC_ONLY = _RANKINGS | {"LAG", "LEAD"}  # window heads that take a partition and an order but no frame
 _RUNNING_FRAME = "ROWS BETWEEN UNBOUNDED PRECEDING AND CURRENT ROW"
 _LITERAL_TYPES = (int, bool, float, str, datetime.date, datetime.datetime, datetime.timedelta)
 TEMPORAL_LITERALS = (datetime.date, datetime.datetime, datetime.timedelta)
@@ -407,7 +408,8 @@ class ColumnExpr:
         return functions.regexp_matches(self, pattern)
 
     def over(self, running: bool = False, rows: Optional[Tuple[Optional[int], Optional[int]]] = None,
-             range: Optional[Tuple[Any, Any]] = None) -> "ColumnExpr":  # noqa: A002 - the SQL word
+             range: Optional[Tuple[Any, Any]] = None,  # noqa: A002 - the SQL word
+             partition_by: Optional[Sequence[Any]] = None, order_by: Optional[Sequence[Any]] = None) -> "ColumnExpr":
         """The aggregation as a window function of a ``ColumnMap``: over the whole logical partition
         (``running=False``, the value repeated on every row), over the rows up to and including the
         current one in presort order (``running=True``), over a moving frame ``rows=(start, end)``:
@@ -416,7 +418,22 @@ class ColumnExpr:
         BETWEEN`` offsets in the units of the presort column (``int``, finite ``float`` or
         ``datetime.timedelta``; 0 is CURRENT ROW, the current row's peers).  ``rows=(None, 0)`` is
         ``running=True``, and ``rows=(None, None)`` and ``range=(None, None)`` are the whole partition: they
-        give those nodes.  ``range=(None, 0)`` is not ``running=True``: it includes the current row's peers."""
+        give those nodes.  ``range=(None, 0)`` is not ``running=True``: it includes the current row's peers.
+
+        ``partition_by`` (names or expressions) and ``order_by`` (names, expressions or ``(name_or_expr,
+        ascending)`` pairs) make the node explicit: it carries its own partition and order, SQL's ``OVER
+        (PARTITION BY .. ORDER BY ..)``, and runs in ``select / assign / filter`` and SQL, not in a ``ColumnMap``.
+        Either one given, even as ``[]``, makes it explicit; ``partition_by=[]`` alone is ``OVER ()``, the whole
+        table.  NULLs sort last in both directions.  The frame keeps the meaning above (the default is the whole
+        partition, not SQL's running default of a statement with ORDER BY).  ROW_NUMBER, RANK, DENSE_RANK, LAG and
+        LEAD take a spec and no frame; a percentile takes ``partition_by`` only."""
+        explicit = partition_by is not None or order_by is not None
+        spec = _window_spec(self, partition_by, order_by) if explicit else {}
+        if self.kind == Kind.WINDOW and self.head in _SPEC_ONLY and explicit and not is_explicit(self):
+            if running or rows is not None or range is not None:
+                raise ValueError(f"{self}: {self.head} takes no frame")
+            return ColumnExpr(Kind.WINDOW, self.head, self.args, {**self.kwargs, **spec}, False, self.as_name,
+                              self.as_type)
         if self.kind != Kind.AGG:
             raise ValueError(f"{self} is not an aggregation: only an aggregation has an OVER form")
         if self.is_distinct:
@@ -429,7 +446,10 @@ class ColumnExpr:
         if a.frames == "none":
             if running or rows is not None or range is not None:
                 raise ValueError(f"{self}: a percentile covers the whole partition; it takes no frame")
-            return ColumnExpr(Kind.WINDOW, self.head, self.args, self.kwargs, False, self.as_name, self.as_type)
+            if spec.get("order_by"):
+                raise ValueError(f"{self}: a percentile covers the whole partition; it takes no ORDER BY")
+            return ColumnExpr(Kind.WINDOW, self.head, self.args, {**self.kwargs, **spec}, False, self.as_name,
+                              self.as_type)
         if range is not None:
             if running or rows is not None:
                 raise ValueError("over() takes one of running=True, rows and range")
@@ -451,17 +471,22 @@ class ColumnExpr:
             elif rows == (None, None):
                 rows = None
         if a.frames == "running" and (rows is not None or range is not None):
+            hint = "; write ROWS BETWEEN UNBOUNDED PRECEDING AND CURRENT ROW for the running form" \
+                if range == (None, 0) else ""
             raise NotImplementedError(f"{self}: {self.head} runs over the whole partition or running=True; "
-                                      "ROWS and RANGE frames are not supported")
-        if any(is_agg(a) or has_window(a) for a in self.args):
+                                      f"ROWS and RANGE frames are not supported{hint}")
+        # a window over GROUP BY results (explicit only) may read aggregations; nothing reads a window
+        if any((is_agg(a) and not explicit) or has_window(a) for a in self.args):
             raise ValueError(f"nested aggregation {self}")
         if a.family == "pick" and self.args[0].kind == Kind.WILDCARD:
             raise ValueError(f"{self}: {self.head} needs a column")
+        if explicit and range is not None and any(b not in (None, 0) for b in range) and len(spec["order_by"]) != 1:
+            raise ValueError(f"{self}: a RANGE frame with an offset needs exactly one ORDER BY expression")
         if range is not None:
             kwargs: Dict[str, Any] = {"range": range}
         else:
             kwargs = {"running": running} if rows is None else {"rows": (rows[0], rows[1])}
-        return ColumnExpr(Kind.WINDOW, self.head, self.args, kwargs, False, self.as_name, self.as_type)
+        return ColumnExpr(Kind.WINDOW, self.head, self.args, {**kwargs, **spec}, False, self.as_name, self.as_type)
 
     def __bool__(self) -> bool:
         raise TypeError("a column expression has no truth value; use & | ~ to combine conditions")
@@ -489,6 +514,8 @@ def _canon(v: Any) -> str:
         inner = ",".join(_canon(a) for a in v.args) + ";" + ",".join(k + "=" + _canon(x) for k, x in v.kwargs.items())
         return (f"<{int(v.kind)}|{type(v.head).__name__}:{v.head!r}|{inner}|{int(v.is_distinct)}|{v.as_name}|"
                 f"{v.as_type}>")
+    if isinstance(v, tuple) and any(isinstance(x, (ColumnExpr, tuple)) for x in v):  # a window spec
+        return "(" + ",".join(_canon(x) for x in v) + ")"
     return f"{type(v).__name__}:{v!r}"
 
 
@@ -568,6 +595,19 @@ def _within_group(e: ColumnExpr, show: Any) -> str:
     return f"{e.head}({e.kwargs['q']!r}) WITHIN GROUP (ORDER BY {show(e.args[0])})"
 
 
+def _children(e: ColumnExpr) -> Iterator[ColumnExpr]:
+    """The sub-expressions of a node: its arguments, its keyword arguments and the expressions of a window spec."""
+    def walk(v: Any) -> Iterator[ColumnExpr]:
+        if isinstance(v, ColumnExpr):
+            yield v
+        elif isinstance(v, tuple):
+            for x in v:
+                yield from walk(x)
+
+    for v in list(e.args) + list(e.kwargs.values()):
+        yield from walk(v)
+
+
 def is_agg(column: Any) -> bool:
     """True when the expression contains an aggregation anywhere."""
     if not isinstance(column, ColumnExpr):
@@ -576,7 +616,7 @@ def is_agg(column: Any) -> bool:
         return True
     if column.kind == Kind.WINDOW:  # a window function is evaluated per row: not a GROUP BY aggregation
         return False
-    return any(is_agg(x) for x in column.args) or any(is_agg(x) for x in column.kwargs.values())
+    return any(is_agg(x) for x in _children(column))
 
 
 def has_window(column: Any) -> bool:
@@ -585,13 +625,78 @@ def has_window(column: Any) -> bool:
         return False
     if column.kind == Kind.WINDOW:
         return True
-    return any(has_window(x) for x in column.args) or any(has_window(x) for x in column.kwargs.values())
+    return any(has_window(x) for x in _children(column))
+
+
+def is_explicit(column: Any) -> bool:
+    """True for a window node with its own PARTITION BY / ORDER BY (``over(partition_by=.., order_by=..)``)."""
+    return isinstance(column, ColumnExpr) and column.kind == Kind.WINDOW and "partition_by" in column.kwargs
+
+
+def has_bare_window(column: Any) -> bool:
+    """True when the expression contains a window node without a spec: one that only a ``ColumnMap`` evaluates."""
+    if not isinstance(column, ColumnExpr):
+        return False
+    if column.kind == Kind.WINDOW and not is_explicit(column):
+        return True
+    return any(has_bare_window(x) for x in _children(column))
+
+
+def has_explicit_window(column: Any) -> bool:
+    """True when the expression contains a window node with its own PARTITION BY / ORDER BY."""
+    if not isinstance(column, ColumnExpr):
+        return False
+    return is_explicit(column) or any(has_explicit_window(x) for x in _children(column))
+
+
+def window_reads_agg(column: Any) -> bool:
+    """True when a window function of the expression reads an aggregation: a window over GROUP BY results."""
+    if not isinstance(column, ColumnExpr):
+        return False
+    if column.kind == Kind.WINDOW:
+        return any(is_agg(x) for x in _children(column))
+    return any(window_reads_agg(x) for x in _children(column))
+
+
+def _window_spec(e: ColumnExpr, partition_by: Any, order_by: Any) -> Dict[str, Any]:
+    """The ``partition_by`` / ``order_by`` kwargs of an explicit window node: a tuple of expressions and a tuple of
+    (expression, ascending) pairs, aliases dropped."""
+    def item(x: Any) -> ColumnExpr:
+        c = col(x) if isinstance(x, (str, ColumnExpr)) else None
+        if c is None or c.kind == Kind.WILDCARD or c.kind == Kind.LITERAL:
+            raise ValueError(f"{e}: a window partitions and orders by column expressions, got {x!r}")
+        if has_window(c):
+            raise ValueError(f"{e}: a window function inside another window's PARTITION BY / ORDER BY: {c}")
+        return c.alias("")
+
+    for what, v in (("partition_by", partition_by), ("order_by", order_by)):
+        if v is not None and (isinstance(v, (str, ColumnExpr)) or not isinstance(v, (list, tuple))):
+            raise ValueError(f"{what} must be a list, got {v!r}")
+    order = []
+    for x in order_by or []:
+        if isinstance(x, tuple):
+            if len(x) != 2 or not isinstance(x[1], bool):
+                raise ValueError(f"an ORDER BY item is a name, an expression or a (name_or_expr, ascending) pair, "
+                                 f"got {x!r}")
+            order.append((item(x[0]), x[1]))
+        else:
+            order.append((item(x), True))
+    return {"partition_by": tuple(item(x) for x in partition_by or []), "order_by": tuple(order)}
 
 
 def _window_text(e: ColumnExpr, show: Any) -> str:
-    """``FUNC(args) OVER (frame)`` of a WINDOW node; ``show`` renders one argument."""
+    """``FUNC(args) OVER (spec frame)`` of a WINDOW node; ``show`` renders one argument.  A bare node shows its
+    frame; an explicit one shows its frame only where it is not SQL's default for its spec (RANGE BETWEEN
+    UNBOUNDED PRECEDING AND CURRENT ROW with ORDER BY, the whole partition without), so that its text parses
+    back to the same node."""
+    spec = []
+    if is_explicit(e):
+        if e.kwargs["partition_by"]:
+            spec.append("PARTITION BY " + ", ".join(show(x) for x in e.kwargs["partition_by"]))
+        if e.kwargs["order_by"]:
+            spec.append("ORDER BY " + ", ".join(show(x) + ("" if asc else " DESC") for x, asc in e.kwargs["order_by"]))
     if e.head in PERCENTILES:
-        return _within_group(e, show) + " OVER ()"
+        return _within_group(e, show) + f" OVER ({' '.join(spec)})"
     parts = [show(x) for x in e.args]
     if e.head in ("LAG", "LEAD"):
         parts += [str(e.kwargs["n"]), _show_literal(e.kwargs["default"])]
@@ -600,7 +705,11 @@ def _window_text(e: ColumnExpr, show: Any) -> str:
         if unit in e.kwargs:
             frame = f"{unit.upper()} BETWEEN {_frame_bound(e.kwargs[unit][0], 'PRECEDING')} AND " \
                     f"{_frame_bound(e.kwargs[unit][1], 'FOLLOWING')}"
-    return f"{e.head}({','.join(parts)}) OVER ({frame})"
+    if is_explicit(e) and e.head not in _SPEC_ONLY:
+        default = "RANGE BETWEEN UNBOUNDED PRECEDING AND CURRENT ROW" if e.kwargs["order_by"] else ""
+        whole = "ROWS BETWEEN UNBOUNDED PRECEDING AND UNBOUNDED FOLLOWING"
+        frame = "" if frame == default else (frame or whole)
+    return f"{e.head}({','.join(parts)}) OVER ({' '.join(spec + ([frame] if frame else []))})"
 
 
 def _frame_bound(b: Any, unbounded: str) -> str:
@@ -651,13 +760,13 @@ def _range_frame(frame: Any) -> Tuple[Any, Any]:
     return start, end
 
 
-def _offset_fn(name: str, c: Any, n: Any, default: Any) -> ColumnExpr:
+def _offset_fn(name: str, c: Any, n: Any, default: Any, aggregated: bool = False) -> ColumnExpr:
     if isinstance(n, bool) or not isinstance(n, int) or n < 0:
         raise ValueError(f"{name}: n must be a non-negative int, got {n!r}")
     if not (default is None or isinstance(default, _LITERAL_TYPES)):
         raise ValueError(f"{name}: default must be a literal or None, got {default!r}")
     arg = col(c)
-    if arg.kind == Kind.WILDCARD or is_agg(arg) or has_window(arg):
+    if arg.kind == Kind.WILDCARD or (is_agg(arg) and not aggregated) or has_window(arg):
         raise ValueError(f"{name} needs a row-wise column expression, got {arg}")
     return ColumnExpr(Kind.WINDOW, name, [arg], {"n": n, "default": default})
 
@@ -765,9 +874,7 @@ def column_mentions(column: Any) -> Iterator[str]:
     if isinstance(column, ColumnExpr):
         if column.kind == Kind.NAMED:
             yield column.head
-        for a in column.args:
-            yield from column_mentions(a)
-        for a in column.kwargs.values():
+        for a in _children(column):
             yield from column_mentions(a)
 
 
@@ -1210,7 +1317,7 @@ class SelectColumns:
             if self._wildcards:
                 raise ValueError(f"'*' can't be used in aggregation: {self}")
             self.group_keys = [c.alias("").cast(None) for c in self.all_cols
-                               if self._role(c) in ("simple", "func")]
+                               if self._role(c) in ("simple", "func") and not has_window(c)]
 
     @staticmethod
     def _role(c: ColumnExpr) -> str:
@@ -1218,7 +1325,7 @@ class SelectColumns:
             return "literal"
         if c.kind in (Kind.NAMED, Kind.WILDCARD):
             return "simple"
-        return "agg" if is_agg(c) else "func"
+        return "agg" if is_agg(c) or window_reads_agg(c) else "func"
 
     def __str__(self) -> str:
         return "[" + ", ".join(str(x) for x in self.all_cols) + "]"

@@ -246,6 +246,33 @@ fb_gather_rows_kernel(const void* const* __restrict__ src_cols, void* const* __r
   }
 }
 
+// ---- row scatter: the inverse of the gather ----------------------------------------------------------
+// One thread per source row moves that row of every column, so the permutation is read once for all of
+// them.  idx is a permutation (the host passes argsort results), so every destination row is written once.
+__global__ void __launch_bounds__(256)
+fb_scatter_rows_kernel(const void* const* __restrict__ src_cols, void* const* __restrict__ dst_cols,
+                       const int32_t* __restrict__ widths, const uint8_t* const* __restrict__ src_valid,
+                       uint8_t* const* __restrict__ dst_valid, const int64_t* __restrict__ idx, int64_t n,
+                       int ncols) {
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n;
+       i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t r = idx[i];
+    for (int c = 0; c < ncols; ++c) {
+      switch (widths[c]) {
+        case 8: ((uint64_t*)dst_cols[c])[r] = ((const uint64_t*)src_cols[c])[i]; break;
+        case 4: ((uint32_t*)dst_cols[c])[r] = ((const uint32_t*)src_cols[c])[i]; break;
+        case 2: ((uint16_t*)dst_cols[c])[r] = ((const uint16_t*)src_cols[c])[i]; break;
+        default: ((uint8_t*)dst_cols[c])[r] = ((const uint8_t*)src_cols[c])[i]; break;
+      }
+      uint8_t* dv = dst_valid[c];
+      if (dv != nullptr) {
+        const uint8_t* sv = src_valid[c];
+        dv[r] = sv != nullptr ? sv[i] : (uint8_t)1;
+      }
+    }
+  }
+}
+
 // ---- stream compaction: indices of the non-zero bytes of a mask, in order ---------------------
 __global__ void __launch_bounds__(kScanBlock)
 fb_mask_tile_counts_kernel(const uint8_t* __restrict__ mask, int64_t n, int64_t* __restrict__ counts) {
@@ -765,6 +792,19 @@ int fb_gather_rows(int dev, void* stream, int ncols, const void* const* d_src_co
   return 0;
 }
 
+int fb_scatter_rows(int dev, void* stream, int ncols, const void* const* d_src_cols, void* const* d_dst_cols,
+                    const int32_t* d_widths, const uint8_t* const* d_src_valid, uint8_t* const* d_dst_valid,
+                    const int64_t* idx, int64_t n) {
+  FB_CHECK(ncols >= 0 && n >= 0, "negative count");
+  if (ncols == 0 || n == 0) return 0;
+  FB_CHECK(d_src_valid != nullptr && d_dst_valid != nullptr, "validity pointer tables are NULL");
+  FbDeviceGuard guard(dev);
+  FB_CHECK(guard.ok, "cannot select device %d", dev);
+  fb_scatter_rows_kernel<<<grid_for(dev, n, 4), 256, 0, (cudaStream_t)stream>>>(
+      d_src_cols, d_dst_cols, d_widths, d_src_valid, d_dst_valid, idx, n, ncols);
+  FB_CUDA(cudaGetLastError());
+  return 0;
+}
 
 // ---- K7 fast path (see the kernels above) ------------------------------------------------------------
 size_t fb_join2_table_bytes(int64_t capacity) { return capacity > 0 ? (size_t)capacity * sizeof(uint32_t) : 0; }

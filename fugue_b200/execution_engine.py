@@ -282,6 +282,25 @@ def _deviations(devs: Dict[Tuple[int, int], Any], add: Any, v: torch.Tensor, m: 
     return devs[k]
 
 
+def _check_windows(e: Any) -> None:
+    """A window node without its own spec belongs to a ColumnMap (the PartitionSpec gives its partition)."""
+    from .column import has_bare_window
+
+    assert_or_throw(not has_bare_window(e), lambda: NotImplementedError(
+        f"{e}: a window function needs PARTITION BY / ORDER BY; use over(partition_by=.., order_by=..), or use it in "
+        "a ColumnMap of fa.transform"))
+
+
+def _project_windows(t: B200Table, exprs: List[Any]) -> B200Table:
+    """``SELECT exprs FROM t`` where ``exprs`` hold explicit window nodes: the windows (``evaluate_windows``), then
+    one evaluator pass over ``t`` and the window columns."""
+    from . import expr as X
+    from .colmap import evaluate_windows
+
+    w = evaluate_windows(t, exprs)
+    return X.project(w, [X.rewrite(e, w.window_column) for e in exprs])
+
+
 def finish_avgs(res: "B200DataFrame", post: List[Any], want: List[str]) -> "B200DataFrame":
     """Replace the (sum, count) column pairs of ``decompose_aggs`` by their quotient."""
     if not post:
@@ -905,6 +924,11 @@ class B200ExecutionEngine(EngineLifecycle):
                 dicts[out] = w.dictionaries[nm]
         return B200DataFrame(B200Table(Schema(fields), cols, valids, dicts))
 
+    def _check_window_world(self, windowed: bool) -> None:
+        assert_or_throw(not windowed or self.get_current_parallelism() <= 1, lambda: NotImplementedError(
+            "window functions on the multi-GPU engine: a rank holds only its own rows, so a partition's rows on "
+            "other ranks would be missing from its windows"))
+
     # ---- select / filter / assign (K8) ---------------------------------------------------
     def select(self, df: Any, cols: Any, where: Any = None, having: Any = None) -> B200DataFrame:
         """``ExecutionEngine.select`` (execution_engine.py:736-806): ``SELECT cols FROM df [WHERE ...]
@@ -914,11 +938,15 @@ class B200ExecutionEngine(EngineLifecycle):
         from . import expr as X
         from . import relational as R
         from .column import (AGGREGATES, BIVARIATES, PERCENTILES, ColumnExpr, Kind, SelectColumns, agg as _agg, col,
-                             has_window, is_agg)
+                             column_mentions, has_window, is_agg)
 
         for e in list(cols.all_cols) + [where, having]:
-            assert_or_throw(not has_window(e), lambda: NotImplementedError(
-                f"{e}: a window function needs PARTITION BY / ORDER BY; use it in a ColumnMap of fa.transform"))
+            _check_windows(e)
+        for clause, e in (("WHERE", where), ("HAVING", having)):
+            assert_or_throw(not has_window(e), lambda: ValueError(
+                f"{e}: a window function in {clause}; windows run after {clause}, filter on them with QUALIFY"))
+        windowed = any(has_window(c) for c in cols.all_cols)
+        self._check_window_world(windowed)
         edf = self.to_df(df)
         t: B200Table = edf.native
         sel: SelectColumns = cols.replace_wildcard(t.schema).assert_all_with_names()
@@ -927,7 +955,7 @@ class B200ExecutionEngine(EngineLifecycle):
             t = X.filter_table(t, where)
         if not sel.has_agg:
             assert_or_throw(having is None, ValueError("HAVING needs an aggregation"))
-            res = B200DataFrame(X.project(t, sel.all_cols))
+            res = B200DataFrame(_project_windows(t, sel.all_cols) if windowed else X.project(t, sel.all_cols))
             return R.distinct(self, res) if sel.is_distinct else res
         # ---- aggregation: pre-project (group keys, aggregation arguments) -> group-by -> post-project
         pre: List[Any] = []        # expressions of the temporary table
@@ -1028,7 +1056,16 @@ class B200ExecutionEngine(EngineLifecycle):
         if having is not None:
             g = X.filter_table(g, to_group_table(having.alias("")))
         outs = [to_group_table(c).alias(c.output_name) for c in sel.all_cols]
-        res = B200DataFrame(X.project(g, outs))
+        if windowed:  # windows over the groups: they read only group keys and aggregates (DESIGN §7p)
+            for c, o in zip(sel.all_cols, outs):
+                if has_window(c):
+                    loose = [m for m in column_mentions(o) if m not in g.schema]
+                    assert_or_throw(not loose, lambda: ValueError(
+                        f"{c}: a window over GROUP BY results reads {loose[0]}, which is neither a group key nor "
+                        "aggregated"))
+            res = B200DataFrame(_project_windows(g, outs))
+        else:
+            res = B200DataFrame(X.project(g, outs))
         # MIN/MAX/plain keys keep the input type when the expression says so (correct_select_schema)
         fix = {}
         for c in sel.all_cols:
@@ -1044,13 +1081,20 @@ class B200ExecutionEngine(EngineLifecycle):
         """``ExecutionEngine.filter`` (execution_engine.py:808-834): rows where ``condition`` is TRUE
         (predicate evaluated on the device, stream compaction + gather).  Pins: execution_suite.py:85-95."""
         from . import expr as X
-        from .column import has_window, is_agg
+        from .colmap import evaluate_windows
+        from .column import col, has_window, is_agg
 
         assert_or_throw(not is_agg(condition), lambda: ValueError(f"{condition} has aggregation functions"))
-        assert_or_throw(not has_window(condition), lambda: NotImplementedError(
-            f"{condition}: a window function needs PARTITION BY / ORDER BY; use it in a ColumnMap of fa.transform"))
+        _check_windows(condition)
+        self._check_window_world(has_window(condition))
         edf = self.to_df(df)
-        res = B200DataFrame(X.filter_table(edf.native, condition))
+        if has_window(condition):  # QUALIFY: the windows first, then the predicate over them
+            t = edf.native
+            w = evaluate_windows(t, [condition])
+            kept = X.filter_table(w, X.rewrite(condition, w.window_column))
+            res = B200DataFrame(X.project(kept, [col(n) for n in t.schema.names]))
+        else:
+            res = B200DataFrame(X.filter_table(edf.native, condition))
         if edf.has_metadata:
             res.reset_metadata(edf.metadata)
         return res
@@ -1058,12 +1102,14 @@ class B200ExecutionEngine(EngineLifecycle):
     def assign(self, df: Any, columns: List[Any]) -> B200DataFrame:
         """``ExecutionEngine.assign`` (execution_engine.py:836-887): replace / append columns.
         Pins: execution_suite.py:157-174."""
-        from .column import SelectColumns, col, has_window
+        from .column import SelectColumns, col
 
         SelectColumns(*columns).assert_no_wildcard().assert_all_with_names().assert_no_agg()
+        from .column import has_window
+
         for c in columns:
-            assert_or_throw(not has_window(c), lambda: NotImplementedError(
-                f"{c}: a window function needs PARTITION BY / ORDER BY; use it in a ColumnMap of fa.transform"))
+            _check_windows(c)
+        self._check_window_world(any(has_window(c) for c in columns))
         edf = self.to_df(df)
         pos = {n: i for i, n in enumerate(edf.schema.names)}
         cols: List[Any] = [col(n) for n in pos]

@@ -41,7 +41,7 @@ import torch
 from . import kernels as K
 from . import strings as ST
 from .column import (REGEX_PREDICATES, TEMPORAL_LITERALS, TIME_FIELDS, TIME_PARTS, ColumnExpr, Kind, Scalar,
-                     case_string_results, check_call, col as _col, is_string_build, lit as _lit, result_args, round_digits,
+                     _children, case_string_results, check_call, col as _col, is_string_build, lit as _lit, result_args, round_digits,
                      scalar_head)
 from .schema import Schema
 from .table import B200Table, _storage_dtype, expr_type
@@ -1169,9 +1169,17 @@ def rewrite(e: Any, mapper: Any) -> Any:
         return rep.alias(e.as_name) if e.as_name != "" else rep
     if e.has_args:
         args = [rewrite(a, mapper) for a in e.args]
-        kwargs = {k: rewrite(v, mapper) for k, v in e.kwargs.items()}
+        kwargs = {k: _rewrite_spec(v, mapper) for k, v in e.kwargs.items()}
         return ColumnExpr(e.kind, e.head, args, kwargs, e.is_distinct, e.as_name, e.as_type)
     return e
+
+
+def _rewrite_spec(v: Any, mapper: Any) -> Any:
+    """A keyword argument rewritten: the expressions of a window spec (tuples of nodes and of (node, ascending)
+    pairs) as well."""
+    if isinstance(v, tuple):
+        return tuple(_rewrite_spec(x, mapper) for x in v)
+    return rewrite(v, mapper)
 
 
 def find_aggs(e: Any, out: List[ColumnExpr]) -> None:
@@ -1180,7 +1188,5 @@ def find_aggs(e: Any, out: List[ColumnExpr]) -> None:
     if e.kind == Kind.AGG:
         out.append(e)
     elif e.has_args:
-        for a in e.args:
-            find_aggs(a, out)
-        for a in e.kwargs.values():
+        for a in _children(e):
             find_aggs(a, out)

@@ -854,6 +854,28 @@ def gather_rows(cols: Sequence[torch.Tensor], valid: Sequence[Optional[torch.Ten
     return outs, outv
 
 
+def scatter_rows(cols: Sequence[torch.Tensor], valid: Sequence[Optional[torch.Tensor]], idx: torch.Tensor
+                 ) -> Tuple[List[torch.Tensor], List[Optional[torch.Tensor]]]:
+    """out[c][idx[i]] = cols[c][i], validity likewise (None stays None): the inverse of ``gather_rows`` for a
+    permutation ``idx`` (``fb_scatter_rows``; only argsort results may be passed), all columns in one launch."""
+    lib = _lib.load()
+    if len(cols) == 0:
+        return [], []
+    dev = idx.device
+    n = int(idx.shape[0])
+    assert all(int(c.shape[0]) == n for c in cols), "scatter_rows: every column needs one row per index"
+    outs = [torch.empty(n, dtype=c.dtype, device=dev) for c in cols]
+    outv = [None if v is None else torch.empty(n, dtype=torch.uint8, device=dev) for v in valid]
+    sp = torch.tensor([c.data_ptr() for c in cols], dtype=torch.int64, device=dev)
+    dp = torch.tensor([c.data_ptr() for c in outs], dtype=torch.int64, device=dev)
+    w = torch.tensor([c.element_size() for c in cols], dtype=torch.int32, device=dev)
+    sv = torch.tensor([0 if v is None else v.data_ptr() for v in valid], dtype=torch.int64, device=dev)
+    dv = torch.tensor([0 if v is None else v.data_ptr() for v in outv], dtype=torch.int64, device=dev)
+    _lib.check(lib.fb_scatter_rows(dev.index, _stream_ptr(dev), len(cols), sp.data_ptr(), dp.data_ptr(),
+                                   w.data_ptr(), sv.data_ptr(), dv.data_ptr(), idx.contiguous().data_ptr(), n))
+    return outs, outv
+
+
 def row_hash64(keys: Sequence[torch.Tensor], valid: Optional[Sequence[Optional[torch.Tensor]]] = None
                ) -> torch.Tensor:
     """64-bit hash of each row's key tuple (same function as the partitioner, before ``% num``)."""

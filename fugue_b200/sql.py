@@ -8,11 +8,29 @@ fugue/workflow/workflow.py:2109-2166) and ``ExecutionEngine.aggregate`` reaches 
 (native_execution_engine.py:59-66); here:
 
     SELECT [DISTINCT] <expr [AS a], ...> FROM t [WHERE <expr>] [GROUP BY <expr, ...>] [HAVING <expr>]
-             [ORDER BY c [ASC|DESC], ...] [LIMIT n]
+             [QUALIFY <expr>] [ORDER BY c [ASC|DESC], ...] [LIMIT n]
         -> parsed into column expressions (fugue_b200.column) and run by ``engine.select``: row-wise
            parts in the device expression evaluator, SUM/COUNT/MIN/MAX/AVG and VAR_SAMP / VARIANCE / VAR_POP /
            STDDEV_SAMP / STDDEV / STDDEV_POP, SKEWNESS / SKEW / SKEWNESS_POP / KURTOSIS / KURT / KURTOSIS_POP and
-           CORR / COVAR_POP / COVAR_SAMP / REGR_* in the hash group-by kernel
+           CORR / COVAR_POP / COVAR_SAMP / REGR_* in the hash group-by kernel, window functions by the window
+           kernels (K9, K10) after a sort per spec; evaluation order FROM, WHERE, GROUP BY, HAVING, windows,
+           QUALIFY, the select list, DISTINCT, ORDER BY, LIMIT.  QUALIFY may name output aliases.
+
+Window functions (DESIGN §7p):
+
+    <call> OVER ( [PARTITION BY <expr>, ...] [ORDER BY <expr> [ASC|DESC] [NULLS LAST], ...] [<frame>] )
+    <call>  ::= any aggregate above | ROW_NUMBER() | RANK() | DENSE_RANK() | LAG(x[, n[, default]])
+              | LEAD(x[, n[, default]]) | PERCENTILE_CONT / PERCENTILE_DISC(q) WITHIN GROUP (ORDER BY x)
+    <frame> ::= ROWS | RANGE  BETWEEN <bound> AND <bound>  |  ROWS | RANGE <bound>
+    <bound> ::= UNBOUNDED PRECEDING | n PRECEDING | CURRENT ROW | n FOLLOWING | UNBOUNDED FOLLOWING
+                (a RANGE offset n may be an INTERVAL '..' DAY / DAY TO SECOND literal)
+
+    With ORDER BY and no frame the frame is RANGE BETWEEN UNBOUNDED PRECEDING AND CURRENT ROW (peers
+    included), without ORDER BY the whole partition.  NULLs sort last in both directions.  A window over a
+    GROUP BY reads group keys and aggregates only (``RANK() OVER (ORDER BY SUM(v) DESC)``).  GROUPS frames,
+    EXCLUDE, named windows (WINDOW w AS, OVER w) and NULLS FIRST raise NotImplementedError, and so do
+    ROW_NUMBER / RANK / DENSE_RANK / LAG / LEAD without OVER; a window in WHERE, GROUP BY, HAVING or in another
+    window's arguments raises ValueError.
     SELECT * FROM a [INNER|LEFT|RIGHT|FULL [OUTER]|LEFT SEMI|LEFT ANTI|CROSS] JOIN b
              [USING (k, ...) | ON a.k = b.k [AND ...]]                        -> hash join kernels
 
@@ -33,8 +51,8 @@ from typing import Any, Dict, List, Tuple
 
 import pyarrow as pa
 
-from .column import (BIVARIATES, ColumnExpr, Kind, SelectColumns, all_cols, check_arity, col, function, functions, is_agg,
-                     lit, null, scalar_head)
+from .column import (_SPEC_ONLY, BIVARIATES, PERCENTILES, ColumnExpr, Kind, SelectColumns, _offset_fn, all_cols,
+                     check_arity, col, function, functions, has_window, is_agg, lit, null, scalar_head)
 from .dataframe import DataFrame
 
 _AGG = r"(SUM|COUNT|MIN|MAX|AVG|MEAN)\s*\(\s*(\*|[A-Za-z_][\w]*)\s*\)"
@@ -203,10 +221,26 @@ class B200SQLEngine:
             for k in probe.group_keys:
                 if k.fingerprint() not in listed:
                     raise ValueError(f"{k} is neither aggregated nor in GROUP BY: {sql}")
-        res = self._engine.select(df, SelectColumns(*cols, arg_distinct=st.distinct), where=st.where,
-                                  having=st.having)
+        if st.qualify is not None:
+            # QUALIFY: a hidden column of the same SELECT (its windows are evaluated with the select list's), then
+            # a filter on it, then DISTINCT; an output alias stands for its expression, an input column for itself
+            alias = {c.output_name: c.alias("") for c in cols if c.kind != Kind.WILDCARD and c.output_name != ""}
+            from .expr import rewrite
+
+            qualify = rewrite(st.qualify, lambda e: alias[e.name] if e.kind == Kind.NAMED and
+                              e.name in alias and e.name not in df.schema else None)
+            if not has_window(qualify):
+                raise ValueError(f"QUALIFY needs a window function: {sql}")
+            cols.append(qualify.alias("__fb_q"))
+            hidden.append("__fb_q")
+        res = self._engine.select(df, SelectColumns(*cols, arg_distinct=st.distinct and st.qualify is None),
+                                  where=st.where, having=st.having)
+        if st.qualify is not None:
+            res = self._engine.filter(res, col("__fb_q"))
         if hidden:
             res = res[[n for n in res.columns if n not in hidden]]
+        if st.distinct and st.qualify is not None:
+            res = self._engine.distinct(res)
         if st.order_by:
             from collections import OrderedDict
 
@@ -303,6 +337,7 @@ class _Select:
         self.where: Any = None
         self.group_by: List[ColumnExpr] = []
         self.having: Any = None
+        self.qualify: Any = None
         self.order_by: List[Tuple[str, bool]] = []
         self.limit: Any = None
 
@@ -323,7 +358,7 @@ _AGG_FUNCS = {"SUM": functions.sum, "COUNT": functions.count, "MIN": functions.m
               "KURTOSIS": functions.kurtosis, "KURT": functions.kurt, "KURTOSIS_POP": functions.kurtosis_pop}
 # CORR(a, b), COVAR_POP / COVAR_SAMP(a, b), REGR_*(y, x): two arguments, in SQL's order
 _BIVARIATE_FUNCS = {name: getattr(functions, name.lower()) for name in BIVARIATES}
-_CLAUSES = ("WHERE", "GROUP", "HAVING", "ORDER", "LIMIT")
+_CLAUSES = ("WHERE", "GROUP", "HAVING", "QUALIFY", "WINDOW", "ORDER", "LIMIT")
 _CASE_WORDS = ("WHEN", "THEN", "ELSE", "END")  # never a column name or an implicit alias
 _FIELD_FUNCS = {"YEAR": "year", "MONTH": "month", "DAY": "day", "HOUR": "hour", "MINUTE": "minute", "SECOND": "second",
                 "QUARTER": "quarter", "DAYOFWEEK": "dow", "DAYOFYEAR": "doy", "WEEK": "week"}
@@ -644,6 +679,110 @@ class _Parser:
         return col(name)
 
     def _call(self, fn: str) -> ColumnExpr:
+        e = self._window_call(fn) if fn in _SPEC_ONLY else self._plain_call(fn)
+        if self.at_kw("OVER"):
+            return self._over(e)
+        if e.kind == Kind.WINDOW:
+            self.fail(f"{fn} without OVER (...)")
+        if e.kind == Kind.AGG and any(has_window(a) for a in e.args):
+            raise ValueError(f"a window function inside the aggregation {e} in: {self.sql}")
+        return e
+
+    def _window_call(self, fn: str) -> ColumnExpr:
+        """``ROW_NUMBER() / RANK() / DENSE_RANK()`` or ``LAG / LEAD(x[, n[, default]])``: n an integer literal,
+        default a literal."""
+        self.i += 2  # name (
+        if fn in ("ROW_NUMBER", "RANK", "DENSE_RANK"):
+            self.expect(")")
+            return getattr(functions, fn.lower())()
+        args = [self.expr()]
+        while self.op(","):
+            args.append(self.expr())
+        self.expect(")")
+        if len(args) > 3:
+            raise ValueError(f"{fn} takes 1 to 3 arguments, got {len(args)} in: {self.sql}")
+        for what, x in zip(("n", "default"), args[1:]):
+            if x.kind != Kind.LITERAL or x.as_type is not None:
+                raise ValueError(f"{fn}: {what} must be a literal, got {x} in: {self.sql}")
+        n = args[1].value if len(args) > 1 else 1
+        default = args[2].value if len(args) > 2 else None
+        return _offset_fn(fn, args[0], n, default, aggregated=True)
+
+    def _over(self, e: ColumnExpr) -> ColumnExpr:
+        """``<call> OVER ([PARTITION BY e, ..] [ORDER BY e [ASC|DESC] [NULLS LAST], ..] [frame])``.  SQL's default
+        frame: with ORDER BY, RANGE BETWEEN UNBOUNDED PRECEDING AND CURRENT ROW (the current row's peers
+        included), without it the whole partition."""
+        self.i += 1  # OVER
+        if self.peek() != ("op", "("):
+            self.fail("named windows (OVER w)")
+        self.i += 1
+        partition: List[ColumnExpr] = []
+        order: List[Tuple[ColumnExpr, bool]] = []
+        if self.kw("PARTITION", "BY"):
+            partition.append(self.expr())
+            while self.op(","):
+                partition.append(self.expr())
+        if self.kw("ORDER", "BY"):
+            while True:
+                x = self.expr()
+                asc = not self.kw("DESC")
+                if asc:
+                    self.kw("ASC")
+                if self.kw("NULLS", "FIRST"):
+                    self.fail("NULLS FIRST (a window orders NULLs last)")
+                self.kw("NULLS", "LAST")
+                order.append((x, asc))
+                if not self.op(","):
+                    break
+        frame: Dict[str, Any] = {}
+        if self.at_kw("GROUPS"):
+            self.fail("GROUPS frames")
+        if self.at_kw("ROWS") or self.at_kw("RANGE"):
+            unit = self.peek()[1].lower()
+            self.i += 1
+            if self.kw("BETWEEN"):
+                start = self._frame_bound(True)
+                if not self.kw("AND"):
+                    self.fail("BETWEEN without AND in a frame")
+                end = self._frame_bound(False)
+            else:  # the short form: ROWS <bound> is BETWEEN <bound> AND CURRENT ROW
+                start, end = self._frame_bound(True), 0
+            frame[unit] = (start, end)
+        elif order and e.head not in _SPEC_ONLY and e.head not in PERCENTILES:
+            frame["range"] = (None, 0)
+        if self.at_kw("EXCLUDE"):
+            self.fail("EXCLUDE in a frame")
+        self.expect(")")
+        return e.over(partition_by=partition, order_by=order, **frame)
+
+    def _frame_bound(self, start: bool) -> Any:
+        """UNBOUNDED PRECEDING / FOLLOWING (None), CURRENT ROW (0), ``x PRECEDING`` (-x), ``x FOLLOWING`` (x); x a
+        number or an ``INTERVAL '..' DAY [TO SECOND]`` literal."""
+        if self.kw("UNBOUNDED"):
+            if self.kw("PRECEDING" if start else "FOLLOWING"):
+                return None
+            raise ValueError(f"a frame {'starts' if start else 'ends'} at UNBOUNDED "
+                             f"{'PRECEDING' if start else 'FOLLOWING'} only, in: {self.sql}")
+        if self.kw("CURRENT", "ROW"):
+            return 0
+        kind, val = self.peek()
+        if kind == "num":
+            self.i += 1
+            x: Any = _number(val)
+        elif kind == "id" and val.upper() == "INTERVAL" and self.peek(1)[0] == "str":
+            x = self._temporal_literal("INTERVAL")
+            if x.kind != Kind.LITERAL or not isinstance(x.value, datetime.timedelta):
+                self.fail("a frame offset interval in days, hours, minutes or seconds")
+            x = x.value
+        else:
+            return self.fail("a frame bound")
+        if self.kw("PRECEDING"):
+            return -x
+        if self.kw("FOLLOWING"):
+            return x
+        return self.fail("a frame offset without PRECEDING or FOLLOWING")
+
+    def _plain_call(self, fn: str) -> ColumnExpr:
         self.i += 2  # name (
         if fn in _AGG_FUNCS:
             distinct = self.kw("DISTINCT")
@@ -811,6 +950,10 @@ def _parse_select(items: str, rest: str, sql: str) -> _Select:
                 break
     if p.kw("HAVING"):
         st.having = p.expr()
+    if p.kw("QUALIFY"):
+        st.qualify = p.expr()
+    if p.at_kw("WINDOW"):
+        p.fail("named windows (WINDOW w AS ...)")
     if p.kw("ORDER", "BY"):
         while True:
             kind, val = p.peek()
@@ -835,4 +978,8 @@ def _parse_select(items: str, rest: str, sql: str) -> _Select:
         p.fail(f"unsupported SQL near {p.peek()[1]!r}")
     if st.where is not None and is_agg(st.where):
         raise ValueError(f"aggregation in WHERE: {sql}")
+    for clause, es in (("WHERE", [st.where]), ("GROUP BY", st.group_by), ("HAVING", [st.having])):
+        if any(has_window(e) for e in es):
+            raise ValueError(f"a window function in {clause}: windows run after {clause}; filter on them with "
+                             f"QUALIFY in: {sql}")
     return st

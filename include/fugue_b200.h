@@ -444,6 +444,13 @@ int fb_segmented_quantile(int dev, void* stream, int64_t nrows, int64_t nseg, co
  *   fb_join_mark_matched     matched[build_row] = 1 (right / full outer joins)
  *   fb_gather_rows           dst[c][o] = src[c][idx[o]] (idx < 0 -> NULL): all pointer tables
  *                            and widths are DEVICE arrays
+ *   fb_scatter_rows          the inverse: dst[c][idx[i]] = src[c][i] for widths 1 / 2 / 4 / 8, and
+ *                            dst_valid[c][idx[i]] = src_valid[c][i] (1 where src_valid[c] is NULL) for
+ *                            every column whose dst_valid[c] is not NULL; one thread per row moves all
+ *                            columns, so idx is read once.  PRECONDITION: idx is a permutation of
+ *                            [0, n) (an argsort result); a repeated or out-of-range entry is a race or an
+ *                            out-of-bounds store, and is not checked.  Pointer tables and widths are
+ *                            DEVICE arrays; both validity tables must be given (entries may be NULL)
  * --------------------------------------------------------------------------- */
 size_t fb_join_table_bytes(int64_t capacity);
 int fb_join_build_u64(int dev, void* stream, int64_t nbuild, const void* keys, const uint8_t* key_valid,
@@ -469,6 +476,9 @@ int fb_compact_indices(int dev, void* stream, const uint8_t* mask, int64_t n, in
 int fb_gather_rows(int dev, void* stream, int ncols, const void* const* d_src_cols, void* const* d_dst_cols,
                    const int32_t* d_widths, const uint8_t* const* d_src_valid, uint8_t* const* d_dst_valid,
                    const int64_t* idx, int64_t n);
+int fb_scatter_rows(int dev, void* stream, int ncols, const void* const* d_src_cols, void* const* d_dst_cols,
+                    const int32_t* d_widths, const uint8_t* const* d_src_valid, uint8_t* const* d_dst_valid,
+                    const int64_t* idx, int64_t n);
 
 /* K7 fast path: inner / left-outer join on one 8-byte key with 4-byte slots (build row + 1; keys are
  * compared through the build key column) and a fused probe -> output assembly.

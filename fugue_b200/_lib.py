@@ -108,6 +108,8 @@ SIGNATURES = {
     "fb_compact_indices": (C.c_int, [C.c_int, _vp, _vp, C.c_int64, _vp, _vp, _vp, C.c_size_t]),
     "fb_gather_rows": (C.c_int, [C.c_int, _vp, C.c_int, _vp, _vp, _vp, _vp, _vp, _vp, C.c_int64]),
     "fb_scatter_rows": (C.c_int, [C.c_int, _vp, C.c_int, _vp, _vp, _vp, _vp, _vp, _vp, C.c_int64]),
+    "fb_asof_search": (C.c_int, [C.c_int, _vp, C.c_int64, _vp, _vp, _vp, _vp, _vp, _vp, C.c_int, C.c_int, C.c_int,
+                                 C.c_int, C.c_uint64, _vp]),
     "fb_copy_runs_dma": (C.c_int, [C.c_int, _vp, C.c_int64, _vp, _vp, _vp]),
     "fb_copy_runs_dma_streams": (C.c_int, [C.c_int, C.c_int64, _vp, _vp, _vp, _vp, C.c_int]),
     "fb_pull_runs_tma": (C.c_int, [C.c_int, _vp, C.c_int, _vp, _vp, _vp, C.c_int]),

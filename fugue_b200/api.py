@@ -534,6 +534,21 @@ def join(df1: Any, df2: Any, *dfs: Any, how: str, on: Optional[Iterable[str]] = 
     return res.as_pandas() if res.is_local else res.native
 
 
+def asof_join(df1: Any, df2: Any, on: Optional[Iterable[str]], asof: str, how: str = "inner",
+              direction: str = "backward", allow_exact_matches: bool = True, tolerance: Any = None, engine: Any = None,
+              engine_conf: Any = None, as_fugue: bool = False, as_local: bool = False) -> Any:
+    """As-of join of two dataframes with ``pandas.merge_asof`` semantics (``B200ExecutionEngine.asof_join``):
+    ``on`` are the equality keys (None: the common columns but ``asof``; empty: one group), ``asof`` the column
+    matched by the latest (``direction="backward"``), next (``"forward"``) or nearest value."""
+    e = make_execution_engine(engine, engine_conf, infer_by=[df1, df2])
+    res: DataFrame = e.asof_join(e.to_df(df1), e.to_df(df2), on=None if on is None else list(on), asof=asof, how=how,
+                                 direction=direction, allow_exact_matches=allow_exact_matches, tolerance=tolerance)
+    res = e.convert_yield_dataframe(res, as_local)
+    if as_fugue or any(isinstance(x, DataFrame) for x in (df1, df2)):
+        return res
+    return res.as_pandas() if res.is_local else res.native
+
+
 def inner_join(df1: Any, df2: Any, *dfs: Any, **kwargs: Any) -> Any:
     return join(df1, df2, *dfs, how="inner", **kwargs)
 

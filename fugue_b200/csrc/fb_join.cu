@@ -273,6 +273,84 @@ fb_scatter_rows_kernel(const void* const* __restrict__ src_cols, void* const* __
   }
 }
 
+// ---- as-of search: per left row, the one right row of its run it matches --------------------------------
+// The right side is sorted by (key, as-of value); run r = rows [run_off[r], run_off[r + 1]) of one key, its as-of
+// values as unsigned order codes that ascend within the run (PRECONDITION: the host passes the codes of an
+// argsort_rows result; it is not checked).  Codes of one integer class differ by exactly the values' distance
+// (a signed code is the value + 2^63 mod 2^64), so an integer distance is one unsigned 64-bit subtraction of the
+// larger code minus the smaller, in [0, 2^64) and never wrapping; a float distance is one f64 subtraction.
+constexpr uint64_t kAsofSign = 0x8000000000000000ull;
+
+__device__ __forceinline__ double asof_f64(uint64_t code) {  // inverse of the float order code (sort.py)
+  return __longlong_as_double((long long)((code & kAsofSign) ? (code ^ kAsofSign) : ~code));
+}
+
+// first position in [lo, hi) whose code is > x (kUpper) or >= x, hi if none
+template <bool kUpper>
+__device__ __forceinline__ int64_t asof_bound(const uint64_t* __restrict__ codes, int64_t lo, int64_t hi,
+                                              uint64_t x) {
+  while (lo < hi) {
+    const int64_t m = lo + ((hi - lo) >> 1);
+    const uint64_t c = __ldg((const unsigned long long*)codes + m);
+    if (kUpper ? c <= x : c < x) lo = m + 1; else hi = m;
+  }
+  return lo;
+}
+
+// distance of codes a <= b: cls FB_RANGE_KEY_F64 compares the f64 in `f`, the integer classes the exact `u`
+struct AsofDist {
+  uint64_t u;
+  double f;
+};
+
+__device__ __forceinline__ AsofDist asof_dist(uint64_t a, uint64_t b, bool is_float) {
+  AsofDist d{0, 0.0};
+  if (!is_float) d.u = b - a;
+  else if (a != b) d.f = asof_f64(b) - asof_f64(a);  // equal codes are distance 0, also for +-inf
+  return d;
+}
+
+__device__ __forceinline__ bool asof_le(const AsofDist& a, const AsofDist& b, bool is_float) {
+  return is_float ? a.f <= b.f : a.u <= b.u;
+}
+
+__global__ void __launch_bounds__(256)
+fb_asof_search_kernel(int64_t n, const int64_t* __restrict__ run, const int64_t* __restrict__ run_off,
+                      const uint64_t* __restrict__ left_codes, const uint8_t* __restrict__ left_valid,
+                      const uint64_t* __restrict__ codes, const int64_t* __restrict__ rows, int cls, int direction,
+                      int strict, int has_tol, uint64_t tol, int64_t* __restrict__ out) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  int64_t res = -1;
+  const int64_t r = __ldg((const long long*)run + i);
+  if (r >= 0 && (left_valid == nullptr || __ldg(left_valid + i) != 0)) {
+    const bool is_float = cls == FB_RANGE_KEY_F64;
+    const AsofDist limit{tol, __longlong_as_double((long long)tol)};
+    const int64_t s = __ldg((const long long*)run_off + r), e = __ldg((const long long*)run_off + r + 1);
+    const uint64_t x = __ldg((const unsigned long long*)left_codes + i);
+    int64_t b = -1, f = -1;  // backward / forward candidate positions in the sorted run
+    AsofDist db{0, 0.0}, df{0, 0.0};
+    if (direction != FB_ASOF_FORWARD) {  // the last code <= x (< x when strict): the last such row in input order
+      const int64_t p = (strict ? asof_bound<false>(codes, s, e, x) : asof_bound<true>(codes, s, e, x)) - 1;
+      if (p >= s) {
+        db = asof_dist(__ldg((const unsigned long long*)codes + p), x, is_float);
+        if (!has_tol || asof_le(db, limit, is_float)) b = p;
+      }
+    }
+    if (direction != FB_ASOF_BACKWARD) {  // the first code >= x (> x when strict): the first such row
+      const int64_t q = strict ? asof_bound<true>(codes, s, e, x) : asof_bound<false>(codes, s, e, x);
+      if (q < e) {
+        df = asof_dist(x, __ldg((const unsigned long long*)codes + q), is_float);
+        if (!has_tol || asof_le(df, limit, is_float)) f = q;
+      }
+    }
+    // nearest: the backward candidate unless the forward one is strictly closer
+    const int64_t pick = b < 0 ? f : (f < 0 || asof_le(db, df, is_float) ? b : f);
+    if (pick >= 0) res = __ldg((const long long*)rows + pick);
+  }
+  out[i] = res;
+}
+
 // ---- stream compaction: indices of the non-zero bytes of a mask, in order ---------------------
 __global__ void __launch_bounds__(kScanBlock)
 fb_mask_tile_counts_kernel(const uint8_t* __restrict__ mask, int64_t n, int64_t* __restrict__ counts) {
@@ -802,6 +880,25 @@ int fb_scatter_rows(int dev, void* stream, int ncols, const void* const* d_src_c
   FB_CHECK(guard.ok, "cannot select device %d", dev);
   fb_scatter_rows_kernel<<<grid_for(dev, n, 4), 256, 0, (cudaStream_t)stream>>>(
       d_src_cols, d_dst_cols, d_widths, d_src_valid, d_dst_valid, idx, n, ncols);
+  FB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int fb_asof_search(int dev, void* stream, int64_t nleft, const int64_t* d_run, const int64_t* d_run_offsets,
+                   const uint64_t* d_left_codes, const uint8_t* d_left_valid, const uint64_t* d_right_codes,
+                   const int64_t* d_right_rows, int key_class, int direction, int allow_exact_matches,
+                   int has_tolerance, uint64_t tolerance, int64_t* d_out) {
+  FB_CHECK(nleft >= 0, "negative count");
+  FB_CHECK(key_class == FB_RANGE_KEY_I64 || key_class == FB_RANGE_KEY_U64 || key_class == FB_RANGE_KEY_F64,
+           "unknown key class %d", key_class);
+  FB_CHECK(direction == FB_ASOF_BACKWARD || direction == FB_ASOF_FORWARD || direction == FB_ASOF_NEAREST,
+           "unknown direction %d", direction);
+  if (nleft == 0) return 0;
+  FbDeviceGuard guard(dev);
+  FB_CHECK(guard.ok, "cannot select device %d", dev);
+  fb_asof_search_kernel<<<(unsigned)((nleft + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
+      nleft, d_run, d_run_offsets, d_left_codes, d_left_valid, d_right_codes, d_right_rows, key_class, direction,
+      allow_exact_matches ? 0 : 1, has_tolerance ? 1 : 0, tolerance, d_out);
   FB_CUDA(cudaGetLastError());
   return 0;
 }

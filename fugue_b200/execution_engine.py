@@ -1129,6 +1129,22 @@ class B200ExecutionEngine(EngineLifecycle):
 
         return device_join(self, self.to_df(df1), self.to_df(df2), how, on)
 
+    def asof_join(self, df1: Any, df2: Any, on: Optional[List[str]], asof: str, how: str = "inner",
+                  direction: str = "backward", allow_exact_matches: bool = True,
+                  tolerance: Any = None) -> B200DataFrame:
+        """As-of join with ``pandas.merge_asof`` semantics (DESIGN §7q): every row of ``df1``, in input order, with
+        the row of ``df2`` of equal ``on`` key whose ``asof`` value is the latest at or before the row's
+        (``direction="backward"``), the earliest at or after it (``"forward"``) or the closer of the two
+        (``"nearest"``, ties to the backward one).  ``allow_exact_matches=False`` makes the inequality strict;
+        ``tolerance`` bounds the distance.  ``how`` is ``"inner"`` (unmatched rows dropped) or ``"left_outer"``
+        (they get NULLs).  Output schema: ``df1.schema`` followed by df2's columns other than ``on`` and ``asof``."""
+        from .join import device_asof_join
+
+        assert_or_throw(self.get_current_parallelism() <= 1, lambda: NotImplementedError(
+            "as-of joins on the multi-GPU engine: a rank holds only its own rows of the right table"))
+        return device_asof_join(self.to_df(df1), self.to_df(df2), on, asof, how, direction, allow_exact_matches,
+                                tolerance)
+
     # ---- set operations, NULL handling, sampling, IO (fugue_b200/relational.py) -----------
     def union(self, df1: Any, df2: Any, distinct: bool = True) -> B200DataFrame:
         from . import relational as R

@@ -5,6 +5,8 @@ Reference semantics:
   * join types / NULL keys             fugue/execution/native_execution_engine.py:230-241,
                                        fugue_test/execution_suite.py:366-543
 """
+import datetime
+from collections import OrderedDict
 from typing import Any, List, Optional, Tuple
 
 import pyarrow as pa
@@ -14,7 +16,7 @@ import torch
 from . import kernels as K
 from .dataframe import B200DataFrame
 from .schema import Schema, SchemaError
-from .sort import float_key
+from .sort import _unsigned_order_key, argsort_rows, float_key, float_key_valid, group_starts, take_rows
 from .table import B200Table, widen
 
 _JOIN_TYPES = ["semi", "left_semi", "anti", "left_anti", "inner", "left_outer", "right_outer",
@@ -257,6 +259,161 @@ def _drop_collisions(t1, t2, keys, li, ri, outer_side):
     else:
         li[first_bad] = -1
     return li[keep], ri[keep]
+
+
+ASOF_JOIN_TYPES = ["inner", "left_outer"]
+ASOF_DIRECTIONS = {"backward": K.ASOF_BACKWARD, "forward": K.ASOF_FORWARD, "nearest": K.ASOF_NEAREST}
+
+
+def get_asof_schemas(df1: Any, df2: Any, on: Optional[List[str]], asof: str) -> Tuple[List[str], Schema]:
+    """(equality keys, output schema) of an as-of join.  ``on=None`` takes every common column but ``asof``; an
+    empty list is one group.  The output is ``df1.schema`` followed by df2's columns other than the keys and
+    ``asof``; any other common column raises SchemaError, as ``get_join_schemas`` does."""
+    if not isinstance(asof, str):
+        raise ValueError(f"asof must be one column name, got {asof!r}")
+    if on is None:
+        other = set(df2.columns)
+        on = [c for c in df1.columns if c in other and c != asof]
+    on = list(on)
+    if len(on) != len(set(on)):
+        raise AssertionError(f"{on} has duplication")
+    if asof in on:
+        raise ValueError(f"the as-of column {asof} is also an equality key {on}")
+    for k in on + [asof]:
+        if k not in df1.schema or k not in df2.schema:
+            raise SchemaError(f"{k} is not in both {df1.schema} and {df2.schema}")
+        if df1.schema[k].type != df2.schema[k].type:
+            raise SchemaError(f"join key {k} has different types: {df1.schema[k].type} vs {df2.schema[k].type}")
+    names2 = [n for n in df2.schema.names if n not in on and n != asof]
+    common = [n for n in names2 if n in df1.schema]
+    if common:
+        raise SchemaError(f"{common} are common columns of {df1.schema} and {df2.schema} but not join keys")
+    return on, Schema(df1.schema, df2.schema.extract(names2))
+
+
+def asof_key_class(name: str, tp: pa.DataType, is_string: bool) -> int:
+    """The ``RANGE_KEY_*`` class of an as-of column: the key types RANGE frames take; anything else is a ValueError."""
+    temporal = pa.types.is_date(tp) or pa.types.is_timestamp(tp) or pa.types.is_duration(tp) or \
+        pa.types.is_time64(tp)
+    if is_string or not (pa.types.is_integer(tp) or pa.types.is_floating(tp) or temporal):
+        raise ValueError(f"an as-of column must be numeric or temporal; {name} is {tp}")
+    if pa.types.is_floating(tp):
+        return K.RANGE_KEY_F64
+    return K.RANGE_KEY_U64 if pa.types.is_unsigned_integer(tp) else K.RANGE_KEY_I64
+
+
+def asof_tolerance(name: str, tp: pa.DataType, tolerance: Any) -> Any:
+    """``tolerance`` in the as-of column's units, by the rules of a RANGE frame's offset (``colmap._range_offsets``):
+    an int in storage units, a float for float columns, a timedelta as a whole number of the column's units.
+    None stays None; a negative tolerance is a ValueError."""
+    from types import SimpleNamespace
+
+    from .colmap import _range_offsets
+    from .column import _range_frame
+
+    if tolerance is None:
+        return None
+    tol = _range_frame((tolerance, tolerance))[0]
+    if tol == 0:
+        return 0.0 if pa.types.is_floating(tp) else 0
+    if (tol.total_seconds() if isinstance(tol, datetime.timedelta) else tol) < 0:
+        raise ValueError(f"tolerance must be >= 0, got {tolerance!r}")
+    presort = SimpleNamespace(logical_order=[name], schema=Schema([pa.field(name, tp)]), dictionaries={})
+    return _range_offsets(presort, (tol, tol))[1]  # type: ignore[arg-type]
+
+
+def device_asof_join(df1: B200DataFrame, df2: B200DataFrame, on: Optional[List[str]], asof: str, how: str = "inner",
+                     direction: str = "backward", allow_exact_matches: bool = True,
+                     tolerance: Any = None) -> B200DataFrame:
+    """As-of join (``pandas.merge_asof`` semantics, DESIGN §7q): every left row, in input order, with the right
+    row of equal key whose ``asof`` value is the latest at or before its own (``backward``), the earliest at or
+    after (``forward``) or the closer of those two (``nearest``, ties to the backward one)."""
+    how = how.lower() if isinstance(how, str) else how
+    if how not in ASOF_JOIN_TYPES:
+        raise ValueError(f"an as-of join is {' or '.join(ASOF_JOIN_TYPES)}, got {how!r}")
+    if direction not in ASOF_DIRECTIONS:
+        raise ValueError(f"direction must be one of {list(ASOF_DIRECTIONS)}, got {direction!r}")
+    if not isinstance(allow_exact_matches, bool):
+        raise ValueError(f"allow_exact_matches must be a bool, got {allow_exact_matches!r}")
+    keys, out_schema = get_asof_schemas(df1, df2, on, asof)
+    t1, t2 = df1.native, df2.native
+    tp = t1.schema[asof].type
+    cls = asof_key_class(asof, tp, asof in t1.dictionaries or asof in t2.dictionaries)
+    tol = asof_tolerance(asof, tp, tolerance)
+    return _asof_assemble(t1, t2, keys, out_schema, asof_rows(t1, t2, keys, asof, cls, direction,
+                                                                allow_exact_matches, tol), how)
+
+
+def _asof_value(t: B200Table, name: str, cls: int) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
+    """Order codes of an as-of column and its validity (a float NaN is NULL)."""
+    i = t.schema.index_of_key(name)
+    v = t.valid[i]
+    if cls == K.RANGE_KEY_F64:
+        v = float_key_valid(widen(t.columns[i], t.schema.types[i]), v)
+    return _unsigned_order_key(t, name, True), v
+
+
+def asof_rows(t1: B200Table, t2: B200Table, keys: List[str], asof: str, cls: int, direction: str,
+              allow_exact_matches: bool, tolerance: Any) -> torch.Tensor:
+    """Per left row, the right row it matches, -1 for none (int64)."""
+    dev = t1.device
+    n1, n2 = t1.num_rows, t2.num_rows
+    if n1 == 0:
+        return torch.empty(0, dtype=torch.int64, device=dev)
+    # 1. right side: drop the rows that can never match, sort the rest by (keys..., asof), stable
+    c2, av2 = _asof_value(t2, asof, cls)
+    if keys:
+        k1, v1, k2, v2, exact = _key64(t1, t2, keys)
+        keep = v2 if av2 is None else (av2 if v2 is None else v2 & av2)
+    else:
+        keep = av2
+    kept = torch.arange(n2, dtype=torch.int64, device=dev) if keep is None else K.compact_indices(keep.contiguous())
+    sub = take_rows(B200Table(t2.schema.extract(keys + [asof]), [t2.column(k) for k in keys + [asof]],
+                              [t2.valid[t2.schema.index_of_key(k)] for k in keys + [asof]],
+                              {k: t2.dictionaries[k] for k in keys if k in t2.dictionaries}), kept)
+    if kept.shape[0] == 0:
+        return torch.full((n1,), -1, dtype=torch.int64, device=dev)
+    perm = argsort_rows(sub, OrderedDict([(k, True) for k in keys] + [(asof, True)]))
+    rows = kept[perm].contiguous()
+    codes = c2[rows].contiguous()
+    # 2. runs of equal keys, and every left row's run
+    if keys:
+        heads = K.compact_indices(group_starts(take_rows(sub, perm), keys).contiguous())
+        head_rows = rows[heads]
+        tab = K.JoinTable(k2[head_rows].contiguous(), None)
+        if exact:  # one surrogate per key value: the first match is the run
+            run = torch.empty(n1, dtype=torch.int64, device=dev)
+            tab.probe_counts(k1.contiguous(), v1, outer=False, first=run)
+        else:  # hashed surrogates: a candidate run counts only if its head has the row's key values
+            li, ri = tab.probe(k1.contiguous(), v1, outer=False)
+            ok = _verify(t1, t2, keys, li, head_rows[ri])
+            run = torch.full((n1,), -1, dtype=torch.int64, device=dev)
+            run[li[ok]] = ri[ok]
+        run_offsets = torch.cat([heads, torch.tensor([rows.shape[0]], dtype=torch.int64, device=dev)])
+    else:  # one group
+        run = torch.zeros(n1, dtype=torch.int64, device=dev)
+        run_offsets = torch.tensor([0, rows.shape[0]], dtype=torch.int64, device=dev)
+    # 3. the search
+    c1, av1 = _asof_value(t1, asof, cls)
+    return K.asof_search(run, run_offsets.contiguous(), c1, av1, codes, rows, cls, ASOF_DIRECTIONS[direction],
+                         allow_exact_matches, tolerance)
+
+
+def _asof_assemble(t1: B200Table, t2: B200Table, keys: List[str], out_schema: Schema, match: torch.Tensor,
+                   how: str) -> B200DataFrame:
+    """df1's rows (all, or the matched ones for ``inner``) with df2's output columns gathered from their match."""
+    names2 = out_schema.names[len(t1.columns):]
+    idx2 = [t2.schema.index_of_key(n) for n in names2]
+    lcols, lvalid = list(t1.columns), list(t1.valid)
+    if how == "inner":
+        li = K.compact_indices((match >= 0).contiguous())
+        lcols, lvalid = K.gather_rows(lcols, lvalid, li, want_valid=False)
+        match = match[li].contiguous()
+    rcols, rvalid = K.gather_rows([t2.columns[i] for i in idx2], [t2.valid[i] for i in idx2], match,
+                                  want_valid=how == "left_outer")
+    dicts = dict(t1.dictionaries)
+    dicts.update({n: t2.dictionaries[n] for n in names2 if n in t2.dictionaries})
+    return B200DataFrame(B200Table(out_schema, lcols + rcols, lvalid + rvalid, dicts))
 
 
 def _assemble(t1: B200Table, t2: B200Table, keys: List[str], out_schema: Schema, li: torch.Tensor,

@@ -876,6 +876,43 @@ def scatter_rows(cols: Sequence[torch.Tensor], valid: Sequence[Optional[torch.Te
     return outs, outv
 
 
+ASOF_BACKWARD, ASOF_FORWARD, ASOF_NEAREST = 0, 1, 2   # FB_ASOF_*
+
+
+def asof_search(run: torch.Tensor, run_offsets: torch.Tensor, left_codes: torch.Tensor,
+                left_valid: Optional[torch.Tensor], right_codes: torch.Tensor, right_rows: torch.Tensor, key_class: int,
+                direction: int, allow_exact_matches: bool, tolerance: Optional[Any]) -> torch.Tensor:
+    """``fb_asof_search``: per left row i, the right row it matches in its run ``run[i]`` (-1: none) of the sorted
+    right side, or -1.  ``right_codes`` (order codes, ascending within each run ``[run_offsets[r],
+    run_offsets[r + 1])``: only argsort results may be passed) and ``right_rows`` (the sort permutation) are in sorted
+    order; ``left_codes`` / ``left_valid`` in left order.  ``tolerance``: None, an int >= 0 for the integer classes,
+    a float for ``RANGE_KEY_F64``."""
+    lib = _lib.load()
+    dev = run.device
+    n = int(run.shape[0])
+    for t in (run, run_offsets, right_rows):
+        assert t.dtype == torch.int64 and t.is_cuda and t.is_contiguous()
+    for t in (left_codes, right_codes):
+        assert t.element_size() == 8 and t.device == dev and t.is_contiguous()
+    assert left_codes.shape[0] == n and right_codes.shape[0] == right_rows.shape[0]
+    if left_valid is not None:
+        assert left_valid.dtype == torch.uint8 and left_valid.device == dev and left_valid.is_contiguous()
+    if tolerance is None:
+        tol = 0
+    elif key_class == RANGE_KEY_F64:
+        tol = struct.unpack("<Q", struct.pack("<d", float(tolerance)))[0]
+    else:
+        assert 0 <= tolerance < (1 << 63), f"tolerance {tolerance} outside [0, 2^63)"
+        tol = int(tolerance)
+    out = torch.empty(n, dtype=torch.int64, device=dev)
+    _lib.check(lib.fb_asof_search(dev.index, _stream_ptr(dev), n, run.data_ptr(), run_offsets.data_ptr(),
+                                  left_codes.data_ptr(), 0 if left_valid is None else left_valid.data_ptr(),
+                                  right_codes.data_ptr(), right_rows.data_ptr(), key_class, direction,
+                                  1 if allow_exact_matches else 0, 0 if tolerance is None else 1, tol,
+                                  out.data_ptr()))
+    return out
+
+
 def row_hash64(keys: Sequence[torch.Tensor], valid: Optional[Sequence[Optional[torch.Tensor]]] = None
                ) -> torch.Tensor:
     """64-bit hash of each row's key tuple (same function as the partitioner, before ``% num``)."""

@@ -33,6 +33,8 @@ Window functions (DESIGN §7p):
     window's arguments raises ValueError.
     SELECT * FROM a [INNER|LEFT|RIGHT|FULL [OUTER]|LEFT SEMI|LEFT ANTI|CROSS] JOIN b
              [USING (k, ...) | ON a.k = b.k [AND ...]]                        -> hash join kernels
+    SELECT * FROM a ASOF [LEFT [OUTER]] JOIN b
+             USING (k, ..., t) | ON a.k = b.k [AND ...] AND a.t >= | > | <= | < b.t  -> as-of join (DESIGN §7q)
 
 Expressions: + - * / %, comparisons (= == != <> < <= > >=), AND / OR / NOT, IS [NOT] NULL, [NOT] IN (...),
 [NOT] BETWEEN, x [NOT] LIKE 'pattern' [ESCAPE 'c'], CAST(x AS type), CASE [x] WHEN .. THEN .. [ELSE ..] END,
@@ -261,6 +263,10 @@ class B200SQLEngine:
     def _join(self, items: str, rest: str, tables: Dict[str, DataFrame], sql: str) -> DataFrame:
         if items.strip() != "*":
             raise NotImplementedError(f"only SELECT * is supported for joins: {sql}")
+        m = re.match(rf"(?is)^(`?{_IDENT}`?)(?:\s+AS)?(?:\s+({_IDENT}))?\s+ASOF\s+(?:(INNER|LEFT|RIGHT|FULL)(?:\s+OUTER)?\s+)?"
+                     rf"JOIN\s+(`?{_IDENT}`?)(?:\s+AS)?(?:\s+({_IDENT}))?(?:\s+(USING|ON)\s+(.+))?$", rest)
+        if m is not None:
+            return self._asof_join(m, tables, sql)
         m = re.match(rf"(?is)^(`?{_IDENT}`?)(?:\s+AS)?(?:\s+({_IDENT}))?\s+"
                      r"((?:INNER|CROSS|LEFT SEMI|LEFT ANTI|SEMI|ANTI|LEFT OUTER|RIGHT OUTER|FULL OUTER|"
                      r"LEFT|RIGHT|FULL)\s+)?JOIN\s+"
@@ -285,6 +291,61 @@ class B200SQLEngine:
                         raise NotImplementedError(f"only equi-joins on equally named columns: {sql}")
                     on.append(mm.group(1))
         return self._engine.join(t1, t2, how=how, on=on)
+
+    def _asof_join(self, m: Any, tables: Dict[str, DataFrame], sql: str) -> DataFrame:
+        """``a ASOF [LEFT] JOIN b ON a.k = b.k AND a.t >= b.t`` (DuckDB's form): equalities on equally named
+        columns and one inequality on the as-of column, whose operands name both tables.  ``a.t >= b.t`` is a
+        backward search, ``>`` a strict one, ``<=`` / ``<`` forward.  ``USING (k, ..., t)``: equality on every
+        column but the last, ``>=`` on the last."""
+        t1, t2 = self._table(m.group(1), tables, sql), self._table(m.group(4), tables, sql)
+        kind = (m.group(3) or "INNER").upper()
+        if kind not in ("INNER", "LEFT"):
+            raise NotImplementedError(f"ASOF {kind} JOIN: an as-of join is inner or left outer: {sql}")
+        how = "left_outer" if kind == "LEFT" else "inner"
+        if m.group(6) is None:
+            raise NotImplementedError(f"an as-of join needs ON or USING: {sql}")
+        cond = m.group(7).strip()
+        if m.group(6).upper() == "USING":
+            names = [c.strip().strip("`") for c in cond.strip("() ").split(",")]
+            return self._engine.asof_join(t1, t2, on=names[:-1], asof=names[-1], how=how, direction="backward",
+                                          allow_exact_matches=True)
+        left_names = {m.group(1).strip("`").lower()} | ({m.group(2).lower()} if m.group(2) else set())
+        right_names = {m.group(4).strip("`").lower()} | ({m.group(5).lower()} if m.group(5) else set())
+        on: List[str] = []
+        ineq: List[Tuple[str, str]] = []
+        for part in re.split(r"(?i)\s+AND\s+", cond):
+            mm = re.match(rf"^\(?\s*(?:({_IDENT})\.)?({_IDENT})\s*(>=|<=|=|>|<)\s*(?:({_IDENT})\.)?({_IDENT})\s*\)?$",
+                          part.strip())
+            if mm is None or mm.group(2) != mm.group(5):
+                raise NotImplementedError(f"an as-of join compares equally named columns: {sql}")
+            if mm.group(3) == "=":
+                on.append(mm.group(2))
+                continue
+            # a qualifier names a table or its alias; one that names neither (a dataframe handed to raw_sql has a
+            # generated name) is the table the other operand does not name, and if neither operand names one the
+            # operands are in FROM order: left table first
+            quals = [(q or "").lower() for q in (mm.group(1), mm.group(4))]
+            if "" in quals:
+                raise NotImplementedError(f"the as-of inequality must qualify both columns: {sql}")
+            sides = ["left" if q in left_names - right_names else "right" if q in right_names - left_names else None
+                     for q in quals]
+            if sides == [None, None] and quals[0] != quals[1]:
+                sides = ["left", "right"]
+            elif None in sides:
+                known = sides[1 - sides.index(None)]
+                sides = [s or ("right" if known == "left" else "left") for s in sides]
+            if sides[0] == sides[1]:
+                raise NotImplementedError(f"the as-of inequality must name each table once: {sql}")
+            op = mm.group(3)
+            if sides[0] == "right":  # b.t <= a.t is a.t >= b.t
+                op = {">=": "<=", "<=": ">=", ">": "<", "<": ">"}[op]
+            ineq.append((mm.group(2), op))
+        if len(ineq) != 1:
+            raise NotImplementedError(f"an as-of join needs exactly one inequality, got {len(ineq)}: {sql}")
+        asof, op = ineq[0]
+        return self._engine.asof_join(t1, t2, on=on, asof=asof, how=how,
+                                      direction="backward" if op in (">=", ">") else "forward",
+                                      allow_exact_matches=op in (">=", "<="))
 
 
 def _top_level_from(sql: str) -> Any:

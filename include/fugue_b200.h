@@ -480,6 +480,27 @@ int fb_scatter_rows(int dev, void* stream, int ncols, const void* const* d_src_c
                     const int32_t* d_widths, const uint8_t* const* d_src_valid, uint8_t* const* d_dst_valid,
                     const int64_t* idx, int64_t n);
 
+/* As-of join search (B200ExecutionEngine.asof_join; pandas.merge_asof semantics).  The right side is sorted by
+ * (key, as-of value); run r is rows [d_run_offsets[r], d_run_offsets[r + 1]) of one key, and d_right_codes holds
+ * their as-of values as unsigned 64-bit order codes (sort.py _unsigned_order_key) of key_class FB_RANGE_KEY_*.
+ * PRECONDITION: the codes ascend within every run (the host passes argsort_rows results); it is not checked.
+ * One thread per left row i: d_run[i] is its run (-1: none), d_left_codes[i] its own code, d_left_valid[i] == 0
+ * (NULL allowed) a NULL as-of value, which matches nothing.  The candidate is, in the run:
+ *   FB_ASOF_BACKWARD  the last row with code <= the row's (< without allow_exact_matches)
+ *   FB_ASOF_FORWARD   the first row with code >= the row's (>)
+ *   FB_ASOF_NEAREST   the closer of those two; on equal distance the backward one
+ * With has_tolerance, a candidate farther than `tolerance` (an int64 >= 0 in storage units for the integer
+ * classes, the bits of an f64 for FB_RANGE_KEY_F64) is no candidate.  Integer distances are exact; a float
+ * distance is one f64 subtraction (0 for equal values).  d_out[i] = d_right_rows[candidate] (the row before the
+ * sort), -1 where there is none. */
+#define FB_ASOF_BACKWARD 0
+#define FB_ASOF_FORWARD 1
+#define FB_ASOF_NEAREST 2
+int fb_asof_search(int dev, void* stream, int64_t nleft, const int64_t* d_run, const int64_t* d_run_offsets,
+                   const uint64_t* d_left_codes, const uint8_t* d_left_valid, const uint64_t* d_right_codes,
+                   const int64_t* d_right_rows, int key_class, int direction, int allow_exact_matches,
+                   int has_tolerance, uint64_t tolerance, int64_t* d_out);
+
 /* K7 fast path: inner / left-outer join on one 8-byte key with 4-byte slots (build row + 1; keys are
  * compared through the build key column) and a fused probe -> output assembly.
  *   fb_join2_build  : clear + insert (one 32-bit CAS per build row); d_status[0] = 1 on region overflow,

@@ -21,9 +21,11 @@ window semantics.  The map engine sorts by (keys, presort) first for such a map.
                  schema="key:long,v0:double,w:double", partition=PartitionSpec(by="key", algo="hash", num=256))
 """
 import datetime
+import math
 import struct
 from typing import Any, Dict, List, Optional, Tuple
 
+import numpy as np
 import pyarrow as pa
 import torch
 
@@ -32,7 +34,7 @@ from . import kernels as K
 from .aggregates import bivariate_of
 from .column import (AGGREGATES, PERCENTILES, ColumnExpr, Kind, SelectColumns, bivariate_xy, col as _col, has_window,
                      has_explicit_window, is_agg, is_explicit, result_type)
-from .table import B200Table, narrow, widen
+from .table import B200Table, _storage_dtype, narrow, widen
 
 
 def _f64_bits(v: float) -> int:
@@ -442,6 +444,10 @@ def evaluate_windows(t: B200Table, exprs: List[ColumnExpr]) -> _WindowTable:
         kw = {k: v for k, v in node.kwargs.items() if k not in ("partition_by", "order_by")}
         specs.setdefault((pb, ob), []).append((uid, ColumnExpr(Kind.WINDOW, node.head, args, kw)))
     base = X.project(t, pre) if len(pre) > len(t.schema) else t
+    for members in specs.values():  # a LAG / LEAD default the argument's type cannot hold fails before the sorts
+        for _, m in members:
+            if m.func in ("LAG", "LEAD") and m.kwargs["default"] is not None:
+                offset_default(m.kwargs["default"], base.schema.types[base.schema.index_of_key(m.arg.name)], m)
     n, dev = t.num_rows, t.device
     names, types = list(t.schema.names), list(t.schema.types)
     columns, valid, dicts = list(t.columns), list(t.valid), dict(t.dictionaries)
@@ -581,13 +587,93 @@ def _range_offsets(t: B200Table, frame: Tuple[Any, Any]) -> Tuple[Optional[int],
     return cls, start, end
 
 
-def _offset_value(base: B200Table,bare: ColumnExpr, arg_name: Dict[str, str], rows: torch.Tensor,
+_INT_RANGE = {8: (-(1 << 7), 1 << 7), 16: (-(1 << 15), 1 << 15), 32: (-(1 << 31), 1 << 31), 64: (-(1 << 63), 1 << 63)}
+
+
+def offset_default(default: Any, tp: pa.DataType, what: Any) -> Optional[int]:
+    """The storage of LAG / LEAD's ``default`` in a column of type ``tp``, as the unsigned integer of the storage's
+    bits (None for a string column, whose dictionary code is found when the gather runs).  The default is converted
+    as a literal in a CAST to ``tp`` would be: float16 / float32 round to nearest, once, from the float64 value (a
+    NaN keeps its sign and the top bits of its payload, as ``table.narrow``), integers take the type's range (uint64
+    all of ``[0, 2^64)``), bool takes True / False, a date or timestamp column takes DATE / TIMESTAMP literals in its
+    own units (a naive timestamp is UTC, an aware one is converted to UTC), a duration column a timedelta.  A default
+    the type cannot hold raises ValueError: a non-integer number for an integer column, an integer out of range (of
+    float64 too, for a float column), a number for a temporal column, a temporal literal that is not a whole number of
+    the column's units, a string for a column that is not a string, anything but a string for one that is."""
+    from .expr import _in_unit, time_unit
+
+    def bad(why: str) -> ValueError:
+        return ValueError(f"{what}: the default {default!r} {why} ({tp})")
+
+    if pa.types.is_string(tp) or pa.types.is_large_string(tp):
+        if not isinstance(default, str):
+            raise bad("is not a string, the column is")
+        return None
+    width = _storage_dtype(tp).itemsize * 8
+    if isinstance(default, str):
+        raise bad("is a string, the column is not")
+    if pa.types.is_boolean(tp):
+        if not isinstance(default, bool):
+            raise bad("is not a boolean")
+        return int(default)
+    if isinstance(default, bool):
+        raise bad("is a boolean, the column is not")
+    if pa.types.is_floating(tp):
+        if not isinstance(default, (int, float)):
+            raise bad("is not a number")
+        try:
+            x = float(default)
+        except OverflowError as e:
+            raise bad("is out of the float64 range") from e
+        if tp == pa.float16() and not math.isnan(x):
+            # numpy's float64 -> half rounds once; torch's CPU conversion rounds twice, through float32
+            with np.errstate(over="ignore"):
+                return int(np.array([x], np.float64).astype(np.float16).view(np.uint16)[0])
+        v = torch.tensor([x], dtype=torch.float64)
+        return int(narrow(v, tp).view(_BITS[width])[0]) & ((1 << width) - 1)
+    unit = time_unit(tp)
+    if unit is not None:
+        kind, code = unit
+        if not isinstance(default, (datetime.date, datetime.timedelta)) or \
+                (kind == "span") != isinstance(default, datetime.timedelta):
+            raise bad("is not a " + ("timedelta" if kind == "span" else "DATE or TIMESTAMP literal"))
+        if isinstance(default, datetime.datetime) and default.tzinfo is not None:
+            default = default.astimezone(datetime.timezone.utc).replace(tzinfo=None)
+        v, exact = _in_unit(default, code)
+        if not exact:
+            raise bad("is not a whole number of the column's units")
+        lo, hi = _INT_RANGE[width]
+    elif pa.types.is_integer(tp):
+        if isinstance(default, float):
+            if not default.is_integer():
+                raise bad("is not an integer")
+            default = int(default)
+        if not isinstance(default, int):
+            raise bad("is not an integer")
+        v = default
+        lo, hi = (0, 1 << tp.bit_width) if pa.types.is_unsigned_integer(tp) else _INT_RANGE[tp.bit_width]
+    else:
+        raise bad("has no conversion to the column's type")
+    if not lo <= v < hi:
+        raise bad("is out of the column's range")
+    return v & ((1 << width) - 1)
+
+
+_BITS = {8: torch.uint8, 16: torch.int16, 32: torch.int32, 64: torch.int64}
+
+
+def _offset_value(base: B200Table, bare: ColumnExpr, arg_name: Dict[str, str], rows: torch.Tensor,
                   seg_first: Any, seg_last: Any) -> Any:
-    """LAG / LEAD: a gather of the row ``n`` before / after, NULL (then ``default``) across a partition bound."""
+    """LAG / LEAD: a gather of the row ``n`` before / after, NULL (then ``default``) across a partition bound.
+    The default is converted to the argument's type here, when the plan is built (``offset_default``); ``n`` is
+    clamped to the row count, so that ``rows + n`` cannot wrap: every ``n`` at or past a partition's length gives
+    the default on all its rows."""
     name = arg_name[bare.arg.fingerprint()]
     ci = base.schema.index_of_key(name)
     c, m, tp = base.columns[ci], base.valid[ci], base.schema.types[ci]
-    k, default = bare.kwargs["n"], bare.kwargs["default"]
+    k, default = min(bare.kwargs["n"], int(rows.shape[0])), bare.kwargs["default"]
+    d = base.dictionaries.get(name)
+    bits = None if default is None else offset_default(default, tp, bare)
 
     def run(_: Any) -> Any:
         if bare.func == "LAG":
@@ -598,23 +684,21 @@ def _offset_value(base: B200Table,bare: ColumnExpr, arg_name: Dict[str, str], ro
             ok = src <= seg_last()
         idx = torch.where(ok, src, torch.full_like(src, -1)).contiguous()
         (g,), (gv,) = K.gather_rows([c], [m], idx, want_valid=True)
-        d = base.dictionaries.get(name)
+        dd = d
         if default is not None:
-            if d is not None:
-                if not isinstance(default, str):
-                    raise NotImplementedError(f"non-string default of {bare} on a string column")
-                hit = d.index(default).as_py() if len(d) > 0 else -1
+            if dd is not None:
+                hit = dd.index(default).as_py() if len(dd) > 0 else -1
                 if hit is None or hit < 0:
-                    hit = len(d)
-                    d = pa.concat_arrays([d, pa.array([default], type=d.type)])
+                    hit = len(dd)
+                    dd = pa.concat_arrays([dd, pa.array([default], type=dd.type)])
                 fill = torch.full_like(g, hit)
-            elif isinstance(default, str):
-                raise NotImplementedError(f"string default of {bare} on a {tp} column")
             else:
-                fill = torch.full((), default, dtype=torch.float64 if isinstance(default, float) else torch.int64,
-                                  device=g.device).to(g.dtype).expand_as(g)
+                gb = g.view(_BITS[g.element_size() * 8])
+                signed = bits - (1 << (8 * g.element_size())) if gb.dtype != torch.uint8 and \
+                    bits >= (1 << (8 * g.element_size() - 1)) else bits
+                fill = torch.full_like(gb, signed).view(g.dtype)
             g = torch.where(ok, g, fill).contiguous()
             gv = torch.where(ok, gv, torch.ones_like(gv)).contiguous()
-        return g, gv, tp, d
+        return g, gv, tp, dd
 
     return run

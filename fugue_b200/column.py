@@ -761,6 +761,10 @@ def _range_frame(frame: Any) -> Tuple[Any, Any]:
 
 
 def _offset_fn(name: str, c: Any, n: Any, default: Any, aggregated: bool = False) -> ColumnExpr:
+    """LAG / LEAD of ``c`` by ``n >= 0`` rows, ``default`` (a literal) where that row is outside the partition.  The
+    default is converted to the argument's type as a literal in a CAST would be, when the plan is built, and one the
+    type cannot hold exactly (2.5 for an integer, 1000 for int8, -1 for uint64, noon for a date, a string for a number)
+    raises ValueError (``colmap.offset_default``, DESIGN §7p); any ``n`` at or past a partition's length gives it."""
     if isinstance(n, bool) or not isinstance(n, int) or n < 0:
         raise ValueError(f"{name}: n must be a non-negative int, got {n!r}")
     if not (default is None or isinstance(default, _LITERAL_TYPES)):

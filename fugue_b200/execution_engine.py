@@ -1045,7 +1045,7 @@ class B200ExecutionEngine(EngineLifecycle):
             def mapper(node: Any) -> Any:
                 if node.kind == Kind.AGG:
                     return col(agg_col[node.alias("").cast(None).fingerprint()])
-                if node.kind == Kind.LITERAL:
+                if node.kind in (Kind.LITERAL, Kind.WILDCARD):  # COUNT(*) OVER (...) counts the group rows
                     return None
                 uid = node.alias("").cast(None).fingerprint()
                 if uid in key_of:

@@ -22,6 +22,9 @@ the window nodes of ``fugue_b200.column`` mean with SQL window semantics over th
 :func:`segmented_scan` is the scan itself on numpy arrays (what ``fb_segmented_scan`` computes);
 :func:`window_map` evaluates a whole ``ColumnMap`` on an Arrow table.
 """
+import datetime
+import math
+import struct
 from collections import OrderedDict
 from typing import Any, Dict, List, Optional, Sequence, Tuple
 
@@ -81,6 +84,92 @@ def segmented_scan(values: Optional[np.ndarray], valid: Optional[np.ndarray], of
     return np.where(counts > 0, out, 0), counts
 
 
+# ---- LAG / LEAD defaults ----------------------------------------------------------------------------
+_INT_BITS = {pa.int8(): (8, True), pa.int16(): (16, True), pa.int32(): (32, True), pa.int64(): (64, True),
+             pa.uint8(): (8, False), pa.uint16(): (16, False), pa.uint32(): (32, False), pa.uint64(): (64, False)}
+_PER_UNIT_US = {"D": (86_400_000_000, 1), "s": (1_000_000, 1), "ms": (1000, 1), "us": (1, 1), "ns": (1, 1000)}
+
+
+def _small_float_bits(x: float, fmt: str, width: int, mbits: int) -> int:
+    """``x`` rounded to nearest in the IEEE format of ``width`` bits (``struct`` format ``fmt``); a NaN keeps its
+    sign and the top ``mbits`` bits of its payload (the lowest bit set if none is left)."""
+    b64 = struct.unpack("<Q", struct.pack("<d", x))[0]
+    sign = b64 >> 63
+    if math.isnan(x):
+        mant = (b64 >> (52 - mbits)) & ((1 << mbits) - 1)
+        expo = ((1 << (width - 1 - mbits)) - 1) << mbits
+        return (sign << (width - 1)) | expo | (mant or 1)
+    try:
+        return struct.unpack("<H" if width == 16 else "<I", struct.pack(fmt, x))[0]
+    except OverflowError:  # rounds past the largest finite value: the infinity of its sign
+        return struct.unpack("<H" if width == 16 else "<I", struct.pack(fmt, math.copysign(math.inf, x)))[0]
+
+
+def offset_default(d: Any, tp: pa.DataType) -> pa.Array:
+    """LAG / LEAD's default as a one-element array of the argument's type, converted as a literal in a CAST to ``tp``:
+    floats rounded to nearest once from the float64 value, integers in the type's range, True / False for bool, DATE / TIMESTAMP literals in a
+    date or timestamp column's units, a timedelta in a duration's, a string for a string.  ValueError where the type
+    cannot hold the default exactly."""
+    def bad() -> ValueError:
+        return ValueError(f"a LAG / LEAD default {d!r} does not convert exactly to {tp}")
+
+    if pa.types.is_string(tp) or pa.types.is_large_string(tp):
+        if not isinstance(d, str):
+            raise bad()
+        return pa.array([d], type=tp)
+    if isinstance(d, str):
+        raise bad()
+    if pa.types.is_boolean(tp):
+        if not isinstance(d, bool):
+            raise bad()
+        return pa.array([d], type=tp)
+    if isinstance(d, bool):
+        raise bad()
+    if pa.types.is_floating(tp):
+        if not isinstance(d, (int, float)):
+            raise bad()
+        try:
+            x = float(d)
+        except OverflowError as e:  # an integer past float64
+            raise bad() from e
+        if tp == pa.float64():
+            return pa.array([x], type=tp)
+        if tp == pa.float32():
+            return pa.array(np.array([_small_float_bits(x, "<f", 32, 23)], np.uint32).view(np.float32))
+        return pa.array(np.array([_small_float_bits(x, "<e", 16, 10)], np.uint16).view(np.float16))
+    if tp in _INT_BITS:
+        if isinstance(d, float) and d.is_integer():
+            d = int(d)
+        if not isinstance(d, int):
+            raise bad()
+        bits, signed = _INT_BITS[tp]
+        lo, hi = (-(1 << (bits - 1)), 1 << (bits - 1)) if signed else (0, 1 << bits)
+        if not lo <= d < hi:
+            raise bad()
+        return pa.array([d], type=tp)
+    span = pa.types.is_duration(tp)
+    if pa.types.is_date(tp) or pa.types.is_timestamp(tp) or span:
+        if not isinstance(d, (datetime.date, datetime.timedelta)) or span != isinstance(d, datetime.timedelta):
+            raise bad()
+        if isinstance(d, datetime.timedelta):
+            us = d // datetime.timedelta(microseconds=1)
+        else:
+            dt = d if isinstance(d, datetime.datetime) else datetime.datetime(d.year, d.month, d.day)
+            if dt.tzinfo is not None:  # an aware timestamp: its UTC time
+                dt = dt.astimezone(datetime.timezone.utc).replace(tzinfo=None)
+            us = (dt - datetime.datetime(1970, 1, 1)) // datetime.timedelta(microseconds=1)
+        unit = "D" if pa.types.is_date32(tp) else ("ms" if pa.types.is_date64(tp) else tp.unit)
+        per, mul = _PER_UNIT_US[unit]
+        if (us * mul) % per:
+            raise bad()
+        v = us * mul // per
+        bits = 32 if pa.types.is_date32(tp) else 64
+        if not -(1 << (bits - 1)) <= v < (1 << (bits - 1)):
+            raise bad()
+        return pa.array([v], type=pa.int32() if bits == 32 else pa.int64()).cast(tp)
+    raise bad()
+
+
 # ---- whole maps -----------------------------------------------------------------------------------
 def _column(t: pa.Table, name: str) -> Tuple[np.ndarray, np.ndarray, pa.DataType]:
     a = t.column(name).combine_chunks()
@@ -136,13 +225,16 @@ def window_map(table: pa.Table, keys: Sequence[str], presort: "OrderedDict[str, 
             v, _ = segmented_scan(peer.astype(np.int64), None, offsets, "SUM_I64")
             return pa.array(v, type=pa.int64())
         if fn in ("LAG", "LEAD"):
-            v, ok, tp = arg_of(e.arg)
-            src = pos - e.kwargs["n"] if fn == "LAG" else pos + e.kwargs["n"]
-            inside = (src >= first) if fn == "LAG" else (src <= last)
-            srcc = np.clip(src, 0, max(n - 1, 0))
+            if e.arg.kind == Kind.NAMED and e.arg.as_type is None:
+                a = st.column(e.arg.name).combine_chunks()
+            else:
+                a = pa.array(ox.evaluate(e.arg, pdf), from_pandas=True)
             d = e.kwargs["default"]
-            vals = [(v[j] if ok[j] else None) if ins else d for j, ins in zip(srcc.tolist(), inside.tolist())]
-            return pa.array(vals, type=tp)
+            # the source row in python ints, exact for every n >= 0; outside the partition: the appended default
+            step = -e.kwargs["n"] if fn == "LAG" else e.kwargs["n"]
+            src = [p + step if lo <= p + step <= hi else n for p, lo, hi in zip(range(n), first.tolist(), last.tolist())]
+            tail = pa.nulls(1, a.type) if d is None else offset_default(d, a.type)
+            return pa.concat_arrays([a, tail]).take(pa.array(src, type=pa.int64()))
         whole = not e.kwargs["running"]
 
         def fin(x: np.ndarray) -> np.ndarray:

@@ -110,6 +110,10 @@ SIGNATURES = {
     "fb_scatter_rows": (C.c_int, [C.c_int, _vp, C.c_int, _vp, _vp, _vp, _vp, _vp, _vp, C.c_int64]),
     "fb_asof_search": (C.c_int, [C.c_int, _vp, C.c_int64, _vp, _vp, _vp, _vp, _vp, _vp, C.c_int, C.c_int, C.c_int,
                                  C.c_int, C.c_uint64, _vp]),
+    "fb_range_join_count": (C.c_int, [C.c_int, _vp, C.c_int64, _vp, _vp, _vp, _vp, C.c_int64, _vp, _vp, _vp,
+                                      C.c_size_t, C.c_int, C.c_int, _vp]),
+    "fb_range_join_emit": (C.c_int, [C.c_int, _vp, C.c_int64, _vp, _vp, _vp, _vp, C.c_int64, _vp, _vp, _vp,
+                                     C.c_size_t, _vp, C.c_int, C.c_int, _vp, _vp, _vp, _vp]),
     "fb_copy_runs_dma": (C.c_int, [C.c_int, _vp, C.c_int64, _vp, _vp, _vp]),
     "fb_copy_runs_dma_streams": (C.c_int, [C.c_int, C.c_int64, _vp, _vp, _vp, _vp, C.c_int]),
     "fb_pull_runs_tma": (C.c_int, [C.c_int, _vp, C.c_int, _vp, _vp, _vp, C.c_int]),
@@ -138,6 +142,7 @@ SIGNATURES = {
     "fb_window_bounded_scratch_bytes": (C.c_size_t, [C.c_int64, C.c_int]),
     "fb_window_bounded": (C.c_int, [C.c_int, _vp, C.c_int64, _vp, _vp, C.c_int, _i32p, _vpp, _vpp, _vpp, _vpp, _vp,
                                     C.c_size_t]),
+    "fb_window_tree": (C.c_int, [C.c_int, _vp, C.c_int64, C.c_int, _i32p, _vpp, _vpp, _vp, C.c_size_t]),
     "fb_quantile_scratch_bytes": (C.c_size_t, [C.c_int, C.c_int64, C.c_int64]),
     "fb_segmented_quantile": (C.c_int, [C.c_int, _vp, C.c_int64, C.c_int64, _vp, _vp, _vp, C.c_int, C.c_int,
                                         C.POINTER(C.c_double), _i32p, _vp, _vpp, _vp, C.c_size_t]),

@@ -549,6 +549,22 @@ def asof_join(df1: Any, df2: Any, on: Optional[Iterable[str]], asof: str, how: s
     return res.as_pandas() if res.is_local else res.native
 
 
+def range_join(df1: Any, df2: Any, on: Optional[Iterable[str]], at: str, start: str, end: str, how: str = "inner",
+               closed: str = "both", engine: Any = None, engine_conf: Any = None, as_fugue: bool = False,
+               as_local: bool = False) -> Any:
+    """Range join of two dataframes (``B200ExecutionEngine.range_join``): every row of ``df1`` with every row of
+    ``df2`` of equal ``on`` key (None: the common columns but ``at``; empty: one group) whose interval
+    [``start``, ``end``] holds its ``at`` value; ``closed`` ("both", "left", "right", "neither") says which
+    ends belong to the interval."""
+    e = make_execution_engine(engine, engine_conf, infer_by=[df1, df2])
+    res: DataFrame = e.range_join(e.to_df(df1), e.to_df(df2), on=None if on is None else list(on), at=at,
+                                  start=start, end=end, how=how, closed=closed)
+    res = e.convert_yield_dataframe(res, as_local)
+    if as_fugue or any(isinstance(x, DataFrame) for x in (df1, df2)):
+        return res
+    return res.as_pandas() if res.is_local else res.native
+
+
 def inner_join(df1: Any, df2: Any, *dfs: Any, **kwargs: Any) -> Any:
     return join(df1, df2, *dfs, how="inner", **kwargs)
 

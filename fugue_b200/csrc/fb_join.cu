@@ -13,6 +13,7 @@
 // 8-byte gather).  Output order: probe-row major, deterministic for a given table.
 // Algorithmic bytes (SURVEY.md 8d, config 5): 16 + 16 read + 24 written per output row.
 #include "fb_common.cuh"
+#include "fb_tree.cuh"
 
 namespace {
 
@@ -349,6 +350,105 @@ fb_asof_search_kernel(int64_t n, const int64_t* __restrict__ run, const int64_t*
     if (pick >= 0) res = __ldg((const long long*)rows + pick);
   }
   out[i] = res;
+}
+
+// ---- range join: per left row, every interval of its run that holds its value ----------------------------
+// The right side is sorted by (key, start); run r = rows [run_off[r], run_off[r + 1]).  `ends` holds every sorted
+// row's end code with the sign bit flipped (so a signed compare orders the unsigned codes), and `tv` the levels
+// >= 1 of the aligned MAX tree over `ends` (fb_window_tree, layout TreeLevels): node (l, m) is the largest
+// end of rows [m 2^l, (m + 1) 2^l).  A row with value x has its candidates in [s, p), p the end of the rows whose
+// start passes the lower test; the hits among them are the rows whose flipped end is >= t (the upper test).
+struct RangeTree {
+  const int64_t* ends;  // level 0
+  const int64_t* tv;    // levels >= 1
+};
+
+__device__ __forceinline__ int64_t range_node(const RangeTree& T, const TreeLevels& L, int level, int64_t m) {
+  return level == 0 ? __ldg((const long long*)T.ends + m) : __ldg((const long long*)T.tv + L.off[level] + m);
+}
+
+// the last row of [s, q) whose end is >= t, -1 if none: the blocks of [s, q)'s canonical decomposition from
+// right to left (the right-hand blocks by rising level, then the left-hand ones by falling level), then down
+// the first block that holds a hit, to its rightmost row.  O(log (q - s)).
+__device__ __forceinline__ int64_t range_prev_hit(const RangeTree& T, const TreeLevels& L, int64_t s, int64_t q,
+                                                  int64_t t) {
+  int64_t lo = s, hi = q;
+  int level = 0;
+  uint64_t left_levels = 0;  // levels with a left-hand block: block ceil(s / 2^l) there
+  int64_t b = -1;
+  for (; lo < hi; ++level, lo >>= 1, hi >>= 1) {
+    if ((hi & 1) && range_node(T, L, level, hi - 1) >= t) {
+      b = hi - 1;
+      break;
+    }
+    hi &= ~(int64_t)1;
+    if (lo & 1) {
+      left_levels |= 1ull << level;
+      ++lo;
+    }
+  }
+  if (b < 0) {
+    while (left_levels != 0) {
+      level = 63 - __clzll((long long)left_levels);
+      left_levels &= ~(1ull << level);
+      const int64_t m = (s + ((int64_t)1 << level) - 1) >> level;
+      if (range_node(T, L, level, m) >= t) {
+        b = m;
+        break;
+      }
+    }
+    if (b < 0) return -1;
+  }
+  for (; level > 0; --level) b = range_node(T, L, level - 1, 2 * b + 1) >= t ? 2 * b + 1 : 2 * b;
+  return b;
+}
+
+// kEmit == false: counts[i] = the row's matches (1 for an unmatched row when outer).  kEmit == true: the same walk
+// writes its (left row, right row) pairs into [offsets[i], offsets[i] + counts[i]) from the back, so they come out
+// in ascending sorted position, which is (start, right input order).
+template <bool kEmit>
+__global__ void __launch_bounds__(256)
+fb_range_join_kernel(int64_t n, const int64_t* __restrict__ run, const int64_t* __restrict__ run_off,
+                     const uint64_t* __restrict__ left_codes, const uint8_t* __restrict__ left_valid,
+                     const uint64_t* __restrict__ starts, const RangeTree T, const __grid_constant__ TreeLevels L,
+                     const int64_t* __restrict__ rows, int closed, int outer, int64_t* __restrict__ counts,
+                     const int64_t* __restrict__ offsets, int64_t* __restrict__ out_left,
+                     int64_t* __restrict__ out_right) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  int64_t c = 0, o = 0;
+  if (kEmit) {
+    o = __ldg((const long long*)offsets + i) + __ldg((const long long*)counts + i);  // one past the row's last slot
+  }
+  const int64_t r = __ldg((const long long*)run + i);
+  if (r >= 0 && (left_valid == nullptr || __ldg(left_valid + i) != 0)) {
+    const uint64_t x = __ldg((const unsigned long long*)left_codes + i);
+    const int64_t s = __ldg((const long long*)run_off + r), e = __ldg((const long long*)run_off + r + 1);
+    // lower test start <= x (closed left: the first start > x ends the candidates) or start < x
+    const int64_t p = (closed & FB_RANGE_CLOSED_LEFT) ? asof_bound<true>(starts, s, e, x)
+                                                        : asof_bound<false>(starts, s, e, x);
+    // upper test end >= x (closed right) or end >= x + 1; nothing is > the largest code
+    if ((closed & FB_RANGE_CLOSED_RIGHT) || x != ~0ull) {
+      const int64_t t = (int64_t)(((closed & FB_RANGE_CLOSED_RIGHT) ? x : x + 1) ^ kAsofSign);
+      for (int64_t q = range_prev_hit(T, L, s, p, t); q >= 0; q = range_prev_hit(T, L, s, q, t)) {
+        ++c;
+        if (kEmit) {
+          --o;
+          out_left[o] = i;
+          out_right[o] = __ldg((const long long*)rows + q);
+        }
+      }
+    }
+  }
+  if (c == 0 && outer) {
+    c = 1;
+    if (kEmit) {
+      --o;
+      out_left[o] = i;
+      out_right[o] = -1;
+    }
+  }
+  if (!kEmit) counts[i] = c;
 }
 
 // ---- stream compaction: indices of the non-zero bytes of a mask, in order ---------------------
@@ -713,6 +813,35 @@ fb_join2_emit_kernel(const uint64_t* __restrict__ pkeys, int64_t nprobe, const u
   }
 }
 
+// the checks and the launch shared by fb_range_join_count and fb_range_join_emit
+template <bool kEmit>
+int range_join_launch(int dev, void* stream, int64_t nleft, const int64_t* d_run, const int64_t* d_run_offsets,
+                      const uint64_t* d_left_codes, const uint8_t* d_left_valid, int64_t nright,
+                      const uint64_t* d_start_codes, const int64_t* d_end_keys, const void* d_tree,
+                      size_t tree_bytes, const int64_t* d_right_rows, int closed, int outer, int64_t* d_counts,
+                      const int64_t* d_offsets, int64_t* d_out_left, int64_t* d_out_right) {
+  FB_CHECK(nleft >= 0 && nright >= 0, "negative count");
+  FB_CHECK((closed & ~(FB_RANGE_CLOSED_LEFT | FB_RANGE_CLOSED_RIGHT)) == 0, "unknown closed flags %d", closed);
+  if (nleft == 0) return 0;
+  FB_CHECK(d_run != nullptr && d_run_offsets != nullptr && d_left_codes != nullptr && d_counts != nullptr,
+           "NULL run, offsets, codes or counts");
+  FB_CHECK(nright == 0 || (d_start_codes != nullptr && d_end_keys != nullptr), "NULL start or end codes");
+  const size_t need = fb_window_bounded_scratch_bytes(nright, 1);
+  FB_CHECK(need == 0 || (d_tree != nullptr && tree_bytes >= need), "tree too small: %zu < %zu", tree_bytes, need);
+  FB_CHECK(!kEmit || (d_right_rows != nullptr && d_offsets != nullptr && d_out_left != nullptr &&
+                      d_out_right != nullptr), "NULL rows, offsets or outputs");
+  const int64_t grid = (nleft + 255) / 256;
+  FB_CHECK(grid < (1LL << 31), "too many rows");
+  FbDeviceGuard guard(dev);
+  FB_CHECK(guard.ok, "cannot select device %d", dev);
+  const RangeTree T{d_end_keys, (const int64_t*)d_tree};
+  fb_range_join_kernel<kEmit><<<(unsigned)grid, 256, 0, (cudaStream_t)stream>>>(
+      nleft, d_run, d_run_offsets, d_left_codes, d_left_valid, d_start_codes, T, tree_levels(nright), d_right_rows,
+      closed, outer ? 1 : 0, d_counts, d_offsets, d_out_left, d_out_right);
+  FB_CUDA(cudaGetLastError());
+  return 0;
+}
+
 }  // namespace
 
 extern "C" {
@@ -901,6 +1030,26 @@ int fb_asof_search(int dev, void* stream, int64_t nleft, const int64_t* d_run, c
       allow_exact_matches ? 0 : 1, has_tolerance ? 1 : 0, tolerance, d_out);
   FB_CUDA(cudaGetLastError());
   return 0;
+}
+
+int fb_range_join_count(int dev, void* stream, int64_t nleft, const int64_t* d_run, const int64_t* d_run_offsets,
+                        const uint64_t* d_left_codes, const uint8_t* d_left_valid, int64_t nright,
+                        const uint64_t* d_start_codes, const int64_t* d_end_keys, const void* d_tree,
+                        size_t tree_bytes, int closed, int outer, int64_t* d_counts) {
+  return range_join_launch<false>(dev, stream, nleft, d_run, d_run_offsets, d_left_codes, d_left_valid, nright,
+                                  d_start_codes, d_end_keys, d_tree, tree_bytes, nullptr, closed, outer, d_counts,
+                                  nullptr, nullptr, nullptr);
+}
+
+int fb_range_join_emit(int dev, void* stream, int64_t nleft, const int64_t* d_run, const int64_t* d_run_offsets,
+                       const uint64_t* d_left_codes, const uint8_t* d_left_valid, int64_t nright,
+                       const uint64_t* d_start_codes, const int64_t* d_end_keys, const void* d_tree,
+                       size_t tree_bytes, const int64_t* d_right_rows, int closed, int outer,
+                       const int64_t* d_counts, const int64_t* d_offsets, int64_t* d_out_left,
+                       int64_t* d_out_right) {
+  return range_join_launch<true>(dev, stream, nleft, d_run, d_run_offsets, d_left_codes, d_left_valid, nright,
+                                 d_start_codes, d_end_keys, d_tree, tree_bytes, d_right_rows, closed, outer,
+                                 (int64_t*)d_counts, d_offsets, d_out_left, d_out_right);
 }
 
 // ---- K7 fast path (see the kernels above) ------------------------------------------------------------

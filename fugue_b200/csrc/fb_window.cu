@@ -39,6 +39,7 @@
 #include <mutex>
 
 #include "fb_common.cuh"
+#include "fb_tree.cuh"
 
 namespace {
 
@@ -957,27 +958,7 @@ fb_range_bounds_kernel(int64_t nrows, int64_t nseg, const int64_t* __restrict__ 
 
 // ---- aggregates over arbitrary row intervals: an aligned power-of-two block tree ----------------------
 // Level l >= 1 holds (op, count) of rows [m 2^l, (m + 1) 2^l) for m < nrows >> l, in scratch; level 0 is the
-// input.  Level l starts at node tree_off[l] of a column's nodes.
-constexpr int kTreeMaxLevels = 64;
-
-struct TreeLevels {
-  int64_t off[kTreeMaxLevels];
-  int64_t total;  // nodes of levels >= 1 per column
-  int levels;     // highest level with a node
-};
-
-TreeLevels tree_levels(int64_t nrows) {
-  TreeLevels L;
-  memset(&L, 0, sizeof(L));
-  int64_t acc = 0;
-  for (int l = 1; l < kTreeMaxLevels && (nrows >> l) > 0; ++l) {
-    L.off[l] = acc;
-    acc += nrows >> l;
-    L.levels = l;
-  }
-  L.total = acc;
-  return L;
-}
+// input.  Level l starts at node tree_off[l] of a column's nodes (TreeLevels, fb_tree.cuh).
 
 __device__ __forceinline__ St tree_node(const ScanCols& a, int col, bool is_count, const TreeLevels& L,
                                         const uint64_t* __restrict__ tv, const int64_t* __restrict__ tc, int level,
@@ -1032,6 +1013,21 @@ fb_tree_query_kernel(const __grid_constant__ ScanCols a, const __grid_constant__
     if (a.out_vals[col] != nullptr) ((uint64_t*)a.out_vals[col])[i] = res.c > 0 ? res.v : 0;
     if (a.out_count[col] != nullptr) a.out_count[col][i] = res.c;
   }
+}
+
+// levels 1.. of the tree of every column of `a` into scratch (values, then counts), one launch per level
+int build_tree(int dev, cudaStream_t st, const ScanCols& a, int64_t nrows, void* scratch) {
+  const TreeLevels L = tree_levels(nrows);
+  uint64_t* tv = (uint64_t*)scratch;
+  int64_t* tc = (int64_t*)(tv + (size_t)a.ncols * L.total);
+  const int64_t max_grid = 8 * (int64_t)fb_sm_count(dev);
+  for (int level = 1; level <= L.levels; ++level) {
+    const int64_t blocks = ((nrows >> level) + kThreads - 1) / kThreads;
+    const dim3 grid((unsigned)(blocks < max_grid ? blocks : max_grid), (unsigned)a.ncols);
+    fb_tree_level_kernel<<<grid, kThreads, 0, st>>>(a, L, level, nrows, tv, tc);
+    FB_CUDA(cudaGetLastError());
+  }
+  return 0;
 }
 
 // the column arrays of the C ABI -> ScanCols (checked)
@@ -1298,17 +1294,26 @@ extern "C" int fb_window_bounded(int dev, void* stream, int64_t nrows, const int
   FbDeviceGuard guard(dev);
   FB_CHECK(guard.ok, "cannot select device %d", dev);
   cudaStream_t st = (cudaStream_t)stream;
+  if (build_tree(dev, st, a, nrows, scratch) != 0) return 2;
   const TreeLevels L = tree_levels(nrows);
-  uint64_t* tv = (uint64_t*)scratch;
-  int64_t* tc = (int64_t*)(tv + (size_t)ncols * L.total);
-  const int64_t max_grid = 8 * (int64_t)fb_sm_count(dev);
-  for (int level = 1; level <= L.levels; ++level) {
-    const int64_t blocks = ((nrows >> level) + kThreads - 1) / kThreads;
-    const dim3 grid((unsigned)(blocks < max_grid ? blocks : max_grid), (unsigned)ncols);
-    fb_tree_level_kernel<<<grid, kThreads, 0, st>>>(a, L, level, nrows, tv, tc);
-    FB_CUDA(cudaGetLastError());
-  }
-  fb_tree_query_kernel<<<(unsigned)grid, kThreads, 0, st>>>(a, L, nrows, d_lo, d_hi, tv, tc);
+  const uint64_t* tv = (const uint64_t*)scratch;
+  fb_tree_query_kernel<<<(unsigned)grid, kThreads, 0, st>>>(a, L, nrows, d_lo, d_hi, tv,
+                                                             (const int64_t*)(tv + (size_t)ncols * L.total));
   FB_CUDA(cudaGetLastError());
   return 0;
+}
+
+extern "C" int fb_window_tree(int dev, void* stream, int64_t nrows, int ncols, const int32_t* ops,
+                              const void* const* vals, const uint8_t* const* valid, void* scratch,
+                              size_t scratch_bytes) {
+  FB_CHECK(nrows >= 0, "negative row count");
+  ScanCols a;
+  if (scan_cols(nrows, ncols, ops, vals, valid, nullptr, nullptr, &a) != 0) return 1;
+  if (nrows == 0) return 0;
+  const size_t need = fb_window_bounded_scratch_bytes(nrows, ncols);
+  FB_CHECK(need == 0 || (scratch != nullptr && scratch_bytes >= need), "scratch too small: %zu < %zu", scratch_bytes,
+           need);
+  FbDeviceGuard guard(dev);
+  FB_CHECK(guard.ok, "cannot select device %d", dev);
+  return build_tree(dev, (cudaStream_t)stream, a, nrows, scratch) != 0 ? 2 : 0;
 }

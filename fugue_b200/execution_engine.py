@@ -1145,6 +1145,19 @@ class B200ExecutionEngine(EngineLifecycle):
         return device_asof_join(self.to_df(df1), self.to_df(df2), on, asof, how, direction, allow_exact_matches,
                                 tolerance)
 
+    def range_join(self, df1: Any, df2: Any, on: Optional[List[str]], at: str, start: str, end: str,
+                   how: str = "inner", closed: str = "both") -> B200DataFrame:
+        """Range join (DESIGN §7r): every row of ``df1``, in input order, with every row of ``df2`` of equal ``on``
+        key for which ``start <= at <= end``; ``closed`` ("both", "left", "right", "neither", as
+        ``pandas.Interval``) makes a side strict.  A row's matches come in ascending (``start``, df2 row order).
+        ``how`` is ``"inner"`` (unmatched rows dropped) or ``"left_outer"`` (one row with NULLs).  Output schema:
+        ``df1.schema`` followed by df2's columns other than ``on``."""
+        from .join import device_range_join
+
+        assert_or_throw(self.get_current_parallelism() <= 1, lambda: NotImplementedError(
+            "range joins on the multi-GPU engine: a rank holds only its own rows of the right table"))
+        return device_range_join(self.to_df(df1), self.to_df(df2), on, at, start, end, how, closed)
+
     # ---- set operations, NULL handling, sampling, IO (fugue_b200/relational.py) -----------
     def union(self, df1: Any, df2: Any, distinct: bool = True) -> B200DataFrame:
         from . import relational as R

@@ -291,12 +291,12 @@ def get_asof_schemas(df1: Any, df2: Any, on: Optional[List[str]], asof: str) -> 
     return on, Schema(df1.schema, df2.schema.extract(names2))
 
 
-def asof_key_class(name: str, tp: pa.DataType, is_string: bool) -> int:
+def asof_key_class(name: str, tp: pa.DataType, is_string: bool, what: str = "an as-of column") -> int:
     """The ``RANGE_KEY_*`` class of an as-of column: the key types RANGE frames take; anything else is a ValueError."""
     temporal = pa.types.is_date(tp) or pa.types.is_timestamp(tp) or pa.types.is_duration(tp) or \
         pa.types.is_time64(tp)
     if is_string or not (pa.types.is_integer(tp) or pa.types.is_floating(tp) or temporal):
-        raise ValueError(f"an as-of column must be numeric or temporal; {name} is {tp}")
+        raise ValueError(f"{what} must be numeric or temporal; {name} is {tp}")
     if pa.types.is_floating(tp):
         return K.RANGE_KEY_F64
     return K.RANGE_KEY_U64 if pa.types.is_unsigned_integer(tp) else K.RANGE_KEY_I64
@@ -353,29 +353,32 @@ def _asof_value(t: B200Table, name: str, cls: int) -> Tuple[torch.Tensor, Option
     return _unsigned_order_key(t, name, True), v
 
 
-def asof_rows(t1: B200Table, t2: B200Table, keys: List[str], asof: str, cls: int, direction: str,
-              allow_exact_matches: bool, tolerance: Any) -> torch.Tensor:
-    """Per left row, the right row it matches, -1 for none (int64)."""
+def sorted_runs(t1: B200Table, t2: B200Table, keys: List[str], by: str,
+                values: List[Tuple[torch.Tensor, Optional[torch.Tensor]]], keep: Optional[torch.Tensor] = None
+                ) -> Optional[Tuple[torch.Tensor, List[torch.Tensor], torch.Tensor, torch.Tensor]]:
+    """Steps 1 and 2 of the as-of and range joins (DESIGN §7q, §7r).  ``values`` are (order codes, validity) of
+    df2's value columns, ``by`` first.  1: the right rows that can match - a valid key, every value valid, and
+    ``keep`` (uint8, None: all) - sorted by (keys..., by) with the stable ``argsort_rows``.  2: the runs of equal
+    keys, and every left row's run through a ``JoinTable`` over the run heads.  Returns None when no right row is
+    kept, else (the kept right rows in sorted order, each value's codes in that order, per left row its run or -1,
+    the runs' int64 offsets)."""
     dev = t1.device
     n1, n2 = t1.num_rows, t2.num_rows
-    if n1 == 0:
-        return torch.empty(0, dtype=torch.int64, device=dev)
-    # 1. right side: drop the rows that can never match, sort the rest by (keys..., asof), stable
-    c2, av2 = _asof_value(t2, asof, cls)
+    # 1. right side: drop the rows that can never match, sort the rest by (keys..., by), stable
     if keys:
         k1, v1, k2, v2, exact = _key64(t1, t2, keys)
-        keep = v2 if av2 is None else (av2 if v2 is None else v2 & av2)
-    else:
-        keep = av2
+        keep = v2 if keep is None else (keep if v2 is None else v2 & keep)
+    for _, av2 in values:
+        keep = av2 if keep is None else (keep if av2 is None else keep & av2)
     kept = torch.arange(n2, dtype=torch.int64, device=dev) if keep is None else K.compact_indices(keep.contiguous())
-    sub = take_rows(B200Table(t2.schema.extract(keys + [asof]), [t2.column(k) for k in keys + [asof]],
-                              [t2.valid[t2.schema.index_of_key(k)] for k in keys + [asof]],
+    sub = take_rows(B200Table(t2.schema.extract(keys + [by]), [t2.column(k) for k in keys + [by]],
+                              [t2.valid[t2.schema.index_of_key(k)] for k in keys + [by]],
                               {k: t2.dictionaries[k] for k in keys if k in t2.dictionaries}), kept)
     if kept.shape[0] == 0:
-        return torch.full((n1,), -1, dtype=torch.int64, device=dev)
-    perm = argsort_rows(sub, OrderedDict([(k, True) for k in keys] + [(asof, True)]))
+        return None
+    perm = argsort_rows(sub, OrderedDict([(k, True) for k in keys] + [(by, True)]))
     rows = kept[perm].contiguous()
-    codes = c2[rows].contiguous()
+    codes = [c[rows].contiguous() for c, _ in values]
     # 2. runs of equal keys, and every left row's run
     if keys:
         heads = K.compact_indices(group_starts(take_rows(sub, perm), keys).contiguous())
@@ -393,9 +396,23 @@ def asof_rows(t1: B200Table, t2: B200Table, keys: List[str], asof: str, cls: int
     else:  # one group
         run = torch.zeros(n1, dtype=torch.int64, device=dev)
         run_offsets = torch.tensor([0, rows.shape[0]], dtype=torch.int64, device=dev)
+    return rows, codes, run, run_offsets.contiguous()
+
+
+def asof_rows(t1: B200Table, t2: B200Table, keys: List[str], asof: str, cls: int, direction: str,
+              allow_exact_matches: bool, tolerance: Any) -> torch.Tensor:
+    """Per left row, the right row it matches, -1 for none (int64)."""
+    dev = t1.device
+    n1 = t1.num_rows
+    if n1 == 0:
+        return torch.empty(0, dtype=torch.int64, device=dev)
+    runs = sorted_runs(t1, t2, keys, asof, [_asof_value(t2, asof, cls)])
+    if runs is None:
+        return torch.full((n1,), -1, dtype=torch.int64, device=dev)
+    rows, (codes,), run, run_offsets = runs
     # 3. the search
     c1, av1 = _asof_value(t1, asof, cls)
-    return K.asof_search(run, run_offsets.contiguous(), c1, av1, codes, rows, cls, ASOF_DIRECTIONS[direction],
+    return K.asof_search(run, run_offsets, c1, av1, codes, rows, cls, ASOF_DIRECTIONS[direction],
                          allow_exact_matches, tolerance)
 
 
@@ -445,3 +462,95 @@ def _assemble(t1: B200Table, t2: B200Table, keys: List[str], out_schema: Schema,
             lcols[i1] = torch.where(from_right, c2.to(lcols[i1].dtype), lcols[i1])
             lvalid[i1] = torch.where(from_right, v2, lvalid[i1])
     return B200DataFrame(B200Table(out_schema, lcols + rcols, lvalid + rvalid, dicts))
+
+
+RANGE_JOIN_TYPES = ["inner", "left_outer"]
+RANGE_CLOSED = {"both": K.RANGE_CLOSED_LEFT | K.RANGE_CLOSED_RIGHT, "left": K.RANGE_CLOSED_LEFT,
+                "right": K.RANGE_CLOSED_RIGHT, "neither": 0}
+_SIGN64 = -(1 << 63)
+
+
+def get_range_schemas(df1: Any, df2: Any, on: Optional[List[str]], at: str, start: str,
+                      end: str) -> Tuple[List[str], Schema]:
+    """(equality keys, output schema) of a range join.  ``on=None`` takes every common column but ``at``; an empty
+    list is one group.  ``at`` is a column of df1, ``start`` and ``end`` (possibly one column) of df2, all of one
+    type.  The output is ``df1.schema`` followed by df2's columns other than the keys (``start`` and ``end``
+    included); any other common column raises SchemaError, as ``get_asof_schemas`` does."""
+    for arg, name in (("at", at), ("start", start), ("end", end)):
+        if not isinstance(name, str):
+            raise ValueError(f"{arg} must be one column name, got {name!r}")
+    if on is None:
+        other = set(df2.columns)
+        on = [c for c in df1.columns if c in other and c != at]
+    on = list(on)
+    if len(on) != len(set(on)):
+        raise AssertionError(f"{on} has duplication")
+    for name in (at, start, end):
+        if name in on:
+            raise ValueError(f"the range column {name} is also an equality key {on}")
+    for k in on:
+        if k not in df1.schema or k not in df2.schema:
+            raise SchemaError(f"{k} is not in both {df1.schema} and {df2.schema}")
+        if df1.schema[k].type != df2.schema[k].type:
+            raise SchemaError(f"join key {k} has different types: {df1.schema[k].type} vs {df2.schema[k].type}")
+    if at not in df1.schema:
+        raise SchemaError(f"{at} is not in {df1.schema}")
+    for name in (start, end):
+        if name not in df2.schema:
+            raise SchemaError(f"{name} is not in {df2.schema}")
+        if df2.schema[name].type != df1.schema[at].type:
+            raise SchemaError(f"range columns have different types: {at} is {df1.schema[at].type}, {name} is "
+                              f"{df2.schema[name].type}")
+    names2 = [n for n in df2.schema.names if n not in on]
+    common = [n for n in names2 if n in df1.schema]
+    if common:
+        raise SchemaError(f"{common} are common columns of {df1.schema} and {df2.schema} but not join keys")
+    return on, Schema(df1.schema, df2.schema.extract(names2))
+
+
+def device_range_join(df1: B200DataFrame, df2: B200DataFrame, on: Optional[List[str]], at: str, start: str,
+                      end: str, how: str = "inner", closed: str = "both") -> B200DataFrame:
+    """Range join (DESIGN §7r): every left row, in input order, with every right row of equal key whose interval
+    [start, end] (sides open or closed by ``closed``: both, left, right, neither) holds its ``at`` value, in
+    ascending (start, right input order)."""
+    how = how.lower() if isinstance(how, str) else how
+    if how not in RANGE_JOIN_TYPES:
+        raise ValueError(f"a range join is {' or '.join(RANGE_JOIN_TYPES)}, got {how!r}")
+    if not isinstance(closed, str) or closed not in RANGE_CLOSED:
+        raise ValueError(f"closed must be one of {list(RANGE_CLOSED)}, got {closed!r}")
+    keys, out_schema = get_range_schemas(df1, df2, on, at, start, end)
+    t1, t2 = df1.native, df2.native
+    is_string = at in t1.dictionaries or start in t2.dictionaries or end in t2.dictionaries
+    cls = asof_key_class(at, t1.schema[at].type, is_string, "a range column")
+    li, ri = range_pairs(t1, t2, keys, at, start, end, cls, RANGE_CLOSED[closed], how == "left_outer")
+    return _assemble(t1, t2, keys, out_schema, li, ri, how)
+
+
+def range_pairs(t1: B200Table, t2: B200Table, keys: List[str], at: str, start: str, end: str, cls: int, closed: int,
+                outer: bool) -> Tuple[torch.Tensor, torch.Tensor]:
+    """The (left row, right row) pairs of a range join in output order; right row -1 for an unmatched left row of
+    an outer join."""
+    dev = t1.device
+    n1 = t1.num_rows
+    if n1 == 0:
+        return torch.empty(0, dtype=torch.int64, device=dev), torch.empty(0, dtype=torch.int64, device=dev)
+    # 1-2. the intervals that can match (valid bounds, start <= end) sorted by (keys..., start), and the runs
+    s2 = _asof_value(t2, start, cls)
+    e2 = s2 if end == start else _asof_value(t2, end, cls)
+    ordered = ((s2[0] ^ _SIGN64) <= (e2[0] ^ _SIGN64)).to(torch.uint8)
+    runs = sorted_runs(t1, t2, keys, start, [s2, e2], ordered)
+    if runs is None:
+        if outer:
+            return torch.arange(n1, dtype=torch.int64, device=dev), torch.full((n1,), -1, dtype=torch.int64, device=dev)
+        return torch.empty(0, dtype=torch.int64, device=dev), torch.empty(0, dtype=torch.int64, device=dev)
+    rows, (starts, ends), run, run_offsets = runs
+    # 3. the MAX tree over the end codes, sign-flipped so that the signed MAX orders them
+    ends = (ends ^ _SIGN64).contiguous()
+    tree = K.window_tree(K.AGG_MAX_I64, ends)
+    # 4-6. count, offsets, emit
+    c1, av1 = _asof_value(t1, at, cls)
+    counts = K.range_join_count(run, run_offsets, c1, av1, starts, ends, tree, closed, outer)
+    offsets, total = K.exclusive_scan(counts)
+    return K.range_join_emit(run, run_offsets, c1, av1, starts, ends, tree, rows, closed, outer, counts, offsets,
+                             total)
+

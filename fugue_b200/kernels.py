@@ -913,6 +913,74 @@ def asof_search(run: torch.Tensor, run_offsets: torch.Tensor, left_codes: torch.
     return out
 
 
+RANGE_CLOSED_LEFT, RANGE_CLOSED_RIGHT = 1, 2   # FB_RANGE_CLOSED_*
+
+
+def window_tree(op: int, values: torch.Tensor) -> torch.Tensor:
+    """``fb_window_tree``: the levels >= 1 of the aligned block tree of ``op`` (an ``AGG_*`` op) over one column of
+    8-byte values without NULLs, as the uint8 scratch that holds them (layout: include/fugue_b200.h)."""
+    lib = _lib.load()
+    dev, n = _check_cols([values])
+    assert values.element_size() == 8
+    nb = int(lib.fb_window_bounded_scratch_bytes(n, 1))
+    tree = torch.empty(max(nb, 8), dtype=torch.uint8, device=dev)
+    _lib.check(lib.fb_window_tree(dev.index, _stream_ptr(dev), n, 1, _lib.i32_array([op]),
+                                  _ptrs([values]), _ptrs([None]), tree.data_ptr(), tree.numel()))
+    return tree
+
+
+def _range_join_args(run: torch.Tensor, run_offsets: torch.Tensor, left_codes: torch.Tensor,
+                     left_valid: Optional[torch.Tensor], start_codes: torch.Tensor, end_keys: torch.Tensor,
+                     tree: torch.Tensor) -> List[Any]:
+    dev = run.device
+    for t in (run, run_offsets, end_keys):
+        assert t.dtype == torch.int64 and t.is_cuda and t.is_contiguous()
+    for t in (left_codes, start_codes):
+        assert t.element_size() == 8 and t.device == dev and t.is_contiguous()
+    assert left_codes.shape[0] == run.shape[0] and start_codes.shape[0] == end_keys.shape[0]
+    if left_valid is not None:
+        assert left_valid.dtype == torch.uint8 and left_valid.device == dev and left_valid.is_contiguous()
+    assert tree.dtype == torch.uint8 and tree.device == dev
+    return [dev.index, _stream_ptr(dev), int(run.shape[0]), run.data_ptr(), run_offsets.data_ptr(),
+            left_codes.data_ptr(), 0 if left_valid is None else left_valid.data_ptr(), int(start_codes.shape[0]),
+            start_codes.data_ptr(), end_keys.data_ptr(), tree.data_ptr(), tree.numel()]
+
+
+def range_join_count(run: torch.Tensor, run_offsets: torch.Tensor, left_codes: torch.Tensor,
+                     left_valid: Optional[torch.Tensor], start_codes: torch.Tensor, end_keys: torch.Tensor,
+                     tree: torch.Tensor, closed: int, outer: bool) -> torch.Tensor:
+    """``fb_range_join_count``: per left row the number of intervals of its run ``run[i]`` (-1: none) that hold its
+    value (1 for none when ``outer``).  In sorted right order: ``start_codes`` (order codes, ascending within each
+    run: only argsort results may be passed), ``end_keys`` (end codes ^ 2^63 as int64) and ``tree``
+    (``window_tree(AGG_MAX_I64, end_keys)``); ``closed`` is ``RANGE_CLOSED_*`` flags."""
+    lib = _lib.load()
+    args = _range_join_args(run, run_offsets, left_codes, left_valid, start_codes, end_keys, tree)
+    counts = torch.empty(int(run.shape[0]), dtype=torch.int64, device=run.device)
+    _lib.check(lib.fb_range_join_count(*args, closed, 1 if outer else 0, counts.data_ptr()))
+    return counts
+
+
+def range_join_emit(run: torch.Tensor, run_offsets: torch.Tensor, left_codes: torch.Tensor,
+                    left_valid: Optional[torch.Tensor], start_codes: torch.Tensor, end_keys: torch.Tensor,
+                    tree: torch.Tensor, right_rows: torch.Tensor, closed: int, outer: bool, counts: torch.Tensor,
+                    offsets: torch.Tensor, total: int) -> Tuple[torch.Tensor, torch.Tensor]:
+    """``fb_range_join_emit``: the ``total`` (left row, right row) pairs counted by :func:`range_join_count`, each
+    left row's at ``offsets[i]`` (its exclusive scan) in ascending (start, right row) order; ``right_rows`` maps
+    sorted positions to right rows, and -1 stands for the unmatched row of an outer join."""
+    lib = _lib.load()
+    args = _range_join_args(run, run_offsets, left_codes, left_valid, start_codes, end_keys, tree)
+    for t in (right_rows, counts, offsets):
+        assert t.dtype == torch.int64 and t.device == run.device and t.is_contiguous()
+    assert right_rows.shape[0] == start_codes.shape[0] and counts.shape[0] == offsets.shape[0] == run.shape[0]
+    li = torch.empty(total, dtype=torch.int64, device=run.device)
+    ri = torch.empty(total, dtype=torch.int64, device=run.device)
+    if total == 0:
+        return li, ri
+    _lib.check(lib.fb_range_join_emit(*args, right_rows.data_ptr(), closed, 1 if outer else 0, counts.data_ptr(),
+                                      offsets.data_ptr(), li.data_ptr(), ri.data_ptr()))
+    return li, ri
+
+
 def row_hash64(keys: Sequence[torch.Tensor], valid: Optional[Sequence[Optional[torch.Tensor]]] = None
                ) -> torch.Tensor:
     """64-bit hash of each row's key tuple (same function as the partitioner, before ``% num``)."""

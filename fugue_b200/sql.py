@@ -35,6 +35,9 @@ Window functions (DESIGN §7p):
              [USING (k, ...) | ON a.k = b.k [AND ...]]                        -> hash join kernels
     SELECT * FROM a ASOF [LEFT [OUTER]] JOIN b
              USING (k, ..., t) | ON a.k = b.k [AND ...] AND a.t >= | > | <= | < b.t  -> as-of join (DESIGN §7q)
+    SELECT * FROM a [INNER | LEFT [OUTER]] JOIN b
+             ON [a.k = b.k AND ...] a.t BETWEEN b.s AND b.e                  -> range join (DESIGN §7r)
+             ON [a.k = b.k AND ...] b.s <= | < a.t AND a.t <= | < b.e        (either operand first, any order)
 
 Expressions: + - * / %, comparisons (= == != <> < <= > >=), AND / OR / NOT, IS [NOT] NULL, [NOT] IN (...),
 [NOT] BETWEEN, x [NOT] LIKE 'pattern' [ESCAPE 'c'], CAST(x AS type), CASE [x] WHEN .. THEN .. [ELSE ..] END,
@@ -48,6 +51,7 @@ REGEXP_REPLACE; their string literals are read as written (a backslash is a back
 Anything else raises NotImplementedError (there is no host SQL fallback in this package).
 """
 import datetime
+import itertools
 import re
 from typing import Any, Dict, List, Tuple
 
@@ -267,7 +271,9 @@ class B200SQLEngine:
                      rf"JOIN\s+(`?{_IDENT}`?)(?:\s+AS)?(?:\s+({_IDENT}))?(?:\s+(USING|ON)\s+(.+))?$", rest)
         if m is not None:
             return self._asof_join(m, tables, sql)
-        m = re.match(rf"(?is)^(`?{_IDENT}`?)(?:\s+AS)?(?:\s+({_IDENT}))?\s+"
+        # a join keyword after the left table is not its alias: "a LEFT JOIN b" is a left outer join
+        m = re.match(rf"(?is)^(`?{_IDENT}`?)(?:\s+AS)?(?:\s+(?!(?:INNER|CROSS|LEFT|RIGHT|FULL|SEMI|ANTI|JOIN)\b)"
+                     rf"({_IDENT}))?\s+"
                      r"((?:INNER|CROSS|LEFT SEMI|LEFT ANTI|SEMI|ANTI|LEFT OUTER|RIGHT OUTER|FULL OUTER|"
                      r"LEFT|RIGHT|FULL)\s+)?JOIN\s+"
                      rf"(`?{_IDENT}`?)(?:\s+AS)?(?:\s+({_IDENT}))?(?:\s+(USING|ON)\s+(.+))?$", rest)
@@ -284,6 +290,15 @@ class B200SQLEngine:
             if m.group(6).upper() == "USING":
                 on = [c.strip().strip("`") for c in cond.strip("() ").split(",")]
             else:
+                left_names = {m.group(1).strip("`").lower()} | ({m.group(2).lower()} if m.group(2) else set())
+                right_names = {m.group(4).strip("`").lower()} | ({m.group(5).lower()} if m.group(5) else set())
+                rng = _range_condition(cond, left_names, right_names)
+                if rng is not None:
+                    if how not in ("inner", "left_outer"):
+                        raise NotImplementedError(f"a range join is INNER or LEFT [OUTER], not {kind}: {sql}")
+                    on, at, start, end, closed = rng
+                    return self._engine.range_join(t1, t2, on=on, at=at, start=start, end=end, how=how,
+                                                   closed=closed)
                 on = []
                 for part in re.split(r"(?i)\s+AND\s+", cond):
                     mm = re.match(rf"^\(?\s*(?:{_IDENT}\.)?({_IDENT})\s*=\s*(?:{_IDENT}\.)?({_IDENT})\s*\)?$", part.strip())
@@ -321,19 +336,10 @@ class B200SQLEngine:
             if mm.group(3) == "=":
                 on.append(mm.group(2))
                 continue
-            # a qualifier names a table or its alias; one that names neither (a dataframe handed to raw_sql has a
-            # generated name) is the table the other operand does not name, and if neither operand names one the
-            # operands are in FROM order: left table first
             quals = [(q or "").lower() for q in (mm.group(1), mm.group(4))]
             if "" in quals:
                 raise NotImplementedError(f"the as-of inequality must qualify both columns: {sql}")
-            sides = ["left" if q in left_names - right_names else "right" if q in right_names - left_names else None
-                     for q in quals]
-            if sides == [None, None] and quals[0] != quals[1]:
-                sides = ["left", "right"]
-            elif None in sides:
-                known = sides[1 - sides.index(None)]
-                sides = [s or ("right" if known == "left" else "left") for s in sides]
+            sides = _operand_sides(quals, left_names, right_names)
             if sides[0] == sides[1]:
                 raise NotImplementedError(f"the as-of inequality must name each table once: {sql}")
             op = mm.group(3)
@@ -346,6 +352,81 @@ class B200SQLEngine:
         return self._engine.asof_join(t1, t2, on=on, asof=asof, how=how,
                                       direction="backward" if op in (">=", ">") else "forward",
                                       allow_exact_matches=op in (">=", "<="))
+
+
+def _operand_sides(quals: List[str], left_names: Any, right_names: Any) -> List[Any]:
+    """"left" / "right" for the two qualifiers of a comparison's operands.  A qualifier names a table or its alias;
+    one that names neither (a dataframe handed to raw_sql has a generated name) is the table the other operand
+    does not name, and if neither operand names one the operands are in FROM order: left table first.  Two equal
+    qualifiers that name no table stay [None, None]."""
+    sides = ["left" if q in left_names - right_names else "right" if q in right_names - left_names else None
+             for q in quals]
+    if sides == [None, None] and quals[0] != quals[1]:
+        sides = ["left", "right"]
+    elif None in sides and sides != [None, None]:
+        known = sides[1 - sides.index(None)]
+        sides = [s or ("right" if known == "left" else "left") for s in sides]
+    return sides
+
+
+_COL = rf"(?:({_IDENT})\.)?({_IDENT})"
+_RANGE_FLIP = {">=": "<=", "<=": ">=", ">": "<", "<": ">"}
+
+
+def _range_condition(cond: str, left_names: Any, right_names: Any) -> Any:
+    """(on, at, start, end, closed) of an ON condition that is equalities on equally named columns plus exactly
+    one range form on qualified columns: ``a.t BETWEEN b.s AND b.e``, or one lower and one upper bound of the same
+    left column by right columns (``b.s <= a.t AND a.t < b.e``, either operand first, in any order).  None for
+    any other condition, which the equi-join parser then rejects.  Qualifiers that name no table (raw_sql's
+    generated names) take the sides that make the condition a range form, the first of them on the left when
+    both ways do."""
+    found = list(re.finditer(rf"(?is)(\bNOT\s+)?\b{_COL}\s+BETWEEN\s+{_COL}\s+AND\s+{_COL}\b", cond))
+    cmps: List[Tuple[str, str, str, str, str]] = []  # (qualifier, column, op, qualifier, column)
+    if found:
+        b = found[0]
+        if len(found) > 1 or b.group(1) or None in (b.group(2), b.group(4), b.group(6)):
+            return None
+        cmps += [(b.group(2), b.group(3), ">=", b.group(4), b.group(5)),
+                 (b.group(2), b.group(3), "<=", b.group(6), b.group(7))]
+        cond = cond[:b.start()] + "\x00" + cond[b.end():]
+    on: List[str] = []
+    for part in re.split(r"(?i)\s+AND\s+", cond.strip()):
+        part = part.strip()
+        if re.match(r"^\(?\s*\x00\s*\)?$", part):
+            continue
+        mm = re.match(rf"^\(?\s*{_COL}\s*(>=|<=|=|>|<)\s*{_COL}\s*\)?$", part)
+        if mm is None:
+            return None
+        if mm.group(3) == "=":
+            if mm.group(2) != mm.group(5):
+                return None
+            on.append(mm.group(2))
+        elif mm.group(1) is None or mm.group(4) is None:
+            return None
+        else:
+            cmps.append(mm.groups())  # type: ignore[arg-type]
+    if len(cmps) != 2:
+        return None
+    known = {q: "left" for q in left_names - right_names}
+    known.update({q: "right" for q in right_names - left_names})
+    unknown = list(dict.fromkeys(q.lower() for c in cmps for q in (c[0], c[3]) if q.lower() not in known))
+    for sides in itertools.product(("left", "right"), repeat=len(unknown)):
+        side = dict(known, **dict(zip(unknown, sides)))
+        bounds = {}  # "lower" / "upper" -> (left column, right column, inclusive)
+        for qa, ca, op, qb, cb in cmps:
+            sa, sb = side[qa.lower()], side[qb.lower()]
+            if sa == sb:
+                break
+            if sa == "right":  # b.s <= a.t is a.t >= b.s
+                ca, op, cb = cb, _RANGE_FLIP[op], ca
+            bounds.setdefault("lower" if op in (">=", ">") else "upper", []).append((ca, cb, op in (">=", "<=")))
+        else:
+            lower, upper = bounds.get("lower", []), bounds.get("upper", [])
+            if len(lower) == 1 and len(upper) == 1 and lower[0][0] == upper[0][0]:
+                closed = {(True, True): "both", (True, False): "left", (False, True): "right",
+                          (False, False): "neither"}[(lower[0][2], upper[0][2])]
+                return on, lower[0][0], lower[0][1], upper[0][1], closed
+    return None
 
 
 def _top_level_from(sql: str) -> Any:

@@ -387,6 +387,14 @@ size_t fb_window_bounded_scratch_bytes(int64_t nrows, int ncols);
 int fb_window_bounded(int dev, void* stream, int64_t nrows, const int64_t* d_lo, const int64_t* d_hi, int ncols,
                       const int32_t* ops, const void* const* vals, const uint8_t* const* valid, void* const* out_vals,
                       int64_t* const* out_count, void* scratch, size_t scratch_bytes);
+/* fb_window_tree builds only the tree of fb_window_bounded, for kernels that walk it (fb_range_join_count /
+ * _emit).  Scratch (fb_window_bounded_scratch_bytes(nrows, ncols) bytes) receives, with T the node count of
+ * levels >= 1 (the sum of nrows >> l for l >= 1) and off[l] the sum of nrows >> k for 1 <= k < l: the 8-byte
+ * value of column c's node m of level l at word c T + off[l] + m, then its int64 count at word ncols T +
+ * c T + off[l] + m.  Node (l, m) covers rows [m 2^l, (m + 1) 2^l) and exists for m < nrows >> l; level 0 is
+ * the input itself.  Same ops, validity rules and fixed combination order as fb_window_bounded. */
+int fb_window_tree(int dev, void* stream, int64_t nrows, int ncols, const int32_t* ops, const void* const* vals,
+                   const uint8_t* const* valid, void* scratch, size_t scratch_bytes);
 
 /* ---------------------------------------------------------------------------
  * K10 exact order statistics per segment: PERCENTILE_CONT / PERCENTILE_DISC / MEDIAN of one column over the
@@ -500,6 +508,37 @@ int fb_asof_search(int dev, void* stream, int64_t nleft, const int64_t* d_run, c
                    const uint64_t* d_left_codes, const uint8_t* d_left_valid, const uint64_t* d_right_codes,
                    const int64_t* d_right_rows, int key_class, int direction, int allow_exact_matches,
                    int has_tolerance, uint64_t tolerance, int64_t* d_out);
+
+/* Range join (B200ExecutionEngine.range_join): every left row with every interval of its run that holds its
+ * value.  The right side holds only intervals that can match (valid key, start and end, start <= end), sorted by
+ * (key, start) stably; run r is rows [d_run_offsets[r], d_run_offsets[r + 1]) of one key.  d_start_codes holds
+ * their starts as unsigned 64-bit order codes (sort.py _unsigned_order_key), d_end_keys their end codes with the
+ * sign bit flipped (code ^ 2^63, read as int64), and d_tree (tree_bytes >= fb_window_bounded_scratch_bytes(nright,
+ * 1)) the levels of fb_window_tree with op FB_AGG_MAX_I64 over d_end_keys.  PRECONDITION: the start codes ascend
+ * within every run (the host passes argsort_rows results) and the tree was built over these end keys; neither is
+ * checked.  One thread per left row i: d_run[i] is its run (-1: none), d_left_codes[i] its value's code of the same
+ * class, d_left_valid[i] == 0 (NULL allowed) a NULL value, which matches nothing.  Right row j matches when
+ * start_j <= x (< x without FB_RANGE_CLOSED_LEFT in `closed`) and x <= end_j (< end_j without
+ * FB_RANGE_CLOSED_RIGHT), compared as unsigned codes.  The rows whose start passes are a prefix [s, p) of the run
+ * (one binary search); the hits among them are found from the right, each by a walk over the MAX tree to the
+ * next row to the left whose end passes: O(log run + (1 + matches) log run) per left row, whatever the nesting.
+ *   fb_range_join_count  d_counts[i] = the matches of row i; outer != 0: an unmatched row counts 1
+ *   fb_range_join_emit   with d_offsets the exclusive scan of those counts (fb_exclusive_scan_i64): the pairs
+ *                        (d_out_left, d_out_right)[d_offsets[i] + k] = (i, d_right_rows[j_k]) for the row's
+ *                        matches j_0 < j_1 < ... in sorted position, i.e. ascending (start, right row); an
+ *                        unmatched row of an outer join gets (i, -1) */
+#define FB_RANGE_CLOSED_LEFT 1
+#define FB_RANGE_CLOSED_RIGHT 2
+int fb_range_join_count(int dev, void* stream, int64_t nleft, const int64_t* d_run, const int64_t* d_run_offsets,
+                        const uint64_t* d_left_codes, const uint8_t* d_left_valid, int64_t nright,
+                        const uint64_t* d_start_codes, const int64_t* d_end_keys, const void* d_tree,
+                        size_t tree_bytes, int closed, int outer, int64_t* d_counts);
+int fb_range_join_emit(int dev, void* stream, int64_t nleft, const int64_t* d_run, const int64_t* d_run_offsets,
+                       const uint64_t* d_left_codes, const uint8_t* d_left_valid, int64_t nright,
+                       const uint64_t* d_start_codes, const int64_t* d_end_keys, const void* d_tree,
+                       size_t tree_bytes, const int64_t* d_right_rows, int closed, int outer,
+                       const int64_t* d_counts, const int64_t* d_offsets, int64_t* d_out_left,
+                       int64_t* d_out_right);
 
 /* K7 fast path: inner / left-outer join on one 8-byte key with 4-byte slots (build row + 1; keys are
  * compared through the build key column) and a fused probe -> output assembly.

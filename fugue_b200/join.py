@@ -54,6 +54,10 @@ def get_join_schemas(df1: Any, df2: Any, how: str, on: Optional[List[str]]) -> T
             raise SchemaError(f"invalid cross join, two dataframes have common columns {cs}")
     elif len(on) == 0:
         raise SchemaError("join on columns must be specified")
+    else:  # the output holds one column of each name: a common column must be a key
+        cs = [c for c in df1.schema.names if c in schema2.names and c not in on]
+        if len(cs) > 0:
+            raise SchemaError(f"{cs} are in both dataframes but not join keys {on}")
     return cm, df1.schema.union(schema2)
 
 

@@ -31,8 +31,15 @@ Window functions (DESIGN §7p):
     EXCLUDE, named windows (WINDOW w AS, OVER w) and NULLS FIRST raise NotImplementedError, and so do
     ROW_NUMBER / RANK / DENSE_RANK / LAG / LEAD without OVER; a window in WHERE, GROUP BY, HAVING or in another
     window's arguments raises ValueError.
-    SELECT * FROM a [INNER|LEFT|RIGHT|FULL [OUTER]|LEFT SEMI|LEFT ANTI|CROSS] JOIN b
-             [USING (k, ...) | ON a.k = b.k [AND ...]]                        -> hash join kernels
+    SELECT * FROM a [[AS] x] [INNER | LEFT [OUTER] | RIGHT [OUTER] | FULL [OUTER] | [LEFT] SEMI | [LEFT] ANTI] JOIN
+             b [[AS] y] USING (k, ...) | ON x.k = y.k [AND ...]              -> hash join kernels
+    SELECT * FROM a CROSS JOIN b  |  a NATURAL [<kind above>] JOIN b        -> cross product / common columns
+
+    Each equality names one column of each side (by table or alias; ``k = k`` unqualified); a repeated one counts
+    once.  A table ``fa.raw_sql`` named (``_0``, ``_1``) and gave no alias may be named by any qualifier.  A join
+    without ON / USING (other than CROSS and NATURAL), CROSS or NATURAL with one, ``a OUTER JOIN b``, ``ON a.k = a.k``
+    and qualifiers that name no table raise NotImplementedError.  (In the range and as-of conditions below a
+    qualifier that names no table takes the side the condition needs, as DESIGN §7q / §7r describe.)
     SELECT * FROM a ASOF [LEFT [OUTER]] JOIN b
              USING (k, ..., t) | ON a.k = b.k [AND ...] AND a.t >= | > | <= | < b.t  -> as-of join (DESIGN §7q)
     SELECT * FROM a [INNER | LEFT [OUTER]] JOIN b
@@ -267,44 +274,50 @@ class B200SQLEngine:
     def _join(self, items: str, rest: str, tables: Dict[str, DataFrame], sql: str) -> DataFrame:
         if items.strip() != "*":
             raise NotImplementedError(f"only SELECT * is supported for joins: {sql}")
-        m = re.match(rf"(?is)^(`?{_IDENT}`?)(?:\s+AS)?(?:\s+({_IDENT}))?\s+ASOF\s+(?:(INNER|LEFT|RIGHT|FULL)(?:\s+OUTER)?\s+)?"
-                     rf"JOIN\s+(`?{_IDENT}`?)(?:\s+AS)?(?:\s+({_IDENT}))?(?:\s+(USING|ON)\s+(.+))?$", rest)
+        m = re.match(rf"(?is)^{_TABLE_AS}\s+ASOF\s+(?:(INNER|LEFT|RIGHT|FULL)(?:\s+OUTER)?\s+)?"
+                     rf"JOIN\s+{_TABLE_AS}(?:\s+(USING|ON)\s+(.+))?$", rest)
         if m is not None:
             return self._asof_join(m, tables, sql)
-        # a join keyword after the left table is not its alias: "a LEFT JOIN b" is a left outer join
-        m = re.match(rf"(?is)^(`?{_IDENT}`?)(?:\s+AS)?(?:\s+(?!(?:INNER|CROSS|LEFT|RIGHT|FULL|SEMI|ANTI|JOIN)\b)"
-                     rf"({_IDENT}))?\s+"
-                     r"((?:INNER|CROSS|LEFT SEMI|LEFT ANTI|SEMI|ANTI|LEFT OUTER|RIGHT OUTER|FULL OUTER|"
-                     r"LEFT|RIGHT|FULL)\s+)?JOIN\s+"
-                     rf"(`?{_IDENT}`?)(?:\s+AS)?(?:\s+({_IDENT}))?(?:\s+(USING|ON)\s+(.+))?$", rest)
+        # a join keyword after a table is not its alias: "a LEFT JOIN b" is a left outer join, "a OUTER JOIN b" no join
+        m = re.match(rf"(?is)^{_TABLE_AS}\s+(NATURAL\s+)?((?:INNER|CROSS|LEFT\s+SEMI|LEFT\s+ANTI|SEMI|ANTI|"
+                     rf"(?:LEFT|RIGHT|FULL)(?:\s+OUTER)?)\s+)?JOIN\s+{_TABLE_AS}(?:\s+(USING|ON)\s+(.+))?$", rest)
         if m is None:
             raise NotImplementedError(f"unsupported join SQL: {sql}")
-        t1, t2 = self._table(m.group(1), tables, sql), self._table(m.group(4), tables, sql)
-        kind = (m.group(3) or "INNER").strip().upper()
+        t1, t2 = self._table(m.group(1), tables, sql), self._table(m.group(5), tables, sql)
+        kind = re.sub(r"\s+", " ", (m.group(4) or "INNER").strip().upper())
         how = {"INNER": "inner", "CROSS": "cross", "LEFT SEMI": "semi", "SEMI": "semi", "LEFT ANTI": "anti",
                "ANTI": "anti", "LEFT OUTER": "left_outer", "LEFT": "left_outer", "RIGHT OUTER": "right_outer",
                "RIGHT": "right_outer", "FULL OUTER": "full_outer", "FULL": "full_outer"}[kind]
-        on = None
-        if m.group(6):
-            cond = m.group(7).strip()
-            if m.group(6).upper() == "USING":
-                on = [c.strip().strip("`") for c in cond.strip("() ").split(",")]
-            else:
-                left_names = {m.group(1).strip("`").lower()} | ({m.group(2).lower()} if m.group(2) else set())
-                right_names = {m.group(4).strip("`").lower()} | ({m.group(5).lower()} if m.group(5) else set())
-                rng = _range_condition(cond, left_names, right_names)
-                if rng is not None:
-                    if how not in ("inner", "left_outer"):
-                        raise NotImplementedError(f"a range join is INNER or LEFT [OUTER], not {kind}: {sql}")
-                    on, at, start, end, closed = rng
-                    return self._engine.range_join(t1, t2, on=on, at=at, start=start, end=end, how=how,
-                                                   closed=closed)
-                on = []
-                for part in re.split(r"(?i)\s+AND\s+", cond):
-                    mm = re.match(rf"^\(?\s*(?:{_IDENT}\.)?({_IDENT})\s*=\s*(?:{_IDENT}\.)?({_IDENT})\s*\)?$", part.strip())
-                    if mm is None or mm.group(1) != mm.group(2):
-                        raise NotImplementedError(f"only equi-joins on equally named columns: {sql}")
-                    on.append(mm.group(1))
+        if m.group(3):  # NATURAL: equality on every column the two tables share
+            if how == "cross" or m.group(7):
+                raise NotImplementedError(f"NATURAL {kind} JOIN takes no ON or USING and is not CROSS: {sql}")
+            return self._engine.join(t1, t2, how=how, on=None)
+        if how == "cross":
+            if m.group(7):
+                raise NotImplementedError(f"CROSS JOIN takes no ON or USING (write INNER JOIN): {sql}")
+            return self._engine.join(t1, t2, how=how, on=None)
+        if not m.group(7):
+            raise NotImplementedError(f"{kind} JOIN needs ON or USING (or write NATURAL JOIN / CROSS JOIN): {sql}")
+        cond = m.group(8).strip()
+        if m.group(7).upper() == "USING":
+            on = list(dict.fromkeys(c.strip().strip("`") for c in cond.strip("() ").split(",")))
+            return self._engine.join(t1, t2, how=how, on=on)
+        sides = _from_sides(m.group(1), m.group(2), m.group(5), m.group(6))
+        rng = _range_condition(cond, sides[0], sides[1])
+        if rng is not None:
+            if how not in ("inner", "left_outer"):
+                raise NotImplementedError(f"a range join is INNER or LEFT [OUTER], not {kind}: {sql}")
+            on, at, start, end, closed = rng
+            return self._engine.range_join(t1, t2, on=on, at=at, start=start, end=end, how=how, closed=closed)
+        on = []
+        for part in re.split(r"(?i)\s+AND\s+", cond.strip()):
+            mm = re.match(rf"^\(?\s*{_QCOL}\s*=\s*{_QCOL}\s*\)?$", part.strip())
+            if mm is None or mm.group(2) != mm.group(4):
+                raise NotImplementedError(f"only equi-joins on equally named columns: {sql}")
+            if not _equality_sides(mm.group(1), mm.group(3), *sides):
+                raise NotImplementedError(f"{part.strip()} does not name one column of each table: {sql}")
+            if mm.group(2) not in on:
+                on.append(mm.group(2))
         return self._engine.join(t1, t2, how=how, on=on)
 
     def _asof_join(self, m: Any, tables: Dict[str, DataFrame], sql: str) -> DataFrame:
@@ -324,8 +337,7 @@ class B200SQLEngine:
             names = [c.strip().strip("`") for c in cond.strip("() ").split(",")]
             return self._engine.asof_join(t1, t2, on=names[:-1], asof=names[-1], how=how, direction="backward",
                                           allow_exact_matches=True)
-        left_names = {m.group(1).strip("`").lower()} | ({m.group(2).lower()} if m.group(2) else set())
-        right_names = {m.group(4).strip("`").lower()} | ({m.group(5).lower()} if m.group(5) else set())
+        left_names, right_names, _ = _from_sides(m.group(1), m.group(2), m.group(4), m.group(5))
         on: List[str] = []
         ineq: List[Tuple[str, str]] = []
         for part in re.split(r"(?i)\s+AND\s+", cond):
@@ -334,13 +346,15 @@ class B200SQLEngine:
             if mm is None or mm.group(2) != mm.group(5):
                 raise NotImplementedError(f"an as-of join compares equally named columns: {sql}")
             if mm.group(3) == "=":
+                if not _equality_sides(mm.group(1), mm.group(4), left_names, right_names, _ANY_SIDE):
+                    raise NotImplementedError(f"{part.strip()} does not name one column of each table: {sql}")
                 on.append(mm.group(2))
                 continue
             quals = [(q or "").lower() for q in (mm.group(1), mm.group(4))]
             if "" in quals:
                 raise NotImplementedError(f"the as-of inequality must qualify both columns: {sql}")
-            sides = _operand_sides(quals, left_names, right_names)
-            if sides[0] == sides[1]:
+            sides = _operand_sides(quals, left_names, right_names, _ANY_SIDE)
+            if None in sides or sides[0] == sides[1]:
                 raise NotImplementedError(f"the as-of inequality must name each table once: {sql}")
             op = mm.group(3)
             if sides[0] == "right":  # b.t <= a.t is a.t >= b.t
@@ -354,19 +368,52 @@ class B200SQLEngine:
                                       allow_exact_matches=op in (">=", "<="))
 
 
-def _operand_sides(quals: List[str], left_names: Any, right_names: Any) -> List[Any]:
-    """"left" / "right" for the two qualifiers of a comparison's operands.  A qualifier names a table or its alias;
-    one that names neither (a dataframe handed to raw_sql has a generated name) is the table the other operand
-    does not name, and if neither operand names one the operands are in FROM order: left table first.  Two equal
-    qualifiers that name no table stay [None, None]."""
+_JOIN_WORDS = r"(?:AS|INNER|CROSS|LEFT|RIGHT|FULL|OUTER|SEMI|ANTI|NATURAL|ASOF|JOIN|ON|USING)\b"
+_TABLE_AS = rf"(`?{_IDENT}`?)(?:\s+AS)?(?:\s+(?!{_JOIN_WORDS})(`?{_IDENT}`?))?"  # table [[AS] alias]
+_QCOL = rf"(?:`?({_IDENT})`?\.)?`?({_IDENT})`?"  # [qualifier.]column
+
+
+_ANY_SIDE = frozenset(("left", "right"))  # a qualifier that names no table may stand for either side
+
+
+def _from_sides(t1: str, a1: Any, t2: str, a2: Any) -> Tuple[Any, Any, Any]:
+    """(left names, right names, anonymous sides) of ``t1 [AS a1] JOIN t2 [AS a2]``: each side is named by its
+    table and its alias, lower-cased.  A side is anonymous when its table has a name ``fa.raw_sql`` generated
+    (``_0``, ``_1``, ...: the text never spells it) and no alias; a qualifier of an equi-join's equality that names
+    no table may stand for it.  (The range and as-of conditions let such a qualifier stand for either side.)"""
+    names, anonymous = [], set()
+    for side, t, a in (("left", t1, a1), ("right", t2, a2)):
+        t = t.strip("`")
+        names.append({t.lower()} | ({a.strip("`").lower()} if a else set()))
+        if a is None and re.fullmatch(r"_\d+", t):
+            anonymous.add(side)
+    return names[0], names[1], anonymous
+
+
+def _operand_sides(quals: List[str], left_names: Any, right_names: Any, anonymous: Any) -> List[Any]:
+    """"left" / "right" for the two qualifiers of a comparison's operands, None where a qualifier names no side.
+    A qualifier names a table or its alias.  One that names neither may stand for a side in ``anonymous`` (an
+    equi-join's: raw_sql's unaliased tables, see ``_from_sides``; ``_ANY_SIDE`` for the range and as-of
+    conditions): the side the other operand does not name, and if neither operand names one the operands are in
+    FROM order: left table first."""
     sides = ["left" if q in left_names - right_names else "right" if q in right_names - left_names else None
              for q in quals]
-    if sides == [None, None] and quals[0] != quals[1]:
+    if sides == [None, None] and quals[0] != quals[1] and set(anonymous) == {"left", "right"}:
         sides = ["left", "right"]
     elif None in sides and sides != [None, None]:
-        known = sides[1 - sides.index(None)]
-        sides = [s or ("right" if known == "left" else "left") for s in sides]
+        free = "right" if sides[1 - sides.index(None)] == "left" else "left"
+        if free in anonymous:
+            sides = [s or free for s in sides]
     return sides
+
+
+def _equality_sides(q1: Any, q2: Any, left_names: Any, right_names: Any, anonymous: Any) -> bool:
+    """Whether ``[q1.]k = [q2.]k`` compares the k of one table with the k of the other.  Unqualified, it does;
+    qualified, the qualifiers must name the two sides (``a.k = a.k`` and unknown qualifiers do not)."""
+    if q1 is None and q2 is None:
+        return True
+    return sorted(map(str, _operand_sides([(q1 or "").lower(), (q2 or "").lower()], left_names, right_names,
+                                          anonymous))) == ["left", "right"]
 
 
 _COL = rf"(?:({_IDENT})\.)?({_IDENT})"
@@ -379,7 +426,7 @@ def _range_condition(cond: str, left_names: Any, right_names: Any) -> Any:
     left column by right columns (``b.s <= a.t AND a.t < b.e``, either operand first, in any order).  None for
     any other condition, which the equi-join parser then rejects.  Qualifiers that name no table (raw_sql's
     generated names) take the sides that make the condition a range form, the first of them on the left when
-    both ways do."""
+    both ways do; an equality whose qualifiers name the same table is no range form."""
     found = list(re.finditer(rf"(?is)(\bNOT\s+)?\b{_COL}\s+BETWEEN\s+{_COL}\s+AND\s+{_COL}\b", cond))
     cmps: List[Tuple[str, str, str, str, str]] = []  # (qualifier, column, op, qualifier, column)
     if found:
@@ -398,9 +445,11 @@ def _range_condition(cond: str, left_names: Any, right_names: Any) -> Any:
         if mm is None:
             return None
         if mm.group(3) == "=":
-            if mm.group(2) != mm.group(5):
+            if mm.group(2) != mm.group(5) or not _equality_sides(mm.group(1), mm.group(4), left_names, right_names,
+                                                                  _ANY_SIDE):
                 return None
-            on.append(mm.group(2))
+            if mm.group(2) not in on:
+                on.append(mm.group(2))
         elif mm.group(1) is None or mm.group(4) is None:
             return None
         else:

@@ -196,6 +196,7 @@ def test_sql_forms(cond, direction, exact):
     "SELECT * FROM ta a ASOF JOIN tb b ON a.t >= a.t",
     "SELECT * FROM ta a ASOF JOIN tb b ON a.k = b.j AND a.t >= b.t",
     "SELECT * FROM ta a ASOF JOIN tb b",
+    "SELECT * FROM ta a ASOF JOIN tb b ON a.k = a.k AND a.t >= b.t",         # an equality within one table
 ])
 def test_sql_rejections(sql):
     from fugue_b200.sql import B200SQLEngine

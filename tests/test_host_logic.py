@@ -202,6 +202,7 @@ def test_join_schemas():
         (Exception, a, b, None, []), (ValueError, a, b, "x", []), (ValueError, a, c, "outer", ["a"]),
         (SchemaError, a, b, "CROSS", ["a"]), (SchemaError, a, c, "CROSS", ["a"]), (SchemaError, a, c, "CROSS", []),
         (SchemaError, a, b, "inner", ["a"]), (SchemaError, wide1, wide2, "inner", ["a"]),
+        (SchemaError, wide1, wide2, "inner", ["c"]), (SchemaError, wide1, wide2, "full_outer", ["b"]),  # b, c common
     ]:
         with raises(exc):
             get_join_schemas(l, r, how=how, on=on)

@@ -380,6 +380,8 @@ def test_sql_forms(cond, on, closed):
     "SELECT * FROM ta a LEFT SEMI JOIN tb b ON a.t BETWEEN b.s AND b.e",
     "SELECT * FROM ta a LEFT ANTI JOIN tb b ON a.t BETWEEN b.s AND b.e",
     "SELECT a.t FROM ta a JOIN tb b ON a.t BETWEEN b.s AND b.e",
+    "SELECT * FROM ta a JOIN tb b ON a.k = a.k AND a.t BETWEEN b.s AND b.e",  # an equality within one table
+    "SELECT * FROM ta a JOIN tb b ON b.k = b.k AND b.s <= a.t AND a.t < b.e",
 ])
 def test_sql_rejections(sql):
     from fugue_b200.sql import B200SQLEngine

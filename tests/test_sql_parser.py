@@ -1,4 +1,5 @@
 """The SELECT parser of B200SQLEngine (host logic): SQL text -> column expressions (fugue_b200.column)."""
+import pytest
 from pytest import raises
 
 from fugue_b200.sql import StructuredRawSQL, _parse_select
@@ -132,3 +133,99 @@ def test_sql_engine_hands_select_the_right_trees():
         sql.select({"t": t}, "SELECT key FROM nope")
     out = sql.select({"t": t}, "SELECT DISTINCT key k, v0 FROM t")
     assert eng.calls[-1][0].is_distinct and out.columns == ["k", "v0"]
+
+
+class _JoinRecorder:
+    """Records the join the SQL engine asks for: (method, left, right, keyword arguments)."""
+    is_distinct = False
+
+    def __init__(self):
+        self.calls = []
+
+    def to_df(self, df):
+        return df
+
+    def __getattr__(self, name):
+        if name not in ("join", "range_join", "asof_join"):
+            raise AttributeError(name)
+
+        def method(df1, df2, **kw):
+            self.calls.append((name, df1, df2, kw))
+            return df1
+
+        return method
+
+
+_TA, _TB = _FakeDF(["k", "j", "v"]), _FakeDF(["k", "j", "w"])
+
+
+def _join_call(rest, tables=None):
+    from fugue_b200.sql import B200SQLEngine
+
+    eng = _JoinRecorder()
+    B200SQLEngine(eng).select(tables or {"a": _TA, "b": _TB}, "SELECT * FROM " + rest)
+    (call,) = eng.calls
+    return call
+
+
+@pytest.mark.parametrize("rest,how,on", [
+    ("a JOIN b ON a.k = b.k", "inner", ["k"]),
+    ("a INNER JOIN b USING (k)", "inner", ["k"]),
+    ("a inner join b using (k, j)", "inner", ["k", "j"]),
+    ("a LEFT JOIN b ON a.k = b.k", "left_outer", ["k"]),
+    ("a LEFT OUTER JOIN b ON b.k = a.k", "left_outer", ["k"]),
+    ("a RIGHT JOIN b ON a.k = b.k", "right_outer", ["k"]),
+    ("a RIGHT OUTER JOIN b ON a.k = b.k", "right_outer", ["k"]),
+    ("a FULL JOIN b ON a.k = b.k", "full_outer", ["k"]),
+    ("a FULL OUTER JOIN b ON a.k = b.k AND a.j = b.j", "full_outer", ["k", "j"]),
+    ("a SEMI JOIN b ON a.k = b.k", "semi", ["k"]),
+    ("a LEFT SEMI JOIN b ON a.k = b.k", "semi", ["k"]),
+    ("a ANTI JOIN b USING (k)", "anti", ["k"]),
+    ("a LEFT ANTI JOIN b ON a.k = b.k", "anti", ["k"]),
+    ("a CROSS JOIN b", "cross", None),
+    ("a AS x JOIN b AS y ON x.k = y.k", "inner", ["k"]),
+    ("a x LEFT JOIN b y ON (y.k = x.k) AND (x.j = y.j)", "left_outer", ["k", "j"]),
+    ("a x left\n  outer join b ON (x.k = b.k AND a.j = b.j)", "left_outer", ["k", "j"]),
+    ("`a` JOIN `b` ON `a`.`k` = `b`.`k`", "inner", ["k"]),
+    ("a JOIN b ON k = k", "inner", ["k"]),
+    # the join texts that used to run another join
+    ("a LEFT JOIN b ON a.k = b.k AND a.k = b.k", "left_outer", ["k"]),     # ran with on=['k', 'k']
+    ("a LEFT JOIN b ON a.k = b.k AND b.k = a.k", "left_outer", ["k"]),
+    ("a NATURAL JOIN b", "inner", None),                                     # NATURAL was read as a's alias
+    ("a NATURAL LEFT JOIN b", "left_outer", None),
+    ("a x NATURAL FULL OUTER JOIN b", "full_outer", None),
+    # raw_sql's dataframes have generated names (_0, _1) the text cannot spell: any qualifier may stand for them
+    ("_0 JOIN _1 ON orders.k = prices.k", "inner", ["k"]),
+    ("_0 o LEFT JOIN _1 ON o.k = p.k", "left_outer", ["k"]),
+])
+def test_join_spellings(rest, how, on):
+    tables = {"_0": _TA, "_1": _TB} if rest.startswith("_0") else None
+    name, d1, d2, kw = _join_call(rest, tables)
+    assert name == "join" and d1 is _TA and d2 is _TB and kw == dict(how=how, on=on)
+
+
+@pytest.mark.parametrize("rest", [
+    "a OUTER JOIN b USING (k)",             # ran an inner join: OUTER was read as a's alias
+    "a CROSS JOIN b ON a.k = b.k",          # ran the cross product and dropped the ON
+    "a CROSS JOIN b USING (k)",
+    "a JOIN b ON a.k = a.k",                # ran an inner join on k: both operands name a
+    "a x JOIN b y ON y.k = y.k",
+    "a JOIN b ON z.k = q.k",                # ran an inner join on k: neither qualifier names a table
+    "a x JOIN b y ON a.k = q.k",
+    "a JOIN b",                             # ran a natural join; SQLite runs a cross join
+    "a LEFT JOIN b",
+    "a NATURAL JOIN b USING (k)",
+    "a NATURAL JOIN b ON a.k = b.k",
+    "a NATURAL CROSS JOIN b",
+    "a JOIN b ON a.k = b.j",
+    "a JOIN b ON a.k = b.k OR a.j = b.j",
+    "a JOIN b ON a.k < b.k",
+    "a x y JOIN b ON a.k = b.k",
+])
+def test_join_texts_that_must_not_run(rest):
+    from fugue_b200.sql import B200SQLEngine
+
+    eng = _JoinRecorder()
+    with raises(NotImplementedError):
+        B200SQLEngine(eng).select({"a": _TA, "b": _TB}, "SELECT * FROM " + rest)
+    assert eng.calls == []

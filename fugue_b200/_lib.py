@@ -143,6 +143,11 @@ SIGNATURES = {
     "fb_window_bounded": (C.c_int, [C.c_int, _vp, C.c_int64, _vp, _vp, C.c_int, _i32p, _vpp, _vpp, _vpp, _vpp, _vp,
                                     C.c_size_t]),
     "fb_window_tree": (C.c_int, [C.c_int, _vp, C.c_int64, C.c_int, _i32p, _vpp, _vpp, _vp, C.c_size_t]),
+    "fb_window_value": (C.c_int, [C.c_int, _vp, C.c_int64, C.c_int64, _vp, C.c_int64, C.c_int64, C.c_int, _vp, _vp,
+                                  C.c_int, C.POINTER(C.c_int64), _i32p, _vpp, _vpp, _vpp, _vpp]),
+    "fb_window_distribution_scratch_bytes": (C.c_size_t, [C.c_int64]),
+    "fb_window_distribution": (C.c_int, [C.c_int, _vp, C.c_int64, C.c_int64, _vp, _vp, _vp, _vp, C.c_int,
+                                         C.POINTER(C.c_int64), _vpp, _vp, C.c_size_t]),
     "fb_quantile_scratch_bytes": (C.c_size_t, [C.c_int, C.c_int64, C.c_int64]),
     "fb_segmented_quantile": (C.c_int, [C.c_int, _vp, C.c_int64, C.c_int64, _vp, _vp, _vp, C.c_int, C.c_int,
                                         C.POINTER(C.c_double), _i32p, _vp, _vpp, _vp, C.c_size_t]),

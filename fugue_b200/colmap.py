@@ -32,8 +32,8 @@ import torch
 from . import aggregates as A
 from . import kernels as K
 from .aggregates import bivariate_of
-from .column import (AGGREGATES, PERCENTILES, ColumnExpr, Kind, SelectColumns, bivariate_xy, col as _col, has_window,
-                     has_explicit_window, is_agg, is_explicit, result_type)
+from .column import (AGGREGATES, DISTRIBUTIONS, PERCENTILES, VALUE_HEADS, ColumnExpr, Kind, SelectColumns,
+                     bivariate_xy, col as _col, has_window, has_explicit_window, is_agg, is_explicit, result_type)
 from .table import B200Table, _storage_dtype, narrow, widen
 
 
@@ -185,7 +185,9 @@ def _with_windows(t: B200Table, cols: List[ColumnExpr]) -> B200Table:
     by the evaluator (K8), running / partition aggregates and ranks by the segmented scan (K9), moving
     frames (``rows``) by the frame kernel, value frames (``range``) by the bounds kernel (or the peer groups)
     and the block tree, all with the same finishers, FIRST / LAST / partition values / LAG / LEAD by row
-    gathers, percentiles by the quantile kernel (K10), one call per argument column with all its q values."""
+    gathers, percentiles by the quantile kernel (K10), one call per argument column with all its q values,
+    FIRST_VALUE / LAST_VALUE / NTH_VALUE by one ``fb_window_value`` call per frame, NTILE / PERCENT_RANK / CUME_DIST by
+    one ``fb_window_distribution`` call over the peer heads."""
     from . import expr as X
     from . import sort as S
     from .schema import Schema
@@ -243,6 +245,8 @@ def _with_windows(t: B200Table, cols: List[ColumnExpr]) -> B200Table:
     comoments: Dict[Tuple[str, str], int] = {}  # (x, y) argument columns of a pair -> its pair of the co-moments scan
     pair_sums: Dict[Tuple[str, str], Tuple[Any, Any]] = {}  # (x, y) -> the running SUM scans of x and y over the pair
     finish: List[Any] = []     # per node: (fingerprint, fn(scan results) -> (column, validity, type, dictionary))
+    values: Dict[Any, List[Any]] = {}  # frame -> (values, validity, nth) of its FIRST / LAST / NTH_VALUE nodes
+    dist: Dict[str, Any] = {"PERCENT_RANK": False, "CUME_DIST": False, "NTILE": []}  # this spec's distribution heads
 
     def scan(op: int, v: Any, m: Any, frame: Any = None) -> Tuple[Any, int]:
         cols_ = scans.setdefault(frame, [])
@@ -270,6 +274,29 @@ def _with_windows(t: B200Table, cols: List[ColumnExpr]) -> B200Table:
             else:
                 i = scan(K.AGG_SUM_I64, heads.to(torch.int64), None)
             finish.append((uid, lambda r, i=i: (r[i][0], None, pa.int64(), None)))
+            continue
+        if fn in DISTRIBUTIONS:  # one fb_window_distribution call for all of them
+            if fn == "NTILE":
+                dist["NTILE"].append(bare.kwargs["n"])
+                key: Any = ("NTILE", len(dist["NTILE"]) - 1)
+            else:
+                dist[fn] = True
+                key = (fn,)
+            finish.append((uid, lambda r, key=key: (r[("dist",) + key], None, result_type_of(key[0]), None)))
+            continue
+        if fn in VALUE_HEADS:  # one fb_window_value call per frame for all of them
+            kw = bare.kwargs
+            if "range" in kw:
+                vframe: Any = ("range",) + _range_offsets(t, kw["range"])
+            else:
+                vframe = ("rows",) + (kw["rows"] if "rows" in kw else ((None, 0) if kw.get("running") else (None, None)))
+            name = arg_name[bare.arg.fingerprint()]
+            ci = base.schema.index_of_key(name)
+            nth = kw["n"] if fn == "NTH_VALUE" else (1 if fn == "FIRST_VALUE" else K.VALUE_LAST)
+            vcols = values.setdefault(vframe, [])
+            vcols.append((base.columns[ci], base.valid[ci], nth))
+            finish.append((uid, lambda r, j=(vframe, len(vcols) - 1), tp=base.schema.types[ci],
+                           d=base.dictionaries.get(name): (*r[("value",) + j], tp, d)))
             continue
         frame = bare.kwargs.get("rows")  # ROWS BETWEEN frame[0] AND frame[1]: the moving-frame kernel
         if "range" in bare.kwargs:  # RANGE BETWEEN: ("range", key class or None, start, end), the block tree
@@ -368,6 +395,14 @@ def _with_windows(t: B200Table, cols: List[ColumnExpr]) -> B200Table:
         else:
             res = K.window_frame(off.contiguous(), n, frame[0], frame[1], spec)
         results.update(((frame, j), r) for j, r in enumerate(res))
+    for vframe, vcols in values.items():
+        how = ("bounds",) + tuple(b.contiguous() for b in range_bounds(*vframe[1:])) if vframe[0] == "range" else vframe
+        results.update((("value", vframe, j), r) for j, r in enumerate(K.window_value(off.contiguous(), n, how, vcols)))
+    if dist["PERCENT_RANK"] or dist["CUME_DIST"] or dist["NTILE"]:
+        pr, cd, nts = K.window_distribution(off.contiguous(), peer_heads().contiguous(), dist["PERCENT_RANK"],
+                                            dist["CUME_DIST"], dist["NTILE"])
+        results.update({("dist", "PERCENT_RANK"): pr, ("dist", "CUME_DIST"): cd})
+        results.update((("dist", "NTILE", j), x) for j, x in enumerate(nts))
     for name, qs in quantiles.items():
         results[("quantile", name)] = K.segmented_quantile(off.contiguous(), *quantile_input(base, name), qs)
 
@@ -399,6 +434,11 @@ def _with_windows(t: B200Table, cols: List[ColumnExpr]) -> B200Table:
     out = _WindowTable(Schema([pa.field(a, b) for a, b in zip(names, types)]), columns, valid, dicts)
     out.window_names = window_names
     return out
+
+
+def result_type_of(fn: str) -> pa.DataType:
+    """The result type of a distribution head: NTILE is int64, PERCENT_RANK and CUME_DIST float64."""
+    return pa.int64() if fn == "NTILE" else pa.float64()
 
 
 def evaluate_windows(t: B200Table, exprs: List[ColumnExpr]) -> _WindowTable:

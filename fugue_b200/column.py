@@ -21,7 +21,9 @@ from an expression is a function of ``(kind, head, args)``:
     WINDOW    head in the AGG functions (their args, kwargs ``running``, ``rows`` or ``range``; a percentile keeps
               its ``q`` and covers the whole partition; a variance, a shape statistic or a two-argument aggregate takes ``running``
               only), ``ROW_NUMBER RANK
-              DENSE_RANK`` (no arg) or ``LAG LEAD`` (one arg, kwargs ``n`` and ``default``): evaluated over the logical
+              DENSE_RANK PERCENT_RANK CUME_DIST`` (no arg), ``NTILE`` (no arg, kwarg ``n``), ``LAG LEAD`` (one arg,
+              kwargs ``n`` and ``default``) or ``FIRST_VALUE LAST_VALUE NTH_VALUE`` (one arg, NTH_VALUE's kwarg ``n``,
+              and the frame kwargs of an aggregate, none for the whole partition): evaluated over the logical
               partitions of ``fa.transform`` (PartitionSpec keys, presort order) by a ``ColumnMap``
 
 plus an optional output alias and an optional cast of the node's result.  ``fugue_b200/expr.py`` compiles
@@ -95,7 +97,11 @@ SHAPES = frozenset(h for h, a in AGGREGATES.items() if a.family == "shape")
 BIVARIATES = frozenset(h for h, a in AGGREGATES.items() if a.family == "bivariate")
 _AGG_ALIASES = {"STDDEV": "STDDEV_SAMP", "VARIANCE": "VAR_SAMP", "SKEW": "SKEWNESS", "KURT": "KURTOSIS"}
 _RANKINGS = frozenset(["ROW_NUMBER", "RANK", "DENSE_RANK"])
-_SPEC_ONLY = _RANKINGS | {"LAG", "LEAD"}  # window heads that take a partition and an order but no frame
+# window-only heads: NTILE (kwarg ``n``), PERCENT_RANK and CUME_DIST take a spec and no frame; FIRST_VALUE, LAST_VALUE
+# and NTH_VALUE (kwarg ``n``) take the frames an aggregate takes.  Neither set belongs to AGGREGATES or SCALARS.
+DISTRIBUTIONS = frozenset(["NTILE", "PERCENT_RANK", "CUME_DIST"])
+VALUE_HEADS = frozenset(["FIRST_VALUE", "LAST_VALUE", "NTH_VALUE"])
+_SPEC_ONLY = _RANKINGS | DISTRIBUTIONS | {"LAG", "LEAD"}  # window heads that take a partition and an order but no frame
 _RUNNING_FRAME = "ROWS BETWEEN UNBOUNDED PRECEDING AND CURRENT ROW"
 _LITERAL_TYPES = (int, bool, float, str, datetime.date, datetime.datetime, datetime.timedelta)
 TEMPORAL_LITERALS = (datetime.date, datetime.datetime, datetime.timedelta)
@@ -333,7 +339,10 @@ class ColumnExpr:
                 return pa.string() if case_string_results(self) is not None else None
             return None if rule is None else pa.type_for_alias(rule)
         if k == Kind.WINDOW:
-            return pa.int64() if self.head in _RANKINGS else self.args[0].infer_type(schema)  # LAG LEAD: the arg's
+            if self.head in ("PERCENT_RANK", "CUME_DIST"):
+                return pa.float64()
+            # LAG LEAD FIRST_VALUE LAST_VALUE NTH_VALUE: the arg's
+            return pa.int64() if self.head in _RANKINGS or self.head == "NTILE" else self.args[0].infer_type(schema)
         return None
 
     # ---- text -------------------------------------------------------------------------------------
@@ -425,8 +434,9 @@ class ColumnExpr:
         (PARTITION BY .. ORDER BY ..)``, and runs in ``select / assign / filter`` and SQL, not in a ``ColumnMap``.
         Either one given, even as ``[]``, makes it explicit; ``partition_by=[]`` alone is ``OVER ()``, the whole
         table.  NULLs sort last in both directions.  The frame keeps the meaning above (the default is the whole
-        partition, not SQL's running default of a statement with ORDER BY).  ROW_NUMBER, RANK, DENSE_RANK, LAG and
-        LEAD take a spec and no frame; a percentile takes ``partition_by`` only."""
+        partition, not SQL's running default of a statement with ORDER BY).  ROW_NUMBER, RANK, DENSE_RANK, NTILE,
+        PERCENT_RANK, CUME_DIST, LAG and LEAD take a spec and no frame; a percentile takes ``partition_by`` only;
+        FIRST_VALUE, LAST_VALUE and NTH_VALUE take every frame and spec an aggregate takes, once."""
         explicit = partition_by is not None or order_by is not None
         spec = _window_spec(self, partition_by, order_by) if explicit else {}
         if self.kind == Kind.WINDOW and self.head in _SPEC_ONLY and explicit and not is_explicit(self):
@@ -434,6 +444,17 @@ class ColumnExpr:
                 raise ValueError(f"{self}: {self.head} takes no frame")
             return ColumnExpr(Kind.WINDOW, self.head, self.args, {**self.kwargs, **spec}, False, self.as_name,
                               self.as_type)
+        if self.kind == Kind.WINDOW and self.head in VALUE_HEADS:
+            if is_explicit(self) or any(k in self.kwargs for k in ("running", "rows", "range")):
+                raise ValueError(f"{self} already has its window")
+            if not isinstance(running, bool):
+                raise ValueError(f"running must be a bool, got {running!r}")
+            running, rows, range = _normalise_frame(running, rows, range)
+            if explicit and range is not None and any(b not in (None, 0) for b in range) and \
+                    len(spec["order_by"]) != 1:
+                raise ValueError(f"{self}: a RANGE frame with an offset needs exactly one ORDER BY expression")
+            return ColumnExpr(Kind.WINDOW, self.head, self.args, {**self.kwargs, **_frame_kwargs(running, rows, range),
+                                                                   **spec}, False, self.as_name, self.as_type)
         if self.kind != Kind.AGG:
             raise ValueError(f"{self} is not an aggregation: only an aggregation has an OVER form")
         if self.is_distinct:
@@ -450,26 +471,7 @@ class ColumnExpr:
                 raise ValueError(f"{self}: a percentile covers the whole partition; it takes no ORDER BY")
             return ColumnExpr(Kind.WINDOW, self.head, self.args, {**self.kwargs, **spec}, False, self.as_name,
                               self.as_type)
-        if range is not None:
-            if running or rows is not None:
-                raise ValueError("over() takes one of running=True, rows and range")
-            range = _range_frame(range)
-            if range == (None, None):
-                range = None
-        if rows is not None:
-            if running:
-                raise ValueError("over() takes running=True or rows, not both")
-            if not isinstance(rows, tuple) or len(rows) != 2:
-                raise ValueError(f"rows must be a (start, end) tuple, got {rows!r}")
-            for b in rows:
-                if isinstance(b, bool) or not (b is None or isinstance(b, int)):
-                    raise ValueError(f"a frame bound must be an int or None, got {b!r}")
-            if rows[0] is not None and rows[1] is not None and rows[0] > rows[1]:
-                raise ValueError(f"frame start {rows[0]} is after its end {rows[1]}")
-            if rows == (None, 0):
-                running, rows = True, None
-            elif rows == (None, None):
-                rows = None
+        running, rows, range = _normalise_frame(running, rows, range)
         if a.frames == "running" and (rows is not None or range is not None):
             hint = "; write ROWS BETWEEN UNBOUNDED PRECEDING AND CURRENT ROW for the running form" \
                 if range == (None, 0) else ""
@@ -482,16 +484,45 @@ class ColumnExpr:
             raise ValueError(f"{self}: {self.head} needs a column")
         if explicit and range is not None and any(b not in (None, 0) for b in range) and len(spec["order_by"]) != 1:
             raise ValueError(f"{self}: a RANGE frame with an offset needs exactly one ORDER BY expression")
-        if range is not None:
-            kwargs: Dict[str, Any] = {"range": range}
-        else:
-            kwargs = {"running": running} if rows is None else {"rows": (rows[0], rows[1])}
-        return ColumnExpr(Kind.WINDOW, self.head, self.args, {**kwargs, **spec}, False, self.as_name, self.as_type)
+        return ColumnExpr(Kind.WINDOW, self.head, self.args, {**_frame_kwargs(running, rows, range), **spec}, False,
+                          self.as_name, self.as_type)
 
     def __bool__(self) -> bool:
         raise TypeError("a column expression has no truth value; use & | ~ to combine conditions")
 
     __hash__ = object.__hash__
+
+
+def _normalise_frame(running: bool, rows: Any, range: Any) -> Tuple[bool, Any, Any]:  # noqa: A002 - the SQL word
+    """The checked frame of ``over()``: ``rows=(None, 0)`` is ``running=True``, ``rows=(None, None)`` and ``range=(None,
+    None)`` the whole partition."""
+    if range is not None:
+        if running or rows is not None:
+            raise ValueError("over() takes one of running=True, rows and range")
+        range = _range_frame(range)
+        if range == (None, None):
+            range = None
+    if rows is not None:
+        if running:
+            raise ValueError("over() takes running=True or rows, not both")
+        if not isinstance(rows, tuple) or len(rows) != 2:
+            raise ValueError(f"rows must be a (start, end) tuple, got {rows!r}")
+        for b in rows:
+            if isinstance(b, bool) or not (b is None or isinstance(b, int)):
+                raise ValueError(f"a frame bound must be an int or None, got {b!r}")
+        if rows[0] is not None and rows[1] is not None and rows[0] > rows[1]:
+            raise ValueError(f"frame start {rows[0]} is after its end {rows[1]}")
+        if rows == (None, 0):
+            running, rows = True, None
+        elif rows == (None, None):
+            rows = None
+    return running, rows, range
+
+
+def _frame_kwargs(running: bool, rows: Any, range: Any) -> Dict[str, Any]:  # noqa: A002 - the SQL word
+    if range is not None:
+        return {"range": range}
+    return {"running": running} if rows is None else {"rows": (rows[0], rows[1])}
 
 
 def _binary_method(op: str, swap: bool) -> Any:
@@ -700,6 +731,8 @@ def _window_text(e: ColumnExpr, show: Any) -> str:
     parts = [show(x) for x in e.args]
     if e.head in ("LAG", "LEAD"):
         parts += [str(e.kwargs["n"]), _show_literal(e.kwargs["default"])]
+    elif e.head in ("NTILE", "NTH_VALUE"):
+        parts.append(str(e.kwargs["n"]))
     frame = _RUNNING_FRAME if e.kwargs.get("running", False) else ""
     for unit in ("rows", "range"):
         if unit in e.kwargs:
@@ -773,6 +806,21 @@ def _offset_fn(name: str, c: Any, n: Any, default: Any, aggregated: bool = False
     if arg.kind == Kind.WILDCARD or (is_agg(arg) and not aggregated) or has_window(arg):
         raise ValueError(f"{name} needs a row-wise column expression, got {arg}")
     return ColumnExpr(Kind.WINDOW, name, [arg], {"n": n, "default": default})
+
+
+def _nth(name: str, n: Any) -> int:
+    if isinstance(n, bool) or not isinstance(n, int) or n < 1:
+        raise ValueError(f"{name}: n must be an int >= 1, got {n!r}")
+    return n
+
+
+def _value_fn(name: str, c: Any, kwargs: Dict[str, Any], aggregated: bool = False) -> ColumnExpr:
+    """FIRST_VALUE / LAST_VALUE / NTH_VALUE of the row-wise expression ``c`` (over GROUP BY results, ``aggregated``,
+    it may read aggregations)."""
+    arg = col(c)
+    if arg.kind == Kind.WILDCARD or (is_agg(arg) and not aggregated) or has_window(arg):
+        raise ValueError(f"{name} needs a row-wise column expression, got {arg}")
+    return ColumnExpr(Kind.WINDOW, name, [arg], kwargs)
 
 
 def scalar_head(name: str) -> Optional[Tuple[str, Scalar]]:
@@ -1286,6 +1334,39 @@ class functions:
     def lead(c: Any, n: int = 1, default: Any = None) -> ColumnExpr:
         """``c`` of the row ``n`` rows later in the same logical partition, else ``default``."""
         return _offset_fn("LEAD", c, n, default)
+
+    @staticmethod
+    def ntile(n: int) -> ColumnExpr:
+        """SQL NTILE: the bucket 1..n of the row in partition order, bucket sizes differing by at most one, the
+        larger buckets first (1..N when the partition has N < n rows)."""
+        return ColumnExpr(Kind.WINDOW, "NTILE", [], {"n": _nth("NTILE", n)})
+
+    @staticmethod
+    def percent_rank() -> ColumnExpr:
+        """SQL PERCENT_RANK: (RANK - 1) / (partition rows - 1), 0 in a partition of one row (float64)."""
+        return ColumnExpr(Kind.WINDOW, "PERCENT_RANK")
+
+    @staticmethod
+    def cume_dist() -> ColumnExpr:
+        """SQL CUME_DIST: the rows up to and including the current row's last peer over the partition's rows."""
+        return ColumnExpr(Kind.WINDOW, "CUME_DIST")
+
+    @staticmethod
+    def first_value(c: Any) -> ColumnExpr:
+        """SQL FIRST_VALUE: ``c`` at the first row of the frame, NULL included (FIRST skips NULLs); NULL for an empty
+        frame.  The frame is the whole partition unless ``over()`` gives one."""
+        return _value_fn("FIRST_VALUE", c, {})
+
+    @staticmethod
+    def last_value(c: Any) -> ColumnExpr:
+        """SQL LAST_VALUE: ``c`` at the last row of the frame, NULL included; NULL for an empty frame."""
+        return _value_fn("LAST_VALUE", c, {})
+
+    @staticmethod
+    def nth_value(c: Any, n: int) -> ColumnExpr:
+        """SQL NTH_VALUE: ``c`` at the frame's ``n``-th row (``n >= 1``), NULL included; NULL when the frame has fewer
+        than ``n`` rows."""
+        return _value_fn("NTH_VALUE", c, {"n": _nth("NTH_VALUE", n)})
 
 
 def _time_word(fn: str, what: str, word: Any, known: Tuple[str, ...]) -> str:

@@ -622,6 +622,14 @@ __device__ __forceinline__ uint32_t frame_code(int lo, int hi, int blk_lo, int b
   return mode | (uint32_t)lo << 2 | (uint32_t)hi << 13;
 }
 
+// Row i's ROWS frame [lo, hi] inside its segment [sa, sb) (lo > hi: empty), with start / end clipped by make_frame
+// so that i + start and i + end cannot wrap.  The combine pass and fb_window_value both call it.
+__device__ __forceinline__ void rows_frame(int64_t i, int64_t sa, int64_t sb, int64_t start, int64_t end, int flags,
+                                           int64_t* lo, int64_t* hi) {
+  *lo = (flags & FB_FRAME_UNBOUNDED_START) || i + start < sa ? sa : i + start;
+  *hi = (flags & FB_FRAME_UNBOUNDED_END) || i + end > sb - 1 ? sb - 1 : i + end;
+}
+
 struct FrameSmem {
   uint64_t pv[padded(kFrameSpan)];  // staged values, then P
   uint64_t sv[padded(kFrameSpan)];
@@ -774,8 +782,8 @@ fb_window_frame_combine_kernel(int64_t nrows, int64_t nseg, const int64_t* __res
   for (int64_t i = t0 + threadIdx.x; i < t1; i += kThreads) {
     const int64_t q = q0 + upper_bound(offsets + q0, nq, i) - 1;
     const int64_t sa = __ldg(offsets + q), sb = __ldg(offsets + q + 1);
-    const int64_t lo = (flags & FB_FRAME_UNBOUNDED_START) || i + start < sa ? sa : i + start;
-    const int64_t hi = (flags & FB_FRAME_UNBOUNDED_END) || i + end > sb - 1 ? sb - 1 : i + end;
+    int64_t lo, hi;
+    rows_frame(i, sa, sb, start, end, flags, &lo, &hi);
     uint32_t mode = kFrameEmpty;
     if (lo <= hi) {
       if (flags & FB_FRAME_UNBOUNDED_START) mode = kFrameP;
@@ -1028,6 +1036,242 @@ int build_tree(int dev, cudaStream_t st, const ScanCols& a, int64_t nrows, void*
     FB_CUDA(cudaGetLastError());
   }
   return 0;
+}
+
+// ---- value heads: FIRST_VALUE / LAST_VALUE / NTH_VALUE ------------------------------------------------
+struct ValueCols {
+  const void* vals[FB_SCAN_MAX_COLS];
+  const uint8_t* valid[FB_SCAN_MAX_COLS];
+  void* out[FB_SCAN_MAX_COLS];
+  uint8_t* out_valid[FB_SCAN_MAX_COLS];
+  int64_t nth[FB_SCAN_MAX_COLS];  // >= 1: the frame's nth row (at most nrows + 1); FB_VALUE_LAST: its last row
+  int32_t width[FB_SCAN_MAX_COLS];
+  int32_t ncols;
+};
+
+// One thread per row: the row's frame (ROWS: rows_frame over its segment; else [d_lo, d_hi] clamped to the table),
+// the picked row, then every column's value and validity at that row.  Neighbouring rows pick neighbouring rows.
+__global__ void __launch_bounds__(kRangeThreads)
+fb_window_value_kernel(int64_t nrows, int64_t nseg, const int64_t* __restrict__ offsets, int64_t start, int64_t end,
+                       int flags, const int64_t* __restrict__ d_lo, const int64_t* __restrict__ d_hi,
+                       const __grid_constant__ ValueCols a) {
+  __shared__ int64_t range[2];
+  const int64_t t0 = (int64_t)blockIdx.x * kRangeThreads;
+  const int64_t t1 = t0 + kRangeThreads < nrows ? t0 + kRangeThreads : nrows;
+  const int64_t i = t0 + threadIdx.x;
+  int64_t lo, hi;
+  if (d_lo == nullptr) {  // uniform across the CTA
+    if (threadIdx.x == 0) {
+      range[0] = upper_bound(offsets, nseg + 1, t0) - 1;
+      range[1] = upper_bound(offsets, nseg + 1, t1 - 1) + 1;
+    }
+    __syncthreads();
+    if (i >= t1) return;
+    const int64_t q0 = range[0];
+    const int64_t q = q0 + upper_bound(offsets + q0, range[1] - q0, i) - 1;
+    rows_frame(i, __ldg(offsets + q), __ldg(offsets + q + 1), start, end, flags, &lo, &hi);
+  } else {
+    if (i >= t1) return;
+    lo = __ldg((const long long*)d_lo + i);
+    hi = __ldg((const long long*)d_hi + i);
+    lo = lo < 0 ? 0 : lo;
+    hi = hi > nrows - 1 ? nrows - 1 : hi;
+  }
+  for (int c = 0; c < a.ncols; ++c) {
+    const int64_t n = a.nth[c];
+    const int64_t j = n == FB_VALUE_LAST ? hi : lo + n - 1;  // lo <= nrows and n <= nrows + 1: no wrap
+    const bool hit = lo <= hi && j <= hi;
+    const uint8_t* vm = a.valid[c];
+    const bool ok = hit && (vm == nullptr || __ldg(vm + j) != 0);
+    switch (a.width[c]) {
+      case 1: ((uint8_t*)a.out[c])[i] = ok ? __ldg((const uint8_t*)a.vals[c] + j) : 0; break;
+      case 2: ((uint16_t*)a.out[c])[i] = ok ? __ldg((const unsigned short*)a.vals[c] + j) : 0; break;
+      case 4: ((uint32_t*)a.out[c])[i] = ok ? __ldg((const unsigned int*)a.vals[c] + j) : 0; break;
+      default: ((uint64_t*)a.out[c])[i] = ok ? __ldg((const unsigned long long*)a.vals[c] + j) : 0; break;
+    }
+    a.out_valid[c][i] = ok ? 1 : 0;
+  }
+}
+
+// ---- distribution heads: PERCENT_RANK / CUME_DIST / NTILE ---------------------------------------------
+// A peer group is the rows from one head byte to the next (or to its segment's bound).  Head bytes are not
+// monotone, so no search over them bounds its loads by the distance; instead each tile of kTile rows publishes
+// the first and last head row inside it, one CTA turns those into the last head before every tile and the first
+// head after it (a max / min scan over tiles), and the row pass resolves every row's peer group from its tile's
+// heads in shared memory plus those two carries: O(1) per row whatever the size of the peer group.
+struct DistCols {
+  int64_t n[FB_SCAN_MAX_COLS];
+  int64_t* out[FB_SCAN_MAX_COLS];
+  int32_t ncols;
+};
+
+constexpr int64_t kNoHead = INT64_MAX;
+
+__device__ __forceinline__ int64_t max64(int64_t a, int64_t b) { return a > b ? a : b; }
+__device__ __forceinline__ int64_t min64(int64_t a, int64_t b) { return a < b ? a : b; }
+
+// Per tile: the first head row in it (kNoHead: none) and the last (-1: none).
+__global__ void __launch_bounds__(kThreads)
+fb_peer_tile_kernel(int64_t nrows, const uint8_t* __restrict__ heads, int64_t* __restrict__ tile_first,
+                    int64_t* __restrict__ tile_last) {
+  __shared__ int64_t wf[kThreads / 32], wl[kThreads / 32];
+  const int64_t t0 = (int64_t)blockIdx.x * kTile;
+  int64_t f = kNoHead, l = -1;
+  for (int k = 0; k < kItems; ++k) {
+    const int64_t i = t0 + threadIdx.x + (int64_t)kThreads * k;
+    if (i < nrows && __ldg(heads + i) != 0) {
+      f = min64(f, i);
+      l = i;
+    }
+  }
+#pragma unroll
+  for (int d = 16; d > 0; d >>= 1) {
+    f = min64(f, __shfl_xor_sync(0xFFFFFFFFu, f, d));
+    l = max64(l, __shfl_xor_sync(0xFFFFFFFFu, l, d));
+  }
+  if ((threadIdx.x & 31) == 0) {
+    wf[threadIdx.x >> 5] = f;
+    wl[threadIdx.x >> 5] = l;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int w = 1; w < kThreads / 32; ++w) {
+      f = min64(f, wf[w]);
+      l = max64(l, wl[w]);
+    }
+    tile_first[blockIdx.x] = min64(f, wf[0]);
+    tile_last[blockIdx.x] = max64(l, wl[0]);
+  }
+}
+
+constexpr int kCarryThreads = 1024;
+
+// One CTA, in place: tile_last[t] := the last head row before tile t (-1: none), tile_first[t] := the first head row
+// after it (kNoHead: none).  Thread k owns a contiguous run of tiles; the runs' totals are scanned in shared memory.
+__global__ void __launch_bounds__(kCarryThreads, 1)
+fb_peer_carry_kernel(int64_t ntiles, int64_t* __restrict__ tile_first, int64_t* __restrict__ tile_last) {
+  __shared__ int64_t sl[kCarryThreads], sf[kCarryThreads];
+  const int64_t per = (ntiles + kCarryThreads - 1) / kCarryThreads;
+  const int64_t b0 = min64((int64_t)threadIdx.x * per, ntiles), b1 = min64(b0 + per, ntiles);
+  int64_t l = -1, f = kNoHead;
+  for (int64_t t = b0; t < b1; ++t) {
+    l = max64(l, tile_last[t]);
+    f = min64(f, tile_first[t]);
+  }
+  sl[threadIdx.x] = l;
+  sf[threadIdx.x] = f;
+  __syncthreads();
+  for (int d = 1; d < kCarryThreads; d <<= 1) {  // inclusive: max from the left, min from the right
+    const int k = threadIdx.x;
+    const int64_t xl = k >= d ? sl[k - d] : -1;
+    const int64_t xf = k + d < kCarryThreads ? sf[k + d] : kNoHead;
+    __syncthreads();
+    sl[k] = max64(sl[k], xl);
+    sf[k] = min64(sf[k], xf);
+    __syncthreads();
+  }
+  l = threadIdx.x > 0 ? sl[threadIdx.x - 1] : -1;
+  f = threadIdx.x + 1 < kCarryThreads ? sf[threadIdx.x + 1] : kNoHead;
+  for (int64_t t = b0; t < b1; ++t) {
+    const int64_t x = tile_last[t];
+    tile_last[t] = l;
+    l = max64(l, x);
+  }
+  for (int64_t t = b1 - 1; t >= b0; --t) {
+    const int64_t x = tile_first[t];
+    tile_first[t] = f;
+    f = min64(f, x);
+  }
+}
+
+// Max (kRev: min) over the threads before (kRev: after) this one of x, and of seed: exact and order-free.
+template <bool kRev>
+__device__ __forceinline__ int64_t block_exclusive_extreme(int64_t x, int64_t seed, int64_t* warp_tot) {
+  constexpr int kWarps = kThreads / 32;
+  const int lane = kRev ? 31 - (threadIdx.x & 31) : threadIdx.x & 31;
+  const int w = kRev ? kWarps - 1 - (int)(threadIdx.x >> 5) : threadIdx.x >> 5;
+  auto op = [](int64_t p, int64_t q) { return kRev ? min64(p, q) : max64(p, q); };
+  int64_t inc = x;
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) {
+    const int64_t o = kRev ? __shfl_down_sync(0xFFFFFFFFu, inc, d) : __shfl_up_sync(0xFFFFFFFFu, inc, d);
+    if (lane >= d) inc = op(inc, o);
+  }
+  const int64_t ex = kRev ? __shfl_down_sync(0xFFFFFFFFu, inc, 1) : __shfl_up_sync(0xFFFFFFFFu, inc, 1);
+  if (lane == 31) warp_tot[w] = inc;
+  __syncthreads();
+  int64_t pre = seed;
+  for (int k = 0; k < w; ++k) pre = op(pre, warp_tot[k]);
+  __syncthreads();  // warp_tot is reused by the next call
+  return lane == 0 ? pre : op(pre, ex);
+}
+
+// One CTA per kTile rows.  Thread t reads head bytes of rows 8t .. 8t + 7 of the tile from shared memory and finds
+// every row's last head at or before it and first head after it; then rows are striped over threads for the
+// segment search and the coalesced stores.
+__global__ void __launch_bounds__(kThreads)
+fb_window_distribution_kernel(int64_t nrows, int64_t nseg, const int64_t* __restrict__ offsets,
+                              const uint8_t* __restrict__ heads, const int64_t* __restrict__ tile_first,
+                              const int64_t* __restrict__ tile_last, double* __restrict__ percent_rank,
+                              double* __restrict__ cume_dist, const __grid_constant__ DistCols d) {
+  __shared__ uint8_t hd[kTile];
+  __shared__ int64_t pf[kTile], nx[kTile];
+  __shared__ int64_t warp_tot[kThreads / 32];
+  __shared__ int64_t range[2];
+  const int64_t t0 = (int64_t)blockIdx.x * kTile;
+  const int64_t t1 = t0 + kTile < nrows ? t0 + kTile : nrows;
+  if (threadIdx.x == 0) {
+    range[0] = upper_bound(offsets, nseg + 1, t0) - 1;
+    range[1] = upper_bound(offsets, nseg + 1, t1 - 1) + 1;
+  }
+  for (int j = threadIdx.x; j < kTile; j += kThreads) hd[j] = t0 + j < t1 ? __ldg(heads + t0 + j) : 0;
+  __syncthreads();
+  const int j0 = threadIdx.x * kItems;
+  int64_t last = -1, first = kNoHead;
+#pragma unroll
+  for (int k = 0; k < kItems; ++k) {
+    if (hd[j0 + k]) {
+      last = t0 + j0 + k;
+      first = min64(first, t0 + j0 + k);
+    }
+  }
+  int64_t p = block_exclusive_extreme<false>(last, tile_last[blockIdx.x], warp_tot);
+  int64_t q = block_exclusive_extreme<true>(first, tile_first[blockIdx.x], warp_tot);
+#pragma unroll
+  for (int k = 0; k < kItems; ++k) {
+    if (hd[j0 + k]) p = t0 + j0 + k;
+    pf[j0 + k] = p;
+  }
+#pragma unroll
+  for (int k = kItems - 1; k >= 0; --k) {
+    nx[j0 + k] = q;
+    if (hd[j0 + k]) q = t0 + j0 + k;
+  }
+  __syncthreads();
+  const int64_t q0 = range[0], nq = range[1] - q0;
+  for (int j = threadIdx.x; j < kTile; j += kThreads) {
+    const int64_t i = t0 + j;
+    if (i >= t1) break;
+    const int64_t s = q0 + upper_bound(offsets + q0, nq, i) - 1;
+    const int64_t a = __ldg(offsets + s), b = __ldg(offsets + s + 1);
+    const int64_t first_peer = max64(pf[j], a), last_peer = min64(nx[j], b) - 1;
+    const int64_t rows = b - a;
+    if (percent_rank != nullptr)  // (rank - 1) / (N - 1): one IEEE division of two exact integers
+      percent_rank[i] = rows > 1 ? (double)(first_peer - a) / (double)(rows - 1) : 0.0;
+    if (cume_dist != nullptr) cume_dist[i] = (double)(last_peer - a + 1) / (double)rows;
+    const int64_t r = i - a;
+    for (int c = 0; c < d.ncols; ++c) {  // SQLite's NTILE: N / n rows a bucket, the first N % n buckets one more
+      const int64_t n = d.n[c], size = rows / n;
+      int64_t bucket;
+      if (size == 0) {
+        bucket = r + 1;
+      } else {
+        const int64_t large = rows - n * size, small_from = large * (size + 1);
+        bucket = r < small_from ? 1 + r / (size + 1) : 1 + large + (r - small_from) / size;
+      }
+      d.out[c][i] = bucket;
+    }
+  }
 }
 
 // the column arrays of the C ABI -> ScanCols (checked)
@@ -1316,4 +1560,88 @@ extern "C" int fb_window_tree(int dev, void* stream, int64_t nrows, int ncols, c
   FbDeviceGuard guard(dev);
   FB_CHECK(guard.ok, "cannot select device %d", dev);
   return build_tree(dev, (cudaStream_t)stream, a, nrows, scratch) != 0 ? 2 : 0;
+}
+
+extern "C" int fb_window_value(int dev, void* stream, int64_t nrows, int64_t nseg, const int64_t* d_offsets,
+                               int64_t start, int64_t end, int flags, const int64_t* d_lo, const int64_t* d_hi,
+                               int ncols, const int64_t* nths, const int32_t* widths, const void* const* vals,
+                               const uint8_t* const* valid, void* const* out_vals, uint8_t* const* out_valid) {
+  FB_CHECK(nrows >= 0 && nseg >= 0, "negative row or segment count");
+  FB_CHECK((flags & ~(FB_FRAME_UNBOUNDED_START | FB_FRAME_UNBOUNDED_END)) == 0, "unknown frame flags %d", flags);
+  FB_CHECK((d_lo == nullptr) == (d_hi == nullptr), "give both of d_lo / d_hi or neither");
+  FB_CHECK(ncols >= 1 && ncols <= FB_SCAN_MAX_COLS, "ncols=%d out of range [1,%d]", ncols, FB_SCAN_MAX_COLS);
+  FB_CHECK(nths != nullptr && widths != nullptr && vals != nullptr && out_vals != nullptr && out_valid != nullptr,
+           "NULL column arrays");
+  ValueCols a;
+  memset(&a, 0, sizeof(a));
+  a.ncols = ncols;
+  for (int c = 0; c < ncols; ++c) {
+    FB_CHECK(nths[c] == FB_VALUE_LAST || nths[c] >= 1, "column %d: nth %lld < 1", c, (long long)nths[c]);
+    FB_CHECK(widths[c] == 1 || widths[c] == 2 || widths[c] == 4 || widths[c] == 8, "column %d: width %d", c,
+             widths[c]);
+    a.nth[c] = nths[c] > nrows ? nrows + 1 : nths[c];  // past every frame either way; lo + n - 1 cannot wrap
+    a.width[c] = widths[c];
+    a.vals[c] = vals[c];
+    a.valid[c] = valid != nullptr ? valid[c] : nullptr;
+    a.out[c] = out_vals[c];
+    a.out_valid[c] = out_valid[c];
+    FB_CHECK(nrows == 0 || (a.vals[c] != nullptr && a.out[c] != nullptr && a.out_valid[c] != nullptr),
+             "column %d: NULL values or outputs", c);
+  }
+  if (nrows == 0) return 0;
+  FB_CHECK(d_lo != nullptr || (nseg >= 1 && d_offsets != nullptr), "%lld rows need at least one segment",
+           (long long)nrows);
+  if (d_lo == nullptr) FB_CHECK(flags != 0 || start <= end, "frame start %lld > end %lld", (long long)start,
+                                (long long)end);
+  const Frame f = make_frame(nrows, start, end, flags);
+  const int64_t grid = (nrows + kRangeThreads - 1) / kRangeThreads;
+  FB_CHECK(grid < (1LL << 31), "too many rows");
+  FbDeviceGuard guard(dev);
+  FB_CHECK(guard.ok, "cannot select device %d", dev);
+  fb_window_value_kernel<<<(unsigned)grid, kRangeThreads, 0, (cudaStream_t)stream>>>(
+      nrows, nseg, d_offsets, f.start, f.end, f.flags, d_lo, d_hi, a);
+  FB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+extern "C" size_t fb_window_distribution_scratch_bytes(int64_t nrows) {
+  return nrows > 0 ? 2 * sizeof(int64_t) * (size_t)num_tiles(nrows) : 0;
+}
+
+extern "C" int fb_window_distribution(int dev, void* stream, int64_t nrows, int64_t nseg, const int64_t* d_offsets,
+                                      const uint8_t* d_heads, double* d_percent_rank, double* d_cume_dist,
+                                      int nntile, const int64_t* ntiles, int64_t* const* d_ntile, void* scratch,
+                                      size_t scratch_bytes) {
+  FB_CHECK(nrows >= 0 && nseg >= 0, "negative row or segment count");
+  FB_CHECK(nntile >= 0 && nntile <= FB_SCAN_MAX_COLS, "nntile=%d out of range [0,%d]", nntile, FB_SCAN_MAX_COLS);
+  DistCols d;
+  memset(&d, 0, sizeof(d));
+  d.ncols = nntile;
+  for (int c = 0; c < nntile; ++c) {
+    FB_CHECK(ntiles != nullptr && d_ntile != nullptr, "NULL NTILE arrays");
+    FB_CHECK(ntiles[c] >= 1, "NTILE %d: n = %lld < 1", c, (long long)ntiles[c]);
+    FB_CHECK(nrows == 0 || d_ntile[c] != nullptr, "NTILE %d: NULL output", c);
+    d.n[c] = ntiles[c];
+    d.out[c] = d_ntile[c];
+  }
+  if (nrows == 0) return 0;
+  FB_CHECK(nseg >= 1 && d_offsets != nullptr && d_heads != nullptr, "%lld rows need segments and head bytes",
+           (long long)nrows);
+  const int64_t tiles = num_tiles(nrows);
+  FB_CHECK(tiles < (1LL << 31), "too many rows");
+  FB_CHECK(scratch != nullptr && scratch_bytes >= fb_window_distribution_scratch_bytes(nrows),
+           "scratch too small: %zu < %zu", scratch_bytes, fb_window_distribution_scratch_bytes(nrows));
+  FbDeviceGuard guard(dev);
+  FB_CHECK(guard.ok, "cannot select device %d", dev);
+  cudaStream_t st = (cudaStream_t)stream;
+  int64_t* tile_first = (int64_t*)scratch;
+  int64_t* tile_last = tile_first + tiles;
+  fb_peer_tile_kernel<<<(unsigned)tiles, kThreads, 0, st>>>(nrows, d_heads, tile_first, tile_last);
+  FB_CUDA(cudaGetLastError());
+  fb_peer_carry_kernel<<<1, kCarryThreads, 0, st>>>(tiles, tile_first, tile_last);
+  FB_CUDA(cudaGetLastError());
+  fb_window_distribution_kernel<<<(unsigned)tiles, kThreads, 0, st>>>(nrows, nseg, d_offsets, d_heads, tile_first,
+                                                                       tile_last, d_percent_rank, d_cume_dist, d);
+  FB_CUDA(cudaGetLastError());
+  return 0;
 }

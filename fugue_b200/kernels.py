@@ -622,6 +622,88 @@ def window_bounded(lo: torch.Tensor, hi: torch.Tensor,
                                                            hi.data_ptr(), *args))
 
 
+VALUE_LAST = 0   # FB_VALUE_LAST: the frame's last row
+
+
+def _i64_array(vals: Sequence[int]) -> Any:
+    arr = (C.c_int64 * max(len(vals), 1))()
+    for i, v in enumerate(vals):
+        arr[i] = int(v)
+    return arr
+
+
+def window_value(offsets: Optional[torch.Tensor], nrows: int, frame: Any,
+                 columns: Sequence[Tuple[torch.Tensor, Optional[torch.Tensor], int]]
+                 ) -> List[Tuple[torch.Tensor, torch.Tensor]]:
+    """K9: FIRST_VALUE / LAST_VALUE / NTH_VALUE (``fb_window_value``).  ``frame`` is ``("rows", start, end)`` over the
+    segments ``offsets`` (``None``: unbounded; as :func:`window_frame`) or ``("bounds", lo, hi)``, every row's first
+    and last frame row (int64, as :func:`window_range_bounds` returns them).  ``columns`` = one ``(values of any width,
+    validity or None, nth)`` per column: nth >= 1 picks the frame's nth row, ``VALUE_LAST`` its last.  Returns per
+    column (value, uint8 validity): NULL for an empty frame, a pick past its end or a NULL at the picked row.  Up to
+    ``SCAN_MAX_COLS`` columns share one launch."""
+    lib = _lib.load()
+    dev = columns[0][0].device
+    lo = hi = None
+    start = end = flags = 0
+    nseg = 0
+    if frame[0] == "rows":
+        _, s, e = frame
+        dev, nseg = _segments(offsets)
+        if s is not None and s <= -nrows:
+            s = None
+        if e is not None and e >= nrows:
+            e = None
+        flags = (FRAME_UNBOUNDED_START if s is None else 0) | (FRAME_UNBOUNDED_END if e is None else 0)
+        start, end = (0 if s is None else s), (0 if e is None else e)
+    else:
+        _, lo, hi = frame
+        for b_ in (lo, hi):
+            assert b_.dtype == torch.int64 and b_.device == dev and b_.is_contiguous() and b_.shape[0] == nrows
+    res: List[Tuple[torch.Tensor, torch.Tensor]] = []
+    for b in range(0, len(columns), SCAN_MAX_COLS):
+        batch = columns[b:b + SCAN_MAX_COLS]
+        for v, m, nth in batch:
+            assert v.device == dev and v.is_contiguous() and v.dim() == 1 and v.shape[0] == nrows
+            assert v.element_size() in (1, 2, 4, 8)
+            assert nth == VALUE_LAST or nth >= 1
+            _check_rows(m, dev, nrows, torch.uint8)
+        outs = [(torch.empty_like(v), torch.empty(nrows, dtype=torch.uint8, device=dev)) for v, _, _ in batch]
+        _lib.check(lib.fb_window_value(
+            dev.index, _stream_ptr(dev), nrows, nseg, 0 if offsets is None else offsets.data_ptr(), start, end, flags,
+            0 if lo is None else lo.data_ptr(), 0 if hi is None else hi.data_ptr(), len(batch),
+            _i64_array([min(nth, nrows + 1) for _, _, nth in batch]),
+            _lib.i32_array([v.element_size() for v, _, _ in batch]), _ptrs([v for v, _, _ in batch]),
+            _ptrs([m for _, m, _ in batch]), _ptrs([o for o, _ in outs]), _ptrs([ov for _, ov in outs])))
+        res.extend(outs)
+    return res
+
+
+def window_distribution(offsets: torch.Tensor, heads: torch.Tensor, percent_rank: bool, cume_dist: bool,
+                        ntiles: Sequence[int]) -> Tuple[Optional[torch.Tensor], Optional[torch.Tensor], List[torch.Tensor]]:
+    """K9: PERCENT_RANK, CUME_DIST and NTILE(n) of every row over the segments ``offsets`` (``fb_window_distribution``);
+    ``heads`` (bool or uint8, one per row) marks the first row of every peer group.  Returns (float64 PERCENT_RANK or
+    None, float64 CUME_DIST or None, one int64 column per n of ``ntiles``); ``SCAN_MAX_COLS`` NTILEs a launch."""
+    lib = _lib.load()
+    dev, nseg = _segments(offsets)
+    nrows = int(heads.shape[0])
+    heads = heads.view(torch.uint8) if heads.dtype == torch.bool else heads
+    _check_rows(heads, dev, nrows, torch.uint8)
+    pr = torch.empty(nrows, dtype=torch.float64, device=dev) if percent_rank else None
+    cd = torch.empty(nrows, dtype=torch.float64, device=dev) if cume_dist else None
+    nts = [torch.empty(nrows, dtype=torch.int64, device=dev) for _ in ntiles]
+    nb = int(lib.fb_window_distribution_scratch_bytes(nrows))
+    scratch = torch.empty(max(nb, 8), dtype=torch.uint8, device=dev)
+    for b in range(0, max(len(ntiles), 1), SCAN_MAX_COLS):
+        ns, outs = ntiles[b:b + SCAN_MAX_COLS], nts[b:b + SCAN_MAX_COLS]
+        assert all(n >= 1 for n in ns)
+        first = b == 0
+        _lib.check(lib.fb_window_distribution(
+            dev.index, _stream_ptr(dev), nrows, nseg, offsets.data_ptr(), heads.data_ptr(),
+            0 if pr is None or not first else pr.data_ptr(), 0 if cd is None or not first else cd.data_ptr(),
+            len(ns), _i64_array([min(n, 1 << 62) for n in ns]), _ptrs(outs), scratch.data_ptr(), scratch.numel()))
+    return pr, cd, nts
+
+
 QUANTILE_TILE_ROWS = 2048   # FB_QUANTILE_TILE_ROWS: longest segment of the one-pass shared-memory path
 QUANTILE_MAX_Q = 16
 QUANTILE_CONT = 0

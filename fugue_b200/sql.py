@@ -21,6 +21,9 @@ Window functions (DESIGN §7p):
     <call> OVER ( [PARTITION BY <expr>, ...] [ORDER BY <expr> [ASC|DESC] [NULLS LAST], ...] [<frame>] )
     <call>  ::= any aggregate above | ROW_NUMBER() | RANK() | DENSE_RANK() | LAG(x[, n[, default]])
               | LEAD(x[, n[, default]]) | PERCENTILE_CONT / PERCENTILE_DISC(q) WITHIN GROUP (ORDER BY x)
+              | NTILE(n) | PERCENT_RANK() | CUME_DIST() | FIRST_VALUE(x) | LAST_VALUE(x) | NTH_VALUE(x, n)
+                (n an integer literal >= 1; NTILE, PERCENT_RANK and CUME_DIST take no frame; the value functions
+                respect NULLs: IGNORE NULLS and FROM LAST raise NotImplementedError)
     <frame> ::= ROWS | RANGE  BETWEEN <bound> AND <bound>  |  ROWS | RANGE <bound>
     <bound> ::= UNBOUNDED PRECEDING | n PRECEDING | CURRENT ROW | n FOLLOWING | UNBOUNDED FOLLOWING
                 (a RANGE offset n may be an INTERVAL '..' DAY / DAY TO SECOND literal)
@@ -29,7 +32,8 @@ Window functions (DESIGN §7p):
     included), without ORDER BY the whole partition.  NULLs sort last in both directions.  A window over a
     GROUP BY reads group keys and aggregates only (``RANK() OVER (ORDER BY SUM(v) DESC)``).  GROUPS frames,
     EXCLUDE, named windows (WINDOW w AS, OVER w) and NULLS FIRST raise NotImplementedError, and so do
-    ROW_NUMBER / RANK / DENSE_RANK / LAG / LEAD without OVER; a window in WHERE, GROUP BY, HAVING or in another
+    ROW_NUMBER / RANK / DENSE_RANK / NTILE / PERCENT_RANK / CUME_DIST / LAG / LEAD / FIRST_VALUE / LAST_VALUE /
+    NTH_VALUE without OVER; a window in WHERE, GROUP BY, HAVING or in another
     window's arguments raises ValueError.
     SELECT * FROM a [[AS] x] [INNER | LEFT [OUTER] | RIGHT [OUTER] | FULL [OUTER] | [LEFT] SEMI | [LEFT] ANTI] JOIN
              b [[AS] y] USING (k, ...) | ON x.k = y.k [AND ...]              -> hash join kernels
@@ -64,8 +68,9 @@ from typing import Any, Dict, List, Tuple
 
 import pyarrow as pa
 
-from .column import (_SPEC_ONLY, BIVARIATES, PERCENTILES, ColumnExpr, Kind, SelectColumns, _offset_fn, all_cols,
-                     check_arity, col, function, functions, has_window, is_agg, lit, null, scalar_head)
+from .column import (_SPEC_ONLY, BIVARIATES, PERCENTILES, VALUE_HEADS, ColumnExpr, Kind, SelectColumns, _nth,
+                     _offset_fn, _value_fn, all_cols, check_arity, col, function, functions, has_window, is_agg, lit,
+                     null, scalar_head)
 from .dataframe import DataFrame
 
 _AGG = r"(SUM|COUNT|MIN|MAX|AVG|MEAN)\s*\(\s*(\*|[A-Za-z_][\w]*)\s*\)"
@@ -870,7 +875,7 @@ class _Parser:
         return col(name)
 
     def _call(self, fn: str) -> ColumnExpr:
-        e = self._window_call(fn) if fn in _SPEC_ONLY else self._plain_call(fn)
+        e = self._window_call(fn) if fn in _SPEC_ONLY or fn in VALUE_HEADS else self._plain_call(fn)
         if self.at_kw("OVER"):
             return self._over(e)
         if e.kind == Kind.WINDOW:
@@ -883,13 +888,17 @@ class _Parser:
         """``ROW_NUMBER() / RANK() / DENSE_RANK()`` or ``LAG / LEAD(x[, n[, default]])``: n an integer literal,
         default a literal."""
         self.i += 2  # name (
-        if fn in ("ROW_NUMBER", "RANK", "DENSE_RANK"):
+        if fn in ("ROW_NUMBER", "RANK", "DENSE_RANK", "PERCENT_RANK", "CUME_DIST"):
             self.expect(")")
             return getattr(functions, fn.lower())()
         args = [self.expr()]
         while self.op(","):
             args.append(self.expr())
+        if fn in VALUE_HEADS and (self.at_kw("IGNORE") or self.at_kw("RESPECT")):
+            self.fail(f"{fn}(... {self.peek()[1].upper()} NULLS)")
         self.expect(")")
+        if fn in ("NTILE", "FIRST_VALUE", "LAST_VALUE", "NTH_VALUE"):
+            return self._value_call(fn, args)
         if len(args) > 3:
             raise ValueError(f"{fn} takes 1 to 3 arguments, got {len(args)} in: {self.sql}")
         for what, x in zip(("n", "default"), args[1:]):
@@ -898,6 +907,34 @@ class _Parser:
         n = args[1].value if len(args) > 1 else 1
         default = args[2].value if len(args) > 2 else None
         return _offset_fn(fn, args[0], n, default, aggregated=True)
+
+    def _value_call(self, fn: str, args: List[ColumnExpr]) -> ColumnExpr:
+        """``NTILE(n)``, ``FIRST_VALUE(x)``, ``LAST_VALUE(x)`` or ``NTH_VALUE(x, n)`` [FROM FIRST] [RESPECT NULLS]: n an
+        integer literal >= 1 (any other literal is a ValueError, an expression NotImplementedError).  IGNORE NULLS and
+        FROM LAST raise NotImplementedError."""
+        want = {"NTILE": 1, "NTH_VALUE": 2}.get(fn, 1)
+        if len(args) != want:
+            raise ValueError(f"{fn} takes {want} argument{'s' if want > 1 else ''}, got {len(args)} in: {self.sql}")
+        if fn == "NTH_VALUE" and self.kw("FROM"):
+            if not self.kw("FIRST"):
+                self.fail(f"{fn} ... FROM LAST")
+        if self.kw("IGNORE", "NULLS"):
+            self.fail(f"{fn} ... IGNORE NULLS")
+        self.kw("RESPECT", "NULLS")
+        if fn in ("NTILE", "NTH_VALUE"):
+            x = args[-1]
+            if x.kind == Kind.UNARY and x.head == "-" and x.args[0].kind == Kind.LITERAL:
+                x = lit(-x.args[0].value) if isinstance(x.args[0].value, (int, float)) else x
+            if x.kind != Kind.LITERAL or x.as_type is not None:
+                self.fail(f"{fn} with the non-literal n {x}")
+            try:
+                n = _nth(fn, x.value)
+            except ValueError as ex:
+                raise ValueError(f"{ex} in: {self.sql}") from None
+            if fn == "NTILE":
+                return functions.ntile(n)
+            return _value_fn(fn, args[0], {"n": n}, aggregated=True)
+        return _value_fn(fn, args[0], {}, aggregated=True)
 
     def _over(self, e: ColumnExpr) -> ColumnExpr:
         """``<call> OVER ([PARTITION BY e, ..] [ORDER BY e [ASC|DESC] [NULLS LAST], ..] [frame])``.  SQL's default

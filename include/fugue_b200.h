@@ -396,6 +396,38 @@ int fb_window_bounded(int dev, void* stream, int64_t nrows, const int64_t* d_lo,
 int fb_window_tree(int dev, void* stream, int64_t nrows, int ncols, const int32_t* ops, const void* const* vals,
                    const uint8_t* const* valid, void* scratch, size_t scratch_bytes);
 
+/* K9  value heads: FIRST_VALUE / LAST_VALUE / NTH_VALUE over a frame, NULLs respected.  Row i's frame [lo, hi] is
+ * either its ROWS frame (d_lo == d_hi == NULL: segments d_offsets, start / end / flags exactly as fb_window_frame,
+ * found by the same arithmetic) or [d_lo[i], d_hi[i]] clamped to [0, nrows) (both given, as fb_window_range_bounds
+ * writes them; d_offsets unused).  For each of the ncols <= FB_SCAN_MAX_COLS columns c the picked row is
+ * lo + nths[c] - 1 (nths[c] >= 1) or hi (nths[c] == FB_VALUE_LAST); an empty frame, a pick past hi or a NULL at the
+ * picked row (valid[c][j] == 0) gives out_valid[c][i] = 0 and an all-zero value, else out_vals[c][i] is the
+ * widths[c]-byte value (1 / 2 / 4 / 8) of vals[c] at the picked row and out_valid[c][i] = 1.  Any nths[c] >= 1 is
+ * accepted (one past nrows selects nothing).  One thread per row, one launch for every column: no bound array is
+ * written.  nths, widths, vals, valid (NULL, or entries NULL: all valid), out_vals and out_valid (entries required)
+ * are HOST arrays. */
+#define FB_VALUE_LAST 0
+int fb_window_value(int dev, void* stream, int64_t nrows, int64_t nseg, const int64_t* d_offsets, int64_t start,
+                    int64_t end, int flags, const int64_t* d_lo, const int64_t* d_hi, int ncols, const int64_t* nths,
+                    const int32_t* widths, const void* const* vals, const uint8_t* const* valid,
+                    void* const* out_vals, uint8_t* const* out_valid);
+
+/* K9  distribution heads over the segments of fb_segmented_scan.  d_heads[i] != 0 marks a row that starts a peer
+ * group (rows equal on every ORDER BY key; a segment start always starts one, marked or not).  With N = b - a the
+ * row count of row i's segment [a, b) and [pf, pl] its peer group, writes (any output may be NULL):
+ *   d_percent_rank[i]  (pf - a) / (N - 1), 0 when N = 1 (f64, one IEEE division of two exact integers)
+ *   d_cume_dist[i]     (pl - a + 1) / N (f64, likewise)
+ *   d_ntile[c][i]      NTILE(ntiles[c]) (int64, ntiles[c] >= 1): with s = N / n and L = N - n s, rows r = i - a below
+ *                      L (s + 1) take bucket 1 + r / (s + 1), the rest 1 + L + (r - L (s + 1)) / s; 1 + r when s = 0
+ * for nntile <= FB_SCAN_MAX_COLS NTILE columns (ntiles and d_ntile are HOST arrays).  Three launches: the first
+ * and last head row of every tile of 2048 rows, one CTA scanning those into the last head before and first head
+ * after every tile, then the rows: O(1) per row for any peer-group size.  Scratch:
+ * fb_window_distribution_scratch_bytes. */
+size_t fb_window_distribution_scratch_bytes(int64_t nrows);
+int fb_window_distribution(int dev, void* stream, int64_t nrows, int64_t nseg, const int64_t* d_offsets,
+                           const uint8_t* d_heads, double* d_percent_rank, double* d_cume_dist, int nntile,
+                           const int64_t* ntiles, int64_t* const* d_ntile, void* scratch, size_t scratch_bytes);
+
 /* ---------------------------------------------------------------------------
  * K10 exact order statistics per segment: PERCENTILE_CONT / PERCENTILE_DISC / MEDIAN of one column over the
  *     segments [d_offsets[s], d_offsets[s + 1]) of fb_segmented_scan (logical partitions, sorted groups)

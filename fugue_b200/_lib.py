@@ -133,6 +133,10 @@ SIGNATURES = {
     "fb_segmented_shape_moments_scratch_bytes": (C.c_size_t, [C.c_int64, C.c_int]),
     "fb_segmented_shape_moments": (C.c_int, [C.c_int, _vp, C.c_int64, C.c_int64, _vp, C.c_int, _vpp, _vpp, _vpp,
                                              _vpp, _vpp, _vpp, _vp, C.c_size_t]),
+    "fb_segmented_ewm_scratch_bytes": (C.c_size_t, [C.c_int64, C.c_int]),
+    "fb_segmented_ewm": (C.c_int, [C.c_int, _vp, C.c_int64, C.c_int64, _vp, C.c_int, _vpp, _vpp, C.POINTER(C.c_double),
+                                   _i32p, _i32p, _vpp, C.POINTER(C.c_double), _vpp, _vpp, _vpp, _vpp, _vpp, _vp,
+                                   C.c_size_t]),
     "fb_window_frame_scratch_bytes": (C.c_size_t, [C.c_int64, C.c_int, C.c_int64, C.c_int64, C.c_int]),
     "fb_window_frame": (C.c_int, [C.c_int, _vp, C.c_int64, C.c_int64, _vp, C.c_int64, C.c_int64, C.c_int, C.c_int,
                                   _i32p, _vpp, _vpp, _vpp, _vpp, _vp, C.c_size_t]),
@@ -209,6 +213,13 @@ def ptr_array(ptrs) -> "C.Array":
     arr = (C.c_void_p * max(len(ptrs), 1))()
     for i, p in enumerate(ptrs):
         arr[i] = p
+    return arr
+
+
+def f64_array(vals) -> "C.Array":
+    arr = (C.c_double * max(len(vals), 1))()
+    for i, v in enumerate(vals):
+        arr[i] = float(v)
     return arr
 
 

@@ -13,7 +13,7 @@ import torch
 
 from . import kernels as K
 from . import sort as S
-from .column import AGGREGATES, result_type
+from .column import AGGREGATES, EWM_HEADS, result_type
 from .table import B200Table, narrow, widen
 
 # (function, values are float64) -> the K6 / K9 op; FIRST / LAST reduce the row numbers of the valid rows
@@ -27,7 +27,7 @@ def check_argument(fn: str, name: str, tp: pa.DataType, is_dictionary: bool) -> 
     """Reject an argument column ``name`` of arrow type ``tp`` that ``fn`` does not take: the variances and the
     shape statistics and the two-argument functions need integer or float columns, and a string column takes no SUM
     or AVG."""
-    if AGGREGATES[fn].family in ("variance", "shape", "bivariate"):
+    if fn in EWM_HEADS or AGGREGATES[fn].family in ("variance", "shape", "bivariate"):
         if is_dictionary or not (pa.types.is_integer(tp) or pa.types.is_floating(tp)):
             raise NotImplementedError(f"{fn} needs integer or float columns; {name} is {tp}")
     elif is_dictionary and fn in ("SUM", "AVG"):
@@ -137,6 +137,28 @@ def shape_of(fn: str, m: torch.Tensor, m2: torch.Tensor, m3: torch.Tensor,
         else:
             v = g - 3.0
     v = torch.where(flat, torch.zeros_like(v), v)
+    return torch.where(has, v, torch.zeros_like(v)).contiguous(), has.to(torch.uint8)
+
+
+def ewm_of(fn: str, m: torch.Tensor, mean: torch.Tensor, w: torch.Tensor, w2: torch.Tensor, c: torch.Tensor, bias: bool,
+           min_periods: int) -> Tuple[torch.Tensor, torch.Tensor]:
+    """``fn`` (an ``EWM_HEADS`` head) from the running observation count m, weighted mean, W, W2 and C of
+    ``fb_segmented_ewm``: (float64 values, validity).  NULL before the first observation and while m < min_periods.
+    EWM_VAR is C / W, times W^2 / (W^2 - W2) unless ``bias``, as pandas computes it, and NULL where W^2 - W2 <= 0
+    (one observation); EWM_STD is its square root."""
+    has = m >= max(min_periods, 1)
+    if fn == "EWM_MEAN":
+        v = mean
+    else:
+        ws = torch.where(has, w, torch.ones_like(w))
+        v = c / ws
+        if not bias:
+            num = ws * ws
+            den = num - w2
+            has = has & (den > 0)
+            v = num / torch.where(den > 0, den, torch.ones_like(den)) * v
+        if fn == "EWM_STD":
+            v = torch.sqrt(v)
     return torch.where(has, v, torch.zeros_like(v)).contiguous(), has.to(torch.uint8)
 
 

@@ -32,8 +32,9 @@ import torch
 from . import aggregates as A
 from . import kernels as K
 from .aggregates import bivariate_of
-from .column import (AGGREGATES, DISTRIBUTIONS, PERCENTILES, VALUE_HEADS, ColumnExpr, Kind, SelectColumns,
-                     bivariate_xy, col as _col, has_window, has_explicit_window, is_agg, is_explicit, result_type)
+from .column import (AGGREGATES, DISTRIBUTIONS, EWM_HEADS, PERCENTILES, VALUE_HEADS, ColumnExpr, Kind, SelectColumns,
+                     bivariate_xy, col as _col, ewm_alpha, has_window, has_explicit_window, is_agg, is_explicit,
+                     result_type)
 from .table import B200Table, _storage_dtype, narrow, widen
 
 
@@ -243,6 +244,8 @@ def _with_windows(t: B200Table, cols: List[ColumnExpr]) -> B200Table:
     moments: Dict[str, int] = {}  # argument column of a variance -> its column of the moments scan
     shapes: Dict[str, int] = {}  # argument column of a skewness or kurtosis -> its column of the shape-moments scan
     comoments: Dict[Tuple[str, str], int] = {}  # (x, y) argument columns of a pair -> its pair of the co-moments scan
+    ewms: Dict[Tuple[Any, ...], int] = {}  # (argument column, _ewm_decay) -> its column of the ewm scan
+    ewm_spread: set = set()  # the ewm scan columns an EWM_VAR or EWM_STD reads
     pair_sums: Dict[Tuple[str, str], Tuple[Any, Any]] = {}  # (x, y) -> the running SUM scans of x and y over the pair
     finish: List[Any] = []     # per node: (fingerprint, fn(scan results) -> (column, validity, type, dictionary))
     values: Dict[Any, List[Any]] = {}  # frame -> (values, validity, nth) of its FIRST / LAST / NTH_VALUE nodes
@@ -297,6 +300,15 @@ def _with_windows(t: B200Table, cols: List[ColumnExpr]) -> B200Table:
             vcols.append((base.columns[ci], base.valid[ci], nth))
             finish.append((uid, lambda r, j=(vframe, len(vcols) - 1), tp=base.schema.types[ci],
                            d=base.dictionaries.get(name): (*r[("value",) + j], tp, d)))
+            continue
+        if fn in EWM_HEADS:  # the ewm scan: one column per argument and decay, shared by its heads
+            name = arg_name[bare.arg.fingerprint()]
+            A.check_argument(fn, name, base.schema.types[base.schema.index_of_key(name)], name in base.dictionaries)
+            j = ewms.setdefault((name,) + _ewm_decay(t, bare), len(ewms))
+            if fn != "EWM_MEAN":  # a variance reads W, W2 and C as well; a mean alone writes only count and mean
+                ewm_spread.add(j)
+            finish.append((uid, lambda r, j=j, fn=fn, kw=bare.kwargs: (
+                *A.ewm_of(fn, *r[("ewm", j)], kw.get("bias", False), kw["min_periods"]), pa.float64(), None)))
             continue
         frame = bare.kwargs.get("rows")  # ROWS BETWEEN frame[0] AND frame[1]: the moving-frame kernel
         if "range" in bare.kwargs:  # RANGE BETWEEN: ("range", key class or None, start, end), the block tree
@@ -418,6 +430,10 @@ def _with_windows(t: B200Table, cols: List[ColumnExpr]) -> B200Table:
     if comoments:
         pairs = [f64_valid(x) + f64_valid(y) for x, y in comoments]
         results.update((("comoments", j), r) for j, r in enumerate(K.segmented_comoments(off.contiguous(), n, pairs)))
+    if ewms:
+        ecols = [f64_valid(name) + (alpha, adjust, pos, _ewm_times(t) if pos == K.EWM_TIMES else None, scale,
+                                    j in ewm_spread) for (name, alpha, adjust, pos, scale), j in ewms.items()]
+        results.update((("ewm", j), r) for j, r in enumerate(K.segmented_ewm(off.contiguous(), n, ecols)))
     names, types, columns, valid = list(base.schema.names), list(base.schema.types), list(base.columns), list(base.valid)
     dicts = dict(base.dictionaries)
     window_names: Dict[str, str] = {}
@@ -571,6 +587,52 @@ def _percentile_value(base: B200Table, name: str, j: int, cont: bool, lengths: t
         return g, gv, tp, base.dictionaries.get(name)
 
     return run
+
+
+def _ewm_decay(t: B200Table, node: ColumnExpr) -> Tuple[float, bool, int, float]:
+    """(alpha, adjust, positions, 1 / halflife) of an EWM node for ``K.segmented_ewm``: pandas' alpha, and for a time
+    decay the halflife as a number (whole or not) of units of the single ascending order column of ``t``."""
+    kw = node.kwargs
+    if not kw["times"]:
+        return ewm_alpha(kw), kw["adjust"], K.EWM_OBSERVATIONS if kw["ignore_na"] else K.EWM_ROWS, 1.0
+    name = _ewm_time_column(t, node)
+    tp = t.schema[name].type
+    h = kw["halflife"]
+    if pa.types.is_integer(tp):
+        if isinstance(h, datetime.timedelta):
+            raise ValueError(f"{node}: a timedelta halflife needs a temporal order column; {name} is {tp}")
+        units = float(h)
+    else:
+        if not isinstance(h, datetime.timedelta):
+            raise ValueError(f"{node}: the temporal order column {name} ({tp}) needs a timedelta halflife, got {h!r}")
+        # any number of units, whole or not: only the scale 1 / halflife reaches the device
+        unit = "D" if pa.types.is_date32(tp) else ("ms" if pa.types.is_date64(tp) else tp.unit)
+        us = h // datetime.timedelta(microseconds=1)
+        units = us * 1000.0 if unit == "ns" else us / (86_400_000_000 if unit == "D" else _TIME_UNIT_US[unit])
+    return ewm_alpha(kw), kw["adjust"], K.EWM_TIMES, 1.0 / units
+
+
+def _ewm_time_column(t: B200Table, node: Any = None) -> str:
+    """The order column of a time decay: the single ascending presort (or ORDER BY) column of ``t``, an integer, date,
+    timestamp or duration column."""
+    order = list(getattr(t, "logical_order", None) or [])
+    if len(order) != 1:
+        raise ValueError(f"{node}: time decay needs exactly one presort / ORDER BY column, got {order}")
+    if not (getattr(t, "logical_ascending", None) or [True])[0]:
+        raise ValueError(f"{node}: time decay needs ascending times; {order[0]} is sorted descending")
+    tp = t.schema[order[0]].type
+    if order[0] in t.dictionaries or not (pa.types.is_integer(tp) or pa.types.is_date(tp) or
+                                          pa.types.is_timestamp(tp) or pa.types.is_duration(tp)):
+        raise ValueError(f"{node}: time decay needs an integer or temporal order column; {order[0]} is {tp}")
+    return order[0]
+
+
+def _ewm_times(t: B200Table) -> torch.Tensor:
+    """The time-decay order column of ``t`` as contiguous int64; ValueError for a NULL time."""
+    i = t.schema.index_of_key(_ewm_time_column(t))
+    if t.valid[i] is not None and not bool(t.valid[i].all()):
+        raise ValueError(f"time decay needs non-NULL times; {t.schema.names[i]} holds a NULL")
+    return widen(t.columns[i], t.schema.types[i]).contiguous()
 
 
 _TIME_UNIT_US = {"s": 1_000_000, "ms": 1_000, "us": 1}  # microseconds per unit ("ns": 1 / 1000)

@@ -101,7 +101,10 @@ _RANKINGS = frozenset(["ROW_NUMBER", "RANK", "DENSE_RANK"])
 # and NTH_VALUE (kwarg ``n``) take the frames an aggregate takes.  Neither set belongs to AGGREGATES or SCALARS.
 DISTRIBUTIONS = frozenset(["NTILE", "PERCENT_RANK", "CUME_DIST"])
 VALUE_HEADS = frozenset(["FIRST_VALUE", "LAST_VALUE", "NTH_VALUE"])
-_SPEC_ONLY = _RANKINGS | DISTRIBUTIONS | {"LAG", "LEAD"}  # window heads that take a partition and an order but no frame
+# window-only exponentially weighted heads (pandas' ewm): a spec and no frame, the decay and options as kwargs
+EWM_HEADS = frozenset(["EWM_MEAN", "EWM_VAR", "EWM_STD"])
+# window heads that take a partition and an order but no frame
+_SPEC_ONLY = _RANKINGS | DISTRIBUTIONS | EWM_HEADS | {"LAG", "LEAD"}
 _RUNNING_FRAME = "ROWS BETWEEN UNBOUNDED PRECEDING AND CURRENT ROW"
 _LITERAL_TYPES = (int, bool, float, str, datetime.date, datetime.datetime, datetime.timedelta)
 TEMPORAL_LITERALS = (datetime.date, datetime.datetime, datetime.timedelta)
@@ -339,7 +342,7 @@ class ColumnExpr:
                 return pa.string() if case_string_results(self) is not None else None
             return None if rule is None else pa.type_for_alias(rule)
         if k == Kind.WINDOW:
-            if self.head in ("PERCENT_RANK", "CUME_DIST"):
+            if self.head in ("PERCENT_RANK", "CUME_DIST") or self.head in EWM_HEADS:
                 return pa.float64()
             # LAG LEAD FIRST_VALUE LAST_VALUE NTH_VALUE: the arg's
             return pa.int64() if self.head in _RANKINGS or self.head == "NTILE" else self.args[0].infer_type(schema)
@@ -442,6 +445,12 @@ class ColumnExpr:
         if self.kind == Kind.WINDOW and self.head in _SPEC_ONLY and explicit and not is_explicit(self):
             if running or rows is not None or range is not None:
                 raise ValueError(f"{self}: {self.head} takes no frame")
+            if self.head in EWM_HEADS and self.kwargs["times"]:
+                order = spec["order_by"]
+                if len(order) != 1:
+                    raise ValueError(f"{self}: time decay needs exactly one ORDER BY expression")
+                if not order[0][1]:
+                    raise ValueError(f"{self}: time decay needs ascending times; ORDER BY is DESC")
             return ColumnExpr(Kind.WINDOW, self.head, self.args, {**self.kwargs, **spec}, False, self.as_name,
                               self.as_type)
         if self.kind == Kind.WINDOW and self.head in VALUE_HEADS:
@@ -733,6 +742,8 @@ def _window_text(e: ColumnExpr, show: Any) -> str:
         parts += [str(e.kwargs["n"]), _show_literal(e.kwargs["default"])]
     elif e.head in ("NTILE", "NTH_VALUE"):
         parts.append(str(e.kwargs["n"]))
+    elif e.head in EWM_HEADS:
+        parts += _ewm_text(e.kwargs)
     frame = _RUNNING_FRAME if e.kwargs.get("running", False) else ""
     for unit in ("rows", "range"):
         if unit in e.kwargs:
@@ -743,6 +754,26 @@ def _window_text(e: ColumnExpr, show: Any) -> str:
         whole = "ROWS BETWEEN UNBOUNDED PRECEDING AND UNBOUNDED FOLLOWING"
         frame = "" if frame == default else (frame or whole)
     return f"{e.head}({','.join(parts)}) OVER ({' '.join(spec + ([frame] if frame else []))})"
+
+
+def _ewm_text(kw: Dict[str, Any]) -> List[str]:
+    """The arguments after x of an EWM node: SQL's ``alpha [, adjust]`` or ``INTERVAL halflife [, adjust]``, and
+    ``name=value`` for what SQL does not spell (com, span, a numeric halflife, ignore_na, min_periods, bias)."""
+    key = next(k for k in EWM_DECAYS if k in kw)
+    sql = key == "alpha" or (kw["times"] and isinstance(kw[key], datetime.timedelta))
+    if sql:
+        parts = [_interval_text(kw[key]) if kw["times"] else repr(kw[key])]
+    else:
+        parts = [f"{key}={kw[key]!r}"] + (["times=TRUE"] if kw["times"] else [])
+    if not kw["adjust"]:
+        parts.append("FALSE" if sql else "adjust=FALSE")
+    if kw["ignore_na"]:
+        parts.append("ignore_na=TRUE")
+    if kw["min_periods"]:
+        parts.append(f"min_periods={kw['min_periods']}")
+    if kw.get("bias"):
+        parts.append("bias=TRUE")
+    return parts
 
 
 def _frame_bound(b: Any, unbounded: str) -> str:
@@ -806,6 +837,69 @@ def _offset_fn(name: str, c: Any, n: Any, default: Any, aggregated: bool = False
     if arg.kind == Kind.WILDCARD or (is_agg(arg) and not aggregated) or has_window(arg):
         raise ValueError(f"{name} needs a row-wise column expression, got {arg}")
     return ColumnExpr(Kind.WINDOW, name, [arg], {"n": n, "default": default})
+
+
+EWM_DECAYS = ("alpha", "com", "span", "halflife")
+
+
+def _ewm_fn(name: str, c: Any, decay: Dict[str, Any], adjust: Any, ignore_na: Any, min_periods: Any, times: Any,
+            bias: Any = None) -> ColumnExpr:
+    """An EWM node: ``decay`` the given ones of com / span / halflife / alpha (exactly one), checked as pandas checks
+    them; ``times`` a time decay over the node's single order column (``halflife`` only: a ``timedelta`` for a temporal
+    column, a positive number for a numeric one)."""
+    given = {k: v for k, v in decay.items() if v is not None}
+    if len(given) != 1:
+        raise ValueError(f"{name}: give exactly one of com, span, halflife and alpha, got {sorted(given) or 'none'}")
+    for what, v in (("adjust", adjust), ("ignore_na", ignore_na), ("times", times)) + \
+            ((("bias", bias),) if bias is not None else ()):
+        if not isinstance(v, bool):
+            raise ValueError(f"{name}: {what} must be a bool, got {v!r}")
+    if isinstance(min_periods, bool) or not isinstance(min_periods, int) or min_periods < 0:
+        raise ValueError(f"{name}: min_periods must be an int >= 0, got {min_periods!r}")
+    (key, v), = given.items()
+    if times:
+        if key != "halflife":
+            raise ValueError(f"{name}: time decay takes halflife, not {key}")
+        if ignore_na:
+            raise NotImplementedError(f"{name}: time decay with ignore_na=True is not supported")
+        if name != "EWM_MEAN":
+            raise NotImplementedError(f"{name}: time decay is supported for EWM_MEAN only")
+    if isinstance(v, datetime.timedelta):
+        if not (times and key == "halflife"):
+            raise ValueError(f"{name}: a timedelta {key} needs times=True")
+        if v <= datetime.timedelta(0):
+            raise ValueError(f"{name}: halflife must be > 0, got {v}")
+    else:
+        if isinstance(v, bool) or not isinstance(v, (int, float)) or not math.isfinite(v):
+            raise ValueError(f"{name}: {key} must be a finite number, got {v!r}")
+        v = float(v) if key != "halflife" or not times or isinstance(v, float) else v
+        low = {"alpha": "0 < alpha <= 1", "com": "com >= 0", "span": "span >= 1", "halflife": "halflife > 0"}[key]
+        ok = {"alpha": 0 < v <= 1, "com": v >= 0, "span": v >= 1, "halflife": v > 0}[key]
+        if not ok:
+            raise ValueError(f"{name}: {key} must satisfy {low}, got {v!r}")
+    arg = col(c)
+    if arg.kind == Kind.WILDCARD or is_agg(arg) or has_window(arg):
+        raise ValueError(f"{name} needs a row-wise column expression, got {arg}")
+    kw: Dict[str, Any] = {key: v, "adjust": adjust, "ignore_na": ignore_na, "min_periods": min_periods, "times": times}
+    if bias is not None:
+        kw["bias"] = bias
+    return ColumnExpr(Kind.WINDOW, name, [arg], kw)
+
+
+def ewm_alpha(kw: Dict[str, Any]) -> float:
+    """pandas' alpha of an EWM node's decay, in float64 as pandas computes it: through the center of mass, 1 / (1 +
+    com).  A time decay runs with pandas' default com = 1 (alpha 0.5): its weights decay by 0.5^(dt / halflife)."""
+    if kw["times"]:
+        return 0.5
+    if "com" in kw:
+        com = kw["com"]
+    elif "span" in kw:
+        com = (kw["span"] - 1) / 2
+    elif "halflife" in kw:
+        com = 1 / (1 - math.exp(math.log(0.5) / kw["halflife"])) - 1
+    else:
+        com = (1 - kw["alpha"]) / kw["alpha"]
+    return float(1 / (1 + com))
 
 
 def _nth(name: str, n: Any) -> int:
@@ -1361,6 +1455,34 @@ class functions:
     def last_value(c: Any) -> ColumnExpr:
         """SQL LAST_VALUE: ``c`` at the last row of the frame, NULL included; NULL for an empty frame."""
         return _value_fn("LAST_VALUE", c, {})
+
+    @staticmethod
+    def ewm_mean(c: Any, com: Any = None, span: Any = None, halflife: Any = None, alpha: Any = None, *,
+                 adjust: bool = True, ignore_na: bool = False, min_periods: int = 0, times: bool = False) -> ColumnExpr:
+        """pandas' ``ewm(...).mean()`` over the logical partition in presort (or ORDER BY) order, as a window function
+        (float64).  Exactly one of ``com``, ``span``, ``halflife`` and ``alpha`` gives the decay; ``times=True`` decays
+        by 0.5^(dt / halflife) over the single order column (ascending, no NULLs).  An observation is a non-NULL,
+        non-NaN value of ``c`` (an integer or float column); NULL before the first observation and while fewer than
+        ``min_periods`` observations are in, and a row without a value repeats the last result.  No frame."""
+        return _ewm_fn("EWM_MEAN", c, dict(com=com, span=span, halflife=halflife, alpha=alpha), adjust, ignore_na,
+                       min_periods, times)
+
+    @staticmethod
+    def ewm_var(c: Any, com: Any = None, span: Any = None, halflife: Any = None, alpha: Any = None, *,
+                adjust: bool = True, ignore_na: bool = False, min_periods: int = 0, bias: bool = False,
+                times: bool = False) -> ColumnExpr:
+        """pandas' ``ewm(...).var(bias=bias)``: the weighted variance C / W about the weighted mean, times W^2 / (W^2 -
+        W2) unless ``bias`` (NULL below two observations).  Options as :meth:`ewm_mean`; time decay is not supported."""
+        return _ewm_fn("EWM_VAR", c, dict(com=com, span=span, halflife=halflife, alpha=alpha), adjust, ignore_na,
+                       min_periods, times, bias)
+
+    @staticmethod
+    def ewm_std(c: Any, com: Any = None, span: Any = None, halflife: Any = None, alpha: Any = None, *,
+                adjust: bool = True, ignore_na: bool = False, min_periods: int = 0, bias: bool = False,
+                times: bool = False) -> ColumnExpr:
+        """pandas' ``ewm(...).std(bias=bias)``: the square root of :meth:`ewm_var`."""
+        return _ewm_fn("EWM_STD", c, dict(com=com, span=span, halflife=halflife, alpha=alpha), adjust, ignore_na,
+                       min_periods, times, bias)
 
     @staticmethod
     def nth_value(c: Any, n: int) -> ColumnExpr:

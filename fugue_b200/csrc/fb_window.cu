@@ -193,6 +193,88 @@ __device__ __forceinline__ SSt combine(int, const SSt& a, const SSt& b) {
              a.f};
 }
 
+// ---- exponentially weighted moments (fb_segmented_ewm) ----
+// A column's decay over a position difference dt (int64, exact): beta^dt = exp2(k dt), k = log2(1 - alpha) when the
+// positions are row indices or observation ordinals (obs), -1 / halflife when they are times.  A new observation weighs
+// 1 with adjust, else alpha times the total weight before it.
+struct EwOp {
+  double k, alpha;
+  int32_t adjust, obs;
+};
+__device__ __forceinline__ bool is_count_op(const EwOp&) { return false; }
+__device__ __forceinline__ double decay(const EwOp& op, int64_t dt) { return dt == 0 ? 1.0 : exp2(op.k * (double)dt); }
+
+// The observations of a run of consecutive rows: their count c, the positions t1 and tl of the first and the last, the
+// first value x1, q and, over the others, (w, w2, mean, cm): the sums of the weights and of their squares, the weighted
+// mean and the sum of w (x - mean)^2, every weight seen from tl.  With adjust the weights are absolute and q is x1's
+// own weight (beta^(tl - t1)); the total weight of a run is at least its last observation's 1.  Without adjust every
+// weight is a share of the run's total weight at tl (so q + w = 1): q is the share of all that came before the run's
+// second observation (x1 and, for a run inside a partition, the rows before the run).  Keeping shares rather than
+// pandas' running total T, which shrinks or grows by beta^g + alpha at every gap, is what keeps a long partition
+// from overflowing or underflowing (DESIGN §7s).
+struct EwSt {
+  int64_t c, t1, tl;
+  double x1, q, w, w2, mean, cm;
+  int32_t f;
+  static constexpr int kWords = 9;
+  template <class A, class B, class G>
+  __device__ __forceinline__ static void zip(A& a, B& b, G&& g) {
+    g(a.c, b.c); g(a.t1, b.t1); g(a.tl, b.tl); g(a.x1, b.x1); g(a.q, b.q);
+    g(a.w, b.w); g(a.w2, b.w2); g(a.mean, b.mean); g(a.cm, b.cm);
+  }
+};
+
+// (sum of weights, of squared weights, weighted mean, sum of w (x - mean)^2) of a weighted set
+struct EwSum {
+  double w, w2, mean, cm;
+};
+
+// `a` followed by `b`: the weighted Chan update.  A non-finite mean difference means a non-finite value: the mean is
+// then the weighted sum of the two, as in CSt's combine.  A weight decayed to 0 (alpha = 1, or an underflow) leaves
+// nothing of `a` but its sums, so that 0 / 0 never occurs.  The weights divide, not multiply by a reciprocal: a total
+// weight decayed below 2^-1022 has no finite reciprocal.
+__device__ __forceinline__ EwSum ew_merge(const EwSum& a, const EwSum& b) {
+  if (a.w == 0.0) return EwSum{b.w, a.w2 + b.w2, b.mean, a.cm + b.cm};
+  const double w = a.w + b.w;
+  const double d = b.mean - a.mean;
+  const double wb = b.w / w;
+  return EwSum{w, a.w2 + b.w2, isfinite(d) ? a.mean + d * wb : (a.mean * a.w + b.mean * b.w) / w,
+               a.cm + b.cm + d * d * a.w * wb};
+}
+
+// a run's first observation (weight q) merged with its others: the sums of the run from its partition's first
+// observation on, when the run holds it
+__device__ __forceinline__ EwSum ew_total(const EwSt& s) {
+  const EwSum p{s.q, s.q * s.q, s.x1, s.x1 - s.x1};
+  return s.c > 1 ? ew_merge(p, EwSum{s.w, s.w2, s.mean, s.cm}) : p;
+}
+
+// `a` followed by `b`: a's others (scaled by fa), b's first observation (weight w1) and b's others merge in that order,
+// and everything a held up to its second observation keeps the share a.q fa.  With adjust, fa = beta^(b.tl - a.tl) and
+// w1 = b.q.  Without adjust, a's total (1 at a.tl) decays to beta^g at b's first observation, which then weighs alpha:
+// a keeps beta^g / (beta^g + alpha) and b's first observation alpha / (beta^g + alpha) of the total there, and b.q of
+// that total is what is left of it at b.tl; b's others are already shares of the total at b.tl.  A run without an
+// observation takes no part.
+__device__ __forceinline__ EwSt combine(const EwOp& op, const EwSt& a, const EwSt& b) {
+  if (b.f) return b;
+  if (b.c == 0) return a;
+  if (a.c == 0) return EwSt{b.c, b.t1, b.tl, b.x1, b.q, b.w, b.w2, b.mean, b.cm, a.f};
+  double fa, w1;
+  if (op.adjust) {
+    fa = decay(op, op.obs ? b.c : b.tl - a.tl);
+    w1 = b.q;
+  } else {
+    const double bg = decay(op, op.obs ? 1 : b.t1 - a.tl);
+    const double den = bg + op.alpha;
+    fa = b.q * (bg / den);
+    w1 = b.q * (op.alpha / den);
+  }
+  EwSum r{w1, w1 * w1, b.x1, b.x1 - b.x1};
+  if (a.c > 1) r = ew_merge(EwSum{a.w * fa, a.w2 * fa * fa, a.mean, a.cm * fa}, r);
+  if (b.c > 1) r = ew_merge(r, EwSum{b.w, b.w2, b.mean, b.cm});
+  return EwSt{a.c + b.c, a.t1, b.tl, a.x1, a.q * fa, r.w, r.w2, r.mean, r.cm, a.f};
+}
+
 template <class S>
 __device__ __forceinline__ S shfl_up(const S& s, int d) {
   S r;
@@ -210,9 +292,9 @@ __device__ __forceinline__ S shfl_down(const S& s, int d) {
 }
 
 // Exclusive scan of one state per thread across the CTA, and the CTA total; fixed combination order.
-// kRev: the scan runs from the last thread to the first.  S: St, or MSt / CSt / SSt (op unused).
-template <int kWarps, bool kRev = false, class S = St>
-__device__ __forceinline__ S block_exclusive(int op, const S& x, S* warp_tot, S* total) {
+// kRev: the scan runs from the last thread to the first.  S: St, or MSt / CSt / SSt (op unused), or EwSt (op: EwOp).
+template <int kWarps, bool kRev = false, class S = St, class Op = int>
+__device__ __forceinline__ S block_exclusive(const Op& op, const S& x, S* warp_tot, S* total) {
   const int lane = kRev ? 31 - (threadIdx.x & 31) : threadIdx.x & 31;
   const int w = kRev ? kWarps - 1 - (int)(threadIdx.x >> 5) : threadIdx.x >> 5;
   S inc = x;
@@ -294,8 +376,8 @@ __device__ __forceinline__ void mark_heads(int64_t nrows, int64_t nseg, const in
 
 // ---- the segmented scans: one tile kernel, one carry kernel and one launch sequence over a scan's traits ----
 // A scan's traits give its State (with combine, its 8-byte words and the flag f), its Cols, the kInputs input
-// columns a tile stages, the state of one row (entry), its kOut output words (out), the carry CTA size and how
-// pass 3 stores:
+// columns a tile stages, the state of one row (entry), its kOut output words (out for a staged scan, outs for all
+// kOut at once otherwise), the carry CTA size and how pass 3 stores:
 //   - kStaged: the one output word and the count go through shared memory, then striped (coalesced) stores;
 //   - otherwise a thread stores its kItems consecutive rows straight from registers: several outputs per row do
 //     not fit the staging buffers, and the stores of a warp still cover whole lines together.
@@ -313,6 +395,7 @@ struct StatCols {
 // a column's op (0 for the f64 families), input k, its validity and output word o
 __device__ __forceinline__ int col_op(const ScanCols& a, int col) { return a.op[col]; }
 __device__ __forceinline__ int col_op(const StatCols&, int) { return 0; }
+__device__ __forceinline__ bool is_count_op(int op) { return op == FB_AGG_COUNT; }
 __device__ __forceinline__ const uint64_t* col_input(const ScanCols& a, int col, int) {
   return (const uint64_t*)a.vals[col];
 }
@@ -323,6 +406,11 @@ __device__ __forceinline__ const uint8_t* col_valid(const ScanCols& a, int col, 
 __device__ __forceinline__ const uint8_t* col_valid(const StatCols& a, int col, int k) { return a.valid[k][col]; }
 __device__ __forceinline__ uint64_t* col_output(const ScanCols& a, int col, int) { return (uint64_t*)a.out_vals[col]; }
 __device__ __forceinline__ uint64_t* col_output(const StatCols& a, int col, int o) { return (uint64_t*)a.out[o][col]; }
+// the 8-byte word of input `src` at row r
+template <class Cols>
+__device__ __forceinline__ uint64_t col_load(const Cols&, const uint64_t* src, int64_t r) {
+  return __ldg((const unsigned long long*)src + r);
+}
 
 __device__ __forceinline__ double f64_of(uint64_t b) { return __longlong_as_double((long long)b); }
 __device__ __forceinline__ uint64_t f64_bits(double x) { return (uint64_t)__double_as_longlong(x); }
@@ -338,7 +426,7 @@ struct OpScan {
     const int c = sm.valid[j];
     return St{c && op != FB_AGG_COUNT ? sm.buf[0][padded(j)] : 0, c, sm.head[j]};
   }
-  __device__ __forceinline__ static uint64_t out(const St& s, int) { return s.v; }
+  __device__ __forceinline__ static uint64_t out(int, const St& s, int) { return s.v; }
 };
 
 // running count and M2 (fb_segmented_moments)
@@ -354,7 +442,7 @@ struct MomentScan {
     const double x = c ? f64_of(sm.buf[0][padded(j)]) : 0.0;
     return MSt{c, x, x - x, sm.head[j]};
   }
-  __device__ __forceinline__ static uint64_t out(const MSt& s, int) { return f64_bits(s.m2); }
+  __device__ __forceinline__ static uint64_t out(int, const MSt& s, int) { return f64_bits(s.m2); }
 };
 
 // running count, mean x, mean y, Sxx, Syy and Sxy of the rows where x and y are both valid (fb_segmented_comoments)
@@ -373,9 +461,8 @@ struct CoMomentScan {
     const double z = (x - x) * (y - y);
     return CSt{c, x, y, z, z, z, sm.head[j]};
   }
-  __device__ __forceinline__ static uint64_t out(const CSt& s, int o) {
-    const double v[5] = {s.mx, s.my, s.sxx, s.syy, s.sxy};
-    return f64_bits(v[o]);
+  __device__ __forceinline__ static void outs(int, const CSt& s, uint64_t (&v)[kOut]) {
+    v[0] = f64_bits(s.mx); v[1] = f64_bits(s.my); v[2] = f64_bits(s.sxx); v[3] = f64_bits(s.syy); v[4] = f64_bits(s.sxy);
   }
 };
 
@@ -395,9 +482,53 @@ struct ShapeScan {
     const double z = x - x;
     return SSt{c, x, z, z, z, sm.head[j]};
   }
-  __device__ __forceinline__ static uint64_t out(const SSt& s, int o) {
-    const double v[3] = {s.m2, s.m3, s.m4};
-    return f64_bits(v[o]);
+  __device__ __forceinline__ static void outs(int, const SSt& s, uint64_t (&v)[kOut]) {
+    v[0] = f64_bits(s.m2); v[1] = f64_bits(s.m3); v[2] = f64_bits(s.m4);
+  }
+};
+
+// the columns of fb_segmented_ewm: x with its validity, the positions (times, or NULL: the row index), the count and
+// the mean, w, w2 and cm of ew_total out
+struct EwCols {
+  const double* x[FB_SCAN_MAX_COLS];
+  const uint8_t* valid[FB_SCAN_MAX_COLS];
+  const int64_t* t[FB_SCAN_MAX_COLS];
+  int64_t* out_count[FB_SCAN_MAX_COLS];
+  double* out[4][FB_SCAN_MAX_COLS];
+  EwOp op[FB_SCAN_MAX_COLS];
+  int32_t ncols;
+};
+
+__device__ __forceinline__ EwOp col_op(const EwCols& a, int col) { return a.op[col]; }
+__device__ __forceinline__ const uint64_t* col_input(const EwCols& a, int col, int k) {
+  return k == 0 ? (const uint64_t*)a.x[col] : (const uint64_t*)a.t[col];
+}
+__device__ __forceinline__ const uint8_t* col_valid(const EwCols& a, int col, int k) {
+  return k == 0 ? a.valid[col] : nullptr;
+}
+__device__ __forceinline__ uint64_t* col_output(const EwCols& a, int col, int o) { return (uint64_t*)a.out[o][col]; }
+__device__ __forceinline__ uint64_t col_load(const EwCols&, const uint64_t* src, int64_t r) {
+  return src != nullptr ? __ldg((const unsigned long long*)src + r) : (uint64_t)r;
+}
+
+// running exponentially weighted count, mean, w, w2 and cm (fb_segmented_ewm)
+struct EwScan {
+  using State = EwSt;
+  using Cols = EwCols;
+  // an EwSt is nine 8-byte words and a flag; at the co-moments carry's 512 threads the carry kernel does not spill
+  static constexpr int kInputs = 2, kOut = 4, kCarryThreads = 512;
+  static constexpr bool kStaged = false, kFrames = false;
+  // a row is an observation when x is valid and not NaN; it enters as (1, t, t, x, 1, 0, 0, 0, 0)
+  template <class Sm>
+  __device__ __forceinline__ static EwSt entry(const EwOp&, const Sm& sm, int j) {
+    const double x = f64_of(sm.buf[0][padded(j)]);
+    const int64_t t = (int64_t)sm.buf[1][padded(j)];
+    return EwSt{sm.valid[j] && x == x, t, t, x, 1.0, 0.0, 0.0, 0.0, 0.0, sm.head[j]};
+  }
+  // the mean, W, W2 and C of ew_total, merged once per row
+  __device__ __forceinline__ static void outs(const EwOp&, const EwSt& s, uint64_t (&v)[kOut]) {
+    const EwSum r = ew_total(s);
+    v[0] = f64_bits(r.mean); v[1] = f64_bits(r.w); v[2] = f64_bits(r.w2); v[3] = f64_bits(r.cm);
   }
 };
 
@@ -472,7 +603,7 @@ fb_segscan_tile_kernel(int64_t nrows, int64_t nseg, const int64_t* __restrict__ 
   mark_heads<kReverse, kBlocks>(nrows, nseg, offsets, start, end, block, sm.head, sm.seg_range);
   const int j0 = threadIdx.x * kItems;
   for (int col = 0; col < a.ncols; ++col) {
-    const int op = col_op(a, col);
+    const auto op = col_op(a, col);
     const uint64_t* src[T::kInputs];
     const uint8_t* vm[T::kInputs];
 #pragma unroll
@@ -482,13 +613,13 @@ fb_segscan_tile_kernel(int64_t nrows, int64_t nseg, const int64_t* __restrict__ 
     }
     // striped (coalesced) loads into shared memory; rows past the end are invalid.  They read the tile's first row
     // instead, so that every load stays in bounds and none waits on a branch.  A COUNT scan reads no values.
-    const bool is_count = op == FB_AGG_COUNT;
+    const bool is_count = is_count_op(op);
     for (int i = threadIdx.x; i < kTile; i += kThreads) {
       const bool in = i < nloc;
       const int64_t r = row(in ? i : 0);
 #pragma unroll
       for (int k = 0; k < T::kInputs; ++k)
-        if (!is_count) sm.buf[k][padded(i)] = in ? __ldg((const unsigned long long*)src[k] + r) : 0;
+        if (!is_count) sm.buf[k][padded(i)] = in ? col_load(a, src[k], r) : 0;
       bool ok = true;
 #pragma unroll
       for (int k = 0; k < T::kInputs; ++k) ok = ok && (vm[k] == nullptr || __ldg(vm[k] + r) != 0);
@@ -515,7 +646,7 @@ fb_segscan_tile_kernel(int64_t nrows, int64_t nseg, const int64_t* __restrict__ 
       for (int k = 0; k < kItems; ++k) {
         const int j = j0 + k;
         run = combine(op, run, T::entry(op, sm, j));
-        sm.buf[0][padded(j)] = run.c > 0 ? T::out(run, 0) : 0;  // no valid row yet: 0, not whatever preceded the segment
+        sm.buf[0][padded(j)] = run.c > 0 ? T::out(op, run, 0) : 0;  // no valid row yet: 0, not whatever preceded the segment
         sm.buf[T::kInputs][padded(j)] = (uint64_t)run.c;
       }
       __syncthreads();
@@ -534,10 +665,12 @@ fb_segscan_tile_kernel(int64_t nrows, int64_t nseg, const int64_t* __restrict__ 
         if (j >= nloc) continue;
         const bool any = run.c > 0;  // no valid row yet: 0, not whatever preceded the segment
         if (oc != nullptr) oc[row(j)] = run.c;
+        uint64_t v[T::kOut];
+        T::outs(op, run, v);
 #pragma unroll
         for (int o = 0; o < T::kOut; ++o) {
           uint64_t* __restrict__ ov = col_output(a, col, o);
-          if (ov != nullptr) ov[row(j)] = any ? T::out(run, o) : 0;
+          if (ov != nullptr) ov[row(j)] = any ? v[o] : 0;
         }
       }
     }
@@ -553,7 +686,7 @@ fb_segscan_carry_kernel(int64_t ntiles, const __grid_constant__ typename T::Cols
   using S = typename T::State;
   __shared__ S warp_tot[T::kCarryThreads / 32];
   const int col = blockIdx.x;
-  const int op = col_op(a, col);
+  const auto op = col_op(a, col);
   const int64_t o = (int64_t)col * ntiles;
   const int64_t per = (ntiles + T::kCarryThreads - 1) / T::kCarryThreads;
   const int64_t b = threadIdx.x * per;
@@ -1408,6 +1541,48 @@ extern "C" int fb_segmented_shape_moments(int dev, void* stream, int64_t nrows, 
                                                c);
                                     return 0;
                                   });
+}
+
+extern "C" size_t fb_segmented_ewm_scratch_bytes(int64_t nrows, int ncols) {
+  return segscan_scratch_bytes<EwScan>(nrows, ncols);
+}
+
+extern "C" int fb_segmented_ewm(int dev, void* stream, int64_t nrows, int64_t nseg, const int64_t* d_offsets,
+                                int ncols, const void* const* vals, const uint8_t* const* valid, const double* alpha,
+                                const int32_t* adjust, const int32_t* positions, const void* const* times,
+                                const double* time_scale, int64_t* const* out_count, void* const* out_mean,
+                                void* const* out_w, void* const* out_w2, void* const* out_c, void* scratch,
+                                size_t scratch_bytes) {
+  return segscan_entry<EwScan>(dev, stream, nrows, nseg, d_offsets, ncols, "ncols", scratch, scratch_bytes,
+                               [&](EwCols& a) {
+                                 FB_CHECK(alpha != nullptr && adjust != nullptr && positions != nullptr,
+                                          "NULL alpha, adjust or positions");
+                                 void* const* outs[4] = {out_mean, out_w, out_w2, out_c};
+                                 for (int c = 0; c < ncols; ++c) {
+                                   const int pos = positions[c];
+                                   FB_CHECK(pos >= FB_EWM_ROWS && pos <= FB_EWM_TIMES, "column %d: unknown positions %d",
+                                            c, pos);
+                                   FB_CHECK(alpha[c] > 0.0 && alpha[c] <= 1.0, "column %d: alpha %g not in (0, 1]", c,
+                                            alpha[c]);
+                                   a.x[c] = vals != nullptr ? (const double*)vals[c] : nullptr;
+                                   a.valid[c] = valid != nullptr ? valid[c] : nullptr;
+                                   FB_CHECK(nrows == 0 || a.x[c] != nullptr, "column %d needs a value column", c);
+                                   double k = log2(1.0 - alpha[c]);
+                                   if (pos == FB_EWM_TIMES) {
+                                     FB_CHECK(times != nullptr && (nrows == 0 || times[c] != nullptr),
+                                              "column %d: time decay needs a times column", c);
+                                     FB_CHECK(time_scale != nullptr && time_scale[c] > 0.0 && isfinite(time_scale[c]),
+                                              "column %d: time scale must be finite and > 0", c);
+                                     a.t[c] = (const int64_t*)times[c];
+                                     k = -time_scale[c];
+                                   }
+                                   a.op[c] = EwOp{k, alpha[c], adjust[c] != 0, pos == FB_EWM_OBSERVATIONS};
+                                   a.out_count[c] = out_count != nullptr ? out_count[c] : nullptr;
+                                   for (int o = 0; o < 4; ++o)
+                                     a.out[o][c] = outs[o] != nullptr ? (double*)outs[o][c] : nullptr;
+                                 }
+                                 return 0;
+                               });
 }
 
 extern "C" size_t fb_window_frame_scratch_bytes(int64_t nrows, int ncols, int64_t start, int64_t end, int flags) {

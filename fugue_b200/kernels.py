@@ -539,6 +539,42 @@ def segmented_comoments(offsets: torch.Tensor, nrows: int,
                         scratch.numel()))
 
 
+EWM_ROWS = 0           # FB_EWM_*: the positions of fb_segmented_ewm: row index (pandas' ignore_na=False),
+EWM_OBSERVATIONS = 1   # observation ordinal (ignore_na=True),
+EWM_TIMES = 2          # an int64 times column, decaying by 0.5^(dt * scale)
+
+
+def segmented_ewm(offsets: torch.Tensor, nrows: int,
+                  columns: Sequence[Tuple[torch.Tensor, Optional[torch.Tensor], float, bool, int,
+                                          Optional[torch.Tensor], float, bool]]) -> List[Tuple[Any, ...]]:
+    """K9: running exponentially weighted moments restarting at every segment ``[offsets[s], offsets[s + 1])``.
+    ``columns`` = one ``(float64 values, validity or None, alpha, adjust, positions, int64 times or None, scale,
+    spread)`` per column, ``positions`` one of ``EWM_*`` (``times`` and ``scale`` = 1 / halflife only for
+    ``EWM_TIMES``).  An observation is a valid, non-NaN value.  Returns per column ``(count of observations (int64),
+    weighted mean, W, W2, C)`` up to each row (float64, 0 where the count is 0), with W / W2 the sums of the weights
+    and of their squares and C the weighted sum of squared deviations from the mean, each weight a share of the total
+    without ``adjust`` (``fb_segmented_ewm``); W, W2 and C are None unless ``spread``, and then not written.  Up to
+    ``SCAN_MAX_COLS`` columns share one launch sequence."""
+    lib = _lib.load()
+    dev, nseg = _segments(offsets)
+
+    def outputs(v: torch.Tensor, m: Optional[torch.Tensor], alpha: float, adjust: bool, pos: int,
+                times: Optional[torch.Tensor], scale: float, spread: bool) -> Tuple[Any, ...]:
+        _check_rows(v, dev, nrows, torch.float64)
+        _check_rows(m, dev, nrows, torch.uint8)
+        assert (times is not None) == (pos == EWM_TIMES)
+        _check_rows(times, dev, nrows, torch.int64)
+        return _stat_outputs(dev, nrows, 4 if spread else 1) + (() if spread else (None, None, None))
+
+    return _batched(columns, dev, outputs, lambda n: lib.fb_segmented_ewm_scratch_bytes(nrows, n),
+                    lambda batch, outs, scratch: lib.fb_segmented_ewm(
+                        dev.index, _stream_ptr(dev), nrows, nseg, offsets.data_ptr(), len(batch),
+                        _ptrs([c[0] for c in batch]), _ptrs([c[1] for c in batch]),
+                        _lib.f64_array([c[2] for c in batch]), _lib.i32_array([c[3] for c in batch]),
+                        _lib.i32_array([c[4] for c in batch]), _ptrs([c[5] for c in batch]),
+                        _lib.f64_array([c[6] for c in batch]), *outs, scratch.data_ptr(), scratch.numel()))
+
+
 FRAME_TILE_MAX_WIDTH = 1024   # FB_FRAME_TILE_MAX_WIDTH: widest frame of the one-pass kernel
 FRAME_UNBOUNDED_START = 1
 FRAME_UNBOUNDED_END = 2

@@ -22,8 +22,13 @@ Window functions (DESIGN §7p):
     <call>  ::= any aggregate above | ROW_NUMBER() | RANK() | DENSE_RANK() | LAG(x[, n[, default]])
               | LEAD(x[, n[, default]]) | PERCENTILE_CONT / PERCENTILE_DISC(q) WITHIN GROUP (ORDER BY x)
               | NTILE(n) | PERCENT_RANK() | CUME_DIST() | FIRST_VALUE(x) | LAST_VALUE(x) | NTH_VALUE(x, n)
-                (n an integer literal >= 1; NTILE, PERCENT_RANK and CUME_DIST take no frame; the value functions
-                respect NULLs: IGNORE NULLS and FROM LAST raise NotImplementedError)
+              | EWM_MEAN(x, <decay>[, adjust]) | EWM_VAR(x, <decay>[, adjust]) | EWM_STD(x, <decay>[, adjust])
+                (n an integer literal >= 1; NTILE, PERCENT_RANK, CUME_DIST and the EWM functions take no frame; the
+                value functions respect NULLs: IGNORE NULLS and FROM LAST raise NotImplementedError)
+    <decay> ::= alpha | INTERVAL '..' DAY [TO SECOND]
+                (pandas' ewm: alpha a numeric literal in (0, 1]; an INTERVAL is the halflife of a time decay over the
+                single ORDER BY expression, EWM_MEAN only; adjust a boolean literal, TRUE by default; ignore_na FALSE,
+                min_periods 0 and the sample variance)
     <frame> ::= ROWS | RANGE  BETWEEN <bound> AND <bound>  |  ROWS | RANGE <bound>
     <bound> ::= UNBOUNDED PRECEDING | n PRECEDING | CURRENT ROW | n FOLLOWING | UNBOUNDED FOLLOWING
                 (a RANGE offset n may be an INTERVAL '..' DAY / DAY TO SECOND literal)
@@ -68,7 +73,7 @@ from typing import Any, Dict, List, Tuple
 
 import pyarrow as pa
 
-from .column import (_SPEC_ONLY, BIVARIATES, PERCENTILES, VALUE_HEADS, ColumnExpr, Kind, SelectColumns, _nth,
+from .column import (_SPEC_ONLY, BIVARIATES, EWM_HEADS, PERCENTILES, VALUE_HEADS, ColumnExpr, Kind, SelectColumns, _nth,
                      _offset_fn, _value_fn, all_cols, check_arity, col, function, functions, has_window, is_agg, lit,
                      null, scalar_head)
 from .dataframe import DataFrame
@@ -899,6 +904,8 @@ class _Parser:
         self.expect(")")
         if fn in ("NTILE", "FIRST_VALUE", "LAST_VALUE", "NTH_VALUE"):
             return self._value_call(fn, args)
+        if fn in EWM_HEADS:
+            return self._ewm_call(fn, args)
         if len(args) > 3:
             raise ValueError(f"{fn} takes 1 to 3 arguments, got {len(args)} in: {self.sql}")
         for what, x in zip(("n", "default"), args[1:]):
@@ -907,6 +914,25 @@ class _Parser:
         n = args[1].value if len(args) > 1 else 1
         default = args[2].value if len(args) > 2 else None
         return _offset_fn(fn, args[0], n, default, aggregated=True)
+
+    def _ewm_call(self, fn: str, args: List[ColumnExpr]) -> ColumnExpr:
+        """``EWM_MEAN / EWM_VAR / EWM_STD(x, alpha [, adjust])``: alpha a numeric literal in (0, 1], or an ``INTERVAL``
+        literal, the halflife of a time decay over the single ORDER BY expression; adjust a boolean literal (TRUE).
+        pandas' defaults otherwise: ignore_na FALSE, min_periods 0, the sample variance."""
+        if len(args) not in (2, 3):
+            raise ValueError(f"{fn} takes 2 or 3 arguments, got {len(args)} in: {self.sql}")
+        for what, x in zip(("alpha", "adjust"), args[1:]):
+            if x.kind != Kind.LITERAL or x.as_type is not None:
+                raise ValueError(f"{fn}: {what} must be a literal, got {x} in: {self.sql}")
+        decay, adjust = args[1].value, args[2].value if len(args) > 2 else True
+        if not isinstance(adjust, bool):
+            raise ValueError(f"{fn}: adjust must be TRUE or FALSE, got {args[2]} in: {self.sql}")
+        if isinstance(decay, datetime.timedelta):
+            return getattr(functions, fn.lower())(args[0], halflife=decay, adjust=adjust, times=True)
+        if isinstance(decay, bool) or not isinstance(decay, (int, float)):
+            raise ValueError(f"{fn}: alpha must be a number in (0, 1] or an INTERVAL halflife, got {args[1]} in: "
+                             f"{self.sql}")
+        return getattr(functions, fn.lower())(args[0], alpha=decay, adjust=adjust)
 
     def _value_call(self, fn: str, args: List[ColumnExpr]) -> ColumnExpr:
         """``NTILE(n)``, ``FIRST_VALUE(x)``, ``LAST_VALUE(x)`` or ``NTH_VALUE(x, n)`` [FROM FIRST] [RESPECT NULLS]: n an

@@ -337,6 +337,38 @@ int fb_segmented_shape_moments(int dev, void* stream, int64_t nrows, int64_t nse
                                void* const* out_m2, void* const* out_m3, void* const* out_m4, void* scratch,
                                size_t scratch_bytes);
 
+/* K9  segmented exponentially weighted moments (pandas' ewm): over the same segments, per column c and row i, the
+ * observations of i's segment up to and including i.  An observation is a row whose f64 value vals[c] is valid
+ * (valid[c], or NULL: every row) and not NaN.  Observation j carries the weight w_j beta^(p_last - p_j), p_last being
+ * the position of the last of them, beta = 1 - alpha[c]:
+ *   positions[c] FB_EWM_ROWS          p = the row index (pandas' ignore_na=False)
+ *                FB_EWM_OBSERVATIONS  p = the observation ordinal (ignore_na=True)
+ *                FB_EWM_TIMES         p = times[c][i] (int64) times time_scale[c], beta = 1/2: 0.5^(dt / halflife)
+ * w = 1 for the segment's first observation and, with adjust[c], for every other; without adjust, observation k
+ * weighs alpha T_(k-1), T being the running total weight (T_1 = 1, T_k = T_(k-1) (beta^(p_k - p_(k-1)) + alpha)).
+ * Writes
+ *   out_count[c][i]                          the number of observations (int64)
+ *   out_mean[c][i], out_w, out_w2, out_c     the weighted mean, W = sum of the weights, W2 = sum of their squares and
+ *                                            C = sum of w (x - mean)^2 (f64), 0 where the count is 0
+ * Without adjust, W, W2 and C are taken with every weight divided by the total (so W = 1 up to rounding): pandas' T
+ * overflows or underflows over long partitions with gaps, and mean, C / W and W2 / W^2 do not depend on the scale.
+ * A row without an observation repeats the previous row's values.  Once a +-inf is among the observations C is NaN
+ * and the mean is what the weighted sum gives (+-inf, or NaN).  Position differences are exact int64 differences.
+ * The state (count, first and last position, first value and its weight, W, W2, mean, C of the others) is combined
+ * with a decayed, weighted Chan update; same launch sequence and fixed combination order as fb_segmented_scan: bit-identical runs.
+ * alpha must be in (0, 1]; time_scale (1 / halflife) finite and > 0 for FB_EWM_TIMES (times and time_scale may be NULL
+ * when no column uses times).  Every pointer argument but d_offsets and scratch is a HOST array of
+ * ncols <= FB_SCAN_MAX_COLS entries (an output may be NULL: not written); scratch: fb_segmented_ewm_scratch_bytes. */
+#define FB_EWM_ROWS 0
+#define FB_EWM_OBSERVATIONS 1
+#define FB_EWM_TIMES 2
+size_t fb_segmented_ewm_scratch_bytes(int64_t nrows, int ncols);
+int fb_segmented_ewm(int dev, void* stream, int64_t nrows, int64_t nseg, const int64_t* d_offsets, int ncols,
+                     const void* const* vals, const uint8_t* const* valid, const double* alpha, const int32_t* adjust,
+                     const int32_t* positions, const void* const* times, const double* time_scale,
+                     int64_t* const* out_count, void* const* out_mean, void* const* out_w, void* const* out_w2,
+                     void* const* out_c, void* scratch, size_t scratch_bytes);
+
 /* K9  moving-window aggregate: ROWS BETWEEN start AND end over the same segments.  For row i of segment
  * [a, b) the frame is rows [max(a, i + start), min(b - 1, i + end)] (may be empty); a negative bound is
  * PRECEDING, 0 CURRENT ROW, a positive one FOLLOWING.  FB_FRAME_UNBOUNDED_START / _END in `flags` make a
